@@ -29,6 +29,14 @@ class Cfg(C.Structure):
     ]
 
 
+class Hparams(C.Structure):
+    _fields_ = [
+        ("gamma", C.c_double), ("reward_scale", C.c_double), ("tau", C.c_double),
+        ("lr_critic", C.c_double), ("lr_actor", C.c_double), ("lr_alpha", C.c_double),
+        ("tau_se", C.c_double), ("lr_ctx", C.c_double),
+    ]
+
+
 class TensorDesc(C.Structure):
     _fields_ = [("name", C.c_char * 48), ("offset", C.c_int64), ("rows", C.c_int32), ("cols", C.c_int32),
                 ("trainable", C.c_int32), ("opt", C.c_int32), ("pitch", C.c_int32), ("reserved", C.c_int32)]
@@ -51,6 +59,9 @@ SYMBOLS = {
     "b200sac_arena_ptr": (C.c_int, [_VP, C.c_int32, C.POINTER(_VP), C.POINTER(C.c_int64)]),
     "b200sac_get_steps": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int64)]),
     "b200sac_set_steps": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int64)]),
+    "b200sac_get_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams)]),
+    "b200sac_set_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams), _VP]),
+    "b200sac_copy_replica": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
     "b200sac_step": (C.c_int, [_VP] + [_VP] * 7 + [_VP]),
     "b200sac_step_host": (C.c_int, [_VP] + [_VP] * 7 + [_VP, _VP]),
     "b200sac_step_sampled": (C.c_int, [_VP, _VP, C.c_int32, _VP]),

@@ -317,6 +317,32 @@ class SacCore:
         s = (C.c_int64 * 4)(*vals[:4])
         _lib.check(self.lib.b200sac_set_steps(self._h, replica, s))
 
+    # ---- per-replica hyperparameters (b200sac_get/set_hparams) -------------------------------------------
+    HPARAMS = tuple(name for name, _ in _lib.Hparams._fields_)
+
+    def get_hparams(self, replica=0) -> Dict[str, float]:
+        """{gamma, reward_scale, tau, lr_critic, lr_actor, lr_alpha, tau_se, lr_ctx} of one replica (no synchronisation)."""
+        hp = _lib.Hparams()
+        _lib.check(self.lib.b200sac_get_hparams(self._h, int(replica), C.byref(hp)))
+        return {name: float(getattr(hp, name)) for name in self.HPARAMS}
+
+    def set_hparams(self, replica=None, **values):
+        """Change hyperparameters of one replica (replica=None: all of them) on the current stream; fields not named keep
+        their value.  Steps enqueued afterwards use the new values, steps already enqueued do not."""
+        unknown = set(values) - set(self.HPARAMS)
+        if unknown:
+            raise TypeError(f"unknown hyperparameters {sorted(unknown)}; known: {self.HPARAMS}")
+        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+            cur = self.get_hparams(r)
+            cur.update({k: float(v) for k, v in values.items()})
+            hp = _lib.Hparams(**cur)
+            _lib.check(self.lib.b200sac_set_hparams(self._h, r, C.byref(hp), _stream()))
+
+    def copy_replica(self, src: int, dst: int):
+        """Replica dst's parameters (targets, log_alpha included), Adam moments and step counters become a copy of src's,
+        device to device on the current stream.  Hyperparameters and replay data stay dst's own."""
+        _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
+
     def soft_update(self, tau: float):
         _lib.check(self.lib.b200sac_soft_update(self._h, float(tau), _stream()))
 

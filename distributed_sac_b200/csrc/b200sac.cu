@@ -9,6 +9,7 @@
 #include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <functional>
 #include <map>
 #include <mutex>
@@ -266,6 +267,8 @@ struct b200sac {
   // arenas
   float *params = nullptr, *adam_m = nullptr, *adam_v = nullptr, *grads = nullptr;
   Counters* cnt = nullptr;
+  HParams* hp = nullptr;          // [R] per-replica hyperparameters (K.hp points here)
+  std::vector<b200sac_hparams> hp_host;   // host mirror of the values as given (b200sac_get_hparams does not synchronise)
   float* losses = nullptr;        // [kLossSlots][R][4]
   long long host_steps = 0;       // steps enqueued so far
   // work slab
@@ -372,7 +375,7 @@ static int destroy_impl(b200sac* h) {
   cudaSetDevice(h->device);
   for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
   cudaFree(h->params); cudaFree(h->adam_m); cudaFree(h->adam_v); cudaFree(h->grads); cudaFree(h->grads_x);
-  cudaFree(h->cnt); cudaFree(h->losses); cudaFree(h->slab); cudaFree(h->d_probs); cudaFree(h->d_tprobs);
+  cudaFree(h->cnt); cudaFree(h->hp); cudaFree(h->losses); cudaFree(h->slab); cudaFree(h->d_probs); cudaFree(h->d_tprobs);
   for (int i = 0; i < 2; ++i) {
     if (h->stage_h[i]) cudaFreeHost(h->stage_h[i]);
     cudaFree(h->stage_d[i]);
@@ -671,7 +674,6 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& ada
       O.params = h->params; O.m = h->adam_m; O.v = h->adam_v; O.grads = h->grads;
       O.rsP = rsP; O.rsM = rsG;
       O.target_delta = which == 0 ? L.target_delta : 0;
-      O.lr = which == 0 ? c.lr_critic : c.lr_actor;
       O.cnt = h->cnt;
     }
     int tiles = 0;
@@ -1258,9 +1260,7 @@ static int build_plan(b200sac* h) {
     P.gx = h->grads_x ? h->grads_x + beg : nullptr; P.xs = (long long)R * L.trainable; P.nx = h->gslices - 1;
     P.target_delta = which == 0 ? L.target_delta : 0;
     P.tau2_begin = (which == 0 && c.care) ? (L.cse_begin - L.critic_begin) : (long long)1 << 60;
-    P.tau2 = (float)c.tau_se; P.one_minus_tau2 = (float)(1.0 - c.tau_se);
     P.which = which == 2 ? 4 : which;                    // counter slot: 0 critic, 1 actor, 4 context encoder
-    P.lr = which == 0 ? c.lr_critic : (which == 1 ? c.lr_actor : c.lr_ctx);
     P.cnt = h->cnt;
     P.tail = which == 0 ? TAIL_CRITIC_LOSS : (which == 1 ? TAIL_ALPHA_AND_LOSSES : TAIL_NONE);
     if (mode == 1) P.tail = TAIL_NONE;
@@ -1758,6 +1758,17 @@ extern "C" int b200sac_launches_per_step(b200sac_t* h, int32_t* n) {
   return 0;
 }
 
+// The device row of a replica's hyperparameters, rounded the way the kernels consume them.
+static HParams hparams_row(const b200sac_hparams& v) {
+  HParams r;
+  memset(&r, 0, sizeof(r));
+  r.lr[0] = v.lr_critic; r.lr[1] = v.lr_actor; r.lr[2] = v.lr_alpha; r.lr[4] = v.lr_ctx;
+  r.gamma = (float)v.gamma; r.reward_scale = (float)v.reward_scale;
+  r.tau = (float)v.tau; r.one_minus_tau = (float)(1.0 - v.tau);
+  r.tau_se = (float)v.tau_se; r.one_minus_tau_se = (float)(1.0 - v.tau_se);
+  return r;
+}
+
 extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t seed, b200sac_t** out) {
   if (!out) return fail(B200SAC_ERR_INVALID, "out is NULL");
   *out = nullptr;
@@ -1785,12 +1796,10 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   const int ldxa = K.ldxa, ldx = K.ldx;
   K.Ha = cfg->actor_hidden[cfg->n_actor_hidden - 1];
   K.Hc = cfg->critic_hidden[cfg->n_critic_hidden - 1];
-  K.gamma = (float)cfg->gamma; K.reward_scale = (float)cfg->reward_scale; K.action_scale = (float)cfg->action_scale;
+  K.action_scale = (float)cfg->action_scale;
   K.c_loss = (float)(1.0 / B / (cfg->weighted_loss ? (double)B : 1.0));
   K.inv_B = (float)(1.0 / B);
-  K.tau = (float)cfg->tau; K.one_minus_tau = (float)(1.0 - cfg->tau);
   K.hbar = -(float)A;
-  K.lr_actor = cfg->lr_actor; K.lr_critic = cfg->lr_critic; K.lr_alpha = cfg->lr_alpha;
   K.beta1 = cfg->beta1; K.beta2 = cfg->beta2; K.adam_eps = cfg->adam_eps;
   K.seed = seed;
 
@@ -1826,6 +1835,17 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CUH(cudaMemcpy(h->cnt, c0.data(), sizeof(Counters) * R, cudaMemcpyHostToDevice));
   }
   CUH(cudaMemset(h->losses, 0, sizeof(float) * kLossSlots * R * 4));
+  {
+    b200sac_hparams hp0;
+    hp0.gamma = cfg->gamma; hp0.reward_scale = cfg->reward_scale; hp0.tau = cfg->tau;
+    hp0.lr_critic = cfg->lr_critic; hp0.lr_actor = cfg->lr_actor; hp0.lr_alpha = cfg->lr_alpha;
+    hp0.tau_se = cfg->tau_se; hp0.lr_ctx = cfg->lr_ctx;
+    h->hp_host.assign((size_t)R, hp0);
+    const std::vector<HParams> rows((size_t)R, hparams_row(hp0));
+    CUH(cudaMalloc(&h->hp, sizeof(HParams) * R));
+    CUH(cudaMemcpy(h->hp, rows.data(), sizeof(HParams) * R, cudaMemcpyHostToDevice));
+    K.hp = h->hp;
+  }
 
   // work slab
   size_t cur = 0;
@@ -2102,6 +2122,54 @@ struct StreamBridge {
     return 0;
   }
 };
+
+// ------------------------------------------------------------------------------------------
+// Per-replica hyperparameters.  The step reads them from a device table [R] (HParams), so replicas of one handle can
+// train with different values and a value can change between steps: the row is written by a one-thread kernel in stream
+// order, which the captured step graphs simply read at their next launch.
+// ------------------------------------------------------------------------------------------
+extern "C" int b200sac_get_hparams(b200sac_t* h, int32_t replica, b200sac_hparams* out) {
+  if (!h || !out) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  *out = h->hp_host[(size_t)replica];
+  return 0;
+}
+
+extern "C" int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp, void* stream) {
+  if (!h || !hp) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  const double all[8] = {hp->gamma, hp->reward_scale, hp->tau, hp->lr_critic, hp->lr_actor, hp->lr_alpha, hp->tau_se, hp->lr_ctx};
+  for (double x : all)
+    if (!std::isfinite(x)) return fail(B200SAC_ERR_INVALID, "hyperparameters must be finite");
+  if (hp->tau < 0.0 || hp->tau > 1.0 || hp->tau_se < 0.0 || hp->tau_se > 1.0)
+    return fail(B200SAC_ERR_INVALID, "0 <= tau, tau_se <= 1 required (got %g, %g)", hp->tau, hp->tau_se);
+  if (hp->lr_critic < 0.0 || hp->lr_actor < 0.0 || hp->lr_alpha < 0.0 || hp->lr_ctx < 0.0)
+    return fail(B200SAC_ERR_INVALID, "learning rates must be >= 0");
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  set_hparams_kernel<<<1, 1, 0, sb.run>>>(h->hp, replica, hparams_row(*hp));
+  CU(cudaGetLastError());
+  if (int rc = sb.end()) return rc;
+  h->hp_host[(size_t)replica] = *hp;
+  return 0;
+}
+
+extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (src < 0 || src >= h->R || dst < 0 || dst >= h->R)
+    return fail(B200SAC_ERR_INVALID, "replicas %d -> %d out of range (%d in the handle)", src, dst, h->R);
+  if (src == dst) return 0;
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  const size_t na = (size_t)h->L.arena, nt = (size_t)h->L.trainable;
+  CU(cudaMemcpyAsync(h->params + dst * na, h->params + src * na, na * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
+  CU(cudaMemcpyAsync(h->adam_m + dst * nt, h->adam_m + src * nt, nt * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
+  CU(cudaMemcpyAsync(h->adam_v + dst * nt, h->adam_v + src * nt, nt * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
+  CU(cudaMemcpyAsync(h->cnt + dst, h->cnt + src, sizeof(Counters), cudaMemcpyDeviceToDevice, sb.run));
+  return sb.end();
+}
 
 // ------------------------------------------------------------------------------------------
 // Publication path: Learner.get_parameters() -> pickle -> Redis runs after EVERY update in the reference
@@ -2872,12 +2940,11 @@ extern "C" int b200sac_soft_update(b200sac_t* h, double tau, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   CU(cudaSetDevice(h->device));
   // CARE: Learner.soft_update is called per module with its own tau; this entry point applies `tau` to the Q
-  // functions and, unless tau == 1 (hard copy of everything), state_encoder_tau to the state encoder.
+  // functions and, unless tau == 1 (hard copy of everything), the replica's state_encoder_tau to the state encoder.
   const bool hard = (tau == 1.0);
   polyak_kernel<<<dim3(128, h->R), 256, 0, (cudaStream_t)stream>>>(
       h->params + h->L.critic_begin, h->L.arena, h->L.critic_n, h->L.target_delta, (float)tau, (float)(1.0 - tau),
-      (h->cfg.care && !hard) ? (long long)(h->L.cse_begin - h->L.critic_begin) : -1LL, (float)h->cfg.tau_se,
-      (float)(1.0 - h->cfg.tau_se));
+      (h->cfg.care && !hard) ? (long long)(h->L.cse_begin - h->L.critic_begin) : -1LL, h->hp);
   CU(cudaGetLastError());
   return 0;
 }

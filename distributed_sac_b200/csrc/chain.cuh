@@ -290,13 +290,14 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constan
         const float alpha_row = alpha_of(t_row);
         if (lane == 0) {
           const float r = (R.r + rep * R.rsR)[row], d = (R.d + rep * R.rsR)[row];
+          const float gamma = K.hp[rep].gamma, reward_scale = K.hp[rep].reward_scale;
           const float lp = (R.logp + rep * R.rsLogp)[row];
           const float* QT = R.qt + rep * 2 * R.rsY;
           const float* Q = R.q + rep * 2 * R.rsY;
           const float qt1 = QT[row], qt2 = QT[B + row], q1 = Q[row], q2 = Q[B + row];
           const float alpha = alpha_row;
-          const float t1 = K.reward_scale * r;
-          const float t2 = K.gamma * (1.f - d);
+          const float t1 = reward_scale * r;
+          const float t2 = gamma * (1.f - d);
           const float t3 = fminf(qt1, qt2) - alpha * lp;
           const float y = t1 + t2 * t3;
           const float qn = J.net == 0 ? q1 : q2;
@@ -650,12 +651,11 @@ struct WgradJob {
 // tile's fixed-order sum is done, so the separate optimizer launch (one more kernel boundary + a cold pass over p/m/v) is
 // unnecessary.  Same element-wise math as adam_kernel (adam_one, torch _single_tensor_adam).
 struct WgradAdam {
-  int enabled, which;                      // which: Adam step-counter slot (0 critic, 1 actor)
+  int enabled, which;                      // which: Adam step-counter / learning-rate slot (0 critic, 1 actor)
   float* params; float* m; float* v;       // arenas; an element's index = its offset in the gradient arena
   const float* grads;                      // gradient arena base (to turn C pointers into offsets)
   long long rsP, rsM;
   long long target_delta;                  // != 0: params[i + target_delta] is the Polyak target of element i
-  double lr;
   const Counters* cnt;
 };
 struct WgradArgs {
@@ -719,8 +719,12 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   // bias corrections of the fused optimizer step (two counter loads, an fp64 division and square root): evaluated now, while
   // the operand tiles are in flight, instead of heading the epilogue
   const WgradAdam& O = A.adam;
-  float step_size = 0.f, bc2_sqrt = 1.f;
-  if (O.enabled) adam_scalars(O.lr, O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
+  float step_size = 0.f, bc2_sqrt = 1.f, tau = 0.f, one_minus_tau = 0.f;
+  if (O.enabled) {
+    const HParams& H = K.hp[rep];
+    adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
+    tau = H.tau; one_minus_tau = H.one_minus_tau;
+  }
   const float* __restrict__ Ag = J.A + (long long)rep * J.rsA;
   const float* __restrict__ Bg = J.B + (long long)rep * J.rsB;
   const int M = A.M;
@@ -872,8 +876,8 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
       *reinterpret_cast<float4*>(O.v + rep * O.rsM + gi) = v4;
       if (has_t)
         *reinterpret_cast<float4*>(pp + O.target_delta) =
-            make_float4(K.tau * p4.x + K.one_minus_tau * t4.x, K.tau * p4.y + K.one_minus_tau * t4.y,
-                        K.tau * p4.z + K.one_minus_tau * t4.z, K.tau * p4.w + K.one_minus_tau * t4.w);
+            make_float4(tau * p4.x + one_minus_tau * t4.x, tau * p4.y + one_minus_tau * t4.y,
+                        tau * p4.z + one_minus_tau * t4.z, tau * p4.w + one_minus_tau * t4.w);
     }
   }
   if (bias_thread) {
@@ -887,7 +891,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
       *pp = bp;
       (O.m + rep * O.rsM)[bgi] = bm;
       (O.v + rep * O.rsM)[bgi] = bv_;
-      if (has_t) pp[O.target_delta] = K.tau * bp + K.one_minus_tau * bt;
+      if (has_t) pp[O.target_delta] = tau * bp + one_minus_tau * bt;
     }
   }
   WG_STAMP();                              // reduction + optimizer step done

@@ -178,11 +178,12 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
   const int row = row0 + w;
   const bool owner = (w < nrows) && lane == 0;           // lane 0 of warp w owns row w
   int t_row = 0;
-  float r_row = 0.f, d_row = 0.f, lp_row = 0.f, q1_row = 0.f, q2_row = 0.f;
+  float r_row = 0.f, d_row = 0.f, lp_row = 0.f, q1_row = 0.f, q2_row = 0.f, gamma = 0.f, reward_scale = 0.f;
   if (owner) {
     t_row = (R.tid + rep * R.rsR)[row];
     if (A.kind == C2_CRITIC) {
       r_row = (R.r + rep * R.rsR)[row]; d_row = (R.d + rep * R.rsR)[row];
+      gamma = K.hp[rep].gamma; reward_scale = K.hp[rep].reward_scale;
       lp_row = (R.logp + rep * R.rsLogp)[row];
       const float* Q = R.q + rep * 2 * R.rsY;
       q1_row = Q[row]; q2_row = Q[B + row];
@@ -366,8 +367,8 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     const float q_peer = ld_peer_f32(xch + w, my_rank ^ 1u);
     const float qa = J.net == 0 ? q_own : q_peer, qb = J.net == 0 ? q_peer : q_own;
     if (A.kind == C2_CRITIC) {             // qa, qb = Qt1, Qt2
-      const float t1 = K.reward_scale * r_row;
-      const float t2 = K.gamma * (1.f - d_row);
+      const float t1 = reward_scale * r_row;
+      const float t2 = gamma * (1.f - d_row);
       const float t3 = fminf(qa, qb) - alpha_row * lp_row;
       const float y = t1 + t2 * t3;
       const float qn = J.net == 0 ? q1_row : q2_row;

@@ -16,6 +16,17 @@ constexpr int kMaxHeadOut = 16;
 constexpr int kSaveW = 8;       // floats saved per (row, action) by the policy head
 constexpr int kLossSlots = 1024;
 
+// Per-replica hyperparameters: one row per replica in device memory (b200sac_set_hparams), read by the step at its
+// replica index.  The values are not in StepConst because StepConst is captured by value into the CUDA graphs; a row
+// written by a stream-ordered kernel between two graph launches changes the next step without re-instantiating a graph.
+struct HParams {
+  double lr[5];                   // Adam learning rates, indexed like the Counters slots: 0 critic, 1 actor, 2 temperature,
+                                  // 4 CARE(O) context encoder (3 unused)
+  float gamma, reward_scale;
+  float tau, one_minus_tau;       // Polyak rate of the target critics
+  float tau_se, one_minus_tau_se; // CARE: Polyak rate of the target state encoder
+};
+
 // Per-learner constant block (device copy lives in the handle).
 struct StepConst {
   int B, obs, act, T, xw;         // obs = raw observation width (state + one-hot); xw = in_w + act
@@ -23,14 +34,19 @@ struct StepConst {
   int care;
   int ldxa, ldx;                  // row pitches of XA ([2B][in_w]) and of XQ/XT/XP/dx ([B][xw]): multiples of 4 floats
   int Ha, Hc;                     // last hidden widths (actor / critic)
-  float gamma, reward_scale, action_scale;
+  float action_scale;
   float c_loss;                   // 1/B or 1/B^2 (weighted_loss)
   float inv_B;
-  float tau, one_minus_tau;
   float hbar;                     // -act
-  double lr_actor, lr_critic, lr_alpha, beta1, beta2, adam_eps;
+  double beta1, beta2, adam_eps;
   unsigned long long seed;
+  const HParams* hp;              // [R] per-replica hyperparameters
+  // Keeps sizeof(StepConst) at 136 bytes, so that the kernel arguments behind it keep their parameter-space offsets.
+  // ptxas schedules a kernel differently when those move, even one that never reads the table: 32 bytes less cost the
+  // policy head ~1.2 us per step of the 400-wide learners on an H100.
+  unsigned long long reserved[4];
 };
+static_assert(sizeof(StepConst) == 136, "StepConst size moves the offsets of the kernel arguments behind it");
 
 // Mutable per-replica counters in device memory: v[0..2] Adam steps critic/actor/alpha, v[3] step index;
 // b1p/b2p[i] = beta^v[i], kept as running products so no kernel needs a double-precision pow().
@@ -437,6 +453,11 @@ __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   // per-row scalars and the four heads' operands are all requested before anything is consumed
   const int t = (P.tid + rep * P.rsR)[row];
   const float r = (P.r + rep * P.rsR)[row], d = (P.d + rep * P.rsR)[row];
+  // the row's TD-target terms rs*r and gamma*(1-d) are formed as soon as their operands land: holding gamma and rs next
+  // to r and d across the dot products would take two more registers, which this 32-register kernel pays for by
+  // serialising the loads of a head
+  const float t1 = K.hp[rep].reward_scale * r;
+  const float t2 = K.hp[rep].gamma * (1.f - d);
   const float lp = (P.logp + rep * P.rsLogp)[row];
   const float b_t1 = (P.bt[0] + po)[0], b_t2 = (P.bt[1] + po)[0], b_q1 = (P.bq[0] + po)[0], b_q2 = (P.bq[1] + po)[0];
   const float p_t1 = warp_dot_partial(hT, P.Wt[0] + po, H, lane), p_t2 = warp_dot_partial(hT + P.rsHnet, P.Wt[1] + po, H, lane);
@@ -445,8 +466,6 @@ __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   const float qt1 = warp_sum(p_t1) + b_t1, qt2 = warp_sum(p_t2) + b_t2, q1 = warp_sum(p_q1) + b_q1, q2 = warp_sum(p_q2) + b_q2;
   if (lane == 0) {
     const float alpha = (float)exp((double)la_t);
-    const float t1 = K.reward_scale * r;
-    const float t2 = K.gamma * (1.f - d);
     const float t3 = fminf(qt1, qt2) - alpha * lp;
     const float y = t1 + t2 * t3;
     const float e1 = y - q1, e2 = y - q2;
@@ -845,10 +864,8 @@ struct AdamArgs {
   long long rsP, rsM;                                // replica strides: param arena / trainable arena
   long long n;
   long long target_delta;                            // p[i + target_delta] is the Polyak target (0 = none)
-  long long tau2_begin;                              // elements i >= tau2_begin use (tau2, 1 - tau2): CARE state encoder
-  float tau2, one_minus_tau2;
-  int which;                                         // counter index (0 critic, 1 actor)
-  double lr;
+  long long tau2_begin;                              // elements i >= tau2_begin use the replica's tau_se: CARE state encoder
+  int which;                                         // counter / learning-rate slot (0 critic, 1 actor, 4 context encoder)
   const Counters* cnt;
   int tail;
   // tail inputs
@@ -879,13 +896,17 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   KStamp ks_;
   const int rep = blockIdx.y;
   __shared__ float red[256];
-  __shared__ float s_ss, s_bc;
+  __shared__ float s_ss, s_bc, s_tau[4];
   const bool is_tail = (P.tail != TAIL_NONE) && (blockIdx.x == gridDim.x - 1);
   if (!is_tail) {
     if (threadIdx.x == 0) {
+      const HParams& H = K.hp[rep];
       float a, b;
-      adam_scalars(P.lr, P.cnt[rep].b1p[P.which], P.cnt[rep].b2p[P.which], a, b);
+      adam_scalars(H.lr[P.which], P.cnt[rep].b1p[P.which], P.cnt[rep].b2p[P.which], a, b);
       s_ss = a; s_bc = b;
+      // Polyak rates: (tau, 1 - tau) of the target critics, then of the CARE state encoder.  Read from shared memory in
+      // the loop: four more live registers would cost this kernel a resident CTA per SM.
+      s_tau[0] = H.tau; s_tau[1] = H.one_minus_tau; s_tau[2] = H.tau_se; s_tau[3] = H.one_minus_tau_se;
     }
     __syncthreads();
     const float step_size = s_ss, bc2_sqrt = s_bc;
@@ -929,7 +950,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       p4[i] = pv; m4[i] = mv; v4[i] = vv;
       if (t4) {
         const bool second = (i << 2) >= P.tau2_begin;         // tau2_begin is a multiple of 4 (tensor offsets are)
-        const float ta = second ? P.tau2 : K.tau, tb = second ? P.one_minus_tau2 : K.one_minus_tau;
+        const float ta = s_tau[second ? 2 : 0], tb = s_tau[second ? 3 : 1];
         tv.x = ta * pv.x + tb * tv.x; tv.y = ta * pv.y + tb * tv.y;
         tv.z = ta * pv.z + tb * tv.z; tv.w = ta * pv.w + tb * tv.w;
         t4[i] = tv;
@@ -967,7 +988,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
     __shared__ float s_la[64], s_m[64], s_v[64];
     // everything the serial part needs is requested up front, next to the reduction inputs
     if (tid < Teff) { s_la[tid] = la[tid]; s_m[tid] = (P.m_alpha + rep * P.rsM)[tid]; s_v[tid] = (P.v_alpha + rep * P.rsM)[tid]; }
-    const double b1p = P.cnt[rep].b1p[2], b2p = P.cnt[rep].b2p[2];
+    const double b1p = P.cnt[rep].b1p[2], b2p = P.cnt[rep].b2p[2], lr_alpha = K.hp[rep].lr[2];
     float s = 0.f, e = 0.f;
     for (int i = tid; i < B; i += 256) {
       s += (P.la + rep * P.rsY)[i];
@@ -990,7 +1011,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       L[3] = 0.5f * K.act * (1.0f + 1.8378770664093453f) + e * K.inv_B;   // 0.5 A (1+log 2pi) + mean(sum log_std)
       LH[1] = L[1]; LH[3] = L[3];
       float ss, bc;
-      adam_scalars(K.lr_alpha, b1p, b2p, ss, bc);
+      adam_scalars(lr_alpha, b1p, b2p, ss, bc);
       float aloss = 0.f;
       for (int t = 0; t < Teff; ++t) {
         const float grad = -s_gs[t] * K.inv_B;         // d/dlog_alpha[t] of -mean(log_alpha_i (logp_i + Hbar))
@@ -1006,15 +1027,20 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   }
 }
 
-// Stand-alone Polyak (Learner.soft_update outside a step; tau = 1 -> hard copy).
+// Stand-alone Polyak (Learner.soft_update outside a step; tau = 1 -> hard copy).  Elements i >= n_tau1 >= 0 (the CARE
+// state encoder) use the replica's tau_se.
 __global__ void polyak_kernel(float* p, long long rsP, long long n, long long target_delta, float tau,
-                              float one_minus_tau, long long n_tau1 = -1, float tau2 = 0.f, float one_minus_tau2 = 0.f) {
+                              float one_minus_tau, long long n_tau1 = -1, const HParams* hp = nullptr) {
   float* q = p + blockIdx.y * rsP;
+  const float tau2 = n_tau1 >= 0 ? hp[blockIdx.y].tau_se : 0.f, one_minus_tau2 = n_tau1 >= 0 ? hp[blockIdx.y].one_minus_tau_se : 0.f;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
     const bool second = n_tau1 >= 0 && i >= n_tau1;
     q[i + target_delta] = second ? tau2 * q[i] + one_minus_tau2 * q[i + target_delta] : tau * q[i] + one_minus_tau * q[i + target_delta];
   }
 }
+
+// b200sac_set_hparams: one replica's row, written in stream order (a kernel argument, so it is also capturable)
+__global__ void set_hparams_kernel(HParams* hp, int replica, HParams row) { hp[replica] = row; }
 
 // randn init of the mixture-of-encoders weights (state_encoder.py:146-153)
 __global__ void randn_kernel(float* w, long long rsP, long long n, unsigned long long seed, int tag) {

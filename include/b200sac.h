@@ -19,6 +19,9 @@
  *                            build_model/build_optimizer/get_parameters/save_checkpoint
  *                            LunarLander_Distributed_SAC/src/learner.py:100-124,144-163,272-276
  *   b200sac_soft_update      Learner.soft_update()            learner.py:126-137
+ *   b200sac_get/set_hparams, b200sac_copy_replica
+ *                            the hyperparameters build_optimizer / update_SAC / soft_update fix per learner, made per replica
+ *                            LunarLander_Distributed_SAC/src/learner.py:115-137,210; MT10_Distributed_CARE/src/learner.py:136-158,361-367
  *   b200sac_publish_*        Learner.get_parameters()         learner.py:272-276 (called at :298-299)
  *   b200sac_blob_*           server.set('parameters', _pickle.dumps(get_parameters())) in Learner.run()
  *                            learner.py:298-299 (MT10_Distributed_CARE/src/learner.py:442-443): the byte string, device-assembled
@@ -135,6 +138,31 @@ int b200sac_arena_ptr(b200sac_t* h, int32_t which, float** dev_ptr, int64_t* flo
 /* Adam step counters {critic, actor, alpha, context encoder (CARE(O), else unused)} of one replica. */
 int b200sac_get_steps(b200sac_t* h, int32_t replica, int64_t steps[4]);
 int b200sac_set_steps(b200sac_t* h, int32_t replica, const int64_t steps[4]);
+
+/* Per-replica hyperparameters.  The reference fixes them when it builds a learner: the TD target and the Polyak rate
+ * (LunarLander_Distributed_SAC/src/learner.py:126-137,210; MT10_Distributed_CARE/src/learner.py:361-367 with
+ * state_encoder_tau) and the Adam learning rates (LunarLander_Distributed_SAC/src/learner.py:115-124;
+ * MT10_Distributed_CARE/src/learner.py:136-158).  Here every replica of a handle has its own row, initialised from the
+ * cfg by b200sac_create, so co-scheduled learners can sweep them (e.g. population-based training) and a schedule can
+ * change them between steps.  action_scale, the Adam betas / eps and the target entropy stay per handle. */
+typedef struct b200sac_hparams {
+  double gamma, reward_scale, tau;          /* TD target; Polyak rate of the target critics */
+  double lr_critic, lr_actor, lr_alpha;     /* Adam learning rates */
+  double tau_se, lr_ctx;                    /* CARE: state-encoder Polyak rate; CARE(O) context-encoder lr (ignored otherwise) */
+} b200sac_hparams;
+
+/* The values last set for `replica` (host mirror: does not synchronise). */
+int b200sac_get_hparams(b200sac_t* h, int32_t replica, b200sac_hparams* out);
+/* Enqueued on `stream`: applies to every step enqueued after it and to none enqueued before it, including between
+ * launches of the graphs b200sac_prepare instantiated (no graph is rebuilt).  Every value must be finite,
+ * 0 <= tau, tau_se <= 1 and learning rates >= 0; otherwise B200SAC_ERR_INVALID and nothing changes.  b200sac_soft_update
+ * uses the replica's tau_se for the CARE state encoder. */
+int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp, void* stream);
+/* Enqueued on `stream`: replica `dst`'s learner state becomes a copy of `src`'s -- the whole parameter arena (targets,
+ * log_alpha and the CARE embedding included), Adam m and v and the step counters -- device to device, without a host
+ * round trip (the exploit step of population-based training).  Hyperparameters, gradients and replay rings are not
+ * copied. */
+int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream);
 
 /* One gradient step from caller-provided DEVICE minibatches, each
  * [replicas][batch][width] fp32: s,s2 width obs(=state_dim+num_tasks), a width act, r,d width 1.
