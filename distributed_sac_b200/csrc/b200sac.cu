@@ -17,6 +17,7 @@
 #include <random>
 #include <string>
 #include <tuple>
+#include <type_traits>
 #include <unordered_set>
 #include <vector>
 
@@ -332,8 +333,8 @@ struct b200sac {
   int64_t blob_bytes = 0, blob_nf = 0;
   int blob_replica = 0, blob_head = 0, blob_pending = 0;
   cudaEvent_t ev_blob_snap[2] = {nullptr, nullptr}, ev_blob_done[2] = {nullptr, nullptr};
-  CUtensorMap* d_wmaps = nullptr; // layer-chained plan: 2-D maps of the weight-gradient operands, [R][maps per learner]
-  CUtensorMap* d_cmaps = nullptr; // layer-chained plan: 2-D tensor maps of the forward weight matrices, [R][maps per learner]
+  CUtensorMap* d_cmaps = nullptr; // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
+                                  // weight-gradient operands [R][nw]
   long long* chain_dbg = nullptr; // B200SAC_CHAIN_DBG=1: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
   float* split_d = nullptr;       // b200sac_step: handle-owned copy of the caller's minibatch arrays (stable graph pointers)
   float* loss_h = nullptr;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
@@ -399,7 +400,6 @@ static int destroy_impl(b200sac* h) {
   cudaFree(h->split_d);
   cudaFree(h->chain_dbg);
   cudaFree(h->d_cmaps);
-  cudaFree(h->d_wmaps);
   if (h->side) cudaStreamDestroy(h->side);
   if (h->fork) cudaStreamDestroy(h->fork);
   if (h->ev_ingested) cudaEventDestroy(h->ev_ingested);
@@ -543,13 +543,12 @@ static int make_tc_prob(const GemmProb& p, int rep, TcProb& t, int bn = 64) {
 }
 
 // ------------------------------------------------------------------------------------------
-// Layer-chained plan (chain.cuh): 10 launches per step instead of one per layer.
-//   A   forward  {actor on [s';s], Q1, Q2 on (s,a)}  -> policy head / scalar heads
-//   B   forward  {Qt1, Qt2 on (s',a')}               -> scalar heads
-//   C   backward {Q1, Q2}: y, dQ from the per-row scalars, input-gradient chain   -> wgrad -> adam_critic+polyak
-//   D1  forward  {Q1, Q2 on (s,a~)} with the updated critics
-//   D2  backward {Q1, Q2}: min routing, input-gradient chain down to d(action)
-//   E   backward {actor}: d(mu|log_std), input-gradient chain                     -> wgrad -> adam_actor+alpha
+// Layer-chained plan (chain.cuh, chain2.cuh): 7 launches per step after the ingest, whatever the depth of the networks.
+//   A   chain_kernel<FWD>  {actor on [s';s], Q1, Q2 on (s,a)}  -> policy head / scalar heads
+//   BC  chain2_kernel      {Qt1, Qt2 on (s',a')} -> y, dQ -> input-gradient chain of {Q1, Q2}   -> wgrad + Adam + Polyak
+//   D   chain2_kernel      {Q1, Q2 on (s,a~)} with the updated critics -> min routing -> input-gradient chain down to d(action)
+//                          (forked beside E: actor loss, entropy, temperature gradient + its Adam)
+//   E   chain_kernel<BWD>  {actor}: d(mu|log_std), input-gradient chain                          -> wgrad + Adam
 // Eligible: exact-fp32 mode, no CARE, every hidden width a multiple of 4 and <= 256, obs+act <= 252.
 // ------------------------------------------------------------------------------------------
 static bool fused_eligible(const b200sac_cfg& c) {
@@ -561,7 +560,25 @@ static bool fused_eligible(const b200sac_cfg& c) {
   return true;
 }
 
-static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& adam) {
+// Rows per CTA (8, 4 or 2) of a chain launch of `groups` x ceil(rows / ROWS) CTAs per replica.  Every CTA streams the whole
+// weight matrices whatever its row count, so fewer rows per CTA only pay while the launch still fits the GPU: the fewest
+// rows whose launch stays within one wave (one CTA per SM).
+static int chain_rows(long long rows, int groups, int R, int sms) {
+  int bn = 8;
+  for (int r = 4; r >= 2; r >>= 1)
+    if (groups * ((rows + r - 1) / r) * R <= sms) bn = r;
+  return bn;
+}
+
+// f(std::integral_constant<int, ROWS>) for the rows per CTA of a chain launch
+template <typename F>
+static auto with_chain_rows(int bn, F&& f) {
+  if (bn == 8) return f(std::integral_constant<int, 8>{});
+  if (bn == 4) return f(std::integral_constant<int, 4>{});
+  return f(std::integral_constant<int, 2>{});
+}
+
+static int build_plan_fused(b200sac* h, const std::function<void(int, bool)>& adam) {
   const b200sac_cfg& c = h->cfg;
   const Layout& L = h->L;
   const int B = c.batch, R = h->R, A = c.act_dim, sms = sm_count();
@@ -569,15 +586,13 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& ada
   const long long rsP = L.arena, rsG = L.trainable;
   auto W = [&](int64_t off) { return h->params + off; };
   auto Gp = [&](int64_t off) { return h->grads + off; };
-  const int Hc = c.critic_hidden[Lc - 1], Ha = c.actor_hidden[La - 1];
 
   ChainRows rw;
   memset(&rw, 0, sizeof(rw));
   rw.r = h->r.p; rw.d = h->d.p; rw.tid = (const int*)h->tid.p; rw.rsR = h->r.rs;
   rw.logp = h->logp.p; rw.rsLogp = h->logp.rs;
-  rw.log_alpha = W(L.off_alpha);
   rw.alpha = h->alpha.p; rw.rsAlpha = h->alpha.rs;
-  rw.qt = h->qt.p; rw.q = h->q.p; rw.qp = h->qp.p;
+  rw.q = h->q.p;
   rw.y = h->y.p; rw.dq = h->dq.p; rw.lq = h->lq.p; rw.dqa = h->dqa.p; rw.la = h->la.p; rw.qmin = h->qmin.p; rw.rsY = h->y.rs;
   rw.dxP = h->dxP.p; rw.rsDxNet = (long long)B * h->K.ldx; rw.rsDxRep = h->dxP.rs; rw.lddx = h->K.ldx;
   rw.psave = h->psave.p + (long long)B * A * kSaveW; rw.rsSave = h->psave.rs;
@@ -587,12 +602,49 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& ada
   std::vector<WMap> wmaps;                 // weight-gradient operands [B rows][cols] that get a tensor map
   struct FMap { int64_t off; int K, N, ld; };
   std::vector<FMap> fmaps;                 // forward weight matrices that need a tensor map (one per chained forward stage)
-  auto new_chain = [&](const char* label, int early_weights = 1) {
+  if (getenv("B200SAC_CHAIN_DBG")) {
+    CU(cudaMalloc(&h->chain_dbg, sizeof(long long) * CH_DBG_SLOTS * 16));
+    CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
+  }
+  auto dbg_slot = [&]() { return (h->chain_dbg && h->plan.size() < 16) ? h->chain_dbg + h->plan.size() * CH_DBG_SLOTS : nullptr; };
+
+  // Stage tables of one MLP.  Forward: input rows X, hidden layers 0..nh-1, outputs stored to store[l] from row store_row.
+  // Backward (input-gradient chain dh_{l-1} = (dh_l W_l) * [h_{l-1} > 0], l = nh-1 .. 1): gate activations acts[l] and
+  // the gate of the generated dY from row act_row, stores dstore[l] (nullable) from row drow.  J is a ChainJob or a Chain2Job.
+  auto fwd_stages = [&](auto& J, ChainStage* st, const std::vector<LayerOff>& net, int nh, const float* X, long long rsX, int ldx, int K0,
+                        const std::vector<Buf>* store, long long store_row) {
+    J.X = X; J.rsX = rsX; J.ldx = ldx; J.K0 = K0;
+    for (int lyr = 0; lyr < nh; ++lyr) {
+      const LayerOff& lo = net[lyr];
+      ChainStage& S = st[lyr];
+      S.W = W(lo.w); S.bias = W(lo.b); S.ldw = lo.ld; S.K = lo.in; S.N = lo.out;
+      S.tm_idx = (int)fmaps.size();
+      fmaps.push_back(FMap{lo.w, lo.in, lo.out, lo.ld});
+      if (store) { S.out = (*store)[lyr].p + store_row * lo.out; S.rsOut = (*store)[lyr].rs; S.ldo = lo.out; }
+    }
+  };
+  auto bwd_stages = [&](auto& J, ChainStage* st, const std::vector<LayerOff>& net, int nh, const std::vector<Buf>& acts, long long act_row,
+                        const std::vector<Buf>* dstore, long long drow) {
+    const int Hl = net[nh - 1].out;
+    J.hlast = acts[nh - 1].p + act_row * Hl; J.rsHlast = acts[nh - 1].rs; J.ldh = Hl;
+    if (dstore) { J.dylast = (*dstore)[nh - 1].p + drow * Hl; J.rsDy = (*dstore)[nh - 1].rs; J.lddy = Hl; }
+    for (int s = 0; s + 1 < nh; ++s) {
+      const int lyr = nh - 1 - s;
+      const LayerOff& lo = net[lyr];
+      ChainStage& S = st[s];
+      S.W = W(lo.w); S.ldw = lo.ld; S.K = lo.out; S.N = lo.in;
+      S.mask = acts[lyr - 1].p + act_row * lo.in; S.rsMask = acts[lyr - 1].rs; S.ldmask = lo.in;
+      if (dstore) { S.out = (*dstore)[lyr - 1].p + drow * lo.in; S.rsOut = (*dstore)[lyr - 1].rs; S.ldo = lo.in; }
+    }
+  };
+  // chain_kernel launch; its jobs are filled by the caller, then finish_chain sizes the grid
+  auto new_chain = [&](const char* label, int njobs, int early_weights) {
     Launch l;
     l.kind = L_CHAIN;
     l.label = label;
     memset(&l.chain, 0, sizeof(l.chain));
-    l.chain.early_weights = (early_weights && getenv("B200SAC_NO_EARLY_WEIGHTS") == nullptr) ? 1 : 0;
+    l.chain.njobs = njobs;
+    l.chain.early_weights = early_weights;
     l.chain.rsP = rsP;
     l.chain.pol = h->pol;
     l.chain.rw = rw;
@@ -600,82 +652,68 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& ada
     l.smem = CH_SMEM_BYTES;
     return l;
   };
-  if (getenv("B200SAC_CHAIN_DBG")) {
-    CU(cudaMalloc(&h->chain_dbg, sizeof(long long) * CH_DBG_SLOTS * 16));
-    CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
-  }
   auto finish_chain = [&](Launch& l) {
-    if (h->chain_dbg && h->plan.size() < 16) l.chain.dbg = h->chain_dbg + h->plan.size() * CH_DBG_SLOTS;
-    // rows per CTA: every CTA streams the whole weight matrices whatever its row count, so fewer rows per CTA only pay
-    // while the launch still fits the GPU: 8 rows when that already gives >= 96 CTAs, else 4 (twice the CTAs, half the math each)
+    l.chain.dbg = dbg_slot();
     long long total = 0;
-    for (int j = 0; j < l.chain.njobs; ++j) total += l.chain.job[j].rows;
-    l.bn = 8;                                      // (bn is reused as "rows per CTA" for chain launches)
-    for (int rows = 4; rows >= 2; rows >>= 1)      // the fewest rows per CTA whose launch still fits one wave (one CTA per SM)
-      if ((total + rows - 1) / rows * R <= sms) l.bn = rows;
-    if (const char* e = getenv("B200SAC_CHAIN_ROWS")) { const int v = atoi(e); l.bn = (v == 2 || v == 4) ? v : 8; }
-    int maxb = 1;
+    int maxrows = 0;
     for (int j = 0; j < l.chain.njobs; ++j) {
-      const int nb = (l.chain.job[j].rows + l.bn - 1) / l.bn;
-      maxb = nb > maxb ? nb : maxb;
+      total += l.chain.job[j].rows;
+      maxrows = std::max(maxrows, l.chain.job[j].rows);
     }
-    l.grid = dim3(maxb, l.chain.njobs, R);
+    l.bn = chain_rows(total, 1, R, sms);           // (bn is reused as "rows per CTA" for chain launches)
+    l.grid = dim3(std::max(1, (maxrows + l.bn - 1) / l.bn), l.chain.njobs, R);
     h->plan.push_back(l);
   };
-  // forward job of one MLP: input rows X, per-layer stores `store[l]` (+ net offset), head
-  auto fwd_job = [&](ChainJob& J, const std::vector<LayerOff>& net, int nh, const float* X, long long rsX, int ldx, int K0, int rows,
-                     const std::vector<Buf>* store, int net_idx, int rows_per_net) {
-    memset(&J, 0, sizeof(J));
-    J.kind = CJ_FWD; J.rows = rows; J.nstages = nh; J.net = net_idx;
-    J.X = X; J.rsX = rsX; J.ldx = ldx; J.K0 = K0;
-    for (int l = 0; l < nh; ++l) {
-      const LayerOff& lo = net[l];
-      ChainStage& S = J.st[l];
-      S.W = W(lo.w); S.bias = W(lo.b); S.ldw = lo.ld; S.K = lo.in; S.N = lo.out;
-      S.tm_idx = (int)fmaps.size();
-      fmaps.push_back(FMap{lo.w, lo.in, lo.out, lo.ld});
-      if (store) { S.out = (*store)[l].p + (long long)net_idx * rows_per_net * lo.out; S.rsOut = (*store)[l].rs; S.ldo = lo.out; }
+  // chain2_kernel launch: forward of the twins fnet[0..1] on X, their head values swapped, backward of the local critics
+  auto pair_launch = [&](const char* label, int kind, int early, const std::vector<LayerOff>* fnet /* [2] */, const float* X, long long rsX,
+                         const std::vector<Buf>* fstore, const Buf& qf, const std::vector<Buf>& acts, const std::vector<Buf>* dstore,
+                         bool tail) {
+    Launch l;
+    l.kind = L_CHAIN2;
+    l.label = label;
+    memset(&l.chain2, 0, sizeof(l.chain2));
+    Chain2Args& P = l.chain2;
+    P.kind = kind; P.rsP = rsP; P.rw = rw;
+    P.early_weights = early;
+    for (int net = 0; net < 2; ++net) {
+      Chain2Job& J = P.job[net];
+      J.rows = B; J.nfwd = Lc; J.nbwd = Lc - 1; J.net = net;
+      fwd_stages(J, J.st, fnet[net], Lc, X, rsX, h->K.ldx, h->K.xw, fstore, (long long)net * B);
+      const LayerOff& fh = fnet[net][Lc];
+      J.Whf = W(fh.w); J.bhf = W(fh.b); J.Hhf = fh.in;
+      J.qf_out = qf.p + (long long)net * B; J.rsQf = qf.rs;
+      // backward through the LOCAL twin
+      const std::vector<LayerOff>& bn = L.q[net];
+      bwd_stages(J, J.st + Lc, bn, Lc, acts, (long long)net * B, dstore, (long long)net * B);
+      J.Whb = W(bn[Lc].w); J.Hhb = bn[Lc].in;
+      if (tail) {
+        const LayerOff& lo = bn[0];
+        J.W0 = W(lo.w); J.ldw0 = lo.ld; J.col0 = h->K.in_w; J.nact = A; J.H0 = lo.out;
+        J.dx = h->dxP.p + (long long)net * B * h->K.ldx; J.rsDx = h->dxP.rs; J.lddx = h->K.ldx;
+      }
     }
-    const LayerOff& hd = net[nh];
-    J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
+    P.dbg = dbg_slot();
+    l.bn = chain_rows(B, 2, R, sms);
+    l.grid = dim3((B + l.bn - 1) / l.bn, 2, R);
+    l.block = dim3(CH_BLOCK);
+    l.smem = C2_SMEM_BYTES;
+    h->plan.push_back(l);
   };
-  // backward job of one MLP (input-gradient chain): gate activations acts[l], stores dstore[l] (nullable)
-  auto bwd_job = [&](ChainJob& J, int kind, const std::vector<LayerOff>& net, int nh, int rows, const std::vector<Buf>& acts,
-                     long long act_row_off /* rows to skip in acts */, const std::vector<Buf>* dstore, int net_idx) {
-    memset(&J, 0, sizeof(J));
-    J.kind = kind; J.rows = rows; J.nstages = nh - 1; J.net = net_idx;
-    const LayerOff& hd = net[nh];
-    J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
-    const int Hl = net[nh - 1].out;
-    J.hlast = acts[nh - 1].p + ((long long)net_idx * rows + act_row_off) * Hl; J.rsHlast = acts[nh - 1].rs; J.ldh = Hl;
-    if (dstore) { J.dylast = (*dstore)[nh - 1].p + (long long)net_idx * rows * Hl; J.rsDy = (*dstore)[nh - 1].rs; J.lddy = Hl; }
-    for (int s = 0; s + 1 < nh; ++s) {
-      const int l = nh - 1 - s;                    // dh_{l-1} = (dh_l W_l) * [h_{l-1} > 0]
-      const LayerOff& lo = net[l];
-      ChainStage& S = J.st[s];
-      S.W = W(lo.w); S.ldw = lo.ld; S.K = lo.out; S.N = lo.in;
-      S.mask = acts[l - 1].p + ((long long)net_idx * rows + act_row_off) * lo.in; S.rsMask = acts[l - 1].rs; S.ldmask = lo.in;
-      if (dstore) { S.out = (*dstore)[l - 1].p + (long long)net_idx * rows * lo.in; S.rsOut = (*dstore)[l - 1].rs; S.ldo = lo.in; }
-    }
-  };
-  // weight-gradient launch of a group of networks
+  // weight-gradient launch of a group of networks; the CTA that reduces a gradient tile applies Adam (+ Polyak) to it
   struct WNet { const std::vector<LayerOff>* net; int nh; const std::vector<Buf>* dstore; const std::vector<Buf>* acts; long long act_row_off;
                 const float* X; long long rsX; int ldx; const float* dout; long long rsDout; int lddout; int net_idx; };
-  const bool fuse_adam = getenv("B200SAC_NO_FUSED_ADAM") == nullptr;
   auto wgrad_launch = [&](const std::vector<WNet>& nets, const char* label, int which) -> int {
     Launch l;
     l.kind = L_WGRAD;
     l.label = label;
     memset(&l.wg, 0, sizeof(l.wg));
     l.wg.M = B; l.wg.rsG = rsG;
-    if (fuse_adam) {                             // the CTA that reduces a gradient tile applies Adam (+ Polyak) to it
-      WgradAdam& O = l.wg.adam;
-      O.enabled = 1; O.which = which;
-      O.params = h->params; O.m = h->adam_m; O.v = h->adam_v; O.grads = h->grads;
-      O.rsP = rsP; O.rsM = rsG;
-      O.target_delta = which == 0 ? L.target_delta : 0;
-      O.cnt = h->cnt;
-    }
+    WgradAdam& O = l.wg.adam;
+    O.which = which;
+    O.params = h->params; O.m = h->adam_m; O.v = h->adam_v; O.grads = h->grads;
+    O.rsP = rsP; O.rsM = rsG;
+    O.target_delta = which == 0 ? L.target_delta : 0;
+    O.cnt = h->cnt;
     int tiles = 0;
     auto add = [&](const float* Ap, long long rsA, int lda, const float* Bp, long long rsB, int ldb, int64_t offW, int ldc, int64_t offB,
                    int Kout, int Nin) -> int {
@@ -715,210 +753,105 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, int)>& ada
     l.grid = dim3(tiles, R);
     l.block = dim3(WG_THREADS);
     l.smem = WG_SMEM_BYTES;
-    if (h->chain_dbg && h->plan.size() < 16) l.wg.dbg = h->chain_dbg + h->plan.size() * CH_DBG_SLOTS;
+    l.wg.dbg = dbg_slot();
     h->plan.push_back(l);
     return 0;
   };
 
   // ---- A: actor over [s';s], Q1/Q2 over (s,a) ----------------------------------------------------------------------
   {
-    Launch l = new_chain("chain_fwd{actor,q1,q2}");
-    l.chain.njobs = 3;
-    fwd_job(l.chain.job[0], L.actor, La, h->XA.p, h->XA.rs, h->K.ldxa, h->K.in_w, 2 * B, &h->hA, 0, 0);
-    l.chain.job[0].head = CH_HEAD_POLICY;
-    for (int net = 0; net < 2; ++net) {
-      ChainJob& J = l.chain.job[1 + net];
-      fwd_job(J, L.q[net], Lc, h->XQ.p, h->XQ.rs, h->K.ldx, h->K.xw, B, &h->hQ, net, B);
-      J.head = CH_HEAD_SCALAR; J.qout = h->q.p + (long long)net * B; J.rsQ = h->q.rs;
+    Launch l = new_chain("chain_fwd{actor,q1,q2}", 3, 1);
+    for (int j = 0; j < 3; ++j) {
+      ChainJob& J = l.chain.job[j];
+      const int net = j - 1;
+      const std::vector<LayerOff>& mlp = j == 0 ? L.actor : L.q[net];
+      const int nh = j == 0 ? La : Lc;
+      J.kind = CJ_FWD; J.nstages = nh;
+      if (j == 0) {
+        J.rows = 2 * B; J.head = CH_HEAD_POLICY;
+        fwd_stages(J, J.st, mlp, nh, h->XA.p, h->XA.rs, h->K.ldxa, h->K.in_w, &h->hA, 0);
+      } else {
+        J.rows = B; J.head = CH_HEAD_SCALAR; J.qout = h->q.p + (long long)net * B; J.rsQ = h->q.rs;
+        fwd_stages(J, J.st, mlp, nh, h->XQ.p, h->XQ.rs, h->K.ldx, h->K.xw, &h->hQ, (long long)net * B);
+      }
+      const LayerOff& hd = mlp[nh];
+      J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
     }
     h->use_eps_buf_idx = (int)h->plan.size();
     finish_chain(l);
   }
-  // Twin forward + backward in one clustered launch (chain2.cuh) when the critic is shallow enough for its stage tables
-  const bool pair = Lc <= C2_MAXL && getenv("B200SAC_NO_CLUSTER") == nullptr;
-  auto pair_launch = [&](const char* label, int kind, int early, const std::vector<LayerOff>* fnet /* [2] */, const float* X, long long rsX,
-                         const std::vector<Buf>* fstore, const Buf& qf, const std::vector<Buf>& acts, const std::vector<Buf>* dstore,
-                         bool tail) {
-    Launch l;
-    l.kind = L_CHAIN2;
-    l.label = label;
-    memset(&l.chain2, 0, sizeof(l.chain2));
-    Chain2Args& P = l.chain2;
-    P.kind = kind; P.rsP = rsP; P.rw = rw;
-    P.early_weights = (early && getenv("B200SAC_NO_EARLY_WEIGHTS") == nullptr) ? 1 : 0;
-    for (int net = 0; net < 2; ++net) {
-      Chain2Job& J = P.job[net];
-      J.rows = B; J.nfwd = Lc; J.nbwd = Lc - 1; J.net = net;
-      J.X = X; J.rsX = rsX; J.ldx = h->K.ldx; J.K0 = h->K.xw;
-      for (int lyr = 0; lyr < Lc; ++lyr) {
-        const LayerOff& lo = fnet[net][lyr];
-        ChainStage& S = J.fst[lyr];
-        S.W = W(lo.w); S.bias = W(lo.b); S.ldw = lo.ld; S.K = lo.in; S.N = lo.out;
-        S.tm_idx = (int)fmaps.size();
-        fmaps.push_back(FMap{lo.w, lo.in, lo.out, lo.ld});
-        if (fstore) { S.out = (*fstore)[lyr].p + (long long)net * B * lo.out; S.rsOut = (*fstore)[lyr].rs; S.ldo = lo.out; }
-      }
-      const LayerOff& fh = fnet[net][Lc];
-      J.Whf = W(fh.w); J.bhf = W(fh.b); J.Hhf = fh.in;
-      J.qf_out = qf.p + (long long)net * B; J.rsQf = qf.rs;
-      // backward through the LOCAL twin
-      const std::vector<LayerOff>& bn = L.q[net];
-      const int Hl = bn[Lc - 1].out;
-      J.hlast = acts[Lc - 1].p + (long long)net * B * Hl; J.rsHlast = acts[Lc - 1].rs; J.ldh = Hl;
-      if (dstore) { J.dylast = (*dstore)[Lc - 1].p + (long long)net * B * Hl; J.rsDy = (*dstore)[Lc - 1].rs; J.lddy = Hl; }
-      J.Whb = W(bn[Lc].w); J.Hhb = bn[Lc].in;
-      for (int sidx = 0; sidx + 1 < Lc; ++sidx) {
-        const int lyr = Lc - 1 - sidx;
-        const LayerOff& lo = bn[lyr];
-        ChainStage& S = J.bst[sidx];
-        S.W = W(lo.w); S.ldw = lo.ld; S.K = lo.out; S.N = lo.in;
-        S.mask = acts[lyr - 1].p + (long long)net * B * lo.in; S.rsMask = acts[lyr - 1].rs; S.ldmask = lo.in;
-        if (dstore) { S.out = (*dstore)[lyr - 1].p + (long long)net * B * lo.in; S.rsOut = (*dstore)[lyr - 1].rs; S.ldo = lo.in; }
-      }
-      if (tail) {
-        const LayerOff& lo = bn[0];
-        J.W0 = W(lo.w); J.ldw0 = lo.ld; J.col0 = h->K.in_w; J.nact = A; J.H0 = lo.out;
-        J.dx = h->dxP.p + (long long)net * B * h->K.ldx; J.rsDx = h->dxP.rs; J.lddx = h->K.ldx;
-      }
-    }
-    if (h->chain_dbg && h->plan.size() < 16) P.dbg = h->chain_dbg + h->plan.size() * CH_DBG_SLOTS;
-    l.bn = 8;
-    for (int rows = 4; rows >= 2; rows >>= 1)
-      if ((long long)2 * ((B + rows - 1) / rows) * R <= sms) l.bn = rows;
-    if (const char* e = getenv("B200SAC_CHAIN_ROWS")) { const int v = atoi(e); l.bn = (v == 2 || v == 4) ? v : 8; }
-    l.grid = dim3((B + l.bn - 1) / l.bn, 2, R);
-    l.block = dim3(CH_BLOCK);
-    l.smem = C2_SMEM_BYTES;
-    h->plan.push_back(l);
-  };
   // ---- B + C: target critics over (s', a'), TD target, critic backward (one clustered launch), weight gradients, Adam ----
-  if (pair) {
-    pair_launch("chain2{qt->y->bwd q}", C2_CRITIC, 1, L.qt, h->XT.p, h->XT.rs, nullptr, h->qt, h->hQ, &h->dhQ, false);
-  } else {
-    {
-      Launch l = new_chain("chain_fwd{qt1,qt2}");
-      l.chain.njobs = 2;
-      for (int net = 0; net < 2; ++net) {
-        ChainJob& J = l.chain.job[net];
-        fwd_job(J, L.qt[net], Lc, h->XT.p, h->XT.rs, h->K.ldx, h->K.xw, B, nullptr, net, B);
-        J.head = CH_HEAD_SCALAR; J.qout = h->qt.p + (long long)net * B; J.rsQ = h->qt.rs;
-      }
-      finish_chain(l);
-    }
-    Launch l = new_chain("chain_bwd{q1,q2}");
-    l.chain.njobs = 2;
-    for (int net = 0; net < 2; ++net) bwd_job(l.chain.job[net], CJ_BWD_CRITIC, L.q[net], Lc, B, h->hQ, 0, &h->dhQ, net);
-    finish_chain(l);
-  }
+  pair_launch("chain2{qt->y->bwd q}", C2_CRITIC, 1, L.qt, h->XT.p, h->XT.rs, nullptr, h->qt, h->hQ, &h->dhQ, false);
   {
     std::vector<WNet> nets;
     for (int net = 0; net < 2; ++net)
       nets.push_back(WNet{&L.q[net], Lc, &h->dhQ, &h->hQ, 0, h->XQ.p, h->XQ.rs, h->K.ldx, h->dq.p + (long long)net * B, h->dq.rs, 1, net});
-    if (int rc = wgrad_launch(nets, fuse_adam ? "wgrad+adam+polyak{q1,q2}" : "wgrad{q1,q2}", 0)) return rc;
-    if (!fuse_adam) adam(0, 0);
+    if (int rc = wgrad_launch(nets, "wgrad+adam+polyak{q1,q2}", 0)) return rc;
   }
   // ---- D: actor pass through the updated critics ------------------------------------------------------------------------
+  // (the launch right before this one is the critic Adam: no weight request before the dependency wait)
+  pair_launch("chain2{q(s,a~)->min->bwd->d(action)}", C2_ACTORQ, 0, L.q, h->XP.p, h->XP.rs, &h->hP, h->qp, h->hP, nullptr, true);
+  // actor loss / entropy / temperature gradient + its Adam step need only what D produced (the step's alpha is the
+  // snapshot taken at ingest): they run on the fork stream beside the policy backward instead of trailing the actor Adam
+  adam(1, true);
+  // ---- E: policy backward, weight gradients, Adam ----------------------------------------------------------------------
   {
-    if (pair) {
-      // (the launch right before this one is the critic Adam: no weight request before the dependency wait)
-      pair_launch("chain2{q(s,a~)->min->bwd->d(action)}", C2_ACTORQ, 0, L.q, h->XP.p, h->XP.rs, &h->hP, h->qp, h->hP, nullptr, true);
-    } else {
-      // (the launch right before this one is the critic Adam: no weight request before the dependency wait)
-      Launch l = new_chain("chain_fwd{q1,q2}(s,a~)", 0);
-      l.chain.njobs = 2;
-      for (int net = 0; net < 2; ++net) {
-        ChainJob& J = l.chain.job[net];
-        fwd_job(J, L.q[net], Lc, h->XP.p, h->XP.rs, h->K.ldx, h->K.xw, B, &h->hP, net, B);
-        J.head = CH_HEAD_SCALAR; J.qout = h->qp.p + (long long)net * B; J.rsQ = h->qp.rs;
-      }
-      finish_chain(l);
-      Launch l2 = new_chain("chain_bwd{q1,q2}->d(action)");
-      l2.chain.njobs = 2;
-      for (int net = 0; net < 2; ++net) {
-        ChainJob& J = l2.chain.job[net];
-        bwd_job(J, CJ_BWD_ACTORQ, L.q[net], Lc, B, h->hP, 0, nullptr, net);
-        const LayerOff& lo = L.q[net][0];
-        J.head = CH_TAIL_DACTION;
-        J.W0 = W(lo.w); J.ldw0 = lo.ld; J.col0 = h->K.in_w; J.nact = A; J.H0 = lo.out;
-        J.dx = h->dxP.p + (long long)net * B * h->K.ldx; J.rsDx = h->dxP.rs; J.lddx = h->K.ldx;
-      }
-      finish_chain(l2);
-    }
-    // actor loss / entropy / temperature gradient + its Adam step need only what D produced (the step's alpha is the
-    // snapshot taken at ingest): they run on the fork stream beside the policy backward instead of trailing the actor Adam
-    adam(1, fuse_adam ? 3 : 2);
-  }
-  // ---- E: policy backward, weight gradients, Adam + temperature ------------------------------------------------------------
-  {
-    Launch l = new_chain("chain_bwd{actor}");
-    l.chain.njobs = 1;
-    bwd_job(l.chain.job[0], CJ_BWD_POLICY, L.actor, La, B, h->hA, B, &h->dhA, 0);
+    Launch l = new_chain("chain_bwd{actor}", 1, 1);
+    ChainJob& J = l.chain.job[0];
+    J.kind = CJ_BWD_POLICY; J.rows = B; J.nstages = La - 1;
+    const LayerOff& hd = L.actor[La];
+    J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
+    bwd_stages(J, J.st, L.actor, La, h->hA, (long long)B, &h->dhA, 0);
     finish_chain(l);
     std::vector<WNet> nets;
     nets.push_back(WNet{&L.actor, La, &h->dhA, &h->hA, (long long)B, h->XA.p + (long long)B * h->K.ldxa, h->XA.rs, h->K.ldxa,
                         h->dout_dbg.p, h->dout_dbg.rs, 2 * A, 0});
-    if (int rc = wgrad_launch(nets, fuse_adam ? "wgrad+adam{actor}" : "wgrad{actor}", 1)) return rc;
-    if (!fuse_adam) adam(1, 1);
+    if (int rc = wgrad_launch(nets, "wgrad+adam{actor}", 1)) return rc;
   }
-  (void)Hc; (void)Ha;
-  {  // tensor maps [R][n]: W [N][K] row-major (pitch ld), box {32 k, N rows}, SWIZZLE_128B, OOB k zero-filled
-    const int n = (int)fmaps.size();
-    std::vector<CUtensorMap> maps((size_t)R * n);
-    for (int rep = 0; rep < R; ++rep)
-      for (int i = 0; i < n; ++i)
-        if (int rc = make_map(&maps[(size_t)rep * n + i], h->params + (long long)rep * rsP + fmaps[i].off, fmaps[i].K, fmaps[i].N,
-                              fmaps[i].ld, fmaps[i].N))
-          return rc;
-    CU(cudaMalloc(&h->d_cmaps, maps.size() * sizeof(CUtensorMap)));
-    CU(cudaMemcpy(h->d_cmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    for (auto& l : h->plan) {
-      if (l.kind == L_CHAIN)
-        for (int j = 0; j < l.chain.njobs; ++j)
-          if (l.chain.job[j].kind == CJ_FWD)
-            for (int st = 0; st < l.chain.job[j].nstages; ++st) {
-              ChainStage& S = l.chain.job[j].st[st];
-              S.tm = h->d_cmaps + S.tm_idx;
-              S.rsTm = n;
-            }
-      if (l.kind == L_CHAIN2)
-        for (int j = 0; j < 2; ++j)
-          for (int st = 0; st < l.chain2.job[j].nfwd; ++st) {
-            ChainStage& S = l.chain2.job[j].fst[st];
-            S.tm = h->d_cmaps + S.tm_idx;
-            S.rsTm = n;
-          }
-    }
+  // ---- tensor maps ---------------------------------------------------------------------------------------------------
+  // forward weights [R][nf]: W [N][K] row-major (pitch ld), box {32 k, N rows}, SWIZZLE_128B, OOB k zero-filled;
+  // weight-gradient operands [R][nw]: [B rows][cols] row-major, box {32 cols, 256 rows}, dense
+  const int nf = (int)fmaps.size(), nw = (int)wmaps.size();
+  std::vector<CUtensorMap> maps((size_t)R * (nf + nw));
+  for (int rep = 0; rep < R; ++rep) {
+    for (int i = 0; i < nf; ++i)
+      if (int rc = make_map(&maps[(size_t)rep * nf + i], h->params + (long long)rep * rsP + fmaps[i].off, fmaps[i].K, fmaps[i].N,
+                            fmaps[i].ld, fmaps[i].N))
+        return rc;
+    for (int i = 0; i < nw; ++i)
+      if (int rc = make_map(&maps[(size_t)R * nf + (size_t)rep * nw + i], wmaps[i].p + (long long)rep * wmaps[i].rs, wmaps[i].cols, B,
+                            wmaps[i].ld, WG_ROWS, true))
+        return rc;
   }
-  CU(cudaFuncSetAttribute(chain2_kernel<8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain2_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain2_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
-  {  // weight-gradient operand maps [R][n]: [B rows][cols] row-major, box {32 cols, 256 rows}, dense
-    const int n = (int)wmaps.size();
-    std::vector<CUtensorMap> maps((size_t)R * n);
-    for (int rep = 0; rep < R; ++rep)
-      for (int i = 0; i < n; ++i)
-        if (int rc = make_map(&maps[(size_t)rep * n + i], wmaps[i].p + (long long)rep * wmaps[i].rs, wmaps[i].cols, B, wmaps[i].ld, WG_ROWS,
-                              true))
-          return rc;
-    if (n > 0) {
-      CU(cudaMalloc(&h->d_wmaps, maps.size() * sizeof(CUtensorMap)));
-      CU(cudaMemcpy(h->d_wmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-    }
-    for (auto& l : h->plan)
-      if (l.kind == L_WGRAD)
-        for (int j = 0; j < l.wg.njobs; ++j) {
-          WgradJob& J = l.wg.job[j];
-          J.tmA = J.tmA_idx >= 0 ? h->d_wmaps + J.tmA_idx : nullptr;
-          J.tmB = J.tmB_idx >= 0 ? h->d_wmaps + J.tmB_idx : nullptr;
-          J.rsTm = n;
-        }
+  CU(cudaMalloc(&h->d_cmaps, maps.size() * sizeof(CUtensorMap)));
+  CU(cudaMemcpy(h->d_cmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+  const CUtensorMap* fmap = h->d_cmaps;
+  const CUtensorMap* wmap = h->d_cmaps + (size_t)R * nf;
+  auto patch = [&](ChainStage* st, int n) {
+    for (int s = 0; s < n; ++s) { st[s].tm = fmap + st[s].tm_idx; st[s].rsTm = nf; }
+  };
+  for (auto& l : h->plan) {
+    if (l.kind == L_CHAIN && l.chain.job[0].kind == CJ_FWD)
+      for (int j = 0; j < l.chain.njobs; ++j) patch(l.chain.job[j].st, l.chain.job[j].nstages);
+    if (l.kind == L_CHAIN2)
+      for (int j = 0; j < 2; ++j) patch(l.chain2.job[j].st, l.chain2.job[j].nfwd);
+    if (l.kind == L_WGRAD)
+      for (int j = 0; j < l.wg.njobs; ++j) {
+        WgradJob& J = l.wg.job[j];
+        J.tmA = J.tmA_idx >= 0 ? wmap + J.tmA_idx : nullptr;
+        J.tmB = J.tmB_idx >= 0 ? wmap + J.tmB_idx : nullptr;
+        J.rsTm = nw;
+      }
   }
-  CU(cudaFuncSetAttribute(chain_kernel<true, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain_kernel<false, 8>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain_kernel<true, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(chain_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
+  for (int bn : {8, 4, 2})
+    if (int rc = with_chain_rows(bn, [](auto rows) -> int {
+          constexpr int r = decltype(rows)::value;
+          CU(cudaFuncSetAttribute(chain_kernel<true, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
+          CU(cudaFuncSetAttribute(chain_kernel<false, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
+          CU(cudaFuncSetAttribute(chain2_kernel<r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
+          return 0;
+        }))
+      return rc;
   CU(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
   return 0;
 }
@@ -1246,9 +1179,9 @@ static int build_plan(b200sac* h) {
     P.logstd_sum = h->logstd.p;
     P.cnt = h->cnt;
   }
-  // mode 0: parameter update + the tail job (last CTA); 1: parameter update only; 2 / 3: the tail job alone, on the fork
-  // stream (3: + the critic-loss reduction, for plans whose critic Adam is fused into the weight-gradient launch)
-  auto adam = [&](int which, int mode) {
+  // parameter update + the tail job (last CTA); tail_only: the tail job alone, on the fork stream, plus the critic-loss
+  // reduction (the layer-chained plan, whose parameter updates are fused into the weight-gradient launches)
+  auto adam = [&](int which, bool tail_only) {
     Launch l;
     l.kind = L_ADAM;
     AdamArgs& P = l.ad;
@@ -1263,8 +1196,7 @@ static int build_plan(b200sac* h) {
     P.which = which == 2 ? 4 : which;                    // counter slot: 0 critic, 1 actor, 4 context encoder
     P.cnt = h->cnt;
     P.tail = which == 0 ? TAIL_CRITIC_LOSS : (which == 1 ? TAIL_ALPHA_AND_LOSSES : TAIL_NONE);
-    if (mode == 1) P.tail = TAIL_NONE;
-    if (mode == 3) P.tail = TAIL_ALL;              // forked tail that also reduces the critic loss (no critic Adam launch)
+    if (tail_only) P.tail = TAIL_ALL;
     P.lq = h->lq.p; P.la = h->la.p; P.rsY = h->y.rs;
     P.logp_cur = h->logp.p + B; P.logstd_sum = h->logstd.p + B; P.rsLogp = h->logp.rs;
     P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
@@ -1277,7 +1209,7 @@ static int build_plan(b200sac* h) {
     l.grid = dim3(nb + (P.tail != TAIL_NONE ? 1 : 0), R);
     l.block = dim3(256);
     l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
-    if (mode == 2 || mode == 3) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
+    if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
     h->plan.push_back(l);
   };
   if (h->fused) {
@@ -1525,7 +1457,7 @@ static int build_plan(b200sac* h) {
       h->plan.push_back(l2);
     }
   }
-  adam(0, 0);
+  adam(0, false);
   if (c.care) {          // encoded states of s with the UPDATED critic encoder for the actor pass (learner.py:336-341)
     care_tables({2});
     care_encode({EncJob{2, B, B, h->XP.p, h->XP.rs, h->K.ldx, nullptr, 0, 0, 0}});
@@ -1588,8 +1520,8 @@ static int build_plan(b200sac* h) {
       gemm_launch(ps);
     }
   }
-  adam(1, 0);
-  if (c.care == 2) adam(2, 0);        // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
+  adam(1, false);
+  if (c.care == 2) adam(2, false);        // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
   }   // generic (per-layer) plan
 
   if (plan_rc) return plan_rc;
@@ -1720,25 +1652,19 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         ChainArgs a = l.chain;
         a.pol.use_eps_buf = use_eps_buf ? 1 : 0;
         const bool f = a.job[0].kind == CJ_FWD;
-        if (l.bn == 8) {
-          if (f) launch_k(chain_kernel<true, 8>, l.grid, l.block, l.smem, s, a, h->K);
-          else launch_k(chain_kernel<false, 8>, l.grid, l.block, l.smem, s, a, h->K);
-        } else if (l.bn == 4) {
-          if (f) launch_k(chain_kernel<true, 4>, l.grid, l.block, l.smem, s, a, h->K);
-          else launch_k(chain_kernel<false, 4>, l.grid, l.block, l.smem, s, a, h->K);
-        } else {
-          if (f) launch_k(chain_kernel<true, 2>, l.grid, l.block, l.smem, s, a, h->K);
-          else launch_k(chain_kernel<false, 2>, l.grid, l.block, l.smem, s, a, h->K);
-        }
+        with_chain_rows(l.bn, [&](auto rows) {
+          constexpr int r = decltype(rows)::value;
+          return launch_k(f ? chain_kernel<true, r> : chain_kernel<false, r>, l.grid, l.block, l.smem, s, a, h->K);
+        });
         break;
       }
       case L_WGRAD:
         launch_k(wgrad_kernel, l.grid, l.block, l.smem, s, l.wg, h->K);
         break;
       case L_CHAIN2:
-        if (l.bn == 8) launch_pair_k(chain2_kernel<8>, l.grid, l.block, l.smem, s, l.chain2, h->K);
-        else if (l.bn == 4) launch_pair_k(chain2_kernel<4>, l.grid, l.block, l.smem, s, l.chain2, h->K);
-        else launch_pair_k(chain2_kernel<2>, l.grid, l.block, l.smem, s, l.chain2, h->K);
+        with_chain_rows(l.bn, [&](auto rows) {
+          return launch_pair_k(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, h->K);
+        });
         break;
     }
     if (forked) {

@@ -13,16 +13,20 @@
 //             actor pass      min(Q1,Q2) gradient routing                                            learner.py:222-223
 //             policy          closed-form backward of rsample/tanh/log-prob (oracle/sac_manual.py)   model.py:50-60
 //
-// Rows are independent, so nothing is exchanged between CTAs and there is no barrier wider than the CTA.  Every CTA
-// streams the full weight matrices of its network through a 3-stage TMA pipeline of 32-k chunks (32 KB each, landing on
-// mbarriers): forward chunks [<=256 n][32 k] come through a 2-D tensor map with the 128-byte swizzle straight from the
-// nn.Linear-layout matrix (cp.async.bulk.tensor.2d, out-of-range k zero-filled), backward chunks are 32 consecutive rows of
-// the same matrix = one contiguous cp.async.bulk.  One elected thread issues a chunk; nobody's registers or LSU slots are
-// spent on the copy (per-thread cp.async staging costs as much issue as the chunk's math).  The pipeline runs ahead across
-// layer boundaries (weights do not depend on activations); 128 CTAs x 256 KB per 256x256 layer = 32 MB of L2 reads -- the
-// bound of this design.  Inside a chunk the 8 warps split K (warp w takes k = 4w..4w+3 of the 32), each lane holds an 8-row x
-// 8-column accumulator tile (40 shared-memory wavefronts per 256 FFMA), and the eight partial tiles are added in warp
-// order in shared memory: a fixed summation order, bit-reproducible run to run and replica to replica.
+// Two kernels are built from the blocks below: chain_kernel (the forward of the actor and the local critics, the policy
+// backward) and chain2_kernel (chain2.cuh: a twin-critic forward, the per-row scalar that needs both twins, and the
+// backward of one twin, in one launch).
+//
+// Rows are independent, so nothing is exchanged between CTAs (chain2_kernel's twin pair aside) and there is no barrier wider
+// than the CTA.  Every CTA streams the full weight matrices of its network through a 3-stage TMA pipeline of 32-k chunks
+// (32 KB each, landing on mbarriers): forward chunks [<=256 n][32 k] come through a 2-D tensor map with the 128-byte swizzle
+// straight from the nn.Linear-layout matrix (cp.async.bulk.tensor.2d, out-of-range k zero-filled), backward chunks are 32
+// consecutive rows of the same matrix = one contiguous cp.async.bulk.  One elected thread issues a chunk; nobody's registers
+// or LSU slots are spent on the copy (per-thread cp.async staging costs as much issue as the chunk's math).  The pipeline runs
+// ahead across layer boundaries (weights do not depend on activations); 128 CTAs x 256 KB per 256x256 layer = 32 MB of L2
+// reads -- the bound of this design.  Inside a chunk the 8 warps split K (warp w takes k = 4w..4w+3 of the 32), each lane holds
+// an 8-row x 8-column accumulator tile (40 shared-memory wavefronts per 256 FFMA), and the eight partial tiles are added in
+// warp order in shared memory: a fixed summation order, bit-reproducible run to run and replica to replica.
 // The chunk pipeline is warp-specialised: a ninth warp issues the TMA requests and refills a slot as soon as the eight compute
 // warps have released it (a named hardware barrier per slot: bar.arrive by the compute threads, bar.sync by the producer); the
 // compute warps neither issue copies (a cp.async.bulk issue stalls the issuing warp) nor meet at a CTA-wide barrier per chunk
@@ -36,30 +40,30 @@
 
 namespace bsac {
 
-constexpr int CH_ROWS = 8;                 // rows per CTA (template parameter ROWS = 8 or 4; buffers are sized for 8)
+constexpr int CH_ROWS = 8;                 // rows per CTA (template parameter ROWS = 8, 4 or 2; buffers are sized for 8)
 constexpr int CH_MAXW = 256;               // widest layer / widest reduction
 constexpr int CH_KC = 32;                  // k rows per weight chunk
 constexpr int CH_NSTAGE = 3;               // weight chunks in flight
-constexpr int CH_MAXL = 8;                 // dense stages per job
+constexpr int CH_MAXL = 8;                 // dense stages per direction (= B200SAC_MAX_HIDDEN)
 constexpr int CH_THREADS = 256;             // compute threads (8 warps)
 constexpr int CH_WARPS = CH_THREADS / 32;
 constexpr int CH_BLOCK = CH_THREADS + 32;   // + one producer warp: issues every weight chunk, waits on the slots' "empty" barriers
 constexpr int CH_INP = CH_MAXW + 4;        // row pitch of the activation buffers
 constexpr int CH_CHUNK_FLOATS = CH_MAXW * CH_KC;                     // 8192 floats = 32 KB: [256 n][32 k] swizzled | [32 k][256 n]
 constexpr int CH_MAXJOBS = 3;
-// shared memory (floats): two activation buffers, head weights [16][260], d(head out) [8][16], action columns of W0
-// [256][8], partial tiles [8 warps][8 rows][256], weight stages
+// shared memory (floats) of every chain kernel: weight stages, mbarriers (64 B: full[3]), two activation buffers; then the
+// kernel's own buffers, and the partial tiles [8 warps][8 rows][256] last
 constexpr int CH_SM_ACT = CH_ROWS * CH_INP;
+constexpr int CH_SM_BARS = 16;
+constexpr int CH_SM_COMMON = CH_NSTAGE * CH_CHUNK_FLOATS + CH_SM_BARS + 2 * CH_SM_ACT;
+constexpr int CH_SM_PART = CH_WARPS * CH_ROWS * CH_MAXW;
+// chain_kernel's own: head weights [16][260], d(head out) [8][16]
 constexpr int CH_SM_HEADW = kMaxHeadOut * CH_INP;
 constexpr int CH_SM_SD = CH_ROWS * kMaxHeadOut;
-constexpr int CH_SM_W0A = CH_MAXW * kMaxAct;
-constexpr int CH_SM_PART = CH_WARPS * CH_ROWS * CH_MAXW;
-constexpr int CH_SM_BARS = 16;             // mbarriers (64 B): full[3]
-constexpr int CH_SMEM_FLOATS = CH_NSTAGE * CH_CHUNK_FLOATS + CH_SM_BARS + 2 * CH_SM_ACT + CH_SM_HEADW + CH_SM_SD + CH_SM_W0A + CH_SM_PART;
-constexpr size_t CH_SMEM_BYTES = (size_t)CH_SMEM_FLOATS * sizeof(float) + 1024;     // + slack to align the stage buffers to 1 KB
+constexpr size_t CH_SMEM_BYTES = (size_t)(CH_SM_COMMON + CH_SM_HEADW + CH_SM_SD + CH_SM_PART) * sizeof(float) + 1024;  // + slack to align the stage buffers to 1 KB
 
-enum { CJ_FWD = 0, CJ_BWD_CRITIC = 1, CJ_BWD_ACTORQ = 2, CJ_BWD_POLICY = 3 };
-enum { CH_HEAD_NONE = 0, CH_HEAD_SCALAR = 1, CH_HEAD_POLICY = 2, CH_TAIL_DACTION = 3 };
+enum { CJ_FWD = 0, CJ_BWD_POLICY = 1 };
+enum { CH_HEAD_NONE = 0, CH_HEAD_SCALAR = 1, CH_HEAD_POLICY = 2 };
 
 struct ChainStage {
   const float* W;          // parameter arena (replica stride rsP). forward: W[n][k] (nn.Linear layout); backward: the same
@@ -76,24 +80,20 @@ struct ChainStage {
 
 struct ChainJob {
   int kind, rows, nstages, head;
-  int net;                                             // twin index (0/1) into the [2][B] per-row buffers
   const float* X; long long rsX; int ldx, K0;          // FWD: input rows [rows][ldx], K0 valid columns
   const float* hlast; long long rsHlast; int ldh;      // BWD: last hidden activation [rows][Hh] (gate of the generated dY)
   float* dylast; long long rsDy; int lddy;             // BWD: optional store of the generated dY (needed by the weight gradient)
   const float* Wh; const float* bh; int NO, Hh;        // head weights [NO][Hh], bias (arena)
   float* qout; long long rsQ;                          // scalar head: output (row 0 of this net)
-  const float* W0; int ldw0, col0, nact, H0;           // DACTION tail: first-layer weights [H0][ldw0], action columns col0..col0+nact
-  float* dx; long long rsDx; int lddx;                 // DACTION tail: out[rows][lddx] (+col0)
   ChainStage st[CH_MAXL];
 };
 
-// per-row scalars the backward jobs turn into d(head output)
+// per-row scalars the backward parts turn into d(head output)
 struct ChainRows {
   const float* r; const float* d; const int* tid; long long rsR;
   const float* logp; long long rsLogp;                 // [0,B) next-state half, [B,2B) current-state half
-  const float* log_alpha;                              // arena
   const float* alpha; long long rsAlpha;               // exp(log_alpha[t]) of this step, written once by the ingest kernel
-  const float* qt; const float* q; const float* qp;    // [2][B] target / local (s,a) / local (s,a~) head outputs, replica stride 2*rsY
+  const float* q;                                      // [2][B] local (s,a) head outputs, replica stride 2*rsY
   float* y; float* dq; float* lq; float* dqa; float* la; float* qmin; long long rsY;   // dq, dqa: [2][B], replica stride 2*rsY
   const float* dxP; long long rsDxNet, rsDxRep; int lddx;   // critic input gradients [2][B][ldx] (policy job)
   const float* psave; long long rsSave;                // rows B.. (current-state half), pre-offset by the host
@@ -130,73 +130,297 @@ B200_D void ch_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }      //
 B200_D void ch_slot_release(int slot) { asm volatile("bar.arrive %0, 288;" ::"r"(2 + slot) : "memory"); }
 B200_D void ch_slot_acquire(int slot) { asm volatile("bar.sync %0, 288;" ::"r"(2 + slot) : "memory"); }
 
-template <bool FWD, int ROWS>
-__global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constant__ ChainArgs A, StepConst K) {
-  long long* const dbg = (A.dbg != nullptr && (blockIdx.x | blockIdx.y | blockIdx.z) == 0 && threadIdx.x == 0) ? A.dbg : nullptr;
-  int dbg_i = 0;
-#define CH_STAMP() do { if (dbg != nullptr && dbg_i < CH_DBG_SLOTS) dbg[dbg_i++] = clock64(); } while (0)
-  CH_STAMP();                              // 0: kernel entry
-  extern __shared__ __align__(1024) float sm_raw[];
-  // SWIZZLE_128B tiles want 1 KB alignment.  The offset is applied as POINTER arithmetic on the shared array: rounding the
-  // address through an integer makes every later access a generic LD/ST instead of LDS/STS
-  float* sm = sm_raw + (((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u) >> 2);
-  const ChainJob& J = A.job[blockIdx.y];
-  const int rep = blockIdx.z;
-  const int row0 = blockIdx.x * ROWS;
-  const bool live = row0 < J.rows;
-  const int nrows = (J.rows - row0 < ROWS) ? J.rows - row0 : ROWS;
-  const int tid = threadIdx.x, lane = tid & 31, w = tid >> 5;
-  const long long po = (long long)rep * A.rsP;
+// Optional clock64() timeline of thread 0 of CTA (0,0,0) (B200SAC_CHAIN_DBG=1, scripts/chain_timeline.py): one entry per
+// call, at most CH_DBG_SLOTS - 1; the last slot holds the entry count.
+struct DbgStamp {
+  long long* p;
+  int i;
+  B200_D explicit DbgStamp(long long* dbg)
+      : p((dbg != nullptr && (blockIdx.x | blockIdx.y | blockIdx.z) == 0 && threadIdx.x == 0) ? dbg : nullptr), i(0) {}
+  B200_D void operator()() { if (p != nullptr && i < CH_DBG_SLOTS) p[i++] = clock64(); }
+  B200_D void done() const { if (p != nullptr) p[CH_DBG_SLOTS - 1] = i; }
+};
 
-  float* wst = sm;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(wst + CH_NSTAGE * CH_CHUNK_FLOATS);
-  float* actA = wst + CH_NSTAGE * CH_CHUNK_FLOATS + CH_SM_BARS;
-  float* actB = actA + CH_SM_ACT;
-  float* headW = actB + CH_SM_ACT;
-  float* sd = headW + CH_SM_HEADW;
-  float* w0a = sd + CH_SM_SD;
-  float* part = w0a + CH_SM_W0A;
+// alpha[t] of the step's tasks (<= 64): the lanes request alpha[lane] and alpha[lane + 32] up front, so a row's alpha then
+// comes from a shuffle instead of a second, dependent round trip behind its task-id load
+struct TaskAlpha {
+  float lo, hi;
+  B200_D TaskAlpha(const ChainRows& R, const StepConst& K, int rep, int lane)
+      : lo((R.alpha + rep * R.rsAlpha)[lane < (K.T > 0 ? K.T : 1) ? lane : 0]),
+        hi((K.T > 32) ? (R.alpha + rep * R.rsAlpha)[lane + 32 < K.T ? lane + 32 : 0] : 0.f) {}
+  B200_D float of(int t) const {           // every lane of the warp takes part
+    const float a = __shfl_sync(0xffffffffu, lo, t & 31), b = __shfl_sync(0xffffffffu, hi, t & 31);
+    return t < 32 ? a : b;
+  }
+};
 
-  // ---- weight pipeline: thread 0 issues chunk g into stage g % 3; the chunk lands on bars[g % 3] (phase (g / 3) & 1) -------
-  // Forward jobs whose input layer has K <= 32 (8 / 10 columns at LunarLander): that layer is evaluated DIRECTLY -- thread n
-  // holds row n of W0 in registers and does the K-long dot product for every row itself: no weight chunk, no split-K
-  // partials, no reduction (a chunk wait + partial-tile epilogue would cost far more than the 80 FMAs per thread).
-  const bool direct0 = FWD && J.nstages > 1 && J.st[0].K <= CH_KC;
-  int is = direct0 ? 1 : 0, ic = 0, issued = 0;        // next chunk to issue: stage, chunk within the stage, running count
-  // who: the thread that executes it (0: the early requests before griddepcontrol.wait; CH_THREADS: the producer warp's lane 0);
-  // dry: advance the iterator only (the producer skips what thread 0 already requested)
-  auto issue_next = [&](int who, bool dry) {
-    const bool mine = who == 0 ? tid == 0 : tid >= CH_THREADS;        // thread 0 (early requests) | the whole producer warp
-    if (mine && is < J.nstages) {
-      const ChainStage& S = J.st[is];
+// The state a chain kernel's CTA shares between the building blocks below: its rows, its replica, the common shared-memory
+// buffers and the weight pipeline over a flat stage list st[first, nst).  Stages below nfwd are forward (the swizzled [n][k]
+// chunk through the stage's 2-D tensor map), the others backward ([k][n] rows, one contiguous bulk copy).  Chunk g lands in
+// slot g % 3 on bars[g % 3] (phase (g / 3) & 1).
+template <int ROWS>
+struct ChainCta {
+  DbgStamp stamp;
+  int tid, lane, w, rep, row0, nrows;
+  long long po;                            // this replica's offset in the parameter arena
+  float* wst; uint64_t* bars;              // weight stages, their "full" mbarriers
+  float* In; float* Out;                   // activation buffers [ROWS][CH_INP]: the next stage's input, its output
+  float* part;                             // partial tiles [CH_WARPS][ROWS][CH_MAXW] (set by the kernel: last in its layout)
+  const ChainStage* st;
+  int first, nfwd, nst;
+  int is, ic, issued;                      // producer: next chunk to issue (stage, chunk within the stage), chunks issued
+  int g, total;                            // compute warps: next chunk to consume, chunks of the whole list
+
+  // sm_raw: the kernel's dynamic shared memory.  SWIZZLE_128B tiles want 1 KB alignment; the offset is applied as POINTER
+  // arithmetic on the shared array: rounding the address through an integer makes every later access a generic LD/ST
+  B200_D ChainCta(long long* dbg, float* sm_raw, int rows, long long rsP)
+      : stamp(dbg), tid(threadIdx.x), lane(threadIdx.x & 31), w(threadIdx.x >> 5), rep(blockIdx.z), row0(blockIdx.x * ROWS),
+        nrows((rows - (int)blockIdx.x * ROWS < ROWS) ? rows - (int)blockIdx.x * ROWS : ROWS), po((long long)blockIdx.z * rsP) {
+    wst = sm_raw + (((1024u - (smem_u32(sm_raw) & 1023u)) & 1023u) >> 2);
+    bars = reinterpret_cast<uint64_t*>(wst + CH_NSTAGE * CH_CHUNK_FLOATS);
+    In = wst + CH_NSTAGE * CH_CHUNK_FLOATS + CH_SM_BARS;
+    Out = In + CH_SM_ACT;
+    part = nullptr;
+  }
+  B200_D float* own_smem() const { return Out + CH_SM_ACT; }     // start of the kernel's own buffers
+
+  B200_D void set_stages(const ChainStage* st_, int first_, int nfwd_, int nst_) {
+    st = st_; first = first_; nfwd = nfwd_; nst = nst_;
+    is = first; ic = 0; issued = 0; g = 0; total = 0;
+    for (int s = first; s < nst; ++s) total += (((st[s].K + 3) & ~3) + CH_KC - 1) / CH_KC;
+  }
+  // Issue the next chunk (if any).  Run by the whole producer warp (the slot hand-back is a warp-wide bar.sync) or by thread 0
+  // alone for the requests before griddepcontrol.wait; `leader` issues the copy.  dry: only step past a chunk that thread 0
+  // already requested.
+  B200_D void issue_next(bool leader, bool dry) {
+    if (is >= nst) return;
+    const ChainStage& S = st[is];
+    const int K4 = (S.K + 3) & ~3;
+    const int k0 = ic * CH_KC;
+    const int kc = (K4 - k0 < CH_KC) ? K4 - k0 : CH_KC;
+    const int slot = issued % CH_NSTAGE;
+    if (!dry) {
+      if (issued >= CH_NSTAGE) ch_slot_acquire(slot);               // every compute thread is done with the slot's previous chunk
+      if (leader) {
+        const uint32_t bar = smem_u32(bars + slot), dst = smem_u32(wst + slot * CH_CHUNK_FLOATS);
+        if (is < nfwd) {
+          mbar_expect_tx(bar, (uint32_t)S.N * CH_KC * 4u);
+          tma_load_2d(dst, S.tm + (long long)rep * S.rsTm, k0, 0, bar);
+        } else {
+          const uint32_t bytes = (uint32_t)kc * (uint32_t)S.N * 4u;
+          mbar_expect_tx(bar, bytes);
+          bulk_load_1d(dst, S.W + po + (long long)k0 * S.ldw, bytes, bar);
+        }
+      }
+    }
+    ++issued;
+    if (k0 + CH_KC >= K4) { ic = 0; ++is; } else { ++ic; }
+  }
+  // thread 0, before griddepcontrol.wait: the barriers and, when the weights do not come from the launch right before this
+  // one, the first two chunks
+  B200_D void start_pipeline(bool early) {
+    if (first < nfwd) asm volatile("prefetch.tensormap [%0];" ::"l"(st[first].tm + (long long)rep * st[first].rsTm) : "memory");
+#pragma unroll
+    for (int i = 0; i < CH_NSTAGE; ++i) mbar_init(smem_u32(bars + i), 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    if (early) { issue_next(true, false); issue_next(true, false); }
+  }
+  // the producer warp: every chunk thread 0 did not request, in order
+  B200_D void produce(bool early) {
+    if (early) { issue_next(false, true); issue_next(false, true); }
+    while (is < nst) issue_next(tid == CH_THREADS, false);
+  }
+
+  // v[m] = p[row0 + m][tid] of a [rows][ld] buffer (replica stride rs) for this thread's column, 0 outside it
+  B200_D void load_col(float (&v)[ROWS], const float* p, long long rs, int ld, int ncols) const {
+    const float* __restrict__ q = p + (long long)rep * rs + (long long)row0 * ld;
+#pragma unroll
+    for (int m = 0; m < ROWS; ++m) v[m] = (tid < ncols && m < nrows) ? q[(long long)m * ld + tid] : 0.f;
+  }
+  // the CTA's input rows [ROWS][K0] -> In by cp.async (rows past the job's end read as zero); the caller commits the group
+  B200_D void load_input_rows(const float* X, long long rsX, int ldx, int K0) {
+    const float* __restrict__ Xr = X + (long long)rep * rsX + (long long)row0 * ldx;
+    const int k4 = (K0 + 3) >> 2;
+    for (int e = tid; e < ROWS * k4; e += CH_THREADS) {
+      const int m = e / k4, q = e - m * k4;
+      if (m < nrows) cp_async16(In + m * CH_INP + 4 * q, Xr + (long long)m * ldx + 4 * q);
+      else *reinterpret_cast<float4*>(In + m * CH_INP + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
+  B200_D void swap() { float* t = In; In = Out; Out = t; }
+};
+
+// An input layer with K <= 32 (8 / 10 columns at LunarLander) is evaluated DIRECTLY: thread n holds row n of W0 in registers
+// and does the K-long dot product for every row itself -- no weight chunk, no split-K partials, no reduction (a chunk wait +
+// partial-tile epilogue would cost far more than the 80 FMAs per thread).  The row and bias do not depend on the launch
+// before this one, so they are requested before griddepcontrol.wait when the kernel may.
+struct DirectRow {
+  float4 w[CH_KC / 4];
+  float b = 0.f;
+  B200_D void load(const ChainStage& S, long long po, int tid) {
+    if (tid < S.N) {
       const int K4 = (S.K + 3) & ~3;
-      const int k0 = ic * CH_KC;
-      const int kc = (K4 - k0 < CH_KC) ? K4 - k0 : CH_KC;
-      const int slot = issued % CH_NSTAGE;
-      if (!dry) {
-        if (issued >= CH_NSTAGE) ch_slot_acquire(slot);               // every compute thread is done with the slot's previous chunk
-        if (tid == who) {
-          const uint32_t bar = smem_u32(bars + slot), dst = smem_u32(wst + slot * CH_CHUNK_FLOATS);
-          if constexpr (FWD) {
-            mbar_expect_tx(bar, (uint32_t)S.N * CH_KC * 4u);
-            tma_load_2d(dst, S.tm + (long long)rep * S.rsTm, k0, 0, bar);
-          } else {
-            const uint32_t bytes = (uint32_t)kc * (uint32_t)S.N * 4u;
-            mbar_expect_tx(bar, bytes);
-            bulk_load_1d(dst, S.W + po + (long long)k0 * S.ldw, bytes, bar);
+      const float4* __restrict__ wp = reinterpret_cast<const float4*>(S.W + po + (long long)tid * S.ldw);
+#pragma unroll
+      for (int q = 0; q < CH_KC / 4; ++q) w[q] = (4 * q < K4) ? __ldg(wp + q) : make_float4(0.f, 0.f, 0.f, 0.f);
+      b = __ldg(S.bias + po + tid);
+    }
+  }
+};
+template <int ROWS>
+B200_D void direct_layer(ChainCta<ROWS>& c, const ChainStage& S, const DirectRow& r) {
+  const int N = S.N, K4 = (S.K + 3) & ~3;
+  cp_async_wait<0>();
+  ch_sync();                               // the input rows are in shared memory
+  if (c.tid < N) {
+    float* __restrict__ go = S.out ? S.out + (long long)c.rep * S.rsOut + (long long)c.row0 * S.ldo : nullptr;
+#pragma unroll
+    for (int m = 0; m < ROWS; ++m) {
+      float v = 0.f;
+#pragma unroll
+      for (int q = 0; q < CH_KC / 4; ++q)
+        if (4 * q < K4) {
+          const float4 x = *reinterpret_cast<const float4*>(c.In + m * CH_INP + 4 * q);
+          v = fmaf(x.x, r.w[q].x, v); v = fmaf(x.y, r.w[q].y, v); v = fmaf(x.z, r.w[q].z, v); v = fmaf(x.w, r.w[q].w, v);
+        }
+      v = fmaxf(v + r.b, 0.f);
+      c.Out[m * CH_INP + c.tid] = v;
+      if (go && m < c.nrows) go[(long long)m * S.ldo + c.tid] = v;
+    }
+  }
+  ch_sync();
+  c.stamp();                               // input layer done (direct)
+  c.swap();
+}
+
+// One dense stage on the next chunks of the pipeline: forward Out = relu(In W^T + b), backward Out = (In W) * [mask > 0].
+// Widths are multiples of 4 (fused_eligible), so the next stage's K4 == this stage's N and no pad column is left to clear.
+template <bool FWD, int ROWS>
+B200_D void dense_stage(ChainCta<ROWS>& c, const ChainStage& S) {
+  const int tid = c.tid, lane = c.lane, w = c.w;
+  const int N = S.N, K4 = (S.K + 3) & ~3;
+  // epilogue operands of this thread's column, requested now
+  float ebias = 0.f, emask[ROWS];
+  if constexpr (FWD) {
+    if (tid < N) ebias = __ldg(S.bias + c.po + tid);
+  } else {
+    c.load_col(emask, S.mask, S.rsMask, S.ldmask, N);
+  }
+  float acc[ROWS][8];
+#pragma unroll
+  for (int m = 0; m < ROWS; ++m)
+#pragma unroll
+    for (int i = 0; i < 8; ++i) acc[m][i] = 0.f;
+
+  for (int k0 = 0; k0 < K4; k0 += CH_KC, ++c.g) {
+    const int g = c.g;
+    if (g == 0) { cp_async_wait<0>(); ch_sync(); }   // the prologue's cp.async pieces (every thread's) are visible to all
+    mbar_wait(smem_u32(c.bars + g % CH_NSTAGE), (uint32_t)((g / CH_NSTAGE) & 1));
+    c.stamp();                             // per chunk: data landed
+    const int kc = (K4 - k0 < CH_KC) ? K4 - k0 : CH_KC;
+    const float* __restrict__ Wc = c.wst + (g % CH_NSTAGE) * CH_CHUNK_FLOATS;
+    if (4 * w < kc) {
+      // every operand of the chunk is requested before the first FMA (no branches in between: the loads of columns
+      // >= N read stale shared memory into accumulators nobody reads)
+      float4 a[ROWS];
+#pragma unroll
+      for (int m = 0; m < ROWS; ++m) a[m] = *reinterpret_cast<const float4*>(c.In + m * CH_INP + k0 + 4 * w);
+      if constexpr (FWD) {
+        float4 wv[8];
+#pragma unroll
+        for (int i = 0; i < 8; ++i) wv[i] = *reinterpret_cast<const float4*>(Wc + (lane + 32 * i) * CH_KC + 4 * (w ^ (lane & 7)));   // 128-B swizzle: chunk ^ (row & 7)
+        // k component outermost: 64 independent FMAs between two uses of an accumulator (per accumulator the
+        // summation order is still k ascending)
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+#pragma unroll
+          for (int i = 0; i < 8; ++i) {
+            const float wq = q == 0 ? wv[i].x : (q == 1 ? wv[i].y : (q == 2 ? wv[i].z : wv[i].w));
+#pragma unroll
+            for (int m = 0; m < ROWS; ++m) {
+              const float av = q == 0 ? a[m].x : (q == 1 ? a[m].y : (q == 2 ? a[m].z : a[m].w));
+              acc[m][i] = fmaf(av, wq, acc[m][i]);
+            }
+          }
+        }
+      } else {
+        float4 w0[4], w1[4];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float* __restrict__ wr = Wc + (4 * w + q) * N;
+          w0[q] = *reinterpret_cast<const float4*>(wr + 4 * lane);
+          w1[q] = *reinterpret_cast<const float4*>(wr + 128 + 4 * lane);
+        }
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+#pragma unroll
+          for (int m = 0; m < ROWS; ++m) {
+            const float av = q == 0 ? a[m].x : (q == 1 ? a[m].y : (q == 2 ? a[m].z : a[m].w));
+            acc[m][0] = fmaf(av, w0[q].x, acc[m][0]); acc[m][1] = fmaf(av, w0[q].y, acc[m][1]);
+            acc[m][2] = fmaf(av, w0[q].z, acc[m][2]); acc[m][3] = fmaf(av, w0[q].w, acc[m][3]);
+            acc[m][4] = fmaf(av, w1[q].x, acc[m][4]); acc[m][5] = fmaf(av, w1[q].y, acc[m][5]);
+            acc[m][6] = fmaf(av, w1[q].z, acc[m][6]); acc[m][7] = fmaf(av, w1[q].w, acc[m][7]);
           }
         }
       }
-      ++issued;
-      if (k0 + CH_KC >= K4) { ic = 0; ++is; } else { ++ic; }
     }
-  };
-  int total_chunks = 0;                      // (the compute warps hand a slot back only if a later chunk will refill it)
-  for (int s_ = direct0 ? 1 : 0; s_ < J.nstages; ++s_) total_chunks += (((J.st[s_].K + 3) & ~3) + CH_KC - 1) / CH_KC;
+    if (g + CH_NSTAGE < c.total) ch_slot_release(g % CH_NSTAGE);         // this thread is done with the slot
+  }
+  // ---- stage epilogue: the 8 partial tiles -> fixed-order sum -> bias+ReLU | ReLU' gate -> next input -------------------
+  {
+    float* __restrict__ pw = c.part + w * (ROWS * CH_MAXW);
+    if constexpr (FWD) {
+#pragma unroll
+      for (int m = 0; m < ROWS; ++m)
+#pragma unroll
+        for (int i = 0; i < 8; ++i) pw[m * CH_MAXW + lane + 32 * i] = acc[m][i];
+    } else {
+#pragma unroll
+      for (int m = 0; m < ROWS; ++m) {
+        *reinterpret_cast<float4*>(pw + m * CH_MAXW + 4 * lane) = make_float4(acc[m][0], acc[m][1], acc[m][2], acc[m][3]);
+        *reinterpret_cast<float4*>(pw + m * CH_MAXW + 128 + 4 * lane) = make_float4(acc[m][4], acc[m][5], acc[m][6], acc[m][7]);
+      }
+    }
+  }
+  ch_sync();
+  if (tid < N) {
+    float* __restrict__ go = S.out ? S.out + (long long)c.rep * S.rsOut + (long long)c.row0 * S.ldo : nullptr;
+#pragma unroll
+    for (int m = 0; m < ROWS; ++m) {
+      float v = 0.f;
+#pragma unroll
+      for (int ww = 0; ww < CH_WARPS; ++ww) v += c.part[(ww * ROWS + m) * CH_MAXW + tid];
+      if constexpr (FWD) v = fmaxf(v + ebias, 0.f);
+      else if (!(emask[m] > 0.f)) v = 0.f;
+      c.Out[m * CH_INP + tid] = v;
+      if (go && m < c.nrows) go[(long long)m * S.ldo + tid] = v;
+    }
+  }
+  ch_sync();
+  c.stamp();                               // per stage: epilogue done
+  c.swap();
+}
+
+// The forward of the actor and the local critics (FWD: hidden layers, then the policy or scalar head of each job), and the
+// policy backward (!FWD: d(mu|log_std) from the critics' d(action) and the saved policy values, then the input-gradient chain).
+template <bool FWD, int ROWS>
+__global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constant__ ChainArgs A, StepConst K) {
+  const ChainJob& J = A.job[blockIdx.y];
+  extern __shared__ __align__(1024) float sm_raw[];
+  ChainCta<ROWS> c(A.dbg, sm_raw, J.rows, A.rsP);
+  c.stamp();                               // 0: kernel entry
+  const int tid = c.tid, lane = c.lane, w = c.w, rep = c.rep, row0 = c.row0, nrows = c.nrows;
+  const long long po = c.po;
+  const bool live = row0 < J.rows;
+  float* headW = c.own_smem();
+  float* sd = headW + CH_SM_HEADW;
+  c.part = sd + CH_SM_SD;
+
+  const bool direct0 = FWD && J.nstages > 1 && J.st[0].K <= CH_KC;
+  c.set_stages(J.st, direct0 ? 1 : 0, FWD ? J.nstages : 0, J.nstages);
   // weights that do not depend on the launch right before this one: the head matrix (cp.async) and, for a directly
   // evaluated input layer, this thread's row of W0 + its bias (registers)
-  float4 wr0[CH_KC / 4];
-  float b00 = 0.f;
+  DirectRow d0;
   auto request_weights = [&]() {
     if (J.NO > 0) {
       const float* __restrict__ Wh = J.Wh + po;
@@ -206,154 +430,53 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constan
         cp_async16(headW + j * CH_INP + 4 * q, Wh + (long long)j * J.Hh + 4 * q);
       }
     }
-    if constexpr (FWD) {
-      if (direct0 && tid < J.st[0].N) {
-        const ChainStage& S = J.st[0];
-        const int K4 = (S.K + 3) & ~3;
-        const float4* __restrict__ wp = reinterpret_cast<const float4*>(S.W + po + (long long)tid * S.ldw);
-#pragma unroll
-        for (int q = 0; q < CH_KC / 4; ++q) wr0[q] = (4 * q < K4) ? __ldg(wp + q) : make_float4(0.f, 0.f, 0.f, 0.f);
-        b00 = __ldg(S.bias + po + tid);
-      }
-    }
+    if (direct0) d0.load(J.st[0], po, tid);
   };
   if (live) {
-    if (tid == 0) {
-      if constexpr (FWD) asm volatile("prefetch.tensormap [%0];" ::"l"(J.st[0].tm + (long long)rep * J.st[0].rsTm) : "memory");
-#pragma unroll
-      for (int i = 0; i < CH_NSTAGE; ++i) mbar_init(smem_u32(bars + i), 1);
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      if (A.early_weights) { issue_next(0, false); issue_next(0, false); }
-    }
+    if (tid == 0) c.start_pipeline(A.early_weights);
     if (A.early_weights && tid < CH_THREADS) request_weights();
   }
   KStamp ks_;
-  CH_STAMP();                              // 1: predecessor complete (griddepcontrol.wait)
+  c.stamp();                               // 1: predecessor complete (griddepcontrol.wait)
   if (!live) return;
   __syncthreads();                         // barriers initialised (all nine warps)
-  if (tid >= CH_THREADS) {                 // ---- producer warp: every remaining weight chunk, in order ----
-    if (A.early_weights) { issue_next(CH_THREADS, true); issue_next(CH_THREADS, true); }     // thread 0 requested these before the wait
-    while (is < J.nstages) issue_next(CH_THREADS, false);
+  if (tid >= CH_THREADS) {                 // ---- producer warp ----
+    c.produce(A.early_weights);
     return;
   }
   if (!A.early_weights) request_weights();
+  if constexpr (FWD) c.load_input_rows(J.X, J.rsX, J.ldx, J.K0);   // (joins the head weights in the cp.async group)
+  cp_async_commit();
+  c.stamp();                               // 2: prologue loads issued
 
-  float* In = actA;
-  float* Out = actB;
-
-  // ---- prologue: (forward) the input rows join the head weights in the cp.async group ------------------------------------
-  if constexpr (FWD) {
-    const float* __restrict__ X = J.X + (long long)rep * J.rsX + (long long)row0 * J.ldx;
-    const int k4 = (J.K0 + 3) >> 2;
-    for (int e = tid; e < ROWS * k4; e += CH_THREADS) {
-      const int m = e / k4, q = e - m * k4;
-      if (m < nrows) cp_async16(In + m * CH_INP + 4 * q, X + (long long)m * J.ldx + 4 * q);
-      else *reinterpret_cast<float4*>(In + m * CH_INP + 4 * q) = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  }
-
-  cp_async_commit();                       // (the head weights / input rows requested above)
-  CH_STAMP();                              // 2: prologue loads issued
-
-  // ---- backward jobs: d(head output) of the CTA's rows, then dY_last = (dout Wh) * [h_last > 0] -------------------------
+  // ---- policy backward: d(mu|log_std) of the CTA's rows, then dY_last = (dout Wh) * [h_last > 0] -----------------------
   if constexpr (!FWD) {
     const ChainRows& R = A.rw;
-    const int B = K.B, Aa = K.act;
+    const int Aa = K.act;
     const int row = row0 + w;                      // warp w owns row w
-    // gate activations of this thread's column (issued before anything is waited for)
-    float hv[ROWS];
-    {
-      const float* __restrict__ hl = J.hlast + (long long)rep * J.rsHlast + (long long)row0 * J.ldh;
-#pragma unroll
-      for (int m = 0; m < ROWS; ++m) hv[m] = (tid < J.Hh && m < nrows) ? hl[(long long)m * J.ldh + tid] : 0.f;
-    }
-    // action columns of the first-layer weights for the tail: requested now (registers), parked in shared memory after
-    // the d(head output) phase -- the strided gather's latency hides behind it instead of heading the critical path
-    float w0r[CH_MAXW * kMaxAct / CH_THREADS];
-    const bool want_w0a = J.kind == CJ_BWD_ACTORQ && J.nact > 0;
-    if (want_w0a) {
-      const float* __restrict__ W0 = J.W0 + po;
-#pragma unroll
-      for (int i = 0; i < CH_MAXW * kMaxAct / CH_THREADS; ++i) {
-        const int e = tid + i * CH_THREADS, k = e >> 3, j = e & 7;
-        w0r[i] = (k < J.H0 && j < J.nact) ? __ldg(W0 + (long long)k * J.ldw0 + J.col0 + j) : 0.f;
+    float hv[ROWS];                                // gate activations of this thread's column (issued before anything is waited for)
+    c.load_col(hv, J.hlast, J.rsHlast, J.ldh, J.Hh);
+    const TaskAlpha alpha(R, K, rep, lane);
+    if (w < nrows) {                               // lane j < A owns action j
+      const float alpha_row = alpha.of(__shfl_sync(0xffffffffu, lane == 0 ? (R.tid + rep * R.rsR)[row] : 0, 0));
+      if (lane < Aa) {
+        const float* __restrict__ sv = R.psave + rep * R.rsSave + ((long long)row * Aa + lane) * kSaveW;
+        const float* __restrict__ dx0 = R.dxP + rep * R.rsDxRep + (long long)row * R.lddx + K.in_w + lane;
+        const float da = dx0[0] + dx0[R.rsDxNet];
+        float dmu, dls;
+        policy_dout_point(K, sv, da, alpha_row, dmu, dls);
+        sd[w * kMaxHeadOut + lane] = dmu;
+        sd[w * kMaxHeadOut + Aa + lane] = dls;
+        float* o = R.dout_dbg + rep * R.rsDbg + (long long)row * 2 * Aa;
+        o[lane] = dmu;
+        o[Aa + lane] = dls;
+        (R.dact_dbg + rep * R.rsDbg)[(long long)row * Aa + lane] = da;
       }
     }
-    // the step's temperatures (<= 64 tasks) are requested by the lanes up front; the row's alpha[t] then comes from a
-    // shuffle instead of a second, dependent round trip behind the task-id load
-    const float alpha_lo = (R.alpha + rep * R.rsAlpha)[lane < (K.T > 0 ? K.T : 1) ? lane : 0];
-    const float alpha_hi = (K.T > 32) ? (R.alpha + rep * R.rsAlpha)[lane + 32 < K.T ? lane + 32 : 0] : 0.f;
-    auto alpha_of = [&](int t) { const float lo = __shfl_sync(0xffffffffu, alpha_lo, t & 31), hi = __shfl_sync(0xffffffffu, alpha_hi, t & 31); return t < 32 ? lo : hi; };
-    if (w < nrows) {
-      if (J.kind == CJ_BWD_CRITIC) {
-        const int t_row = __shfl_sync(0xffffffffu, lane == 0 ? (R.tid + rep * R.rsR)[row] : 0, 0);
-        const float alpha_row = alpha_of(t_row);
-        if (lane == 0) {
-          const float r = (R.r + rep * R.rsR)[row], d = (R.d + rep * R.rsR)[row];
-          const float gamma = K.hp[rep].gamma, reward_scale = K.hp[rep].reward_scale;
-          const float lp = (R.logp + rep * R.rsLogp)[row];
-          const float* QT = R.qt + rep * 2 * R.rsY;
-          const float* Q = R.q + rep * 2 * R.rsY;
-          const float qt1 = QT[row], qt2 = QT[B + row], q1 = Q[row], q2 = Q[B + row];
-          const float alpha = alpha_row;
-          const float t1 = reward_scale * r;
-          const float t2 = gamma * (1.f - d);
-          const float t3 = fminf(qt1, qt2) - alpha * lp;
-          const float y = t1 + t2 * t3;
-          const float qn = J.net == 0 ? q1 : q2;
-          const float dqv = 2.f * K.c_loss * (qn - y);
-          sd[w * kMaxHeadOut] = dqv;
-          (R.dq + rep * 2 * R.rsY)[J.net * B + row] = dqv;
-          if (J.net == 0) {
-            const float e1 = y - q1, e2 = y - q2;
-            (R.y + rep * R.rsY)[row] = y;
-            (R.lq + rep * R.rsY)[row] = e1 * e1 + e2 * e2;
-          }
-        }
-      } else if (J.kind == CJ_BWD_ACTORQ) {
-        const int t_row = __shfl_sync(0xffffffffu, lane == 0 ? (R.tid + rep * R.rsR)[row] : 0, 0);
-        const float alpha_row = alpha_of(t_row);
-        if (lane == 0) {
-          const float lp = (R.logp + rep * R.rsLogp)[B + row];
-          const float* QP = R.qp + rep * 2 * R.rsY;
-          const float q1 = QP[row], q2 = QP[B + row];
-          float g1, g2;
-          if (q1 == q2) { g1 = g2 = -0.5f * K.c_loss; }
-          else if (q1 < q2) { g1 = -K.c_loss; g2 = 0.f; }
-          else { g1 = 0.f; g2 = -K.c_loss; }
-          const float g = J.net == 0 ? g1 : g2;
-          sd[w * kMaxHeadOut] = g;
-          (R.dqa + rep * 2 * R.rsY)[J.net * B + row] = g;
-          if (J.net == 0) {
-            const float alpha = alpha_row;
-            const float qm = fminf(q1, q2);
-            (R.la + rep * R.rsY)[row] = -(qm - alpha * lp);
-            (R.qmin + rep * R.rsY)[row] = qm;
-          }
-        }
-      } else {                                     // CJ_BWD_POLICY: lane j < A owns action j
-        const int t_row = __shfl_sync(0xffffffffu, lane == 0 ? (R.tid + rep * R.rsR)[row] : 0, 0);
-        const float alpha_row = alpha_of(t_row);
-        if (lane < Aa) {
-          const float* __restrict__ sv = R.psave + rep * R.rsSave + ((long long)row * Aa + lane) * kSaveW;
-          const float* __restrict__ dx0 = R.dxP + rep * R.rsDxRep + (long long)row * R.lddx + K.in_w + lane;
-          const float da = dx0[0] + dx0[R.rsDxNet];
-          const float alpha = alpha_row;
-          float dmu, dls;
-          policy_dout_point(K, sv, da, alpha, dmu, dls);
-          sd[w * kMaxHeadOut + lane] = dmu;
-          sd[w * kMaxHeadOut + Aa + lane] = dls;
-          float* o = R.dout_dbg + rep * R.rsDbg + (long long)row * 2 * Aa;
-          o[lane] = dmu;
-          o[Aa + lane] = dls;
-          (R.dact_dbg + rep * R.rsDbg)[(long long)row * Aa + lane] = da;
-        }
-      }
-    }
-    CH_STAMP();                                    // (bwd) per-row scalars -> d(head output) done by warp 0
+    c.stamp();                                     // (bwd) per-row scalars -> d(head output) done by warp 0
     cp_async_wait<0>();                            // the head weights have landed
-    ch_sync();      
-    CH_STAMP();                                    // (bwd) head weights landed, every warp's d(head output) visible
+    ch_sync();
+    c.stamp();                                     // (bwd) head weights landed, every warp's d(head output) visible
     if (tid < J.Hh) {
       float* __restrict__ dyl = J.dylast ? J.dylast + (long long)rep * J.rsDy + (long long)row0 * J.lddy : nullptr;
 #pragma unroll
@@ -364,163 +487,21 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constan
           if (!(hv[m] > 0.f)) v = 0.f;
           if (dyl) dyl[(long long)m * J.lddy + tid] = v;
         }
-        In[m * CH_INP + tid] = v;
+        c.In[m * CH_INP + tid] = v;
       }
     }
-    if (want_w0a) {
-#pragma unroll
-      for (int i = 0; i < CH_MAXW * kMaxAct / CH_THREADS; ++i) w0a[tid + i * CH_THREADS] = w0r[i];
-    }
-    ch_sync();                                     // In (and the staged action columns) visible to every warp
+    ch_sync();                                     // In visible to every warp
   }
 
-  CH_STAMP();                              // 3: backward prologue done (forward: == 2)
-  // ---- the dense stages ------------------------------------------------------------------------------------------------
-  int g = 0;
-  if constexpr (FWD) {
-    if (direct0) {
-      const ChainStage& S = J.st[0];
-      const int N = S.N, K4 = (S.K + 3) & ~3;
-      const float4 (&wr)[CH_KC / 4] = wr0;          // this thread's row of W0, requested in the prologue
-      const float b0 = b00;
-      cp_async_wait<0>();
-      ch_sync();                        // the input rows are in shared memory
-      if (tid < N) {
-        float* __restrict__ go = S.out ? S.out + (long long)rep * S.rsOut + (long long)row0 * S.ldo : nullptr;
-#pragma unroll
-        for (int m = 0; m < ROWS; ++m) {
-          float v = 0.f;
-#pragma unroll
-          for (int q = 0; q < CH_KC / 4; ++q)
-            if (4 * q < K4) {
-              const float4 x = *reinterpret_cast<const float4*>(In + m * CH_INP + 4 * q);
-              v = fmaf(x.x, wr[q].x, v); v = fmaf(x.y, wr[q].y, v); v = fmaf(x.z, wr[q].z, v); v = fmaf(x.w, wr[q].w, v);
-            }
-          v = fmaxf(v + b0, 0.f);
-          Out[m * CH_INP + tid] = v;
-          if (go && m < nrows) go[(long long)m * S.ldo + tid] = v;
-        }
-      }
-      ch_sync();      
-      CH_STAMP();                       // input layer done (direct)
-      float* t_ = In; In = Out; Out = t_;
-    }
-  }
-  for (int s = direct0 ? 1 : 0; s < J.nstages; ++s) {
-    const ChainStage& S = J.st[s];
-    const int N = S.N, K4 = (S.K + 3) & ~3;
-    // epilogue operands of this thread's column, requested now
-    float ebias = 0.f, emask[ROWS];
-    if constexpr (FWD) {
-      if (tid < N) ebias = __ldg(S.bias + po + tid);
-    } else {
-      const float* __restrict__ mk = S.mask + (long long)rep * S.rsMask + (long long)row0 * S.ldmask;
-#pragma unroll
-      for (int m = 0; m < ROWS; ++m) emask[m] = (tid < N && m < nrows) ? mk[(long long)m * S.ldmask + tid] : 0.f;
-    }
-    float acc[ROWS][8];
-#pragma unroll
-    for (int m = 0; m < ROWS; ++m)
-#pragma unroll
-      for (int i = 0; i < 8; ++i) acc[m][i] = 0.f;
-
-    for (int k0 = 0; k0 < K4; k0 += CH_KC, ++g) {
-      if (g == 0) { cp_async_wait<0>(); ch_sync(); }   // forward: the input rows (every thread's pieces) are visible to all
-      mbar_wait(smem_u32(bars + g % CH_NSTAGE), (uint32_t)((g / CH_NSTAGE) & 1));
-      CH_STAMP();                       // per chunk: data landed
-      const int kc = (K4 - k0 < CH_KC) ? K4 - k0 : CH_KC;
-      const float* __restrict__ Wc = wst + (g % CH_NSTAGE) * CH_CHUNK_FLOATS;
-      if (4 * w < kc) {
-        // every operand of the chunk is requested before the first FMA (no branches in between: the loads of columns
-        // >= N read stale shared memory into accumulators nobody reads)
-        float4 a[ROWS];
-#pragma unroll
-        for (int m = 0; m < ROWS; ++m) a[m] = *reinterpret_cast<const float4*>(In + m * CH_INP + k0 + 4 * w);
-        if constexpr (FWD) {
-          float4 wv[8];
-#pragma unroll
-          for (int i = 0; i < 8; ++i) wv[i] = *reinterpret_cast<const float4*>(Wc + (lane + 32 * i) * CH_KC + 4 * (w ^ (lane & 7)));   // 128-B swizzle: chunk ^ (row & 7)
-          // k component outermost: 64 independent FMAs between two uses of an accumulator (per accumulator the
-          // summation order is still k ascending)
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-              const float wq = q == 0 ? wv[i].x : (q == 1 ? wv[i].y : (q == 2 ? wv[i].z : wv[i].w));
-#pragma unroll
-              for (int m = 0; m < ROWS; ++m) {
-                const float av = q == 0 ? a[m].x : (q == 1 ? a[m].y : (q == 2 ? a[m].z : a[m].w));
-                acc[m][i] = fmaf(av, wq, acc[m][i]);
-              }
-            }
-          }
-        } else {
-          float4 w0[4], w1[4];
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            const float* __restrict__ wr = Wc + (4 * w + q) * N;
-            w0[q] = *reinterpret_cast<const float4*>(wr + 4 * lane);
-            w1[q] = *reinterpret_cast<const float4*>(wr + 128 + 4 * lane);
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-#pragma unroll
-            for (int m = 0; m < ROWS; ++m) {
-              const float av = q == 0 ? a[m].x : (q == 1 ? a[m].y : (q == 2 ? a[m].z : a[m].w));
-              acc[m][0] = fmaf(av, w0[q].x, acc[m][0]); acc[m][1] = fmaf(av, w0[q].y, acc[m][1]);
-              acc[m][2] = fmaf(av, w0[q].z, acc[m][2]); acc[m][3] = fmaf(av, w0[q].w, acc[m][3]);
-              acc[m][4] = fmaf(av, w1[q].x, acc[m][4]); acc[m][5] = fmaf(av, w1[q].y, acc[m][5]);
-              acc[m][6] = fmaf(av, w1[q].z, acc[m][6]); acc[m][7] = fmaf(av, w1[q].w, acc[m][7]);
-            }
-          }
-        }
-      }
-      if (g + CH_NSTAGE < total_chunks) ch_slot_release(g % CH_NSTAGE);         // this thread is done with the slot
-    }
-    CH_STAMP();                         // per stage: last chunk computed
-    // ---- stage epilogue: the 8 partial tiles -> fixed-order sum -> bias+ReLU | ReLU' gate -> next input -----------------
-    {
-      float* __restrict__ pw = part + w * (ROWS * CH_MAXW);
-      if constexpr (FWD) {
-#pragma unroll
-        for (int m = 0; m < ROWS; ++m)
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pw[m * CH_MAXW + lane + 32 * i] = acc[m][i];
-      } else {
-#pragma unroll
-        for (int m = 0; m < ROWS; ++m) {
-          *reinterpret_cast<float4*>(pw + m * CH_MAXW + 4 * lane) = make_float4(acc[m][0], acc[m][1], acc[m][2], acc[m][3]);
-          *reinterpret_cast<float4*>(pw + m * CH_MAXW + 128 + 4 * lane) = make_float4(acc[m][4], acc[m][5], acc[m][6], acc[m][7]);
-        }
-      }
-    }
-    ch_sync();      
-    if (tid < N) {
-      float* __restrict__ go = S.out ? S.out + (long long)rep * S.rsOut + (long long)row0 * S.ldo : nullptr;
-#pragma unroll
-      for (int m = 0; m < ROWS; ++m) {
-        float v = 0.f;
-#pragma unroll
-        for (int ww = 0; ww < CH_WARPS; ++ww) v += part[(ww * ROWS + m) * CH_MAXW + tid];
-        if constexpr (FWD) v = fmaxf(v + ebias, 0.f);
-        else if (!(emask[m] > 0.f)) v = 0.f;
-        Out[m * CH_INP + tid] = v;
-        if (go && m < nrows) go[(long long)m * S.ldo + tid] = v;
-      }
-    } else if (tid < ((N + 3) & ~3)) {             // pad columns of the next reduction read as zero
-#pragma unroll
-      for (int m = 0; m < ROWS; ++m) Out[m * CH_INP + tid] = 0.f;
-    }
-    ch_sync();      
-    CH_STAMP();                         // per stage: epilogue done
-    float* t = In; In = Out; Out = t;
-  }
+  c.stamp();                               // 3: backward prologue done (forward: == 2)
+  if (direct0) direct_layer(c, J.st[0], d0);
+  for (int s = c.first; s < J.nstages; ++s) dense_stage<FWD>(c, J.st[s]);
   cp_async_wait<0>();
   ch_sync();                               // (jobs without dense stages: head weights / inputs visible)
 
-  // ---- head / tail: warp w owns row w ----------------------------------------------------------------------------------
+  // ---- head: warp w owns row w ----------------------------------------------------------------------------------------
   const int row = row0 + w;
-  const float* __restrict__ hr = In + w * CH_INP;
+  const float* __restrict__ hr = c.In + w * CH_INP;
   if (FWD && J.head == CH_HEAD_SCALAR) {
     if (w < nrows) {
       const float bq = __ldg(J.bh + po);           // requested before the dot product, consumed after it
@@ -553,12 +534,12 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constan
       for (int o = G >> 1; o > 0; o >>= 1) accj += __shfl_xor_sync(0xffffffffu, accj, o);
       if (jj < NO && part_ == 0) sd[w * kMaxHeadOut + jj] = accj + __ldg(bias + jj);
     }
-    ch_sync();      
-    CH_STAMP();                                    // (policy head) GEMVs done
+    ch_sync();
+    c.stamp();                                     // (policy head) GEMVs done
     if (w == 0) {
       const PolicyHeadArgs& P = A.pol;
-      float* lp_s = part;                          // [ROWS][A] log-prob terms, [ROWS][A] log-std terms (the partial tiles are free now)
-      float* ls_s = part + ROWS * kMaxAct;
+      float* lp_s = c.part;                        // [ROWS][A] log-prob terms, [ROWS][A] log-std terms (the partial tiles are free now)
+      float* ls_s = c.part + ROWS * kMaxAct;
       for (int e0 = 0; e0 < nrows * Aa; e0 += 32) {
         const int e = e0 + lane;
         if (e < nrows * Aa) {
@@ -587,35 +568,9 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain_kernel(const __grid_constan
         (P.logstd_sum + rep * P.rsLogp)[row0 + lane] = tls;
       }
     }
-  } else if (!FWD && J.head == CH_TAIL_DACTION) {
-    if (w < nrows) {
-      const int H0 = J.H0;
-      float acc[kMaxAct];
-#pragma unroll
-      for (int j = 0; j < kMaxAct; ++j) acc[j] = 0.f;
-      for (int k = lane; k < H0; k += 32) {          // both float4 of the row's action weights are loaded before the FMAs
-        const float dv = hr[k];
-        const float4 wa = *reinterpret_cast<const float4*>(w0a + k * kMaxAct);
-        const float4 wb = *reinterpret_cast<const float4*>(w0a + k * kMaxAct + 4);
-        acc[0] = fmaf(dv, wa.x, acc[0]); acc[1] = fmaf(dv, wa.y, acc[1]); acc[2] = fmaf(dv, wa.z, acc[2]); acc[3] = fmaf(dv, wa.w, acc[3]);
-        acc[4] = fmaf(dv, wb.x, acc[4]); acc[5] = fmaf(dv, wb.y, acc[5]); acc[6] = fmaf(dv, wb.z, acc[6]); acc[7] = fmaf(dv, wb.w, acc[7]);
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-#pragma unroll
-        for (int j = 0; j < kMaxAct; ++j) acc[j] += __shfl_xor_sync(0xffffffffu, acc[j], o);
-      }
-      if (lane == 0) {
-        float* o = J.dx + (long long)rep * J.rsDx + (long long)row * J.lddx + J.col0;
-#pragma unroll
-        for (int j = 0; j < kMaxAct; ++j)
-          if (j < J.nact) o[j] = acc[j];
-      }
-    }
   }
-  CH_STAMP();                              // last: head / tail done
-  if (dbg != nullptr) dbg[CH_DBG_SLOTS - 1] = dbg_i;
-#undef CH_STAMP
+  c.stamp();                               // last: head done
+  c.stamp.done();
 }
 
 // ------------------------------------------------------------------------------------------------------------------------
@@ -647,11 +602,11 @@ struct WgradJob {
   int shape;
   int tmA_idx, tmB_idx, rsTm;              // (host: indices into the map table; replica r at tm + r * rsTm)
 };
-// Optional Adam (+ Polyak) applied by the CTA that just reduced a gradient tile: the gradient value is final the moment the
+// Adam (+ Polyak) applied by the CTA that just reduced a gradient tile: the gradient value is final the moment the
 // tile's fixed-order sum is done, so the separate optimizer launch (one more kernel boundary + a cold pass over p/m/v) is
 // unnecessary.  Same element-wise math as adam_kernel (adam_one, torch _single_tensor_adam).
 struct WgradAdam {
-  int enabled, which;                      // which: Adam step-counter / learning-rate slot (0 critic, 1 actor)
+  int which;                               // Adam step-counter / learning-rate slot (0 critic, 1 actor)
   float* params; float* m; float* v;       // arenas; an element's index = its offset in the gradient arena
   const float* grads;                      // gradient arena base (to turn C pointers into offsets)
   long long rsP, rsM;
@@ -683,10 +638,8 @@ B200_D void wg_stage(float* __restrict__ dst, const float* __restrict__ src, int
 }
 
 __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_constant__ WgradArgs A, StepConst K) {
-  long long* const dbg = (A.dbg != nullptr && (blockIdx.x | blockIdx.y) == 0 && threadIdx.x == 0) ? A.dbg : nullptr;
-  int dbg_i = 0;
-#define WG_STAMP() do { if (dbg != nullptr && dbg_i < CH_DBG_SLOTS) dbg[dbg_i++] = clock64(); } while (0)
-  WG_STAMP();                              // 0: entry
+  DbgStamp stamp(A.dbg);
+  stamp();                                 // 0: entry
   extern __shared__ __align__(128) float wsm_raw[];
   float* sm = wsm_raw + (((128u - (smem_u32(wsm_raw) & 127u)) & 127u) >> 2);      // (pointer arithmetic keeps the shared address space)
   int ji = 0;
@@ -714,17 +667,15 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   KStamp ks_;                              // the operands come from the launch right before this one
-  WG_STAMP();                              // 1: predecessor complete
+  stamp();                                 // 1: predecessor complete
   __syncthreads();
   // bias corrections of the fused optimizer step (two counter loads, an fp64 division and square root): evaluated now, while
   // the operand tiles are in flight, instead of heading the epilogue
   const WgradAdam& O = A.adam;
-  float step_size = 0.f, bc2_sqrt = 1.f, tau = 0.f, one_minus_tau = 0.f;
-  if (O.enabled) {
-    const HParams& H = K.hp[rep];
-    adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
-    tau = H.tau; one_minus_tau = H.one_minus_tau;
-  }
+  float step_size = 0.f, bc2_sqrt = 1.f;
+  const HParams& H = K.hp[rep];
+  adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
+  const float tau = H.tau, one_minus_tau = H.one_minus_tau;
   const float* __restrict__ Ag = J.A + (long long)rep * J.rsA;
   const float* __restrict__ Bg = J.B + (long long)rep * J.rsB;
   const int M = A.M;
@@ -748,7 +699,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
     if (!tmB) wg_stage(Bs, Bg, J.ldb, n0, J.Nin, m0, M, tid);
     if (tmA || tmB) mbar_wait(smem_u32(bar), (uint32_t)(pass & 1));
     __syncthreads();
-    WG_STAMP();                            // per pass: operands landed
+    stamp();                               // per pass: operands landed
     const int mcnt = (M - m0 < WG_ROWS) ? M - m0 : WG_ROWS;
     const int per = (mcnt + 7) >> 3;
     const int mb = w * per, me = (mb + per < mcnt) ? mb + per : mcnt;
@@ -795,7 +746,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
       }
     }
   }
-  WG_STAMP();                              // accumulation done
+  stamp();                                 // accumulation done
   // partial tiles -> fixed-order sum.  Every mapping fills the part of the [32 k][32 n] tile that holds its valid outputs.
   {
     float* pw = part + w * (WG_T * WG_T);
@@ -824,7 +775,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
     }
   }
   __syncthreads();
-  WG_STAMP();                              // partial tiles visible
+  stamp();                                 // partial tiles visible
   float* __restrict__ C = J.C + (long long)rep * A.rsG;
   // fused optimizer step: adam_one per element like adam_kernel
   const float w1 = (float)(1.0 - K.beta1), b2 = (float)K.beta2, omb2 = (float)(1.0 - K.beta2), eps = (float)K.adam_eps;
@@ -833,13 +784,13 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   // and stay zero).  Every operand of the optimizer step is REQUESTED before the first dependent instruction: the (p, m, v
   // [, target]) quadruples would otherwise be sequential global round trips between stores -- and the code is kept compact on
   // purpose: it runs once per CTA out of a cold instruction cache.
-  const bool has_t = O.enabled && O.target_delta != 0;
+  const bool has_t = O.target_delta != 0;
   const int kk = tid >> 3, nn4 = (tid & 7) << 2;
   const bool okq = k0 + kk < J.Kout && n0 + nn4 < J.Nin;
   const long long ci = (long long)(k0 + kk) * J.ldc + n0 + nn4;
   const long long gi = (J.C - O.grads) + ci;
   float4 p4 = make_float4(0.f, 0.f, 0.f, 0.f), m4 = p4, v4 = p4, t4 = p4;
-  if (okq && O.enabled) {
+  if (okq) {
     const float* pp = O.params + rep * O.rsP + gi;
     p4 = *reinterpret_cast<const float4*>(pp);
     m4 = *reinterpret_cast<const float4*>(O.m + rep * O.rsM + gi);
@@ -849,7 +800,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   const bool bias_thread = bn == 0 && J.C2 != nullptr && tid < WG_T && k0 + tid < J.Kout;
   float bp = 0.f, bm = 0.f, bv_ = 0.f, bt = 0.f;
   const long long bgi = bias_thread ? (J.C2 - O.grads) + k0 + tid : 0;
-  if (bias_thread && O.enabled) {
+  if (bias_thread) {
     const float* pp = O.params + rep * O.rsP + bgi;
     bp = *pp;
     bm = (O.m + rep * O.rsM)[bgi];
@@ -862,41 +813,36 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
     const float4 q = *reinterpret_cast<const float4*>(part + ww * (WG_T * WG_T) + kk * WG_T + nn4);
     g4.x += q.x; g4.y += q.y; g4.z += q.z; g4.w += q.w;
   }
-  WG_STAMP();                              // partial tiles summed (optimizer operands still in flight)
+  stamp();                                 // partial tiles summed (optimizer operands still in flight)
   if (okq) {
     *reinterpret_cast<float4*>(C + ci) = g4;
-    if (O.enabled) {
-      adam_one(p4.x, m4.x, v4.x, g4.x, w1, b2, omb2, step_size, bc2_sqrt, eps);
-      adam_one(p4.y, m4.y, v4.y, g4.y, w1, b2, omb2, step_size, bc2_sqrt, eps);
-      adam_one(p4.z, m4.z, v4.z, g4.z, w1, b2, omb2, step_size, bc2_sqrt, eps);
-      adam_one(p4.w, m4.w, v4.w, g4.w, w1, b2, omb2, step_size, bc2_sqrt, eps);
-      float* pp = O.params + rep * O.rsP + gi;
-      *reinterpret_cast<float4*>(pp) = p4;
-      *reinterpret_cast<float4*>(O.m + rep * O.rsM + gi) = m4;
-      *reinterpret_cast<float4*>(O.v + rep * O.rsM + gi) = v4;
-      if (has_t)
-        *reinterpret_cast<float4*>(pp + O.target_delta) =
-            make_float4(tau * p4.x + one_minus_tau * t4.x, tau * p4.y + one_minus_tau * t4.y,
-                        tau * p4.z + one_minus_tau * t4.z, tau * p4.w + one_minus_tau * t4.w);
-    }
+    adam_one(p4.x, m4.x, v4.x, g4.x, w1, b2, omb2, step_size, bc2_sqrt, eps);
+    adam_one(p4.y, m4.y, v4.y, g4.y, w1, b2, omb2, step_size, bc2_sqrt, eps);
+    adam_one(p4.z, m4.z, v4.z, g4.z, w1, b2, omb2, step_size, bc2_sqrt, eps);
+    adam_one(p4.w, m4.w, v4.w, g4.w, w1, b2, omb2, step_size, bc2_sqrt, eps);
+    float* pp = O.params + rep * O.rsP + gi;
+    *reinterpret_cast<float4*>(pp) = p4;
+    *reinterpret_cast<float4*>(O.m + rep * O.rsM + gi) = m4;
+    *reinterpret_cast<float4*>(O.v + rep * O.rsM + gi) = v4;
+    if (has_t)
+      *reinterpret_cast<float4*>(pp + O.target_delta) =
+          make_float4(tau * p4.x + one_minus_tau * t4.x, tau * p4.y + one_minus_tau * t4.y,
+                      tau * p4.z + one_minus_tau * t4.z, tau * p4.w + one_minus_tau * t4.w);
   }
   if (bias_thread) {
     float v = 0.f;
 #pragma unroll
     for (int ww = 0; ww < 8; ++ww) v += bpart[ww * WG_T + tid];
     (J.C2 + (long long)rep * A.rsG)[k0 + tid] = v;
-    if (O.enabled) {
-      adam_one(bp, bm, bv_, v, w1, b2, omb2, step_size, bc2_sqrt, eps);
-      float* pp = O.params + rep * O.rsP + bgi;
-      *pp = bp;
-      (O.m + rep * O.rsM)[bgi] = bm;
-      (O.v + rep * O.rsM)[bgi] = bv_;
-      if (has_t) pp[O.target_delta] = tau * bp + one_minus_tau * bt;
-    }
+    adam_one(bp, bm, bv_, v, w1, b2, omb2, step_size, bc2_sqrt, eps);
+    float* pp = O.params + rep * O.rsP + bgi;
+    *pp = bp;
+    (O.m + rep * O.rsM)[bgi] = bm;
+    (O.v + rep * O.rsM)[bgi] = bv_;
+    if (has_t) pp[O.target_delta] = tau * bp + one_minus_tau * bt;
   }
-  WG_STAMP();                              // reduction + optimizer step done
-  if (dbg != nullptr) dbg[CH_DBG_SLOTS - 1] = dbg_i;
-#undef WG_STAMP
+  stamp();                                 // reduction + optimizer step done
+  stamp.done();
 }
 
 }  // namespace bsac

@@ -440,6 +440,21 @@ B200_D float warp_dot(const float* __restrict__ x, const float* __restrict__ w, 
   return warp_sum(warp_dot_partial(x, w, n, lane));
 }
 
+// SAC per-row math shared by the per-layer heads kernels and chain2_kernel.
+// TD target y = rs r + gamma (1-d)(min(Qt1, Qt2) - alpha logpi') (LL/learner.py:210); the caller forms t1 = rs r and
+// t2 = gamma (1-d) as soon as their operands land.
+B200_D float td_target(float t1, float t2, float qt1, float qt2, float alpha, float lp) {
+  const float t3 = fminf(qt1, qt2) - alpha * lp;
+  return t1 + t2 * t3;
+}
+// gradient of -c min(Q1, Q2) routed to the twins (LL/learner.py:222-223; torch.minimum backward: the smaller head gets
+// the gradient, ties split it)
+B200_D void min_route(float q1, float q2, float c_loss, float& g1, float& g2) {
+  if (q1 == q2) { g1 = g2 = -0.5f * c_loss; }
+  else if (q1 < q2) { g1 = -c_loss; g2 = 0.f; }
+  else { g1 = 0.f; g2 = -c_loss; }
+}
+
 __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   KStamp ks_;
   const int rep = blockIdx.y;
@@ -466,8 +481,7 @@ __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   const float qt1 = warp_sum(p_t1) + b_t1, qt2 = warp_sum(p_t2) + b_t2, q1 = warp_sum(p_q1) + b_q1, q2 = warp_sum(p_q2) + b_q2;
   if (lane == 0) {
     const float alpha = (float)exp((double)la_t);
-    const float t3 = fminf(qt1, qt2) - alpha * lp;
-    const float y = t1 + t2 * t3;
+    const float y = td_target(t1, t2, qt1, qt2, alpha, lp);
     const float e1 = y - q1, e2 = y - q2;
     float* Y = P.y + rep * P.rsY;
     Y[row] = y;
@@ -513,9 +527,7 @@ __global__ void actor_q_heads_kernel(StepConst K, ActorQHeadArgs P) {
     const float alpha = (float)exp((double)la_t);
     const float qm = fminf(q1, q2);
     float g1, g2;
-    if (q1 == q2) { g1 = g2 = -0.5f * K.c_loss; }
-    else if (q1 < q2) { g1 = -K.c_loss; g2 = 0.f; }
-    else { g1 = 0.f; g2 = -K.c_loss; }
+    min_route(q1, q2, K.c_loss, g1, g2);
     float* DQ = P.dqa + rep * 2 * P.rsY;
     DQ[row] = g1; DQ[B + row] = g2;
     (P.la + rep * P.rsY)[row] = -(qm - alpha * lp);

@@ -54,12 +54,20 @@ def test_step_matches_reference_fixture(cuda, name, precision):
     core.close()
 
 
-@pytest.mark.parametrize("precision", [0, 1], ids=["fp32", "tc3xtf32"])
-def test_backward_intermediates_match_manual_oracle(cuda, precision):
+DEEP_CRITIC = [56, 88, 24, 40, 64, 32]
+
+
+@pytest.mark.parametrize("precision,critic_hidden", [
+    pytest.param(0, [56, 88, 24], id="fp32"),
+    pytest.param(1, [56, 88, 24], id="tc3xtf32"),
+    pytest.param(0, DEEP_CRITIC, id="fp32-deep_critic"),      # the layer-chained plan past 4 critic layers
+    pytest.param(1, DEEP_CRITIC, id="tc3xtf32-deep_critic"),
+])
+def test_backward_intermediates_match_manual_oracle(cuda, precision, critic_hidden):
     """d(action), d(mu|log_std) and every gradient tensor against oracle/sac_manual.py."""
     from distributed_sac_b200 import _lib
     from distributed_sac_b200.core import SacCore
-    spec = sp.SacSpec(state_dim=11, act_dim=3, actor_hidden=[72, 40], critic_hidden=[56, 88, 24], batch=200,
+    spec = sp.SacSpec(state_dim=11, act_dim=3, actor_hidden=[72, 40], critic_hidden=critic_hidden, batch=200,
                       num_tasks=5, weighted_loss=False)
     p = sp.init_params(spec, seed=11)
     gen = torch.Generator().manual_seed(5)
@@ -79,6 +87,18 @@ def test_backward_intermediates_match_manual_oracle(cuda, precision):
     for k, ref in {**I["critic_grads"], **I["actor_grads"], "log_alpha": I["alpha_grad"]}.items():
         assert rel_l2(g[k].reshape(ref.shape), ref) <= REL, (k, rel_l2(g[k].reshape(ref.shape), ref))
     core.close()
+
+
+def test_chained_plan_launch_count_does_not_grow_with_critic_depth(cuda):
+    """The twin-critic passes of the layer-chained plan are one clustered launch each at every critic depth it accepts."""
+    from distributed_sac_b200.core import SacCore
+    counts = []
+    for critic_hidden in ([64] * 3, [64] * 6):
+        spec = sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=critic_hidden, batch=256)
+        core = SacCore(core_config(spec, precision=0), 0, seed=0)
+        counts.append(core.launches_per_step)
+        core.close()
+    assert counts[0] == counts[1], counts
 
 
 @pytest.mark.parametrize("state", ["fresh", "trained"])
