@@ -238,10 +238,14 @@ def mlp(params, net, x, tag=None):
     return x
 
 
-def policy_sample(spec, params, obs, eps, tag=None):
-    """LL/model.py:38-65. Returns action, log_prob (B,1), log_std (B,act)."""
+def policy_sample(spec, params, obs, eps, tag=None, keep=None):
+    """LL/model.py:38-65. Returns action, log_prob (B,1), log_std (B,act).  keep (a dict): receives the head output
+    [mu | raw log_std] under "head", with its gradient retained."""
     A = spec.act_dim
     out = mlp(params, "actor", obs, tag)
+    if keep is not None and out.requires_grad:
+        out.retain_grad()
+        keep["head"] = out
     mu = out[:, :A]
     log_std = torch.clamp(out[:, A:], -20, 2)
     std = torch.exp(log_std)
@@ -336,8 +340,11 @@ class PortLearner:
         q_loss.backward()
         self.opt_critic.step()
 
-        a_cur, logp, log_std = policy_sample(spec, p, s, eps_cur, "cur")
+        keep = {} if want_intermediates else None
+        a_cur, logp, log_std = policy_sample(spec, p, s, eps_cur, "cur", keep)
         xa = torch.cat([s, a_cur], -1)
+        if want_intermediates:
+            xa.retain_grad()          # its action columns: d(actor loss)/d(action) through the critics alone
         q1n, q2n = mlp(p, "q1", xa, "pi"), mlp(p, "q2", xa, "pi")      # already-updated critics
         qmin = min_tagged(q1n, q2n, "route:pi")
         pi_loss = torch.mean(-(qmin - alpha * logp)) / div
@@ -362,7 +369,8 @@ class PortLearner:
                "alpha_loss": alpha_loss.item(), "entropy": entropy.item()}
         if want_intermediates:
             out.update(y=y, q1=q1.detach(), q2=q2.detach(), a_next=a2, logp_next=logp2,
-                       a_cur=a_cur.detach(), logp_cur=logp.detach(), qmin=qmin.detach())
+                       a_cur=a_cur.detach(), logp_cur=logp.detach(), qmin=qmin.detach(),
+                       d_action=xa.grad[:, spec.obs_dim:].clone(), d_head=keep["head"].grad.clone())
         return out
 
 

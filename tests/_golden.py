@@ -220,14 +220,15 @@ def check_forced(tape, forced, what=""):
     return flips
 
 
-def kink_checked_step(core, port, spec, batch, e1, e2, replica=0, care=False, step_cuda=None):
+def kink_checked_step(core, port, spec, batch, e1, e2, replica=0, care=False, step_cuda=None, want_intermediates=False):
     """One step of `core` (from the port's state) and of `port` with the CUDA masks forced; returns (port outputs,
-    {tag: flipped bits}).  Raises AssertionError if a flipped bit is not a kink."""
+    {tag: flipped bits}).  Raises AssertionError if a flipped bit is not a kink.  want_intermediates: the port's outputs
+    include its per-row intermediates (computed with the forced masks)."""
     sync_core_to_port(core, port, replica)
     (step_cuda or (lambda: core.step(*batch, e1, e2)))()
     forced = cuda_relu_masks(core, spec, replica, care)
     with sp.ReluTape(forced) as tape:
-        out = (port.update if care else port.update_SAC)(*batch, e1, e2)
+        out = (port.update if care else port.update_SAC)(*batch, e1, e2, want_intermediates=want_intermediates)
     flips = check_forced(tape, forced)
     return out, flips
 

@@ -57,3 +57,21 @@ def test_manual_gradients_match_autograd_fp64():
             assert rel_l2(man.p[k], v.detach()) < 1e-9, k
     finally:
         torch.set_default_dtype(torch.float32)
+
+
+def test_port_backward_intermediates_match_manual():
+    """The autograd port's d(action) (through the critics alone) and d(mu|log_std) -- the per-row references of the CUDA
+    step's backward -- against the hand-derived ones, on a ragged MT problem with act_dim 1 and one hidden layer."""
+    for spec in (sp.SacSpec(state_dim=7, act_dim=3, actor_hidden=[20, 12], critic_hidden=[16, 24, 8], batch=33,
+                            num_tasks=4, weighted_loss=True),
+                 sp.SacSpec(state_dim=5, act_dim=1, actor_hidden=[36], critic_hidden=[20], batch=37)):
+        p = sp.init_params(spec, seed=2)
+        g = torch.Generator().manual_seed(8)
+        p = {k: v + 0.05 * torch.randn(v.shape, generator=g) for k, v in p.items()}
+        b = sp.synthetic_batch(spec, seed=4)
+        e1, e2 = torch.randn(spec.batch, spec.act_dim, generator=g), torch.randn(spec.batch, spec.act_dim, generator=g)
+        o = sp.PortLearner(spec, p).update_SAC(*b, e1, e2, want_intermediates=True)
+        I = smn.ManualLearner(spec, p, None, np.float32).update_SAC(*b, e1, e2)
+        for k in ("d_action", "d_head"):
+            assert o[k].shape == I[k].shape, (k, tuple(o[k].shape), I[k].shape)
+            assert rel_l2(o[k], I[k]) <= REL, (k, rel_l2(o[k], I[k]))
