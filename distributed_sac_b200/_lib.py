@@ -87,6 +87,11 @@ SYMBOLS = {
     "b200sac_replay_fill_synthetic": (C.c_int, [_VP, C.c_int64, C.c_uint64, _VP]),
     "b200sac_replay_size": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int64)]),
     "b200sac_replay_sample": (C.c_int, [_VP, C.c_int32] + [_VP] * 5 + [_VP]),
+    "b200sac_replay_create_prioritized": (C.c_int, [_VP, C.c_int64, C.c_uint64, C.c_double, C.c_double, C.c_double, C.POINTER(_VP)]),
+    "b200sac_replay_set_beta": (C.c_int, [_VP, C.c_int32, C.c_double, _VP]),
+    "b200sac_replay_set_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP]),
+    "b200sac_replay_get_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP]),
+    "b200sac_replay_sample_prioritized": (C.c_int, [_VP, C.c_int32] + [_VP] * 5 + [_VP, _VP]),
 }
 
 _lib = None

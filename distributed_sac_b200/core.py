@@ -419,14 +419,20 @@ class SacCore:
 
     def debug(self, name: str, replica=0) -> torch.Tensor:
         """Per-step intermediates (b200sac_debug_read): y, q1, ..., and the hidden activations "hA.<l>", "hQ.<l>", "hP.<l>",
-        "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used."""
+        "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used.  After a step from a prioritized
+        ring: "isw" (importance weights), "prio" (leaf values written) and "idx" (ring indices, int32)."""
         cap = self.cfg.batch * max(2 * self.cfg.act_dim, 1)
+        if name == "idx":                       # int32 ring indices (prioritized replay)
+            return self._debug_raw(name, replica, cap).view(torch.int32)
         if name == "psave":
             cap = 2 * self.cfg.batch * self.cfg.act_dim * 8
         elif name[0] == "h" or name.startswith("mixH"):
             widest = max(list(self.cfg.actor_hidden) + list(self.cfg.critic_hidden) + [4 * ((w + 3) // 4) * self.cfg.num_encoders
                                                                                         for w in self.cfg.mix_hidden])
             cap = 2 * self.cfg.batch * widest
+        return self._debug_raw(name, replica, cap)
+
+    def _debug_raw(self, name, replica, cap):
         out = torch.empty(cap)
         n = C.c_int64(0)
         _lib.check(self.lib.b200sac_debug_read(self._h, name.encode(), replica, _ptr(out), cap, C.byref(n), _stream()))
@@ -434,16 +440,29 @@ class SacCore:
 
 
 class Replay:
-    """Replay ring in HBM (where='device') or pinned host DRAM (where='host')."""
+    """Replay ring in HBM (where='device') or pinned host DRAM (where='host').
 
-    def __init__(self, core: SacCore, capacity: int, where: str = "device", seed: int = 0):
+    prioritized=dict(alpha=, beta=, eps=) makes a prioritized device ring (sum-tree sampling, importance-weighted critic
+    loss, priorities updated inside every step; see include/b200sac.h)."""
+
+    def __init__(self, core: SacCore, capacity: int, where: str = "device", seed: int = 0, prioritized=None):
         self.core = core
         self.lib = core.lib
         self._h = C.c_void_p(0)
         w = {"device": 0, "host": 1}[where]
-        _lib.check(self.lib.b200sac_replay_create(core._h, int(capacity), w, C.c_uint64(seed), C.byref(self._h)))
+        self.prioritized = None if prioritized is None else dict(prioritized)
+        if self.prioritized is not None:
+            if where != "device":
+                raise ValueError("prioritized replay needs the device ring (where='device')")
+            unknown = set(self.prioritized) - {"alpha", "beta", "eps"}
+            if unknown or len(self.prioritized) != 3:
+                raise ValueError(f"prioritized= takes exactly alpha, beta and eps (got {sorted(self.prioritized)})")
+            p = self.prioritized
+            _lib.check(self.lib.b200sac_replay_create_prioritized(core._h, int(capacity), C.c_uint64(seed), float(p["alpha"]),
+                                                                  float(p["beta"]), float(p["eps"]), C.byref(self._h)))
+        else:
+            _lib.check(self.lib.b200sac_replay_create(core._h, int(capacity), w, C.c_uint64(seed), C.byref(self._h)))
         self.where = where
-
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value and self.core._h.value:
             self.lib.b200sac_replay_destroy(self._h)
@@ -476,3 +495,37 @@ class Replay:
         idx = torch.empty(B, dtype=torch.int64)
         _lib.check(self.lib.b200sac_replay_sample(self._h, replica, _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d), _ptr(idx)))
         return (s, a, r, s2, d, idx) if with_indices else (s, a, r, s2, d)
+
+    # ---- prioritized replay -----------------------------------------------------------------
+    def set_beta(self, beta: float, replica=None):
+        """Importance-sampling exponent of one replica (None: all), in stream order: steps enqueued afterwards use it."""
+        for r in range(self.core.cfg.replicas) if replica is None else [int(replica)]:
+            _lib.check(self.lib.b200sac_replay_set_beta(self._h, r, float(beta), _stream()))
+
+    def set_priorities(self, idx, prio, replica=0):
+        """Raw priorities (>= 0; (prio + eps)^alpha is stored) of filled ring slots `idx`; a later entry wins a duplicate."""
+        idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1))
+        prio = np.ascontiguousarray(np.asarray(prio, dtype=np.float32).reshape(-1))
+        if idx.size != prio.size:
+            raise ValueError("idx and prio differ in length")
+        _lib.check(self.lib.b200sac_replay_set_priorities(self._h, int(replica), idx.size, C.c_void_p(idx.ctypes.data),
+                                                          C.c_void_p(prio.ctypes.data)))
+
+    def priorities(self, idx, replica=0) -> np.ndarray:
+        """Leaf values p of ring slots `idx` (an index -1 - t gives task t's root sum)."""
+        idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1))
+        out = np.empty(idx.size, dtype=np.float32)
+        _lib.check(self.lib.b200sac_replay_get_priorities(self._h, int(replica), idx.size, C.c_void_p(idx.ctypes.data),
+                                                          C.c_void_p(out.ctypes.data)))
+        return out
+
+    def sample_prioritized(self, replica=0):
+        """(s, a, r, s2, d, idx, w): one draw of the device PER sampler (its own draw counter), as CPU tensors."""
+        c = self.core.cfg
+        B = c.batch
+        s, a, r = torch.empty(B, c.obs_dim), torch.empty(B, c.act_dim), torch.empty(B, 1)
+        s2, d = torch.empty(B, c.obs_dim), torch.empty(B, 1)
+        idx, w = torch.empty(B, dtype=torch.int64), torch.empty(B)
+        _lib.check(self.lib.b200sac_replay_sample_prioritized(self._h, int(replica), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
+                                                              _ptr(idx), _ptr(w)))
+        return s, a, r, s2, d, idx, w

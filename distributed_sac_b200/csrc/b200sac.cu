@@ -29,6 +29,7 @@
 #include "care_kernels.cuh"
 #include "chain.cuh"
 #include "chain2.cuh"
+#include "per_kernels.cuh"
 
 using namespace bsac;
 
@@ -339,6 +340,11 @@ struct b200sac {
   float* split_d = nullptr;       // b200sac_step: handle-owned copy of the caller's minibatch arrays (stable graph pointers)
   float* loss_h = nullptr;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
   float* loss_h_dev = nullptr;    // its device-side address
+  // prioritized replay (allocated with the first prioritized ring): [3][R][B] importance weights of the step, leaf values
+  // the step wrote, its ring indices (int32); a forked stream for the priority update
+  float* per_buf = nullptr;
+  cudaStream_t per_fork = nullptr;
+  cudaEvent_t ev_per_src = nullptr, ev_per_done = nullptr;
 };
 
 struct b200sac_replay {
@@ -356,6 +362,16 @@ struct b200sac_replay {
   std::mutex mu;
   cudaEvent_t ev_gather = nullptr;   // device ring: recorded after the last enqueued gather (pushes wait for it under `mu`)
   bool gather_pending = false;
+  // prioritized ring (per_kernels.cuh): sum-trees, per-replica beta, and what the synchronous calls work with
+  bool per = false;
+  PerTree tr;
+  double* d_beta = nullptr;       // [R]
+  std::vector<long long> draws;   // [R] b200sac_replay_sample_prioritized calls so far (its Philox counter)
+  cudaStream_t st = nullptr;      // push / set / get / sample_prioritized work, synchronised before those calls return
+  long long* s_lidx = nullptr;    // scratch [kPerMaxB]
+  int* s_idx = nullptr;           // scratch [kPerMaxB]
+  float* s_f = nullptr;           // scratch [kPerMaxB]
+  float* s_rows = nullptr;        // scratch [B][row_stride]
 };
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -400,6 +416,10 @@ static int destroy_impl(b200sac* h) {
   cudaFree(h->split_d);
   cudaFree(h->chain_dbg);
   cudaFree(h->d_cmaps);
+  cudaFree(h->per_buf);
+  if (h->per_fork) cudaStreamDestroy(h->per_fork);
+  if (h->ev_per_src) cudaEventDestroy(h->ev_per_src);
+  if (h->ev_per_done) cudaEventDestroy(h->ev_per_done);
   if (h->side) cudaStreamDestroy(h->side);
   if (h->fork) cudaStreamDestroy(h->fork);
   if (h->ev_ingested) cudaEventDestroy(h->ev_ingested);
@@ -1581,8 +1601,24 @@ static cudaError_t launch_pair_k(void (*kern)(KArgs...), dim3 grid, dim3 block, 
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* evs = nullptr, bool allow_fork = false) {
-  bool fork_pending = false;
+// Prioritized replay: the draw of one step (indices into rb->d_idx, importance weights into the handle's per_buf).
+static cudaError_t per_sample_on(b200sac* h, b200sac_replay* rb, cudaStream_t s) {
+  return launch_k(per_sample_kernel, dim3(h->R), dim3(h->cfg.batch > 256 ? 512 : 256), 0, s, h->K, rb->tr, (const Counters*)h->cnt,
+                  0LL, 0, (const long long*)rb->d_fill, (const double*)rb->d_beta, rb->d_idx, h->per_buf, (long long)h->cfg.batch,
+                  rb->seed);
+}
+
+// The launch whose rows carry the step's TD target and pre-update critic values (the priority update follows it).
+static bool forms_critic_loss(const Launch& l) { return l.kind == L_CHEADS || (l.kind == L_CHAIN2 && l.chain2.kind == C2_CRITIC); }
+
+// per: prioritized ring of a sampled step -- the critic loss is importance-weighted and the priority update runs after the
+// critic-loss launch (forked off the critical path when allow_fork, joined before the step ends); per_next: the next step's
+// draw follows that update on the same stream (ev_sampled).
+static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* evs = nullptr, bool allow_fork = false,
+                    b200sac_replay* per = nullptr, bool per_next = false) {
+  bool fork_pending = false, per_pending = false;
+  StepConst K = h->K;
+  if (per) K.isw = h->per_buf;
   for (size_t i = 0; i < h->plan.size(); ++i) {
     Launch& l = h->plan[i];
     if (evs) CU(cudaEventRecord(evs[i], st));
@@ -1599,7 +1635,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
     }
     switch (l.kind) {
       case L_POLICY_DOUT:
-        launch_k(policy_dout_kernel, l.grid, l.block, 0, s, h->K, l.pdo);
+        launch_k(policy_dout_kernel, l.grid, l.block, 0, s, K, l.pdo);
         break;
       case L_CARE_TAB:
         launch_k(care_tables_kernel, l.grid, l.block, 0, s, l.ctab);
@@ -1632,21 +1668,21 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
       case L_POLICY: {
         PolicyHeadArgs P = l.pol;
         P.use_eps_buf = use_eps_buf ? 1 : 0;
-        launch_k(policy_head_kernel, l.grid, l.block, 0, s, h->K, P);
+        launch_k(policy_head_kernel, l.grid, l.block, 0, s, K, P);
         break;
       }
       case L_CHEADS:
-        launch_k(critic_heads_kernel, l.grid, l.block, 0, s, h->K, l.ch);
+        launch_k(critic_heads_kernel, l.grid, l.block, 0, s, K, l.ch);
         break;
       case L_AQHEADS:
-        launch_k(actor_q_heads_kernel, l.grid, l.block, 0, s, h->K, l.aq);
+        launch_k(actor_q_heads_kernel, l.grid, l.block, 0, s, K, l.aq);
         break;
       case L_HEADBWD:
-        if (l.bn == 4) launch_k(head_bwd4_kernel<1>, l.grid, l.block, l.smem, s, h->K, l.hb);
-        else launch_k(head_bwd_kernel, l.grid, l.block, l.smem, s, h->K, l.hb);
+        if (l.bn == 4) launch_k(head_bwd4_kernel<1>, l.grid, l.block, l.smem, s, K, l.hb);
+        else launch_k(head_bwd_kernel, l.grid, l.block, l.smem, s, K, l.hb);
         break;
       case L_ADAM:
-        launch_k(adam_kernel, l.grid, l.block, 0, s, h->K, l.ad);
+        launch_k(adam_kernel, l.grid, l.block, 0, s, K, l.ad);
         break;
       case L_CHAIN: {
         ChainArgs a = l.chain;
@@ -1654,16 +1690,16 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         const bool f = a.job[0].kind == CJ_FWD;
         with_chain_rows(l.bn, [&](auto rows) {
           constexpr int r = decltype(rows)::value;
-          return launch_k(f ? chain_kernel<true, r> : chain_kernel<false, r>, l.grid, l.block, l.smem, s, a, h->K);
+          return launch_k(f ? chain_kernel<true, r> : chain_kernel<false, r>, l.grid, l.block, l.smem, s, a, K);
         });
         break;
       }
       case L_WGRAD:
-        launch_k(wgrad_kernel, l.grid, l.block, l.smem, s, l.wg, h->K);
+        launch_k(wgrad_kernel, l.grid, l.block, l.smem, s, l.wg, K);
         break;
       case L_CHAIN2:
         with_chain_rows(l.bn, [&](auto rows) {
-          return launch_pair_k(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, h->K);
+          return launch_pair_k(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, K);
         });
         break;
     }
@@ -1671,8 +1707,29 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
       CU(cudaEventRecord(h->ev_fork_done, h->fork));
       fork_pending = true;
     }
+    if (per && forms_critic_loss(l)) {
+      cudaStream_t ps = st;
+      if (allow_fork) {
+        CU(cudaEventRecord(h->ev_per_src, s));
+        CU(cudaStreamWaitEvent(h->per_fork, h->ev_per_src, 0));
+        ps = h->per_fork;
+      }
+      const int B = h->cfg.batch, R = h->R;
+      launch_k(per_update_kernel, dim3(R), dim3(256), 0, ps, per->tr, 0, (const int*)per->d_idx, (long long)B, B,
+               (const float*)h->y.p, (const float*)h->q.p, h->y.rs, (const float*)nullptr, h->per_buf + (size_t)R * B,
+               (int*)(h->per_buf + (size_t)2 * R * B), (long long)B);
+      if (allow_fork) {
+        CU(cudaEventRecord(h->ev_per_done, ps));
+        per_pending = true;
+      }
+      if (per_next) {                                   // the next step's draw sees this step's priorities
+        per_sample_on(h, per, ps);
+        CU(cudaEventRecord(h->ev_sampled, ps));
+      }
+    }
   }
   if (fork_pending) CU(cudaStreamWaitEvent(st, h->ev_fork_done, 0));
+  if (per_pending) CU(cudaStreamWaitEvent(st, h->ev_per_done, 0));
   if (evs) CU(cudaEventRecord(evs[h->plan.size()], st));
   CU(cudaGetLastError());
   return 0;
@@ -2299,6 +2356,7 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     }
   } else {
     auto sample_on = [&](cudaStream_t s2) {
+      if (rb->per) return per_sample_on(h, rb, s2);
       return launch_k(sample_indices_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, s2, h->K,   // __launch_bounds__(512): 512 threads fit
                       (const Counters*)h->cnt, (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx, (long long)B, rb->seed);
     };
@@ -2306,7 +2364,7 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     else CU(cudaStreamWaitEvent(st, h->ev_sampled, 0));
     launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
              (const int*)rb->d_idx, (long long)B);
-    if (fork_next) {
+    if (fork_next && !rb->per) {                // (prioritized: the next draw follows this step's priority update)
       CU(cudaEventRecord(h->ev_ingested, st));
       CU(cudaStreamWaitEvent(h->fork, h->ev_ingested, 0));
       sample_on(h->fork);
@@ -2314,7 +2372,8 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     }
   }
   CU(cudaGetLastError());
-  return run_plan(h, st, use_eps, evs ? evs + 1 : nullptr, evs == nullptr && !h->stamping);
+  const bool per = variant == 2 && rb->per;
+  return run_plan(h, st, use_eps, evs ? evs + 1 : nullptr, evs == nullptr && !h->stamping, per ? rb : nullptr, per && fork_next);
 }
 
 // nsteps > 1 (device-ring sampling only): that many consecutive gradient steps captured in ONE graph, so a pipelined
@@ -2670,7 +2729,7 @@ extern "C" int b200sac_graph_timeline(b200sac_t* h, b200sac_replay_t* rb, int32_
                                       int32_t* n_out, void* stream) {
   if (!h || !rb || rb->h != h || rb->where != 0 || !out_us || !n_out) return fail(B200SAC_ERR_INVALID, "graph_timeline needs a device ring");
   CU(cudaSetDevice(h->device));
-  const int n = (int)h->plan.size() + 2;       // sample + ingest + plan
+  const int n = (int)h->plan.size() + 2 + (rb->per ? 1 : 0);   // sample + ingest + plan (+ the priority update)
   *n_out = n;
   if (cap < n) return fail(B200SAC_ERR_INVALID, "need room for %d launches", n);
   const int total = n * (iters + 1);
@@ -2899,6 +2958,10 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "d_action") { src = h->dact_dbg.p + replica * h->dact_dbg.rs; n = (int64_t)B * A; }
   else if (nm == "d_head") { src = h->dout_dbg.p + replica * h->dout_dbg.rs; n = (int64_t)B * 2 * A; }
   else if (nm == "psave") { src = h->psave.p + replica * h->psave.rs; n = (int64_t)2 * B * A * kSaveW; }   // [2B][A][8]: std, diff, tanh, act, jac, EPS, mask, logp_j
+  else if (nm == "isw" || nm == "prio" || nm == "idx") {   // prioritized replay: [B] weights, leaf values, ring indices (int32 bits)
+    if (!h->per_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a prioritized replay ring", name);
+    src = h->per_buf + ((nm == "isw" ? 0 : nm == "prio" ? 1 : 2) * (size_t)h->R + replica) * B; n = B;
+  }
   else if (nm == "chain_dbg") {
     if (!h->chain_dbg) return fail(B200SAC_ERR_INVALID, "chain_dbg needs B200SAC_CHAIN_DBG=1 at create time");
     src = reinterpret_cast<const float*>(h->chain_dbg); n = 2 * CH_DBG_SLOTS * 16;     // int64 stamps viewed as float pairs
@@ -2983,6 +3046,9 @@ extern "C" int b200sac_replay_destroy(b200sac_replay_t* rb) {
   if (rb->where == 0) cudaFree(rb->rows); else cudaFreeHost(rb->rows);
   cudaFree(rb->d_fill); cudaFree(rb->d_idx);
   if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
+  cudaFree(rb->tr.tree); cudaFree(rb->tr.maxp); cudaFree(rb->d_beta);
+  cudaFree(rb->s_lidx); cudaFree(rb->s_idx); cudaFree(rb->s_f); cudaFree(rb->s_rows);
+  if (rb->st) cudaStreamDestroy(rb->st);
   delete rb;
   return 0;
 }
@@ -3030,10 +3096,16 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
       float* dst = rb->rows + (size_t)replica * rb->rs_rows + ((size_t)task * rb->cap_per_task + hd) * rs;
       if (rb->where == 0) CU(cudaMemcpy(dst, src + (size_t)done * rs, (size_t)run * rs * sizeof(float), cudaMemcpyHostToDevice));
       else memcpy(dst, src + (size_t)done * rs, (size_t)run * rs * sizeof(float));
+      if (rb->per)                                 // the new rows get the current max p
+        per_fill_kernel<<<dim3(1, 1), 1024, 0, rb->st>>>(rb->tr, task, replica, hd, hd + run, hd + run);
       hd = (hd + run) % rb->cap_per_task;
       fl = std::min(fl + run, rb->cap_per_task);
       done += run;
     }
+  }
+  if (rb->per) {
+    CU(cudaGetLastError());
+    CU(cudaStreamSynchronize(rb->st));
   }
   if (rb->where == 0)
     CU(cudaMemcpy(rb->d_fill + (size_t)replica * rb->Teff, rb->fill.data() + (size_t)replica * rb->Teff,
@@ -3065,6 +3137,11 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
     CU(cudaFree(tmp));
   }
   std::lock_guard<std::mutex> lk(rb->mu);
+  if (rb->per) {                                   // rows [0, per) of every sub-ring get the current max p, the rest are empty
+    if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
+    per_fill_kernel<<<dim3(rb->Teff, h->R), 1024, 0, st>>>(rb->tr, 0, 0, 0, rb->tr.P, per);
+    CU(cudaGetLastError());
+  }
   for (auto& f : rb->fill) f = per;
   for (auto& hd : rb->head) hd = per % rb->cap_per_task;
   if (rb->where == 0)
@@ -3104,6 +3181,7 @@ extern "C" int b200sac_replay_sample(b200sac_replay_t* rb, int32_t replica, floa
   if (!rb || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
   b200sac* h = rb->h;
   if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica out of range");
+  if (rb->per) return fail(B200SAC_ERR_INVALID, "prioritized ring: sample with b200sac_replay_sample_prioritized (rows, indices, weights)");
   CU(cudaSetDevice(h->device));
   const int B = h->cfg.batch, obs = h->K.obs, A = h->K.act, rs = h->row_stride;
   std::vector<long long> idx;
@@ -3192,4 +3270,156 @@ extern "C" int b200sac_step_sampled(b200sac_t* h, b200sac_replay_t* rb, int32_t 
     h->prefetch_rb = rb;
   }
   return sb.end();
+}
+
+// ------------------------------------------------------------------------------------------
+// prioritized replay (per_kernels.cuh): a device ring with one sum-tree per (replica, task) sub-ring
+// ------------------------------------------------------------------------------------------
+extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity, uint64_t seed, double alpha, double beta,
+                                                 double eps, b200sac_replay_t** out) {
+  if (!h || !out) return fail(B200SAC_ERR_INVALID, "null argument");
+  *out = nullptr;
+  if (!(alpha >= 0.0) || !std::isfinite(alpha)) return fail(B200SAC_ERR_INVALID, "prioritized replay: alpha must be finite and >= 0 (got %g)", alpha);
+  if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "prioritized replay: beta must be in [0, 1] (got %g)", beta);
+  if (!(eps > 0.0) || !std::isfinite(eps)) return fail(B200SAC_ERR_INVALID, "prioritized replay: eps must be finite and > 0 (got %g)", eps);
+  b200sac_replay_t* rb = nullptr;
+  if (int rc = b200sac_replay_create(h, capacity, 0, seed, &rb)) return rc;
+  rb->per = true;
+  PerTree& tr = rb->tr;
+  tr.cap = rb->cap_per_task; tr.T = rb->Teff; tr.alpha = alpha; tr.eps = eps;
+  tr.P = 1; tr.levels = 0;
+  while (tr.P < tr.cap) { tr.P <<= 1; ++tr.levels; }
+  rb->draws.assign((size_t)h->R, 0);
+  const size_t nt = (size_t)h->R * tr.T;
+  std::vector<float> ones(nt, 1.f);
+  std::vector<double> betas((size_t)h->R, beta);
+  auto fail_free = [&](const char* what) {
+    b200sac_replay_destroy(rb);
+    return fail(B200SAC_ERR_NOMEM, "prioritized replay: %s failed", what);
+  };
+  if (cudaMalloc(&tr.tree, nt * 2 * (size_t)tr.P * sizeof(float)) != cudaSuccess ||
+      cudaMemset(tr.tree, 0, nt * 2 * (size_t)tr.P * sizeof(float)) != cudaSuccess)
+    return fail_free("sum-tree allocation");
+  if (cudaMalloc(&tr.maxp, nt * sizeof(float)) != cudaSuccess || cudaMalloc(&rb->d_beta, (size_t)h->R * sizeof(double)) != cudaSuccess ||
+      cudaMemcpy(tr.maxp, ones.data(), nt * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMemcpy(rb->d_beta, betas.data(), (size_t)h->R * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
+      cudaMalloc(&rb->s_lidx, kPerMaxB * sizeof(long long)) != cudaSuccess || cudaMalloc(&rb->s_idx, kPerMaxB * sizeof(int)) != cudaSuccess ||
+      cudaMalloc(&rb->s_f, kPerMaxB * sizeof(float)) != cudaSuccess ||
+      cudaMalloc(&rb->s_rows, (size_t)h->cfg.batch * h->row_stride * sizeof(float)) != cudaSuccess ||
+      cudaStreamCreateWithFlags(&rb->st, cudaStreamNonBlocking) != cudaSuccess)
+    return fail_free("allocation");
+  if (!h->per_buf) {
+    const size_t n = (size_t)3 * h->R * h->cfg.batch;
+    if (cudaMalloc(&h->per_buf, n * sizeof(float)) != cudaSuccess || cudaMemset(h->per_buf, 0, n * sizeof(float)) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&h->per_fork, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->ev_per_src, cudaEventDisableTiming) != cudaSuccess ||
+        cudaEventCreateWithFlags(&h->ev_per_done, cudaEventDisableTiming) != cudaSuccess)
+      return fail_free("step buffer allocation");
+  }
+  *out = rb;
+  return 0;
+}
+
+static int per_check(b200sac_replay* rb, int32_t replica) {
+  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
+  if (!rb->per) return fail(B200SAC_ERR_INVALID, "not a prioritized ring (b200sac_replay_create_prioritized)");
+  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  return 0;
+}
+
+// Waits (under rb->mu) until every step enqueued so far is done with the trees.
+static int per_quiesce(b200sac_replay* rb) {
+  if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
+  return 0;
+}
+
+extern "C" int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, double beta, void* stream) {
+  if (int rc = per_check(rb, replica)) return rc;
+  if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "beta must be in [0, 1] (got %g)", beta);
+  CU(cudaSetDevice(rb->h->device));
+  per_set_beta_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(rb->d_beta, replica, beta);
+  CU(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, const float* prio) {
+  if (int rc = per_check(rb, replica)) return rc;
+  if (n < 0 || (n > 0 && (!idx || !prio))) return fail(B200SAC_ERR_INVALID, "bad argument");
+  CU(cudaSetDevice(rb->h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  std::vector<int> ix((size_t)n);
+  for (int64_t i = 0; i < n; ++i) {
+    const long long k = idx[i];
+    if (k < 0 || k >= rb->cap) return fail(B200SAC_ERR_INVALID, "index %lld outside the ring [0, %lld)", k, rb->cap);
+    if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
+      return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
+    if (!(prio[i] >= 0.f) || !std::isfinite(prio[i])) return fail(B200SAC_ERR_INVALID, "priority %lld is not a finite value >= 0", (long long)i);
+    ix[(size_t)i] = (int)k;
+  }
+  if (int rc = per_quiesce(rb)) return rc;
+  for (int64_t i0 = 0; i0 < n; i0 += kPerMaxB) {          // chunks in order: a later index wins, as inside one chunk
+    const int m = (int)std::min<int64_t>(kPerMaxB, n - i0);
+    CU(cudaMemcpyAsync(rb->s_idx, ix.data() + i0, m * sizeof(int), cudaMemcpyHostToDevice, rb->st));
+    CU(cudaMemcpyAsync(rb->s_f, prio + i0, m * sizeof(float), cudaMemcpyHostToDevice, rb->st));
+    per_update_kernel<<<1, 256, 0, rb->st>>>(rb->tr, replica, rb->s_idx, 0, m, nullptr, nullptr, 0, rb->s_f, nullptr, nullptr, 0);
+    CU(cudaGetLastError());
+  }
+  CU(cudaStreamSynchronize(rb->st));
+  return 0;
+}
+
+extern "C" int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, float* p_out) {
+  if (int rc = per_check(rb, replica)) return rc;
+  if (n < 0 || (n > 0 && (!idx || !p_out))) return fail(B200SAC_ERR_INVALID, "bad argument");
+  for (int64_t i = 0; i < n; ++i)
+    if (idx[i] >= rb->cap || idx[i] < -(long long)rb->Teff)
+      return fail(B200SAC_ERR_INVALID, "index %lld: neither a ring slot [0, %lld) nor a task root [-%d, -1]", (long long)idx[i], rb->cap, rb->Teff);
+  CU(cudaSetDevice(rb->h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  if (int rc = per_quiesce(rb)) return rc;
+  for (int64_t i0 = 0; i0 < n; i0 += kPerMaxB) {
+    const int m = (int)std::min<int64_t>(kPerMaxB, n - i0);
+    CU(cudaMemcpyAsync(rb->s_lidx, idx + i0, m * sizeof(long long), cudaMemcpyHostToDevice, rb->st));
+    per_read_kernel<<<(m + 255) / 256, 256, 0, rb->st>>>(rb->tr, replica, rb->s_lidx, m, rb->s_f);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(p_out + i0, rb->s_f, m * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+    CU(cudaStreamSynchronize(rb->st));
+  }
+  return 0;
+}
+
+extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
+                                                 float* d, int64_t* idx_out, float* w_out) {
+  if (int rc = per_check(rb, replica)) return rc;
+  if (!s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
+  b200sac* h = rb->h;
+  const int B = h->cfg.batch, obs = h->K.obs, A = h->K.act, rs = h->row_stride, per = B / rb->Teff;
+  CU(cudaSetDevice(h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  for (int t = 0; t < rb->Teff; ++t)
+    if (rb->fill[(size_t)replica * rb->Teff + t] < 4LL * per)
+      return fail(B200SAC_ERR_STATE, "replay not ready: task %d holds %lld transitions, need >= %d (4 x per-task batch)", t,
+                  rb->fill[(size_t)replica * rb->Teff + t], 4 * per);
+  if (int rc = per_quiesce(rb)) return rc;
+  per_sample_kernel<<<1, B > 256 ? 512 : 256, 0, rb->st>>>(h->K, rb->tr, nullptr, rb->draws[(size_t)replica]++, replica,
+                                                           rb->d_fill, rb->d_beta, rb->s_idx, rb->s_f, (long long)B, rb->seed);
+  per_gather_kernel<<<B, 128, 0, rb->st>>>(rb->rows + (size_t)replica * rb->rs_rows, rs, rb->s_idx, rb->s_rows);
+  CU(cudaGetLastError());
+  std::vector<int> ix((size_t)B);
+  std::vector<float> rows((size_t)B * rs), w((size_t)B);
+  CU(cudaMemcpyAsync(ix.data(), rb->s_idx, B * sizeof(int), cudaMemcpyDeviceToHost, rb->st));
+  CU(cudaMemcpyAsync(w.data(), rb->s_f, B * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+  CU(cudaMemcpyAsync(rows.data(), rb->s_rows, rows.size() * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+  CU(cudaStreamSynchronize(rb->st));
+  for (int i = 0; i < B; ++i) {
+    const float* src = rows.data() + (size_t)i * rs;
+    memcpy(s + (size_t)i * obs, src, obs * sizeof(float));
+    memcpy(a + (size_t)i * A, src + obs, A * sizeof(float));
+    r[i] = src[obs + A];
+    memcpy(s2 + (size_t)i * obs, src + obs + A + 1, obs * sizeof(float));
+    d[i] = src[2 * obs + A + 1];
+    if (idx_out) idx_out[i] = ix[(size_t)i];
+    if (w_out) w_out[i] = w[(size_t)i];
+  }
+  return 0;
 }

@@ -167,13 +167,17 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     if (A.kind == C2_CRITIC) {             // qa, qb = Qt1, Qt2
       const float y = td_target(reward_scale * r_row, gamma * (1.f - d_row), qa, qb, alpha_row, lp_row);
       const float qn = J.net == 0 ? q1_row : q2_row;
-      const float dqv = 2.f * K.c_loss * (qn - y);
+      float dqv = 2.f * K.c_loss * (qn - y);
+      const float iw = K.isw ? K.isw[(long long)rep * B + row] : 1.f;   // prioritized replay: importance weight
+      if (K.isw) dqv = dqv * iw;
       sd[w] = dqv;
       (R.dq + rep * 2 * R.rsY)[J.net * B + row] = dqv;
       if (J.net == 0) {
         const float e1 = y - q1_row, e2 = y - q2_row;
+        float l = e1 * e1 + e2 * e2;
+        if (K.isw) l = l * iw;
         (R.y + rep * R.rsY)[row] = y;
-        (R.lq + rep * R.rsY)[row] = e1 * e1 + e2 * e2;
+        (R.lq + rep * R.rsY)[row] = l;
       }
     } else {                               // qa, qb = Q1, Q2 at (s, a~)
       float g1, g2;

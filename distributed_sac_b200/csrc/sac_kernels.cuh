@@ -41,10 +41,11 @@ struct StepConst {
   double beta1, beta2, adam_eps;
   unsigned long long seed;
   const HParams* hp;              // [R] per-replica hyperparameters
+  const float* isw;               // prioritized replay: [R][B] importance weights of the critic loss; null = uniform replay
   // Keeps sizeof(StepConst) at 136 bytes, so that the kernel arguments behind it keep their parameter-space offsets.
   // ptxas schedules a kernel differently when those move, even one that never reads the table: 32 bytes less cost the
   // policy head ~1.2 us per step of the 400-wide learners on an H100.
-  unsigned long long reserved[4];
+  unsigned long long reserved[3];
 };
 static_assert(sizeof(StepConst) == 136, "StepConst size moves the offsets of the kernel arguments behind it");
 
@@ -487,10 +488,15 @@ __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
     Y[row] = y;
     float* Q = P.q + rep * 2 * P.rsY;
     Q[row] = q1; Q[B + row] = q2;
+    float g1 = 2.f * K.c_loss * (q1 - y), g2 = 2.f * K.c_loss * (q2 - y), l = e1 * e1 + e2 * e2;
+    if (K.isw) {                                 // prioritized replay: importance-weighted critic loss
+      const float w = K.isw[(long long)rep * B + row];
+      g1 = g1 * w; g2 = g2 * w; l = l * w;
+    }
     float* DQ = P.dq + rep * 2 * P.rsY;
-    DQ[row] = 2.f * K.c_loss * (q1 - y);
-    DQ[B + row] = 2.f * K.c_loss * (q2 - y);
-    (P.lq + rep * P.rsY)[row] = e1 * e1 + e2 * e2;
+    DQ[row] = g1;
+    DQ[B + row] = g2;
+    (P.lq + rep * P.rsY)[row] = l;
   }
 }
 

@@ -83,7 +83,10 @@ class _BaseLearner:
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
-                     replay_where, precision=1):
+                     replay_where, precision=1, prioritized=None):
+        if prioritized is not None and replay_where != "device":
+            raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
+        self.prioritized = prioritized
         self.cfg = cfg_read(cfg_path)
         self.precision = precision
         self.write_mode = write_mode
@@ -108,6 +111,12 @@ class _BaseLearner:
         if checkpoint_path is not None:
             self.load_checkpoint(checkpoint_path)
             print("######## load checkpoint completely ########")
+
+    def set_per_beta(self, beta: float):
+        """Importance-sampling exponent of the prioritized ring (annealing), effective from the next update()."""
+        if self.prioritized is None:
+            raise ValueError("this learner was built without prioritized=")
+        self.memory.ring.set_beta(beta)
 
     def _core_config(self):
         c = self.cfg
@@ -424,11 +433,11 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
-                 precision=1):
+                 precision=1, prioritized=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision)
+                          precision, prioritized)
 
     def _set_dims(self):
         c = self.cfg
@@ -442,7 +451,7 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def _make_memory(self, where):
         return ReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, server=self.server, core=self.core,
-                            where=where)
+                            where=where, prioritized=self.prioritized)
 
 
 class VSACLearner(_TwoCriticMixin, _BaseLearner):
@@ -451,9 +460,9 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     log_name = "MT1_Distributed_VSAC"
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
-                 device_index=0, seed=0, replay_where="host", precision=1):
+                 device_index=0, seed=0, replay_where="host", precision=1, prioritized=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision)
+                          precision, prioritized)
 
     def _set_dims(self):
         c = self.cfg
@@ -467,7 +476,7 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def _make_memory(self, where):
         return ReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, server=self.server, core=self.core,
-                            where=where)
+                            where=where, prioritized=self.prioritized)
 
 
 class MTSACLearner(_BaseLearner):
@@ -478,10 +487,10 @@ class MTSACLearner(_BaseLearner):
     _iteration_key = "update_iteration"
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
-                 *, server=None, device_index=0, seed=0, replay_where="host", precision=1):
+                 *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision)
+                          precision, prioritized)
 
     def _set_dims(self):
         c = self.cfg
@@ -500,7 +509,7 @@ class MTSACLearner(_BaseLearner):
 
     def _make_memory(self, where):
         return MTReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, self.num_tasks, server=self.server,
-                              core=self.core, where=where)
+                              core=self.core, where=where, prioritized=self.prioritized)
 
     def _critic_checkpoint_entries(self, named):
         loc = {**self._module_state_dict("q1", named=named), **self._module_state_dict("q2", named=named)}

@@ -21,7 +21,7 @@ from .core import Replay
 
 
 class ReplayBuffer(threading.Thread):
-    def __init__(self, buffer_size, batch_size, seed, device, server=None, *, core=None, where="host"):
+    def __init__(self, buffer_size, batch_size, seed, device, server=None, *, core=None, where="host", prioritized=None):
         super().__init__()
         self.daemon = True
         if core is None:
@@ -34,7 +34,7 @@ class ReplayBuffer(threading.Thread):
         self.batch_size = int(batch_size)
         self.device = torch.device(device)
         self.core = core
-        self.ring = Replay(core, int(buffer_size), where=where, seed=int(seed))
+        self.ring = Replay(core, int(buffer_size), where=where, seed=int(seed), prioritized=prioritized)
         self._stop_evt = threading.Event()
 
     # ---- ingestion (reference: run(), replay_buffer.py:43-61) -------------------------------
@@ -70,7 +70,8 @@ class ReplayBuffer(threading.Thread):
 
     # ---- sampling --------------------------------------------------------------------------
     def sample(self):
-        """(states, actions, rewards, next_states, dones) fp32 on `device` (replay_buffer.py:63-73)."""
+        """(states, actions, rewards, next_states, dones) fp32 on `device` (replay_buffer.py:63-73).  A prioritized ring
+        draws with ring.sample_prioritized() instead (it also returns the indices and importance weights)."""
         return tuple(t.to(self.device, non_blocking=False) for t in self.ring.sample())
 
     def enqueue_step(self, core):
@@ -89,10 +90,11 @@ class MTReplayBuffer(ReplayBuffer):
     """ReplayBuffer(buffer_size, batch_size, seed, device, num_tasks, server): one sub-ring per task,
     B/T samples from each, then one shuffle (MS/replay_buffers.py:67-100)."""
 
-    def __init__(self, buffer_size, batch_size, seed, device, num_tasks, server=None, *, core=None, where="host"):
+    def __init__(self, buffer_size, batch_size, seed, device, num_tasks, server=None, *, core=None, where="host",
+                 prioritized=None):
         if core is not None and core.cfg.num_tasks != int(num_tasks):
             raise ValueError("num_tasks must match the learner's")
-        super().__init__(buffer_size, batch_size, seed, device, server, core=core, where=where)
+        super().__init__(buffer_size, batch_size, seed, device, server, core=core, where=where, prioritized=prioritized)
         self.num_tasks = int(num_tasks)
 
     def _unpack(self, data):

@@ -250,7 +250,9 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * log-prob term), or a hidden
  * activation whose sign pattern is the ReLU mask the step used: "hA.<l>" [2B][H] (rows [s';s]), "hQ.<l>" / "hP.<l>" /
  * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT),
- * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders). */
+ * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
+ * importance weights of its critic loss), "prio" [B] (the leaf values p it wrote) and "idx" [B] (its ring indices, int32
+ * bit patterns). */
 int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replica, float* out_host, int64_t cap_floats,
                        int64_t* n_floats, void* stream);
 
@@ -300,6 +302,31 @@ int b200sac_replay_size(b200sac_replay_t* rb, int32_t replica, int64_t* n);
  * (reference-shaped ReplayBuffer.sample()); idx_out (nullable) gets the ring indices. */
 int b200sac_replay_sample(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
                           float* d, int64_t* idx_out);
+
+/* ---- prioritized replay (device ring only) ------------------------------------------
+ * Each (replica, task) sub-ring has a sum-tree over its slots.  Leaf i holds p_i = (prio_i + eps)^alpha (fp32, the power in
+ * fp64 rounded once); internal nodes are recomputed sums of their children; empty slots hold 0 and are never drawn.
+ * A step draws, per task, B/T rows (B when num_tasks = 0) stratified with replacement: slot j draws u = (j + U(0,1)) S / (B/T)
+ * (S = the task's root sum) and descends; the Philox key is (seed, replica, step counter, slot).  Importance weights
+ * w_i = (N_t p_i / S_t)^-beta (N_t = fill of the sub-ring), divided by their maximum over the minibatch (fp64, rounded once),
+ * multiply the per-row critic gradient and loss term: dQk = (2c (Qk - y)) w, lq = (e1^2 + e2^2) w.  After the critic loss, in
+ * the step's graph, the sampled leaves get prio_i = (|y - Q1| + |y - Q2|) / 2 (the highest batch slot wins a duplicated
+ * index) and a running max p per (replica, task), initially 1, is raised; rows written by push / fill_synthetic get it.
+ * b200sac_step_sampled, b200sac_update and b200sac_prepare accept a prioritized ring; b200sac_replay_sample does not.
+ * alpha >= 0, 0 <= beta <= 1, eps > 0, else B200SAC_ERR_INVALID. */
+int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity, uint64_t seed, double alpha, double beta, double eps,
+                                      b200sac_replay_t** out);
+/* beta of one replica, in stream order on `stream`: steps enqueued afterwards use it (no graph is rebuilt). */
+int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, double beta, void* stream);
+/* Raw priorities (|delta|-like, >= 0; the exponent is applied inside) of n filled ring slots, e.g. actor-computed initial
+ * priorities; a later entry wins a duplicated index.  Raises max p.  Synchronous; ordered after every enqueued step. */
+int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, const float* prio);
+/* Leaf values p of n ring slots; an index -1 - t reads task t's root sum instead.  Synchronous, like set_priorities. */
+int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, float* p_out);
+/* Reference-shaped PER sample(): one draw of the device sampler with its own draw counter (0, 1, ... per replica) in place
+ * of the step counter; rows, ring indices (nullable) and importance weights (nullable) to HOST arrays. */
+int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
+                                      float* d, int64_t* idx_out, float* w_out);
 
 #ifdef __cplusplus
 }
