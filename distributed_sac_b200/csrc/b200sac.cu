@@ -1361,7 +1361,7 @@ static int build_plan(b200sac* h) {
     const int cols = wide ? kHb4Cols : kHbCols;
     l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
     l.block = dim3(256);
-    l.smem = ((size_t)rows_per * P.NO + (wide ? 1024 : 256) * (size_t)P.NO) * sizeof(float);
+    l.smem = ((((size_t)rows_per * P.NO + 3) & ~(size_t)3) + (wide ? 1024 : 256) * (size_t)P.NO) * sizeof(float);   // head_bwd4: red 16-B aligned
     h->plan.push_back(l);
   };
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
@@ -1468,10 +1468,12 @@ static int build_plan(b200sac* h) {
       Q.trunk = h->care_trunk; Q.ctx = h->care_ctx;
       Q.T = c.num_tasks; Q.K = Kenc; Q.co = c.ctx_out;
       Q.original = c.care == 2 ? 1 : 0; Q.off_ctx = h->care_off_ctx;
-      size_t fl = 0;
-      for (int j = 0; j < Q.trunk.n; ++j) fl += (size_t)c.num_tasks * Q.trunk.dims[j + 1];
-      for (int j = 0; j < Q.ctx.n; ++j) fl += (size_t)c.num_tasks * Q.ctx.dims[j + 1];
-      l2.smem = fl * sizeof(float);
+      int fl = 0;                                   // backward-chain floats of one task
+      for (int j = 0; j < Q.trunk.n; ++j) fl += Q.trunk.dims[j + 1];
+      for (int j = 0; j < Q.ctx.n; ++j) fl += Q.ctx.dims[j + 1];
+      if (fl > kCareTabWgradSmemFloats) plan_rc = fail(B200SAC_ERR_INVALID, "internal: one task's CARE backward chains exceed %d floats", kCareTabWgradSmemFloats);
+      Q.tchunk = std::max(1, std::min(c.num_tasks, kCareTabWgradSmemFloats / fl));
+      l2.smem = (size_t)Q.tchunk * fl * sizeof(float);
       l2.grid = dim3(sms, R);
       l2.block = dim3(256);
       h->plan.push_back(l2);

@@ -283,71 +283,88 @@ struct CareTabWgradArgs {
   CareNet trunk, ctx;
   int T, K, co;
   int original, off_ctx;              // CARE(O): trunk layer-0 input = z (table, off_ctx); ctx layer-0 input = relu(E[t])
+  int tchunk;                         // tasks whose backward chains are held in shared memory at once
 };
+
+// Shared memory of care_tab_wgrad_kernel: the default 48 KiB (no opt-in).  One task's chains are at most
+// 8 x 512 + 32 (trunk) + 9 x 512 (context net) = 8 736 floats, so every configuration check_cfg accepts fits one task at least.
+constexpr int kCareTabWgradSmemFloats = 12288;
 
 // grid (nblk, R), block 256.  Every CTA re-derives the (tiny) per-task backward chains in shared memory, then
 // takes a slice of the weight / bias gradient elements: dW_j[o][i] = sum_t dz_j[t][o] * a_{j-1}[t][i].
+// The tasks are taken in chunks of P.tchunk (T x the chains of one task can reach 2.2 MB): every gradient element's sum over
+// t continues from the value its thread stored after the previous chunk, so the summation order (t ascending) and with it
+// the result do not depend on the chunk size.
 __global__ void __launch_bounds__(256) care_tab_wgrad_kernel(CareTabWgradArgs P) {
   KStamp ks_;
   extern __shared__ float sm[];
-  const int rep = blockIdx.y, T = P.T;
+  const int rep = blockIdx.y;
   const float* __restrict__ par = P.params + rep * P.rsP;
-  const float* __restrict__ tab = P.tab + rep * P.rsTab;
-  const float* __restrict__ dtab = P.dtab + rep * P.rsDtab;
-  // dz storage: for net n, layer j: dz[n][j] is [T][dims[j+1]]
-  int dz_off[2][kCareMaxLayers];
-  int cur = 0;
-  for (int n = 0; n < 2; ++n) {
-    const CareNet& N = n == 0 ? P.trunk : P.ctx;
-    for (int j = 0; j < N.n; ++j) { dz_off[n][j] = cur; cur += T * N.dims[j + 1]; }
-  }
-  for (int n = 0; n < 2; ++n) {
-    const CareNet& N = n == 0 ? P.trunk : P.ctx;
-    const int last = N.n - 1, nlast = N.dims[N.n];
-    for (int e = threadIdx.x; e < T * nlast; e += 256) {
-      const int t = e / nlast, o = e % nlast;
-      sm[dz_off[n][last] + e] = dtab[(long long)t * (P.K + P.co) + (n == 0 ? o : P.K + o)];
+  const float* __restrict__ tab0 = P.tab + rep * P.rsTab;
+  const float* __restrict__ dtab0 = P.dtab + rep * P.rsDtab;
+  float* __restrict__ G = P.grads + rep * P.rsG;
+  const long long gstart = (long long)blockIdx.x * 256 + threadIdx.x, gstride = (long long)gridDim.x * 256;
+  for (int t0 = 0; t0 < P.T; t0 += P.tchunk) {
+    const int T = P.T - t0 < P.tchunk ? P.T - t0 : P.tchunk;       // tasks t0 .. t0 + T - 1
+    const float* __restrict__ tab = tab0 + (long long)t0 * P.row_w;
+    const float* __restrict__ dtab = dtab0 + (long long)t0 * (P.K + P.co);
+    const float* __restrict__ emb = par + P.emb_off + (long long)t0 * P.ctx.dims[0];
+    if (t0 > 0) __syncthreads();                       // every thread is done with the previous chunk's chains
+    // dz storage: for net n, layer j: dz[n][j] is [T][dims[j+1]]
+    int dz_off[2][kCareMaxLayers];
+    int cur = 0;
+    for (int n = 0; n < 2; ++n) {
+      const CareNet& N = n == 0 ? P.trunk : P.ctx;
+      for (int j = 0; j < N.n; ++j) { dz_off[n][j] = cur; cur += T * N.dims[j + 1]; }
     }
-    __syncthreads();
-    for (int j = last; j >= 1; --j) {                  // dz_{j-1} = (dz_j W_j) * [a_{j-1} > 0]
-      const int nin = N.dims[j], nout = N.dims[j + 1];
-      const float* __restrict__ W = par + N.w[j];
-      for (int e = threadIdx.x; e < T * nin; e += 256) {
-        const int t = e / nin, i = e % nin;
-        float s = 0.f;
-        for (int o = 0; o < nout; ++o) s = fmaf(sm[dz_off[n][j] + t * nout + o], __ldg(W + (long long)o * nin + i), s);
-        const float a = tab[(long long)t * P.row_w + N.act_off[j - 1] + i];
-        sm[dz_off[n][j - 1] + e] = a > 0.f ? s : 0.f;
+    for (int n = 0; n < 2; ++n) {
+      const CareNet& N = n == 0 ? P.trunk : P.ctx;
+      const int last = N.n - 1, nlast = N.dims[N.n];
+      for (int e = threadIdx.x; e < T * nlast; e += 256) {
+        const int t = e / nlast, o = e % nlast;
+        sm[dz_off[n][last] + e] = dtab[(long long)t * (P.K + P.co) + (n == 0 ? o : P.K + o)];
       }
       __syncthreads();
+      for (int j = last; j >= 1; --j) {                // dz_{j-1} = (dz_j W_j) * [a_{j-1} > 0]
+        const int nin = N.dims[j], nout = N.dims[j + 1];
+        const float* __restrict__ W = par + N.w[j];
+        for (int e = threadIdx.x; e < T * nin; e += 256) {
+          const int t = e / nin, i = e % nin;
+          float s = 0.f;
+          for (int o = 0; o < nout; ++o) s = fmaf(sm[dz_off[n][j] + t * nout + o], __ldg(W + (long long)o * nin + i), s);
+          const float a = tab[(long long)t * P.row_w + N.act_off[j - 1] + i];
+          sm[dz_off[n][j - 1] + e] = a > 0.f ? s : 0.f;
+        }
+        __syncthreads();
+      }
     }
-  }
-  // gradient elements of every (net, layer): [weights | bias], grid-strided per layer
-  const long long gstart = (long long)blockIdx.x * 256 + threadIdx.x, gstride = (long long)gridDim.x * 256;
-  for (int n = 0; n < 2; ++n) {
-    const CareNet& N = n == 0 ? P.trunk : P.ctx;
-    for (int j = 0; j < N.n; ++j) {
-      const int nin = N.dims[j], nout = N.dims[j + 1];
-      const long long nw = (long long)nin * nout, tot = nw + nout;
-      for (long long q = gstart; q < tot; q += gstride) {
-        float s = 0.f;
-        if (q < nw) {
-          const int o = (int)(q / nin), i = (int)(q % nin);
-          for (int t = 0; t < T; ++t) {
-            float a;
-            if (j > 0) a = tab[(long long)t * P.row_w + N.act_off[j - 1] + i];
-            else if (P.original && n == 0) a = tab[(long long)t * P.row_w + P.off_ctx + i];          // trunk(z.detach())
-            else {
-              a = par[P.emb_off + (long long)t * nin + i];
-              if (P.original) a = fmaxf(a, 0.f);                                                  // header(relu(E))
+    // gradient elements of every (net, layer): [weights | bias], grid-strided per layer
+    for (int n = 0; n < 2; ++n) {
+      const CareNet& N = n == 0 ? P.trunk : P.ctx;
+      for (int j = 0; j < N.n; ++j) {
+        const int nin = N.dims[j], nout = N.dims[j + 1];
+        const long long nw = (long long)nin * nout, tot = nw + nout;
+        for (long long q = gstart; q < tot; q += gstride) {
+          if (q < nw) {
+            const int o = (int)(q / nin), i = (int)(q % nin);
+            float s = t0 > 0 ? G[N.w[j] + q] : 0.f;
+            for (int t = 0; t < T; ++t) {
+              float a;
+              if (j > 0) a = tab[(long long)t * P.row_w + N.act_off[j - 1] + i];
+              else if (P.original && n == 0) a = tab[(long long)t * P.row_w + P.off_ctx + i];        // trunk(z.detach())
+              else {
+                a = emb[(long long)t * nin + i];
+                if (P.original) a = fmaxf(a, 0.f);                                                // header(relu(E))
+              }
+              s = fmaf(sm[dz_off[n][j] + t * nout + o], a, s);
             }
-            s = fmaf(sm[dz_off[n][j] + t * nout + o], a, s);
+            G[N.w[j] + q] = s;
+          } else {
+            const int o = (int)(q - nw);
+            float s = t0 > 0 ? G[N.b[j] + o] : 0.f;
+            for (int t = 0; t < T; ++t) s += sm[dz_off[n][j] + t * nout + o];
+            G[N.b[j] + o] = s;
           }
-          (P.grads + rep * P.rsG)[N.w[j] + q] = s;
-        } else {
-          const int o = (int)(q - nw);
-          for (int t = 0; t < T; ++t) s += sm[dz_off[n][j] + t * nout + o];
-          (P.grads + rep * P.rsG)[N.b[j] + o] = s;
         }
       }
     }

@@ -752,7 +752,7 @@ __global__ void __launch_bounds__(256) head_bwd4_kernel(StepConst K, HeadBwdArgs
   const int M = r1 - r0;
   if (M <= 0) return;
   float* sd = sm;                                   // [M][NO]
-  float* red = sm + (size_t)rows_per * NO;          // [16 row groups][16 col quads][NO][4]
+  float* red = sm + (((size_t)rows_per * NO + 3) & ~(size_t)3);   // [16 row groups][16 col quads][NO][4], 16-B aligned (float4)
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
 
   if (P.policy_mode) {

@@ -45,6 +45,8 @@ CASES = {
 # Just outside the envelope: each must take the per-layer fp32 plan (and still match the oracle there).
 OUTSIDE = {
     "width260": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[64, 48], critic_hidden=[260, 40], batch=64),
+    # (a batch that is not a multiple of 4: head_bwd4_kernel's scratch follows the batch's head gradients in shared memory)
+    "width260_b67": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[64, 48], critic_hidden=[260, 40], batch=67),
     "width254": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[254, 40], critic_hidden=[64, 48], batch=64),
     "input253": dict(state_dim=245, num_tasks=4, act_dim=4, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=48),
 }
