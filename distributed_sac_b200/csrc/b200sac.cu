@@ -231,6 +231,8 @@ struct Launch {
   GemmGroup grp;
   const TcProb* tprobs = nullptr;
   int bn = 64;
+  bool pair128 = false;  // L_GEMM_TC with bn = 128: the paired tile flavour (fixed when the plan is built)
+  int split = 1;         // GEMM launches: K slices of the group's weight gradients
   PolicyDoutArgs pdo;
   CareTabArgs ctab;
   CareMixArgs cmix;
@@ -479,11 +481,12 @@ static bool tc_eligible(const GemmProb& p) {
 }
 
 // Tile variants of the wgmma GEMM (gemm_tc.cuh): 128x64, 128x128 (B200SAC_TC_PAIR128=1: the paired flavour), 128x160.
+// A step plan reads the switch once, when it is built, and keeps the choice on its launches (Launch::pair128).
 typedef void (*TcKernel)(const TcProb*);
 static bool tc_pair128() { const char* e = getenv("B200SAC_TC_PAIR128"); return e && e[0] == '1'; }
-static TcKernel tc_kernel(int bn) {
+static TcKernel tc_kernel(int bn, bool pair128) {
   if (bn == 160) return gemm_tc_kernel<160, false>;
-  if (bn == 128) return tc_pair128() ? (TcKernel)gemm_tc_kernel<128, true> : (TcKernel)gemm_tc_kernel<128, false>;
+  if (bn == 128) return pair128 ? (TcKernel)gemm_tc_kernel<128, true> : (TcKernel)gemm_tc_kernel<128, false>;
   return gemm_tc_kernel<64, false>;
 }
 static size_t tc_smem(int bn) {
@@ -931,6 +934,7 @@ static int build_plan(b200sac* h) {
       return o;
     };
     std::vector<GemmProb> ps;
+    int split = 1;                        // what expand did to this group's weight gradients (launch labels)
     {
       int S = kSplitK;
       if (c.precision == 1) {
@@ -953,6 +957,8 @@ static int build_plan(b200sac* h) {
         }
       }
       expand(S, ps);
+      for (auto& p : ps_in)
+        if (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) split = S;
     }
     if (c.precision == 1) {
       std::vector<GemmProb> tc, rest;
@@ -972,6 +978,8 @@ static int build_plan(b200sac* h) {
         l.kind = L_GEMM_TC;
         l.branch = cur_branch;
         l.bn = bn;
+        l.pair128 = bn == 128 && tc_pair128();
+        l.split = split;
         l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
         l.block = dim3(TC_THREADS);
         l.smem = tc_smem(bn);
@@ -1002,6 +1010,7 @@ static int build_plan(b200sac* h) {
     for (auto& p : ps) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
     l.kind = L_GEMM_SMALL;
     l.branch = cur_branch;
+    l.split = split;
     l.grid = dim3((maxN + GS_T - 1) / GS_T, (maxM + GS_T - 1) / GS_T, (unsigned)(ps.size() * R));
     l.block = dim3(GS_THREADS);
     if (thin) {        // input-layer weight / input gradients (N = obs+act <= 16): gemm_thin.cuh
@@ -1665,7 +1674,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         launch_k(gemm_thin_kernel, l.grid, l.block, 0, s, l.grp);
         break;
       case L_GEMM_TC:
-        launch_k(tc_kernel(l.bn), l.grid, l.block, l.smem, s, l.tprobs);
+        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, l.tprobs);
         break;
       case L_POLICY: {
         PolicyHeadArgs P = l.pol;
@@ -2551,29 +2560,32 @@ extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, c
   return sb.end();
 }
 
-static const char* launch_name(const Launch& l, const std::vector<GemmProb>& hp, const GemmProb* dbase) {
+// Label of a plan launch.  GEMM launches name the engine, the wgmma tile (128x64 | 128x128 | 128x128 paired | 128x160) and,
+// when the group holds weight gradients, their K slices ("split S"); head_bwd names the 128-bit column mapping and its row
+// slices.  The part before '(' and the "wgmma" substring are what bench.py groups kernels by.
+static std::string launch_name(const Launch& l, const std::vector<GemmProb>& hp, const GemmProb* dbase) {
   switch (l.kind) {
-    case L_GEMM_TC: {
-      const GemmProb& p0 = hp[(size_t)(l.probs - dbase)];
-      const GemmProb& pl = hp[(size_t)(l.probs - dbase) + l.G - 1];
-      const bool w = l.bn == 128;
-      if (p0.mode == GEMM_FWD) return w ? "gemm_fwd(wgmma 128x128)" : "gemm_fwd(wgmma)";
-      if (p0.mode == GEMM_WGRAD && pl.mode == GEMM_DGRAD) return w ? "gemm_wgrad+dgrad(wgmma 128x128)" : "gemm_wgrad+dgrad(wgmma)";
-      if (p0.mode == GEMM_WGRAD) return w ? "gemm_wgrad(wgmma 128x128)" : "gemm_wgrad(wgmma)";
-      return w ? "gemm_dgrad(wgmma 128x128)" : "gemm_dgrad(wgmma)";
-    }
+    case L_GEMM_TC:
     case L_GEMM_BIG:
-    case L_GEMM_SMALL: {
-      const GemmProb& p0 = hp[(size_t)(l.probs - dbase)];
-      const GemmProb& pl = hp[(size_t)(l.probs - dbase) + l.G - 1];
-      if (p0.mode == GEMM_FWD) return "gemm_fwd(ffma)";
-      if (p0.mode == GEMM_WGRAD && pl.mode == GEMM_DGRAD) return "gemm_wgrad+dgrad(ffma)";
-      if (p0.mode == GEMM_WGRAD) return "gemm_wgrad(ffma)";
-      return "gemm_dgrad(ffma)";
-    }
+    case L_GEMM_SMALL:
     case L_GEMM_THIN: {
-      const GemmProb& p0 = hp[(size_t)(l.probs - dbase)];
-      return p0.mode == GEMM_WGRAD ? "gemm_wgrad(thin)" : "gemm_dgrad(thin)";
+      const size_t i0 = (size_t)(l.probs - dbase);
+      const GemmProb& p0 = hp[i0];
+      const GemmProb& pl = hp[i0 + l.G - 1];
+      bool wg = false;
+      for (int i = 0; i < l.G; ++i) wg = wg || hp[i0 + i].mode == GEMM_WGRAD;
+      // (thin launches are named after their first problem alone, as they always have been)
+      std::string s = p0.mode == GEMM_FWD ? "gemm_fwd(" : p0.mode == GEMM_DGRAD ? "gemm_dgrad(" :
+                      (pl.mode == GEMM_DGRAD && l.kind != L_GEMM_THIN) ? "gemm_wgrad+dgrad(" : "gemm_wgrad(";
+      if (l.kind == L_GEMM_TC) s += "wgmma 128x" + std::to_string(l.bn) + (l.pair128 ? " paired" : "");
+      else s += l.kind == L_GEMM_THIN ? "thin" : "ffma";
+      if (wg) s += ", split " + std::to_string(l.split);
+      return s + ")";
+    }
+    case L_HEADBWD: {
+      std::string s = (l.hb.policy_mode || l.hb.NO > 1) ? "head_bwd(policy, " : "head_bwd(q, ";
+      if (l.bn == 4) s += "128-bit, ";
+      return s + "row slices " + std::to_string(l.hb.row_slices) + ")";
     }
     case L_POLICY_DOUT: return "policy_dout";
     case L_CARE_TAB: return "care_tables";
@@ -2585,7 +2597,6 @@ static const char* launch_name(const Launch& l, const std::vector<GemmProb>& hp,
     case L_POLICY: return "policy_head";
     case L_CHEADS: return "critic_heads";
     case L_AQHEADS: return "actor_q_heads";
-    case L_HEADBWD: return (l.hb.policy_mode || l.hb.NO > 1) ? "head_bwd(policy)" : "head_bwd(q)";
     case L_CHAIN:
     case L_CHAIN2:
     case L_WGRAD: return l.label ? l.label : "chain";
@@ -2688,7 +2699,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  tc_kernel(bn)<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d);
+  tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
   cudaFree(d);
@@ -2717,7 +2728,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  for (int it = 0; it < 3; ++it) tc_kernel(bn)<<<grid, TC_THREADS, tc_smem(bn)>>>(d);
+  for (int it = 0; it < 3; ++it) tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn)>>>(d);
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out96, dbg, 96 * 8, cudaMemcpyDeviceToHost));
   cudaFree(A); cudaFree(B); cudaFree(C); cudaFree(dbg); cudaFree(d);
