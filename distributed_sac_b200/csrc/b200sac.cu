@@ -369,7 +369,7 @@ struct b200sac_replay {
   PerTree tr;
   double* d_beta = nullptr;       // [R]
   std::vector<long long> draws;   // [R] b200sac_replay_sample_prioritized calls so far (its Philox counter)
-  cudaStream_t st = nullptr;      // push / set / get / sample_prioritized work, synchronised before those calls return
+  cudaStream_t st = nullptr;      // device ring: push (and prioritized set / get / sample) work, synchronised before those calls return
   long long* s_lidx = nullptr;    // scratch [kPerMaxB]
   int* s_idx = nullptr;           // scratch [kPerMaxB]
   float* s_f = nullptr;           // scratch [kPerMaxB]
@@ -3037,8 +3037,10 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
     if (cudaMalloc(&rb->d_fill, sizeof(long long) * h->R * Teff) != cudaSuccess ||
         cudaMalloc(&rb->d_idx, sizeof(int) * h->R * h->cfg.batch) != cudaSuccess ||
         cudaMemset(rb->d_fill, 0, sizeof(long long) * h->R * Teff) != cudaSuccess ||
-        cudaEventCreateWithFlags(&rb->ev_gather, cudaEventDisableTiming) != cudaSuccess) {
+        cudaEventCreateWithFlags(&rb->ev_gather, cudaEventDisableTiming) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&rb->st, cudaStreamNonBlocking) != cudaSuccess) {
       cudaFree(rb->rows); cudaFree(rb->d_fill); cudaFree(rb->d_idx);
+      if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
       delete rb;
       return fail(B200SAC_ERR_NOMEM, "replay index allocation failed");
     }
@@ -3107,7 +3109,8 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
     while (done < cnt) {
       const long long run = std::min(cnt - done, rb->cap_per_task - hd);
       float* dst = rb->rows + (size_t)replica * rb->rs_rows + ((size_t)task * rb->cap_per_task + hd) * rs;
-      if (rb->where == 0) CU(cudaMemcpy(dst, src + (size_t)done * rs, (size_t)run * rs * sizeof(float), cudaMemcpyHostToDevice));
+      if (rb->where == 0)
+        CU(cudaMemcpyAsync(dst, src + (size_t)done * rs, (size_t)run * rs * sizeof(float), cudaMemcpyHostToDevice, rb->st));
       else memcpy(dst, src + (size_t)done * rs, (size_t)run * rs * sizeof(float));
       if (rb->per)                                 // the new rows get the current max p
         per_fill_kernel<<<dim3(1, 1), 1024, 0, rb->st>>>(rb->tr, task, replica, hd, hd + run, hd + run);
@@ -3116,13 +3119,15 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
       done += run;
     }
   }
-  if (rb->per) {
-    CU(cudaGetLastError());
+  if (rb->per) CU(cudaGetLastError());
+  // A copy from pageable memory may return before its DMA has landed, and a step enqueued on a non-blocking stream is not
+  // ordered after the legacy stream: the rows and the fill go on the ring's own stream, which is drained before the mutex
+  // is released, so every step enqueued after this call gathers the new rows.
+  if (rb->where == 0) {
+    CU(cudaMemcpyAsync(rb->d_fill + (size_t)replica * rb->Teff, rb->fill.data() + (size_t)replica * rb->Teff,
+                       sizeof(long long) * rb->Teff, cudaMemcpyHostToDevice, rb->st));
     CU(cudaStreamSynchronize(rb->st));
   }
-  if (rb->where == 0)
-    CU(cudaMemcpy(rb->d_fill + (size_t)replica * rb->Teff, rb->fill.data() + (size_t)replica * rb->Teff,
-                  sizeof(long long) * rb->Teff, cudaMemcpyHostToDevice));
   return 0;
 }
 
@@ -3318,8 +3323,7 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
       cudaMemcpy(rb->d_beta, betas.data(), (size_t)h->R * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
       cudaMalloc(&rb->s_lidx, kPerMaxB * sizeof(long long)) != cudaSuccess || cudaMalloc(&rb->s_idx, kPerMaxB * sizeof(int)) != cudaSuccess ||
       cudaMalloc(&rb->s_f, kPerMaxB * sizeof(float)) != cudaSuccess ||
-      cudaMalloc(&rb->s_rows, (size_t)h->cfg.batch * h->row_stride * sizeof(float)) != cudaSuccess ||
-      cudaStreamCreateWithFlags(&rb->st, cudaStreamNonBlocking) != cudaSuccess)
+      cudaMalloc(&rb->s_rows, (size_t)h->cfg.batch * h->row_stride * sizeof(float)) != cudaSuccess)
     return fail_free("allocation");
   if (!h->per_buf) {
     const size_t n = (size_t)3 * h->R * h->cfg.batch;
