@@ -10,13 +10,11 @@
 
 #include <algorithm>
 #include <cmath>
-#include <functional>
 #include <map>
 #include <mutex>
 #include <new>
 #include <random>
 #include <string>
-#include <tuple>
 #include <type_traits>
 #include <unordered_set>
 #include <vector>
@@ -218,7 +216,7 @@ struct Buf {           // [R][n] fp32 (or int32) slab slice
   long long rs = 0;    // replica stride in floats
 };
 
-enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_BIG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2 };
+enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2 };
 
 struct Launch {
   LaunchKind kind;
@@ -516,8 +514,15 @@ static double tc_group_cost(const std::vector<GemmProb>& v, int bn, int R) {
   const long long waves = (tiles * R + sms - 1) / sms;
   return (double)waves * tile;
 }
+// B200SAC_TC_BN forces the tile width: 128 or 160 select that width, any other value 64; unset, `unforced` is returned.
+static int tc_forced_bn(int unforced) {
+  const char* e = getenv("B200SAC_TC_BN");
+  if (!e) return unforced;
+  const int b = atoi(e);
+  return b == 128 ? 128 : (b == 160 ? 160 : 64);
+}
 static int tc_pick_bn(const std::vector<GemmProb>& v, int R) {
-  if (const char* e = getenv("B200SAC_TC_BN")) { const int b = atoi(e); return b == 128 ? 128 : (b == 160 ? 160 : 64); }
+  if (const int b = tc_forced_bn(0)) return b;
   int maxN = 0;
   for (auto& p : v) maxN = std::max(maxN, p.N);
   if (getenv("B200SAC_TC_OLDRULE")) {             // round-1 rule: 128 when the group still fills most of the GPU with 128x128 tiles
@@ -601,15 +606,448 @@ static auto with_chain_rows(int bn, F&& f) {
   return f(std::integral_constant<int, 2>{});
 }
 
-static int build_plan_fused(b200sac* h, const std::function<void(int, bool)>& adam) {
-  const b200sac_cfg& c = h->cfg;
-  const Layout& L = h->L;
-  const int B = c.batch, R = h->R, A = c.act_dim, sms = sm_count();
-  const int La = c.n_actor_hidden, Lc = c.n_critic_hidden;
-  const long long rsP = L.arena, rsG = L.trainable;
-  auto W = [&](int64_t off) { return h->params + off; };
-  auto Gp = [&](int64_t off) { return h->grads + off; };
+// ------------------------------------------------------------------------------------------
+// Launch descriptions shared by the step plan and batched inference (b200sac_act).  The plan describes every replica at
+// once (an operand and its replica stride); inference describes one replica: its base pointers and stride 0.
+// ------------------------------------------------------------------------------------------
+// the whole buffer (rep < 0) or replica rep of it alone
+static Buf rep_view(const Buf& b, int rep) { return rep < 0 ? b : Buf{b.p + (long long)rep * b.rs, 0}; }
+static int pitch(int w) { return (w + 3) & ~3; }   // row pitch of the CARE work buffers
 
+// forward of one layer over M rows: out = relu(X W^T + b), W and b from the parameter arena `par`
+static GemmProb fwd_prob(const Buf& par, const float* X, long long rsX, int M, const LayerOff& lo, float* out, long long rsOut) {
+  GemmProb p;
+  memset(&p, 0, sizeof(p));
+  p.A = X; p.rsA = rsX; p.lda = lo.ld;
+  p.B = par.p + lo.w; p.rsB = par.rs; p.ldb = lo.ld;
+  p.bias = par.p + lo.b; p.rsBias = par.rs;
+  p.C = out; p.rsC = rsOut; p.ldc = lo.out;
+  p.M = M; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = 1;
+  return p;
+}
+// weight and bias gradient of one layer over K rows into the gradient arena `grd`: dW = dZ^T X, db = column sums of dZ
+static GemmProb wgrad_prob(const Buf& grd, const float* dZ, long long rsdZ, const float* X, long long rsX, const LayerOff& lo, int K) {
+  GemmProb p;
+  memset(&p, 0, sizeof(p));
+  p.A = dZ; p.rsA = rsdZ; p.lda = lo.out;
+  p.B = X; p.rsB = rsX; p.ldb = lo.ld;
+  p.C = grd.p + lo.w; p.rsC = grd.rs; p.ldc = lo.ld;
+  p.C2 = grd.p + lo.b; p.rsC2 = grd.rs;
+  p.M = lo.out; p.N = lo.in; p.K = K; p.mode = GEMM_WGRAD;
+  return p;
+}
+// input gradient of one layer over M rows: out = (dZ W) * [mask > 0] (no mask: ungated)
+static GemmProb dgrad_prob(const Buf& par, const float* dZ, long long rsdZ, const LayerOff& lo, const float* mask, long long rsMask,
+                           float* out, long long rsOut, int M) {
+  GemmProb p;
+  memset(&p, 0, sizeof(p));
+  p.A = dZ; p.rsA = rsdZ; p.lda = lo.out;
+  p.B = par.p + lo.w; p.rsB = par.rs; p.ldb = lo.ld;
+  p.mask = mask; p.rsMask = rsMask; p.ldmask = lo.ld;
+  p.C = out; p.rsC = rsOut; p.ldc = lo.ld;
+  p.M = M; p.N = lo.in; p.K = lo.out; p.mode = GEMM_DGRAD;
+  return p;
+}
+
+// CARE encoder instances: 0 = critic's on [s';s] (2B rows), 1 = target's on s', 2 = critic's after its Adam step on s.
+// The K problems of mixture layer l of instance `inst` on XS rows [row0, row0 + rows), appended to ps.  Instance 0 keeps
+// the rows at the same place in its buffers, the others from row 0.
+static void mix_fwd_probs(const b200sac* h, int rep, int inst, int l, int row0, int rows, std::vector<GemmProb>& ps) {
+  const Layout& L = h->L;
+  const int rows_buf = inst == 0 ? 2 * h->cfg.batch : h->cfg.batch;   // rows held by the instance's buffers
+  const int out_row0 = inst == 0 ? row0 : 0;
+  const LayerOff& lo = L.mix[l];
+  const long long delta = inst == 1 ? L.target_delta : 0;
+  const bool last = (l == (int)L.mix.size() - 1);
+  const Buf par = rep_view(Buf{h->params, L.arena}, rep), xs = rep_view(h->XS, rep);
+  const Buf ob = rep_view(last ? h->mixZ[inst] : h->mixH[inst][l], rep);
+  for (int k = 0; k < h->cfg.num_encoders; ++k) {
+    GemmProb p;
+    memset(&p, 0, sizeof(p));
+    if (l == 0) { p.A = xs.p + (long long)row0 * h->K.obs; p.rsA = xs.rs; p.lda = h->K.obs; }
+    else {
+      const Buf ib = rep_view(h->mixH[inst][l - 1], rep);
+      p.A = ib.p + ((long long)k * rows_buf + out_row0) * pitch(lo.in); p.rsA = ib.rs; p.lda = pitch(lo.in);
+    }
+    p.B = par.p + delta + lo.w + (long long)k * lo.out * lo.in; p.rsB = par.rs; p.ldb = lo.in;
+    p.bias = par.p + delta + lo.b + (long long)k * lo.out; p.rsBias = par.rs;
+    p.C = ob.p + ((long long)k * rows_buf + out_row0) * pitch(lo.out); p.rsC = ob.rs; p.ldc = pitch(lo.out);
+    p.M = rows; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = last ? 0 : 1;
+    ps.push_back(p);
+  }
+}
+
+// per-task tables (trunk attention logits, context code) of the encoder instances insts, one per blockIdx.y
+static CareTabArgs care_tab_args(const b200sac* h, int rep, const std::vector<int>& insts) {
+  const b200sac_cfg& c = h->cfg;
+  CareTabArgs P;
+  memset(&P, 0, sizeof(P));
+  const Buf par = rep_view(Buf{h->params, h->L.arena}, rep);
+  P.params = par.p; P.rsP = par.rs; P.emb_off = h->L.off_emb;
+  P.trunk = h->care_trunk; P.ctx = h->care_ctx;
+  P.T = c.num_tasks; P.K = c.num_encoders; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
+  P.original = c.care == 2 ? 1 : 0;
+  for (size_t i = 0; i < insts.size(); ++i) {
+    P.inst_delta[i] = insts[i] == 1 ? h->L.target_delta : 0;
+    P.tab[i] = rep_view(h->careTab[insts[i]], rep).p;
+  }
+  P.rsTab = rep_view(h->careTab[0], rep).rs;
+  return P;
+}
+
+// Encoding of `rows` XS rows from xs_row0 by instance `inst`: [mixed state | context code] rows written to d1 and, from
+// row off2 of the job on, to d2 (d2.p = nullptr: none).
+struct EncJob { int inst, xs_row0, rows; Buf d1; int ld1; Buf d2; int ld2; int off2; };
+
+// attention mix of the instance's K encoder outputs with its task tables
+static CareMixArgs care_mix_args(const b200sac* h, int rep, const EncJob& e) {
+  const b200sac_cfg& c = h->cfg;
+  CareMixArgs P;
+  memset(&P, 0, sizeof(P));
+  const int rows_buf = e.inst == 0 ? 2 * c.batch : c.batch;
+  const Buf Z = rep_view(h->mixZ[e.inst], rep), tab = rep_view(h->careTab[e.inst], rep), tid = rep_view(h->tid, rep);
+  P.Z = Z.p; P.rsZ = Z.rs; P.kstride = (long long)rows_buf * pitch(c.mix_out); P.ldz = pitch(c.mix_out);
+  P.tab = tab.p; P.rsTab = tab.rs; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
+  P.off_ctx = h->care_off_ctx;
+  P.tid = (const int*)tid.p; P.rsR = tid.rs;
+  P.rows = e.rows; P.B = c.batch; P.K = c.num_encoders; P.mo = c.mix_out; P.co = c.ctx_out;
+  P.dst1 = e.d1.p; P.rsD1 = e.d1.rs; P.ld1 = e.ld1; P.dst2 = e.d2.p; P.rsD2 = e.d2.rs; P.ld2 = e.ld2; P.row_off2 = e.off2;
+  return P;
+}
+
+// ------------------------------------------------------------------------------------------
+// Step plan: build_plan sets the policy-head arguments, then build_plan_fused (the layer-chained plan) or
+// build_plan_layered (the per-layer plan) appends the launches of one step to h->plan with the launch builders below.
+// ------------------------------------------------------------------------------------------
+struct PlanBuilder {
+  b200sac* h;
+  const b200sac_cfg& c;
+  const Layout& L;
+  const int B, R, A, La, Lc, sms;
+  const long long rsP, rsG;
+  const Buf par, grd;       // parameter and gradient arenas
+  int branch = 0;           // branch tag given to the launches gemm_launch creates
+  int rc = 0;               // error met by a builder that cannot return one; build_plan returns it
+
+  explicit PlanBuilder(b200sac* hh)
+      : h(hh), c(hh->cfg), L(hh->L), B(c.batch), R(hh->R), A(c.act_dim), La(c.n_actor_hidden), Lc(c.n_critic_hidden),
+        sms(sm_count()), rsP(L.arena), rsG(L.trainable), par{hh->params, L.arena}, grd{hh->grads, L.trainable} {}
+  float* W(int64_t off) const { return h->params + off; }
+  float* Gp(int64_t off) const { return h->grads + off; }
+
+  void gemm_launch(const std::vector<GemmProb>& ps_in);
+  void care_tables(const std::vector<int>& insts);
+  void care_encode(const std::vector<EncJob>& jobs);
+  void head_bwd(bool policy, bool want_wgrad);
+  void adam(int which, bool tail_only);
+  int build_plan_fused();
+  void build_plan_layered();
+};
+
+void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
+  // Split-K for the weight gradients: K = batch (1024 / 1280) is the long dimension and M x N = out x in gives only a
+  // handful of tiles, so one CTA would walk 32-40 k chunks alone.
+  // WGRAD operands are both [K][*] row-major, so a K slice is just a row offset: slice s of a problem becomes its own
+  // problem writing gradient slice s; Adam adds the slices in index order (deterministic, no atomics).
+  auto expand = [&](int Smax, std::vector<GemmProb>& out) {
+    for (auto& p : ps_in) {
+      const int S = (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) ? Smax : 1;
+      if (S == 1) { out.push_back(p); continue; }
+      const int len = (((p.K + S - 1) / S) + 31) & ~31;
+      const long long coff = p.C - h->grads, c2off = p.C2 ? p.C2 - h->grads : 0;
+      if (coff < 0 || coff >= L.trainable) { rc = fail(B200SAC_ERR_INVALID, "internal: split-K output outside the gradient arena"); out.push_back(p); continue; }
+      for (int sidx = 0; sidx < S; ++sidx) {
+        const int kb = sidx * len;
+        if (kb >= p.K) break;
+        GemmProb q = p;
+        q.A = p.A + (long long)kb * p.lda; q.B = p.B + (long long)kb * p.ldb;
+        q.K = (p.K - kb < len) ? p.K - kb : len;
+        if (sidx > 0) {
+          float* base = h->grads_x + (long long)(sidx - 1) * R * L.trainable;
+          q.C = base + coff;
+          if (p.C2) q.C2 = base + c2off;
+        }
+        out.push_back(q);
+      }
+    }
+  };
+  // tensor-core tiles hold one CTA per SM: take the split factor (and with it the tile width) whose launch is cheapest under
+  // tc_group_cost's model -- a finer split shortens the k loop but a second wave of CTAs costs a whole tile time; the FFMA
+  // engine (several CTAs per SM) always takes the finest.
+  auto tc_only = [&](const std::vector<GemmProb>& v) {
+    std::vector<GemmProb> o;
+    for (auto& p : v) if (tc_eligible(p)) o.push_back(p);
+    return o;
+  };
+  std::vector<GemmProb> ps;
+  int split = 1;                        // what expand did to this group's weight gradients (launch labels)
+  {
+    int S = kSplitK;
+    if (c.precision == 1) {
+      double best = 1e300;
+      for (int s_ = kSplitK; s_ >= 1; s_ >>= 1) {
+        std::vector<GemmProb> trial;
+        expand(s_, trial);
+        const std::vector<GemmProb> o = tc_only(trial);
+        if (o.empty()) { S = s_; break; }
+        if (getenv("B200SAC_TC_OLDRULE")) {          // round-1 rule: the finest split that fits one wave
+          const int bn = tc_pick_bn(o, R);
+          long long ct = 0;
+          for (auto& p : o) ct += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
+          S = s_;
+          if (ct * R <= sms) break;
+          continue;
+        }
+        const double cost = tc_group_cost(o, tc_pick_bn(o, R), R);
+        if (cost < best) { best = cost; S = s_; }
+      }
+    }
+    expand(S, ps);
+    for (auto& p : ps_in)
+      if (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) split = S;
+  }
+  if (c.precision == 1) {
+    std::vector<GemmProb> tc, rest;
+    for (auto& p : ps) (tc_eligible(p) ? tc : rest).push_back(p);
+    if (!tc.empty()) {
+      Launch l;
+      int maxM = 0, maxN = 0;
+      for (auto& p : tc) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; }
+      const int bn = tc_pick_bn(tc, R);          // tile width: the cheapest of 64 / 128 / 160 under tc_group_cost's model
+      if (getenv("B200SAC_PLAN_DBG")) {
+        long long tiles = 0;
+        for (auto& p : tc) tiles += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
+        fprintf(stderr, "[plan] launch %zu: wgmma bn=%d problems=%zu tiles=%lld:", h->plan.size(), bn, tc.size(), tiles);
+        for (auto& p : tc) fprintf(stderr, " %s%dx%dx%d", p.mode == GEMM_FWD ? "F" : (p.mode == GEMM_DGRAD ? "D" : "W"), p.M, p.N, p.K);
+        fprintf(stderr, "\n");
+      }
+      l.kind = L_GEMM_TC;
+      l.branch = branch;
+      l.bn = bn;
+      l.pair128 = bn == 128 && tc_pair128();
+      l.split = split;
+      l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
+      l.block = dim3(TC_THREADS);
+      l.smem = tc_smem(bn);
+      l.G = (int)tc.size();
+      l.tprobs = (const TcProb*)(uintptr_t)h->h_tprobs.size();
+      l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // keep the SIMT descriptors too (labels)
+      for (int rep = 0; rep < R; ++rep)
+        for (auto& p : tc) {
+          TcProb t;
+          if (int e = make_tc_prob(p, rep, t, bn)) rc = e;
+          h->h_tprobs.push_back(t);
+        }
+      for (auto& p : tc) h->h_probs.push_back(p);
+      h->plan.push_back(l);
+    }
+    ps = rest;
+  }
+  // More problems than one parameter block holds: one launch per GS_MAXG of them, each labelled as a group of its own
+  // whose weight gradients need no further K slicing ("split 1").
+  if (ps.size() > GS_MAXG) split = 1;
+  for (size_t i0 = 0; i0 < ps.size(); i0 += GS_MAXG) {
+    const std::vector<GemmProb> g(ps.begin() + i0, ps.begin() + std::min(ps.size(), i0 + GS_MAXG));
+    Launch l;
+    int maxM = 0, maxN = 0;
+    bool thin = getenv("B200SAC_NO_THIN") == nullptr;
+    for (auto& p : g) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
+    l.kind = L_GEMM_SMALL;
+    l.branch = branch;
+    l.split = split;
+    l.grid = dim3((maxN + GS_T - 1) / GS_T, (maxM + GS_T - 1) / GS_T, (unsigned)(g.size() * R));
+    l.block = dim3(GS_THREADS);
+    if (thin) {        // input-layer weight / input gradients (N = obs+act <= 16): gemm_thin.cuh
+      int rows = 1;
+      for (auto& p : g) {
+        const int per = p.mode == GEMM_WGRAD ? GT_ROWS_WGRAD : GT_ROWS_DGRAD, r = (p.M + per - 1) / per;
+        rows = r > rows ? r : rows;
+      }
+      l.kind = L_GEMM_THIN;
+      l.grid = dim3(1, rows, (unsigned)(g.size() * R));
+      l.block = dim3(GT_THREADS);
+    }
+    l.G = (int)g.size();
+    memset(&l.grp, 0, sizeof(l.grp));
+    l.grp.G = l.G;
+    for (size_t i = 0; i < g.size(); ++i) l.grp.p[i] = g[i];
+    l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // index for now; rebased later
+    for (auto& p : g) h->h_probs.push_back(p);
+    h->plan.push_back(l);
+  }
+}
+
+void PlanBuilder::care_tables(const std::vector<int>& insts) {
+  Launch l;
+  l.kind = L_CARE_TAB;
+  l.ctab = care_tab_args(h, -1, insts);
+  l.grid = dim3(c.num_tasks, (unsigned)insts.size(), R);
+  l.block = dim3(512);
+  h->plan.push_back(l);
+}
+
+// mixture layers + attention mix of up to three encoder instances in ONE launch (care_mixfwd_kernel: all mixture weights of
+// an instance resident in shared memory); falls back to grouped GEMMs and care_mix_kernel when the weights do not fit
+void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
+  const int Kenc = c.num_encoders, nmix = (int)L.mix.size();
+  CareMixFwdArgs A;
+  memset(&A, 0, sizeof(A));
+  A.njobs = (int)jobs.size(); A.nl = nmix; A.K = Kenc; A.B = B;
+  if (const char* e = getenv("B200SAC_CMF_SKIP")) A.dbg_skip = atoi(e);
+  A.params = h->params; A.rsP = rsP;
+  A.XS = h->XS.p; A.rsXS = h->XS.rs; A.ldx = h->K.obs;
+  A.tid = (const int*)h->tid.p; A.rsR = h->r.rs;
+  A.row_w = h->care_row_w; A.off_att = h->care_off_att; A.off_ctx = h->care_off_ctx; A.mo = c.mix_out; A.co = c.ctx_out;
+  bool ok = nmix >= 1 && nmix <= CMF_MAXL && (int)jobs.size() <= CMF_MAXJOBS && getenv("B200SAC_NO_CARE_FUSED") == nullptr;
+  for (int l = 0; ok && l < nmix; ++l) {
+    A.w_off[l] = L.mix[l].w; A.b_off[l] = L.mix[l].b; A.in[l] = L.mix[l].in; A.out[l] = L.mix[l].out;
+    A.maxw = std::max(A.maxw, L.mix[l].out);
+  }
+  int cta = 0;
+  for (size_t i = 0; ok && i < jobs.size(); ++i) {
+    const EncJob& e = jobs[i];
+    CareMixFwdJob& J = A.job[i];
+    const int rows_buf = e.inst == 0 ? 2 * B : B;
+    J.inst_delta = e.inst == 1 ? L.target_delta : 0;
+    J.rows = e.rows; J.xs_row0 = e.xs_row0; J.out_row0 = e.inst == 0 ? e.xs_row0 : 0; J.rows_buf = rows_buf;
+    J.cta0 = cta; cta += (e.rows + CMF_ROWS - 1) / CMF_ROWS;
+    J.tab = h->careTab[e.inst].p; J.rsTab = h->careTab[e.inst].rs;
+    for (int l = 0; l < nmix; ++l) {
+      const Buf& ob = (l == nmix - 1) ? h->mixZ[e.inst] : h->mixH[e.inst][l];
+      J.H[l] = ob.p; J.rsH[l] = ob.rs;
+    }
+    J.dst1 = e.d1.p; J.rsD1 = e.d1.rs; J.ld1 = e.ld1; J.dst2 = e.d2.p; J.rsD2 = e.d2.rs; J.ld2 = e.ld2; J.row_off2 = e.off2;
+  }
+  const size_t smem = ok ? care_mixfwd_smem_floats(A) * sizeof(float) : 0;
+  if (ok && smem <= 225 * 1024 &&
+      cudaFuncSetAttribute(care_mixfwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) == cudaSuccess) {
+    Launch l;
+    l.kind = L_CARE_MIXFWD;
+    l.cmf = A;
+    l.grid = dim3(cta, R);
+    l.block = dim3(CMF_THREADS);
+    l.smem = smem;
+    h->plan.push_back(l);
+    return;
+  }
+  for (int l = 0; l < nmix; ++l) {
+    std::vector<GemmProb> ps;
+    for (const EncJob& e : jobs) mix_fwd_probs(h, -1, e.inst, l, e.xs_row0, e.rows, ps);
+    gemm_launch(ps);
+  }
+  for (const EncJob& e : jobs) {
+    Launch l;
+    l.kind = L_CARE_MIX;
+    l.cmix = care_mix_args(h, -1, e);
+    l.grid = dim3((e.rows + 7) / 8, R);
+    l.block = dim3(256);
+    h->plan.push_back(l);
+  }
+}
+
+void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
+  const int Hc = c.critic_hidden[Lc - 1], Ha = c.actor_hidden[La - 1];
+  Launch l;
+  l.kind = L_HEADBWD;
+  HeadBwdArgs& P = l.hb;
+  memset(&P, 0, sizeof(P));
+  P.M = B;
+  P.rsP = rsP; P.rsG = rsG;
+  if (!policy) {
+    P.NO = 1; P.Kdim = Hc; P.nets = 2;
+    for (int net = 0; net < 2; ++net) {
+      P.W[net] = W(L.q[net][Lc].w);
+      P.dW[net] = want_wgrad ? Gp(L.q[net][Lc].w) : nullptr;
+      P.db[net] = want_wgrad ? Gp(L.q[net][Lc].b) : nullptr;
+    }
+    const Buf& hb = want_wgrad ? h->hQ[Lc - 1] : h->hP[Lc - 1];
+    const Buf& dq = want_wgrad ? h->dq : h->dqa;
+    P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = 2 * h->y.rs;
+    P.h = hb.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hb.rs; P.ldh = Hc;
+    P.dh = h->dhQ[Lc - 1].p; P.rsDhNet = (long long)B * Hc; P.rsDhRep = h->dhQ[Lc - 1].rs; P.lddh = Hc;
+  } else {
+    const bool split = (long long)B * A > 2048;      // large batch: one tiny kernel computes d(mu|log_std) for all rows
+    if (split) {
+      Launch pl;
+      pl.kind = L_POLICY_DOUT;
+      PolicyDoutArgs& Q = pl.pdo;
+      memset(&Q, 0, sizeof(Q));
+      Q.dx = h->dxP.p; Q.rsDxNet = (long long)B * h->K.ldx; Q.rsDxRep = h->dxP.rs; Q.lddx = h->K.ldx;
+      Q.psave = h->psave.p + (long long)B * A * kSaveW; Q.rsSave = h->psave.rs;
+      Q.tid = (const int*)h->tid.p; Q.rsR = h->r.rs;
+      Q.log_alpha = W(L.off_alpha); Q.rsP = rsP;
+      Q.dout = h->dout_dbg.p; Q.dact = h->dact_dbg.p; Q.rsDout = h->dout_dbg.rs;
+      Q.M = B;
+      pl.grid = dim3((B * A + 255) / 256, R);
+      pl.block = dim3(256);
+      h->plan.push_back(pl);
+    }
+    P.NO = 2 * A; P.Kdim = Ha; P.nets = 1; P.policy_mode = split ? 0 : 1;
+    if (split) { P.dout = h->dout_dbg.p; P.rsDoutNet = 0; P.rsDoutRep = h->dout_dbg.rs; }
+    const LayerOff& lo = L.actor[La];
+    P.W[0] = W(lo.w); P.dW[0] = Gp(lo.w); P.db[0] = Gp(lo.b);
+    P.h = h->hA[La - 1].p + (long long)B * Ha; P.rsHrep = h->hA[La - 1].rs; P.ldh = Ha;   // rows B..2B-1 (= s half)
+    P.dh = h->dhA[La - 1].p; P.rsDhRep = h->dhA[La - 1].rs; P.lddh = Ha;
+    P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
+    P.psave = h->psave.p + (long long)B * A * kSaveW; P.rsSave = h->psave.rs;
+    P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
+    P.log_alpha = W(L.off_alpha);
+    P.dout_dbg = h->dout_dbg.p; P.dact_dbg = h->dact_dbg.p; P.rsDbg = h->dout_dbg.rs;
+  }
+  // large batches: rows cut into slices (4x the CTAs, a quarter of the serial row loop each); slice s >= 1 leaves its
+  // partial head-weight gradient in gradient slice s, exactly like the split-K GEMM weight gradients
+  P.row_slices = h->gslices;
+  P.xs = (long long)R * L.trainable;
+  for (int net = 0; net < P.nets; ++net)
+    if (P.dW[net] && h->grads_x) { P.dWx[net] = h->grads_x + (P.dW[net] - h->grads); P.dbx[net] = h->grads_x + (P.db[net] - h->grads); }
+  const int rows_per = (B + P.row_slices - 1) / P.row_slices;
+  // 128-bit column mapping when every row pitch / tensor offset involved is a multiple of 4 floats (l.bn = 4 marks it)
+  // -- for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
+  // few to fill the GPU
+  const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0 && getenv("B200SAC_HEADBWD_NARROW") == nullptr;
+  l.bn = wide ? 4 : 1;
+  const int cols = wide ? kHb4Cols : kHbCols;
+  l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
+  l.block = dim3(256);
+  l.smem = ((((size_t)rows_per * P.NO + 3) & ~(size_t)3) + (wide ? 1024 : 256) * (size_t)P.NO) * sizeof(float);   // head_bwd4: red 16-B aligned
+  h->plan.push_back(l);
+}
+
+// parameter update + the tail job (last CTA); tail_only: the tail job alone, on the fork stream, plus the critic-loss
+// reduction (the layer-chained plan, whose parameter updates are fused into the weight-gradient launches)
+void PlanBuilder::adam(int which, bool tail_only) {
+  Launch l;
+  l.kind = L_ADAM;
+  AdamArgs& P = l.ad;
+  memset(&P, 0, sizeof(P));
+  const int64_t beg = which == 0 ? L.critic_begin : (which == 1 ? L.actor_begin : L.cenc_begin);
+  const int64_t n = which == 0 ? L.critic_n : (which == 1 ? L.actor_n : L.cenc_n);
+  P.p = h->params + beg; P.m = h->adam_m + beg; P.v = h->adam_v + beg; P.g = h->grads + beg;
+  P.rsP = rsP; P.rsM = rsG; P.n = n;
+  P.gx = h->grads_x ? h->grads_x + beg : nullptr; P.xs = (long long)R * L.trainable; P.nx = h->gslices - 1;
+  P.target_delta = which == 0 ? L.target_delta : 0;
+  P.tau2_begin = (which == 0 && c.care) ? (L.cse_begin - L.critic_begin) : (long long)1 << 60;
+  P.which = which == 2 ? 4 : which;                    // counter slot: 0 critic, 1 actor, 4 context encoder
+  P.cnt = h->cnt;
+  P.tail = which == 0 ? TAIL_CRITIC_LOSS : (which == 1 ? TAIL_ALPHA_AND_LOSSES : TAIL_NONE);
+  if (tail_only) P.tail = TAIL_ALL;
+  P.lq = h->lq.p; P.la = h->la.p; P.rsY = h->y.rs;
+  P.logp_cur = h->logp.p + B; P.logstd_sum = h->logstd.p + B; P.rsLogp = h->logp.rs;
+  P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
+  P.log_alpha = h->params + L.off_alpha;
+  P.m_alpha = h->adam_m + L.off_alpha; P.v_alpha = h->adam_v + L.off_alpha; P.g_alpha = h->grads + L.off_alpha;
+  P.losses = h->losses; P.losses_host = h->loss_h_dev; P.R = R;
+  int nb = (int)((n + 256 * 4 - 1) / (256 * 4));
+  if (nb < 1) nb = 1;
+  if (nb > 592) nb = 592;
+  l.grid = dim3(nb + (P.tail != TAIL_NONE ? 1 : 0), R);
+  l.block = dim3(256);
+  l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
+  if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
+  h->plan.push_back(l);
+}
+
+int PlanBuilder::build_plan_fused() {
   ChainRows rw;
   memset(&rw, 0, sizeof(rw));
   rw.r = h->r.p; rw.d = h->d.p; rw.tid = (const int*)h->tid.p; rw.rsR = h->r.rs;
@@ -879,389 +1317,37 @@ static int build_plan_fused(b200sac* h, const std::function<void(int, bool)>& ad
   return 0;
 }
 
-// Build the launch list of one gradient step (everything after the ingest kernel).
-static int build_plan(b200sac* h) {
-  const b200sac_cfg& c = h->cfg;
-  const Layout& L = h->L;
-  const int B = c.batch, R = h->R, A = c.act_dim, sms = sm_count();
-  const int La = c.n_actor_hidden, Lc = c.n_critic_hidden;
-  const long long rsP = L.arena, rsG = L.trainable;
-  std::vector<std::vector<GemmProb>> groups;
-  struct Pending { int group; };
-  auto W = [&](int64_t off) { return h->params + off; };
-  auto Gp = [&](int64_t off) { return h->grads + off; };
-
-  int plan_rc = 0;
-  int cur_branch = 0;            // branch tag given to the launches gemm_launch creates
+// ---- per-layer plan: one grouped GEMM launch per layer (and kind) of the networks --------------------------------
+void PlanBuilder::build_plan_layered() {
+  const int Kenc = c.num_encoders, nmix = c.care ? (int)L.mix.size() : 0;
   // FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads the rest of the
   // backward chain.  The weight-gradient launch goes to the fork stream and the chain continues at once (the kernels hold
   // <= 2 CTAs per SM, so both fit); Adam joins.  (tensor-core tiles own a whole SM each: grouping is better there.)
   const bool use_fork = (c.precision == 0) && !c.care && getenv("B200SAC_NO_FORK") == nullptr;
-  std::function<void(std::vector<GemmProb>)> gemm_launch_ref;
-  auto gemm_launch = [&](std::vector<GemmProb> ps_in) {
-    // Split-K for the weight gradients: K = batch (1024 / 1280) is the long dimension and M x N = out x in gives only a
-    // handful of tiles, so one CTA would walk 32-40 k chunks alone.
-    // WGRAD operands are both [K][*] row-major, so a K slice is just a row offset: slice s of a problem becomes its own
-    // problem writing gradient slice s; Adam adds the slices in index order (deterministic, no atomics).
-    auto expand = [&](int Smax, std::vector<GemmProb>& out) {
-      for (auto& p : ps_in) {
-        const int S = (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) ? Smax : 1;
-        if (S == 1) { out.push_back(p); continue; }
-        const int len = (((p.K + S - 1) / S) + 31) & ~31;
-        const long long coff = p.C - h->grads, c2off = p.C2 ? p.C2 - h->grads : 0;
-        if (coff < 0 || coff >= L.trainable) { plan_rc = fail(B200SAC_ERR_INVALID, "internal: split-K output outside the gradient arena"); out.push_back(p); continue; }
-        for (int sidx = 0; sidx < S; ++sidx) {
-          const int kb = sidx * len;
-          if (kb >= p.K) break;
-          GemmProb q = p;
-          q.A = p.A + (long long)kb * p.lda; q.B = p.B + (long long)kb * p.ldb;
-          q.K = (p.K - kb < len) ? p.K - kb : len;
-          if (sidx > 0) {
-            float* base = h->grads_x + (long long)(sidx - 1) * R * L.trainable;
-            q.C = base + coff;
-            if (p.C2) q.C2 = base + c2off;
-          }
-          out.push_back(q);
-        }
-      }
-    };
-    // tensor-core tiles hold one CTA per SM: take the split factor (and with it the tile width) whose launch is cheapest under
-    // tc_group_cost's model -- a finer split shortens the k loop but a second wave of CTAs costs a whole tile time; the FFMA
-    // engine (several CTAs per SM) always takes the finest.
-    auto tc_only = [&](const std::vector<GemmProb>& v) {
-      std::vector<GemmProb> o;
-      for (auto& p : v) if (tc_eligible(p)) o.push_back(p);
-      return o;
-    };
-    std::vector<GemmProb> ps;
-    int split = 1;                        // what expand did to this group's weight gradients (launch labels)
-    {
-      int S = kSplitK;
-      if (c.precision == 1) {
-        double best = 1e300;
-        for (int s_ = kSplitK; s_ >= 1; s_ >>= 1) {
-          std::vector<GemmProb> trial;
-          expand(s_, trial);
-          const std::vector<GemmProb> o = tc_only(trial);
-          if (o.empty()) { S = s_; break; }
-          if (getenv("B200SAC_TC_OLDRULE")) {          // round-1 rule: the finest split that fits one wave
-            const int bn = tc_pick_bn(o, R);
-            long long ct = 0;
-            for (auto& p : o) ct += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
-            S = s_;
-            if (ct * R <= sms) break;
-            continue;
-          }
-          const double cost = tc_group_cost(o, tc_pick_bn(o, R), R);
-          if (cost < best) { best = cost; S = s_; }
-        }
-      }
-      expand(S, ps);
-      for (auto& p : ps_in)
-        if (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) split = S;
-    }
-    if (c.precision == 1) {
-      std::vector<GemmProb> tc, rest;
-      for (auto& p : ps) (tc_eligible(p) ? tc : rest).push_back(p);
-      if (!tc.empty()) {
-        Launch l;
-        int maxM = 0, maxN = 0;
-        for (auto& p : tc) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; }
-        const int bn = tc_pick_bn(tc, R);          // tile width: the cheapest of 64 / 128 / 160 under tc_group_cost's model
-        if (getenv("B200SAC_PLAN_DBG")) {
-          long long tiles = 0;
-          for (auto& p : tc) tiles += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
-          fprintf(stderr, "[plan] launch %zu: wgmma bn=%d problems=%zu tiles=%lld:", h->plan.size(), bn, tc.size(), tiles);
-          for (auto& p : tc) fprintf(stderr, " %s%dx%dx%d", p.mode == GEMM_FWD ? "F" : (p.mode == GEMM_DGRAD ? "D" : "W"), p.M, p.N, p.K);
-          fprintf(stderr, "\n");
-        }
-        l.kind = L_GEMM_TC;
-        l.branch = cur_branch;
-        l.bn = bn;
-        l.pair128 = bn == 128 && tc_pair128();
-        l.split = split;
-        l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
-        l.block = dim3(TC_THREADS);
-        l.smem = tc_smem(bn);
-        l.G = (int)tc.size();
-        l.tprobs = (const TcProb*)(uintptr_t)h->h_tprobs.size();
-        l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // keep the SIMT descriptors too (labels)
-        for (int rep = 0; rep < R; ++rep)
-          for (auto& p : tc) {
-            TcProb t;
-            if (int rc = make_tc_prob(p, rep, t, bn)) plan_rc = rc;
-            h->h_tprobs.push_back(t);
-          }
-        for (auto& p : tc) h->h_probs.push_back(p);
-        h->plan.push_back(l);
-      }
-      if (rest.empty()) return;
-      ps = rest;
-    }
-    if (ps.size() > GS_MAXG) {            // more problems than one parameter block holds: several launches
-      std::vector<GemmProb> head(ps.begin(), ps.begin() + GS_MAXG), tail(ps.begin() + GS_MAXG, ps.end());
-      gemm_launch_ref(head);
-      gemm_launch_ref(tail);
-      return;
-    }
-    Launch l;
-    int maxM = 0, maxN = 0;
-    bool thin = getenv("B200SAC_NO_THIN") == nullptr;
-    for (auto& p : ps) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
-    l.kind = L_GEMM_SMALL;
-    l.branch = cur_branch;
-    l.split = split;
-    l.grid = dim3((maxN + GS_T - 1) / GS_T, (maxM + GS_T - 1) / GS_T, (unsigned)(ps.size() * R));
-    l.block = dim3(GS_THREADS);
-    if (thin) {        // input-layer weight / input gradients (N = obs+act <= 16): gemm_thin.cuh
-      int rows = 1;
-      for (auto& p : ps) {
-        const int per = p.mode == GEMM_WGRAD ? GT_ROWS_WGRAD : GT_ROWS_DGRAD, r = (p.M + per - 1) / per;
-        rows = r > rows ? r : rows;
-      }
-      l.kind = L_GEMM_THIN;
-      l.grid = dim3(1, rows, (unsigned)(ps.size() * R));
-      l.block = dim3(GT_THREADS);
-    }
-    l.G = (int)ps.size();
-    if (ps.size() > GS_MAXG) plan_rc = fail(B200SAC_ERR_INVALID, "internal: more than %d problems in one GEMM group", GS_MAXG);
-    memset(&l.grp, 0, sizeof(l.grp));
-    l.grp.G = l.G;
-    for (size_t i = 0; i < ps.size() && i < GS_MAXG; ++i) l.grp.p[i] = ps[i];
-    l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // index for now; rebased later
-    for (auto& p : ps) h->h_probs.push_back(p);
-    h->plan.push_back(l);
-  };
-  gemm_launch_ref = gemm_launch;
-
-  // ---- CARE helpers ------------------------------------------------------------------------
-  const int Kenc = c.num_encoders, nmix = c.care ? (int)L.mix.size() : 0;
-  auto pitch = [](int w) { return (w + 3) & ~3; };
-  // mixture-of-encoders forward of encoder instance `inst` (0: critic's on XS rows [row0, row0+rows) into the
-  // instance-0 buffers at the same rows; 1: target's; 2: critic's after its Adam step)
-  auto care_tables = [&](std::vector<int> insts) {
-    Launch l;
-    l.kind = L_CARE_TAB;
-    CareTabArgs& P = l.ctab;
-    memset(&P, 0, sizeof(P));
-    P.params = h->params; P.rsP = rsP; P.emb_off = L.off_emb;
-    P.trunk = h->care_trunk; P.ctx = h->care_ctx;
-    P.T = c.num_tasks; P.K = Kenc; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
-    P.original = c.care == 2 ? 1 : 0;
-    for (size_t i = 0; i < insts.size(); ++i) {
-      P.inst_delta[i] = insts[i] == 1 ? L.target_delta : 0;
-      P.tab[i] = h->careTab[insts[i]].p;
-    }
-    P.rsTab = h->careTab[0].rs;
-    l.grid = dim3(c.num_tasks, (unsigned)insts.size(), R);
-    l.block = dim3(512);
-    h->plan.push_back(l);
-  };
-  auto care_mixture_fwd = [&](std::vector<std::tuple<int, int, int>> jobs /* (inst, xs_row0, rows) */) {
-    for (int l = 0; l < nmix; ++l) {
-      std::vector<GemmProb> ps;
-      for (auto& jb : jobs) {
-        const int inst = std::get<0>(jb), row0 = std::get<1>(jb), rows = std::get<2>(jb);
-        const int rows_buf = inst == 0 ? 2 * B : B;             // rows held by the instance's buffers
-        const int out_row0 = inst == 0 ? row0 : 0;
-        const LayerOff& lo = L.mix[l];
-        const long long delta = inst == 1 ? L.target_delta : 0;
-        const bool last = (l == nmix - 1);
-        const Buf& ob = last ? h->mixZ[inst] : h->mixH[inst][l];
-        for (int k = 0; k < Kenc; ++k) {
-          GemmProb p;
-          memset(&p, 0, sizeof(p));
-          if (l == 0) { p.A = h->XS.p + (long long)row0 * h->K.obs; p.rsA = h->XS.rs; p.lda = h->K.obs; }
-          else {
-            const Buf& ib = h->mixH[inst][l - 1];
-            p.A = ib.p + ((long long)k * rows_buf + out_row0) * pitch(lo.in); p.rsA = ib.rs; p.lda = pitch(lo.in);
-          }
-          p.B = W(delta + lo.w + (long long)k * lo.out * lo.in); p.rsB = rsP; p.ldb = lo.in;
-          p.bias = W(delta + lo.b + (long long)k * lo.out); p.rsBias = rsP;
-          p.C = ob.p + ((long long)k * rows_buf + out_row0) * pitch(lo.out); p.rsC = ob.rs; p.ldc = pitch(lo.out);
-          p.M = rows; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = last ? 0 : 1;
-          ps.push_back(p);
-        }
-      }
-      gemm_launch(ps);
-    }
-  };
-  auto care_mix = [&](int inst, int rows, float* d1, long long rs1, int ld1, float* d2, long long rs2, int ld2, int off2) {
-    Launch l;
-    l.kind = L_CARE_MIX;
-    CareMixArgs& P = l.cmix;
-    memset(&P, 0, sizeof(P));
-    const int rows_buf = inst == 0 ? 2 * B : B;
-    P.Z = h->mixZ[inst].p; P.rsZ = h->mixZ[inst].rs; P.kstride = (long long)rows_buf * pitch(c.mix_out); P.ldz = pitch(c.mix_out);
-    P.tab = h->careTab[inst].p; P.rsTab = h->careTab[inst].rs; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
-    P.off_ctx = h->care_off_ctx;
-    P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
-    P.rows = rows; P.B = B; P.K = Kenc; P.mo = c.mix_out; P.co = c.ctx_out;
-    P.dst1 = d1; P.rsD1 = rs1; P.ld1 = ld1; P.dst2 = d2; P.rsD2 = rs2; P.ld2 = ld2; P.row_off2 = off2;
-    l.grid = dim3((rows + 7) / 8, R);
-    l.block = dim3(256);
-    h->plan.push_back(l);
-  };
-  // mixture layers + attention mix of up to three encoder instances in ONE launch (care_mixfwd_kernel: all mixture weights of
-  // an instance resident in shared memory); falls back to the grouped-GEMM path when the weights do not fit
-  struct EncJob { int inst, xs_row0, rows; float* d1; long long rs1; int ld1; float* d2; long long rs2; int ld2; int off2; };
-  auto care_encode = [&](std::vector<EncJob> jobs) {
-    CareMixFwdArgs A;
-    memset(&A, 0, sizeof(A));
-    A.njobs = (int)jobs.size(); A.nl = nmix; A.K = Kenc; A.B = B;
-    if (const char* e = getenv("B200SAC_CMF_SKIP")) A.dbg_skip = atoi(e);
-    A.params = h->params; A.rsP = rsP;
-    A.XS = h->XS.p; A.rsXS = h->XS.rs; A.ldx = h->K.obs;
-    A.tid = (const int*)h->tid.p; A.rsR = h->r.rs;
-    A.row_w = h->care_row_w; A.off_att = h->care_off_att; A.off_ctx = h->care_off_ctx; A.mo = c.mix_out; A.co = c.ctx_out;
-    bool ok = nmix >= 1 && nmix <= CMF_MAXL && (int)jobs.size() <= CMF_MAXJOBS && getenv("B200SAC_NO_CARE_FUSED") == nullptr;
-    for (int l = 0; ok && l < nmix; ++l) {
-      A.w_off[l] = L.mix[l].w; A.b_off[l] = L.mix[l].b; A.in[l] = L.mix[l].in; A.out[l] = L.mix[l].out;
-      A.maxw = std::max(A.maxw, L.mix[l].out);
-    }
-    int cta = 0;
-    for (size_t i = 0; ok && i < jobs.size(); ++i) {
-      const EncJob& e = jobs[i];
-      CareMixFwdJob& J = A.job[i];
-      const int rows_buf = e.inst == 0 ? 2 * B : B;
-      J.inst_delta = e.inst == 1 ? L.target_delta : 0;
-      J.rows = e.rows; J.xs_row0 = e.xs_row0; J.out_row0 = e.inst == 0 ? e.xs_row0 : 0; J.rows_buf = rows_buf;
-      J.cta0 = cta; cta += (e.rows + CMF_ROWS - 1) / CMF_ROWS;
-      J.tab = h->careTab[e.inst].p; J.rsTab = h->careTab[e.inst].rs;
-      for (int l = 0; l < nmix; ++l) {
-        const Buf& ob = (l == nmix - 1) ? h->mixZ[e.inst] : h->mixH[e.inst][l];
-        J.H[l] = ob.p; J.rsH[l] = ob.rs;
-      }
-      J.dst1 = e.d1; J.rsD1 = e.rs1; J.ld1 = e.ld1; J.dst2 = e.d2; J.rsD2 = e.rs2; J.ld2 = e.ld2; J.row_off2 = e.off2;
-    }
-    const size_t smem = ok ? care_mixfwd_smem_floats(A) * sizeof(float) : 0;
-    if (ok && smem <= 225 * 1024 &&
-        cudaFuncSetAttribute(care_mixfwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) == cudaSuccess) {
-      Launch l;
-      l.kind = L_CARE_MIXFWD;
-      l.cmf = A;
-      l.grid = dim3(cta, R);
-      l.block = dim3(CMF_THREADS);
-      l.smem = smem;
-      h->plan.push_back(l);
-      return;
-    }
-    std::vector<std::tuple<int, int, int>> mj;
-    for (auto& e : jobs) mj.push_back(std::make_tuple(e.inst, e.xs_row0, e.rows));
-    care_mixture_fwd(mj);
-    for (auto& e : jobs) care_mix(e.inst, e.rows, e.d1, e.rs1, e.ld1, e.d2, e.rs2, e.ld2, e.off2);
-  };
   if (c.care) {
     // encoded states of [s'; s] with the critic's (== actor's, tied) encoder and of s' with the target's
     care_tables({0, 1});
-    care_encode({EncJob{0, 0, 2 * B, h->XA.p, h->XA.rs, h->K.ldxa, h->XQ.p, h->XQ.rs, h->K.ldx, B},
-                 EncJob{1, 0, B, h->XT.p, h->XT.rs, h->K.ldx, nullptr, 0, 0, 0}});
+    care_encode({EncJob{0, 0, 2 * B, h->XA, h->K.ldxa, h->XQ, h->K.ldx, B}, EncJob{1, 0, B, h->XT, h->K.ldx, Buf{}, 0, 0}});
   }
-
-  auto fwd = [&](const float* Ain, long long rsA, int M, const LayerOff& lo, bool target_or_local_params, float* out,
-                 long long rsOut) {
-    (void)target_or_local_params;
-    GemmProb p;
-    memset(&p, 0, sizeof(p));
-    p.A = Ain; p.rsA = rsA; p.lda = lo.ld;
-    p.B = W(lo.w); p.rsB = rsP; p.ldb = lo.ld;
-    p.bias = W(lo.b); p.rsBias = rsP;
-    p.C = out; p.rsC = rsOut; p.ldc = lo.out;
-    p.M = M; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = 1;
-    return p;
-  };
-  auto wgrad = [&](const float* dZ, long long rsdZ, const float* X, long long rsX, const LayerOff& lo) {
-    GemmProb p;
-    memset(&p, 0, sizeof(p));
-    p.A = dZ; p.rsA = rsdZ; p.lda = lo.out;
-    p.B = X; p.rsB = rsX; p.ldb = lo.ld;
-    p.C = Gp(lo.w); p.rsC = rsG; p.ldc = lo.ld;
-    p.C2 = Gp(lo.b); p.rsC2 = rsG;
-    p.M = lo.out; p.N = lo.in; p.K = B; p.mode = GEMM_WGRAD;
-    return p;
-  };
-  auto dgrad = [&](const float* dZ, long long rsdZ, const LayerOff& lo, const float* mask, long long rsMask, float* out,
-                   long long rsOut) {
-    GemmProb p;
-    memset(&p, 0, sizeof(p));
-    p.A = dZ; p.rsA = rsdZ; p.lda = lo.out;
-    p.B = W(lo.w); p.rsB = rsP; p.ldb = lo.ld;
-    p.mask = mask; p.rsMask = rsMask; p.ldmask = lo.ld;
-    p.C = out; p.rsC = rsOut; p.ldc = lo.ld;
-    p.M = B; p.N = lo.in; p.K = lo.out; p.mode = GEMM_DGRAD;
-    return p;
-  };
   auto netp = [&](const Buf& b, int net, int H) { return b.p + (long long)net * B * H; };
-
-  {  // policy head arguments (the generic plan's policy_head launch, the chained forward kernel and b200sac_act share them)
-    PolicyHeadArgs& P = h->pol;
-    memset(&P, 0, sizeof(P));
-    const LayerOff& lo = L.actor[La];
-    P.h = h->hA[La - 1].p; P.rsH = h->hA[La - 1].rs; P.ldh = lo.in;
-    P.W = W(lo.w); P.b = W(lo.b); P.rsP = rsP;
-    P.eps = h->eps.p; P.rsEps = h->eps.rs; P.use_eps_buf = 0;
-    P.pout = h->pout.p; P.rsPout = h->pout.rs;
-    P.psave = h->psave.p; P.rsSave = h->psave.rs;
-    P.XT = h->XT.p; P.XP = h->XP.p; P.rsX = h->XT.rs;
-    P.act_out = h->act_out.p; P.rsAct = h->act_out.rs;
-    P.logp = h->logp.p; P.rsLogp = h->logp.rs;
-    P.logstd_sum = h->logstd.p;
-    P.cnt = h->cnt;
-  }
-  // parameter update + the tail job (last CTA); tail_only: the tail job alone, on the fork stream, plus the critic-loss
-  // reduction (the layer-chained plan, whose parameter updates are fused into the weight-gradient launches)
-  auto adam = [&](int which, bool tail_only) {
-    Launch l;
-    l.kind = L_ADAM;
-    AdamArgs& P = l.ad;
-    memset(&P, 0, sizeof(P));
-    const int64_t beg = which == 0 ? L.critic_begin : (which == 1 ? L.actor_begin : L.cenc_begin);
-    const int64_t n = which == 0 ? L.critic_n : (which == 1 ? L.actor_n : L.cenc_n);
-    P.p = h->params + beg; P.m = h->adam_m + beg; P.v = h->adam_v + beg; P.g = h->grads + beg;
-    P.rsP = rsP; P.rsM = rsG; P.n = n;
-    P.gx = h->grads_x ? h->grads_x + beg : nullptr; P.xs = (long long)R * L.trainable; P.nx = h->gslices - 1;
-    P.target_delta = which == 0 ? L.target_delta : 0;
-    P.tau2_begin = (which == 0 && c.care) ? (L.cse_begin - L.critic_begin) : (long long)1 << 60;
-    P.which = which == 2 ? 4 : which;                    // counter slot: 0 critic, 1 actor, 4 context encoder
-    P.cnt = h->cnt;
-    P.tail = which == 0 ? TAIL_CRITIC_LOSS : (which == 1 ? TAIL_ALPHA_AND_LOSSES : TAIL_NONE);
-    if (tail_only) P.tail = TAIL_ALL;
-    P.lq = h->lq.p; P.la = h->la.p; P.rsY = h->y.rs;
-    P.logp_cur = h->logp.p + B; P.logstd_sum = h->logstd.p + B; P.rsLogp = h->logp.rs;
-    P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
-    P.log_alpha = h->params + L.off_alpha;
-    P.m_alpha = h->adam_m + L.off_alpha; P.v_alpha = h->adam_v + L.off_alpha; P.g_alpha = h->grads + L.off_alpha;
-    P.losses = h->losses; P.losses_host = h->loss_h_dev; P.R = R;
-    int nb = (int)((n + 256 * 4 - 1) / (256 * 4));
-    if (nb < 1) nb = 1;
-    if (nb > 592) nb = 592;
-    l.grid = dim3(nb + (P.tail != TAIL_NONE ? 1 : 0), R);
-    l.block = dim3(256);
-    l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
-    if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
-    h->plan.push_back(l);
-  };
-  if (h->fused) {
-    if (int rc = build_plan_fused(h, adam)) return rc;
-  } else {
   // ---- Phase A: actor over [s2; s] and Q1,Q2 over (s,a), layer by layer -----------------
   for (int l = 0; l < (La > Lc ? La : Lc); ++l) {
     std::vector<GemmProb> ps;
     if (l < La) {
       const LayerOff& lo = L.actor[l];
-      ps.push_back(fwd(l == 0 ? h->XA.p : h->hA[l - 1].p, l == 0 ? h->XA.rs : h->hA[l - 1].rs, 2 * B, lo, true,
+      ps.push_back(fwd_prob(par, l == 0 ? h->XA.p : h->hA[l - 1].p, l == 0 ? h->XA.rs : h->hA[l - 1].rs, 2 * B, lo,
                        h->hA[l].p, h->hA[l].rs));
     }
     if (l < Lc)
       for (int net = 0; net < 2; ++net) {
         const LayerOff& lo = L.q[net][l];
-        ps.push_back(fwd(l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in), l == 0 ? h->XQ.rs : h->hQ[l - 1].rs, B, lo,
-                         true, netp(h->hQ[l], net, lo.out), h->hQ[l].rs));
+        ps.push_back(fwd_prob(par, l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in), l == 0 ? h->XQ.rs : h->hQ[l - 1].rs, B, lo,
+                         netp(h->hQ[l], net, lo.out), h->hQ[l].rs));
       }
     if (use_fork && La == Lc) {
       // Q1,Q2 on (s,a) are not needed before critic_heads, while the actor's output heads the policy_head -> target-critic
       // chain: the critics' layer goes to the fork stream (joined at critic_heads), the actor's stays on the main stream.
-      cur_branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end())); cur_branch = 0;
+      branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end())); branch = 0;
       gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 1));
     } else {
       gemm_launch(ps);
@@ -1281,12 +1367,12 @@ static int build_plan(b200sac* h) {
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.qt[net][l];
-      ps.push_back(fwd(l == 0 ? h->XT.p : netp(h->hT[l - 1], net, lo.in), l == 0 ? h->XT.rs : h->hT[l - 1].rs, B, lo,
-                       true, netp(h->hT[l], net, lo.out), h->hT[l].rs));
+      ps.push_back(fwd_prob(par, l == 0 ? h->XT.p : netp(h->hT[l - 1], net, lo.in), l == 0 ? h->XT.rs : h->hT[l - 1].rs, B, lo,
+                       netp(h->hT[l], net, lo.out), h->hT[l].rs));
     }
     gemm_launch(ps);
   }
-  const int Hc = c.critic_hidden[Lc - 1], Ha = c.actor_hidden[La - 1];
+  const int Hc = c.critic_hidden[Lc - 1];
   {  // critic heads: y, Q1, Q2, dQ
     Launch l;
     l.kind = L_CHEADS;
@@ -1307,72 +1393,6 @@ static int build_plan(b200sac* h) {
     P.y = h->y.p; P.q = h->q.p; P.dq = h->dq.p; P.lq = h->lq.p; P.rsY = h->y.rs;
     h->plan.push_back(l);
   }
-  auto head_bwd = [&](bool policy, bool want_wgrad) {
-    Launch l;
-    l.kind = L_HEADBWD;
-    HeadBwdArgs& P = l.hb;
-    memset(&P, 0, sizeof(P));
-    P.M = B;
-    P.rsP = rsP; P.rsG = rsG;
-    if (!policy) {
-      P.NO = 1; P.Kdim = Hc; P.nets = 2;
-      for (int net = 0; net < 2; ++net) {
-        P.W[net] = W(L.q[net][Lc].w);
-        P.dW[net] = want_wgrad ? Gp(L.q[net][Lc].w) : nullptr;
-        P.db[net] = want_wgrad ? Gp(L.q[net][Lc].b) : nullptr;
-      }
-      const Buf& hb = want_wgrad ? h->hQ[Lc - 1] : h->hP[Lc - 1];
-      const Buf& dq = want_wgrad ? h->dq : h->dqa;
-      P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = 2 * h->y.rs;
-      P.h = hb.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hb.rs; P.ldh = Hc;
-      P.dh = h->dhQ[Lc - 1].p; P.rsDhNet = (long long)B * Hc; P.rsDhRep = h->dhQ[Lc - 1].rs; P.lddh = Hc;
-    } else {
-      const bool split = (long long)B * A > 2048;      // large batch: one tiny kernel computes d(mu|log_std) for all rows
-      if (split) {
-        Launch pl;
-        pl.kind = L_POLICY_DOUT;
-        PolicyDoutArgs& Q = pl.pdo;
-        memset(&Q, 0, sizeof(Q));
-        Q.dx = h->dxP.p; Q.rsDxNet = (long long)B * h->K.ldx; Q.rsDxRep = h->dxP.rs; Q.lddx = h->K.ldx;
-        Q.psave = h->psave.p + (long long)B * A * kSaveW; Q.rsSave = h->psave.rs;
-        Q.tid = (const int*)h->tid.p; Q.rsR = h->r.rs;
-        Q.log_alpha = W(L.off_alpha); Q.rsP = rsP;
-        Q.dout = h->dout_dbg.p; Q.dact = h->dact_dbg.p; Q.rsDout = h->dout_dbg.rs;
-        Q.M = B;
-        pl.grid = dim3((B * A + 255) / 256, R);
-        pl.block = dim3(256);
-        h->plan.push_back(pl);
-      }
-      P.NO = 2 * A; P.Kdim = Ha; P.nets = 1; P.policy_mode = split ? 0 : 1;
-      if (split) { P.dout = h->dout_dbg.p; P.rsDoutNet = 0; P.rsDoutRep = h->dout_dbg.rs; }
-      const LayerOff& lo = L.actor[La];
-      P.W[0] = W(lo.w); P.dW[0] = Gp(lo.w); P.db[0] = Gp(lo.b);
-      P.h = h->hA[La - 1].p + (long long)B * Ha; P.rsHrep = h->hA[La - 1].rs; P.ldh = Ha;   // rows B..2B-1 (= s half)
-      P.dh = h->dhA[La - 1].p; P.rsDhRep = h->dhA[La - 1].rs; P.lddh = Ha;
-      P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
-      P.psave = h->psave.p + (long long)B * A * kSaveW; P.rsSave = h->psave.rs;
-      P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
-      P.log_alpha = W(L.off_alpha);
-      P.dout_dbg = h->dout_dbg.p; P.dact_dbg = h->dact_dbg.p; P.rsDbg = h->dout_dbg.rs;
-    }
-    // large batches: rows cut into slices (4x the CTAs, a quarter of the serial row loop each); slice s >= 1 leaves its
-    // partial head-weight gradient in gradient slice s, exactly like the split-K GEMM weight gradients
-    P.row_slices = h->gslices;
-    P.xs = (long long)R * L.trainable;
-    for (int net = 0; net < P.nets; ++net)
-      if (P.dW[net] && h->grads_x) { P.dWx[net] = h->grads_x + (P.dW[net] - h->grads); P.dbx[net] = h->grads_x + (P.db[net] - h->grads); }
-    const int rows_per = (B + P.row_slices - 1) / P.row_slices;
-    // 128-bit column mapping when every row pitch / tensor offset involved is a multiple of 4 floats (l.bn = 4 marks it)
-    // -- for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
-    // few to fill the GPU
-    const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0 && getenv("B200SAC_HEADBWD_NARROW") == nullptr;
-    l.bn = wide ? 4 : 1;
-    const int cols = wide ? kHb4Cols : kHbCols;
-    l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
-    l.block = dim3(256);
-    l.smem = ((((size_t)rows_per * P.NO + 3) & ~(size_t)3) + (wide ? 1024 : 256) * (size_t)P.NO) * sizeof(float);   // head_bwd4: red 16-B aligned
-    h->plan.push_back(l);
-  };
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
   for (int l = Lc - 1; l >= 0; --l) {
@@ -1381,22 +1401,22 @@ static int build_plan(b200sac* h) {
       const LayerOff& lo = L.q[net][l];
       const float* X = l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in);
       const long long rsX = l == 0 ? h->XQ.rs : h->hQ[l - 1].rs;
-      ps.push_back(wgrad(netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, X, rsX, lo));
+      ps.push_back(wgrad_prob(grd, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, X, rsX, lo, B));
     }
     if (l > 0)
       for (int net = 0; net < 2; ++net) {
         const LayerOff& lo = L.q[net][l];
-        ps.push_back(dgrad(netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hQ[l - 1], net, lo.in), h->hQ[l - 1].rs,
-                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs));
+        ps.push_back(dgrad_prob(par, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hQ[l - 1], net, lo.in), h->hQ[l - 1].rs,
+                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs, B));
       }
     else if (c.care)     // the critic loss also trains the critic's state encoder: need d(loss)/d(encoded state)
       for (int net = 0; net < 2; ++net) {
         const LayerOff& lo = L.q[net][0];
-        ps.push_back(dgrad(netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
-                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs));
+        ps.push_back(dgrad_prob(par, netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
+                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs, B));
       }
     if (use_fork && l > 0) {        // ps = {wgrad q1, wgrad q2, dgrad q1, dgrad q2}
-      cur_branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 2)); cur_branch = 0;
+      branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 2)); branch = 0;
       gemm_launch(std::vector<GemmProb>(ps.begin() + 2, ps.end()));
     } else {
       gemm_launch(ps);
@@ -1480,7 +1500,7 @@ static int build_plan(b200sac* h) {
       int fl = 0;                                   // backward-chain floats of one task
       for (int j = 0; j < Q.trunk.n; ++j) fl += Q.trunk.dims[j + 1];
       for (int j = 0; j < Q.ctx.n; ++j) fl += Q.ctx.dims[j + 1];
-      if (fl > kCareTabWgradSmemFloats) plan_rc = fail(B200SAC_ERR_INVALID, "internal: one task's CARE backward chains exceed %d floats", kCareTabWgradSmemFloats);
+      if (fl > kCareTabWgradSmemFloats) rc = fail(B200SAC_ERR_INVALID, "internal: one task's CARE backward chains exceed %d floats", kCareTabWgradSmemFloats);
       Q.tchunk = std::max(1, std::min(c.num_tasks, kCareTabWgradSmemFloats / fl));
       l2.smem = (size_t)Q.tchunk * fl * sizeof(float);
       l2.grid = dim3(sms, R);
@@ -1491,14 +1511,14 @@ static int build_plan(b200sac* h) {
   adam(0, false);
   if (c.care) {          // encoded states of s with the UPDATED critic encoder for the actor pass (learner.py:336-341)
     care_tables({2});
-    care_encode({EncJob{2, B, B, h->XP.p, h->XP.rs, h->K.ldx, nullptr, 0, 0, 0}});
+    care_encode({EncJob{2, B, B, h->XP, h->K.ldx, Buf{}, 0, 0}});
   }
   // ---- Phase D: actor pass through the updated critics ---------------------------------------
   for (int l = 0; l < Lc; ++l) {
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.q[net][l];
-      ps.push_back(fwd(l == 0 ? h->XP.p : netp(h->hP[l - 1], net, lo.in), l == 0 ? h->XP.rs : h->hP[l - 1].rs, B, lo, true,
+      ps.push_back(fwd_prob(par, l == 0 ? h->XP.p : netp(h->hP[l - 1], net, lo.in), l == 0 ? h->XP.rs : h->hP[l - 1].rs, B, lo,
                        netp(h->hP[l], net, lo.out), h->hP[l].rs));
     }
     gemm_launch(ps);
@@ -1525,11 +1545,11 @@ static int build_plan(b200sac* h) {
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.q[net][l];
       if (l > 0)
-        ps.push_back(dgrad(netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hP[l - 1], net, lo.in), h->hP[l - 1].rs,
-                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs));
+        ps.push_back(dgrad_prob(par, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hP[l - 1], net, lo.in), h->hP[l - 1].rs,
+                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs, B));
       else
-        ps.push_back(dgrad(netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
-                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs));
+        ps.push_back(dgrad_prob(par, netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
+                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs, B));
     }
     gemm_launch(ps);
   }
@@ -1540,12 +1560,12 @@ static int build_plan(b200sac* h) {
     const LayerOff& lo = L.actor[l];
     const float* X = l == 0 ? h->XA.p + (long long)B * lo.ld : h->hA[l - 1].p + (long long)B * lo.ld;
     const long long rsX = l == 0 ? h->XA.rs : h->hA[l - 1].rs;
-    ps.push_back(wgrad(h->dhA[l].p, h->dhA[l].rs, X, rsX, lo));
+    ps.push_back(wgrad_prob(grd, h->dhA[l].p, h->dhA[l].rs, X, rsX, lo, B));
     if (l > 0)
-      ps.push_back(dgrad(h->dhA[l].p, h->dhA[l].rs, lo, h->hA[l - 1].p + (long long)B * lo.ld, h->hA[l - 1].rs,
-                         h->dhA[l - 1].p, h->dhA[l - 1].rs));
+      ps.push_back(dgrad_prob(par, h->dhA[l].p, h->dhA[l].rs, lo, h->hA[l - 1].p + (long long)B * lo.ld, h->hA[l - 1].rs,
+                         h->dhA[l - 1].p, h->dhA[l - 1].rs, B));
     if (use_fork && l > 0) {
-      cur_branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 1)); cur_branch = 0;
+      branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 1)); branch = 0;
       gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end()));
     } else {
       gemm_launch(ps);
@@ -1553,9 +1573,33 @@ static int build_plan(b200sac* h) {
   }
   adam(1, false);
   if (c.care == 2) adam(2, false);        // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
-  }   // generic (per-layer) plan
+}
 
-  if (plan_rc) return plan_rc;
+// Build the launch list of one gradient step (everything after the ingest kernel).
+static int build_plan(b200sac* h) {
+  PlanBuilder pb(h);
+  {  // policy head arguments (the per-layer plan's policy_head launch, the chained forward kernel and b200sac_act share them)
+    PolicyHeadArgs& P = h->pol;
+    memset(&P, 0, sizeof(P));
+    const int La = pb.La;
+    const LayerOff& lo = h->L.actor[La];
+    P.h = h->hA[La - 1].p; P.rsH = h->hA[La - 1].rs; P.ldh = lo.in;
+    P.W = pb.W(lo.w); P.b = pb.W(lo.b); P.rsP = pb.rsP;
+    P.eps = h->eps.p; P.rsEps = h->eps.rs; P.use_eps_buf = 0;
+    P.pout = h->pout.p; P.rsPout = h->pout.rs;
+    P.psave = h->psave.p; P.rsSave = h->psave.rs;
+    P.XT = h->XT.p; P.XP = h->XP.p; P.rsX = h->XT.rs;
+    P.act_out = h->act_out.p; P.rsAct = h->act_out.rs;
+    P.logp = h->logp.p; P.rsLogp = h->logp.rs;
+    P.logstd_sum = h->logstd.p;
+    P.cnt = h->cnt;
+  }
+  if (h->fused) {
+    if (int rc = pb.build_plan_fused()) return rc;
+  } else {
+    pb.build_plan_layered();
+  }
+  if (pb.rc) return pb.rc;
   // upload problem tables and rebase
   if (!h->h_tprobs.empty()) {
     CU(cudaMalloc(&h->d_tprobs, h->h_tprobs.size() * sizeof(TcProb)));
@@ -1567,7 +1611,7 @@ static int build_plan(b200sac* h) {
     CU(cudaMemcpy(h->d_probs, h->h_probs.data(), h->h_probs.size() * sizeof(GemmProb), cudaMemcpyHostToDevice));
   }
   for (auto& l : h->plan) {
-    if (l.kind == L_GEMM_BIG || l.kind == L_GEMM_SMALL || l.kind == L_GEMM_THIN || l.kind == L_GEMM_TC) l.probs = h->d_probs + (size_t)(uintptr_t)l.probs;
+    if (l.kind == L_GEMM_SMALL || l.kind == L_GEMM_THIN || l.kind == L_GEMM_TC) l.probs = h->d_probs + (size_t)(uintptr_t)l.probs;
     if (l.kind == L_GEMM_TC) l.tprobs = h->d_tprobs + (size_t)(uintptr_t)l.tprobs;
   }
   size_t max_smem = 0;
@@ -1581,34 +1625,28 @@ static int build_plan(b200sac* h) {
 
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor
 // drains; every kernel begins with griddepcontrol.wait (common.cuh::kstamp), so data dependencies hold.
+// CLUSTER_Y > 1: thread-block clusters of (1, CLUSTER_Y, 1) -- the CTAs with equal blockIdx.x / z are co-scheduled and can
+// read each other's shared memory.
 static bool g_use_pdl = true;
-template <typename... KArgs, typename... Args>
+template <int CLUSTER_Y = 1, typename... KArgs, typename... Args>
 static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = g_use_pdl ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
-}
-
-// the same with a thread-block cluster of (1, 2, 1): the two CTAs with equal blockIdx.x / z are co-scheduled and can read
-// each other's shared memory
-template <typename... KArgs, typename... Args>
-static cudaError_t launch_pair_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-  cudaLaunchConfig_t cfg;
-  memset(&cfg, 0, sizeof(cfg));
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 2; attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
+  int n = 0;
+  if (CLUSTER_Y > 1) {
+    attr[n].id = cudaLaunchAttributeClusterDimension;
+    attr[n].val.clusterDim.x = 1; attr[n].val.clusterDim.y = CLUSTER_Y; attr[n].val.clusterDim.z = 1;
+    ++n;
+  }
+  if (g_use_pdl) {
+    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[n].val.programmaticStreamSerializationAllowed = 1;
+    ++n;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = g_use_pdl ? 2 : 1;
+  cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
@@ -1666,7 +1704,6 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
       case L_CARE_TABWG:
         launch_k(care_tab_wgrad_kernel, l.grid, l.block, l.smem, s, l.ctwg);
         break;
-      case L_GEMM_BIG:
       case L_GEMM_SMALL:
         launch_k(gemm_simt_kernel, l.grid, l.block, 0, s, l.grp);
         break;
@@ -1710,7 +1747,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         break;
       case L_CHAIN2:
         with_chain_rows(l.bn, [&](auto rows) {
-          return launch_pair_k(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, K);
+          return launch_k<2>(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, K);
         });
         break;
     }
@@ -2351,13 +2388,9 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     const float* rows = (const float*)p[0];
     const float* e = (const float*)p[1];
     use_eps = e != nullptr;
-    if (use_eps) {
-      // eps staged as [R][B][A] next, then [R][B][A] cur: reuse the split ingest just for the noise
-      // (rows carry the transition itself)
-    }
     launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, rows, (long long)B * h->row_stride, h->row_stride,
              (const int*)nullptr, (long long)0);
-    if (use_eps) {
+    if (use_eps) {      // (rows carry the transition itself) eps staged as [R][B][A] next, then [R][B][A] cur
       const size_t n = (size_t)B * h->cfg.act_dim * sizeof(float);
       for (int rep = 0; rep < R; ++rep) {
         CU(cudaMemcpyAsync(h->eps.p + rep * h->eps.rs, e + (size_t)rep * B * h->cfg.act_dim, n, cudaMemcpyDeviceToDevice, st));
@@ -2566,7 +2599,6 @@ extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, c
 static std::string launch_name(const Launch& l, const std::vector<GemmProb>& hp, const GemmProb* dbase) {
   switch (l.kind) {
     case L_GEMM_TC:
-    case L_GEMM_BIG:
     case L_GEMM_SMALL:
     case L_GEMM_THIN: {
       const size_t i0 = (size_t)(l.probs - dbase);
@@ -2690,8 +2722,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   p.A = A; p.B = B; p.bias = bias; p.mask = mask; p.C = C; p.C2 = C2;
   p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = ldb; p.ldc = ldc; p.ldmask = ldmask; p.mode = mode; p.relu = relu;
   if (!tc_eligible(p)) return fail(B200SAC_ERR_INVALID, "problem not eligible for the wgmma path (need 16-B aligned operands, lda/ldb %% 4 == 0, M,N,K >= 32)");
-  int bn = 64;
-  if (const char* e = getenv("B200SAC_TC_BN")) { const int b = atoi(e); bn = b == 128 ? 128 : (b == 160 ? 160 : 64); }
+  const int bn = tc_forced_bn(64);
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   TcProb* d = nullptr;
@@ -2718,8 +2749,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   memset(&p, 0, sizeof(p));
   p.A = A; p.B = B; p.C = C; p.M = M; p.N = N; p.K = K; p.mode = mode;
   p.lda = mode == GEMM_WGRAD ? M : K; p.ldb = mode == GEMM_FWD ? K : N; p.ldc = N;
-  int bn = 64;
-  if (const char* e = getenv("B200SAC_TC_BN")) { const int b = atoi(e); bn = b == 128 ? 128 : (b == 160 ? 160 : 64); }
+  const int bn = tc_forced_bn(64);
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   t.dbg = dbg;
@@ -2811,63 +2841,32 @@ __global__ void act_task_ids_kernel(const float* __restrict__ X, int obs, int T,
   tid[i] = t;
 }
 
+// one replica's problems of equal M and N on gemm_simt_kernel, GS_MAXG per launch
+static void act_gemm(const std::vector<GemmProb>& ps, cudaStream_t st) {
+  for (size_t i0 = 0; i0 < ps.size(); i0 += GS_MAXG) {
+    GemmGroup grp;
+    memset(&grp, 0, sizeof(grp));
+    grp.G = (int)std::min(ps.size() - i0, (size_t)GS_MAXG);
+    for (int q = 0; q < grp.G; ++q) grp.p[q] = ps[i0 + q];
+    const GemmProb& p = grp.p[0];
+    gemm_simt_kernel<<<dim3((p.N + GS_T - 1) / GS_T, (p.M + GS_T - 1) / GS_T, grp.G), GS_THREADS, 0, st>>>(grp);
+  }
+}
+
 // CARE actors (MT10_Distributed_CARE/src/player.py:199-209: z = context_encoder(mtobs); actor.get_action(mtobs, z)):
 // encode the n observation rows sitting in XS[0..n) of `replica` with the critic's state encoder -- the actor's is its
 // hard copy (learner.py:402) -- into XA[0..n): per-task tables, K mixture encoders, attention mix.
 static int care_encode_rows(b200sac* h, cudaStream_t st, int replica, int n) {
-  const b200sac_cfg& c = h->cfg;
-  const Layout& L = h->L;
-  const int B = c.batch, Kenc = c.num_encoders, nmix = (int)L.mix.size();
-  auto pitch = [](int w) { return (w + 3) & ~3; };
-  float* par = h->params + (long long)replica * L.arena;
-  float* XS = h->XS.p + (long long)replica * h->XS.rs;
-  int* tid = (int*)(h->tid.p + (long long)replica * h->tid.rs);
-  act_task_ids_kernel<<<(n + 255) / 256, 256, 0, st>>>(XS, h->K.obs, c.num_tasks, n, tid);
-  {
-    CareTabArgs P;
-    memset(&P, 0, sizeof(P));
-    P.params = par; P.rsP = 0; P.emb_off = L.off_emb;
-    P.trunk = h->care_trunk; P.ctx = h->care_ctx;
-    P.T = c.num_tasks; P.K = Kenc; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
-    P.original = c.care == 2 ? 1 : 0;
-    P.inst_delta[0] = 0;
-    P.tab[0] = h->careTab[0].p + (long long)replica * h->careTab[0].rs; P.rsTab = 0;
-    care_tables_kernel<<<dim3(c.num_tasks, 1, 1), 512, 0, st>>>(P);
+  act_task_ids_kernel<<<(n + 255) / 256, 256, 0, st>>>(rep_view(h->XS, replica).p, h->K.obs, h->cfg.num_tasks, n,
+                                                       (int*)rep_view(h->tid, replica).p);
+  care_tables_kernel<<<dim3(h->cfg.num_tasks, 1, 1), 512, 0, st>>>(care_tab_args(h, replica, {0}));
+  for (int l = 0; l < (int)h->L.mix.size(); ++l) {
+    std::vector<GemmProb> ps;
+    mix_fwd_probs(h, replica, 0, l, 0, n, ps);
+    act_gemm(ps, st);
   }
-  for (int l = 0; l < nmix; ++l) {
-    const LayerOff& lo = L.mix[l];
-    const bool last = (l == nmix - 1);
-    const Buf& ob = last ? h->mixZ[0] : h->mixH[0][l];
-    GemmGroup grp;
-    memset(&grp, 0, sizeof(grp));
-    for (int k0 = 0; k0 < Kenc; k0 += GS_MAXG) {
-      const int cnt = (Kenc - k0 < GS_MAXG) ? Kenc - k0 : GS_MAXG;
-      grp.G = cnt;
-      for (int q = 0; q < cnt; ++q) {
-        const int k = k0 + q;
-        GemmProb& p = grp.p[q];
-        memset(&p, 0, sizeof(p));
-        if (l == 0) { p.A = XS; p.lda = h->K.obs; }
-        else { p.A = h->mixH[0][l - 1].p + (long long)replica * h->mixH[0][l - 1].rs + (long long)k * 2 * B * pitch(lo.in); p.lda = pitch(lo.in); }
-        p.B = par + lo.w + (long long)k * lo.out * lo.in; p.ldb = lo.in;
-        p.bias = par + lo.b + (long long)k * lo.out;
-        p.C = ob.p + (long long)replica * ob.rs + (long long)k * 2 * B * pitch(lo.out); p.ldc = pitch(lo.out);
-        p.M = n; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = last ? 0 : 1;
-      }
-      gemm_simt_kernel<<<dim3((lo.out + GS_T - 1) / GS_T, (n + GS_T - 1) / GS_T, cnt), GS_THREADS, 0, st>>>(grp);
-    }
-  }
-  {
-    CareMixArgs P;
-    memset(&P, 0, sizeof(P));
-    P.Z = h->mixZ[0].p + (long long)replica * h->mixZ[0].rs; P.rsZ = 0; P.kstride = (long long)2 * B * pitch(c.mix_out); P.ldz = pitch(c.mix_out);
-    P.tab = h->careTab[0].p + (long long)replica * h->careTab[0].rs; P.rsTab = 0; P.row_w = h->care_row_w; P.off_att = h->care_off_att;
-    P.off_ctx = h->care_off_ctx;
-    P.tid = tid; P.rsR = 0;
-    P.rows = n; P.B = B; P.K = Kenc; P.mo = c.mix_out; P.co = c.ctx_out;
-    P.dst1 = h->XA.p + (long long)replica * h->XA.rs; P.rsD1 = 0; P.ld1 = h->K.ldxa;
-    care_mix_kernel<<<dim3((n + 7) / 8, 1), 256, 0, st>>>(P);
-  }
+  const EncJob job{0, 0, n, rep_view(h->XA, replica), h->K.ldxa, Buf{}, 0, 0};
+  care_mix_kernel<<<dim3((n + 7) / 8, 1), 256, 0, st>>>(care_mix_args(h, replica, job));
   CU(cudaGetLastError());
   return 0;
 }
@@ -2894,18 +2893,10 @@ extern "C" int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float
     CU(cudaMemcpy2DAsync(XA, (size_t)h->K.ldxa * sizeof(float), obs, (size_t)obs_w * sizeof(float), (size_t)obs_w * sizeof(float),
                          (size_t)n, cudaMemcpyDefault, st));
   }
+  const Buf par = rep_view(Buf{h->params, L.arena}, replica);
   for (int l = 0; l < La; ++l) {
-    const LayerOff& lo = L.actor[l];
-    GemmGroup grp;
-    memset(&grp, 0, sizeof(grp));
-    grp.G = 1;
-    GemmProb& p = grp.p[0];
-    p.A = (l == 0 ? XA : h->hA[l - 1].p + (long long)replica * h->hA[l - 1].rs); p.lda = lo.ld;
-    p.B = h->params + (long long)replica * L.arena + lo.w; p.ldb = lo.ld;
-    p.bias = h->params + (long long)replica * L.arena + lo.b;
-    p.C = h->hA[l].p + (long long)replica * h->hA[l].rs; p.ldc = lo.out;
-    p.M = n; p.N = lo.out; p.K = lo.in; p.mode = GEMM_FWD; p.relu = 1;
-    gemm_simt_kernel<<<dim3((p.N + GS_T - 1) / GS_T, (p.M + GS_T - 1) / GS_T, 1), GS_THREADS, 0, st>>>(grp);
+    const Buf X = rep_view(l == 0 ? h->XA : h->hA[l - 1], replica), out = rep_view(h->hA[l], replica);
+    act_gemm({fwd_prob(par, X.p, X.rs, n, L.actor[l], out.p, out.rs)}, st);
   }
   PolicyHeadArgs P = h->pol;
   P.h += replica * P.rsH; P.W += replica * P.rsP; P.b += replica * P.rsP; P.eps += replica * P.rsEps;

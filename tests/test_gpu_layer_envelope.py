@@ -1,4 +1,4 @@
-"""The per-layer step plan (build_plan in b200sac.cu, plain SAC / MTSAC outside the layer-chained envelope) at both precisions,
+"""The per-layer step plan (build_plan_layered in b200sac.cu, plain SAC / MTSAC outside the layer-chained envelope) at both precisions,
 against the autograd oracle.
 
 The per-layer plan carries every precision = 1 learner, the 400-wide VS / MS shapes, the many-learner configurations and
@@ -74,7 +74,7 @@ H100_SMS = 132
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# mirror of the per-layer plan builder (build_plan / gemm_launch / head_bwd in b200sac.cu)
+# mirror of the per-layer plan builder (build_plan_layered / gemm_launch / head_bwd in b200sac.cu)
 # ---------------------------------------------------------------------------------------------------------------------
 FWD, DGRAD, WGRAD = "fwd", "dgrad", "wgrad"
 SPLIT_K, SPLIT_K_MIN = 4, 512          # kSplitK, kSplitKMin
