@@ -91,6 +91,7 @@ SYMBOLS = {
     "b200sac_replay_set_beta": (C.c_int, [_VP, C.c_int32, C.c_double, _VP]),
     "b200sac_replay_set_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP]),
     "b200sac_replay_get_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP]),
+    "b200sac_replay_get_tree": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int64, _VP]),
     "b200sac_replay_sample_prioritized": (C.c_int, [_VP, C.c_int32] + [_VP] * 5 + [_VP, _VP]),
 }
 

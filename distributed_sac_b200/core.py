@@ -449,6 +449,7 @@ class Replay:
         self.core = core
         self.lib = core.lib
         self._h = C.c_void_p(0)
+        self.capacity = int(capacity)
         w = {"device": 0, "host": 1}[where]
         self.prioritized = None if prioritized is None else dict(prioritized)
         if self.prioritized is not None:
@@ -517,6 +518,16 @@ class Replay:
         out = np.empty(idx.size, dtype=np.float32)
         _lib.check(self.lib.b200sac_replay_get_priorities(self._h, int(replica), idx.size, C.c_void_p(idx.ctypes.data),
                                                           C.c_void_p(out.ctypes.data)))
+        return out
+
+    def tree(self, task=0, replica=0) -> np.ndarray:
+        """The whole sum-tree of one (replica, task) sub-ring: [2P] fp32 in heap order (node 1 = root, leaf i = node P + i)."""
+        cap_t = self.capacity // max(self.core.cfg.num_tasks, 1)
+        P = 1
+        while P < cap_t:
+            P *= 2
+        out = np.empty(2 * P, dtype=np.float32)
+        _lib.check(self.lib.b200sac_replay_get_tree(self._h, int(replica), int(task), out.size, C.c_void_p(out.ctypes.data)))
         return out
 
     def sample_prioritized(self, replica=0):

@@ -3291,6 +3291,13 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
   if (!(alpha >= 0.0) || !std::isfinite(alpha)) return fail(B200SAC_ERR_INVALID, "prioritized replay: alpha must be finite and >= 0 (got %g)", alpha);
   if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "prioritized replay: beta must be in [0, 1] (got %g)", beta);
   if (!(eps > 0.0) || !std::isfinite(eps)) return fail(B200SAC_ERR_INVALID, "prioritized replay: eps must be finite and > 0 (got %g)", eps);
+  // The smallest leaf a filled slot can hold is (0 + eps)^alpha, rounded to fp32 as per_leaf_value does.  It must be > 0:
+  // then every sub-ring the sampler visits has a root > 0 and the descent, which never enters a zero-sum child, ends on a
+  // filled slot.  (With a zero root it would end on leaf P - 1, past the sub-ring's filled slots or past the sub-ring.)
+  const float min_leaf = (float)std::pow(eps, alpha);
+  if (!(min_leaf > 0.f) || !std::isfinite(min_leaf))
+    return fail(B200SAC_ERR_INVALID, "prioritized replay: the leaf of a zero priority, (0 + eps)^alpha = %g, must be > 0 and finite in fp32 "
+                "(alpha %g, eps %g)", std::pow(eps, alpha), alpha, eps);
   b200sac_replay_t* rb = nullptr;
   if (int rc = b200sac_replay_create(h, capacity, 0, seed, &rb)) return rc;
   rb->per = true;
@@ -3362,6 +3369,8 @@ extern "C" int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t repli
     if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
       return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
     if (!(prio[i] >= 0.f) || !std::isfinite(prio[i])) return fail(B200SAC_ERR_INVALID, "priority %lld is not a finite value >= 0", (long long)i);
+    if (!std::isfinite((float)std::pow((double)prio[i] + rb->tr.eps, rb->tr.alpha)))     // (alpha > 1) an inf leaf: NaN weights
+      return fail(B200SAC_ERR_INVALID, "priority %lld: (%g + eps)^alpha overflows fp32", (long long)i, (double)prio[i]);
     ix[(size_t)i] = (int)k;
   }
   if (int rc = per_quiesce(rb)) return rc;
@@ -3393,6 +3402,19 @@ extern "C" int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t repli
     CU(cudaMemcpyAsync(p_out + i0, rb->s_f, m * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
     CU(cudaStreamSynchronize(rb->st));
   }
+  return 0;
+}
+
+extern "C" int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, float* out) {
+  if (int rc = per_check(rb, replica)) return rc;
+  if (task < 0 || task >= rb->Teff) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
+  if (!out || n != 2 * rb->tr.P) return fail(B200SAC_ERR_INVALID, "a tree is 2P = %lld floats (got n = %lld)", 2 * rb->tr.P, (long long)n);
+  CU(cudaSetDevice(rb->h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  if (int rc = per_quiesce(rb)) return rc;
+  const float* src = rb->tr.tree + ((size_t)replica * rb->tr.T + task) * 2 * rb->tr.P;
+  CU(cudaMemcpyAsync(out, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+  CU(cudaStreamSynchronize(rb->st));
   return 0;
 }
 

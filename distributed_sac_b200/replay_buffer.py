@@ -71,8 +71,10 @@ class ReplayBuffer(threading.Thread):
     # ---- sampling --------------------------------------------------------------------------
     def sample(self):
         """(states, actions, rewards, next_states, dones) fp32 on `device` (replay_buffer.py:63-73).  A prioritized ring
-        draws with ring.sample_prioritized() instead (it also returns the indices and importance weights)."""
-        return tuple(t.to(self.device, non_blocking=False) for t in self.ring.sample())
+        draws with ring.sample_prioritized() instead (which also returns the indices and importance weights: call it
+        directly to get them)."""
+        batch = self.ring.sample() if self.ring.prioritized is None else self.ring.sample_prioritized()[:5]
+        return tuple(t.to(self.device, non_blocking=False) for t in batch)
 
     def enqueue_step(self, core):
         """sample + one gradient step, fused in the library (pinned staging, side-stream H2D); asynchronous."""

@@ -313,7 +313,10 @@ int b200sac_replay_sample(b200sac_replay_t* rb, int32_t replica, float* s, float
  * the step's graph, the sampled leaves get prio_i = (|y - Q1| + |y - Q2|) / 2 (the highest batch slot wins a duplicated
  * index) and a running max p per (replica, task), initially 1, is raised; rows written by push / fill_synthetic get it.
  * b200sac_step_sampled, b200sac_update and b200sac_prepare accept a prioritized ring; b200sac_replay_sample does not.
- * alpha >= 0, 0 <= beta <= 1, eps > 0, else B200SAC_ERR_INVALID. */
+ * alpha >= 0, 0 <= beta <= 1, eps > 0, and (0 + eps)^alpha > 0 and finite in fp32, else B200SAC_ERR_INVALID: a filled
+ * slot's leaf is then always > 0, so every sub-ring the sampler visits has a root > 0 and every draw lands on a filled slot.
+ * With alpha > 1 a large priority can still give an inf leaf: set_priorities refuses one; in the step's own update it can
+ * only come from a TD error near 1e38^(1/alpha), i.e. a critic that has already diverged, and the weights are then NaN. */
 int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity, uint64_t seed, double alpha, double beta, double eps,
                                       b200sac_replay_t** out);
 /* beta of one replica, in stream order on `stream`: steps enqueued afterwards use it (no graph is rebuilt). */
@@ -323,6 +326,9 @@ int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, double beta, 
 int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, const float* prio);
 /* Leaf values p of n ring slots; an index -1 - t reads task t's root sum instead.  Synchronous, like set_priorities. */
 int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, float* p_out);
+/* The whole sum-tree of one (replica, task) sub-ring, n = 2P floats in heap order (out[1] = root, leaf i = out[P + i],
+ * out[0] unused), P = the power of two >= cap_per_task.  Synchronous, like set_priorities. */
+int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, float* out);
 /* Reference-shaped PER sample(): one draw of the device sampler with its own draw counter (0, 1, ... per replica) in place
  * of the step counter; rows, ring indices (nullable) and importance weights (nullable) to HOST arrays. */
 int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,

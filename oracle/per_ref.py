@@ -39,6 +39,38 @@ def root(leaves):
     return build_tree(leaves)[1]
 
 
+U_MAX = 1.0 - 2.0 ** -53          # the largest U(0, 1) the sampler draws (53 random bits)
+
+
+def descend(tree, u):
+    """per_sample_kernel's descent of one draw through a heap-ordered fp32 tree from the fp64 offset u: into the left child
+    while u < its sum, else into the right child with u reduced by the left sum (fp64); a zero-sum child is never entered,
+    so rounding in u cannot reach an empty slot.  When both children are 0 -- a zero root -- it goes right at every level
+    and ends on leaf P - 1.  Returns the leaf index in [0, P)."""
+    P = len(tree) // 2
+    node, u = 1, float(u)
+    while node < P:
+        lv, rv = tree[2 * node], tree[2 * node + 1]
+        if lv > 0 and (u < float(lv) or not rv > 0):
+            node = 2 * node
+        else:
+            u -= float(lv)
+            node = 2 * node + 1
+    return node - P
+
+
+def stratified_draw(tree, per, U):
+    """The leaves drawn by a task's per batch slots: slot j descends from u = (j + U[j]) S / per (S = the root, fp64)."""
+    S = float(tree[1])
+    return np.array([descend(tree, (j + float(U[j])) * S / per) for j in range(per)], dtype=np.int64)
+
+
+def strata(tree, per):
+    """(lo, hi): the lowest and highest leaf slot j of a task can draw, over every U in [0, 1).  The descent is monotone in
+    u, so a draw of slot j lies in [lo[j], hi[j]] whatever its U."""
+    return stratified_draw(tree, per, np.zeros(per)), stratified_draw(tree, per, np.full(per, U_MAX))
+
+
 def is_weights(p, S, N, beta):
     """Batch-max-normalised importance weights of leaf values p drawn from trees with root sums S and fills N."""
     raw = np.power(np.asarray(N, dtype=np.float64) * np.asarray(p, dtype=np.float32).astype(np.float64)

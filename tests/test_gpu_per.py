@@ -159,22 +159,26 @@ def test_priority_update_duplicates_and_root(cuda):
     core.close()
 
 
-@pytest.mark.parametrize("T", [0, 4])
-def test_sampling_distribution(cuda, T):
-    """2000 draws of a 4096-slot ring with skewed priorities, some of them zero: counts fit p_i/S (chi-square), no zero
-    slot is drawn, each task gets B/T rows, and the weights equal (N p / S)^-beta over their batch maximum."""
+@pytest.mark.parametrize("T", [0, 4, 16])
+def test_sampling_distribution_on_partly_filled_rings(cuda, T):
+    """2000 draws of a 4096-slot ring, each sub-ring 15/16 filled, with skewed priorities, some of them zero: counts fit
+    p_i/S (chi-square), no empty slot is drawn, each task gets B/T rows, and the weights equal (N p / S)^-beta over their
+    batch maximum.  (A zero priority's leaf is (0 + eps)^alpha > 0: creation refuses an alpha, eps that round it to 0.)"""
     spec = sp.SacSpec(state_dim=6, act_dim=2, actor_hidden=[32], critic_hidden=[32], batch=256, num_tasks=T)
     core = _core(spec, False, 1)
-    cap, beta = 4096, 0.7
-    rb, _ = _filled_ring(core, spec, False, cap, cap, prioritized=dict(alpha=2.0, beta=beta, eps=1e-30))
-    i = np.arange(cap)
-    prio = ((i * 37) % 101 / 25.0).astype(np.float32)
-    prio[i % 13 == 0] = 0.0                          # (0 + 1e-30)^2 rounds to 0 in fp32: never drawn
-    rb.set_priorities(i, prio)
-    leaves = rb.priorities(i)
-    assert (leaves[prio == 0] == 0).all() and (leaves[prio > 0] > 0).all()
+    cap, beta, eps = 4096, 0.7, 1e-6
     Tn = max(T, 1)
     cap_t = cap // Tn
+    n = Tn * (cap_t * 15 // 16)                      # the last 1/16 of every sub-ring stays empty
+    rb, _ = _filled_ring(core, spec, False, n, cap, prioritized=dict(alpha=2.0, beta=beta, eps=eps))
+    i = np.arange(cap)
+    filled = i % cap_t < n // Tn
+    prio = ((i * 37) % 101 / 25.0).astype(np.float32)
+    prio[i % 13 == 0] = 0.0                          # (0 + eps)^2 = 1e-12: rare, but a filled slot's leaf is > 0
+    rb.set_priorities(i[filled], prio[filled])
+    leaves = rb.priorities(i)
+    assert (leaves[~filled] == 0).all() and (leaves[filled] > 0).all()
+    assert (leaves[filled & (prio == 0)] == per_ref.leaf_values([0.0], 2.0, eps)[0]).all()
     roots = rb.priorities(-1 - np.arange(Tn))
     counts = np.zeros(cap, np.int64)
     per = spec.batch // Tn
@@ -185,9 +189,9 @@ def test_sampling_distribution(cuda, T):
         assert (np.bincount(idx // cap_t, minlength=Tn) == per).all()
         if k < 20:
             t = idx // cap_t
-            want = per_ref.is_weights(leaves[idx], roots[t], cap_t, beta)
+            want = per_ref.is_weights(leaves[idx], roots[t], n // Tn, beta)
             np.testing.assert_allclose(w.numpy(), want, rtol=1e-6)
-    assert counts[leaves == 0].sum() == 0
+    assert counts[~filled].sum() == 0
     for t in range(Tn):
         sl = slice(t * cap_t, (t + 1) * cap_t)
         lt = leaves[sl]
@@ -294,9 +298,12 @@ def test_rejections(cuda):
     core = _core(spec, care, precision)
     with pytest.raises(ValueError, match="device"):
         Replay(core, 4096, where="host", prioritized=PER)
-    for bad in (dict(PER, alpha=-0.1), dict(PER, beta=1.5), dict(PER, beta=-0.1), dict(PER, eps=0.0), dict(PER, eps=-1e-6)):
+    # (the last two: (0 + eps)^alpha rounds to 0 in fp32, so a sub-ring of zero priorities would have a zero root)
+    for bad in (dict(PER, alpha=-0.1), dict(PER, beta=1.5), dict(PER, beta=-0.1), dict(PER, eps=0.0), dict(PER, eps=-1e-6),
+                dict(alpha=2.0, beta=0.5, eps=1e-30), dict(alpha=9.0, beta=0.5, eps=1e-6)):
         with pytest.raises(RuntimeError, match="alpha|beta|eps"):
             Replay(core, 4096, prioritized=bad)
+    Replay(core, 4096, prioritized=dict(alpha=2.0, beta=0.5, eps=1e-20)).close()     # 1e-40: a denormal, still > 0
     rb, _ = _filled_ring(core, spec, care, 1024, 1024)
     with pytest.raises(RuntimeError, match="_prioritized"):
         rb.sample()
@@ -304,5 +311,11 @@ def test_rejections(cuda):
         rb.set_beta(2.0)
     with pytest.raises(RuntimeError, match="empty slot|outside"):
         rb.set_priorities([5000], [1.0])
+    rb.close()
+    rb, _ = _filled_ring(core, spec, care, 1024, 1024, prioritized=dict(alpha=2.0, beta=0.5, eps=1e-6))
+    rb.set_priorities([3], [1e19])                    # 1e38: the largest leaf fp32 holds
+    with pytest.raises(RuntimeError, match="overflows"):
+        rb.set_priorities([3, 4], [1.0, 1e20])        # 1e40 would be an inf leaf (NaN weights); nothing is written
+    assert rb.priorities([3, 4]).tolist() == [per_ref.leaf_values(np.float32([1e19]), 2.0, 1e-6)[0], 1.0]
     rb.close()
     core.close()

@@ -34,6 +34,38 @@ def test_leaf_values_and_weights():
     assert np.array_equal(per_ref.td_priority(y, q1, q2), [0.75, 0.5])
 
 
+def test_descent_model_against_build_tree():
+    """The numpy model of per_sample_kernel's descent: over a padded tree (cap 1000, P 1024, some empty slots) every draw
+    lands on a filled slot of its stratum's prefix-sum interval, u = S (the rounding edge) stays off the empty tail, and
+    with a zero root the descent ends on leaf P - 1 -- past a sub-ring of 1000 slots, i.e. in the next task's rows, which
+    is why creation refuses an alpha, eps whose zero-priority leaf rounds to 0."""
+    rng = np.random.default_rng(1)
+    cap, fill, per = 1000, 950, 64
+    leaves = np.zeros(cap, np.float32)
+    leaves[:fill] = per_ref.leaf_values(rng.exponential(1.0, fill) ** 3, 0.6, 1e-6)
+    tree = per_ref.build_tree(leaves)
+    P = len(tree) // 2
+    assert P == 1024
+    cum = np.concatenate([[0.0], np.cumsum(tree[P:].astype(np.float64))])
+    S = float(tree[1])
+    lo, hi = per_ref.strata(tree, per)
+    assert (np.diff(lo) >= 0).all() and (lo <= hi).all() and (hi[:-1] <= lo[1:]).all()
+    for U in (np.zeros(per), np.full(per, per_ref.U_MAX), rng.random(per)):
+        got = per_ref.stratified_draw(tree, per, U)
+        assert (got < fill).all() and (tree[P + got] > 0).all() and (lo <= got).all() and (got <= hi).all()
+        # the leaf's prefix-sum interval meets its stratum's (to fp32 rounding of the partial sums)
+        j = np.arange(per)
+        tol = 1e-6 * S
+        assert (cum[got] <= (j + 1) * S / per + tol).all() and (cum[got + 1] >= j * S / per - tol).all()
+    assert per_ref.descend(tree, S) == fill - 1 and per_ref.descend(tree, 2 * S) == fill - 1
+    assert per_ref.descend(tree, 0.0) == 0
+    # a zero root (every filled leaf 0): leaf P - 1, beyond the 1000 slots of the sub-ring
+    zero = per_ref.build_tree(np.zeros(cap, np.float32))
+    assert {int(x) for x in per_ref.stratified_draw(zero, per, rng.random(per))} == {P - 1} and P - 1 >= cap
+    # which (alpha, eps) give such leaves: (0 + eps)^alpha rounding to 0 in fp32
+    assert per_ref.leaf_values([0.0], 2.0, 1e-30)[0] == 0 and per_ref.leaf_values([0.0], 2.0, 1e-20)[0] > 0
+
+
 def _problem(weighted_loss):
     spec = sp.SacSpec(state_dim=6, act_dim=3, actor_hidden=[32, 16], critic_hidden=[24, 40], batch=20,
                       num_tasks=4 if weighted_loss else 0, weighted_loss=weighted_loss)
