@@ -62,6 +62,8 @@ SYMBOLS = {
     "b200sac_get_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams)]),
     "b200sac_set_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams), _VP]),
     "b200sac_copy_replica": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
+    "b200sac_set_update_intervals": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "b200sac_get_update_intervals": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_step": (C.c_int, [_VP] + [_VP] * 7 + [_VP]),
     "b200sac_step_host": (C.c_int, [_VP] + [_VP] * 7 + [_VP, _VP]),
     "b200sac_step_sampled": (C.c_int, [_VP, _VP, C.c_int32, _VP]),

@@ -338,9 +338,26 @@ class SacCore:
             hp = _lib.Hparams(**cur)
             _lib.check(self.lib.b200sac_set_hparams(self._h, r, C.byref(hp), _stream()))
 
+    # ---- per-replica update intervals (b200sac_get/set_update_intervals) -------------------------------------
+    def get_update_intervals(self, replica=0):
+        """(actor_every, target_every) of one replica (no synchronisation)."""
+        a, t = C.c_int32(0), C.c_int32(0)
+        _lib.check(self.lib.b200sac_get_update_intervals(self._h, int(replica), C.byref(a), C.byref(t)))
+        return a.value, t.value
+
+    def set_update_intervals(self, actor_every=None, target_every=None, replica=None):
+        """Update the actor (and temperature) only on steps whose critic step count n is a multiple of actor_every, and the
+        targets only when n is a multiple of target_every, for one replica (replica=None: all of them) on the current
+        stream; an interval not named keeps its value.  Steps enqueued afterwards follow the new schedule."""
+        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+            a, t = self.get_update_intervals(r)
+            a = a if actor_every is None else int(actor_every)
+            t = t if target_every is None else int(target_every)
+            _lib.check(self.lib.b200sac_set_update_intervals(self._h, r, a, t, _stream()))
+
     def copy_replica(self, src: int, dst: int):
         """Replica dst's parameters (targets, log_alpha included), Adam moments and step counters become a copy of src's,
-        device to device on the current stream.  Hyperparameters and replay data stay dst's own."""
+        device to device on the current stream.  Hyperparameters, update intervals and replay data stay dst's own."""
         _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
 
     def soft_update(self, tau: float):

@@ -231,6 +231,7 @@ struct Launch {
   int bn = 64;
   bool pair128 = false;  // L_GEMM_TC with bn = 128: the paired tile flavour (fixed when the plan is built)
   int split = 1;         // GEMM launches: K slices of the group's weight gradients
+  const int* sched = nullptr;   // L_GEMM_TC: actor-side launch, replica 0's schedule word (gemm_tc_kernel)
   PolicyDoutArgs pdo;
   CareTabArgs ctab;
   CareMixArgs cmix;
@@ -271,6 +272,8 @@ struct b200sac {
   Counters* cnt = nullptr;
   HParams* hp = nullptr;          // [R] per-replica hyperparameters (K.hp points here)
   std::vector<b200sac_hparams> hp_host;   // host mirror of the values as given (b200sac_get_hparams does not synchronise)
+  int* ivl = nullptr;             // [R][2] update intervals (actor_every, target_every), read by the ingest
+  std::vector<int> ivl_host;      // host mirror (b200sac_get_update_intervals does not synchronise)
   float* losses = nullptr;        // [kLossSlots][R][4]
   long long host_steps = 0;       // steps enqueued so far
   // work slab
@@ -392,7 +395,7 @@ static int destroy_impl(b200sac* h) {
   cudaSetDevice(h->device);
   for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
   cudaFree(h->params); cudaFree(h->adam_m); cudaFree(h->adam_v); cudaFree(h->grads); cudaFree(h->grads_x);
-  cudaFree(h->cnt); cudaFree(h->hp); cudaFree(h->losses); cudaFree(h->slab); cudaFree(h->d_probs); cudaFree(h->d_tprobs);
+  cudaFree(h->cnt); cudaFree(h->hp); cudaFree(h->ivl); cudaFree(h->losses); cudaFree(h->slab); cudaFree(h->d_probs); cudaFree(h->d_tprobs);
   for (int i = 0; i < 2; ++i) {
     if (h->stage_h[i]) cudaFreeHost(h->stage_h[i]);
     cudaFree(h->stage_d[i]);
@@ -480,7 +483,7 @@ static bool tc_eligible(const GemmProb& p) {
 
 // Tile variants of the wgmma GEMM (gemm_tc.cuh): 128x64, 128x128 (B200SAC_TC_PAIR128=1: the paired flavour), 128x160.
 // A step plan reads the switch once, when it is built, and keeps the choice on its launches (Launch::pair128).
-typedef void (*TcKernel)(const TcProb*);
+typedef void (*TcKernel)(const TcProb*, const int*, int, int);
 static bool tc_pair128() { const char* e = getenv("B200SAC_TC_PAIR128"); return e && e[0] == '1'; }
 static TcKernel tc_kernel(int bn, bool pair128) {
   if (bn == 160) return gemm_tc_kernel<160, false>;
@@ -727,6 +730,7 @@ struct PlanBuilder {
   const long long rsP, rsG;
   const Buf par, grd;       // parameter and gradient arenas
   int branch = 0;           // branch tag given to the launches gemm_launch creates
+  bool actor_side = false;  // the launches being built belong to the actor update: skipped on critic-only steps
   int rc = 0;               // error met by a builder that cannot return one; build_plan returns it
 
   explicit PlanBuilder(b200sac* hh)
@@ -825,6 +829,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
       l.branch = branch;
       l.bn = bn;
       l.pair128 = bn == 128 && tc_pair128();
+      l.sched = actor_side ? &h->cnt[0].sched : nullptr;
       l.split = split;
       l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
       l.block = dim3(TC_THREADS);
@@ -870,6 +875,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
     l.G = (int)g.size();
     memset(&l.grp, 0, sizeof(l.grp));
     l.grp.G = l.G;
+    l.grp.sched = actor_side ? &h->cnt[0].sched : nullptr; l.grp.sched_stride = kSchedStride;
     for (size_t i = 0; i < g.size(); ++i) l.grp.p[i] = g[i];
     l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // index for now; rebased later
     for (auto& p : g) h->h_probs.push_back(p);
@@ -881,6 +887,7 @@ void PlanBuilder::care_tables(const std::vector<int>& insts) {
   Launch l;
   l.kind = L_CARE_TAB;
   l.ctab = care_tab_args(h, -1, insts);
+  l.ctab.sched = actor_side ? &h->cnt[0].sched : nullptr; l.ctab.sched_stride = kSchedStride;
   l.grid = dim3(c.num_tasks, (unsigned)insts.size(), R);
   l.block = dim3(512);
   h->plan.push_back(l);
@@ -898,6 +905,7 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
   A.XS = h->XS.p; A.rsXS = h->XS.rs; A.ldx = h->K.obs;
   A.tid = (const int*)h->tid.p; A.rsR = h->r.rs;
   A.row_w = h->care_row_w; A.off_att = h->care_off_att; A.off_ctx = h->care_off_ctx; A.mo = c.mix_out; A.co = c.ctx_out;
+  A.sched = actor_side ? &h->cnt[0].sched : nullptr; A.sched_stride = kSchedStride;
   bool ok = nmix >= 1 && nmix <= CMF_MAXL && (int)jobs.size() <= CMF_MAXJOBS && getenv("B200SAC_NO_CARE_FUSED") == nullptr;
   for (int l = 0; ok && l < nmix; ++l) {
     A.w_off[l] = L.mix[l].w; A.b_off[l] = L.mix[l].b; A.in[l] = L.mix[l].in; A.out[l] = L.mix[l].out;
@@ -939,6 +947,7 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
     Launch l;
     l.kind = L_CARE_MIX;
     l.cmix = care_mix_args(h, -1, e);
+    l.cmix.sched = actor_side ? &h->cnt[0].sched : nullptr; l.cmix.sched_stride = kSchedStride;
     l.grid = dim3((e.rows + 7) / 8, R);
     l.block = dim3(256);
     h->plan.push_back(l);
@@ -951,6 +960,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   l.kind = L_HEADBWD;
   HeadBwdArgs& P = l.hb;
   memset(&P, 0, sizeof(P));
+  P.actor_side = (policy || !want_wgrad) ? 1 : 0;       // the actor pass / the policy backward, not the critic update
   P.M = B;
   P.rsP = rsP; P.rsG = rsG;
   if (!policy) {
@@ -1309,7 +1319,8 @@ int PlanBuilder::build_plan_fused() {
           constexpr int r = decltype(rows)::value;
           CU(cudaFuncSetAttribute(chain_kernel<true, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
           CU(cudaFuncSetAttribute(chain_kernel<false, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-          CU(cudaFuncSetAttribute(chain2_kernel<r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
+          CU(cudaFuncSetAttribute(chain2_kernel<r, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
+          CU(cudaFuncSetAttribute(chain2_kernel<r, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
           return 0;
         }))
       return rc;
@@ -1509,6 +1520,9 @@ void PlanBuilder::build_plan_layered() {
     }
   }
   adam(0, false);
+  // ---- the actor update (D, E): every launch below returns at entry on a critic-only step; adam(1) skips its own body and
+  // its tail writes NaN for the actor-side losses.  adam(2) (CARE(O) context encoder, trained by the critic loss) always runs.
+  actor_side = true;
   if (c.care) {          // encoded states of s with the UPDATED critic encoder for the actor pass (learner.py:336-341)
     care_tables({2});
     care_encode({EncJob{2, B, B, h->XP, h->K.ldx, Buf{}, 0, 0}});
@@ -1571,6 +1585,7 @@ void PlanBuilder::build_plan_layered() {
       gemm_launch(ps);
     }
   }
+  actor_side = false;
   adam(1, false);
   if (c.care == 2) adam(2, false);        // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
 }
@@ -1711,7 +1726,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         launch_k(gemm_thin_kernel, l.grid, l.block, 0, s, l.grp);
         break;
       case L_GEMM_TC:
-        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, l.tprobs);
+        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, l.tprobs, l.sched, l.G, kSchedStride);
         break;
       case L_POLICY: {
         PolicyHeadArgs P = l.pol;
@@ -1747,7 +1762,9 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* 
         break;
       case L_CHAIN2:
         with_chain_rows(l.bn, [&](auto rows) {
-          return launch_k<2>(chain2_kernel<decltype(rows)::value>, l.grid, l.block, l.smem, s, l.chain2, K);
+          constexpr int r = decltype(rows)::value;
+          return launch_k<2>(l.chain2.kind == C2_ACTORQ ? chain2_kernel<r, true> : chain2_kernel<r, false>, l.grid, l.block, l.smem, s,
+                             l.chain2, K);
         });
         break;
     }
@@ -1876,6 +1893,10 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CUH(cudaMalloc(&h->hp, sizeof(HParams) * R));
     CUH(cudaMemcpy(h->hp, rows.data(), sizeof(HParams) * R, cudaMemcpyHostToDevice));
     K.hp = h->hp;
+    h->ivl_host.assign((size_t)2 * R, 1);          // every step updates the actor and the targets
+    CUH(cudaMalloc(&h->ivl, sizeof(int) * 2 * R));
+    CUH(cudaMemcpy(h->ivl, h->ivl_host.data(), sizeof(int) * 2 * R, cudaMemcpyHostToDevice));
+    K.cnt = h->cnt;
   }
 
   // work slab
@@ -1971,7 +1992,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
 
   IngestOut& O = h->ing;
   O.XA = h->XA.p; O.XQ = h->XQ.p; O.XT = h->XT.p; O.XP = h->XP.p; O.r = h->r.p; O.d = h->d.p; O.eps = h->eps.p;
-  O.tid = (int*)h->tid.p; O.cnt = h->cnt;
+  O.tid = (int*)h->tid.p; O.cnt = h->cnt; O.ivl = h->ivl;
   O.rsXA = h->XA.rs; O.rsXQ = h->XQ.rs; O.rsR = h->r.rs; O.rsEps = h->eps.rs;
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
@@ -2183,6 +2204,38 @@ extern "C" int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_
   CU(cudaGetLastError());
   if (int rc = sb.end()) return rc;
   h->hp_host[(size_t)replica] = *hp;
+  return 0;
+}
+
+// Per-replica update intervals: the ingest of each step turns them and the critic's step count into the step's schedule
+// (Counters::sched), so a change is ordered with the steps like set_hparams and reaches already instantiated graphs.
+__global__ void set_intervals_kernel(int* ivl, int replica, int actor_every, int target_every) {
+  ivl[2 * replica] = actor_every;
+  ivl[2 * replica + 1] = target_every;
+}
+
+extern "C" int b200sac_get_update_intervals(b200sac_t* h, int32_t replica, int32_t* actor_every, int32_t* target_every) {
+  if (!h || !actor_every || !target_every) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  *actor_every = h->ivl_host[2 * (size_t)replica];
+  *target_every = h->ivl_host[2 * (size_t)replica + 1];
+  return 0;
+}
+
+extern "C" int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32_t actor_every, int32_t target_every, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  constexpr int32_t kMaxEvery = 1 << 30;
+  if (actor_every < 1 || actor_every > kMaxEvery || target_every < 1 || target_every > kMaxEvery)
+    return fail(B200SAC_ERR_INVALID, "update intervals must be in [1, 2^30] (got actor %d, target %d)", actor_every, target_every);
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  set_intervals_kernel<<<1, 1, 0, sb.run>>>(h->ivl, replica, actor_every, target_every);
+  CU(cudaGetLastError());
+  if (int rc = sb.end()) return rc;
+  h->ivl_host[2 * (size_t)replica] = actor_every;
+  h->ivl_host[2 * (size_t)replica + 1] = target_every;
   return 0;
 }
 
@@ -2730,7 +2783,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d);
+  tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
   cudaFree(d);
@@ -2758,7 +2811,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  for (int it = 0; it < 3; ++it) tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn)>>>(d);
+  for (int it = 0; it < 3; ++it) tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out96, dbg, 96 * 8, cudaMemcpyDeviceToHost));
   cudaFree(A); cudaFree(B); cudaFree(C); cudaFree(dbg); cudaFree(d);

@@ -36,15 +36,18 @@ struct CareTabArgs {
   CareNet trunk, ctx;
   int T, K, row_w, off_att;
   int original;                       // CARE(O): ctx = the shared, trainable context encoder on relu(E[t]); the trunk reads its output
+  int sched_stride; const int* sched; // actor-side launch: replica 0's schedule word (skipped on critic-only steps); null = always runs
 };
 
 // grid (T, n_inst, R), block 512: 16 warps, one output neuron per warp at a time, up to 24 independent
 // loads in flight per lane (the 768-long dot products are pure latency otherwise)
 __global__ void __launch_bounds__(512) care_tables_kernel(CareTabArgs P) {
+  const int sched = P.sched ? sched_word(P.sched + (int)blockIdx.z * P.sched_stride) : SCHED_ACTOR;
   KStamp ks_;
   __shared__ float xe[2048];
   __shared__ float bufA[512], bufB[512];
   const int t = blockIdx.x, inst = blockIdx.y, rep = blockIdx.z;
+  if (!(sched & SCHED_ACTOR)) return;
   const float* __restrict__ par = P.params + rep * P.rsP;
   const float* __restrict__ E = par + P.emb_off + (long long)t * P.ctx.dims[0];
   float* __restrict__ row = P.tab[inst] + rep * P.rsTab + (long long)t * P.row_w;
@@ -151,14 +154,17 @@ struct CareMixArgs {
   int rows, B, K, mo, co;
   float* dst1; long long rsD1; int ld1;                 // every row r -> dst1[r]
   float* dst2; long long rsD2; int ld2; int row_off2;   // rows r >= row_off2 -> dst2[r - row_off2]   (nullable)
+  int sched_stride; const int* sched;                   // as in CareTabArgs
 };
 
 // one warp per row; grid (ceil(rows/8), R), block 256
 __global__ void __launch_bounds__(256) care_mix_kernel(CareMixArgs P) {
+  const int sched = P.sched ? sched_word(P.sched + (int)blockIdx.y * P.sched_stride) : SCHED_ACTOR;
   KStamp ks_;
   const int rep = blockIdx.y, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int r = blockIdx.x * 8 + warp;
   if (r >= P.rows) return;
+  if (!(sched & SCHED_ACTOR)) return;
   const int t = (P.tid + rep * P.rsR)[r % P.B];        // the CURRENT observation's task, also for the s' rows
   const float* __restrict__ trow = P.tab + rep * P.rsTab + (long long)t * P.row_w;
   float den = 0.f;
@@ -409,6 +415,7 @@ struct CareMixFwdArgs {
   int maxw;                                // widest hidden / output layer
   int dbg_skip;                            // measurement only (B200SAC_CMF_SKIP): 1 skip the encoder tasks, 2 the mix, 4 the weight load
   CareMixFwdJob job[CMF_MAXJOBS];
+  int sched_stride; const int* sched;      // as in CareTabArgs
 };
 
 // shared memory (floats): weights + biases of every layer, xs [in0][RP], ha / hb [K][maxw][RP] (ping-pong hidden tiles),
@@ -446,9 +453,12 @@ __global__ void __launch_bounds__(CMF_THREADS, 1) care_mixfwd_kernel(const __gri
   float* xs = cmf_sm + xs_off;
   float* zs = cmf_sm + zs_off;
   float* att = cmf_sm + att_off;
+  // The encoder pass of the actor update on a critic-only step: decided before the weight requests below (the word may be
+  // read before griddepcontrol.wait: sched_word), so that no copy is in flight when the CTA leaves.
+  const bool skip = A.sched && !(sched_word(A.sched + rep * A.sched_stride) & SCHED_ACTOR);
   // ---- weights: do not depend on the launch before this one (the optimizer step that wrote them is further back) ----------
   const float* par = A.params + (long long)rep * A.rsP + J.inst_delta;
-  {
+  if (!skip) {
     int wpos = 0, bpos = wtot;
     for (int l = 0; l < A.nl && !(A.dbg_skip & 4); ++l) {
       const int nW = K * A.out[l] * A.in[l], nb = K * A.out[l];
@@ -470,6 +480,7 @@ __global__ void __launch_bounds__(CMF_THREADS, 1) care_mixfwd_kernel(const __gri
   }
   asm volatile("cp.async.commit_group;" ::: "memory");
   KStamp ks_;                              // XS / the task tables come from the launches before this one
+  if (skip) return;
   // ---- input rows, transposed: xs[i][r] ------------------------------------------------------------------------------
   {
     const float* X = A.XS + (long long)rep * A.rsXS + (long long)(J.xs_row0 + r0) * A.ldx;

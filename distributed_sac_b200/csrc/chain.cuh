@@ -640,6 +640,7 @@ B200_D void wg_stage(float* __restrict__ dst, const float* __restrict__ src, int
 __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_constant__ WgradArgs A, StepConst K) {
   DbgStamp stamp(A.dbg);
   stamp();                                 // 0: entry
+  const WgradAdam& O = A.adam;
   extern __shared__ __align__(128) float wsm_raw[];
   float* sm = wsm_raw + (((128u - (smem_u32(wsm_raw) & 127u)) & 127u) >> 2);      // (pointer arithmetic keeps the shared address space)
   int ji = 0;
@@ -671,10 +672,12 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   __syncthreads();
   // bias corrections of the fused optimizer step (two counter loads, an fp64 division and square root): evaluated now, while
   // the operand tiles are in flight, instead of heading the epilogue
-  const WgradAdam& O = A.adam;
   float step_size = 0.f, bc2_sqrt = 1.f;
   const HParams& H = K.hp[rep];
   adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
+  // the step's schedule (same cache line as the counters just read); consumed once the first operand tiles have landed, so
+  // that a full step never waits for it
+  const int sched = sched_of(O.cnt, rep);
   const float tau = H.tau, one_minus_tau = H.one_minus_tau;
   const float* __restrict__ Ag = J.A + (long long)rep * J.rsA;
   const float* __restrict__ Bg = J.B + (long long)rep * J.rsB;
@@ -699,6 +702,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
     if (!tmB) wg_stage(Bs, Bg, J.ldb, n0, J.Nin, m0, M, tid);
     if (tmA || tmB) mbar_wait(smem_u32(bar), (uint32_t)(pass & 1));
     __syncthreads();
+    if (pass == 0 && O.which == 1 && !(sched & SCHED_ACTOR)) return;   // the actor's gradients + Adam on a critic-only step
     stamp();                               // per pass: operands landed
     const int mcnt = (M - m0 < WG_ROWS) ? M - m0 : WG_ROWS;
     const int per = (mcnt + 7) >> 3;
@@ -784,7 +788,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   // and stay zero).  Every operand of the optimizer step is REQUESTED before the first dependent instruction: the (p, m, v
   // [, target]) quadruples would otherwise be sequential global round trips between stores -- and the code is kept compact on
   // purpose: it runs once per CTA out of a cold instruction cache.
-  const bool has_t = O.target_delta != 0;
+  const bool has_t = O.target_delta != 0 && (sched & SCHED_TARGET);   // targets untouched on a step without a target update
   const int kk = tid >> 3, nn4 = (tid & 7) << 2;
   const bool okq = k0 + kk < J.Kout && n0 + nn4 < J.Nin;
   const long long ci = (long long)(k0 + kk) * J.ldc + n0 + nn4;

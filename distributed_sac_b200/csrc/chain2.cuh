@@ -55,7 +55,9 @@ B200_D float ld_peer_f32(const float* my_smem_addr, uint32_t peer_rank) {
   return v;
 }
 
-template <int ROWS>
+// GATED: the actor pass (C2_ACTORQ), skipped on critic-only steps; its own instantiation, so that the critic update's
+// launch carries no trace of the schedule.
+template <int ROWS, bool GATED>
 __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_constant__ Chain2Args A, StepConst K) {
   const Chain2Job& J = A.job[blockIdx.y];
   extern __shared__ __align__(1024) float sm2_raw[];
@@ -85,10 +87,20 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     for (int e = tid; e < (J.Hhb >> 2); e += CH_THREADS) cp_async16(headB + 4 * e, J.Whb + po + 4 * e);
     if (direct0) d0.load(J.st[0], po, tid);
   };
+  // The actor pass on a critic-only step: both CTAs of a cluster belong to replica `rep` and read the same word, so they
+  // leave together, before any cluster barrier.  The word is requested before griddepcontrol.wait (sched_word) and consumed
+  // after it; a CTA that skips first drains what it requested early (no copy may outlive it).
+  const int sched = GATED ? sched_of(K.cnt, rep) : SCHED_ACTOR;
   if (tid == 0) c.start_pipeline(A.early_weights);
   if (A.early_weights && tid < CH_THREADS) request_weights();
   KStamp ks_;
   c.stamp();
+  if (GATED && !(sched & SCHED_ACTOR)) {
+    if (tid == 0)
+      for (int i = 0; i < c.issued; ++i) mbar_wait(smem_u32(c.bars + i), 0u);
+    asm volatile("cp.async.wait_all;" ::: "memory");
+    return;
+  }
   __syncthreads();                         // barriers initialised (all nine warps)
   if (tid >= CH_THREADS) {
     // ---- producer warp: every remaining weight chunk of the forward AND the backward part, in order.  It takes part in the

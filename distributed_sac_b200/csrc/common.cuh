@@ -10,6 +10,20 @@ namespace bsac {
 
 constexpr int kWarp = 32;
 
+// Schedule of the step in flight, one word per replica (Counters::sched), written by the ingest: SCHED_ACTOR = actor and
+// temperature update, SCHED_TARGET = Polyak update of the targets.  A step without SCHED_ACTOR is a critic-only step.
+enum { SCHED_ACTOR = 1, SCHED_TARGET = 2 };
+
+// A replica's schedule word (null: a launch that always runs).  Every launch that reads it is at least two launches behind
+// the ingest that wrote it on the same stream, or behind a full (event) dependency, so a kernel may read it BEFORE its
+// griddepcontrol.wait, where the L2 round trip hides behind the wait instead of delaying the kernel: a kernel starts only
+// after every CTA of the launch before it has exited, each of those passed its own griddepcontrol.wait, so the launch two
+// back -- and every earlier one, the ingest included -- has completed and its writes are visible.  A kernel that skips its
+// work still passes its own griddepcontrol.wait before it returns, which keeps that argument true for the launches after it.
+// A full step must not wait for the word: kernels consume it where they wait for something else anyway.
+// (__ldcg: an L2 load; nothing this SM cached can stand in for it.)
+B200_D int sched_word(const int* sched) { return sched != nullptr ? __ldcg(sched) : SCHED_ACTOR | SCHED_TARGET; }
+
 // ---------------------------------------------------------------------------------
 // Philox4x32-10 counter-based generator (in-kernel noise + replay index sampling).
 // ---------------------------------------------------------------------------------

@@ -51,6 +51,8 @@ constexpr int GS_INFLIGHT = 4;         // k chunks whose loads are issued before
 struct GemmGroup {
   GemmProb p[GS_MAXG];
   int G;
+  int sched_stride;    // ints between two replicas' schedule words
+  const int* sched;    // actor-side launch: replica 0's schedule word (the launch is skipped on critic-only steps); null = always runs
 };
 
 // Fetch one operand chunk into registers (2 x float4 per thread).
@@ -131,6 +133,7 @@ __device__ int g_gs_prof_n = 0;
 #endif
 
 __global__ void __launch_bounds__(GS_THREADS) gemm_simt_kernel(const __grid_constant__ GemmGroup grp) {
+  const int sched = grp.sched ? sched_word(grp.sched + (int)(blockIdx.z / grp.G) * grp.sched_stride) : SCHED_ACTOR;
   KStamp ks_;
 #ifdef GS_PROF
   unsigned long long prof_t[4] = {0, 0, 0, 0};
@@ -142,6 +145,7 @@ __global__ void __launch_bounds__(GS_THREADS) gemm_simt_kernel(const __grid_cons
   const GemmProb& P = grp.p[g];
   const int m0 = blockIdx.y * GS_T, n0 = blockIdx.x * GS_T;
   if (m0 >= P.M || n0 >= P.N) return;
+  if (!(sched & SCHED_ACTOR)) return;
 
   const float* __restrict__ A = P.A + (long long)rep * P.rsA;
   const float* __restrict__ Bm = P.B + (long long)rep * P.rsB;

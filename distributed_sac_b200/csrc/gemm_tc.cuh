@@ -258,15 +258,19 @@ B200_D void tc_split(const uint8_t* raw, uint8_t* hi, uint8_t* lo, bool mn, int 
 }
 
 template <int BN, bool PAIRED>
-__global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc_kernel(const TcProb* __restrict__ probs) {
+// sched: an actor-side launch's replica-0 schedule word (replica blockIdx.z / G at sched_stride ints further; the launch is
+// skipped on critic-only steps); null = always runs.
+__global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc_kernel(const TcProb* __restrict__ probs, const int* sched_base, int G,
+                                                                int sched_stride) {
   static_assert(!PAIRED || BN == 128, "the paired variant is the 128-wide tile");
   constexpr int NACC = PAIRED ? 2 * BN : BN;                   // accumulator columns: [main | cross] when paired
   using Cfg = TcCfg<BN>;
   constexpr int B_BYTES = Cfg::kBBytes, STAGE = Cfg::kStageBytes, S = Cfg::kStages;
   constexpr int HI_A = TC_A_BYTES, LO_A = 2 * TC_A_BYTES, RAW_B = 3 * TC_A_BYTES, HI_B = RAW_B + B_BYTES, LO_B = RAW_B + 2 * B_BYTES;
+  const int sched = sched_base ? sched_word(sched_base + (int)(blockIdx.z / G) * sched_stride) : SCHED_ACTOR;   // (sched_word)
   KStamp ks_;
-  extern __shared__ uint8_t smem_raw[];
   const TcProb* P = probs + blockIdx.z;
+  extern __shared__ uint8_t smem_raw[];
   const int M = P->M, N = P->N, K = P->K;
   const int m0 = blockIdx.y * TC_BM, n0 = blockIdx.x * BN;
   if (m0 >= M || n0 >= N) return;
@@ -308,6 +312,11 @@ __global__ void __launch_bounds__(TC_THREADS, 1) gemm_tc_kernel(const TcProb* __
     for (int kc = 0; kc < S && kc < nk; ++kc) load(kc);
   }
   __syncthreads();
+  if (!(sched & SCHED_ACTOR)) {                                // critic-only step: drain the stages requested above, leave
+    if (t == 0)
+      for (int kc = 0; kc < S && kc < nk; ++kc) mbar_wait(full_bar(kc), 0u);
+    return;
+  }
   if (t == 0) TC_STAMP(1);
 
   const bool want_bsum = (P->mode == GEMM_WGRAD) && (P->C2 != nullptr) && (blockIdx.x == 0);

@@ -27,6 +27,7 @@ constexpr int GT_ROWS_WGRAD = 32, GT_ROWS_DGRAD = GT_WARPS;
 B200_HD bool gemm_is_thin(const GemmProb& p) { return p.mode != GEMM_FWD && p.N <= GT_NMAX; }
 
 __global__ void __launch_bounds__(GT_THREADS) gemm_thin_kernel(const __grid_constant__ GemmGroup grp) {
+  const int sched = grp.sched ? sched_word(grp.sched + (int)(blockIdx.z / grp.G) * grp.sched_stride) : SCHED_ACTOR;
   KStamp ks_;
   const int G = grp.G;
   const int g = blockIdx.z % G, rep = blockIdx.z / G;
@@ -35,6 +36,7 @@ __global__ void __launch_bounds__(GT_THREADS) gemm_thin_kernel(const __grid_cons
   const bool wgrad = P.mode == GEMM_WGRAD;
   const int m0 = blockIdx.y * (wgrad ? GT_ROWS_WGRAD : GT_ROWS_DGRAD);
   if (m0 >= M) return;
+  if (!(sched & SCHED_ACTOR)) return;
 
   // B chunk [k][GT_LDB]; after the last pass the same storage holds the per-warp partial sums [16][32][17]
   __shared__ __align__(16) float sm[GT_KC * GT_LDB];

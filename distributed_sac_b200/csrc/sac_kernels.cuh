@@ -27,6 +27,14 @@ struct HParams {
   float tau_se, one_minus_tau_se; // CARE: Polyak rate of the target state encoder
 };
 
+// Mutable per-replica counters in device memory: v[0..2] Adam steps critic/actor/alpha, v[3] step index;
+// b1p/b2p[i] = beta^v[i], kept as running products so no kernel needs a double-precision pow().
+// v[4] = Adam step of the CARE(O) context encoder.
+// sched: the schedule of the step in flight (SCHED_* bits), decided by the ingest from the critic count and the replica's
+// update intervals (b200sac_set_update_intervals); every later kernel of the step reads it.
+struct Counters { long long v[5]; double b1p[5]; double b2p[5]; int sched; };
+constexpr int kSchedStride = (int)(sizeof(Counters) / sizeof(int));   // ints between two replicas' schedule words
+
 // Per-learner constant block (device copy lives in the handle).
 struct StepConst {
   int B, obs, act, T, xw;         // obs = raw observation width (state + one-hot); xw = in_w + act
@@ -42,17 +50,17 @@ struct StepConst {
   unsigned long long seed;
   const HParams* hp;              // [R] per-replica hyperparameters
   const float* isw;               // prioritized replay: [R][B] importance weights of the critic loss; null = uniform replay
+  const Counters* cnt;            // [R] step counters; .sched tells the actor-side kernels whether to run
   // Keeps sizeof(StepConst) at 136 bytes, so that the kernel arguments behind it keep their parameter-space offsets.
   // ptxas schedules a kernel differently when those move, even one that never reads the table: 32 bytes less cost the
   // policy head ~1.2 us per step of the 400-wide learners on an H100.
-  unsigned long long reserved[3];
+  unsigned long long reserved[2];
 };
 static_assert(sizeof(StepConst) == 136, "StepConst size moves the offsets of the kernel arguments behind it");
 
-// Mutable per-replica counters in device memory: v[0..2] Adam steps critic/actor/alpha, v[3] step index;
-// b1p/b2p[i] = beta^v[i], kept as running products so no kernel needs a double-precision pow().
-// v[4] = Adam step of the CARE(O) context encoder.
-struct Counters { long long v[5]; double b1p[5]; double b2p[5]; };
+// Schedule word of replica rep (read before griddepcontrol.wait: see sched_word).  On a critic-only step (no SCHED_ACTOR)
+// the actor-side launches return right after their wait.
+B200_D int sched_of(const Counters* cnt, int rep) { return __ldcg(&cnt[rep].sched); }
 
 // ------------------------------------------------------------------------------------------
 // Ingest: scatter one minibatch into the four pre-concatenated layer-0 inputs
@@ -74,6 +82,7 @@ struct IngestOut {
   // (LL/learner.py:250, MS/learner.py:337): evaluated ONCE here (fp64, rounded once) for the layer-chained kernels
   const float* log_alpha; long long rsP;     // parameter arena pointer
   float* alpha; long long rsAlpha;           // [max(T,1)] per replica
+  const int* ivl;                            // [R][2] update intervals (actor_every, target_every)
 };
 
 B200_D void ingest_row(const StepConst& K, const IngestOut& O, int rep, int i, const float* s, const float* a,
@@ -121,11 +130,20 @@ B200_D void snapshot_alpha(const StepConst& K, const IngestOut& O, int rep, int 
     (O.alpha + rep * O.rsAlpha)[t] = (float)exp((double)(O.log_alpha + rep * O.rsP)[t]);
 }
 
-B200_D void bump_counters(Counters* cnt, int rep, double beta1, double beta2) {
-  Counters* c = cnt + rep;
-  c->v[0] += 1; c->v[1] += 1; c->v[2] += 1; c->v[3] += 1; c->v[4] += 1;
+// The step's schedule is decided here, once: with n = the critic's Adam step after this step, it is an actor step iff
+// n % actor_every == 0 and a target step iff n % target_every == 0.  Only actor steps advance the actor and temperature
+// counters (torch: an optimizer whose step() is not called keeps its step count).
+B200_D void bump_counters(const IngestOut& O, int rep, double beta1, double beta2) {
+  Counters* c = O.cnt + rep;
+  const long long n = c->v[0] + 1;
+  const int ae = O.ivl[2 * rep], te = O.ivl[2 * rep + 1];
+  const bool act = ae == 1 || n % ae == 0, tgt = te == 1 || n % te == 0;   // (no 64-bit division for the default schedule)
+  c->v[0] = n; c->v[3] += 1; c->v[4] += 1;
+  if (act) { c->v[1] += 1; c->v[2] += 1; }
 #pragma unroll
-  for (int i = 0; i < 5; ++i) { c->b1p[i] *= beta1; c->b2p[i] *= beta2; }
+  for (int i = 0; i < 5; ++i)
+    if (act || (i != 1 && i != 2)) { c->b1p[i] *= beta1; c->b2p[i] *= beta2; }
+  c->sched = (act ? SCHED_ACTOR : 0) | (tgt ? SCHED_TARGET : 0);
 }
 
 // minibatch given as five separate arrays [R][B][w]
@@ -137,7 +155,7 @@ __global__ void ingest_split_kernel(StepConst K, IngestOut O, const float* __res
   const int rep = blockIdx.y;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, wpb = blockDim.x / 32;
   const int B = K.B;
-  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O.cnt, rep, K.beta1, K.beta2);
+  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O, rep, K.beta1, K.beta2);
   if (blockIdx.x == gridDim.x - 1) snapshot_alpha(K, O, rep, threadIdx.x);
   for (int i = blockIdx.x * wpb + warp; i < B; i += gridDim.x * wpb) {
     const long long ri = (long long)rep * B + i;
@@ -160,7 +178,7 @@ __global__ void ingest_rows_kernel(StepConst K, IngestOut O, const float* __rest
   const int rep = blockIdx.y;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, wpb = blockDim.x / 32;
   const int B = K.B;
-  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O.cnt, rep, K.beta1, K.beta2);
+  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O, rep, K.beta1, K.beta2);
   if (blockIdx.x == gridDim.x - 1) snapshot_alpha(K, O, rep, threadIdx.x);
   for (int i = blockIdx.x * wpb + warp; i < B; i += gridDim.x * wpb) {
     const long long src = idx ? (long long)idx[rep * rs_idx + i] : (long long)i;
@@ -515,8 +533,10 @@ struct ActorQHeadArgs {
 };
 
 __global__ void actor_q_heads_kernel(StepConst K, ActorQHeadArgs P) {
-  KStamp ks_;
   const int rep = blockIdx.y;
+  const int sched = sched_of(K.cnt, rep);
+  KStamp ks_;
+  if (!(sched & SCHED_ACTOR)) return;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int row = blockIdx.x * (blockDim.x / 32) + warp;
   const int B = K.B, H = K.Hc;
@@ -565,6 +585,7 @@ struct HeadBwdArgs {
   const float* log_alpha;
   float* dout_dbg; long long rsDbg;                          // optional dump of dout / d_action
   float* dact_dbg;
+  int actor_side;                                            // actor pass / policy backward: skipped on critic-only steps
 };
 
 // d(loss)/d(mu | log_std) of one (row, action) from the values the policy head saved: the closed-form backward of
@@ -593,8 +614,10 @@ struct PolicyDoutArgs {
 
 // Large batches: compute the policy-head output gradient once (instead of in every head_bwd CTA).
 __global__ void __launch_bounds__(256) policy_dout_kernel(StepConst K, PolicyDoutArgs P) {
-  KStamp ks_;
   const int rep = blockIdx.y, A = K.act;
+  const int sched = sched_of(K.cnt, rep);
+  KStamp ks_;
+  if (!(sched & SCHED_ACTOR)) return;
   const int e = blockIdx.x * 256 + threadIdx.x;
   if (e >= P.M * A) return;
   const int m = e / A, j = e % A;
@@ -614,9 +637,11 @@ constexpr int kHbCols = 8;     // hidden columns per CTA
 constexpr int kHbRows = 32;    // row groups per CTA (256 threads = 8 cols x 32 row groups)
 
 __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs P) {
+  const int net = blockIdx.y, rep = blockIdx.z;
+  const bool skip = P.actor_side && !(sched_of(K.cnt, rep) & SCHED_ACTOR);
   KStamp ks_;
   extern __shared__ float sm[];
-  const int net = blockIdx.y, rep = blockIdx.z;
+  if (skip) return;
   const int NO = P.NO, KD = P.Kdim;
   const int ncb = (KD + kHbCols - 1) / kHbCols;
   const int slice = blockIdx.x / ncb, cb = blockIdx.x - slice * ncb;
@@ -741,9 +766,11 @@ constexpr int kHb4Rows = 16;   // row groups per CTA
 
 template <int NOMAX>
 __global__ void __launch_bounds__(256) head_bwd4_kernel(StepConst K, HeadBwdArgs P) {
+  const int net = blockIdx.y, rep = blockIdx.z;
+  const bool skip = P.actor_side && !(sched_of(K.cnt, rep) & SCHED_ACTOR);
   KStamp ks_;
   extern __shared__ float sm[];
-  const int net = blockIdx.y, rep = blockIdx.z;
+  if (skip) return;
   const int NO = P.NO, KD = P.Kdim;
   const int ncb = (KD + kHb4Cols - 1) / kHb4Cols;
   const int slice = blockIdx.x / ncb, cb = blockIdx.x - slice * ncb;
@@ -915,6 +942,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   const int rep = blockIdx.y;
   __shared__ float red[256];
   __shared__ float s_ss, s_bc, s_tau[4];
+  __shared__ int s_sched;
   const bool is_tail = (P.tail != TAIL_NONE) && (blockIdx.x == gridDim.x - 1);
   if (!is_tail) {
     if (threadIdx.x == 0) {
@@ -922,11 +950,14 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       float a, b;
       adam_scalars(H.lr[P.which], P.cnt[rep].b1p[P.which], P.cnt[rep].b2p[P.which], a, b);
       s_ss = a; s_bc = b;
+      s_sched = sched_of(P.cnt, rep);        // the step's schedule (same cache line as the counters)
       // Polyak rates: (tau, 1 - tau) of the target critics, then of the CARE state encoder.  Read from shared memory in
       // the loop: four more live registers would cost this kernel a resident CTA per SM.
       s_tau[0] = H.tau; s_tau[1] = H.one_minus_tau; s_tau[2] = H.tau_se; s_tau[3] = H.one_minus_tau_se;
     }
     __syncthreads();
+    const int sched = s_sched;
+    if (P.which == 1 && !(sched & SCHED_ACTOR)) return;     // the actor's Adam on a critic-only step
     const float step_size = s_ss, bc2_sqrt = s_bc;
     const float w1 = (float)(1.0 - K.beta1), b2 = (float)K.beta2, omb2 = (float)(1.0 - K.beta2);
     const float eps = (float)K.adam_eps;
@@ -942,7 +973,8 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
     float4* __restrict__ m4 = reinterpret_cast<float4*>(m);
     float4* __restrict__ v4 = reinterpret_cast<float4*>(v);
     const float4* __restrict__ g4 = reinterpret_cast<const float4*>(g);
-    float4* __restrict__ t4 = P.target_delta != 0 ? reinterpret_cast<float4*>(p + P.target_delta) : nullptr;
+    // the targets are not written at all on a step without a target update (tau = 0 would turn a -0 target into +0)
+    float4* __restrict__ t4 = (P.target_delta != 0 && (sched & SCHED_TARGET)) ? reinterpret_cast<float4*>(p + P.target_delta) : nullptr;
     for (long long i = (long long)blockIdx.x * 256 + threadIdx.x; i < n4; i += (long long)nb * 256) {
       float4 pv = p4[i], mv = m4[i], vv = v4[i];
       float4 gv = g4[i];
@@ -989,6 +1021,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
     __syncthreads();
   };
   const long long slot = (P.cnt[rep].v[3] - 1) % kLossSlots;
+  const int sched = sched_of(P.cnt, rep);
   float* L = P.losses + ((long long)slot * P.R + rep) * 4;
   float* LH = P.losses_host + ((long long)slot * P.R + rep) * 4;
   if (P.tail == TAIL_CRITIC_LOSS || P.tail == TAIL_ALL) {
@@ -997,6 +1030,11 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
     block_sum2(s, 0.f, s, dummy);
     if (tid == 0) { L[0] = s * K.c_loss; LH[0] = L[0]; }
     if (P.tail == TAIL_CRITIC_LOSS) return;
+  }
+  if (!(sched & SCHED_ACTOR)) {    // no actor pass ran this step (its per-row terms are stale): no actor-side losses, no temperature step
+    if (tid == 0)
+      for (int j = 1; j < 4; ++j) { L[j] = __int_as_float(0x7fc00000); LH[j] = L[j]; }
+    return;
   }
   // TAIL_ALPHA_AND_LOSSES: actor loss, entropy, temperature gradient + its Adam step
   {

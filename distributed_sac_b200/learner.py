@@ -83,7 +83,7 @@ class _BaseLearner:
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
-                     replay_where, precision=1, prioritized=None):
+                     replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -103,6 +103,10 @@ class _BaseLearner:
         for key in list(self.server.scan_iter()):      # LL/learner.py:34-36
             self.server.delete(key)
         self.core = SacCore(self._core_config(), self.device_index, seed=seed)
+        # update() on a critic-only step (critic step count not a multiple of actor_update_interval) updates the critics
+        # only and reports NaN actor loss / entropy; the targets move when the count is a multiple of target_update_interval
+        if (actor_update_interval, target_update_interval) != (1, 1):
+            self.core.set_update_intervals(actor_update_interval, target_update_interval)
         self.memory = self._make_memory(replay_where)
         self.memory.start()
         self.save_model_path = os.path.join("saved_models", self.log_name, self.datetime)
@@ -433,11 +437,11 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
-                 precision=1, prioritized=None):
+                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized)
+                          precision, prioritized, actor_update_interval, target_update_interval)
 
     def _set_dims(self):
         c = self.cfg
@@ -460,9 +464,10 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     log_name = "MT1_Distributed_VSAC"
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
-                 device_index=0, seed=0, replay_where="host", precision=1, prioritized=None):
+                 device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
+                 target_update_interval=1):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized)
+                          precision, prioritized, actor_update_interval, target_update_interval)
 
     def _set_dims(self):
         c = self.cfg
@@ -487,10 +492,11 @@ class MTSACLearner(_BaseLearner):
     _iteration_key = "update_iteration"
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
-                 *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None):
+                 *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
+                 actor_update_interval=1, target_update_interval=1):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized)
+                          precision, prioritized, actor_update_interval, target_update_interval)
 
     def _set_dims(self):
         c = self.cfg

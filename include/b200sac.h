@@ -22,6 +22,9 @@
  *   b200sac_get/set_hparams, b200sac_copy_replica
  *                            the hyperparameters build_optimizer / update_SAC / soft_update fix per learner, made per replica
  *                            LunarLander_Distributed_SAC/src/learner.py:115-137,210; MT10_Distributed_CARE/src/learner.py:136-158,361-367
+ *   b200sac_get/set_update_intervals
+ *                            actor / target update intervals (TD3 policy_delay, pytorch_sac actor_update_frequency and
+ *                            critic_target_update_frequency, SB3 target_update_interval), per replica
  *   b200sac_publish_*        Learner.get_parameters()         learner.py:272-276 (called at :298-299)
  *   b200sac_blob_*           server.set('parameters', _pickle.dumps(get_parameters())) in Learner.run()
  *                            learner.py:298-299 (MT10_Distributed_CARE/src/learner.py:442-443): the byte string, device-assembled
@@ -164,11 +167,31 @@ int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp
  * copied. */
 int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream);
 
+/* Per-replica update intervals, both 1 (every step is a full step) after b200sac_create.  Let n be the replica's critic
+ * Adam step count after a step (steps[0] of b200sac_get_steps).  The step is
+ *   - an ACTOR step iff n % actor_every == 0: it updates the actor and the temperature log_alpha (Adam), as always.  On any
+ *     other step (a critic-only step) the actor parameters, log_alpha, their Adam m / v and the actor and temperature step
+ *     counters are left bit for bit as they were: exactly as if the reference skipped actor_optimizer.step() and
+ *     alpha_optimizer.step(), so Adam's bias correction counts only the updates that happened;
+ *   - a TARGET step iff n % target_every == 0: the target critics get their Polyak update (tau) and, with CARE, the target
+ *     state encoder its update (tau_se).  On other steps the targets are not written at all.
+ * Everything else runs on every step: the critic update (TD target with the current actor and the temperature of the
+ * step), prioritized-replay weights and priority updates, the CARE(O) context encoder's Adam, the step index.
+ * The phase follows the counters, so it carries over b200sac_set_steps, checkpoint restores and b200sac_copy_replica
+ * (which copies the counters but, like the hyperparameters, not the intervals).
+ * Set: enqueued on `stream` like b200sac_set_hparams -- applies to every step enqueued after it and to none enqueued before
+ * it, including between launches of the graphs b200sac_prepare instantiated.  Both values must be in [1, 2^30]; otherwise
+ * B200SAC_ERR_INVALID and nothing changes.  Get: the values last set (host mirror: does not synchronise). */
+int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32_t actor_every, int32_t target_every, void* stream);
+int b200sac_get_update_intervals(b200sac_t* h, int32_t replica, int32_t* actor_every, int32_t* target_every);
+
 /* One gradient step from caller-provided DEVICE minibatches, each
  * [replicas][batch][width] fp32: s,s2 width obs(=state_dim+num_tasks), a width act, r,d width 1.
  * eps_next / eps_cur: [replicas][batch][act] standard-normal noise for the two
  * rsample() calls (next-state actor first), or NULL to draw in-kernel (Philox).
- * Losses land in an internal device ring; fetch with b200sac_read_losses. */
+ * Losses land in an internal device ring; fetch with b200sac_read_losses.
+ * Every step entry point (b200sac_step, _step_host, _step_sampled, _update) follows each replica's update intervals
+ * (b200sac_set_update_intervals): a critic-only step updates the critics only. */
 int b200sac_step(b200sac_t* h, const float* s, const float* a, const float* r, const float* s2,
                  const float* d, const float* eps_next, const float* eps_cur, void* stream);
 
@@ -197,7 +220,8 @@ int b200sac_prepare(b200sac_t* h, b200sac_replay_t* rb, void* stream);
 int b200sac_update(b200sac_t* h, b200sac_replay_t* rb, float* losses_host, void* stream);
 
 /* Losses of the most recent `n_last` steps (<= 1024 kept): out[n_last][replicas][4].
- * Synchronises the stream. */
+ * On a replica's critic-only step (b200sac_set_update_intervals) the actor loss, alpha loss and entropy entries are NaN
+ * (the same holds for b200sac_step_host and b200sac_update).  Synchronises the stream. */
 int b200sac_read_losses(b200sac_t* h, int32_t n_last, float* out_host, void* stream);
 
 /* Polyak update of the target critics outside a step (Learner.soft_update; tau = 1 is
