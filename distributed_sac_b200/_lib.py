@@ -72,8 +72,6 @@ SYMBOLS = {
     "b200sac_read_losses": (C.c_int, [_VP, C.c_int32, _VP, _VP]),
     "b200sac_soft_update": (C.c_int, [_VP, C.c_double, _VP]),
     "b200sac_act": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_int32, _VP, _VP]),
-    "b200sac_publish_begin": (C.c_int, [_VP, C.c_int32, C.c_int32, C.POINTER(C.c_int64), C.POINTER(C.c_int64), _VP]),
-    "b200sac_publish_wait": (C.c_int, [_VP, C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.c_int64)]),
     "b200sac_blob_template": (C.c_int, [_VP, C.c_int32, _VP, C.c_int64, C.c_int64, _VP, _VP]),
     "b200sac_blob_begin": (C.c_int, [_VP, _VP]),
     "b200sac_blob_wait": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(C.c_int64)]),

@@ -163,7 +163,7 @@ class SacCore:
     def _unpack(self, name, flat, off):
         """One layout-table entry read out of `flat` (float32 numpy array) at float offset `off`, as a fresh CPU tensor in
         the reference's shape.  numpy copies on purpose: a 256x256 torch .clone() fans out to the intra-op thread pool,
-        which costs milliseconds on a busy host -- this runs after every update (publication path)."""
+        which costs milliseconds on a busy host."""
         return torch.from_numpy(np.array(self._view(name, flat, off), dtype=np.float32, order="C", copy=True))
 
     def _view(self, name, flat, off):
@@ -188,43 +188,12 @@ class SacCore:
         _lib.check(self.lib.b200sac_act(self._h, replica, n, _ptr(obs), _ptr(e), 1 if stochastic else (-1 if no_tanh else 0), _ptr(out), _stream()))
         return out
 
-    # ---- publication path (Learner.get_parameters, LL/learner.py:272-276) ---------------------------
-    def publish_begin(self, tensor_names, replica=0):
-        """Enqueue a consistent snapshot of the named parameter tensors and start its async copy to pinned host
-        memory (b200sac_publish_begin); steps enqueued afterwards overlap it.  Collect with publish_wait()."""
-        ents = sorted((self.table[n][0], self.table[n][1] * self.table[n][5], n) for n in tensor_names)
-        ranges, where = [], {}                   # merge neighbouring tensors (16-B alignment gaps of <= 3 floats are copied along)
-        for off, cnt, n in ents:
-            if ranges and 0 <= off - (ranges[-1][0] + ranges[-1][1]) <= 3:
-                ranges[-1][1] = off + cnt - ranges[-1][0]
-            else:
-                ranges.append([off, cnt])
-            where[n] = sum(r[1] for r in ranges[:-1]) + (off - ranges[-1][0])
-        offs = (C.c_int64 * len(ranges))(*[r[0] for r in ranges])
-        cnts = (C.c_int64 * len(ranges))(*[r[1] for r in ranges])
-        _lib.check(self.lib.b200sac_publish_begin(self._h, replica, len(ranges), offs, cnts, _stream()))
-        self._pub_where = where
-
     def read_named(self, name, which=_lib.PARAMS, replica=0) -> torch.Tensor:
         """One small tensor (e.g. log_alpha) straight from the device: a few floats cross PCIe, not the arena."""
         off, rows, cols, _t, _o, pitch = self.table[name]
         out = torch.empty(rows * pitch)
         _lib.check(self.lib.b200sac_read_range(self._h, which, replica, off, rows * pitch, _ptr(out), _stream()))
         return self._unpack(name, out.numpy(), 0)
-
-    def publish_views(self) -> Dict[str, np.ndarray]:
-        """Like publish_wait(), but returns numpy VIEWS of the pinned snapshot in the reference's shapes (no copy); valid
-        until the next publish_begin()."""
-        ptr, n = C.POINTER(C.c_float)(), C.c_int64()
-        _lib.check(self.lib.b200sac_publish_wait(self._h, C.byref(ptr), C.byref(n)))
-        flat = np.ctypeslib.as_array(ptr, shape=(n.value,))
-        return {name: self._view(name, flat, at) for name, at in self._pub_where.items()}
-
-    def publish_wait(self) -> Dict[str, torch.Tensor]:
-        ptr, n = C.POINTER(C.c_float)(), C.c_int64()
-        _lib.check(self.lib.b200sac_publish_wait(self._h, C.byref(ptr), C.byref(n)))
-        flat = np.ctypeslib.as_array(ptr, shape=(n.value,))       # view of the pinned buffer; _unpack copies out of it
-        return {name: self._unpack(name, flat, at) for name, at in self._pub_where.items()}
 
     # ---- blob publication (b200sac_blob_*): the published byte string is assembled on the device -------------------
     def tensor_shape(self, name):

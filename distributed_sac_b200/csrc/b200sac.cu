@@ -319,17 +319,11 @@ struct b200sac {
   bool stage_used[2] = {false, false};
   int prefetch_slot = -1;         // host-ring step_sampled: minibatch already drawn, gathered and in flight (H2D)
   b200sac_replay* prefetch_rb = nullptr;
-  // publication path (b200sac_publish_*): device snapshot -> pinned host, on its own stream
-  // two snapshot slots: the caller may build the published blob from snapshot k while snapshot k+1 (begun after the next
-  // step was enqueued) is still landing
-  cudaStream_t pub = nullptr;
-  cudaEvent_t ev_pub_snap[2] = {nullptr, nullptr}, ev_pub_done[2] = {nullptr, nullptr};
-  float* pub_d[2] = {nullptr, nullptr};   // device snapshots (consistent: taken in stream order between two steps)
-  float* pub_h[2] = {nullptr, nullptr};   // pinned host copies handed to the caller
-  int64_t pub_cap = 0, pub_n[2] = {0, 0};
-  int pub_head = 0, pub_pending = 0;      // next slot to fill; snapshots begun and not yet collected (<= 2)
   // blob publication (b200sac_blob_*): the published byte string is assembled ON THE DEVICE (constant bytes + float payloads
-  // gathered from the arena by a kernel) and crosses PCIe as one copy; the host never touches individual tensors
+  // gathered from the arena by a kernel) and crosses PCIe as one copy on its own stream; the host never touches individual
+  // tensors.  Two image slots: the caller may hand on blob k while blob k+1 (begun after the next step was enqueued) is
+  // still landing
+  cudaStream_t pub = nullptr;
   uint8_t* blob_d[2] = {nullptr, nullptr};
   uint8_t* blob_h[2] = {nullptr, nullptr};
   int* blob_src = nullptr;                // [blob_nf] arena index of payload float j
@@ -405,10 +399,6 @@ static int destroy_impl(b200sac* h) {
   if (h->loss_h) cudaFreeHost(h->loss_h);
   if (h->pub) { cudaStreamSynchronize(h->pub); cudaStreamDestroy(h->pub); }
   for (int i = 0; i < 2; ++i) {
-    if (h->ev_pub_snap[i]) cudaEventDestroy(h->ev_pub_snap[i]);
-    if (h->ev_pub_done[i]) cudaEventDestroy(h->ev_pub_done[i]);
-    cudaFree(h->pub_d[i]);
-    if (h->pub_h[i]) cudaFreeHost(h->pub_h[i]);
     if (h->ev_blob_snap[i]) cudaEventDestroy(h->ev_blob_snap[i]);
     if (h->ev_blob_done[i]) cudaEventDestroy(h->ev_blob_done[i]);
     cudaFree(h->blob_d[i]);
@@ -2253,80 +2243,6 @@ extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void
   CU(cudaMemcpyAsync(h->adam_v + dst * nt, h->adam_v + src * nt, nt * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
   CU(cudaMemcpyAsync(h->cnt + dst, h->cnt + src, sizeof(Counters), cudaMemcpyDeviceToDevice, sb.run));
   return sb.end();
-}
-
-// ------------------------------------------------------------------------------------------
-// Publication path: Learner.get_parameters() -> pickle -> Redis runs after EVERY update in the reference
-// (LunarLander_Distributed_SAC/src/learner.py:272-276,298-299; MT10_Distributed_CARE/src/learner.py:412-417,442-443)
-// and costs one synchronous .cpu() per tensor.  Here: a device-to-device snapshot of the requested arena
-// ranges is enqueued in stream order (so it is the state after the steps enqueued so far, never a torn
-// one), the D2H copy into pinned memory runs on a private stream behind the next steps, and the host
-// only blocks in publish_wait.
-// ------------------------------------------------------------------------------------------
-extern "C" int b200sac_publish_begin(b200sac_t* h, int32_t replica, int32_t n_ranges, const int64_t* offsets, const int64_t* counts,
-                                     void* stream) {
-  if (!h || !offsets || !counts || n_ranges <= 0) return fail(B200SAC_ERR_INVALID, "bad argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  int64_t total = 0;
-  for (int i = 0; i < n_ranges; ++i) {
-    if (offsets[i] < 0 || counts[i] <= 0 || offsets[i] + counts[i] > h->L.arena)
-      return fail(B200SAC_ERR_INVALID, "range %d [%lld, +%lld) outside the %lld-float parameter arena", i, (long long)offsets[i],
-                  (long long)counts[i], (long long)h->L.arena);
-    total += counts[i];
-  }
-  CU(cudaSetDevice(h->device));
-  if (!h->pub) {
-    CU(cudaStreamCreateWithFlags(&h->pub, cudaStreamNonBlocking));
-    for (int i = 0; i < 2; ++i) {
-      CU(cudaEventCreateWithFlags(&h->ev_pub_snap[i], cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(&h->ev_pub_done[i], cudaEventDisableTiming));
-    }
-  }
-  if (h->pub_pending == 2) {            // both slots hold uncollected snapshots: the older one is superseded
-    CU(cudaEventSynchronize(h->ev_pub_done[h->pub_head]));
-    h->pub_pending = 1;
-  }
-  if (total > h->pub_cap) {
-    CU(cudaStreamSynchronize(h->pub));
-    for (int i = 0; i < 2; ++i) {
-      cudaFree(h->pub_d[i]); h->pub_d[i] = nullptr;
-      if (h->pub_h[i]) { cudaFreeHost(h->pub_h[i]); h->pub_h[i] = nullptr; }
-      CU(cudaMalloc(&h->pub_d[i], (size_t)total * sizeof(float)));
-      CU(cudaHostAlloc(&h->pub_h[i], (size_t)total * sizeof(float), cudaHostAllocDefault));
-    }
-    h->pub_cap = total;
-    h->pub_pending = 0;
-  }
-  const int slot = h->pub_head;
-  StreamBridge sb(h, stream);
-  if (int rc = sb.begin()) return rc;
-  const float* base = h->params + (size_t)replica * h->L.arena;
-  int64_t at = 0;
-  for (int i = 0; i < n_ranges; ++i) {
-    CU(cudaMemcpyAsync(h->pub_d[slot] + at, base + offsets[i], (size_t)counts[i] * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
-    at += counts[i];
-  }
-  CU(cudaEventRecord(h->ev_pub_snap[slot], sb.run));
-  if (int rc = sb.end()) return rc;
-  CU(cudaStreamWaitEvent(h->pub, h->ev_pub_snap[slot], 0));
-  CU(cudaMemcpyAsync(h->pub_h[slot], h->pub_d[slot], (size_t)total * sizeof(float), cudaMemcpyDeviceToHost, h->pub));
-  CU(cudaEventRecord(h->ev_pub_done[slot], h->pub));
-  h->pub_n[slot] = total;
-  h->pub_head ^= 1;
-  h->pub_pending += 1;
-  return 0;
-}
-
-extern "C" int b200sac_publish_wait(b200sac_t* h, const float** host_ptr, int64_t* n_floats) {
-  if (!h || !host_ptr || !n_floats) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (h->pub_pending <= 0) return fail(B200SAC_ERR_STATE, "publish_wait without publish_begin");
-  CU(cudaSetDevice(h->device));
-  const int slot = (h->pub_head + 2 - h->pub_pending) & 1;      // the oldest snapshot not collected yet
-  CU(cudaEventSynchronize(h->ev_pub_done[slot]));
-  h->pub_pending -= 1;
-  *host_ptr = h->pub_h[slot];
-  *n_floats = h->pub_n[slot];
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------

@@ -186,22 +186,12 @@ class _BaseLearner:
     # ---- parameter publication (LL/learner.py:272-276; consumed by Player.pull_parameters, player.py:75-85) ----
     _published = ("actor",)
 
-    def publish_begin(self):
-        """Start an asynchronous snapshot of the published modules (b200sac_publish_begin): a device-side copy in
-        stream order after the steps enqueued so far, then D2H into pinned memory on a private stream."""
-        self._pub_maps = [(net, self._key_map(net)) for net in self._published]
-        # (+ the temperature: the logger's alpha then comes from the same consistent snapshot, not from a second,
-        #  stream-ordered read that would wait for whatever step is running by then)
-        self.core.publish_begin({canon for _, m in self._pub_maps for canon in m.values()} | {"log_alpha"})
-
-    def publish_wait(self):
-        named = self.core.publish_wait()
-        return {net: {ref: named[canon] for ref, canon in m.items()} for net, m in self._pub_maps}
-
     def get_parameters(self):
-        """{'actor': state_dict on the CPU} with the reference's key names -- only the published slices cross PCIe."""
-        self.publish_begin()
-        return self.publish_wait()
+        """{'actor': state_dict on the CPU} with the reference's key names: the unpickled parameters_blob(blocking=True),
+        so only the published floats cross PCIe, in one copy, and the object is exactly what run() publishes.  Like
+        parameters_blob(blocking=True) it returns the OLDEST blob not collected yet: the state after the steps enqueued so
+        far unless a blob_begin() is still outstanding."""
+        return _pickle.loads(self.parameters_blob(blocking=True))
 
     def parameters_blob(self, blocking=True):
         """The bytes Learner.run() stores under the Redis key 'parameters' (LL/learner.py:298-299): _pickle.dumps of
@@ -235,30 +225,6 @@ class _BaseLearner:
         # (+ the temperature behind the image: the logger's alpha then comes from the same consistent snapshot)
         self.core.blob_template(blob, slots, extra=("log_alpha",))
         self._blob_ready = True
-
-    def _blob_from_views(self, views):
-        """Host-side variant (snapshot views -> bytes patched into the pickle template); kept for callers of
-        publish_begin()/core.publish_views()."""
-        tpl = getattr(self, "_blob_tpl", None)
-        if tpl is None:
-            rng = np.random.default_rng(12345)
-            fake = {net: {ref: torch.from_numpy(rng.random(views[canon].shape, dtype=np.float32) + 1.0) for ref, canon in m.items()}
-                    for net, m in self._pub_maps}
-            blob = _pickle.dumps(fake)
-            where = []
-            for net, m in self._pub_maps:
-                for ref, canon in m.items():
-                    payload = fake[net][ref].numpy().tobytes()
-                    at = blob.find(payload)
-                    if at < 0 or blob.find(payload, at + 1) >= 0:
-                        raise RuntimeError(f"cannot locate the payload of {net}.{ref} in the pickle stream")
-                    where.append((canon, at, views[canon].shape))
-            tpl = self._blob_tpl = (blob, where)
-        blob, where = tpl
-        buf = bytearray(blob)
-        for canon, at, shape in where:
-            np.frombuffer(buf, dtype=np.float32, count=int(np.prod(shape)), offset=at).reshape(shape)[...] = views[canon]
-        return bytes(buf)
 
     def my_print(self, content):
         os.makedirs(os.path.dirname(self.log_file), exist_ok=True)

@@ -16,8 +16,8 @@
  *                            LunarLander_Distributed_SAC/src/replay_buffer.py:43-77
  *                            MT10_Distributed_MTSAC/src/replay_buffers.py:47-107
  *   b200sac_layout/export/import
- *                            build_model/build_optimizer/get_parameters/save_checkpoint
- *                            LunarLander_Distributed_SAC/src/learner.py:100-124,144-163,272-276
+ *                            build_model/build_optimizer/save_checkpoint
+ *                            LunarLander_Distributed_SAC/src/learner.py:100-124,144-163
  *   b200sac_soft_update      Learner.soft_update()            learner.py:126-137
  *   b200sac_get/set_hparams, b200sac_copy_replica
  *                            the hyperparameters build_optimizer / update_SAC / soft_update fix per learner, made per replica
@@ -25,9 +25,9 @@
  *   b200sac_get/set_update_intervals
  *                            actor / target update intervals (TD3 policy_delay, pytorch_sac actor_update_frequency and
  *                            critic_target_update_frequency, SB3 target_update_interval), per replica
- *   b200sac_publish_*        Learner.get_parameters()         learner.py:272-276 (called at :298-299)
- *   b200sac_blob_*           server.set('parameters', _pickle.dumps(get_parameters())) in Learner.run()
- *                            learner.py:298-299 (MT10_Distributed_CARE/src/learner.py:442-443): the byte string, device-assembled
+ *   b200sac_blob_*           Learner.get_parameters() and server.set('parameters', _pickle.dumps(get_parameters())) in
+ *                            Learner.run(), learner.py:272-276,298-299 (MT10_Distributed_CARE/src/learner.py:412-417,442-443):
+ *                            the byte string, device-assembled
  *   b200sac_act              Actor.get_action() for a batch of environments
  *                            LunarLander_Distributed_SAC/src/model.py:67-82; MT10_Distributed_CARE/src/player.py:199-209 (CARE handles)
  *
@@ -240,19 +240,6 @@ int b200sac_soft_update(b200sac_t* h, double tau, void* stream);
 int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* eps, int32_t stochastic,
                 float* actions_out, void* stream);
 
-/* Publication path = Learner.get_parameters() (LunarLander_Distributed_SAC/src/learner.py:272-276,298-299;
- * MT10_Distributed_CARE/src/learner.py:412-417,442-443), which the reference runs after every update.
- * publish_begin enqueues, in stream order, a consistent device snapshot of `n_ranges` ranges
- * [offsets[i], offsets[i]+counts[i]) of replica `replica`'s parameter arena (offsets from b200sac_layout)
- * and starts its copy to pinned host memory on a private stream; it does not block, and steps enqueued
- * afterwards overlap the copy.  publish_wait blocks until the OLDEST uncollected snapshot has landed and returns its
- * packed ranges.  Two snapshot slots: publish_begin may be called again before the previous snapshot is collected (the
- * caller then turns snapshot k into the published blob while step k+1 runs and snapshot k+1 lands); the pointer stays
- * valid until the second publish_begin after the one that produced it.  A third begin without a wait supersedes the oldest. */
-int b200sac_publish_begin(b200sac_t* h, int32_t replica, int32_t n_ranges, const int64_t* offsets, const int64_t* counts,
-                          void* stream);
-int b200sac_publish_wait(b200sac_t* h, const float** host_ptr, int64_t* n_floats);
-
 /* Blob publication: the byte string Learner.run() stores under the Redis key 'parameters' after every update
  * (LunarLander_Distributed_SAC/src/learner.py:298-299: _pickle.dumps({'actor': state_dict}); read back by
  * Player.pull_parameters, player.py:75-85) assembled on the device.  blob_template: `image` = the constant bytes of the
@@ -261,7 +248,8 @@ int b200sac_publish_wait(b200sac_t* h, const float** host_ptr, int64_t* n_floats
  * are expressed through the index map).  blob_begin enqueues, in stream order, the gather of all payload floats into a
  * device copy of the image and starts ONE D2H copy of it on a private stream; it does not block and later steps overlap
  * the copy.  blob_wait blocks until the OLDEST uncollected blob has landed in pinned memory and returns it (valid until
- * the second blob_begin after the one that produced it; two image slots, as for publish_begin/wait). */
+ * the second blob_begin after the one that produced it).  Two image slots: blob_begin may be called again before the
+ * previous blob is collected; a third begin without a wait supersedes the oldest. */
 int b200sac_blob_template(b200sac_t* h, int32_t replica, const uint8_t* image, int64_t image_bytes, int64_t n_floats,
                           const int32_t* src_index, const int32_t* dst_byte);
 int b200sac_blob_begin(b200sac_t* h, void* stream);

@@ -181,14 +181,14 @@ def test_care_learner_surface(cuda, tmp_path, modified):
         assert sorted(ceo["state"]) == list(range(1, 11)) and int(ceo["state"][1]["step"]) == 4
         assert ceo["param_groups"][0]["params"] == list(range(11))
         assert ceo["state"][1]["exp_avg"].shape == (100, 768) and ceo["state"][10]["exp_avg"].shape == (50,)
-    # the bytes run() publishes == a plain pickle of get_parameters() once unpickled
+    # the bytes run() publishes, once unpickled == every published module read out of the whole arena
     pub = pickle.loads(lrn.parameters_blob(blocking=True))
-    ref_pub = lrn.get_parameters()
-    assert set(pub) == set(ref_pub)
-    for net in ref_pub:
-        assert set(pub[net]) == set(ref_pub[net])
-        for k in ref_pub[net]:
-            assert pub[net][k].dtype == torch.float32 and torch.equal(pub[net][k], ref_pub[net][k]), (net, k)
+    assert set(pub) == set(lrn._published)
+    for net in pub:
+        full = lrn._module_state_dict(net)
+        assert set(pub[net]) == set(full)
+        for k in full:
+            assert pub[net][k].dtype == torch.float32 and torch.equal(pub[net][k], full[k]), (net, k)
     before = lrn.core.export_arena()
     lrn2 = CARELearner(None, names_, str(p), write_mode=False, server=redis_stub.StrictRedis(host=str(tmp_path) + "d"),
                        seed=5, checkpoint_path=path)
@@ -197,8 +197,8 @@ def test_care_learner_surface(cuda, tmp_path, modified):
     lrn2.memory.stop()
 
 
-def test_publication_snapshot_is_consistent_and_async(cuda, tmp_path):
-    """get_parameters() through b200sac_publish_*: (1) bit-identical to the full-arena export; (2) a snapshot
+def test_published_blob_is_consistent_and_async(cuda, tmp_path):
+    """get_parameters() and the published blob (b200sac_blob_*): (1) bit-identical to the full-arena export; (2) a blob
     begun after step k and collected after further steps were enqueued is the state after step k, not a torn
     or later one (it is what an unmodified Player would load, LL/player.py:75-85)."""
     lrn = _ll_learner(tmp_path, seed=11)
@@ -213,11 +213,8 @@ def test_publication_snapshot_is_consistent_and_async(cuda, tmp_path):
     fast = pickle.loads(lrn.parameters_blob(blocking=True))["actor"]      # template-patched pickle stream (run() publishes this)
     assert set(fast) == set(full) and all(torch.equal(fast[k], full[k]) and fast[k].is_contiguous() for k in full)
     assert torch.equal(lrn.log_alpha, lrn.core.get_named()["log_alpha"])          # small-range read == arena export
-    lrn.publish_begin()                                          # snapshot after step 3 ...
-    lrn.core.blob_begin()                                        # ... and the device-assembled blob of the same state ...
-    lrn.core.step_sampled(lrn.memory.ring, 40)                   # ... while 40 more steps are enqueued behind them
-    snap = lrn.publish_wait()["actor"]
-    assert all(torch.equal(snap[k], full[k]) for k in full)
+    lrn.core.blob_begin()                                        # the device-assembled blob after step 3 ...
+    lrn.core.step_sampled(lrn.memory.ring, 40)                   # ... while 40 more steps are enqueued behind it
     blob3, extra3 = lrn.core.blob_wait()
     snap_b = pickle.loads(blob3)["actor"]
     assert all(torch.equal(snap_b[k], full[k]) for k in full)

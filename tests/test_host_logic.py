@@ -76,62 +76,6 @@ def test_product_fails_loudly_without_cuda():
         SacCore(CoreConfig())
 
 
-def test_publication_ranges_and_unpack_without_a_gpu():
-    """Host side of the publication path (core.publish_begin / publish_wait): adjacent tensors are merged into one copy range,
-    padded first-layer pitches and the (K,in,out) mixture layout are undone, and every returned tensor owns its memory."""
-    import ctypes as C
-    import numpy as np
-    from distributed_sac_b200.core import CoreConfig, SacCore, layout
-
-    cfg = CoreConfig(state_dim=39, act_dim=4, actor_hidden=[16, 12], critic_hidden=[16, 12], batch=60, num_tasks=10, care=True,
-                     num_encoders=3, mix_hidden=[8], mix_out=6, ctx_in=20, ctx_hidden=[7], ctx_out=5)
-    table, arena, _trainable = layout(cfg)
-    flat = np.arange(arena, dtype=np.float32)
-
-    calls = {}
-
-    class StubLib:
-        def b200sac_publish_begin(self, h, replica, n, offs, cnts, stream):
-            calls["ranges"] = [(offs[i], cnts[i]) for i in range(n)]
-            return 0
-
-        def b200sac_publish_wait(self, h, ptr, n):
-            packed = np.concatenate([flat[o:o + c] for o, c in calls["ranges"]])
-            calls["buf"] = packed                                   # keep alive
-            C.cast(ptr, C.POINTER(C.POINTER(C.c_float)))[0] = packed.ctypes.data_as(C.POINTER(C.c_float))
-            C.cast(n, C.POINTER(C.c_int64))[0] = packed.size
-            return 0
-
-    core = object.__new__(SacCore)
-    core.lib, core._h, core.cfg, core.table = StubLib(), None, cfg, table
-    import distributed_sac_b200.core as core_mod
-    real_stream = core_mod._stream
-    core_mod._stream = lambda: None
-    try:
-        names = [n for n in table if n.startswith("actor.")] + [n for n in table if n.startswith("cse.")]
-        core.publish_begin(names)
-        got = core.publish_wait()
-    finally:
-        core_mod._stream = real_stream
-    # actor and cse blocks are each contiguous, and q1/q2 lie between them: exactly two ranges
-    assert len(calls["ranges"]) == 2
-    assert set(got) == set(names)
-    for n, t in got.items():
-        off, rows, cols, _tr, _opt, pitch = table[n]
-        ref = flat[off:off + rows * pitch].reshape(rows, pitch)[:, :cols]
-        if ".mix." in n and n.endswith(".W"):
-            K = cfg.num_encoders
-            assert t.shape == (K, cols, rows // K)
-            assert np.array_equal(t.numpy(), ref.reshape(K, rows // K, cols).transpose(0, 2, 1))
-        elif ".mix." in n:
-            assert t.shape == (cfg.num_encoders, 1, rows // cfg.num_encoders)
-        else:
-            assert np.array_equal(t.numpy().reshape(rows, cols), ref)
-        assert t.numpy().base is None or not np.shares_memory(t.numpy(), calls["buf"])
-    w0 = table["actor.0.weight"]
-    assert w0[5] >= w0[2] and w0[5] % 4 == 0                       # padded pitch of the first layer is hidden from the caller
-
-
 class BlobStubLib:
     """CPU stand-in for b200sac_blob_*: emulates the device gather (payload float j = arena[src[j]] -> image bytes at dst[j])."""
 
@@ -166,7 +110,8 @@ def test_parameters_blob_device_image_round_trips():
     """Learner.parameters_blob(): the pickle stream is built once from tensors of the published shapes and registered as a byte
     image + index maps (core.blob_template); a publication only gathers arena floats into the payload positions.  With the
     gather emulated on the CPU, unpickling must give exactly what a plain pickle.dumps of the state_dict gives -- through the
-    padded first-layer pitch and the CARE (K,in,out) mixture layout."""
+    padded first-layer pitch and the CARE (K,in,out) mixture layout -- get_parameters() must give the same object, and every
+    unpickled tensor owns its memory."""
     import pickle
     import numpy as np
     import torch
@@ -206,9 +151,22 @@ def test_parameters_blob_device_image_round_trips():
                     t = got[net][ref]
                     assert isinstance(t, torch.Tensor) and t.dtype == torch.float32 and tuple(t.shape) == want.shape, (canon, t.shape, want.shape)
                     assert np.array_equal(t.numpy(), want), canon
+                    stored = flat[off:off + rows * pitch].reshape(rows, pitch)[:, :cols]    # pad columns dropped
+                    if ".mix." in canon and canon.endswith(".W"):                         # stored [K][out][in]
+                        K = cfg.num_encoders
+                        assert t.shape == (K, cols, rows // K)
+                        assert np.array_equal(t.numpy(), stored.reshape(K, rows // K, cols).transpose(0, 2, 1)), canon
+                    elif ".mix." in canon:                                                # stored [K][out]
+                        assert t.shape == (cfg.num_encoders, 1, rows // cfg.num_encoders)
+                    else:
+                        assert np.array_equal(t.numpy().reshape(rows, cols), stored), canon
+                    assert not np.shares_memory(t.numpy(), core.lib.out), canon
             plain = pickle.loads(pickle.dumps({net: {ref: torch.from_numpy(np.ascontiguousarray(core._view(c_, flat, table[c_][0])))
                                                      for ref, c_ in m.items()} for net, m in km.items()}))
             assert all(torch.equal(plain[net][k], got[net][k]) for net in km for k in km[net])
+            params = lrn.get_parameters()
+            assert {net: set(sd) for net, sd in params.items()} == {net: set(sd) for net, sd in got.items()}
+            assert all(torch.equal(params[net][k], got[net][k]) for net in km for k in km[net])
             _blob, extra = core.blob_wait()                          # (the stub keeps the last image) the logger's temperature
             assert np.array_equal(extra["log_alpha"], flat[table["log_alpha"][0]:table["log_alpha"][0] + table["log_alpha"][1]])
     finally:
