@@ -71,6 +71,7 @@ SYMBOLS = {
     "b200sac_prepare": (C.c_int, [_VP, _VP, _VP]),
     "b200sac_read_losses": (C.c_int, [_VP, C.c_int32, _VP, _VP]),
     "b200sac_soft_update": (C.c_int, [_VP, C.c_double, _VP]),
+    "b200sac_soft_update_critic": (C.c_int, [_VP, C.c_int32, C.c_double, _VP]),
     "b200sac_act": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_int32, _VP, _VP]),
     "b200sac_blob_template": (C.c_int, [_VP, C.c_int32, _VP, C.c_int64, C.c_int64, _VP, _VP]),
     "b200sac_blob_begin": (C.c_int, [_VP, _VP]),

@@ -329,8 +329,13 @@ class SacCore:
         device to device on the current stream.  Hyperparameters, update intervals and replay data stay dst's own."""
         _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
 
-    def soft_update(self, tau: float):
-        _lib.check(self.lib.b200sac_soft_update(self._h, float(tau), _stream()))
+    def soft_update(self, tau: float, critic: Optional[int] = None):
+        """Polyak update of the targets outside a step: both critics (CARE: and the target state encoder, with the replica's
+        tau_se unless tau == 1), or with critic=1 / 2 only q1_target / q2_target."""
+        if critic is None:
+            _lib.check(self.lib.b200sac_soft_update(self._h, float(tau), _stream()))
+        else:
+            _lib.check(self.lib.b200sac_soft_update_critic(self._h, int(critic), float(tau), _stream()))
 
     # ---- stepping -----------------------------------------------------------------------
     def _shape_check(self, s, a, r, s2, d, eps_next, eps_cur):

@@ -2907,6 +2907,20 @@ extern "C" int b200sac_soft_update(b200sac_t* h, double tau, void* stream) {
   return 0;
 }
 
+extern "C" int b200sac_soft_update_critic(b200sac_t* h, int32_t critic, double tau, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (critic != 1 && critic != 2) return fail(B200SAC_ERR_INVALID, "critic must be 1 or 2, got %d", critic);
+  CU(cudaSetDevice(h->device));
+  // q1 and q2 are each contiguous in [critic_begin, cse_begin), q2 right behind q1; their targets sit at + target_delta
+  const Layout& L = h->L;
+  const int64_t q2_begin = L.q[1][0].w;
+  const int64_t beg = critic == 1 ? L.critic_begin : q2_begin, end = critic == 1 ? q2_begin : L.cse_begin;
+  polyak_kernel<<<dim3(128, h->R), 256, 0, (cudaStream_t)stream>>>(h->params + beg, L.arena, end - beg, L.target_delta,
+                                                                  (float)tau, (float)(1.0 - tau));
+  CU(cudaGetLastError());
+  return 0;
+}
+
 extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replica, float* out_host, int64_t cap_floats,
                                   int64_t* n_floats, void* stream) {
   if (!h || !name || !out_host) return fail(B200SAC_ERR_INVALID, "null argument");

@@ -165,13 +165,20 @@ class _BaseLearner:
         """No-op: gradients never outlive a step in the fused path."""
 
     def soft_update(self, local_model=None, target_model=None, tau=None):
-        """theta_target = tau*theta_local + (1-tau)*theta_target for both critics (LL/learner.py:126-137).
-        The step itself already applies the per-step Polyak update; this entry point exists for the
-        hard copy in run() (tau=1.0) and for callers that drive it by hand.  Called with the same
-        (local, target) pair twice in a row -- as run() does for critic 1 and 2 -- the second call of a
-        tau=1.0 copy is idempotent."""
+        """theta_target = tau*theta_local + (1-tau)*theta_target (LL/learner.py:126-137) for the pair it is given:
+        (local_critic_k, target_critic_k) updates critic k's target only, as the reference's per-critic calls do;
+        (None, None) updates both critics' targets at once (run()'s hard copy, tau=1.0).  The step itself already applies
+        the per-step Polyak update; this entry point is for the hard copy and for callers that drive it by hand."""
         tau = self.tau if tau is None else tau
-        self.core.soft_update(float(tau))
+        if local_model is None and target_model is None:
+            self.core.soft_update(float(tau))
+            return
+        pairs = {("q1", "q1_target"): 1, ("q2", "q2_target"): 2}
+        key = (getattr(local_model, "net", None), getattr(target_model, "net", None))
+        if (key not in pairs or getattr(local_model, "_learner", None) is not self
+                or getattr(target_model, "_learner", None) is not self):
+            raise ValueError(f"soft_update takes (local_critic_k, target_critic_k) of this learner or (None, None), got {key}")
+        self.core.soft_update(float(tau), critic=pairs[key])
 
     def wait_until_memoryReady(self):
         while len(self.memory) <= self.start_memory_len:

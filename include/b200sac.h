@@ -227,6 +227,10 @@ int b200sac_read_losses(b200sac_t* h, int32_t n_last, float* out_host, void* str
 /* Polyak update of the target critics outside a step (Learner.soft_update; tau = 1 is
  * the hard copy Learner.run() does before training, learner.py:287-288). */
 int b200sac_soft_update(b200sac_t* h, double tau, void* stream);
+/* The same for one critic pair only: critic = 1 updates q1_target from q1, critic = 2 q2_target from q2, with `tau`
+ * (Learner.soft_update(local_critic_k, target_critic_k, tau), LunarLander_Distributed_SAC/src/learner.py:126-137,236-237).
+ * Every other target, the CARE target state encoder included, is left as it is. */
+int b200sac_soft_update_critic(b200sac_t* h, int32_t critic, double tau, void* stream);
 
 /* Batched policy inference for n <= 2*batch observation rows obs[n][obs_dim] (obs_dim = state_dim + num_tasks), host or
  * device memory: actions[n][act_dim] = k * tanh(mu + std * eps) -- Actor.get_action
