@@ -94,6 +94,13 @@ SYMBOLS = {
     "b200sac_replay_get_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP]),
     "b200sac_replay_get_tree": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int64, _VP]),
     "b200sac_replay_sample_prioritized": (C.c_int, [_VP, C.c_int32] + [_VP] * 5 + [_VP, _VP]),
+    "b200sac_replay_enable_trajectories": (C.c_int, [_VP]),
+    "b200sac_replay_push_traj": (C.c_int, [_VP, C.c_int32, C.c_int64] + [_VP] * 5 + [_VP, _VP]),
+    "b200sac_replay_close_streams": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP]),
+    "b200sac_replay_set_nstep": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
+    "b200sac_replay_get_nstep": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32)]),
+    "b200sac_replay_get_links": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int64, _VP]),
+    "b200sac_replay_fold": (C.c_int, [_VP, C.c_int32, C.c_int64] + [_VP] * 8),
 }
 
 _lib = None

@@ -411,9 +411,10 @@ class SacCore:
     def debug(self, name: str, replica=0) -> torch.Tensor:
         """Per-step intermediates (b200sac_debug_read): y, q1, ..., and the hidden activations "hA.<l>", "hQ.<l>", "hP.<l>",
         "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used.  After a step from a prioritized
-        ring: "isw" (importance weights), "prio" (leaf values written) and "idx" (ring indices, int32)."""
+        ring: "isw" (importance weights), "prio" (leaf values written) and "idx" (ring indices, int32).  After a step from a
+        ring with trajectory links: "disc" (per-row discount), "nstep_m" (hops folded, int32), "idx"; "r" and "d" are folded."""
         cap = self.cfg.batch * max(2 * self.cfg.act_dim, 1)
-        if name == "idx":                       # int32 ring indices (prioritized replay)
+        if name in ("idx", "nstep_m"):          # int32: ring indices (prioritized / linked ring), hops folded (linked ring)
             return self._debug_raw(name, replica, cap).view(torch.int32)
         if name == "psave":
             cap = 2 * self.cfg.batch * self.cfg.act_dim * 8
@@ -434,9 +435,10 @@ class Replay:
     """Replay ring in HBM (where='device') or pinned host DRAM (where='host').
 
     prioritized=dict(alpha=, beta=, eps=) makes a prioritized device ring (sum-tree sampling, importance-weighted critic
-    loss, priorities updated inside every step; see include/b200sac.h)."""
+    loss, priorities updated inside every step; see include/b200sac.h).  trajectories=True keeps trajectory links on the
+    device ring, so that steps can train on n-step returns (set_nstep)."""
 
-    def __init__(self, core: SacCore, capacity: int, where: str = "device", seed: int = 0, prioritized=None):
+    def __init__(self, core: SacCore, capacity: int, where: str = "device", seed: int = 0, prioritized=None, trajectories=False):
         self.core = core
         self.lib = core.lib
         self._h = C.c_void_p(0)
@@ -455,6 +457,13 @@ class Replay:
         else:
             _lib.check(self.lib.b200sac_replay_create(core._h, int(capacity), w, C.c_uint64(seed), C.byref(self._h)))
         self.where = where
+        self.trajectories = bool(trajectories)
+        if self.trajectories:
+            if where != "device":
+                self.close()
+                raise ValueError("trajectory links (n-step returns) need the device ring (where='device')")
+            _lib.check(self.lib.b200sac_replay_enable_trajectories(self._h))
+
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value and self.core._h.value:
             self.lib.b200sac_replay_destroy(self._h)
@@ -466,10 +475,21 @@ class Replay:
         except Exception:
             pass
 
-    def push(self, s, a, r, s2, d, replica=0):
+    def push(self, s, a, r, s2, d, replica=0, stream=None, cut=None):
+        """Append rows.  stream (scalar or one id per row, in [0, 65536)) says which player / environment each row came from,
+        so that a ring with trajectory links can chain consecutive rows of a stream; cut (scalar or per row) marks a
+        time-limit truncation.  stream=None is the plain push (the rows join no trajectory)."""
         ts = [np.ascontiguousarray(np.asarray(t, dtype=np.float32)) for t in (s, a, r, s2, d)]
         n = ts[2].size
-        _lib.check(self.lib.b200sac_replay_push(self._h, replica, n, *[C.c_void_p(t.ctypes.data) for t in ts]))
+        if stream is None:
+            if cut is not None:
+                raise ValueError("cut= needs stream=")
+            _lib.check(self.lib.b200sac_replay_push(self._h, replica, n, *[C.c_void_p(t.ctypes.data) for t in ts]))
+            return
+        sid = np.ascontiguousarray(np.broadcast_to(np.asarray(stream, dtype=np.int32).reshape(-1), (n,)))
+        ct = None if cut is None else np.ascontiguousarray(np.broadcast_to(np.asarray(cut).astype(np.uint8).reshape(-1), (n,)))
+        _lib.check(self.lib.b200sac_replay_push_traj(self._h, replica, n, *[C.c_void_p(t.ctypes.data) for t in ts],
+                                                     C.c_void_p(sid.ctypes.data), C.c_void_p(0 if ct is None else ct.ctypes.data)))
 
     def fill_synthetic(self, n: int, seed: int = 1234):
         _lib.check(self.lib.b200sac_replay_fill_synthetic(self._h, int(n), C.c_uint64(seed), _stream()))
@@ -531,3 +551,39 @@ class Replay:
         _lib.check(self.lib.b200sac_replay_sample_prioritized(self._h, int(replica), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
                                                               _ptr(idx), _ptr(w)))
         return s, a, r, s2, d, idx, w
+
+    # ---- n-step returns (ring with trajectory links) ---------------------------------------------
+    def set_nstep(self, n: int, replica=None):
+        """Horizon n in [1, 16] of one replica (None: all), in stream order: steps enqueued afterwards fold n-step returns."""
+        for r in range(self.core.cfg.replicas) if replica is None else [int(replica)]:
+            _lib.check(self.lib.b200sac_replay_set_nstep(self._h, r, int(n), _stream()))
+
+    def get_nstep(self, replica=0) -> int:
+        n = C.c_int32(0)
+        _lib.check(self.lib.b200sac_replay_get_nstep(self._h, int(replica), C.byref(n)))
+        return n.value
+
+    def close_streams(self, streams, replica=0):
+        """Forget the open tails of these stream ids: their next rows start new trajectories (for recycling ids)."""
+        ids = np.ascontiguousarray(np.asarray(streams, dtype=np.int32).reshape(-1))
+        if ids.size:
+            _lib.check(self.lib.b200sac_replay_close_streams(self._h, int(replica), ids.size, C.c_void_p(ids.ctypes.data)))
+
+    def links(self, task=0, replica=0) -> np.ndarray:
+        """link[slot] of one (replica, task) sub-ring: the sub-ring-local slot of the successor transition, or -1."""
+        out = np.empty(self.capacity // max(self.core.cfg.num_tasks, 1), dtype=np.int32)
+        _lib.check(self.lib.b200sac_replay_get_links(self._h, int(replica), int(task), out.size, C.c_void_p(out.ctypes.data)))
+        return out
+
+    def fold(self, idx, replica=0):
+        """(s, a, R, s2, d, disc, m) of ring slots `idx` as numpy arrays: the device's n-step fold with the replica's current
+        horizon and gamma (the current stream is synchronised first, so a set_hparams enqueued on it has landed)."""
+        torch.cuda.current_stream().synchronize()
+        idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1))
+        c, n = self.core.cfg, idx.size
+        s, a, R = np.empty((n, c.obs_dim), np.float32), np.empty((n, c.act_dim), np.float32), np.empty(n, np.float32)
+        s2, d, disc = np.empty((n, c.obs_dim), np.float32), np.empty(n, np.float32), np.empty(n, np.float32)
+        m = np.empty(n, np.int32)
+        _lib.check(self.lib.b200sac_replay_fold(self._h, int(replica), n, *[C.c_void_p(t.ctypes.data) for t in
+                                                                            (idx, s, a, R, s2, d, disc, m)]))
+        return s, a, R, s2, d, disc, m

@@ -16,6 +16,7 @@
 #include <random>
 #include <string>
 #include <type_traits>
+#include <unordered_map>
 #include <unordered_set>
 #include <vector>
 
@@ -28,6 +29,7 @@
 #include "chain.cuh"
 #include "chain2.cuh"
 #include "per_kernels.cuh"
+#include "nstep_kernels.cuh"
 
 using namespace bsac;
 
@@ -342,6 +344,9 @@ struct b200sac {
   float* per_buf = nullptr;
   cudaStream_t per_fork = nullptr;
   cudaEvent_t ev_per_src = nullptr, ev_per_done = nullptr;
+  // n-step returns (allocated with the first linked ring): [3][R][B] per-row discount of the step (K.disc), hops folded and
+  // ring indices (int32), written by ingest_nstep_kernel
+  float* ns_buf = nullptr;
 };
 
 struct b200sac_replay {
@@ -369,6 +374,20 @@ struct b200sac_replay {
   int* s_idx = nullptr;           // scratch [kPerMaxB]
   float* s_f = nullptr;           // scratch [kPerMaxB]
   float* s_rows = nullptr;        // scratch [B][row_stride]
+  // trajectory links (nstep_kernels.cuh; b200sac_replay_enable_trajectories)
+  bool traj = false;
+  int* d_link = nullptr;          // [R][cap] sub-ring-local slot of the successor, or -1
+  int* d_nstep = nullptr;         // [R] horizon
+  std::vector<int> nstep_host;    // host mirror (b200sac_replay_get_nstep does not synchronise)
+  std::vector<int> link_h, pred_h;   // [R][cap] host mirror of link, and its inverse (sub-ring-local slot of the predecessor)
+  std::vector<std::unordered_map<int, long long>> tail;      // [R] stream id -> ring index of the stream's open tail
+  std::vector<std::unordered_map<long long, int>> tail_at;   // [R] its inverse
+  cudaEvent_t ev_nstep = nullptr; // recorded after the last set_nstep (b200sac_replay_fold waits for it)
+  int* f_at = nullptr;            // scratch [f_cap] x 2: link changes of one push (ring index, value)
+  size_t f_cap = 0;
+  long long* f_idx = nullptr;     // fold scratch [kNstepChunk], with f_rows [kNstepChunk][row_stride], f_disc, f_m
+  float *f_rows = nullptr, *f_disc = nullptr;
+  int* f_m = nullptr;
 };
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
@@ -410,6 +429,7 @@ static int destroy_impl(b200sac* h) {
   cudaFree(h->chain_dbg);
   cudaFree(h->d_cmaps);
   cudaFree(h->per_buf);
+  cudaFree(h->ns_buf);
   if (h->per_fork) cudaStreamDestroy(h->per_fork);
   if (h->ev_per_src) cudaEventDestroy(h->ev_per_src);
   if (h->ev_per_done) cudaEventDestroy(h->ev_per_done);
@@ -1665,14 +1685,17 @@ static cudaError_t per_sample_on(b200sac* h, b200sac_replay* rb, cudaStream_t s)
 // The launch whose rows carry the step's TD target and pre-update critic values (the priority update follows it).
 static bool forms_critic_loss(const Launch& l) { return l.kind == L_CHEADS || (l.kind == L_CHAIN2 && l.chain2.kind == C2_CRITIC); }
 
-// per: prioritized ring of a sampled step -- the critic loss is importance-weighted and the priority update runs after the
-// critic-loss launch (forked off the critical path when allow_fork, joined before the step ends); per_next: the next step's
-// draw follows that update on the same stream (ev_sampled).
+// rb: the device ring of a sampled step.  Prioritized ring -- the critic loss is importance-weighted and the priority update
+// runs after the critic-loss launch (forked off the critical path when allow_fork, joined before the step ends); per_next:
+// the next step's draw follows that update on the same stream (ev_sampled).  Linked ring -- the TD target discounts every
+// row with what the gather folded for it.
 static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* evs = nullptr, bool allow_fork = false,
-                    b200sac_replay* per = nullptr, bool per_next = false) {
+                    b200sac_replay* rb = nullptr, bool per_next = false) {
   bool fork_pending = false, per_pending = false;
+  b200sac_replay* per = rb && rb->per ? rb : nullptr;
   StepConst K = h->K;
   if (per) K.isw = h->per_buf;
+  if (rb && rb->traj) K.disc = h->ns_buf;
   for (size_t i = 0; i < h->plan.size(); ++i) {
     Launch& l = h->plan[i];
     if (evs) CU(cudaEventRecord(evs[i], st));
@@ -2342,6 +2365,12 @@ extern "C" int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t
 // step's gather has consumed the index buffer and bumped the step counter, draw the NEXT step's indices on the fork stream
 // -- that kernel then overlaps the whole step instead of heading its critical path.
 enum { SAMPLE_INLINE = 0, SAMPLE_DONE = 1 };
+static NstepRing nstep_ring(const b200sac_replay* rb) {
+  NstepRing N;
+  N.link = rb->d_link; N.nstep = rb->d_nstep; N.cap = rb->cap; N.cap_per_task = (int)rb->cap_per_task;
+  return N;
+}
+
 static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* const* p, b200sac_replay* rb,
                         cudaEvent_t* evs = nullptr, int sample_mode = SAMPLE_INLINE, bool fork_next = false) {
   if (evs) CU(cudaEventRecord(evs[0], st));
@@ -2375,8 +2404,12 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     };
     if (sample_mode == SAMPLE_INLINE) sample_on(st);
     else CU(cudaStreamWaitEvent(st, h->ev_sampled, 0));
-    launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
-             (const int*)rb->d_idx, (long long)B);
+    if (rb->traj)                               // linked ring: the same gather with the n-step fold in front of the scatter
+      launch_k(ingest_nstep_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
+               (const int*)rb->d_idx, (long long)B, nstep_ring(rb), h->ns_buf);
+    else
+      launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
+               (const int*)rb->d_idx, (long long)B);
     if (fork_next && !rb->per) {                // (prioritized: the next draw follows this step's priority update)
       CU(cudaEventRecord(h->ev_ingested, st));
       CU(cudaStreamWaitEvent(h->fork, h->ev_ingested, 0));
@@ -2386,7 +2419,7 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
   }
   CU(cudaGetLastError());
   const bool per = variant == 2 && rb->per;
-  return run_plan(h, st, use_eps, evs ? evs + 1 : nullptr, evs == nullptr && !h->stamping, per ? rb : nullptr, per && fork_next);
+  return run_plan(h, st, use_eps, evs ? evs + 1 : nullptr, evs == nullptr && !h->stamping, variant == 2 ? rb : nullptr, per && fork_next);
 }
 
 // nsteps > 1 (device-ring sampling only): that many consecutive gradient steps captured in ONE graph, so a pipelined
@@ -2946,8 +2979,16 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "d_head") { src = h->dout_dbg.p + replica * h->dout_dbg.rs; n = (int64_t)B * 2 * A; }
   else if (nm == "psave") { src = h->psave.p + replica * h->psave.rs; n = (int64_t)2 * B * A * kSaveW; }   // [2B][A][8]: std, diff, tanh, act, jac, EPS, mask, logp_j
   else if (nm == "isw" || nm == "prio" || nm == "idx") {   // prioritized replay: [B] weights, leaf values, ring indices (int32 bits)
-    if (!h->per_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a prioritized replay ring", name);
-    src = h->per_buf + ((nm == "isw" ? 0 : nm == "prio" ? 1 : 2) * (size_t)h->R + replica) * B; n = B;
+    if (nm == "idx" && !h->per_buf && h->ns_buf) {          // a uniform linked ring: the indices its gather folded from
+      src = h->ns_buf + ((size_t)2 * h->R + replica) * B; n = B;
+    } else {
+      if (!h->per_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a prioritized replay ring", name);
+      src = h->per_buf + ((nm == "isw" ? 0 : nm == "prio" ? 1 : 2) * (size_t)h->R + replica) * B; n = B;
+    }
+  }
+  else if (nm == "disc" || nm == "nstep_m") {               // n-step returns: [B] per-row discount, hops folded (int32 bits)
+    if (!h->ns_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a replay ring with trajectory links", name);
+    src = h->ns_buf + ((nm == "disc" ? 0 : 1) * (size_t)h->R + replica) * B; n = B;
   }
   else if (nm == "chain_dbg") {
     if (!h->chain_dbg) return fail(B200SAC_ERR_INVALID, "chain_dbg needs B200SAC_CHAIN_DBG=1 at create time");
@@ -3037,17 +3078,74 @@ extern "C" int b200sac_replay_destroy(b200sac_replay_t* rb) {
   if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
   cudaFree(rb->tr.tree); cudaFree(rb->tr.maxp); cudaFree(rb->d_beta);
   cudaFree(rb->s_lidx); cudaFree(rb->s_idx); cudaFree(rb->s_f); cudaFree(rb->s_rows);
+  cudaFree(rb->d_link); cudaFree(rb->d_nstep); cudaFree(rb->f_at); cudaFree(rb->f_idx); cudaFree(rb->f_rows); cudaFree(rb->f_disc);
+  cudaFree(rb->f_m);
+  if (rb->ev_nstep) cudaEventDestroy(rb->ev_nstep);
   if (rb->st) cudaStreamDestroy(rb->st);
   delete rb;
   return 0;
 }
 
-extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a,
-                                   const float* r, const float* s2, const float* d) {
+// Trajectory links of one push (linked ring; under rb->mu).  Row i of the push went to sub-ring task[i], slot slot[i]
+// (slot -1: a push larger than the sub-ring dropped it).  Rows are replayed in push order, as if appended one by one:
+//   overwrite rule   the new occupant of slot j cuts the link that pointed to j (only if link[pred[j]] is still j), clears
+//                    pred of the slot j pointed to (a stale pred must never cut the new occupant's link later), and a
+//                    stream whose tail was j forgets it;
+//   stream rule      row x becomes the successor of its stream's tail t iff t exists (d_t = 0, cut_t = 0: a closed tail is
+//                    not kept) and both lie in the same task sub-ring.
+// The host mirrors are updated here; `touched` collects the ring indices whose link changed.
+static void push_links(b200sac_replay* rb, int replica, int64_t n, const std::vector<int>& task, const std::vector<long long>& slot,
+                       const float* d, const int32_t* stream, const uint8_t* cut, std::vector<int>& touched) {
+  const long long cpt = rb->cap_per_task;
+  int* link = rb->link_h.data() + (size_t)replica * rb->cap;
+  int* pred = rb->pred_h.data() + (size_t)replica * rb->cap;
+  auto& tail = rb->tail[(size_t)replica];
+  auto& tail_at = rb->tail_at[(size_t)replica];
+  for (int64_t i = 0; i < n; ++i) {
+    const int sid = stream ? stream[i] : -1;
+    if (slot[(size_t)i] < 0) {                     // written and overwritten inside this push: its stream loses its tail
+      if (sid >= 0) {
+        auto it = tail.find(sid);
+        if (it != tail.end()) { tail_at.erase(it->second); tail.erase(it); }
+      }
+      continue;
+    }
+    const long long tb = (long long)task[(size_t)i] * cpt, j = slot[(size_t)i], g = tb + j;
+    const int p = pred[g], nx = link[g];
+    if (p >= 0 && link[tb + p] == (int)j) { link[tb + p] = -1; touched.push_back((int)(tb + p)); }
+    if (nx >= 0 && pred[tb + nx] == (int)j) pred[tb + nx] = -1;
+    auto at = tail_at.find(g);
+    if (at != tail_at.end()) { tail.erase(at->second); tail_at.erase(at); }
+    link[g] = -1; pred[g] = -1;
+    touched.push_back((int)g);
+    if (sid < 0) continue;
+    auto it = tail.find(sid);
+    if (it != tail.end()) {
+      const long long t = it->second;
+      if (t / cpt == task[(size_t)i]) { link[t] = (int)j; pred[g] = (int)(t - tb); touched.push_back((int)t); }
+      tail_at.erase(t);
+      tail.erase(it);
+    }
+    if (d[i] == 0.f && !(cut && cut[i])) { tail[sid] = g; tail_at[g] = sid; }
+  }
+  std::sort(touched.begin(), touched.end());
+  touched.erase(std::unique(touched.begin(), touched.end()), touched.end());
+}
+
+static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a, const float* r,
+                     const float* s2, const float* d, const int32_t* stream, const uint8_t* cut) {
   if (!rb || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
   b200sac* h = rb->h;
   if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica out of range");
+  if (n < 0) return fail(B200SAC_ERR_INVALID, "n < 0");
+  if (stream)
+    for (int64_t i = 0; i < n; ++i)
+      if (stream[i] < 0 || stream[i] >= 65536)
+        return fail(B200SAC_ERR_INVALID, "row %lld: stream id %d outside [0, 65536)", (long long)i, stream[i]);
   CU(cudaSetDevice(h->device));
+  std::vector<int> row_task;
+  std::vector<long long> row_slot;                 // first the row's position in its task bucket, then its slot
+  if (rb->traj) { row_task.resize((size_t)n); row_slot.resize((size_t)n); }
   const int obs = h->K.obs, A = h->K.act, T = h->cfg.num_tasks, rs = h->row_stride;
   // pack the rows, bucketed by task, then copy each bucket as at most two contiguous runs (ring wrap)
   std::vector<std::vector<float>> bucket((size_t)rb->Teff);
@@ -3064,9 +3162,18 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
       for (int q = 1; q < T; ++q)
         if (row[obs - T + q] > best) { best = row[obs - T + q]; task = q; }
     }
+    if (rb->traj) { row_task[(size_t)i] = task; row_slot[(size_t)i] = (long long)(bucket[(size_t)task].size() / (size_t)rs); }
     bucket[(size_t)task].insert(bucket[(size_t)task].end(), row.begin(), row.end());
   }
   std::lock_guard<std::mutex> lk(rb->mu);
+  if (rb->traj) {                                  // bucket position -> slot, with the heads as they are before the copy
+    for (int64_t i = 0; i < n; ++i) {
+      const int task = row_task[(size_t)i];
+      const long long cnt = (long long)(bucket[(size_t)task].size() / (size_t)rs);
+      const long long skip = std::max(0LL, cnt - rb->cap_per_task), k = row_slot[(size_t)i];
+      row_slot[(size_t)i] = k < skip ? -1 : (rb->head[(size_t)replica * rb->Teff + task] + (k - skip)) % rb->cap_per_task;
+    }
+  }
   // Device ring: the gathers of every step enqueued so far must have read their rows before a wrapped ring overwrites
   // them (a torn transition otherwise); step_sampled enqueues under the same mutex, so none can slip in while we copy.
   if (rb->where == 0 && rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
@@ -3094,6 +3201,25 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
     }
   }
   if (rb->per) CU(cudaGetLastError());
+  std::vector<int> touched, vals;
+  if (rb->traj) {                                  // the link changes travel with the rows
+    push_links(rb, replica, n, row_task, row_slot, d, stream, cut, touched);
+    const size_t m = touched.size();
+    if (m > rb->f_cap) {
+      cudaFree(rb->f_at); rb->f_at = nullptr; rb->f_cap = 0;
+      if (cudaMalloc(&rb->f_at, 2 * m * sizeof(int)) != cudaSuccess) return fail(B200SAC_ERR_NOMEM, "link scratch allocation failed");
+      rb->f_cap = m;
+    }
+    vals.resize(m);
+    for (size_t i = 0; i < m; ++i) vals[i] = rb->link_h[(size_t)replica * rb->cap + touched[i]];
+    if (m > 0) {
+      CU(cudaMemcpyAsync(rb->f_at, touched.data(), m * sizeof(int), cudaMemcpyHostToDevice, rb->st));
+      CU(cudaMemcpyAsync(rb->f_at + rb->f_cap, vals.data(), m * sizeof(int), cudaMemcpyHostToDevice, rb->st));
+      nstep_scatter_links_kernel<<<(unsigned)((m + 255) / 256), 256, 0, rb->st>>>(rb->d_link + (size_t)replica * rb->cap, rb->f_at,
+                                                                                 rb->f_at + rb->f_cap, (int)m);
+      CU(cudaGetLastError());
+    }
+  }
   // A copy from pageable memory may return before its DMA has landed, and a step enqueued on a non-blocking stream is not
   // ordered after the legacy stream: the rows and the fill go on the ring's own stream, which is drained before the mutex
   // is released, so every step enqueued after this call gathers the new rows.
@@ -3103,6 +3229,19 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
     CU(cudaStreamSynchronize(rb->st));
   }
   return 0;
+}
+
+extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a,
+                                   const float* r, const float* s2, const float* d) {
+  return push_impl(rb, replica, n, s, a, r, s2, d, nullptr, nullptr);
+}
+
+extern "C" int b200sac_replay_push_traj(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a,
+                                        const float* r, const float* s2, const float* d, const int32_t* stream,
+                                        const uint8_t* cut) {
+  if (!rb || !stream) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!rb->traj) return fail(B200SAC_ERR_STATE, "push_traj needs a ring with trajectory links (b200sac_replay_enable_trajectories)");
+  return push_impl(rb, replica, n, s, a, r, s2, d, stream, cut);
 }
 
 extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, uint64_t seed, void* stream) {
@@ -3138,6 +3277,19 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   for (auto& hd : rb->head) hd = per % rb->cap_per_task;
   if (rb->where == 0)
     CU(cudaMemcpyAsync(rb->d_fill, rb->fill.data(), sizeof(long long) * rb->fill.size(), cudaMemcpyHostToDevice, st));
+  if (rb->traj) {                                  // slot i -> i + 1 unless d_i != 0 or i is the last filled slot; no open streams
+    if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
+    nstep_fill_links_kernel<<<dim3(256, h->R), 256, 0, st>>>(rb->d_link, rb->cap, (int)rb->cap_per_task, rb->rows, rb->rs_rows,
+                                                            h->row_stride, 2 * h->K.obs + h->K.act + 1, per);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(rb->link_h.data(), rb->d_link, rb->link_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::fill(rb->pred_h.begin(), rb->pred_h.end(), -1);
+    for (size_t g = 0; g < rb->link_h.size(); ++g)
+      if (rb->link_h[g] >= 0) rb->pred_h[g + 1] = (int)(g % (size_t)rb->cap_per_task);
+    for (auto& t : rb->tail) t.clear();
+    for (auto& t : rb->tail_at) t.clear();
+  }
   CU(cudaStreamSynchronize(st));
   return 0;
 }
@@ -3433,6 +3585,147 @@ extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t r
     d[i] = src[2 * obs + A + 1];
     if (idx_out) idx_out[i] = ix[(size_t)i];
     if (w_out) w_out[i] = w[(size_t)i];
+  }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// n-step returns (nstep_kernels.cuh): trajectory links on a device ring, folded by the step's gather
+// ------------------------------------------------------------------------------------------
+static int traj_check(b200sac_replay* rb, int32_t replica) {
+  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
+  if (!rb->traj) return fail(B200SAC_ERR_STATE, "the ring has no trajectory links (b200sac_replay_enable_trajectories)");
+  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  return 0;
+}
+
+extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
+  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
+  if (rb->where != 0) return fail(B200SAC_ERR_INVALID, "trajectory links need the device ring");
+  b200sac* h = rb->h;
+  std::lock_guard<std::mutex> lk(rb->mu);
+  if (rb->traj) return fail(B200SAC_ERR_STATE, "the ring already has trajectory links");
+  for (auto f : rb->fill)
+    if (f != 0) return fail(B200SAC_ERR_STATE, "trajectory links can only be enabled on an empty ring");
+  CU(cudaSetDevice(h->device));
+  const size_t nl = (size_t)h->R * rb->cap, rs = (size_t)h->row_stride;
+  std::vector<int> ones((size_t)h->R, 1);
+  int* link = nullptr; int* nstep = nullptr; long long* f_idx = nullptr; float* f_rows = nullptr; float* f_disc = nullptr; int* f_m = nullptr;
+  float* ns_buf = h->ns_buf;
+  cudaEvent_t ev = nullptr;
+  const size_t nb = (size_t)3 * h->R * h->cfg.batch;
+  const bool ok =
+      cudaMalloc(&link, nl * sizeof(int)) == cudaSuccess && cudaMemset(link, 0xff, nl * sizeof(int)) == cudaSuccess &&
+      cudaMalloc(&nstep, (size_t)h->R * sizeof(int)) == cudaSuccess &&
+      cudaMemcpy(nstep, ones.data(), (size_t)h->R * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
+      cudaMalloc(&f_idx, kNstepChunk * sizeof(long long)) == cudaSuccess && cudaMalloc(&f_rows, kNstepChunk * rs * sizeof(float)) == cudaSuccess &&
+      cudaMalloc(&f_disc, kNstepChunk * sizeof(float)) == cudaSuccess && cudaMalloc(&f_m, kNstepChunk * sizeof(int)) == cudaSuccess &&
+      cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess &&
+      (ns_buf || (cudaMalloc(&ns_buf, nb * sizeof(float)) == cudaSuccess && cudaMemset(ns_buf, 0, nb * sizeof(float)) == cudaSuccess));
+  if (!ok) {
+    cudaGetLastError();
+    cudaFree(link); cudaFree(nstep); cudaFree(f_idx); cudaFree(f_rows); cudaFree(f_disc); cudaFree(f_m);
+    if (ns_buf != h->ns_buf) cudaFree(ns_buf);
+    if (ev) cudaEventDestroy(ev);
+    return fail(B200SAC_ERR_NOMEM, "trajectory link allocation failed");
+  }
+  // graphs captured for this ring before it was linked hold the unlinked gather
+  for (auto it = h->graphs.begin(); it != h->graphs.end();) {
+    if (it->first.p[8] == rb) { cudaGraphExecDestroy(it->second); it = h->graphs.erase(it); }
+    else ++it;
+  }
+  h->ns_buf = ns_buf;
+  rb->d_link = link; rb->d_nstep = nstep; rb->f_idx = f_idx; rb->f_rows = f_rows; rb->f_disc = f_disc; rb->f_m = f_m; rb->ev_nstep = ev;
+  rb->nstep_host.assign((size_t)h->R, 1);
+  rb->link_h.assign(nl, -1);
+  rb->pred_h.assign(nl, -1);
+  rb->tail.assign((size_t)h->R, {});
+  rb->tail_at.assign((size_t)h->R, {});
+  rb->traj = true;
+  return 0;
+}
+
+extern "C" int b200sac_replay_close_streams(b200sac_replay_t* rb, int32_t replica, int64_t n, const int32_t* stream) {
+  if (int rc = traj_check(rb, replica)) return rc;
+  if (n < 0 || (n > 0 && !stream)) return fail(B200SAC_ERR_INVALID, "bad argument");
+  for (int64_t i = 0; i < n; ++i)
+    if (stream[i] < 0 || stream[i] >= 65536) return fail(B200SAC_ERR_INVALID, "stream id %d outside [0, 65536)", stream[i]);
+  std::lock_guard<std::mutex> lk(rb->mu);
+  for (int64_t i = 0; i < n; ++i) {
+    auto it = rb->tail[(size_t)replica].find(stream[i]);
+    if (it != rb->tail[(size_t)replica].end()) { rb->tail_at[(size_t)replica].erase(it->second); rb->tail[(size_t)replica].erase(it); }
+  }
+  return 0;
+}
+
+extern "C" int b200sac_replay_set_nstep(b200sac_replay_t* rb, int32_t replica, int32_t n, void* stream) {
+  if (int rc = traj_check(rb, replica)) return rc;
+  if (n < 1 || n > kNstepMax) return fail(B200SAC_ERR_INVALID, "n-step horizon must be in [1, %d] (got %d)", kNstepMax, n);
+  CU(cudaSetDevice(rb->h->device));
+  StreamBridge sb(rb->h, stream);
+  if (int rc = sb.begin()) return rc;
+  nstep_set_kernel<<<1, 1, 0, sb.run>>>(rb->d_nstep, replica, n);
+  CU(cudaGetLastError());
+  CU(cudaEventRecord(rb->ev_nstep, sb.run));
+  if (int rc = sb.end()) return rc;
+  rb->nstep_host[(size_t)replica] = n;
+  return 0;
+}
+
+extern "C" int b200sac_replay_get_nstep(b200sac_replay_t* rb, int32_t replica, int32_t* n) {
+  if (int rc = traj_check(rb, replica)) return rc;
+  if (!n) return fail(B200SAC_ERR_INVALID, "null argument");
+  *n = rb->nstep_host[(size_t)replica];
+  return 0;
+}
+
+extern "C" int b200sac_replay_get_links(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, int32_t* out) {
+  if (int rc = traj_check(rb, replica)) return rc;
+  if (task < 0 || task >= rb->Teff) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
+  if (!out || n != rb->cap_per_task) return fail(B200SAC_ERR_INVALID, "a sub-ring has %lld slots (got n = %lld)", rb->cap_per_task, (long long)n);
+  CU(cudaSetDevice(rb->h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  CU(cudaMemcpyAsync(out, rb->d_link + (size_t)replica * rb->cap + (size_t)task * rb->cap_per_task, (size_t)n * sizeof(int),
+                     cudaMemcpyDeviceToHost, rb->st));
+  CU(cudaStreamSynchronize(rb->st));
+  return 0;
+}
+
+extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_t n_idx, const int64_t* idx, float* s, float* a,
+                                   float* R, float* s2, float* d, float* disc, int32_t* m) {
+  if (int rc = traj_check(rb, replica)) return rc;
+  if (n_idx < 0 || (n_idx > 0 && (!idx || !s || !a || !R || !s2 || !d || !disc || !m))) return fail(B200SAC_ERR_INVALID, "bad argument");
+  b200sac* h = rb->h;
+  const int obs = h->K.obs, A = h->K.act, rs = h->row_stride;
+  CU(cudaSetDevice(h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  for (int64_t i = 0; i < n_idx; ++i) {
+    const long long k = idx[i];
+    if (k < 0 || k >= rb->cap) return fail(B200SAC_ERR_INVALID, "index %lld outside the ring [0, %lld)", k, rb->cap);
+    if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
+      return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
+  }
+  CU(cudaStreamWaitEvent(rb->st, rb->ev_nstep, 0));
+  std::vector<float> rows((size_t)kNstepChunk * rs);
+  for (int64_t i0 = 0; i0 < n_idx; i0 += kNstepChunk) {
+    const int c = (int)std::min<int64_t>(kNstepChunk, n_idx - i0);
+    CU(cudaMemcpyAsync(rb->f_idx, idx + i0, c * sizeof(long long), cudaMemcpyHostToDevice, rb->st));
+    nstep_fold_kernel<<<(c + 7) / 8, 256, 0, rb->st>>>(rb->rows + (size_t)replica * rb->rs_rows, rs, obs, A,
+                                                       rb->d_link + (size_t)replica * rb->cap, (int)rb->cap_per_task, rb->d_nstep, h->hp,
+                                                       replica, rb->f_idx, c, rb->f_rows, rb->f_disc, rb->f_m);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(rows.data(), rb->f_rows, (size_t)c * rs * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+    CU(cudaMemcpyAsync(disc + i0, rb->f_disc, c * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
+    CU(cudaMemcpyAsync(m + i0, rb->f_m, c * sizeof(int), cudaMemcpyDeviceToHost, rb->st));
+    CU(cudaStreamSynchronize(rb->st));
+    for (int i = 0; i < c; ++i) {
+      const float* src = rows.data() + (size_t)i * rs;
+      memcpy(s + (size_t)(i0 + i) * obs, src, obs * sizeof(float));
+      memcpy(a + (size_t)(i0 + i) * A, src + obs, A * sizeof(float));
+      R[i0 + i] = src[obs + A];
+      memcpy(s2 + (size_t)(i0 + i) * obs, src + obs + A + 1, obs * sizeof(float));
+      d[i0 + i] = src[2 * obs + A + 1];
+    }
   }
   return 0;
 }

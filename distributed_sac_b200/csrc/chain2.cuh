@@ -126,7 +126,7 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     t_row = (R.tid + rep * R.rsR)[row];
     if (A.kind == C2_CRITIC) {
       r_row = (R.r + rep * R.rsR)[row]; d_row = (R.d + rep * R.rsR)[row];
-      gamma = K.hp[rep].gamma; reward_scale = K.hp[rep].reward_scale;
+      gamma = K.disc ? K.disc[(long long)rep * B + row] : K.hp[rep].gamma; reward_scale = K.hp[rep].reward_scale;
       lp_row = (R.logp + rep * R.rsLogp)[row];
       const float* Q = R.q + rep * 2 * R.rsY;
       q1_row = Q[row]; q2_row = Q[B + row];

@@ -54,7 +54,9 @@ struct StepConst {
   // Keeps sizeof(StepConst) at 136 bytes, so that the kernel arguments behind it keep their parameter-space offsets.
   // ptxas schedules a kernel differently when those move, even one that never reads the table: 32 bytes less cost the
   // policy head ~1.2 us per step of the 400-wide learners on an H100.
-  unsigned long long reserved[2];
+  const float* disc;              // n-step returns: [R][B] per-row discount gamma^m of the step's rows (nstep_kernels.cuh); null =
+                                  // every row discounts with the replica's gamma
+  unsigned long long reserved[1];
 };
 static_assert(sizeof(StepConst) == 136, "StepConst size moves the offsets of the kernel arguments behind it");
 
@@ -491,7 +493,7 @@ __global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   // to r and d across the dot products would take two more registers, which this 32-register kernel pays for by
   // serialising the loads of a head
   const float t1 = K.hp[rep].reward_scale * r;
-  const float t2 = K.hp[rep].gamma * (1.f - d);
+  const float t2 = (K.disc ? K.disc[(long long)rep * B + row] : K.hp[rep].gamma) * (1.f - d);
   const float lp = (P.logp + rep * P.rsLogp)[row];
   const float b_t1 = (P.bt[0] + po)[0], b_t2 = (P.bt[1] + po)[0], b_q1 = (P.bq[0] + po)[0], b_q2 = (P.bq[1] + po)[0];
   const float p_t1 = warp_dot_partial(hT, P.Wt[0] + po, H, lane), p_t2 = warp_dot_partial(hT + P.rsHnet, P.Wt[1] + po, H, lane);

@@ -83,10 +83,16 @@ class _BaseLearner:
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
-                     replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1):
+                     replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
+                     n_step=1):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
+        if not 1 <= int(n_step) <= 16:
+            raise ValueError(f"n_step must be in [1, 16] (got {n_step})")
+        if int(n_step) > 1 and replay_where != "device":
+            raise ValueError("n-step returns need replay_where='device' (the trajectory links live beside the device ring)")
+        self.n_step = int(n_step)
         self.cfg = cfg_read(cfg_path)
         self.precision = precision
         self.write_mode = write_mode
@@ -121,6 +127,12 @@ class _BaseLearner:
         if self.prioritized is None:
             raise ValueError("this learner was built without prioritized=")
         self.memory.ring.set_beta(beta)
+
+    def set_n_step(self, n: int):
+        """Horizon of the n-step return, effective from the next update()."""
+        if self.n_step == 1:
+            raise ValueError("this learner was built without n_step= (its ring keeps no trajectory links)")
+        self.memory.ring.set_nstep(n)
 
     def _core_config(self):
         c = self.cfg
@@ -410,11 +422,11 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
-                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1):
+                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
 
     def _set_dims(self):
         c = self.cfg
@@ -428,7 +440,7 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def _make_memory(self, where):
         return ReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, server=self.server, core=self.core,
-                            where=where, prioritized=self.prioritized)
+                            where=where, prioritized=self.prioritized, n_step=self.n_step)
 
 
 class VSACLearner(_TwoCriticMixin, _BaseLearner):
@@ -438,9 +450,9 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1):
+                 target_update_interval=1, n_step=1):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
 
     def _set_dims(self):
         c = self.cfg
@@ -454,7 +466,7 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def _make_memory(self, where):
         return ReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, server=self.server, core=self.core,
-                            where=where, prioritized=self.prioritized)
+                            where=where, prioritized=self.prioritized, n_step=self.n_step)
 
 
 class MTSACLearner(_BaseLearner):
@@ -466,10 +478,10 @@ class MTSACLearner(_BaseLearner):
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
-                 actor_update_interval=1, target_update_interval=1):
+                 actor_update_interval=1, target_update_interval=1, n_step=1):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
 
     def _set_dims(self):
         c = self.cfg
@@ -488,7 +500,7 @@ class MTSACLearner(_BaseLearner):
 
     def _make_memory(self, where):
         return MTReplayBuffer(self.buffer_size, self.batch_size, 0, self.device, self.num_tasks, server=self.server,
-                              core=self.core, where=where, prioritized=self.prioritized)
+                              core=self.core, where=where, prioritized=self.prioritized, n_step=self.n_step)
 
     def _critic_checkpoint_entries(self, named):
         loc = {**self._module_state_dict("q1", named=named), **self._module_state_dict("q2", named=named)}

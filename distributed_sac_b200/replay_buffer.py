@@ -18,10 +18,12 @@ import numpy as np
 import torch
 
 from .core import Replay
+from .stitch import Stitcher
 
 
 class ReplayBuffer(threading.Thread):
-    def __init__(self, buffer_size, batch_size, seed, device, server=None, *, core=None, where="host", prioritized=None):
+    def __init__(self, buffer_size, batch_size, seed, device, server=None, *, core=None, where="host", prioritized=None,
+                 n_step=1):
         super().__init__()
         self.daemon = True
         if core is None:
@@ -34,7 +36,14 @@ class ReplayBuffer(threading.Thread):
         self.batch_size = int(batch_size)
         self.device = torch.device(device)
         self.core = core
-        self.ring = Replay(core, int(buffer_size), where=where, seed=int(seed), prioritized=prioritized)
+        # n_step > 1: the ring keeps trajectory links and the steps train on n-step returns.  The players push single
+        # transitions, interleaved, so add_many stitches every drain back into trajectories (stitch.Stitcher)
+        self.n_step = int(n_step)
+        self.ring = Replay(core, int(buffer_size), where=where, seed=int(seed), prioritized=prioritized,
+                           trajectories=self.n_step > 1)
+        self.stitcher = Stitcher() if self.n_step > 1 else None
+        if self.n_step > 1:
+            self.ring.set_nstep(self.n_step)
         self._stop_evt = threading.Event()
 
     # ---- ingestion (reference: run(), replay_buffer.py:43-61) -------------------------------
@@ -46,8 +55,11 @@ class ReplayBuffer(threading.Thread):
         n = len(rewards)
         f = lambda x, w: np.asarray(x, dtype=np.float32).reshape(n, w)
         c = self.core.cfg
-        self.ring.push(f(states, c.obs_dim), f(actions, c.act_dim), f(rewards, 1), f(next_states, c.obs_dim),
-                       f(np.asarray(dones).astype(np.uint8), 1))
+        s, s2, d = f(states, c.obs_dim), f(next_states, c.obs_dim), f(np.asarray(dones).astype(np.uint8), 1)
+        stream = None if self.stitcher is None else self.stitcher.assign(s, s2, d)
+        self.ring.push(s, f(actions, c.act_dim), f(rewards, 1), s2, d, stream=stream)
+        if self.stitcher is not None:
+            self.ring.close_streams(self.stitcher.take_abandoned())
 
     def drain_once(self):
         pipe = self.server.pipeline()
@@ -93,10 +105,11 @@ class MTReplayBuffer(ReplayBuffer):
     B/T samples from each, then one shuffle (MS/replay_buffers.py:67-100)."""
 
     def __init__(self, buffer_size, batch_size, seed, device, num_tasks, server=None, *, core=None, where="host",
-                 prioritized=None):
+                 prioritized=None, n_step=1):
         if core is not None and core.cfg.num_tasks != int(num_tasks):
             raise ValueError("num_tasks must match the learner's")
-        super().__init__(buffer_size, batch_size, seed, device, server, core=core, where=where, prioritized=prioritized)
+        super().__init__(buffer_size, batch_size, seed, device, server, core=core, where=where, prioritized=prioritized,
+                         n_step=n_step)
         self.num_tasks = int(num_tasks)
 
     def _unpack(self, data):

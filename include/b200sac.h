@@ -268,7 +268,8 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT),
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
  * importance weights of its critic loss), "prio" [B] (the leaf values p it wrote) and "idx" [B] (its ring indices, int32
- * bit patterns). */
+ * bit patterns).  After a step from a linked ring (n-step returns): "disc" [B] (the per-row discount of its TD target),
+ * "nstep_m" [B] (hops folded, int32 bit patterns), "idx" as above, and "r" / "d" hold the folded values. */
 int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replica, float* out_host, int64_t cap_floats,
                        int64_t* n_floats, void* stream);
 
@@ -349,6 +350,51 @@ int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, int32_t task,
  * of the step counter; rows, ring indices (nullable) and importance weights (nullable) to HOST arrays. */
 int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
                                       float* d, int64_t* idx_out, float* w_out);
+
+/* ---- n-step returns (device ring only) --------------------------------------------------
+ * A linked ring records, next to its 1-step transitions, which slot follows which: link[replica][slot] (int32) is the
+ * sub-ring-local slot of the transition that followed this one in its trajectory, or -1.  The n-step return is folded at
+ * sample time, in the gather of the step's graph, so the horizon n and gamma stay per replica and settable between steps.
+ * Fold of a sampled slot i with n = the replica's horizon and gamma = its b200sac_hparams.gamma (fp32, no fused multiply-add):
+ *     j = i;  R = r_j;  g = gamma;  m = 1
+ *     while d_j == 0 and m < n and link[j] >= 0:   j = link[j];  R = R + g * r_j;  g = g * gamma;  m = m + 1
+ * The step trains on the row (s_i, a_i, R, s'_j, d_j) with the TD target y = rs R + g (1 - d_j)(min(Qt1, Qt2) - alpha logpi'):
+ * the horizon is shorter at a terminal, a time-limit cut, a trajectory's current tail (successor not pushed yet) or an
+ * overwritten successor; with m = 1 the row and the target are the unlinked ring's, bit for bit.  On a prioritized ring the
+ * priorities become n-step TD errors by themselves.  The intermediate rows' actions are used uncorrected, as in Ape-X.
+ * Links are made by b200sac_replay_push_traj: every row carries a stream id (one per player / environment); the library
+ * keeps the tail of every (replica, stream), and row x becomes the successor of its stream's tail t iff t exists, d_t == 0,
+ * cut_t == 0 and both lie in the same task sub-ring.  Overwrite rule: when a push overwrites slot j, the link that pointed
+ * to j is reset to -1, and a stream whose tail was j forgets it.  Invariant, at every point in stream order:
+ * link[i] = j >= 0 implies that slot j currently holds the transition that followed slot i's.
+ * b200sac_step_sampled, b200sac_update and b200sac_prepare accept a linked ring (uniform or prioritized); the launch count
+ * of a step does not change.  Links are not part of a checkpoint. */
+/* Valid once, on an empty device ring: B200SAC_ERR_INVALID for a pinned-host ring, B200SAC_ERR_STATE for a ring that holds
+ * rows or is linked already; nothing changes then.  4 bytes per slot; every replica's horizon starts at 1. */
+int b200sac_replay_enable_trajectories(b200sac_replay_t* rb);
+/* b200sac_replay_push (same order, bucketing by task, wrap, "only the newest rows survive", max-p leaf on a prioritized ring)
+ * plus, per row, a stream id in [0, 65536) and a nullable cut flag (time-limit truncation: the episode ended but d = 0, so
+ * the row bootstraps from its own s').  The link changes land with the rows, before the call returns.  Plain
+ * b200sac_replay_push stays legal on a linked ring: its rows get link = -1, obey the overwrite rule and join no stream.
+ * b200sac_replay_fill_synthetic on a linked ring links slot i -> i + 1 of a sub-ring unless d_i != 0 or i is the last
+ * filled slot. */
+int b200sac_replay_push_traj(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a, const float* r,
+                             const float* s2, const float* d, const int32_t* stream, const uint8_t* cut);
+/* Forget the open tails of n streams of one replica (host bookkeeping only, no link changes): the next row of each starts a
+ * new trajectory.  For callers that recycle stream ids of trajectories that ended without a terminal or cut row. */
+int b200sac_replay_close_streams(b200sac_replay_t* rb, int32_t replica, int64_t n, const int32_t* stream);
+/* Horizon of one replica, n in [1, 16], in stream order on `stream` like b200sac_replay_set_beta: steps enqueued afterwards
+ * use it, including launches of graphs b200sac_prepare instantiated.  Get: the value last set (host mirror). */
+int b200sac_replay_set_nstep(b200sac_replay_t* rb, int32_t replica, int32_t n, void* stream);
+int b200sac_replay_get_nstep(b200sac_replay_t* rb, int32_t replica, int32_t* n);
+/* The link table of one (replica, task) sub-ring, n = its slot count.  Synchronous. */
+int b200sac_replay_get_links(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, int32_t* out);
+/* Reference-shaped sample() of a linked ring: the device fold of n_idx caller-given filled ring slots with the replica's
+ * current horizon and gamma, to HOST arrays (s, a, R, s2, d as in b200sac_replay_sample; disc[n_idx] = g; m[n_idx] = hops).
+ * Synchronous; ordered after every b200sac_replay_set_nstep.  A b200sac_set_hparams still in flight on another stream is
+ * not waited for. */
+int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_t n_idx, const int64_t* idx, float* s, float* a, float* R,
+                        float* s2, float* d, float* disc, int32_t* m);
 
 #ifdef __cplusplus
 }
