@@ -10,11 +10,13 @@
 
 #include <algorithm>
 #include <cmath>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <new>
 #include <random>
 #include <string>
+#include <tuple>
 #include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
@@ -252,16 +254,22 @@ struct Launch {
   const char* label = nullptr;
 };
 
+struct b200sac_replay;
+
+// What a step graph reads: the ring it samples (null: a step from rows already in `rows`), its rows buffer (a staging slot,
+// b200sac_step's buffer or the ring's rows), the injected noise (null: drawn in the step; the handle's eps buffer: already
+// in place), the steps it runs, and whether it was captured for the in-graph timeline (unforked).  Every pointer belongs to the handle or to a live ring, so the set of
+// keys is bounded; a ring's graphs go with it (drop_ring_graphs).
 struct GraphKey {
-  int variant;
-  const void* p[9];
+  b200sac_replay* ring;
+  const float* rows;
+  const float* eps;
+  int nsteps;
+  bool stamping;
   bool operator<(const GraphKey& o) const {
-    if (variant != o.variant) return variant < o.variant;
-    return memcmp(p, o.p, sizeof(p)) < 0;
+    return std::tie(ring, rows, eps, nsteps, stamping) < std::tie(o.ring, o.rows, o.eps, o.nsteps, o.stamping);
   }
 };
-
-struct b200sac_replay;
 
 struct b200sac {
   b200sac_cfg cfg;
@@ -336,7 +344,7 @@ struct b200sac {
   CUtensorMap* d_cmaps = nullptr; // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
                                   // weight-gradient operands [R][nw]
   long long* chain_dbg = nullptr; // B200SAC_CHAIN_DBG=1: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
-  float* split_d = nullptr;       // b200sac_step: handle-owned copy of the caller's minibatch arrays (stable graph pointers)
+  float* step_d = nullptr;        // b200sac_step: the caller's minibatch as packed rows [R][B][row_stride] (stable graph pointers)
   float* loss_h = nullptr;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
   float* loss_h_dev = nullptr;    // its device-side address
   // prioritized replay (allocated with the first prioritized ring): [3][R][B] importance weights of the step, leaf values
@@ -390,6 +398,30 @@ struct b200sac_replay {
   int* f_m = nullptr;
 };
 
+// Transition rows [s | a | r | s' | d], padded to row_stride floats: the format of the replay ring, the staging slots and
+// b200sac_step's buffer (ingest_rows_kernel, ingest_nstep_kernel and nstep_fold_kernel read it on the device).  Field k of
+// a row is w[k] floats at offset off[k]; a minibatch outside a row is five field arrays [n][w[k]].
+enum { ROW_S, ROW_A, ROW_R, ROW_S2, ROW_D, ROW_FIELDS };
+struct RowFields { int w[ROW_FIELDS], off[ROW_FIELDS]; };
+static RowFields row_fields(const b200sac* h) {
+  const int obs = h->K.obs, A = h->K.act;
+  return {{obs, A, 1, obs, 1}, {0, obs, obs + A, obs + A + 1, 2 * obs + A + 1}};
+}
+
+// transition i of the field arrays f -> one row
+static void pack_row(const b200sac* h, float* row, const float* const f[ROW_FIELDS], long long i) {
+  const RowFields F = row_fields(h);
+  for (int k = 0; k < ROW_FIELDS; ++k) memcpy(row + F.off[k], f[k] + i * F.w[k], F.w[k] * sizeof(float));
+}
+
+// n consecutive rows -> transitions i0 .. i0 + n - 1 of the field arrays f
+static void unpack_rows(const b200sac* h, const float* rows, long long n, float* const f[ROW_FIELDS], long long i0) {
+  const RowFields F = row_fields(h);
+  for (long long i = 0; i < n; ++i)
+    for (int k = 0; k < ROW_FIELDS; ++k)
+      memcpy(f[k] + (i0 + i) * F.w[k], rows + i * h->row_stride + F.off[k], F.w[k] * sizeof(float));
+}
+
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
 static Buf carve(size_t& cursor, size_t n_per_rep, int R) {
@@ -425,7 +457,7 @@ static int destroy_impl(b200sac* h) {
   }
   cudaFree(h->blob_src);
   cudaFree(h->blob_dst);
-  cudaFree(h->split_d);
+  cudaFree(h->step_d);
   cudaFree(h->chain_dbg);
   cudaFree(h->d_cmaps);
   cudaFree(h->per_buf);
@@ -2039,7 +2071,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   }
 
   // staging (pinned host <-> device), side stream
-  h->row_w = 2 * obs + A + 2;
+  h->row_w = row_fields(h).off[ROW_D] + 1;
   h->row_stride = (h->row_w + 31) / 32 * 32;   // 128-byte aligned transition rows
   h->stage_floats = (size_t)R * B * h->row_stride + (size_t)2 * R * B * A;   // rows + eps_next/eps_cur
   for (int i = 0; i < 2; ++i) {
@@ -2358,9 +2390,9 @@ extern "C" int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t
 }
 
 // ------------------------------------------------------------------------------------------
-// step variants.  variant 0: split device arrays; 1: packed rows (dense, staged); 2: replay gather
+// the step: from packed rows (a staging slot or b200sac_step's buffer) or sampled from a device ring
 // ------------------------------------------------------------------------------------------
-// variant 2 sampling modes (multi-step graphs): SAMPLE_INLINE = sample on `st` right before the gather (one step per graph);
+// ring sampling modes (multi-step graphs): SAMPLE_INLINE = sample on `st` right before the gather (one step per graph);
 // SAMPLE_DONE = the indices of this step were already drawn on the fork stream (wait for them); `fork_next` = once this
 // step's gather has consumed the index buffer and bumped the step counter, draw the NEXT step's indices on the fork stream
 // -- that kernel then overlaps the whole step instead of heading its critical path.
@@ -2371,24 +2403,18 @@ static NstepRing nstep_ring(const b200sac_replay* rb) {
   return N;
 }
 
-static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* const* p, b200sac_replay* rb,
-                        cudaEvent_t* evs = nullptr, int sample_mode = SAMPLE_INLINE, bool fork_next = false) {
+static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, cudaEvent_t* evs = nullptr,
+                        int sample_mode = SAMPLE_INLINE, bool fork_next = false) {
   if (evs) CU(cudaEventRecord(evs[0], st));
   const int B = h->cfg.batch, R = h->R;
   dim3 grid((B + 7) / 8, R), block(256);
   if (grid.x > 64) grid.x = 64;
-  bool use_eps = false;
-  if (variant == 0) {
-    use_eps = p[5] != nullptr;
-    launch_k(ingest_split_kernel, grid, block, 0, st, h->K, h->ing, (const float*)p[0], (const float*)p[1], (const float*)p[2],
-             (const float*)p[3], (const float*)p[4], (const float*)p[5], (const float*)p[6]);
-  } else if (variant == 1) {
-    const float* rows = (const float*)p[0];
-    const float* e = (const float*)p[1];
-    use_eps = e != nullptr;
-    launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, rows, (long long)B * h->row_stride, h->row_stride,
+  b200sac_replay* rb = key.ring;
+  if (!rb) {
+    launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, key.rows, (long long)B * h->row_stride, h->row_stride,
              (const int*)nullptr, (long long)0);
-    if (use_eps) {      // (rows carry the transition itself) eps staged as [R][B][A] next, then [R][B][A] cur
+    if (key.eps && key.eps != h->eps.p) {      // staged eps, [R][B][A] next, then [R][B][A] cur: into the step's buffer
+      const float* e = key.eps;
       const size_t n = (size_t)B * h->cfg.act_dim * sizeof(float);
       for (int rep = 0; rep < R; ++rep) {
         CU(cudaMemcpyAsync(h->eps.p + rep * h->eps.rs, e + (size_t)rep * B * h->cfg.act_dim, n, cudaMemcpyDeviceToDevice, st));
@@ -2418,32 +2444,23 @@ static int enqueue_body(b200sac* h, cudaStream_t st, int variant, const void* co
     }
   }
   CU(cudaGetLastError());
-  const bool per = variant == 2 && rb->per;
-  return run_plan(h, st, use_eps, evs ? evs + 1 : nullptr, evs == nullptr && !h->stamping, variant == 2 ? rb : nullptr, per && fork_next);
+  return run_plan(h, st, key.eps != nullptr, evs ? evs + 1 : nullptr, evs == nullptr && !key.stamping, rb,
+                  rb && rb->per && fork_next);
 }
 
 // nsteps > 1 (device-ring sampling only): that many consecutive gradient steps captured in ONE graph, so a pipelined
 // run pays the graph-launch gap (a few us between two graph launches) once per graph.  A run of n steps is cut
 // greedily into graphs of 8, 4, 2 and 1 steps.
 constexpr int kGraphSteps = 8;
-static int get_graph(b200sac* h, cudaStream_t st, int variant, const void* const* p, int np, b200sac_replay* rb, int nsteps,
-                     cudaGraphExec_t* out) {
-  GraphKey key;
-  memset(&key, 0, sizeof(key));
-  key.variant = variant + 4 * (h->stamping ? 1 : 0) + 16 * (nsteps - 1);      // the timeline run captures unforked graphs
-  for (int i = 0; i < np && i < 9; ++i) key.p[i] = p[i];
-  if (rb) key.p[8] = rb;
+static int get_graph(b200sac* h, cudaStream_t st, const GraphKey& key, cudaGraphExec_t* out) {
   auto it = h->graphs.find(key);
   if (it == h->graphs.end()) {
-    if (h->graphs.size() >= 64) {   // bound the cache: drop everything (pointers churn)
-      for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
-      h->graphs.clear();
-    }
+    const int nsteps = key.nsteps;
     cudaGraph_t g = nullptr;
     CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     int rc = 0;
     for (int k = 0; k < nsteps && rc == 0; ++k)
-      rc = enqueue_body(h, st, variant, p, rb, nullptr, (nsteps > 1 && k > 0) ? SAMPLE_DONE : SAMPLE_INLINE, nsteps > 1 && k + 1 < nsteps);
+      rc = enqueue_body(h, st, key, nullptr, (nsteps > 1 && k > 0) ? SAMPLE_DONE : SAMPLE_INLINE, nsteps > 1 && k + 1 < nsteps);
     cudaError_t e = cudaStreamEndCapture(st, &g);
     if (rc) { if (g) cudaGraphDestroy(g); return rc; }
     if (e != cudaSuccess) return fail(B200SAC_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
@@ -2458,11 +2475,11 @@ static int get_graph(b200sac* h, cudaStream_t st, int variant, const void* const
   return 0;
 }
 
-static int launch_step(b200sac* h, cudaStream_t st, int variant, const void* const* p, int np, b200sac_replay* rb, int nsteps = 1) {
+static int launch_step(b200sac* h, cudaStream_t st, const GraphKey& key) {
   cudaGraphExec_t ge = nullptr;
-  if (int rc = get_graph(h, st, variant, p, np, rb, nsteps, &ge)) return rc;
+  if (int rc = get_graph(h, st, key, &ge)) return rc;
   CU(cudaGraphLaunch(ge, st));
-  h->host_steps += nsteps;
+  h->host_steps += key.nsteps;
   return 0;
 }
 
@@ -2475,14 +2492,11 @@ extern "C" int b200sac_prepare(b200sac_t* h, b200sac_replay_t* rb, void* stream)
   if (int rc = sb.begin()) return rc;
   cudaGraphExec_t ge = nullptr;
   if (rb->where == 0) {
-    const void* p[1] = {rb->rows};
     for (int n = kGraphSteps; n >= 1; n >>= 1)
-      if (int rc = get_graph(h, sb.run, 2, p, 1, rb, n, &ge)) return rc;
+      if (int rc = get_graph(h, sb.run, GraphKey{rb, rb->rows, nullptr, n, h->stamping}, &ge)) return rc;
   } else {
-    for (int slot = 0; slot < 2; ++slot) {
-      const void* p[2] = {h->stage_d[slot], nullptr};
-      if (int rc = get_graph(h, sb.run, 1, p, 2, nullptr, 1, &ge)) return rc;
-    }
+    for (int slot = 0; slot < 2; ++slot)
+      if (int rc = get_graph(h, sb.run, GraphKey{nullptr, h->stage_d[slot], nullptr, 1, h->stamping}, &ge)) return rc;
   }
   if (int rc = sb.end()) return rc;
   CU(cudaStreamSynchronize(sb.run));
@@ -2494,42 +2508,25 @@ extern "C" int b200sac_step(b200sac_t* h, const float* s, const float* a, const 
   if (!h || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null minibatch pointer");
   if ((eps_next == nullptr) != (eps_cur == nullptr)) return fail(B200SAC_ERR_INVALID, "eps_next and eps_cur must both be given or both NULL");
   CU(cudaSetDevice(h->device));
-  // The caller's arrays are copied (device to device, in stream order) into handle-owned buffers, so the captured graph
-  // sees the same pointers whatever tensors the caller passes: one graph per (with / without injected noise), never a
-  // re-capture per call.
-  const size_t RB = (size_t)h->R * h->cfg.batch, obs = (size_t)h->K.obs, A = (size_t)h->K.act;
-  const size_t n_s = RB * obs, n_a = RB * A, n_1 = RB;
-  if (!h->split_d) CU(cudaMalloc(&h->split_d, (2 * n_s + 3 * n_a + 2 * n_1) * sizeof(float)));
-  float* ds = h->split_d; float* da = ds + n_s; float* dr = da + n_a; float* ds2 = dr + n_1; float* dd = ds2 + n_s;
-  float* de1 = dd + n_1; float* de2 = de1 + n_a;
+  // The caller's arrays are copied (in stream order) into handle-owned buffers, so the captured graph sees the same
+  // pointers whatever tensors the caller passes: one graph per (with / without injected noise), never a re-capture per
+  // call.  The transitions become rows laid out like a staging slot's (the staged step's graph body), the noise goes
+  // straight into the step's noise buffer.
+  const size_t RB = (size_t)h->R * h->cfg.batch, nA = (size_t)h->cfg.batch * h->cfg.act_dim;
+  if (!h->step_d) CU(cudaMalloc(&h->step_d, RB * h->row_stride * sizeof(float)));
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
-  CU(cudaMemcpyAsync(ds, s, n_s * sizeof(float), cudaMemcpyDefault, sb.run));
-  CU(cudaMemcpyAsync(da, a, n_a * sizeof(float), cudaMemcpyDefault, sb.run));
-  CU(cudaMemcpyAsync(dr, r, n_1 * sizeof(float), cudaMemcpyDefault, sb.run));
-  CU(cudaMemcpyAsync(ds2, s2, n_s * sizeof(float), cudaMemcpyDefault, sb.run));
-  CU(cudaMemcpyAsync(dd, d, n_1 * sizeof(float), cudaMemcpyDefault, sb.run));
-  if (eps_next) {
-    CU(cudaMemcpyAsync(de1, eps_next, n_a * sizeof(float), cudaMemcpyDefault, sb.run));
-    CU(cudaMemcpyAsync(de2, eps_cur, n_a * sizeof(float), cudaMemcpyDefault, sb.run));
-  }
-  const void* p[7] = {ds, da, dr, ds2, dd, eps_next ? de1 : nullptr, eps_next ? de2 : nullptr};
-  if (int rc = launch_step(h, sb.run, 0, p, 7, nullptr)) return rc;
+  const RowFields F = row_fields(h);
+  const float* f[ROW_FIELDS] = {s, a, r, s2, d};
+  for (int k = 0; k < ROW_FIELDS; ++k)
+    CU(cudaMemcpy2DAsync(h->step_d + F.off[k], h->row_stride * sizeof(float), f[k], F.w[k] * sizeof(float),
+                         F.w[k] * sizeof(float), RB, cudaMemcpyDefault, sb.run));
+  if (eps_next)           // [R][B][A] next and cur -> per replica [B][A] next, then [B][A] cur
+    for (int k = 0; k < 2; ++k)
+      CU(cudaMemcpy2DAsync(h->eps.p + k * nA, h->eps.rs * sizeof(float), k ? eps_cur : eps_next, nA * sizeof(float),
+                           nA * sizeof(float), h->R, cudaMemcpyDefault, sb.run));
+  if (int rc = launch_step(h, sb.run, GraphKey{nullptr, h->step_d, eps_next ? h->eps.p : nullptr, 1, h->stamping})) return rc;
   return sb.end();
-}
-
-// pack one replica-major minibatch into packed rows in pinned staging
-static void pack_rows(const b200sac* h, float* dst, const float* s, const float* a, const float* r, const float* s2,
-                      const float* d) {
-  const int B = h->cfg.batch, R = h->R, obs = h->K.obs, A = h->K.act, rs = h->row_stride;
-  for (long long i = 0; i < (long long)R * B; ++i) {
-    float* row = dst + i * rs;
-    memcpy(row, s + i * obs, obs * sizeof(float));
-    memcpy(row + obs, a + i * A, A * sizeof(float));
-    row[obs + A] = r[i];
-    memcpy(row + obs + A + 1, s2 + i * obs, obs * sizeof(float));
-    row[2 * obs + A + 1] = d[i];
-  }
 }
 
 // stage slot -> device on the side stream, make `st` wait for it, run the step from the staged rows
@@ -2540,8 +2537,8 @@ static int staged_step(b200sac* h, cudaStream_t st, int slot, bool with_eps) {
                      cudaMemcpyHostToDevice, h->side));
   CU(cudaEventRecord(h->ev_copied[slot], h->side));
   CU(cudaStreamWaitEvent(st, h->ev_copied[slot], 0));
-  const void* p[2] = {h->stage_d[slot], with_eps ? h->stage_d[slot] + rows_f : nullptr};
-  if (int rc = launch_step(h, st, 1, p, 2, nullptr)) return rc;
+  const float* eps = with_eps ? h->stage_d[slot] + rows_f : nullptr;
+  if (int rc = launch_step(h, st, GraphKey{nullptr, h->stage_d[slot], eps, 1, h->stamping})) return rc;
   CU(cudaEventRecord(h->ev_consumed[slot], st));
   h->stage_used[slot] = true;
   return 0;
@@ -2582,7 +2579,8 @@ extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, c
   cudaStream_t st = sb.run;
   int slot;
   if (int rc = acquire_slot(h, &slot)) return rc;
-  pack_rows(h, h->stage_h[slot], s, a, r, s2, d);
+  const float* f[ROW_FIELDS] = {s, a, r, s2, d};
+  for (long long i = 0; i < (long long)h->R * h->cfg.batch; ++i) pack_row(h, h->stage_h[slot] + i * h->row_stride, f, i);
   if (eps_next) {
     const size_t rows_f = (size_t)h->R * h->cfg.batch * h->row_stride;
     const size_t n = (size_t)h->R * h->cfg.batch * h->cfg.act_dim;
@@ -2657,9 +2655,8 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   std::vector<cudaEvent_t> evs((size_t)n + 1);
   for (auto& e : evs) CU(cudaEventCreate(&e));
   std::vector<double> acc((size_t)n, 0.0);
-  const void* p[1] = {rb->rows};
   for (int it = 0; it < iters; ++it) {
-    if (int rc = enqueue_body(h, sb.run, 2, p, rb, evs.data())) return rc;
+    if (int rc = enqueue_body(h, sb.run, GraphKey{rb, rb->rows, nullptr, 1, h->stamping}, evs.data())) return rc;
     h->host_steps += 1;
     CU(cudaStreamSynchronize(sb.run));
     for (int i = 0; i < n; ++i) {
@@ -3026,6 +3023,98 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
 // ------------------------------------------------------------------------------------------
 // replay ring
 // ------------------------------------------------------------------------------------------
+// The ring's rules, each written once:
+//   arguments    ring_check: a ring, a replica of its handle, and the kind of ring the call needs;
+//   writers      rows, fill, tree leaves and links are written under rb->mu after ring_quiesce, so no gather already
+//                enqueued by a step reads a torn row and no concurrent writer interleaves;
+//   samplers     ring_ready: every sub-ring a draw reads holds enough transitions;
+//   indices      filled_slot: a ring index the caller names holds a transition;
+//   allocation   RingAlloc: all pieces or none, committed to the ring / handle only when every one succeeded.
+enum { RING_ANY, RING_PER, RING_TRAJ };
+static int ring_check(const b200sac_replay* rb, int32_t replica, int kind = RING_ANY) {
+  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
+  if (kind == RING_PER && !rb->per) return fail(B200SAC_ERR_INVALID, "not a prioritized ring (b200sac_replay_create_prioritized)");
+  if (kind == RING_TRAJ && !rb->traj)
+    return fail(B200SAC_ERR_STATE, "the ring has no trajectory links (b200sac_replay_enable_trajectories)");
+  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  return 0;
+}
+
+// Waits (under rb->mu) until every step enqueued so far has gathered its rows and updated its priorities.
+static int ring_quiesce(b200sac_replay* rb) {
+  if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
+  return 0;
+}
+
+// (under rb->mu) Every task sub-ring of `replica` (kAllReplicas: of every replica) holds at least `batches` per-task
+// batches: 4 for the step's samplers, 1 for a draw without replacement, which would not end with fewer.
+constexpr int kAllReplicas = -1;
+static int ring_ready(const b200sac_replay* rb, int replica, int batches) {
+  const long long need = (long long)batches * (rb->h->cfg.batch / rb->Teff);
+  const int r0 = replica == kAllReplicas ? 0 : replica, r1 = replica == kAllReplicas ? rb->h->R : replica + 1;
+  for (int rep = r0; rep < r1; ++rep)
+    for (int t = 0; t < rb->Teff; ++t)
+      if (rb->fill[(size_t)rep * rb->Teff + t] < need)
+        return fail(B200SAC_ERR_STATE, "replay not ready: replica %d task %d holds %lld transitions, need >= %lld (%d x per-task batch)",
+                    rep, t, rb->fill[(size_t)rep * rb->Teff + t], need, batches);
+  return 0;
+}
+
+// (under rb->mu) ring index k of `replica` holds a transition
+static int filled_slot(const b200sac_replay* rb, int replica, long long k) {
+  if (k < 0 || k >= rb->cap) return fail(B200SAC_ERR_INVALID, "index %lld outside the ring [0, %lld)", k, rb->cap);
+  if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
+    return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
+  return 0;
+}
+
+// All-or-nothing allocation: each piece goes into a local (optionally zero-filled with `byte`, or copied from a host
+// vector); unless commit() succeeds, the destructor releases every piece, so the caller stores them only after commit().
+struct RingAlloc {
+  bool ok = true;
+  std::vector<std::function<void()>> undo;
+  template <class T> T* device(size_t n, int byte = -1) {
+    T* p = nullptr;
+    if (!(ok = ok && cudaMalloc(&p, n * sizeof(T)) == cudaSuccess)) return nullptr;
+    undo.push_back([p] { cudaFree(p); });
+    ok = byte < 0 || cudaMemset(p, byte, n * sizeof(T)) == cudaSuccess;
+    return p;
+  }
+  template <class T> T* device(const std::vector<T>& v) {
+    T* p = device<T>(v.size());
+    ok = ok && cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
+    return p;
+  }
+  float* pinned(size_t n) {
+    float* p = nullptr;
+    if ((ok = ok && cudaMallocHost(&p, n * sizeof(float)) == cudaSuccess)) undo.push_back([p] { cudaFreeHost(p); });
+    return p;
+  }
+  cudaEvent_t event() {
+    cudaEvent_t e = nullptr;
+    if ((ok = ok && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess)) undo.push_back([e] { cudaEventDestroy(e); });
+    return e;
+  }
+  cudaStream_t stream() {
+    cudaStream_t s = nullptr;
+    if ((ok = ok && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess)) undo.push_back([s] { cudaStreamDestroy(s); });
+    return s;
+  }
+  bool commit() {
+    if (ok) undo.clear(); else cudaGetLastError();
+    return ok;
+  }
+  ~RingAlloc() { for (auto& u : undo) u(); }
+};
+
+// Graphs that captured a ring's pointers (its gather) go when the ring goes or its gather changes.
+static void drop_ring_graphs(b200sac* h, const b200sac_replay* rb) {
+  for (auto it = h->graphs.begin(); it != h->graphs.end();) {
+    if (it->first.ring == rb) { cudaGraphExecDestroy(it->second); it = h->graphs.erase(it); }
+    else ++it;
+  }
+}
+
 extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t where, uint64_t seed, b200sac_replay_t** out) {
   if (!h || !out) return fail(B200SAC_ERR_INVALID, "null argument");
   *out = nullptr;
@@ -3045,20 +3134,18 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
   rb->rng.seed(seed);
   rb->fill.assign((size_t)h->R * Teff, 0);
   rb->head.assign((size_t)h->R * Teff, 0);
-  const size_t bytes = (size_t)h->R * rb->rs_rows * sizeof(float);
-  cudaError_t e = where == 0 ? cudaMalloc(&rb->rows, bytes) : cudaMallocHost(&rb->rows, bytes);
-  if (e != cudaSuccess) { delete rb; return fail(B200SAC_ERR_NOMEM, "replay allocation of %zu bytes failed: %s", bytes, cudaGetErrorString(e)); }
+  const size_t n = (size_t)h->R * rb->rs_rows;
+  RingAlloc al;                                    // (the ring is not handed out before commit: its fields are the locals)
+  rb->rows = where == 0 ? al.device<float>(n) : al.pinned(n);
   if (where == 0) {
-    if (cudaMalloc(&rb->d_fill, sizeof(long long) * h->R * Teff) != cudaSuccess ||
-        cudaMalloc(&rb->d_idx, sizeof(int) * h->R * h->cfg.batch) != cudaSuccess ||
-        cudaMemset(rb->d_fill, 0, sizeof(long long) * h->R * Teff) != cudaSuccess ||
-        cudaEventCreateWithFlags(&rb->ev_gather, cudaEventDisableTiming) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&rb->st, cudaStreamNonBlocking) != cudaSuccess) {
-      cudaFree(rb->rows); cudaFree(rb->d_fill); cudaFree(rb->d_idx);
-      if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
-      delete rb;
-      return fail(B200SAC_ERR_NOMEM, "replay index allocation failed");
-    }
+    rb->d_fill = al.device<long long>((size_t)h->R * Teff, 0);
+    rb->d_idx = al.device<int>((size_t)h->R * h->cfg.batch);
+    rb->ev_gather = al.event();
+    rb->st = al.stream();
+  }
+  if (!al.commit()) {
+    delete rb;
+    return fail(B200SAC_ERR_NOMEM, "replay allocation of %zu bytes failed", n * sizeof(float));
   }
   *out = rb;
   return 0;
@@ -3067,12 +3154,8 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
 extern "C" int b200sac_replay_destroy(b200sac_replay_t* rb) {
   if (!rb) return 0;
   cudaSetDevice(rb->h->device);
-  // graphs that captured this ring's pointers must go
   if (rb->h->prefetch_rb == rb) { rb->h->prefetch_slot = -1; rb->h->prefetch_rb = nullptr; }
-  for (auto it = rb->h->graphs.begin(); it != rb->h->graphs.end();) {
-    if (it->first.p[8] == rb) { cudaGraphExecDestroy(it->second); it = rb->h->graphs.erase(it); }
-    else ++it;
-  }
+  drop_ring_graphs(rb->h, rb);
   if (rb->where == 0) cudaFree(rb->rows); else cudaFreeHost(rb->rows);
   cudaFree(rb->d_fill); cudaFree(rb->d_idx);
   if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
@@ -3134,9 +3217,9 @@ static void push_links(b200sac_replay* rb, int replica, int64_t n, const std::ve
 
 static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a, const float* r,
                      const float* s2, const float* d, const int32_t* stream, const uint8_t* cut) {
-  if (!rb || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (int rc = ring_check(rb, replica)) return rc;
+  if (!s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
   b200sac* h = rb->h;
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica out of range");
   if (n < 0) return fail(B200SAC_ERR_INVALID, "n < 0");
   if (stream)
     for (int64_t i = 0; i < n; ++i)
@@ -3146,16 +3229,13 @@ static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const flo
   std::vector<int> row_task;
   std::vector<long long> row_slot;                 // first the row's position in its task bucket, then its slot
   if (rb->traj) { row_task.resize((size_t)n); row_slot.resize((size_t)n); }
-  const int obs = h->K.obs, A = h->K.act, T = h->cfg.num_tasks, rs = h->row_stride;
+  const int obs = h->K.obs, T = h->cfg.num_tasks, rs = h->row_stride;
   // pack the rows, bucketed by task, then copy each bucket as at most two contiguous runs (ring wrap)
   std::vector<std::vector<float>> bucket((size_t)rb->Teff);
   std::vector<float> row((size_t)rs, 0.f);
+  const float* f[ROW_FIELDS] = {s, a, r, s2, d};
   for (int64_t i = 0; i < n; ++i) {
-    memcpy(row.data(), s + i * obs, obs * sizeof(float));
-    memcpy(row.data() + obs, a + i * A, A * sizeof(float));
-    row[obs + A] = r[i];
-    memcpy(row.data() + obs + A + 1, s2 + i * obs, obs * sizeof(float));
-    row[2 * obs + A + 1] = d[i];
+    pack_row(h, row.data(), f, i);
     int task = 0;
     if (T > 0) {
       float best = row[obs - T];
@@ -3174,9 +3254,8 @@ static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const flo
       row_slot[(size_t)i] = k < skip ? -1 : (rb->head[(size_t)replica * rb->Teff + task] + (k - skip)) % rb->cap_per_task;
     }
   }
-  // Device ring: the gathers of every step enqueued so far must have read their rows before a wrapped ring overwrites
-  // them (a torn transition otherwise); step_sampled enqueues under the same mutex, so none can slip in while we copy.
-  if (rb->where == 0 && rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
+  // step_sampled enqueues under the same mutex, so no gather can slip in while we copy
+  if (int rc = ring_quiesce(rb)) return rc;
   for (int task = 0; task < rb->Teff; ++task) {
     const float* src = bucket[(size_t)task].data();
     long long cnt = (long long)(bucket[(size_t)task].size() / (size_t)rs);
@@ -3239,8 +3318,8 @@ extern "C" int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_
 extern "C" int b200sac_replay_push_traj(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a,
                                         const float* r, const float* s2, const float* d, const int32_t* stream,
                                         const uint8_t* cut) {
-  if (!rb || !stream) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!rb->traj) return fail(B200SAC_ERR_STATE, "push_traj needs a ring with trajectory links (b200sac_replay_enable_trajectories)");
+  if (!stream) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   return push_impl(rb, replica, n, s, a, r, s2, d, stream, cut);
 }
 
@@ -3252,6 +3331,8 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   if (per > rb->cap_per_task) per = rb->cap_per_task;
   if (per < 1) return fail(B200SAC_ERR_INVALID, "n too small");
   cudaStream_t st = (cudaStream_t)stream;
+  std::lock_guard<std::mutex> lk(rb->mu);
+  if (int rc = ring_quiesce(rb)) return rc;
   float* dev_rows = rb->rows;
   float* tmp = nullptr;
   if (rb->where == 1) {   // generate on the device, copy down into the pinned ring
@@ -3267,9 +3348,7 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
     CU(cudaStreamSynchronize(st));
     CU(cudaFree(tmp));
   }
-  std::lock_guard<std::mutex> lk(rb->mu);
   if (rb->per) {                                   // rows [0, per) of every sub-ring get the current max p, the rest are empty
-    if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
     per_fill_kernel<<<dim3(rb->Teff, h->R), 1024, 0, st>>>(rb->tr, 0, 0, 0, rb->tr.P, per);
     CU(cudaGetLastError());
   }
@@ -3278,9 +3357,8 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   if (rb->where == 0)
     CU(cudaMemcpyAsync(rb->d_fill, rb->fill.data(), sizeof(long long) * rb->fill.size(), cudaMemcpyHostToDevice, st));
   if (rb->traj) {                                  // slot i -> i + 1 unless d_i != 0 or i is the last filled slot; no open streams
-    if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
     nstep_fill_links_kernel<<<dim3(256, h->R), 256, 0, st>>>(rb->d_link, rb->cap, (int)rb->cap_per_task, rb->rows, rb->rs_rows,
-                                                            h->row_stride, 2 * h->K.obs + h->K.act + 1, per);
+                                                            h->row_stride, row_fields(h).off[ROW_D], per);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(rb->link_h.data(), rb->d_link, rb->link_h.size() * sizeof(int), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -3295,7 +3373,8 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
 }
 
 extern "C" int b200sac_replay_size(b200sac_replay_t* rb, int32_t replica, int64_t* n) {
-  if (!rb || !n || replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (int rc = ring_check(rb, replica)) return rc;
+  if (!n) return fail(B200SAC_ERR_INVALID, "null argument");
   std::lock_guard<std::mutex> lk(rb->mu);
   long long mn = rb->fill[(size_t)replica * rb->Teff];
   for (int t = 1; t < rb->Teff; ++t) mn = std::min(mn, rb->fill[(size_t)replica * rb->Teff + t]);
@@ -3303,13 +3382,13 @@ extern "C" int b200sac_replay_size(b200sac_replay_t* rb, int32_t replica, int64_
   return 0;
 }
 
-// host-side index draw: uniform without replacement, per task (random.sample semantics)
+// host-side index draw (under rb->mu): uniform without replacement, per task (random.sample semantics)
 static int host_draw(b200sac_replay* rb, int replica, std::vector<long long>& idx) {
+  if (int rc = ring_ready(rb, replica, 1)) return rc;
   const int B = rb->h->cfg.batch, per = B / rb->Teff;
   idx.clear();
   for (int t = 0; t < rb->Teff; ++t) {
     const long long n = rb->fill[(size_t)replica * rb->Teff + t];
-    if (n < per) return fail(B200SAC_ERR_STATE, "replay holds %lld transitions for task %d, need %d", n, t, per);
     std::unordered_set<long long> seen;
     while ((int)seen.size() < per) {
       const long long v = (long long)(rb->rng() % (unsigned long long)n);
@@ -3322,24 +3401,21 @@ static int host_draw(b200sac_replay* rb, int replica, std::vector<long long>& id
 
 extern "C" int b200sac_replay_sample(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
                                      float* d, int64_t* idx_out) {
-  if (!rb || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (int rc = ring_check(rb, replica)) return rc;
+  if (!s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
   b200sac* h = rb->h;
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica out of range");
   if (rb->per) return fail(B200SAC_ERR_INVALID, "prioritized ring: sample with b200sac_replay_sample_prioritized (rows, indices, weights)");
   CU(cudaSetDevice(h->device));
-  const int B = h->cfg.batch, obs = h->K.obs, A = h->K.act, rs = h->row_stride;
+  const int B = h->cfg.batch, rs = h->row_stride;
   std::vector<long long> idx;
   std::vector<float> row((size_t)rs);
+  float* const f[ROW_FIELDS] = {s, a, r, s2, d};
   std::lock_guard<std::mutex> lk(rb->mu);
   if (int rc = host_draw(rb, replica, idx)) return rc;
   for (int i = 0; i < B; ++i) {
     const float* src = rb->rows + (size_t)replica * rb->rs_rows + (size_t)idx[i] * rs;
     if (rb->where == 0) { CU(cudaMemcpy(row.data(), src, rs * sizeof(float), cudaMemcpyDeviceToHost)); src = row.data(); }
-    memcpy(s + (size_t)i * obs, src, obs * sizeof(float));
-    memcpy(a + (size_t)i * A, src + obs, A * sizeof(float));
-    r[i] = src[obs + A];
-    memcpy(s2 + (size_t)i * obs, src + obs + A + 1, obs * sizeof(float));
-    d[i] = src[2 * obs + A + 1];
+    unpack_rows(h, src, 1, f, i);
     if (idx_out) idx_out[i] = idx[i];
   }
   return 0;
@@ -3352,23 +3428,20 @@ extern "C" int b200sac_step_sampled(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   cudaStream_t st = sb.run;
-  const int B = h->cfg.batch, per = B / rb->Teff;
+  const int B = h->cfg.batch;
   {
     std::lock_guard<std::mutex> lk(rb->mu);
-    for (auto f : rb->fill)
-      if (f < 4LL * per)
-        return fail(B200SAC_ERR_STATE, "replay not ready: a ring holds %lld transitions, need >= %d (4 x per-task batch)", f, 4 * per);
+    if (int rc = ring_ready(rb, kAllReplicas, 4)) return rc;
   }
   if (rb->where == 0) {
-    std::lock_guard<std::mutex> lk(rb->mu);           // ordered against b200sac_replay_push (see there)
-    const void* p[1] = {rb->rows};
+    std::lock_guard<std::mutex> lk(rb->mu);           // ordered against the ring's writers (ring_quiesce)
     int i = 0;
     if (!h->stamping)                           // (the in-graph timeline wants one step per graph)
       for (int n = kGraphSteps; n > 1; n >>= 1)
         for (; i + n <= n_steps; i += n)
-          if (int rc = launch_step(h, st, 2, p, 1, rb, n)) return rc;
+          if (int rc = launch_step(h, st, GraphKey{rb, rb->rows, nullptr, n, h->stamping})) return rc;
     for (; i < n_steps; ++i)
-      if (int rc = launch_step(h, st, 2, p, 1, rb)) return rc;
+      if (int rc = launch_step(h, st, GraphKey{rb, rb->rows, nullptr, 1, h->stamping})) return rc;
     CU(cudaEventRecord(rb->ev_gather, st));
     rb->gather_pending = true;
     return sb.end();
@@ -3404,8 +3477,7 @@ extern "C" int b200sac_step_sampled(b200sac_t* h, b200sac_replay_t* rb, int32_t 
       if (int rc = prepare(&slot)) return rc;
     h->prefetch_slot = -1;
     CU(cudaStreamWaitEvent(st, h->ev_copied[slot], 0));
-    const void* p[2] = {h->stage_d[slot], nullptr};
-    if (int rc = launch_step(h, st, 1, p, 2, nullptr)) return rc;
+    if (int rc = launch_step(h, st, GraphKey{nullptr, h->stage_d[slot], nullptr, 1, h->stamping})) return rc;
     CU(cudaEventRecord(h->ev_consumed[slot], st));
     h->stage_used[slot] = true;
     int next;
@@ -3442,49 +3514,37 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
   while (tr.P < tr.cap) { tr.P <<= 1; ++tr.levels; }
   rb->draws.assign((size_t)h->R, 0);
   const size_t nt = (size_t)h->R * tr.T;
-  std::vector<float> ones(nt, 1.f);
-  std::vector<double> betas((size_t)h->R, beta);
-  auto fail_free = [&](const char* what) {
-    b200sac_replay_destroy(rb);
-    return fail(B200SAC_ERR_NOMEM, "prioritized replay: %s failed", what);
-  };
-  if (cudaMalloc(&tr.tree, nt * 2 * (size_t)tr.P * sizeof(float)) != cudaSuccess ||
-      cudaMemset(tr.tree, 0, nt * 2 * (size_t)tr.P * sizeof(float)) != cudaSuccess)
-    return fail_free("sum-tree allocation");
-  if (cudaMalloc(&tr.maxp, nt * sizeof(float)) != cudaSuccess || cudaMalloc(&rb->d_beta, (size_t)h->R * sizeof(double)) != cudaSuccess ||
-      cudaMemcpy(tr.maxp, ones.data(), nt * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMemcpy(rb->d_beta, betas.data(), (size_t)h->R * sizeof(double), cudaMemcpyHostToDevice) != cudaSuccess ||
-      cudaMalloc(&rb->s_lidx, kPerMaxB * sizeof(long long)) != cudaSuccess || cudaMalloc(&rb->s_idx, kPerMaxB * sizeof(int)) != cudaSuccess ||
-      cudaMalloc(&rb->s_f, kPerMaxB * sizeof(float)) != cudaSuccess ||
-      cudaMalloc(&rb->s_rows, (size_t)h->cfg.batch * h->row_stride * sizeof(float)) != cudaSuccess)
-    return fail_free("allocation");
-  if (!h->per_buf) {
-    const size_t n = (size_t)3 * h->R * h->cfg.batch;
-    if (cudaMalloc(&h->per_buf, n * sizeof(float)) != cudaSuccess || cudaMemset(h->per_buf, 0, n * sizeof(float)) != cudaSuccess ||
-        cudaStreamCreateWithFlags(&h->per_fork, cudaStreamNonBlocking) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->ev_per_src, cudaEventDisableTiming) != cudaSuccess ||
-        cudaEventCreateWithFlags(&h->ev_per_done, cudaEventDisableTiming) != cudaSuccess)
-      return fail_free("step buffer allocation");
+  RingAlloc al;
+  float* tree = al.device<float>(nt * 2 * (size_t)tr.P, 0);
+  float* maxp = al.device(std::vector<float>(nt, 1.f));
+  double* d_beta = al.device(std::vector<double>((size_t)h->R, beta));
+  long long* s_lidx = al.device<long long>(kPerMaxB);
+  int* s_idx = al.device<int>(kPerMaxB);
+  float* s_f = al.device<float>(kPerMaxB);
+  float* s_rows = al.device<float>((size_t)h->cfg.batch * h->row_stride);
+  // the handle's step buffers, with its first prioritized ring
+  float* per_buf = h->per_buf;
+  cudaStream_t per_fork = h->per_fork;
+  cudaEvent_t ev_src = h->ev_per_src, ev_done = h->ev_per_done;
+  if (!per_buf) {
+    per_buf = al.device<float>((size_t)3 * h->R * h->cfg.batch, 0);
+    per_fork = al.stream();
+    ev_src = al.event();
+    ev_done = al.event();
   }
+  if (!al.commit()) {
+    b200sac_replay_destroy(rb);
+    return fail(B200SAC_ERR_NOMEM, "prioritized replay: allocation failed");
+  }
+  tr.tree = tree; tr.maxp = maxp; rb->d_beta = d_beta;
+  rb->s_lidx = s_lidx; rb->s_idx = s_idx; rb->s_f = s_f; rb->s_rows = s_rows;
+  h->per_buf = per_buf; h->per_fork = per_fork; h->ev_per_src = ev_src; h->ev_per_done = ev_done;
   *out = rb;
   return 0;
 }
 
-static int per_check(b200sac_replay* rb, int32_t replica) {
-  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
-  if (!rb->per) return fail(B200SAC_ERR_INVALID, "not a prioritized ring (b200sac_replay_create_prioritized)");
-  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  return 0;
-}
-
-// Waits (under rb->mu) until every step enqueued so far is done with the trees.
-static int per_quiesce(b200sac_replay* rb) {
-  if (rb->gather_pending) { CU(cudaEventSynchronize(rb->ev_gather)); rb->gather_pending = false; }
-  return 0;
-}
-
 extern "C" int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, double beta, void* stream) {
-  if (int rc = per_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "beta must be in [0, 1] (got %g)", beta);
   CU(cudaSetDevice(rb->h->device));
   per_set_beta_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(rb->d_beta, replica, beta);
@@ -3493,22 +3553,19 @@ extern "C" int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, do
 }
 
 extern "C" int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, const float* prio) {
-  if (int rc = per_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (n < 0 || (n > 0 && (!idx || !prio))) return fail(B200SAC_ERR_INVALID, "bad argument");
   CU(cudaSetDevice(rb->h->device));
   std::lock_guard<std::mutex> lk(rb->mu);
   std::vector<int> ix((size_t)n);
   for (int64_t i = 0; i < n; ++i) {
-    const long long k = idx[i];
-    if (k < 0 || k >= rb->cap) return fail(B200SAC_ERR_INVALID, "index %lld outside the ring [0, %lld)", k, rb->cap);
-    if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
-      return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
+    if (int rc = filled_slot(rb, replica, idx[i])) return rc;
     if (!(prio[i] >= 0.f) || !std::isfinite(prio[i])) return fail(B200SAC_ERR_INVALID, "priority %lld is not a finite value >= 0", (long long)i);
     if (!std::isfinite((float)std::pow((double)prio[i] + rb->tr.eps, rb->tr.alpha)))     // (alpha > 1) an inf leaf: NaN weights
       return fail(B200SAC_ERR_INVALID, "priority %lld: (%g + eps)^alpha overflows fp32", (long long)i, (double)prio[i]);
-    ix[(size_t)i] = (int)k;
+    ix[(size_t)i] = (int)idx[i];
   }
-  if (int rc = per_quiesce(rb)) return rc;
+  if (int rc = ring_quiesce(rb)) return rc;
   for (int64_t i0 = 0; i0 < n; i0 += kPerMaxB) {          // chunks in order: a later index wins, as inside one chunk
     const int m = (int)std::min<int64_t>(kPerMaxB, n - i0);
     CU(cudaMemcpyAsync(rb->s_idx, ix.data() + i0, m * sizeof(int), cudaMemcpyHostToDevice, rb->st));
@@ -3521,14 +3578,14 @@ extern "C" int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t repli
 }
 
 extern "C" int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, float* p_out) {
-  if (int rc = per_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (n < 0 || (n > 0 && (!idx || !p_out))) return fail(B200SAC_ERR_INVALID, "bad argument");
   for (int64_t i = 0; i < n; ++i)
     if (idx[i] >= rb->cap || idx[i] < -(long long)rb->Teff)
       return fail(B200SAC_ERR_INVALID, "index %lld: neither a ring slot [0, %lld) nor a task root [-%d, -1]", (long long)idx[i], rb->cap, rb->Teff);
   CU(cudaSetDevice(rb->h->device));
   std::lock_guard<std::mutex> lk(rb->mu);
-  if (int rc = per_quiesce(rb)) return rc;
+  if (int rc = ring_quiesce(rb)) return rc;
   for (int64_t i0 = 0; i0 < n; i0 += kPerMaxB) {
     const int m = (int)std::min<int64_t>(kPerMaxB, n - i0);
     CU(cudaMemcpyAsync(rb->s_lidx, idx + i0, m * sizeof(long long), cudaMemcpyHostToDevice, rb->st));
@@ -3541,12 +3598,12 @@ extern "C" int b200sac_replay_get_priorities(b200sac_replay_t* rb, int32_t repli
 }
 
 extern "C" int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, float* out) {
-  if (int rc = per_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (task < 0 || task >= rb->Teff) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
   if (!out || n != 2 * rb->tr.P) return fail(B200SAC_ERR_INVALID, "a tree is 2P = %lld floats (got n = %lld)", 2 * rb->tr.P, (long long)n);
   CU(cudaSetDevice(rb->h->device));
   std::lock_guard<std::mutex> lk(rb->mu);
-  if (int rc = per_quiesce(rb)) return rc;
+  if (int rc = ring_quiesce(rb)) return rc;
   const float* src = rb->tr.tree + ((size_t)replica * rb->tr.T + task) * 2 * rb->tr.P;
   CU(cudaMemcpyAsync(out, src, (size_t)n * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
   CU(cudaStreamSynchronize(rb->st));
@@ -3555,17 +3612,14 @@ extern "C" int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, in
 
 extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
                                                  float* d, int64_t* idx_out, float* w_out) {
-  if (int rc = per_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (!s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null argument");
   b200sac* h = rb->h;
-  const int B = h->cfg.batch, obs = h->K.obs, A = h->K.act, rs = h->row_stride, per = B / rb->Teff;
+  const int B = h->cfg.batch, rs = h->row_stride;
   CU(cudaSetDevice(h->device));
   std::lock_guard<std::mutex> lk(rb->mu);
-  for (int t = 0; t < rb->Teff; ++t)
-    if (rb->fill[(size_t)replica * rb->Teff + t] < 4LL * per)
-      return fail(B200SAC_ERR_STATE, "replay not ready: task %d holds %lld transitions, need >= %d (4 x per-task batch)", t,
-                  rb->fill[(size_t)replica * rb->Teff + t], 4 * per);
-  if (int rc = per_quiesce(rb)) return rc;
+  if (int rc = ring_ready(rb, replica, 4)) return rc;
+  if (int rc = ring_quiesce(rb)) return rc;
   per_sample_kernel<<<1, B > 256 ? 512 : 256, 0, rb->st>>>(h->K, rb->tr, nullptr, rb->draws[(size_t)replica]++, replica,
                                                            rb->d_fill, rb->d_beta, rb->s_idx, rb->s_f, (long long)B, rb->seed);
   per_gather_kernel<<<B, 128, 0, rb->st>>>(rb->rows + (size_t)replica * rb->rs_rows, rs, rb->s_idx, rb->s_rows);
@@ -3576,13 +3630,9 @@ extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t r
   CU(cudaMemcpyAsync(w.data(), rb->s_f, B * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
   CU(cudaMemcpyAsync(rows.data(), rb->s_rows, rows.size() * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
   CU(cudaStreamSynchronize(rb->st));
+  float* const f[ROW_FIELDS] = {s, a, r, s2, d};
+  unpack_rows(h, rows.data(), B, f, 0);
   for (int i = 0; i < B; ++i) {
-    const float* src = rows.data() + (size_t)i * rs;
-    memcpy(s + (size_t)i * obs, src, obs * sizeof(float));
-    memcpy(a + (size_t)i * A, src + obs, A * sizeof(float));
-    r[i] = src[obs + A];
-    memcpy(s2 + (size_t)i * obs, src + obs + A + 1, obs * sizeof(float));
-    d[i] = src[2 * obs + A + 1];
     if (idx_out) idx_out[i] = ix[(size_t)i];
     if (w_out) w_out[i] = w[(size_t)i];
   }
@@ -3592,13 +3642,6 @@ extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t r
 // ------------------------------------------------------------------------------------------
 // n-step returns (nstep_kernels.cuh): trajectory links on a device ring, folded by the step's gather
 // ------------------------------------------------------------------------------------------
-static int traj_check(b200sac_replay* rb, int32_t replica) {
-  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
-  if (!rb->traj) return fail(B200SAC_ERR_STATE, "the ring has no trajectory links (b200sac_replay_enable_trajectories)");
-  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  return 0;
-}
-
 extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
   if (rb->where != 0) return fail(B200SAC_ERR_INVALID, "trajectory links need the device ring");
@@ -3608,32 +3651,19 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   for (auto f : rb->fill)
     if (f != 0) return fail(B200SAC_ERR_STATE, "trajectory links can only be enabled on an empty ring");
   CU(cudaSetDevice(h->device));
-  const size_t nl = (size_t)h->R * rb->cap, rs = (size_t)h->row_stride;
-  std::vector<int> ones((size_t)h->R, 1);
-  int* link = nullptr; int* nstep = nullptr; long long* f_idx = nullptr; float* f_rows = nullptr; float* f_disc = nullptr; int* f_m = nullptr;
-  float* ns_buf = h->ns_buf;
-  cudaEvent_t ev = nullptr;
-  const size_t nb = (size_t)3 * h->R * h->cfg.batch;
-  const bool ok =
-      cudaMalloc(&link, nl * sizeof(int)) == cudaSuccess && cudaMemset(link, 0xff, nl * sizeof(int)) == cudaSuccess &&
-      cudaMalloc(&nstep, (size_t)h->R * sizeof(int)) == cudaSuccess &&
-      cudaMemcpy(nstep, ones.data(), (size_t)h->R * sizeof(int), cudaMemcpyHostToDevice) == cudaSuccess &&
-      cudaMalloc(&f_idx, kNstepChunk * sizeof(long long)) == cudaSuccess && cudaMalloc(&f_rows, kNstepChunk * rs * sizeof(float)) == cudaSuccess &&
-      cudaMalloc(&f_disc, kNstepChunk * sizeof(float)) == cudaSuccess && cudaMalloc(&f_m, kNstepChunk * sizeof(int)) == cudaSuccess &&
-      cudaEventCreateWithFlags(&ev, cudaEventDisableTiming) == cudaSuccess &&
-      (ns_buf || (cudaMalloc(&ns_buf, nb * sizeof(float)) == cudaSuccess && cudaMemset(ns_buf, 0, nb * sizeof(float)) == cudaSuccess));
-  if (!ok) {
-    cudaGetLastError();
-    cudaFree(link); cudaFree(nstep); cudaFree(f_idx); cudaFree(f_rows); cudaFree(f_disc); cudaFree(f_m);
-    if (ns_buf != h->ns_buf) cudaFree(ns_buf);
-    if (ev) cudaEventDestroy(ev);
-    return fail(B200SAC_ERR_NOMEM, "trajectory link allocation failed");
-  }
-  // graphs captured for this ring before it was linked hold the unlinked gather
-  for (auto it = h->graphs.begin(); it != h->graphs.end();) {
-    if (it->first.p[8] == rb) { cudaGraphExecDestroy(it->second); it = h->graphs.erase(it); }
-    else ++it;
-  }
+  if (int rc = ring_quiesce(rb)) return rc;
+  const size_t nl = (size_t)h->R * rb->cap;
+  RingAlloc al;
+  int* link = al.device<int>(nl, 0xff);
+  int* nstep = al.device(std::vector<int>((size_t)h->R, 1));
+  long long* f_idx = al.device<long long>(kNstepChunk);
+  float* f_rows = al.device<float>(kNstepChunk * (size_t)h->row_stride);
+  float* f_disc = al.device<float>(kNstepChunk);
+  int* f_m = al.device<int>(kNstepChunk);
+  cudaEvent_t ev = al.event();
+  float* ns_buf = h->ns_buf ? h->ns_buf : al.device<float>((size_t)3 * h->R * h->cfg.batch, 0);   // with the first linked ring
+  if (!al.commit()) return fail(B200SAC_ERR_NOMEM, "trajectory link allocation failed");
+  drop_ring_graphs(h, rb);                         // they hold the unlinked gather
   h->ns_buf = ns_buf;
   rb->d_link = link; rb->d_nstep = nstep; rb->f_idx = f_idx; rb->f_rows = f_rows; rb->f_disc = f_disc; rb->f_m = f_m; rb->ev_nstep = ev;
   rb->nstep_host.assign((size_t)h->R, 1);
@@ -3646,7 +3676,7 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
 }
 
 extern "C" int b200sac_replay_close_streams(b200sac_replay_t* rb, int32_t replica, int64_t n, const int32_t* stream) {
-  if (int rc = traj_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (n < 0 || (n > 0 && !stream)) return fail(B200SAC_ERR_INVALID, "bad argument");
   for (int64_t i = 0; i < n; ++i)
     if (stream[i] < 0 || stream[i] >= 65536) return fail(B200SAC_ERR_INVALID, "stream id %d outside [0, 65536)", stream[i]);
@@ -3659,7 +3689,7 @@ extern "C" int b200sac_replay_close_streams(b200sac_replay_t* rb, int32_t replic
 }
 
 extern "C" int b200sac_replay_set_nstep(b200sac_replay_t* rb, int32_t replica, int32_t n, void* stream) {
-  if (int rc = traj_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (n < 1 || n > kNstepMax) return fail(B200SAC_ERR_INVALID, "n-step horizon must be in [1, %d] (got %d)", kNstepMax, n);
   CU(cudaSetDevice(rb->h->device));
   StreamBridge sb(rb->h, stream);
@@ -3673,14 +3703,14 @@ extern "C" int b200sac_replay_set_nstep(b200sac_replay_t* rb, int32_t replica, i
 }
 
 extern "C" int b200sac_replay_get_nstep(b200sac_replay_t* rb, int32_t replica, int32_t* n) {
-  if (int rc = traj_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (!n) return fail(B200SAC_ERR_INVALID, "null argument");
   *n = rb->nstep_host[(size_t)replica];
   return 0;
 }
 
 extern "C" int b200sac_replay_get_links(b200sac_replay_t* rb, int32_t replica, int32_t task, int64_t n, int32_t* out) {
-  if (int rc = traj_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (task < 0 || task >= rb->Teff) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
   if (!out || n != rb->cap_per_task) return fail(B200SAC_ERR_INVALID, "a sub-ring has %lld slots (got n = %lld)", rb->cap_per_task, (long long)n);
   CU(cudaSetDevice(rb->h->device));
@@ -3693,20 +3723,17 @@ extern "C" int b200sac_replay_get_links(b200sac_replay_t* rb, int32_t replica, i
 
 extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_t n_idx, const int64_t* idx, float* s, float* a,
                                    float* R, float* s2, float* d, float* disc, int32_t* m) {
-  if (int rc = traj_check(rb, replica)) return rc;
+  if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (n_idx < 0 || (n_idx > 0 && (!idx || !s || !a || !R || !s2 || !d || !disc || !m))) return fail(B200SAC_ERR_INVALID, "bad argument");
   b200sac* h = rb->h;
   const int obs = h->K.obs, A = h->K.act, rs = h->row_stride;
   CU(cudaSetDevice(h->device));
   std::lock_guard<std::mutex> lk(rb->mu);
-  for (int64_t i = 0; i < n_idx; ++i) {
-    const long long k = idx[i];
-    if (k < 0 || k >= rb->cap) return fail(B200SAC_ERR_INVALID, "index %lld outside the ring [0, %lld)", k, rb->cap);
-    if (k % rb->cap_per_task >= rb->fill[(size_t)replica * rb->Teff + k / rb->cap_per_task])
-      return fail(B200SAC_ERR_INVALID, "index %lld is an empty slot", k);
-  }
+  for (int64_t i = 0; i < n_idx; ++i)
+    if (int rc = filled_slot(rb, replica, idx[i])) return rc;
   CU(cudaStreamWaitEvent(rb->st, rb->ev_nstep, 0));
   std::vector<float> rows((size_t)kNstepChunk * rs);
+  float* const f[ROW_FIELDS] = {s, a, R, s2, d};
   for (int64_t i0 = 0; i0 < n_idx; i0 += kNstepChunk) {
     const int c = (int)std::min<int64_t>(kNstepChunk, n_idx - i0);
     CU(cudaMemcpyAsync(rb->f_idx, idx + i0, c * sizeof(long long), cudaMemcpyHostToDevice, rb->st));
@@ -3718,14 +3745,7 @@ extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_
     CU(cudaMemcpyAsync(disc + i0, rb->f_disc, c * sizeof(float), cudaMemcpyDeviceToHost, rb->st));
     CU(cudaMemcpyAsync(m + i0, rb->f_m, c * sizeof(int), cudaMemcpyDeviceToHost, rb->st));
     CU(cudaStreamSynchronize(rb->st));
-    for (int i = 0; i < c; ++i) {
-      const float* src = rows.data() + (size_t)i * rs;
-      memcpy(s + (size_t)(i0 + i) * obs, src, obs * sizeof(float));
-      memcpy(a + (size_t)(i0 + i) * A, src + obs, A * sizeof(float));
-      R[i0 + i] = src[obs + A];
-      memcpy(s2 + (size_t)(i0 + i) * obs, src + obs + A + 1, obs * sizeof(float));
-      d[i0 + i] = src[2 * obs + A + 1];
-    }
+    unpack_rows(h, rows.data(), c, f, i0);
   }
   return 0;
 }

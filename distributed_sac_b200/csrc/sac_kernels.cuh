@@ -148,30 +148,6 @@ B200_D void bump_counters(const IngestOut& O, int rep, double beta1, double beta
   c->sched = (act ? SCHED_ACTOR : 0) | (tgt ? SCHED_TARGET : 0);
 }
 
-// minibatch given as five separate arrays [R][B][w]
-__global__ void ingest_split_kernel(StepConst K, IngestOut O, const float* __restrict__ s,
-                                    const float* __restrict__ a, const float* __restrict__ r,
-                                    const float* __restrict__ s2, const float* __restrict__ d,
-                                    const float* __restrict__ eps_next, const float* __restrict__ eps_cur) {
-  KStamp ks_;
-  const int rep = blockIdx.y;
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, wpb = blockDim.x / 32;
-  const int B = K.B;
-  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O, rep, K.beta1, K.beta2);
-  if (blockIdx.x == gridDim.x - 1) snapshot_alpha(K, O, rep, threadIdx.x);
-  for (int i = blockIdx.x * wpb + warp; i < B; i += gridDim.x * wpb) {
-    const long long ri = (long long)rep * B + i;
-    ingest_row(K, O, rep, i, s + ri * K.obs, a + ri * K.act, r[ri], s2 + ri * K.obs, d[ri], lane, 32);
-    if (eps_next != nullptr) {
-      float* E = O.eps + rep * O.rsEps;
-      for (int j = lane; j < K.act; j += 32) {
-        E[(long long)i * K.act + j] = eps_next[ri * K.act + j];
-        E[(long long)(B + i) * K.act + j] = eps_cur[ri * K.act + j];
-      }
-    }
-  }
-}
-
 // minibatch given as packed rows [s | a | r | s2 | d] (+pad), either gathered through idx
 // (device replay ring) or dense (pinned-host staging after the H2D copy).
 __global__ void ingest_rows_kernel(StepConst K, IngestOut O, const float* __restrict__ rows, long long rs_rows,

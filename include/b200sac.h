@@ -311,7 +311,9 @@ int b200sac_replay_destroy(b200sac_replay_t* rb);
 int b200sac_replay_push(b200sac_replay_t* rb, int32_t replica, int64_t n, const float* s, const float* a,
                         const float* r, const float* s2, const float* d);
 /* Fill every replica's ring with `n` synthetic transitions generated on the device
- * (s,s'~N(0,1), a~U(-1,1), r~N(0,1), d~Bernoulli(0.01), task = i mod T). Benchmark helper. */
+ * (s,s'~N(0,1), a~U(-1,1), r~N(0,1), d~Bernoulli(0.01), task = i mod T). Benchmark helper.
+ * Like push, it waits for the gathers of the steps already enqueued before it rewrites the ring, and is thread-safe
+ * against one concurrent sampler.  Synchronises the stream. */
 int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, uint64_t seed, void* stream);
 /* min over tasks of the per-task fill, like ReplayBuffer.__len__ in the MT variant. */
 int b200sac_replay_size(b200sac_replay_t* rb, int32_t replica, int64_t* n);
