@@ -10,8 +10,8 @@
 
 #include <algorithm>
 #include <cmath>
-#include <functional>
 #include <map>
+#include <memory>
 #include <mutex>
 #include <new>
 #include <random>
@@ -20,6 +20,7 @@
 #include <type_traits>
 #include <unordered_map>
 #include <unordered_set>
+#include <utility>
 #include <vector>
 
 #include "../../include/b200sac.h"
@@ -46,15 +47,46 @@ static int fail(int code, const char* fmt, ...) {
   va_end(ap);
   return code;
 }
+// A failed call returns B200SAC_ERR_NOMEM when it ran out of memory, B200SAC_ERR_CUDA otherwise.  Its error is taken off
+// cudaGetLastError, so that the launch check of a later call does not report it again.
 #define CU(call)                                                                                     \
   do {                                                                                               \
     cudaError_t e__ = (call);                                                                        \
-    if (e__ != cudaSuccess)                                                                          \
-      return fail(B200SAC_ERR_CUDA, "%s failed: %s (%s:%d)", #call, cudaGetErrorString(e__), __FILE__, __LINE__); \
+    if (e__ != cudaSuccess) {                                                                        \
+      cudaGetLastError();                                                                            \
+      return fail(e__ == cudaErrorMemoryAllocation ? B200SAC_ERR_NOMEM : B200SAC_ERR_CUDA, "%s failed: %s (%s:%d)", #call, \
+                  cudaGetErrorString(e__), __FILE__, __LINE__);                                      \
+    }                                                                                                \
   } while (0)
 
 extern "C" const char* b200sac_last_error(void) { return g_err; }
 extern "C" const char* b200sac_version(void) { return "b200sac 0.1 (sm_90a)"; }
+
+// Sole owner of one CUDA resource (memory, event, stream, graph): released by Release when the owner is destroyed or
+// reset, and nowhere else.  put() hands the empty slot to the allocating call, e.g. CU(cudaMalloc(buf.put(), bytes)).
+template <class H, auto Release>
+class Own {
+ public:
+  Own() = default;
+  Own(Own&& o) noexcept : h_(std::exchange(o.h_, nullptr)) {}
+  Own& operator=(Own&& o) noexcept {
+    if (this != &o) { reset(); h_ = std::exchange(o.h_, nullptr); }
+    return *this;
+  }
+  ~Own() { reset(); }
+  H get() const { return h_; }
+  operator H() const { return h_; }
+  H* put() { reset(); return &h_; }
+  void reset() { if (h_) Release(std::exchange(h_, nullptr)); }
+ private:
+  H h_ = nullptr;
+};
+template <class T> using DevMem = Own<T*, cudaFree>;
+template <class T> using PinnedMem = Own<T*, cudaFreeHost>;
+using Event = Own<cudaEvent_t, cudaEventDestroy>;
+using Stream = Own<cudaStream_t, cudaStreamDestroy>;
+using Graph = Own<cudaGraph_t, cudaGraphDestroy>;
+using GraphExec = Own<cudaGraphExec_t, cudaGraphExecDestroy>;
 
 // ------------------------------------------------------------------------------------------
 // layout
@@ -278,16 +310,16 @@ struct b200sac {
   StepConst K;
   int R = 1;
   // arenas
-  float *params = nullptr, *adam_m = nullptr, *adam_v = nullptr, *grads = nullptr;
-  Counters* cnt = nullptr;
-  HParams* hp = nullptr;          // [R] per-replica hyperparameters (K.hp points here)
+  DevMem<float> params, adam_m, adam_v, grads;
+  DevMem<Counters> cnt;
+  DevMem<HParams> hp;             // [R] per-replica hyperparameters (K.hp points here)
   std::vector<b200sac_hparams> hp_host;   // host mirror of the values as given (b200sac_get_hparams does not synchronise)
-  int* ivl = nullptr;             // [R][2] update intervals (actor_every, target_every), read by the ingest
+  DevMem<int> ivl;                // [R][2] update intervals (actor_every, target_every), read by the ingest
   std::vector<int> ivl_host;      // host mirror (b200sac_get_update_intervals does not synchronise)
-  float* losses = nullptr;        // [kLossSlots][R][4]
+  DevMem<float> losses;           // [kLossSlots][R][4]
   long long host_steps = 0;       // steps enqueued so far
   // work slab
-  float* slab = nullptr;
+  DevMem<float> slab;
   size_t slab_floats = 0;
   Buf XA, XQ, XT, XP, r, d, tid, eps, pout, psave, act_out, logp, logstd, y, q, dq, lq, dqa, la, qmin, dxP,
       dout_dbg, dact_dbg, qt, qp, alpha;
@@ -301,30 +333,30 @@ struct b200sac {
   int care_row_w = 0, care_off_att = 0, care_off_ctx = 0;
   std::vector<Buf> hA, dhA;       // per actor hidden layer
   std::vector<Buf> hQ, hT, hP, dhQ;   // per critic hidden layer, [2][B][H]
-  GemmProb* d_probs = nullptr;
+  DevMem<GemmProb> d_probs;
   std::vector<GemmProb> h_probs;
-  TcProb* d_tprobs = nullptr;
+  DevMem<TcProb> d_tprobs;
   std::vector<TcProb> h_tprobs;
   std::vector<Launch> plan;
   IngestOut ing;
   int use_eps_buf_idx = -1;       // index of the policy launch in plan (its use_eps_buf flag varies)
   // split-K weight gradients: slices 1..gslices-1 of the gradient arena, [slice-1][R][trainable] (slice 0 = grads)
-  float* grads_x = nullptr;
+  DevMem<float> grads_x;
   int gslices = 1;
   unsigned long long act_calls = 0;     // b200sac_act invocations (noise stream selector)
   // graphs
-  std::map<GraphKey, cudaGraphExec_t> graphs;
+  std::map<GraphKey, GraphExec> graphs;
   // host staging for step_host / pinned replay
-  float* stage_h[2] = {nullptr, nullptr};
-  float* stage_d[2] = {nullptr, nullptr};
+  PinnedMem<float> stage_h[2];
+  DevMem<float> stage_d[2];
   size_t stage_floats = 0;
   int row_w = 0, row_stride = 0;
-  cudaStream_t side = nullptr;
-  cudaStream_t fork = nullptr;    // capture-time fork for the next step's index sampling (multi-step graphs)
-  cudaEvent_t ev_ingested = nullptr, ev_sampled = nullptr, ev_fork_src = nullptr, ev_fork_done = nullptr;
-  cudaStream_t own = nullptr;     // used when the caller hands us the legacy default stream (not capturable)
-  cudaEvent_t ev_in = nullptr, ev_out = nullptr;
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_consumed[2] = {nullptr, nullptr};
+  Stream side;
+  Stream fork;                    // capture-time fork for the next step's index sampling (multi-step graphs)
+  Event ev_ingested, ev_sampled, ev_fork_src, ev_fork_done;
+  Stream own;                     // used when the caller hands us the legacy default stream (not capturable)
+  Event ev_in, ev_out;
+  Event ev_copied[2], ev_consumed[2];
   int stage_slot = 0;
   bool stage_used[2] = {false, false};
   int prefetch_slot = -1;         // host-ring step_sampled: minibatch already drawn, gathered and in flight (H2D)
@@ -333,28 +365,34 @@ struct b200sac {
   // gathered from the arena by a kernel) and crosses PCIe as one copy on its own stream; the host never touches individual
   // tensors.  Two image slots: the caller may hand on blob k while blob k+1 (begun after the next step was enqueued) is
   // still landing
-  cudaStream_t pub = nullptr;
-  uint8_t* blob_d[2] = {nullptr, nullptr};
-  uint8_t* blob_h[2] = {nullptr, nullptr};
-  int* blob_src = nullptr;                // [blob_nf] arena index of payload float j
-  int* blob_dst = nullptr;                // [blob_nf] byte offset of payload float j inside the image
+  Stream pub;
+  DevMem<uint8_t> blob_d[2];
+  PinnedMem<uint8_t> blob_h[2];
+  DevMem<int> blob_src;                   // [blob_nf] arena index of payload float j
+  DevMem<int> blob_dst;                   // [blob_nf] byte offset of payload float j inside the image
   int64_t blob_bytes = 0, blob_nf = 0;
   int blob_replica = 0, blob_head = 0, blob_pending = 0;
-  cudaEvent_t ev_blob_snap[2] = {nullptr, nullptr}, ev_blob_done[2] = {nullptr, nullptr};
-  CUtensorMap* d_cmaps = nullptr; // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
+  Event ev_blob_snap[2], ev_blob_done[2];
+  DevMem<CUtensorMap> d_cmaps;    // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
                                   // weight-gradient operands [R][nw]
-  long long* chain_dbg = nullptr; // B200SAC_CHAIN_DBG=1: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
-  float* step_d = nullptr;        // b200sac_step: the caller's minibatch as packed rows [R][B][row_stride] (stable graph pointers)
-  float* loss_h = nullptr;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
+  DevMem<long long> chain_dbg;    // B200SAC_CHAIN_DBG=1: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
+  DevMem<float> step_d;           // b200sac_step: the caller's minibatch as packed rows [R][B][row_stride] (stable graph pointers)
+  PinnedMem<float> loss_h;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
   float* loss_h_dev = nullptr;    // its device-side address
   // prioritized replay (allocated with the first prioritized ring): [3][R][B] importance weights of the step, leaf values
   // the step wrote, its ring indices (int32); a forked stream for the priority update
-  float* per_buf = nullptr;
-  cudaStream_t per_fork = nullptr;
-  cudaEvent_t ev_per_src = nullptr, ev_per_done = nullptr;
+  DevMem<float> per_buf;
+  Stream per_fork;
+  Event ev_per_src, ev_per_done;
   // n-step returns (allocated with the first linked ring): [3][R][B] per-row discount of the step (K.disc), hops folded and
   // ring indices (int32), written by ingest_nstep_kernel
-  float* ns_buf = nullptr;
+  DevMem<float> ns_buf;
+
+  // The members release their resources; the publication stream's last copy lands first.
+  ~b200sac() {
+    cudaSetDevice(device);
+    if (pub) cudaStreamSynchronize(pub);
+  }
 };
 
 struct b200sac_replay {
@@ -362,40 +400,43 @@ struct b200sac_replay {
   int where = 0;
   long long cap = 0, cap_per_task = 0;
   int Teff = 1;
-  float* rows = nullptr;          // [R][cap][row_stride] device or pinned host
+  float* rows = nullptr;          // [R][cap][row_stride]: rows_dev (device ring) or rows_pinned (pinned-host ring)
+  DevMem<float> rows_dev;
+  PinnedMem<float> rows_pinned;
   long long rs_rows = 0;
   std::vector<long long> fill, head;   // [R][Teff]
-  long long* d_fill = nullptr;    // device copy (device ring)
-  int* d_idx = nullptr;           // [R][B]
+  DevMem<long long> d_fill;       // device copy (device ring)
+  DevMem<int> d_idx;              // [R][B]
   unsigned long long seed = 0;
   std::mt19937_64 rng;
   std::mutex mu;
-  cudaEvent_t ev_gather = nullptr;   // device ring: recorded after the last enqueued gather (pushes wait for it under `mu`)
+  Event ev_gather;                // device ring: recorded after the last enqueued gather (pushes wait for it under `mu`)
   bool gather_pending = false;
   // prioritized ring (per_kernels.cuh): sum-trees, per-replica beta, and what the synchronous calls work with
   bool per = false;
-  PerTree tr;
-  double* d_beta = nullptr;       // [R]
+  PerTree tr;                     // (tr.tree and tr.maxp point into tree and maxp)
+  DevMem<float> tree, maxp;
+  DevMem<double> d_beta;          // [R]
   std::vector<long long> draws;   // [R] b200sac_replay_sample_prioritized calls so far (its Philox counter)
-  cudaStream_t st = nullptr;      // device ring: push (and prioritized set / get / sample) work, synchronised before those calls return
-  long long* s_lidx = nullptr;    // scratch [kPerMaxB]
-  int* s_idx = nullptr;           // scratch [kPerMaxB]
-  float* s_f = nullptr;           // scratch [kPerMaxB]
-  float* s_rows = nullptr;        // scratch [B][row_stride]
+  Stream st;                      // device ring: push (and prioritized set / get / sample) work, synchronised before those calls return
+  DevMem<long long> s_lidx;       // scratch [kPerMaxB]
+  DevMem<int> s_idx;              // scratch [kPerMaxB]
+  DevMem<float> s_f;              // scratch [kPerMaxB]
+  DevMem<float> s_rows;           // scratch [B][row_stride]
   // trajectory links (nstep_kernels.cuh; b200sac_replay_enable_trajectories)
   bool traj = false;
-  int* d_link = nullptr;          // [R][cap] sub-ring-local slot of the successor, or -1
-  int* d_nstep = nullptr;         // [R] horizon
+  DevMem<int> d_link;             // [R][cap] sub-ring-local slot of the successor, or -1
+  DevMem<int> d_nstep;            // [R] horizon
   std::vector<int> nstep_host;    // host mirror (b200sac_replay_get_nstep does not synchronise)
   std::vector<int> link_h, pred_h;   // [R][cap] host mirror of link, and its inverse (sub-ring-local slot of the predecessor)
   std::vector<std::unordered_map<int, long long>> tail;      // [R] stream id -> ring index of the stream's open tail
   std::vector<std::unordered_map<long long, int>> tail_at;   // [R] its inverse
-  cudaEvent_t ev_nstep = nullptr; // recorded after the last set_nstep (b200sac_replay_fold waits for it)
-  int* f_at = nullptr;            // scratch [f_cap] x 2: link changes of one push (ring index, value)
+  Event ev_nstep;                 // recorded after the last set_nstep (b200sac_replay_fold waits for it)
+  DevMem<int> f_at;               // scratch [f_cap] x 2: link changes of one push (ring index, value)
   size_t f_cap = 0;
-  long long* f_idx = nullptr;     // fold scratch [kNstepChunk], with f_rows [kNstepChunk][row_stride], f_disc, f_m
-  float *f_rows = nullptr, *f_disc = nullptr;
-  int* f_m = nullptr;
+  DevMem<long long> f_idx;        // fold scratch [kNstepChunk], with f_rows [kNstepChunk][row_stride], f_disc, f_m
+  DevMem<float> f_rows, f_disc;
+  DevMem<int> f_m;
 };
 
 // Transition rows [s | a | r | s' | d], padded to row_stride floats: the format of the replay ring, the staging slots and
@@ -434,49 +475,6 @@ static Buf carve(size_t& cursor, size_t n_per_rep, int R) {
 }
 
 static void rebase(Buf& b, float* base) { b.p = base + (size_t)(uintptr_t)b.p / sizeof(float); }
-
-static int destroy_impl(b200sac* h) {
-  if (!h) return 0;
-  cudaSetDevice(h->device);
-  for (auto& kv : h->graphs) cudaGraphExecDestroy(kv.second);
-  cudaFree(h->params); cudaFree(h->adam_m); cudaFree(h->adam_v); cudaFree(h->grads); cudaFree(h->grads_x);
-  cudaFree(h->cnt); cudaFree(h->hp); cudaFree(h->ivl); cudaFree(h->losses); cudaFree(h->slab); cudaFree(h->d_probs); cudaFree(h->d_tprobs);
-  for (int i = 0; i < 2; ++i) {
-    if (h->stage_h[i]) cudaFreeHost(h->stage_h[i]);
-    cudaFree(h->stage_d[i]);
-    if (h->ev_copied[i]) cudaEventDestroy(h->ev_copied[i]);
-    if (h->ev_consumed[i]) cudaEventDestroy(h->ev_consumed[i]);
-  }
-  if (h->loss_h) cudaFreeHost(h->loss_h);
-  if (h->pub) { cudaStreamSynchronize(h->pub); cudaStreamDestroy(h->pub); }
-  for (int i = 0; i < 2; ++i) {
-    if (h->ev_blob_snap[i]) cudaEventDestroy(h->ev_blob_snap[i]);
-    if (h->ev_blob_done[i]) cudaEventDestroy(h->ev_blob_done[i]);
-    cudaFree(h->blob_d[i]);
-    if (h->blob_h[i]) cudaFreeHost(h->blob_h[i]);
-  }
-  cudaFree(h->blob_src);
-  cudaFree(h->blob_dst);
-  cudaFree(h->step_d);
-  cudaFree(h->chain_dbg);
-  cudaFree(h->d_cmaps);
-  cudaFree(h->per_buf);
-  cudaFree(h->ns_buf);
-  if (h->per_fork) cudaStreamDestroy(h->per_fork);
-  if (h->ev_per_src) cudaEventDestroy(h->ev_per_src);
-  if (h->ev_per_done) cudaEventDestroy(h->ev_per_done);
-  if (h->side) cudaStreamDestroy(h->side);
-  if (h->fork) cudaStreamDestroy(h->fork);
-  if (h->ev_ingested) cudaEventDestroy(h->ev_ingested);
-  if (h->ev_sampled) cudaEventDestroy(h->ev_sampled);
-  if (h->ev_fork_src) cudaEventDestroy(h->ev_fork_src);
-  if (h->ev_fork_done) cudaEventDestroy(h->ev_fork_done);
-  if (h->own) cudaStreamDestroy(h->own);
-  if (h->ev_in) cudaEventDestroy(h->ev_in);
-  if (h->ev_out) cudaEventDestroy(h->ev_out);
-  delete h;
-  return 0;
-}
 
 // ---- TMA tensor maps (driver entry point resolved at run time: no link-time libcuda dependency) ----
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -1116,7 +1114,7 @@ int PlanBuilder::build_plan_fused() {
   struct FMap { int64_t off; int K, N, ld; };
   std::vector<FMap> fmaps;                 // forward weight matrices that need a tensor map (one per chained forward stage)
   if (getenv("B200SAC_CHAIN_DBG")) {
-    CU(cudaMalloc(&h->chain_dbg, sizeof(long long) * CH_DBG_SLOTS * 16));
+    CU(cudaMalloc(h->chain_dbg.put(), sizeof(long long) * CH_DBG_SLOTS * 16));
     CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
   }
   auto dbg_slot = [&]() { return (h->chain_dbg && h->plan.size() < 16) ? h->chain_dbg + h->plan.size() * CH_DBG_SLOTS : nullptr; };
@@ -1336,7 +1334,7 @@ int PlanBuilder::build_plan_fused() {
                             wmaps[i].ld, WG_ROWS, true))
         return rc;
   }
-  CU(cudaMalloc(&h->d_cmaps, maps.size() * sizeof(CUtensorMap)));
+  CU(cudaMalloc(h->d_cmaps.put(), maps.size() * sizeof(CUtensorMap)));
   CU(cudaMemcpy(h->d_cmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
   const CUtensorMap* fmap = h->d_cmaps;
   const CUtensorMap* wmap = h->d_cmaps + (size_t)R * nf;
@@ -1659,12 +1657,12 @@ static int build_plan(b200sac* h) {
   if (pb.rc) return pb.rc;
   // upload problem tables and rebase
   if (!h->h_tprobs.empty()) {
-    CU(cudaMalloc(&h->d_tprobs, h->h_tprobs.size() * sizeof(TcProb)));
+    CU(cudaMalloc(h->d_tprobs.put(), h->h_tprobs.size() * sizeof(TcProb)));
     CU(cudaMemcpy(h->d_tprobs, h->h_tprobs.data(), h->h_tprobs.size() * sizeof(TcProb), cudaMemcpyHostToDevice));
     CU(tc_set_attrs());
   }
   if (!h->h_probs.empty()) {
-    CU(cudaMalloc(&h->d_probs, h->h_probs.size() * sizeof(GemmProb)));
+    CU(cudaMalloc(h->d_probs.put(), h->h_probs.size() * sizeof(GemmProb)));
     CU(cudaMemcpy(h->d_probs, h->h_probs.data(), h->h_probs.size() * sizeof(GemmProb), cudaMemcpyHostToDevice));
   }
   for (auto& l : h->plan) {
@@ -1710,7 +1708,7 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
 // Prioritized replay: the draw of one step (indices into rb->d_idx, importance weights into the handle's per_buf).
 static cudaError_t per_sample_on(b200sac* h, b200sac_replay* rb, cudaStream_t s) {
   return launch_k(per_sample_kernel, dim3(h->R), dim3(h->cfg.batch > 256 ? 512 : 256), 0, s, h->K, rb->tr, (const Counters*)h->cnt,
-                  0LL, 0, (const long long*)rb->d_fill, (const double*)rb->d_beta, rb->d_idx, h->per_buf, (long long)h->cfg.batch,
+                  0LL, 0, (const long long*)rb->d_fill, (const double*)rb->d_beta, rb->d_idx.get(), h->per_buf.get(), (long long)h->cfg.batch,
                   rb->seed);
 }
 
@@ -1721,7 +1719,7 @@ static bool forms_critic_loss(const Launch& l) { return l.kind == L_CHEADS || (l
 // runs after the critic-loss launch (forked off the critical path when allow_fork, joined before the step ends); per_next:
 // the next step's draw follows that update on the same stream (ev_sampled).  Linked ring -- the TD target discounts every
 // row with what the gather folded for it.
-static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, cudaEvent_t* evs = nullptr, bool allow_fork = false,
+static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* evs = nullptr, bool allow_fork = false,
                     b200sac_replay* rb = nullptr, bool per_next = false) {
   bool fork_pending = false, per_pending = false;
   b200sac_replay* per = rb && rb->per ? rb : nullptr;
@@ -1870,7 +1868,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   CU(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(B200SAC_ERR_INVALID, "device %d out of range (%d visible)", device, ndev);
   CU(cudaSetDevice(device));
-  b200sac* h = new (std::nothrow) b200sac();
+  std::unique_ptr<b200sac> owner(new (std::nothrow) b200sac());   // a failed create releases what it allocated
+  b200sac* h = owner.get();
   if (!h) return fail(B200SAC_ERR_NOMEM, "out of host memory");
   h->cfg = *cfg;
   h->device = device;
@@ -1896,38 +1895,27 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   K.beta1 = cfg->beta1; K.beta2 = cfg->beta2; K.adam_eps = cfg->adam_eps;
   K.seed = seed;
 
-#define CUH(call)                                                                                            \
-  do {                                                                                                       \
-    cudaError_t e__ = (call);                                                                                \
-    if (e__ != cudaSuccess) {                                                                                \
-      int rc__ = fail(e__ == cudaErrorMemoryAllocation ? B200SAC_ERR_NOMEM : B200SAC_ERR_CUDA, "%s failed: %s", #call, \
-                      cudaGetErrorString(e__));                                                              \
-      destroy_impl(h);                                                                                       \
-      return rc__;                                                                                           \
-    }                                                                                                        \
-  } while (0)
-
-  CUH(cudaMalloc(&h->params, sizeof(float) * L.arena * R));
-  CUH(cudaMalloc(&h->adam_m, sizeof(float) * L.trainable * R));
-  CUH(cudaMalloc(&h->adam_v, sizeof(float) * L.trainable * R));
-  CUH(cudaMalloc(&h->grads, sizeof(float) * L.trainable * R));
-  CUH(cudaMalloc(&h->cnt, sizeof(Counters) * R));
-  CUH(cudaMalloc(&h->losses, sizeof(float) * kLossSlots * R * 4));
-  CUH(cudaMemset(h->params, 0, sizeof(float) * L.arena * R));
-  CUH(cudaMemset(h->adam_m, 0, sizeof(float) * L.trainable * R));
-  CUH(cudaMemset(h->adam_v, 0, sizeof(float) * L.trainable * R));
-  CUH(cudaMemset(h->grads, 0, sizeof(float) * L.trainable * R));
+  CU(cudaMalloc(h->params.put(), sizeof(float) * L.arena * R));
+  CU(cudaMalloc(h->adam_m.put(), sizeof(float) * L.trainable * R));
+  CU(cudaMalloc(h->adam_v.put(), sizeof(float) * L.trainable * R));
+  CU(cudaMalloc(h->grads.put(), sizeof(float) * L.trainable * R));
+  CU(cudaMalloc(h->cnt.put(), sizeof(Counters) * R));
+  CU(cudaMalloc(h->losses.put(), sizeof(float) * kLossSlots * R * 4));
+  CU(cudaMemset(h->params, 0, sizeof(float) * L.arena * R));
+  CU(cudaMemset(h->adam_m, 0, sizeof(float) * L.trainable * R));
+  CU(cudaMemset(h->adam_v, 0, sizeof(float) * L.trainable * R));
+  CU(cudaMemset(h->grads, 0, sizeof(float) * L.trainable * R));
   h->gslices = (cfg->batch >= kSplitKMin && getenv("B200SAC_NO_SPLITK") == nullptr) ? kSplitK : 1;   // K of every weight gradient = batch
   if (h->gslices > 1) {     // never-written entries of slices >= 1 must read as zero (Adam sums all slices)
-    CUH(cudaMalloc(&h->grads_x, sizeof(float) * L.trainable * R * (h->gslices - 1)));
-    CUH(cudaMemset(h->grads_x, 0, sizeof(float) * L.trainable * R * (h->gslices - 1)));
+    CU(cudaMalloc(h->grads_x.put(), sizeof(float) * L.trainable * R * (h->gslices - 1)));
+    CU(cudaMemset(h->grads_x, 0, sizeof(float) * L.trainable * R * (h->gslices - 1)));
   }
   {
     std::vector<Counters> c0((size_t)R);
     for (auto& c : c0) { memset(&c, 0, sizeof(c)); for (int i = 0; i < 5; ++i) c.b1p[i] = c.b2p[i] = 1.0; }
-    CUH(cudaMemcpy(h->cnt, c0.data(), sizeof(Counters) * R, cudaMemcpyHostToDevice));
+    CU(cudaMemcpy(h->cnt, c0.data(), sizeof(Counters) * R, cudaMemcpyHostToDevice));
   }
-  CUH(cudaMemset(h->losses, 0, sizeof(float) * kLossSlots * R * 4));
+  CU(cudaMemset(h->losses, 0, sizeof(float) * kLossSlots * R * 4));
   {
     b200sac_hparams hp0;
     hp0.gamma = cfg->gamma; hp0.reward_scale = cfg->reward_scale; hp0.tau = cfg->tau;
@@ -1935,12 +1923,12 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     hp0.tau_se = cfg->tau_se; hp0.lr_ctx = cfg->lr_ctx;
     h->hp_host.assign((size_t)R, hp0);
     const std::vector<HParams> rows((size_t)R, hparams_row(hp0));
-    CUH(cudaMalloc(&h->hp, sizeof(HParams) * R));
-    CUH(cudaMemcpy(h->hp, rows.data(), sizeof(HParams) * R, cudaMemcpyHostToDevice));
+    CU(cudaMalloc(h->hp.put(), sizeof(HParams) * R));
+    CU(cudaMemcpy(h->hp, rows.data(), sizeof(HParams) * R, cudaMemcpyHostToDevice));
     K.hp = h->hp;
     h->ivl_host.assign((size_t)2 * R, 1);          // every step updates the actor and the targets
-    CUH(cudaMalloc(&h->ivl, sizeof(int) * 2 * R));
-    CUH(cudaMemcpy(h->ivl, h->ivl_host.data(), sizeof(int) * 2 * R, cudaMemcpyHostToDevice));
+    CU(cudaMalloc(h->ivl.put(), sizeof(int) * 2 * R));
+    CU(cudaMemcpy(h->ivl, h->ivl_host.data(), sizeof(int) * 2 * R, cudaMemcpyHostToDevice));
     K.cnt = h->cnt;
   }
 
@@ -2016,8 +2004,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     h->mixDZ = carve(cur, (size_t)Kenc * B * pitch(cfg->mix_out), R);
   }
   h->slab_floats = cur;
-  CUH(cudaMalloc(&h->slab, cur * sizeof(float)));
-  CUH(cudaMemset(h->slab, 0, cur * sizeof(float)));
+  CU(cudaMalloc(h->slab.put(), cur * sizeof(float)));
+  CU(cudaMemset(h->slab, 0, cur * sizeof(float)));
   for (Buf* b : {&h->XA, &h->XQ, &h->XT, &h->XP, &h->r, &h->d, &h->tid, &h->eps, &h->pout, &h->psave, &h->act_out, &h->logp,
                  &h->logstd, &h->y, &h->lq, &h->la, &h->qmin, &h->q, &h->dq, &h->dqa, &h->dxP, &h->dout_dbg, &h->dact_dbg, &h->qt, &h->qp, &h->alpha})
     rebase(*b, h->slab);
@@ -2030,10 +2018,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     for (auto* v : {&h->mixH[0], &h->mixH[1], &h->mixH[2], &h->mixDH})
       for (auto& b : *v) rebase(b, h->slab);
   }
-  if (h->q.rs != 2 * h->y.rs || h->dq.rs != 2 * h->y.rs || h->dqa.rs != 2 * h->y.rs || h->qt.rs != 2 * h->y.rs || h->qp.rs != 2 * h->y.rs) {
-    destroy_impl(h);
+  if (h->q.rs != 2 * h->y.rs || h->dq.rs != 2 * h->y.rs || h->dqa.rs != 2 * h->y.rs || h->qt.rs != 2 * h->y.rs || h->qp.rs != 2 * h->y.rs)
     return fail(B200SAC_ERR_INVALID, "internal: q stride");
-  }
 
   IngestOut& O = h->ing;
   O.XA = h->XA.p; O.XQ = h->XQ.p; O.XT = h->XT.p; O.XP = h->XP.p; O.r = h->r.p; O.d = h->d.p; O.eps = h->eps.p;
@@ -2042,10 +2028,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
   if (h->d.rs != h->r.rs || h->tid.rs != h->r.rs || h->lq.rs != h->y.rs || h->la.rs != h->y.rs || h->qmin.rs != h->y.rs ||
-      h->logstd.rs != h->logp.rs) {
-    destroy_impl(h);
+      h->logstd.rs != h->logp.rs)
     return fail(B200SAC_ERR_INVALID, "internal: stride mismatch");
-  }
 
   // parameter init: Xavier-uniform weights, zero biases, log_alpha = cfg; targets = locals
   {
@@ -2065,9 +2049,9 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     }
     std::vector<float> la((size_t)(cfg->num_tasks > 0 ? cfg->num_tasks : 1), (float)cfg->log_alpha_init);
     for (int rep = 0; rep < R; ++rep)
-      CUH(cudaMemcpy(h->params + (size_t)rep * L.arena + L.off_alpha, la.data(), la.size() * sizeof(float), cudaMemcpyHostToDevice));
+      CU(cudaMemcpy(h->params + (size_t)rep * L.arena + L.off_alpha, la.data(), la.size() * sizeof(float), cudaMemcpyHostToDevice));
     polyak_kernel<<<dim3(128, R), 256>>>(h->params + L.critic_begin, L.arena, L.critic_n, L.target_delta, 1.0f, 0.0f);
-    CUH(cudaGetLastError());
+    CU(cudaGetLastError());
   }
 
   // staging (pinned host <-> device), side stream
@@ -2075,35 +2059,35 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   h->row_stride = (h->row_w + 31) / 32 * 32;   // 128-byte aligned transition rows
   h->stage_floats = (size_t)R * B * h->row_stride + (size_t)2 * R * B * A;   // rows + eps_next/eps_cur
   for (int i = 0; i < 2; ++i) {
-    CUH(cudaMallocHost(&h->stage_h[i], h->stage_floats * sizeof(float)));
-    CUH(cudaMalloc(&h->stage_d[i], h->stage_floats * sizeof(float)));
-    CUH(cudaEventCreateWithFlags(&h->ev_copied[i], cudaEventDisableTiming));
-    CUH(cudaEventCreateWithFlags(&h->ev_consumed[i], cudaEventDisableTiming));
+    CU(cudaMallocHost(h->stage_h[i].put(), h->stage_floats * sizeof(float)));
+    CU(cudaMalloc(h->stage_d[i].put(), h->stage_floats * sizeof(float)));
+    CU(cudaEventCreateWithFlags(h->ev_copied[i].put(), cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(h->ev_consumed[i].put(), cudaEventDisableTiming));
   }
-  CUH(cudaHostAlloc(&h->loss_h, sizeof(float) * R * 4 * kLossSlots, cudaHostAllocMapped));
+  CU(cudaHostAlloc(h->loss_h.put(), sizeof(float) * R * 4 * kLossSlots, cudaHostAllocMapped));
   memset(h->loss_h, 0, sizeof(float) * R * 4 * kLossSlots);
-  CUH(cudaHostGetDevicePointer((void**)&h->loss_h_dev, h->loss_h, 0));
-  CUH(cudaStreamCreateWithFlags(&h->side, cudaStreamNonBlocking));
-  CUH(cudaStreamCreateWithFlags(&h->own, cudaStreamNonBlocking));
-  CUH(cudaStreamCreateWithFlags(&h->fork, cudaStreamNonBlocking));
-  CUH(cudaEventCreateWithFlags(&h->ev_ingested, cudaEventDisableTiming));
-  CUH(cudaEventCreateWithFlags(&h->ev_sampled, cudaEventDisableTiming));
-  CUH(cudaEventCreateWithFlags(&h->ev_fork_src, cudaEventDisableTiming));
-  CUH(cudaEventCreateWithFlags(&h->ev_fork_done, cudaEventDisableTiming));
-  CUH(cudaEventCreateWithFlags(&h->ev_in, cudaEventDisableTiming));
-  CUH(cudaEventCreateWithFlags(&h->ev_out, cudaEventDisableTiming));
+  CU(cudaHostGetDevicePointer((void**)&h->loss_h_dev, h->loss_h, 0));
+  CU(cudaStreamCreateWithFlags(h->side.put(), cudaStreamNonBlocking));
+  CU(cudaStreamCreateWithFlags(h->own.put(), cudaStreamNonBlocking));
+  CU(cudaStreamCreateWithFlags(h->fork.put(), cudaStreamNonBlocking));
+  CU(cudaEventCreateWithFlags(h->ev_ingested.put(), cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(h->ev_sampled.put(), cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(h->ev_fork_src.put(), cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(h->ev_fork_done.put(), cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(h->ev_in.put(), cudaEventDisableTiming));
+  CU(cudaEventCreateWithFlags(h->ev_out.put(), cudaEventDisableTiming));
 
   h->fused = fused_eligible(*cfg);
-  if (int rc = build_plan(h)) {
-    destroy_impl(h);
-    return rc;
-  }
-  CUH(cudaDeviceSynchronize());
-  *out = h;
+  if (int rc = build_plan(h)) return rc;
+  CU(cudaDeviceSynchronize());
+  *out = owner.release();
   return 0;
 }
 
-extern "C" int b200sac_destroy(b200sac_t* h) { return destroy_impl(h); }
+extern "C" int b200sac_destroy(b200sac_t* h) {
+  delete h;
+  return 0;
+}
 
 static int arena_of(b200sac* h, int which, float** p, int64_t* n) {
   switch (which) {
@@ -2331,22 +2315,35 @@ extern "C" int b200sac_blob_template(b200sac_t* h, int32_t replica, const uint8_
     if (dst_byte[j] < 0 || (int64_t)dst_byte[j] + 4 > image_bytes) return fail(B200SAC_ERR_INVALID, "payload float %lld lands outside the image", (long long)j);
   }
   CU(cudaSetDevice(h->device));
-  if (!h->pub) CU(cudaStreamCreateWithFlags(&h->pub, cudaStreamNonBlocking));
-  CU(cudaStreamSynchronize(h->pub));
-  for (int i = 0; i < 2; ++i) {
-    if (!h->ev_blob_snap[i]) CU(cudaEventCreateWithFlags(&h->ev_blob_snap[i], cudaEventDisableTiming));
-    if (!h->ev_blob_done[i]) CU(cudaEventCreateWithFlags(&h->ev_blob_done[i], cudaEventDisableTiming));
-    cudaFree(h->blob_d[i]); h->blob_d[i] = nullptr;
-    if (h->blob_h[i]) { cudaFreeHost(h->blob_h[i]); h->blob_h[i] = nullptr; }
-    CU(cudaMalloc(&h->blob_d[i], (size_t)image_bytes));
-    CU(cudaHostAlloc(&h->blob_h[i], (size_t)image_bytes, cudaHostAllocDefault));
-    CU(cudaMemcpy(h->blob_d[i], image, (size_t)image_bytes, cudaMemcpyHostToDevice));
+  // All or nothing: the stream and events are created once, together; the new images and index maps are built aside and
+  // replace the old ones only when all of them exist, so a failed call leaves the previous template working.
+  if (!h->pub) {
+    Stream pub;
+    Event snap[2], done[2];
+    CU(cudaStreamCreateWithFlags(pub.put(), cudaStreamNonBlocking));
+    for (int i = 0; i < 2; ++i) {
+      CU(cudaEventCreateWithFlags(snap[i].put(), cudaEventDisableTiming));
+      CU(cudaEventCreateWithFlags(done[i].put(), cudaEventDisableTiming));
+    }
+    h->pub = std::move(pub);
+    for (int i = 0; i < 2; ++i) { h->ev_blob_snap[i] = std::move(snap[i]); h->ev_blob_done[i] = std::move(done[i]); }
   }
-  cudaFree(h->blob_src); cudaFree(h->blob_dst); h->blob_src = h->blob_dst = nullptr;
-  CU(cudaMalloc(&h->blob_src, (size_t)n_floats * sizeof(int)));
-  CU(cudaMalloc(&h->blob_dst, (size_t)n_floats * sizeof(int)));
-  CU(cudaMemcpy(h->blob_src, src_index, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(h->blob_dst, dst_byte, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
+  DevMem<uint8_t> img_d[2];
+  PinnedMem<uint8_t> img_h[2];
+  DevMem<int> src, dst;
+  for (int i = 0; i < 2; ++i) {
+    CU(cudaMalloc(img_d[i].put(), (size_t)image_bytes));
+    CU(cudaHostAlloc(img_h[i].put(), (size_t)image_bytes, cudaHostAllocDefault));
+    CU(cudaMemcpy(img_d[i], image, (size_t)image_bytes, cudaMemcpyHostToDevice));
+  }
+  CU(cudaMalloc(src.put(), (size_t)n_floats * sizeof(int)));
+  CU(cudaMalloc(dst.put(), (size_t)n_floats * sizeof(int)));
+  CU(cudaMemcpy(src, src_index, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(dst, dst_byte, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
+  CU(cudaStreamSynchronize(h->pub));             // no copy of the old images is in flight
+  for (int i = 0; i < 2; ++i) { std::swap(h->blob_d[i], img_d[i]); std::swap(h->blob_h[i], img_h[i]); }
+  std::swap(h->blob_src, src);
+  std::swap(h->blob_dst, dst);
   h->blob_bytes = image_bytes; h->blob_nf = n_floats; h->blob_replica = replica;
   h->blob_head = 0; h->blob_pending = 0;
   return 0;
@@ -2403,7 +2400,7 @@ static NstepRing nstep_ring(const b200sac_replay* rb) {
   return N;
 }
 
-static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, cudaEvent_t* evs = nullptr,
+static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, const Event* evs = nullptr,
                         int sample_mode = SAMPLE_INLINE, bool fork_next = false) {
   if (evs) CU(cudaEventRecord(evs[0], st));
   const int B = h->cfg.batch, R = h->R;
@@ -2426,13 +2423,13 @@ static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, cudaEv
     auto sample_on = [&](cudaStream_t s2) {
       if (rb->per) return per_sample_on(h, rb, s2);
       return launch_k(sample_indices_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, s2, h->K,   // __launch_bounds__(512): 512 threads fit
-                      (const Counters*)h->cnt, (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx, (long long)B, rb->seed);
+                      (const Counters*)h->cnt, (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx.get(), (long long)B, rb->seed);
     };
     if (sample_mode == SAMPLE_INLINE) sample_on(st);
     else CU(cudaStreamWaitEvent(st, h->ev_sampled, 0));
     if (rb->traj)                               // linked ring: the same gather with the n-step fold in front of the scatter
       launch_k(ingest_nstep_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
-               (const int*)rb->d_idx, (long long)B, nstep_ring(rb), h->ns_buf);
+               (const int*)rb->d_idx, (long long)B, nstep_ring(rb), h->ns_buf.get());
     else
       launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
                (const int*)rb->d_idx, (long long)B);
@@ -2456,20 +2453,19 @@ static int get_graph(b200sac* h, cudaStream_t st, const GraphKey& key, cudaGraph
   auto it = h->graphs.find(key);
   if (it == h->graphs.end()) {
     const int nsteps = key.nsteps;
-    cudaGraph_t g = nullptr;
+    Graph g;
     CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
     int rc = 0;
     for (int k = 0; k < nsteps && rc == 0; ++k)
       rc = enqueue_body(h, st, key, nullptr, (nsteps > 1 && k > 0) ? SAMPLE_DONE : SAMPLE_INLINE, nsteps > 1 && k + 1 < nsteps);
-    cudaError_t e = cudaStreamEndCapture(st, &g);
-    if (rc) { if (g) cudaGraphDestroy(g); return rc; }
+    cudaError_t e = cudaStreamEndCapture(st, g.put());
+    if (rc) return rc;
     if (e != cudaSuccess) return fail(B200SAC_ERR_CUDA, "graph capture failed: %s", cudaGetErrorString(e));
-    cudaGraphExec_t ge = nullptr;
-    e = cudaGraphInstantiate(&ge, g, 0);
-    cudaGraphDestroy(g);
+    GraphExec ge;
+    e = cudaGraphInstantiate(ge.put(), g, 0);
     if (e != cudaSuccess) return fail(B200SAC_ERR_CUDA, "graph instantiate failed: %s", cudaGetErrorString(e));
     if (cudaGraphUpload(ge, st) != cudaSuccess) cudaGetLastError();    // best effort: first launch does not pay the upload
-    it = h->graphs.emplace(key, ge).first;
+    it = h->graphs.emplace(key, std::move(ge)).first;
   }
   *out = it->second;
   return 0;
@@ -2513,7 +2509,7 @@ extern "C" int b200sac_step(b200sac_t* h, const float* s, const float* a, const 
   // call.  The transitions become rows laid out like a staging slot's (the staged step's graph body), the noise goes
   // straight into the step's noise buffer.
   const size_t RB = (size_t)h->R * h->cfg.batch, nA = (size_t)h->cfg.batch * h->cfg.act_dim;
-  if (!h->step_d) CU(cudaMalloc(&h->step_d, RB * h->row_stride * sizeof(float)));
+  if (!h->step_d) CU(cudaMalloc(h->step_d.put(), RB * h->row_stride * sizeof(float)));
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   const RowFields F = row_fields(h);
@@ -2652,8 +2648,8 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   if (cap < n) return fail(B200SAC_ERR_INVALID, "need room for %d launches", n);
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
-  std::vector<cudaEvent_t> evs((size_t)n + 1);
-  for (auto& e : evs) CU(cudaEventCreate(&e));
+  std::vector<Event> evs((size_t)n + 1);
+  for (auto& e : evs) CU(cudaEventCreate(e.put()));
   std::vector<double> acc((size_t)n, 0.0);
   for (int it = 0; it < iters; ++it) {
     if (int rc = enqueue_body(h, sb.run, GraphKey{rb, rb->rows, nullptr, 1, h->stamping}, evs.data())) return rc;
@@ -2666,7 +2662,6 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
     }
   }
   for (int i = 0; i < n; ++i) out_ms[i] = (float)(acc[i] / iters);
-  for (auto& e : evs) cudaEventDestroy(e);
   if (names && names_cap > 0) {
     std::string s = "sample+ingest";
     for (auto& l : h->plan) { s += ";"; s += launch_name(l, h->h_probs, h->d_probs); }
@@ -2724,25 +2719,24 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   const int bn = tc_forced_bn(64);
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
-  TcProb* d = nullptr;
-  CU(cudaMalloc(&d, sizeof(TcProb)));
+  DevMem<TcProb> d;
+  CU(cudaMalloc(d.put(), sizeof(TcProb)));
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
-  cudaFree(d);
   if (e != cudaSuccess) return fail(B200SAC_ERR_CUDA, "gemm_tc_kernel failed: %s", cudaGetErrorString(e));
   return 0;
 }
 
 // clock64() timeline of CTA (0,0) of one warm wgmma GEMM launch (see TC_STAMP indices in gemm_tc.cuh).
 extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int32_t K, long long* out96) {
-  float *A = nullptr, *B = nullptr, *C = nullptr;
-  long long* dbg = nullptr;
+  DevMem<float> A, B, C;
+  DevMem<long long> dbg;
   const size_t na = (size_t)(mode == GEMM_WGRAD ? K * M : M * K), nb = (size_t)(mode == GEMM_FWD ? N * K : K * N);
-  CU(cudaMalloc(&A, na * 4)); CU(cudaMalloc(&B, nb * 4)); CU(cudaMalloc(&C, (size_t)M * N * 4)); CU(cudaMalloc(&dbg, 96 * 8));
+  CU(cudaMalloc(A.put(), na * 4)); CU(cudaMalloc(B.put(), nb * 4)); CU(cudaMalloc(C.put(), (size_t)M * N * 4)); CU(cudaMalloc(dbg.put(), 96 * 8));
   CU(cudaMemset(A, 0, na * 4)); CU(cudaMemset(B, 0, nb * 4)); CU(cudaMemset(dbg, 0, 96 * 8));
   GemmProb p;
   memset(&p, 0, sizeof(p));
@@ -2752,15 +2746,14 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   t.dbg = dbg;
-  TcProb* d = nullptr;
-  CU(cudaMalloc(&d, sizeof(TcProb)));
+  DevMem<TcProb> d;
+  CU(cudaMalloc(d.put(), sizeof(TcProb)));
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   for (int it = 0; it < 3; ++it) tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out96, dbg, 96 * 8, cudaMemcpyDeviceToHost));
-  cudaFree(A); cudaFree(B); cudaFree(C); cudaFree(dbg); cudaFree(d);
   return 0;
 }
 
@@ -2775,10 +2768,10 @@ extern "C" int b200sac_graph_timeline(b200sac_t* h, b200sac_replay_t* rb, int32_
   *n_out = n;
   if (cap < n) return fail(B200SAC_ERR_INVALID, "need room for %d launches", n);
   const int total = n * (iters + 1);
-  unsigned long long* dt = nullptr;
-  int* di = nullptr;
-  CU(cudaMalloc(&dt, sizeof(unsigned long long) * total));
-  CU(cudaMalloc(&di, sizeof(int)));
+  DevMem<unsigned long long> dt;
+  DevMem<int> di;
+  CU(cudaMalloc(dt.put(), sizeof(unsigned long long) * total));
+  CU(cudaMalloc(di.put(), sizeof(int)));
   CU(cudaMemset(di, 0, sizeof(int)));
   StampBuf sb_on = {dt, di, total}, sb_off = {nullptr, nullptr, 0};
   if (int rc = b200sac_step_sampled(h, rb, 5, stream)) return rc;     // warm (graph instantiated)
@@ -2792,7 +2785,6 @@ extern "C" int b200sac_graph_timeline(b200sac_t* h, b200sac_replay_t* rb, int32_
   if (rc) return rc;
   std::vector<unsigned long long> t((size_t)total);
   CU(cudaMemcpy(t.data(), dt, sizeof(unsigned long long) * total, cudaMemcpyDeviceToHost));
-  cudaFree(dt); cudaFree(di);
   for (int i = 0; i < n; ++i) {
     double acc = 0;
     for (int it = 0; it < iters; ++it) acc += (double)(t[(size_t)it * n + i + 1] - t[(size_t)it * n + i]);
@@ -2989,7 +2981,7 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   }
   else if (nm == "chain_dbg") {
     if (!h->chain_dbg) return fail(B200SAC_ERR_INVALID, "chain_dbg needs B200SAC_CHAIN_DBG=1 at create time");
-    src = reinterpret_cast<const float*>(h->chain_dbg); n = 2 * CH_DBG_SLOTS * 16;     // int64 stamps viewed as float pairs
+    src = reinterpret_cast<const float*>(h->chain_dbg.get()); n = 2 * CH_DBG_SLOTS * 16;     // int64 stamps viewed as float pairs
   }
   else {
     // hidden activations (the ReLU masks of the step): "hA.<l>" [2B][H] rows [s';s]; "hQ.<l>" / "hT.<l>" / "hP.<l>" [2][B][H]
@@ -3029,7 +3021,8 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
 //                enqueued by a step reads a torn row and no concurrent writer interleaves;
 //   samplers     ring_ready: every sub-ring a draw reads holds enough transitions;
 //   indices      filled_slot: a ring index the caller names holds a transition;
-//   allocation   RingAlloc: all pieces or none, committed to the ring / handle only when every one succeeded.
+//   allocation   all pieces or none: each goes into a local owner, and they move into the ring / handle only when every
+//                one exists.
 enum { RING_ANY, RING_PER, RING_TRAJ };
 static int ring_check(const b200sac_replay* rb, int32_t replica, int kind = RING_ANY) {
   if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
@@ -3068,49 +3061,10 @@ static int filled_slot(const b200sac_replay* rb, int replica, long long k) {
   return 0;
 }
 
-// All-or-nothing allocation: each piece goes into a local (optionally zero-filled with `byte`, or copied from a host
-// vector); unless commit() succeeds, the destructor releases every piece, so the caller stores them only after commit().
-struct RingAlloc {
-  bool ok = true;
-  std::vector<std::function<void()>> undo;
-  template <class T> T* device(size_t n, int byte = -1) {
-    T* p = nullptr;
-    if (!(ok = ok && cudaMalloc(&p, n * sizeof(T)) == cudaSuccess)) return nullptr;
-    undo.push_back([p] { cudaFree(p); });
-    ok = byte < 0 || cudaMemset(p, byte, n * sizeof(T)) == cudaSuccess;
-    return p;
-  }
-  template <class T> T* device(const std::vector<T>& v) {
-    T* p = device<T>(v.size());
-    ok = ok && cudaMemcpy(p, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice) == cudaSuccess;
-    return p;
-  }
-  float* pinned(size_t n) {
-    float* p = nullptr;
-    if ((ok = ok && cudaMallocHost(&p, n * sizeof(float)) == cudaSuccess)) undo.push_back([p] { cudaFreeHost(p); });
-    return p;
-  }
-  cudaEvent_t event() {
-    cudaEvent_t e = nullptr;
-    if ((ok = ok && cudaEventCreateWithFlags(&e, cudaEventDisableTiming) == cudaSuccess)) undo.push_back([e] { cudaEventDestroy(e); });
-    return e;
-  }
-  cudaStream_t stream() {
-    cudaStream_t s = nullptr;
-    if ((ok = ok && cudaStreamCreateWithFlags(&s, cudaStreamNonBlocking) == cudaSuccess)) undo.push_back([s] { cudaStreamDestroy(s); });
-    return s;
-  }
-  bool commit() {
-    if (ok) undo.clear(); else cudaGetLastError();
-    return ok;
-  }
-  ~RingAlloc() { for (auto& u : undo) u(); }
-};
-
 // Graphs that captured a ring's pointers (its gather) go when the ring goes or its gather changes.
 static void drop_ring_graphs(b200sac* h, const b200sac_replay* rb) {
   for (auto it = h->graphs.begin(); it != h->graphs.end();) {
-    if (it->first.ring == rb) { cudaGraphExecDestroy(it->second); it = h->graphs.erase(it); }
+    if (it->first.ring == rb) it = h->graphs.erase(it);
     else ++it;
   }
 }
@@ -3124,7 +3078,8 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
     return fail(B200SAC_ERR_INVALID, "capacity %lld too small for batch %d", (long long)capacity, h->cfg.batch);
   if ((long long)capacity > 0x7fffffffLL) return fail(B200SAC_ERR_INVALID, "capacity must fit in int32");
   CU(cudaSetDevice(h->device));
-  b200sac_replay* rb = new (std::nothrow) b200sac_replay();
+  std::unique_ptr<b200sac_replay> owner(new (std::nothrow) b200sac_replay());   // a failed create releases what it allocated
+  b200sac_replay* rb = owner.get();
   if (!rb) return fail(B200SAC_ERR_NOMEM, "out of host memory");
   rb->h = h; rb->where = where; rb->Teff = Teff;
   rb->cap_per_task = capacity / Teff;
@@ -3135,19 +3090,19 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
   rb->fill.assign((size_t)h->R * Teff, 0);
   rb->head.assign((size_t)h->R * Teff, 0);
   const size_t n = (size_t)h->R * rb->rs_rows;
-  RingAlloc al;                                    // (the ring is not handed out before commit: its fields are the locals)
-  rb->rows = where == 0 ? al.device<float>(n) : al.pinned(n);
   if (where == 0) {
-    rb->d_fill = al.device<long long>((size_t)h->R * Teff, 0);
-    rb->d_idx = al.device<int>((size_t)h->R * h->cfg.batch);
-    rb->ev_gather = al.event();
-    rb->st = al.stream();
+    CU(cudaMalloc(rb->rows_dev.put(), n * sizeof(float)));
+    rb->rows = rb->rows_dev;
+    CU(cudaMalloc(rb->d_fill.put(), (size_t)h->R * Teff * sizeof(long long)));
+    CU(cudaMemset(rb->d_fill, 0, (size_t)h->R * Teff * sizeof(long long)));
+    CU(cudaMalloc(rb->d_idx.put(), (size_t)h->R * h->cfg.batch * sizeof(int)));
+    CU(cudaEventCreateWithFlags(rb->ev_gather.put(), cudaEventDisableTiming));
+    CU(cudaStreamCreateWithFlags(rb->st.put(), cudaStreamNonBlocking));
+  } else {
+    CU(cudaMallocHost(rb->rows_pinned.put(), n * sizeof(float)));
+    rb->rows = rb->rows_pinned;
   }
-  if (!al.commit()) {
-    delete rb;
-    return fail(B200SAC_ERR_NOMEM, "replay allocation of %zu bytes failed", n * sizeof(float));
-  }
-  *out = rb;
+  *out = owner.release();
   return 0;
 }
 
@@ -3156,15 +3111,6 @@ extern "C" int b200sac_replay_destroy(b200sac_replay_t* rb) {
   cudaSetDevice(rb->h->device);
   if (rb->h->prefetch_rb == rb) { rb->h->prefetch_slot = -1; rb->h->prefetch_rb = nullptr; }
   drop_ring_graphs(rb->h, rb);
-  if (rb->where == 0) cudaFree(rb->rows); else cudaFreeHost(rb->rows);
-  cudaFree(rb->d_fill); cudaFree(rb->d_idx);
-  if (rb->ev_gather) cudaEventDestroy(rb->ev_gather);
-  cudaFree(rb->tr.tree); cudaFree(rb->tr.maxp); cudaFree(rb->d_beta);
-  cudaFree(rb->s_lidx); cudaFree(rb->s_idx); cudaFree(rb->s_f); cudaFree(rb->s_rows);
-  cudaFree(rb->d_link); cudaFree(rb->d_nstep); cudaFree(rb->f_at); cudaFree(rb->f_idx); cudaFree(rb->f_rows); cudaFree(rb->f_disc);
-  cudaFree(rb->f_m);
-  if (rb->ev_nstep) cudaEventDestroy(rb->ev_nstep);
-  if (rb->st) cudaStreamDestroy(rb->st);
   delete rb;
   return 0;
 }
@@ -3285,8 +3231,8 @@ static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const flo
     push_links(rb, replica, n, row_task, row_slot, d, stream, cut, touched);
     const size_t m = touched.size();
     if (m > rb->f_cap) {
-      cudaFree(rb->f_at); rb->f_at = nullptr; rb->f_cap = 0;
-      if (cudaMalloc(&rb->f_at, 2 * m * sizeof(int)) != cudaSuccess) return fail(B200SAC_ERR_NOMEM, "link scratch allocation failed");
+      rb->f_at.reset(); rb->f_cap = 0;
+      CU(cudaMalloc(rb->f_at.put(), 2 * m * sizeof(int)));
       rb->f_cap = m;
     }
     vals.resize(m);
@@ -3334,9 +3280,9 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   std::lock_guard<std::mutex> lk(rb->mu);
   if (int rc = ring_quiesce(rb)) return rc;
   float* dev_rows = rb->rows;
-  float* tmp = nullptr;
+  DevMem<float> tmp;
   if (rb->where == 1) {   // generate on the device, copy down into the pinned ring
-    CU(cudaMalloc(&tmp, (size_t)h->R * rb->rs_rows * sizeof(float)));
+    CU(cudaMalloc(tmp.put(), (size_t)h->R * rb->rs_rows * sizeof(float)));
     dev_rows = tmp;
   }
   CU(cudaMemsetAsync(dev_rows, 0, (size_t)h->R * rb->rs_rows * sizeof(float), st));
@@ -3346,7 +3292,6 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   if (rb->where == 1) {
     CU(cudaMemcpyAsync(rb->rows, tmp, (size_t)h->R * rb->rs_rows * sizeof(float), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    CU(cudaFree(tmp));
   }
   if (rb->per) {                                   // rows [0, per) of every sub-ring get the current max p, the rest are empty
     per_fill_kernel<<<dim3(rb->Teff, h->R), 1024, 0, st>>>(rb->tr, 0, 0, 0, rb->tr.P, per);
@@ -3507,6 +3452,7 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
                 "(alpha %g, eps %g)", std::pow(eps, alpha), alpha, eps);
   b200sac_replay_t* rb = nullptr;
   if (int rc = b200sac_replay_create(h, capacity, 0, seed, &rb)) return rc;
+  std::unique_ptr<b200sac_replay> owner(rb);       // not handed out yet: a failure below releases the whole ring
   rb->per = true;
   PerTree& tr = rb->tr;
   tr.cap = rb->cap_per_task; tr.T = rb->Teff; tr.alpha = alpha; tr.eps = eps;
@@ -3514,32 +3460,33 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
   while (tr.P < tr.cap) { tr.P <<= 1; ++tr.levels; }
   rb->draws.assign((size_t)h->R, 0);
   const size_t nt = (size_t)h->R * tr.T;
-  RingAlloc al;
-  float* tree = al.device<float>(nt * 2 * (size_t)tr.P, 0);
-  float* maxp = al.device(std::vector<float>(nt, 1.f));
-  double* d_beta = al.device(std::vector<double>((size_t)h->R, beta));
-  long long* s_lidx = al.device<long long>(kPerMaxB);
-  int* s_idx = al.device<int>(kPerMaxB);
-  float* s_f = al.device<float>(kPerMaxB);
-  float* s_rows = al.device<float>((size_t)h->cfg.batch * h->row_stride);
-  // the handle's step buffers, with its first prioritized ring
-  float* per_buf = h->per_buf;
-  cudaStream_t per_fork = h->per_fork;
-  cudaEvent_t ev_src = h->ev_per_src, ev_done = h->ev_per_done;
-  if (!per_buf) {
-    per_buf = al.device<float>((size_t)3 * h->R * h->cfg.batch, 0);
-    per_fork = al.stream();
-    ev_src = al.event();
-    ev_done = al.event();
+  const std::vector<float> maxp0(nt, 1.f);
+  const std::vector<double> beta0((size_t)h->R, beta);
+  CU(cudaMalloc(rb->tree.put(), nt * 2 * (size_t)tr.P * sizeof(float)));
+  CU(cudaMemset(rb->tree, 0, nt * 2 * (size_t)tr.P * sizeof(float)));
+  CU(cudaMalloc(rb->maxp.put(), nt * sizeof(float)));
+  CU(cudaMemcpy(rb->maxp, maxp0.data(), nt * sizeof(float), cudaMemcpyHostToDevice));
+  CU(cudaMalloc(rb->d_beta.put(), beta0.size() * sizeof(double)));
+  CU(cudaMemcpy(rb->d_beta, beta0.data(), beta0.size() * sizeof(double), cudaMemcpyHostToDevice));
+  CU(cudaMalloc(rb->s_lidx.put(), kPerMaxB * sizeof(long long)));
+  CU(cudaMalloc(rb->s_idx.put(), kPerMaxB * sizeof(int)));
+  CU(cudaMalloc(rb->s_f.put(), kPerMaxB * sizeof(float)));
+  CU(cudaMalloc(rb->s_rows.put(), (size_t)h->cfg.batch * h->row_stride * sizeof(float)));
+  tr.tree = rb->tree; tr.maxp = rb->maxp;
+  if (!h->per_buf) {                               // the handle's step buffers, with its first prioritized ring
+    const size_t nb = (size_t)3 * h->R * h->cfg.batch * sizeof(float);
+    DevMem<float> per_buf;
+    Stream per_fork;
+    Event ev_src, ev_done;
+    CU(cudaMalloc(per_buf.put(), nb));
+    CU(cudaMemset(per_buf, 0, nb));
+    CU(cudaStreamCreateWithFlags(per_fork.put(), cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(ev_src.put(), cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(ev_done.put(), cudaEventDisableTiming));
+    h->per_buf = std::move(per_buf); h->per_fork = std::move(per_fork);
+    h->ev_per_src = std::move(ev_src); h->ev_per_done = std::move(ev_done);
   }
-  if (!al.commit()) {
-    b200sac_replay_destroy(rb);
-    return fail(B200SAC_ERR_NOMEM, "prioritized replay: allocation failed");
-  }
-  tr.tree = tree; tr.maxp = maxp; rb->d_beta = d_beta;
-  rb->s_lidx = s_lidx; rb->s_idx = s_idx; rb->s_f = s_f; rb->s_rows = s_rows;
-  h->per_buf = per_buf; h->per_fork = per_fork; h->ev_per_src = ev_src; h->ev_per_done = ev_done;
-  *out = rb;
+  *out = owner.release();
   return 0;
 }
 
@@ -3653,19 +3600,30 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   CU(cudaSetDevice(h->device));
   if (int rc = ring_quiesce(rb)) return rc;
   const size_t nl = (size_t)h->R * rb->cap;
-  RingAlloc al;
-  int* link = al.device<int>(nl, 0xff);
-  int* nstep = al.device(std::vector<int>((size_t)h->R, 1));
-  long long* f_idx = al.device<long long>(kNstepChunk);
-  float* f_rows = al.device<float>(kNstepChunk * (size_t)h->row_stride);
-  float* f_disc = al.device<float>(kNstepChunk);
-  int* f_m = al.device<int>(kNstepChunk);
-  cudaEvent_t ev = al.event();
-  float* ns_buf = h->ns_buf ? h->ns_buf : al.device<float>((size_t)3 * h->R * h->cfg.batch, 0);   // with the first linked ring
-  if (!al.commit()) return fail(B200SAC_ERR_NOMEM, "trajectory link allocation failed");
+  const std::vector<int> nstep0((size_t)h->R, 1);
+  DevMem<int> link, nstep, f_m;
+  DevMem<long long> f_idx;
+  DevMem<float> f_rows, f_disc;
+  Event ev;
+  CU(cudaMalloc(link.put(), nl * sizeof(int)));
+  CU(cudaMemset(link, 0xff, nl * sizeof(int)));
+  CU(cudaMalloc(nstep.put(), nstep0.size() * sizeof(int)));
+  CU(cudaMemcpy(nstep, nstep0.data(), nstep0.size() * sizeof(int), cudaMemcpyHostToDevice));
+  CU(cudaMalloc(f_idx.put(), kNstepChunk * sizeof(long long)));
+  CU(cudaMalloc(f_rows.put(), kNstepChunk * (size_t)h->row_stride * sizeof(float)));
+  CU(cudaMalloc(f_disc.put(), kNstepChunk * sizeof(float)));
+  CU(cudaMalloc(f_m.put(), kNstepChunk * sizeof(int)));
+  CU(cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming));
+  if (!h->ns_buf) {                                // the handle's step buffer, with its first linked ring
+    const size_t nb = (size_t)3 * h->R * h->cfg.batch * sizeof(float);
+    DevMem<float> ns_buf;
+    CU(cudaMalloc(ns_buf.put(), nb));
+    CU(cudaMemset(ns_buf, 0, nb));
+    h->ns_buf = std::move(ns_buf);
+  }
   drop_ring_graphs(h, rb);                         // they hold the unlinked gather
-  h->ns_buf = ns_buf;
-  rb->d_link = link; rb->d_nstep = nstep; rb->f_idx = f_idx; rb->f_rows = f_rows; rb->f_disc = f_disc; rb->f_m = f_m; rb->ev_nstep = ev;
+  rb->d_link = std::move(link); rb->d_nstep = std::move(nstep); rb->f_idx = std::move(f_idx); rb->f_rows = std::move(f_rows);
+  rb->f_disc = std::move(f_disc); rb->f_m = std::move(f_m); rb->ev_nstep = std::move(ev);
   rb->nstep_host.assign((size_t)h->R, 1);
   rb->link_h.assign(nl, -1);
   rb->pred_h.assign(nl, -1);

@@ -55,8 +55,8 @@ extern "C" {
 typedef enum b200sac_status {
   B200SAC_OK = 0,
   B200SAC_ERR_INVALID = -1,   /* bad argument / unsupported shape */
-  B200SAC_ERR_CUDA = -2,      /* a CUDA runtime call failed */
-  B200SAC_ERR_NOMEM = -3,
+  B200SAC_ERR_CUDA = -2,      /* a CUDA runtime call failed for any other reason */
+  B200SAC_ERR_NOMEM = -3,     /* out of host memory, or a CUDA runtime call failed with cudaErrorMemoryAllocation */
   B200SAC_ERR_STATE = -4      /* call not valid in this state (e.g. replay too small) */
 } b200sac_status;
 
