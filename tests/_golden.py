@@ -233,8 +233,9 @@ def kink_checked_step(core, port, spec, batch, e1, e2, replica=0, care=False, st
     return out, flips
 
 
-def check_port_state(core, port, replica=0, tol=REL):
-    """CUDA state == port state to 1e-4 per tensor (parameters, targets, Adam moments), log_alpha to 1e-6."""
+def check_port_state(core, port, replica=0, tol=REL, params=True):
+    """CUDA state == port state to 1e-4 per tensor (parameters, targets, Adam moments), log_alpha to 1e-6.  params=False:
+    the Adam moments only, for a caller that checks the parameters through the gradients and the exact optimizer step."""
     from distributed_sac_b200 import _lib
     got, ref = core.get_named(_lib.PARAMS, replica), port.params()
     st = port.adam_state()
@@ -247,7 +248,9 @@ def check_port_state(core, port, replica=0, tol=REL):
         errs = [rel_l2(got[k], v)]
         if k in st["m"]:
             errs += [rel_l2(gm[k], st["m"][k]), rel_l2(gv[k], st["v"][k])]
-        if max(errs) > tol:
+        if not params:
+            errs = errs[1:]
+        if errs and max(errs) > tol:
             bad.append((k, errs))
     assert not bad, f"state differs beyond {tol} with the CUDA masks forced into the oracle: {[(k, [float(f"{e:.1e}") for e in es]) for k, es in bad]}"
 

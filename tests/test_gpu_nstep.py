@@ -16,6 +16,7 @@ import redis_stub
 import sac_port as sp
 from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks,
                      rel_scalar, sync_core_to_port)
+from test_gpu_adam_exact import capture_grads, check_adam, check_grads, new_model, snapshot
 from test_oracle_nstep import _play, random_pushes
 
 pytestmark = pytest.mark.gpu
@@ -200,7 +201,7 @@ def test_fold_of_every_slot_equals_reference(cuda, name, cap, n_rows):
 
 # ---- 4. the step trains on the fold ------------------------------------------------------------------------------------
 @pytest.mark.parametrize("name,prioritized", [("chained", None), ("chained", PER), ("per_layer_p0", None), ("per_layer_p1", None),
-                                              ("mtsac_p0", None)])
+                                              ("mtsac", None), ("mtsac_p0", None)])
 def test_step_matches_oracle_on_the_folded_minibatch(cuda, name, prioritized):
     """With n = 3 and 5 the step's "r", "d", "disc", "nstep_m" equal the fold of its own "idx", and the step matches the
     autograd oracle fed the folded minibatch and the per-row discount (CUDA masks forced, kinks proven) at 1e-4: losses, y,
@@ -209,11 +210,16 @@ def test_step_matches_oracle_on_the_folded_minibatch(cuda, name, prioritized):
     core = _core(spec, care, precision)
     rb, mirror = _ring(core, spec, care, 4096, 4096, prioritized=None if prioritized is None else dict(PER, beta=1.0))
     port = sp.PortLearner(spec, sp.init_params(spec, seed=3))
+    ref_grads = capture_grads(port)
+    model = new_model(core)
     B, A = spec.batch, spec.act_dim
     for step, n in enumerate((3, 5, 3)):
         rb.set_nstep(n)
         sync_core_to_port(core, port)
+        model[0].seed(list(core.get_steps()) + [0])
+        before = snapshot(core, 0)
         core.step_sampled(rb, 1)
+        act = model[0].bump()
         idx = core.debug("idx").long().numpy()
         batch, disc, m = mirror.fold_batch(idx, n, spec.gamma)
         assert np.array_equal(core.debug("r").numpy(), batch[2].reshape(-1).numpy())
@@ -237,7 +243,14 @@ def test_step_matches_oracle_on_the_folded_minibatch(cuda, name, prioritized):
         for key in ("y", "q1", "q2", "logp_next"):
             got, ref = core.debug(key), out[key].reshape(-1)
             assert float((got - ref).abs().max()) <= REL * (float(ref.abs().max()) + 1.0), (name, step, key)
-        check_port_state(core, port)
+        # the gradients the step consumed against the oracle's, and the optimizer step bit for bit
+        check_grads(core, ref_grads, f"{name} step {step}")
+        check_adam(core, model, 0, before, snapshot(core, 0, True), act, f"{name} step {step}")
+        # The parameters themselves are compared only where Adam's g / (|g| + eps) map is well conditioned.  On 3xTF32 the
+        # MTSAC run starts from zero biases, so after its first step a bias IS the update, and q2.1.bias[100] has
+        # |g| = 1.29e-9 ~ eps/8: a gradient 1.7e-11 from the oracle's (that tensor passes the gradient check) moves its update
+        # from 3.48e-5 to 3.44e-5 and the tensor to 1.3e-4 from the oracle.  The two checks above cover it exactly.
+        check_port_state(core, port, params=name != "mtsac")
         if prioritized:
             y, q1, q2 = (out[k].reshape(-1).double() for k in ("y", "q1", "q2"))
             want_p = (((y - q1).abs() + (y - q2).abs()) / 2 + PER["eps"]) ** PER["alpha"]
