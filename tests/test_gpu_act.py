@@ -7,15 +7,9 @@ import torch
 
 import sac_port as sp
 from _golden import Case, REL, core_config, rel_l2
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 @pytest.mark.parametrize("precision", [0, 1], ids=["fp32", "tc3xtf32"])

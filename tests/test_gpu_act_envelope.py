@@ -20,10 +20,8 @@ import torch
 
 import care_port as cp
 import sac_port as sp
-from _golden import REL, CareCase, care_core_config, check_forced, core_config
-from test_gpu_chain_envelope import CASES as CHAIN_CASES, _params
-from test_gpu_hparams import _inputs
-from test_gpu_layer_envelope import CASES as LAYER_CASES, REPLICA_SPEC, REPLICAS
+from _golden import REL, check_forced, core_config
+from _harness import CHAIN_CASES, LAYER_CASES, REPLICA_SPEC, REPLICAS, _core, _inputs, _params, _plan, cuda
 
 gpu = pytest.mark.gpu
 
@@ -35,15 +33,6 @@ ACT_CASES.update({f"layer_{k}_{tag}": (v, p, 1) for k, v in LAYER_CASES.items() 
 ACT_CASES["replicas3"] = (REPLICA_SPEC, 1, REPLICAS)
 
 MODES = ("eps", "det", "mu", "fresh")          # injected noise, k tanh(mu), k mu, fresh Philox noise
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def row_counts(B):
@@ -258,19 +247,13 @@ def test_cases_reach_every_act_branch():
 # ---------------------------------------------------------------------------------------------------------------------
 # 4: acting never changes training, bit for bit
 # ---------------------------------------------------------------------------------------------------------------------
-VS_LIKE = dict(state_dim=39, num_tasks=0, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=300)
-MT10 = dict(state_dim=39, num_tasks=10, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=320,
-            weighted_loss=True)
-NI_PLANS = {"chained_ll": (sp.ll_spec().to_json(), 0), "vs400_tc": (VS_LIKE, 1), "mtsac_t10": (MT10, 1),
-            "care_m": ("care_small_s4", 1), "care_o": ("care_o_small_s4", 1)}
+NI_PLANS = ["chained_ll", "vs400_tc", "mtsac_t10", "care_m", "care_o"]         # _harness._plan ids
 
 
 def _ni_handle(name, R):
-    from distributed_sac_b200.core import Replay, SacCore
-    what, precision = NI_PLANS[name]
-    care = isinstance(what, str)
-    spec = CareCase(what).spec if care else sp.SacSpec(**what)
-    core = SacCore((care_core_config if care else core_config)(spec, replicas=R, precision=precision), 0, seed=4)
+    from distributed_sac_b200.core import Replay
+    spec, care, precision = _plan(name)
+    core = _core(spec, care, precision, R, seed=4)
     for r in range(R):
         core.set_named((cp if care else sp).init_params(spec, seed=20 + r), PARAMS, r)
     cap = 8 * spec.batch
@@ -282,7 +265,7 @@ def _ni_handle(name, R):
 
 
 @gpu
-@pytest.mark.parametrize("name", list(NI_PLANS))
+@pytest.mark.parametrize("name", NI_PLANS)
 def test_acting_never_changes_training(cuda, name):
     R = 2
     plain, spec, care, rings_p = _ni_handle(name, R)

@@ -19,209 +19,21 @@ Bit-exactness on top of wrong gradients would prove nothing, so the first checke
 with the gradients the oracle's optimizers consume (captured at each optimizer's step(), CUDA masks forced) at 1e-4 per
 tensor.  The CPU test at the end ties adam_expect to torch.optim.Adam, the reference's optimizer.
 """
-import math
-
 import numpy as np
 import pytest
 import torch
 
 import care_port as cp
 import sac_port as sp
-import test_gpu_targets_exact as te
-from _golden import REL, care_core_config, core_config, kink_checked_step, rel_l2
-from test_gpu_hparams import ROWS, _inputs
-from test_gpu_targets_exact import LL_CFG, _bits, _learner, export
-
-ADAM_M, ADAM_V, GRADS = 1, 2, 3
-SLOT_OF_OPT = {0: 0, 1: 1, 2: 2, 3: 4}          # layout table "opt" -> Counters slot
-LR_OF_SLOT = {0: "lr_critic", 1: "lr_actor", 2: "lr_alpha", 4: "lr_ctx"}
-SLOT_NAME = {0: "critic", 1: "actor", 2: "temperature", 4: "context encoder"}
-
-MT64 = dict(state_dim=17, num_tasks=64, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=320,
-            weighted_loss=True)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the specification
-# ---------------------------------------------------------------------------------------------------------------------
-def adam_expect(p, m, v, g, lr, b1p, b2p, beta1=0.9, beta2=0.999, eps=1e-8, mode="fp32"):
-    """(p', m', v') of adam_scalars + adam_one: step_size = f32(lr / (1 - b1p)) and bc2_sqrt = f32(sqrt(1 - b2p)) in fp64,
-    then m' = m + w1*(g - m), v' = v*b2 + (omb2*g)*g, p' = p - step_size*(m' / (sqrtf(v')/bc2_sqrt + eps)), one fp32
-    rounding per operation.  mode "fp64": the same formula evaluated in fp64 and rounded once; mode "fma": the multiply-adds
-    contracted (the two diagnostics a failing element is tested against)."""
-    f = np.float32
-    step_size, bc2_sqrt = f(lr / (1.0 - b1p)), f(math.sqrt(1.0 - b2p))
-    w1, b2, omb2, e = f(1.0 - beta1), f(beta2), f(1.0 - beta2), f(eps)
-    p, m, v, g = (np.asarray(x, dtype=np.float32) for x in (p, m, v, g))
-    if mode == "fp64":
-        d = np.float64
-        m1 = m + d(w1) * (g.astype(d) - m)
-        v1 = v * d(b2) + (d(omb2) * g) * g
-        p1 = p - d(step_size) * (m1 / (np.sqrt(v1) / d(bc2_sqrt) + d(e)))
-        return p1.astype(f), m1.astype(f), v1.astype(f)
-    if mode == "fma":
-        d = np.float64
-        m1 = (d(w1) * (g - m) + m).astype(f)
-        v1 = ((omb2 * g).astype(d) * g + v * b2).astype(f)
-        q = m1 / (np.sqrt(v1) / bc2_sqrt + e)
-        return (p.astype(d) - d(step_size) * q).astype(f), m1, v1
-    m1 = m + w1 * (g - m)
-    v1 = v * b2 + (omb2 * g) * g
-    p1 = p - step_size * (m1 / (np.sqrt(v1) / bc2_sqrt + e))
-    return p1, m1, v1
-
-
-class Counts:
-    """fp64 model of one replica's Counters: Adam step and bias-correction products per slot (0 critic, 1 actor,
-    2 temperature, 4 context encoder)."""
-
-    def __init__(self, beta1, beta2):
-        self.beta1, self.beta2 = beta1, beta2
-        self.t, self.b1p, self.b2p = [0] * 5, [1.0] * 5, [1.0] * 5
-
-    def seed(self, steps):
-        """b200sac_set_steps: (critic, actor, alpha, context encoder) -> glibc pow, as on the host side"""
-        for i, s in enumerate(steps):
-            slot = 4 if i == 3 else i
-            self.t[slot] = int(s)
-            self.b1p[slot], self.b2p[slot] = math.pow(self.beta1, s), math.pow(self.beta2, s)
-
-    def bump(self, actor_every=1):
-        """bump_counters: every slot but actor and temperature on a critic-only step; returns 'actor step'."""
-        n = self.t[0] + 1
-        act = actor_every == 1 or n % actor_every == 0
-        for i in range(5):
-            if act or i not in (1, 2):
-                self.t[i] += 1
-                self.b1p[i] *= self.beta1
-                self.b2p[i] *= self.beta2
-        return act
-
-    def copy(self):
-        c = Counts(self.beta1, self.beta2)
-        c.t, c.b1p, c.b2p = list(self.t), list(self.b1p), list(self.b2p)
-        return c
-
-    def steps(self, n):
-        return tuple(self.t[i] for i in (0, 1, 2, 4))[:n]
-
-
-def new_model(core):
-    return [Counts(core.cfg.beta1, core.cfg.beta2) for _ in range(core.cfg.replicas)]
+from _golden import kink_checked_step
+from _harness import (ADAM_M, ADAM_V, LEARNER_CFGS, ROWS, _bits, _handle, _inputs, _learner, adam_expect, capture_grads,
+                      check_adam, check_grads, cuda, new_model, snapshot)
 
 
 def set_steps(core, model, r, steps):
     core.set_steps(steps, r)
     got = core.get_steps(r)
     model[r].seed(list(got) + [0] * (4 - len(got)))      # set_steps reseeds every slot it does not name from its count
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the check
-# ---------------------------------------------------------------------------------------------------------------------
-def _slots(core):
-    """(slot of every trainable float, -1 in the gaps; [(name, offset, floats, slot)] of the trainable tensors)"""
-    if not hasattr(core, "_adam_slots"):
-        slot = np.full(core.trainable_floats, -1, np.int8)
-        tensors = []
-        for name, (off, rows, _cols, tr, opt, pitch) in core.table.items():
-            if tr:
-                slot[off:off + rows * pitch] = SLOT_OF_OPT[opt]
-                tensors.append((name, off, rows * pitch, SLOT_OF_OPT[opt]))
-        core._adam_slots = (slot, tensors)
-    return core._adam_slots
-
-
-def snapshot(core, r, with_grads=False):
-    """(p[:trainable], m, v[, GRADS]) of replica r as numpy arrays"""
-    T = core.trainable_floats
-    out = [export(core, r)[:T], core.export_arena(ADAM_M, r).numpy().copy(), core.export_arena(ADAM_V, r).numpy().copy()]
-    if with_grads:
-        out.append(core.export_arena(GRADS, r).numpy().copy())
-    return out
-
-
-def _slice0(core, r):
-    """The gradient arena without the extra split-K slices (b200sac_read_range reads slice 0 only)."""
-    from distributed_sac_b200 import _lib
-    from distributed_sac_b200.core import _ptr, _stream
-    out = torch.empty(core.trainable_floats)
-    _lib.check(core.lib.b200sac_read_range(core._h, GRADS, r, 0, core.trainable_floats, _ptr(out), _stream()))
-    return out.numpy()
-
-
-def _candidates(core, model, r, s, before, g, sel):
-    """{mistake: (p', m', v')} for the elements sel of slot s of replica r"""
-    cfg, c = core.cfg, model[r]
-    hp = core.get_hparams(r)
-    pb, mb, vb = (x[sel] for x in before)
-    ex = lambda lr, b1p, b2p, gg=None, mode="fp32": None if b1p >= 1.0 else adam_expect(    # (count 0: no step uses it)
-        pb, mb, vb, g[sel] if gg is None else gg, lr, b1p, b2p, cfg.beta1, cfg.beta2, cfg.adam_eps, mode)
-    lr, b1p, b2p = hp[LR_OF_SLOT[s]], c.b1p[s], c.b2p[s]
-    out = {"no update": (pb, mb, vb)}
-    for s2 in (0, 1, 2, 4):
-        if s2 != s:
-            out[f"the {SLOT_NAME[s2]} slot's rate and count"] = ex(hp[LR_OF_SLOT[s2]], c.b1p[s2], c.b2p[s2])
-            out[f"the {SLOT_NAME[s2]} slot's count"] = ex(lr, c.b1p[s2], c.b2p[s2])
-    for q in range(cfg.replicas):
-        if q != r:
-            out[f"replica {q}'s {LR_OF_SLOT[s]}"] = ex(core.get_hparams(q)[LR_OF_SLOT[s]], b1p, b2p)
-            out[f"replica {q}'s count"] = ex(lr, model[q].b1p[s], model[q].b2p[s])
-    out["count t - 1"] = ex(lr, b1p / cfg.beta1, b2p / cfg.beta2)
-    out["count t + 1"] = ex(lr, b1p * cfg.beta1, b2p * cfg.beta2)
-    out["pow(beta, t) instead of the running product"] = ex(lr, math.pow(cfg.beta1, c.t[s]), math.pow(cfg.beta2, c.t[s]))
-    out["the gradient without its split-K slices"] = ex(lr, b1p, b2p, _slice0(core, r)[sel])
-    out["fp64 evaluation"] = ex(lr, b1p, b2p, mode="fp64")
-    out["FMA-contracted evaluation"] = ex(lr, b1p, b2p, mode="fma")
-    return {k: c for k, c in out.items() if c is not None}
-
-
-def check_adam(core, model, r, before, after, act, what):
-    """Every trainable element of replica r after one step == adam_expect of its slot (actor and temperature untouched on
-    a critic-only step), p, m and v bit for bit; the gaps between tensors unchanged.  model[r] holds the counters the step
-    used (bumped).  Returns {slot: elements whose parameter moved}."""
-    cfg = core.cfg
-    slot, tensors = _slots(core)
-    hp = core.get_hparams(r)
-    got = after[:3]
-    g = after[3]
-    want = [np.empty_like(x) for x in before]
-    for s in (0, 1, 2, 4):
-        sel = slot == s
-        if not sel.any():
-            continue
-        if s in (1, 2) and not act:
-            res = [x[sel] for x in before]
-        else:
-            res = adam_expect(before[0][sel], before[1][sel], before[2][sel], g[sel], hp[LR_OF_SLOT[s]], model[r].b1p[s],
-                              model[r].b2p[s], cfg.beta1, cfg.beta2, cfg.adam_eps)
-        for w, x in zip(want, res):
-            w[sel] = x
-    gap = slot < 0
-    for w, b in zip(want, before):
-        w[gap] = b[gap]
-    bad = []
-    for name, off, n, s in tensors:
-        sl = slice(off, off + n)
-        diff = np.zeros(n, bool)
-        for x, w in zip(got, want):
-            diff |= _bits(x[sl]) != _bits(w[sl])
-        if not diff.any():
-            continue
-        sel = np.zeros(core.trainable_floats, bool)
-        sel[sl] = True
-        cands = _candidates(core, model, r, s, before, g, sel)
-        hit = [k for k, c in cands.items() if all(np.array_equal(_bits(x[sl]), _bits(y)) for x, y in zip(got, c))]
-        i = int(np.argmax(diff))
-        bad.append(f"{name} ({SLOT_NAME[s]} slot, t = {model[r].t[s]}, {LR_OF_SLOT[s]} = {hp[LR_OF_SLOT[s]]}; it got "
-                   f"{' / '.join(hit) or 'no candidate'}): {int(diff.sum())} of {n} elements differ, first [{i}] "
-                   f"g = {g[off + i]!r}: (p, m, v) = {tuple(float(x[off + i]) for x in got)} want "
-                   f"{tuple(float(w[off + i]) for w in want)}")
-    assert not bad, f"{what}: " + "; ".join(bad[:6])
-    changed = gap & ((_bits(got[0]) != _bits(before[0])) | (_bits(got[1]) != _bits(before[1])) |
-                     (_bits(got[2]) != _bits(before[2])))
-    assert not changed.any(), f"{what}: {int(changed.sum())} floats between tensors changed, first [{int(np.argmax(changed))}]"
-    return {s: int(((slot == s) & (got[0] != before[0])).sum()) for s in (0, 1, 2, 4) if (slot == s).any()}
 
 
 def plant_edges(core, r):
@@ -286,36 +98,6 @@ def _port_of(core, spec, care, r=0):
     return port
 
 
-def capture_grads(port):
-    """{name: gradient} as each optimizer's step() consumes it (the critic's before pi_loss.backward() adds to it)."""
-    grads = {}
-    names = {id(t): k for k, t in port.p.items()}
-    for opt in (port.opt_critic, port.opt_actor, port.opt_alpha, getattr(port, "opt_ctx", None)):
-        if opt is None:
-            continue
-
-        def step(*a, _opt=opt, _orig=opt.step, **kw):
-            for grp in _opt.param_groups:
-                for t in grp["params"]:
-                    grads[names[id(t)]] = torch.zeros_like(t) if t.grad is None else t.grad.detach().clone()
-            return _orig(*a, **kw)
-        opt.step = step
-    return grads
-
-
-def check_grads(core, ref, what, r=0):
-    """GRADS == the oracle's consumed gradients to 1e-4 per tensor (log_alpha: or 1e-6 absolute)."""
-    got = core.get_named(GRADS, r)
-    bad = []
-    for k, g in got.items():
-        assert k in ref, f"{what}: the oracle has no gradient for {k}"
-        err = rel_l2(g, ref[k].reshape(g.shape))
-        if err > REL and not (k == "log_alpha" and float((g - ref[k].reshape(g.shape)).abs().max()) <= 1e-6):
-            bad.append((k, float(f"{err:.2e}")))
-    assert not bad, f"{what}: gradients differ from the oracle's beyond {REL} (CUDA masks forced): {bad[:8]}"
-    return len(got)
-
-
 def oracle_checked_step(core, spec, care, model, i, what):
     """One step of replica 0 checked twice: GRADS against the oracle's consumed gradients, and the update exactly."""
     port = _port_of(core, spec, care)
@@ -333,37 +115,14 @@ def oracle_checked_step(core, spec, care, model, i, what):
 # ---------------------------------------------------------------------------------------------------------------------
 # 1: every plan and writer: counts of their own per slot, edge elements, gradients against the oracle
 # ---------------------------------------------------------------------------------------------------------------------
-SAC_PLANS = ["chained_ll", "chained_deep8", "chained_big_odd", "vs400_fp32", "vs400_tc", "split517_fp32", "split517_tc",
-             "wide1024_tc", "mtsac_t10", "mtsac_t64"]
-PLANS = SAC_PLANS + ["care_m", "care_o"]
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _make(name, R=1, rows=None):
-    """(core, spec, care): test_gpu_targets_exact's plans and parameters (targets off their locals), plus MTSAC at T = 64;
-    each replica its own parameters and, if given, its own hyperparameter row."""
-    from distributed_sac_b200.core import SacCore
-    spec, care, precision = (sp.SacSpec(**MT64), False, 1) if name == "mtsac_t64" else te._plan(name)
-    core = SacCore((care_core_config if care else core_config)(spec, replicas=R, precision=precision), 0, seed=0)
-    for r in range(R):
-        core.set_named(te._params(spec, care, seed=11 + 7 * r), 0, r)
-        if rows is not None:
-            core.set_hparams(r, **rows[r])
-    return core, spec, care
+PLANS = ["chained_ll", "chained_deep8", "chained_big_odd", "vs400_fp32", "vs400_tc", "split517_fp32", "split517_tc",
+         "wide1024_tc", "mtsac_t10", "mtsac_t64", "care_m", "care_o"]
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", PLANS)
 def test_adam_is_exact(cuda, name):
-    core, spec, care = _make(name)
+    core, spec, care = _handle(name)
     care_o = care and core.cfg.care_original
     model = new_model(core)
     checked_steps(core, spec, care, model, 2, f"{name} warm-up")
@@ -388,7 +147,7 @@ R3_COUNTS = [(10 ** 6, 7, 1, 0), (1, 0, 7, 10 ** 6), (7, 10 ** 6, 0, 1)]   # rep
 @pytest.mark.parametrize("name", R3_PLANS)
 def test_adam_is_exact_per_replica(cuda, name):
     rows = [dict(ROWS[0]), dict(ROWS[1], lr_critic=0.0, lr_actor=0.0, lr_alpha=0.0, lr_ctx=0.0), dict(ROWS[2])]
-    core, spec, care = _make(name, R=3, rows=rows)
+    core, spec, care = _handle(name, R=3, rows=rows)
     model = new_model(core)
     for r in range(3):
         set_steps(core, model, r, R3_COUNTS[r])
@@ -409,7 +168,7 @@ def test_adam_is_exact_per_replica(cuda, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["chained_ll", "vs400_tc", "split517_fp32", "mtsac_t10", "care_o"])
 def test_adam_is_exact_under_update_intervals(cuda, name):
-    core, spec, care = _make(name, R=2, rows=ROWS[:2])
+    core, spec, care = _handle(name, R=2, rows=ROWS[:2])
     core.set_update_intervals(actor_every=3, target_every=2)
     model = new_model(core)
     set_steps(core, model, 1, (4, 1, 1, 4))
@@ -425,7 +184,7 @@ def test_adam_is_exact_under_update_intervals(cuda, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["chained_ll", "split517_tc", "care_o"])
 def test_adam_is_exact_after_copy_replica(cuda, name):
-    core, spec, care = _make(name, R=2, rows=ROWS[:2])
+    core, spec, care = _handle(name, R=2, rows=ROWS[:2])
     model = new_model(core)
     checked_steps(core, spec, care, model, 2, f"{name} warm-up")
     set_steps(core, model, 0, (7, 1, 10 ** 6, 3))
@@ -441,7 +200,7 @@ def test_adam_is_exact_after_copy_replica(cuda, name):
 def test_adam_is_exact_after_checkpoint_restore(cuda, tmp_path, monkeypatch):
     monkeypatch.chdir(tmp_path)
     a = _learner("LL", tmp_path)
-    spec = sp.ll_spec(batch=LL_CFG["batch_size"])
+    spec = sp.ll_spec(batch=LEARNER_CFGS["LL"]["batch_size"])
     try:
         for i in range(3):
             b, e1, e2 = _inputs(spec, False, 1, i)
@@ -469,7 +228,7 @@ def test_adam_is_exact_after_checkpoint_restore(cuda, tmp_path, monkeypatch):
 @pytest.mark.parametrize("name", ["chained_ll", "split517_tc", "care_o"])
 def test_sampled_step_adam_is_exact(cuda, name):
     from distributed_sac_b200.core import Replay
-    core, spec, care = _make(name, R=2, rows=ROWS[:2])
+    core, spec, care = _handle(name, R=2, rows=ROWS[:2])
     model = new_model(core)
     set_steps(core, model, 1, (7, 1, 10 ** 6, 3))
     cap = 4 * spec.batch * max(spec.num_tasks, 1)
@@ -484,7 +243,7 @@ def test_sampled_step_adam_is_exact(cuda, name):
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["vs400_fp32"])
 def test_host_step_adam_is_exact(cuda, name):
-    core, spec, care = _make(name, R=2, rows=ROWS[:2])
+    core, spec, care = _handle(name, R=2, rows=ROWS[:2])
     model = new_model(core)
     set_steps(core, model, 0, (7, 1, 10 ** 6))
 

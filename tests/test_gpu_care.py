@@ -5,15 +5,9 @@ import torch
 
 import care_port as cp
 from _golden import CareCase, REL, care_core_config, check_port_state, check_state, kink_checked_step, rel_l2, rel_scalar
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 @pytest.mark.parametrize("name", ["care_small_s4", "care_o_small_s4", "care_mt1_small_s3"], ids=["CARE(M)", "CARE(O)", "MT1-CARE"])

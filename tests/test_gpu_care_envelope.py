@@ -26,8 +26,9 @@ import torch
 
 import care_port as cp
 import sac_port as sp
-from _golden import (REL, care_core_config, check_forced, check_port_state, cuda_relu_masks, kink_checked_step, rel_scalar,
-                     sync_core_to_port)
+from _golden import check_forced, check_port_state, cuda_relu_masks, sync_core_to_port
+from _harness import (CARE_ROW_OUTPUTS, _bad_elements, _core, _eps, _pad4, _params, _raise_bad, check_active, check_losses,
+                      check_rows, cuda, plan_labels, run_checked)
 
 gpu = pytest.mark.gpu
 
@@ -74,10 +75,6 @@ CASES = {
                          ctx_hidden=[504, 496], ctx_out=480, batch=128),
 }
 
-# per-row outputs of the step: debug name of the CUDA buffer == key of the port's intermediates
-ROW_OUTPUTS = ("q1", "q2", "y", "a_next", "logp_next", "a_cur", "logp_cur", "qmin")
-
-
 def care_spec(name):
     return cp.CareSpec(**{**_MLP, **CASES[name]})
 
@@ -88,10 +85,6 @@ def care_spec(name):
 CMF_ROWS, CMF_RP, CMF_MAXL, CMF_WARPS = 32, 36, 4, 24
 CMF_SMEM_MAX = 225 * 1024
 TAB_WGRAD_FLOATS = 12288          # care_tab_wgrad_kernel's shared memory (kCareTabWgradSmemFloats)
-
-
-def _pad4(x):
-    return (x + 3) // 4 * 4
 
 
 def mixfwd_smem_floats(spec):
@@ -153,113 +146,10 @@ def tab_wgrad_chunks(spec):
     return -(-spec.num_tasks // tc)
 
 
-# ---------------------------------------------------------------------------------------------------------------------
-# helpers
-# ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _params(spec, seed):
-    """care_port.init_params with the mixture weights scaled to unit gain (randn weights grow the activations by
-    sqrt(width) per layer -- 10^4 at nine layers), small random biases on every nn.Linear (targets distinct from the
-    locals), and a different temperature per task, so that a wrong task's alpha or a wrong bias changes the result."""
-    p = cp.init_params(spec, seed=seed)
-    g = torch.Generator().manual_seed(seed + 1000)
-    for k in p:
-        if ".mix." in k and k.endswith(".W"):
-            p[k] = p[k] * (2.0 / p[k].shape[1]) ** 0.5
-        elif k.endswith(".bias"):
-            p[k] = 0.05 * torch.randn(p[k].shape, generator=g)
-    p["log_alpha"] = -0.5 + 0.5 * torch.randn(spec.num_tasks, generator=g)
-    return p
-
-
-def _eps(spec, gen):
-    return torch.randn(spec.batch, spec.act_dim, generator=gen), torch.randn(spec.batch, spec.act_dim, generator=gen)
-
-
-def _bad_elements(got, ref):
-    """|got - ref| > 1e-4 (|ref| + mean |ref|) (or not finite), and the largest |got - ref| / (|ref| + mean |ref|)."""
-    got, ref = got.double().reshape(ref.shape), ref.double()
-    scale = ref.abs() + ref.abs().mean()
-    dev = (got - ref).abs()
-    return (dev > REL * scale) | ~torch.isfinite(got), float((dev / scale.clamp_min(1e-30)).max())
-
-
-def _raise_bad(what, bad, got, ref):
-    rows = sorted({int(i) for i in bad.nonzero()[:, 0]})
-    r, j = (int(x) for x in bad.nonzero()[0])
-    raise AssertionError(f"{what}: {int(bad.sum())} elements beyond {REL} (|ref| + mean|ref|), rows {rows[:12]}"
-                         f"{'...' if len(rows) > 12 else ''}; first [{r}][{j}] got {float(got[r, j]):.7g} ref {float(ref[r, j]):.7g}")
-
-
-def check_rows(core, spec, o, replica=0, what=""):
-    """Every per-row output of the step, element by element; returns the largest relative deviation."""
-    worst = 0.0
-    for k in ROW_OUTPUTS:
-        ref = o[k].detach().double().reshape(spec.batch, -1)
-        got = core.debug(k, replica).double().reshape(ref.shape)
-        bad, w = _bad_elements(got, ref)
-        if bad.any():
-            _raise_bad(f"{what}{k}", bad, got, ref)
-        worst = max(worst, w)
-    return worst
-
-
-def check_losses(core, o, replica=0, what=""):
-    L = core.read_losses(1)[0, replica]
-    assert torch.isfinite(L).all(), f"{what}losses {L.tolist()}"
-    for i, k in ((0, "critic_loss"), (1, "actor_loss"), (3, "entropy")):
-        assert rel_scalar(float(L[i]), o[k]) <= REL, f"{what}{k}: {float(L[i])} vs oracle {o[k]}"
-
-
-def check_active(core, spec, replica=0, what=""):
-    """Every actor / critic hidden layer on each of its inputs, and every mixture hidden layer of all three encoder
-    instances, has between 5 % and 95 % active units in the CUDA step's own masks."""
-    for tag, m in cuda_relu_masks(core, spec, replica, care=True).items():
-        if tag.startswith(("tanh:", "route:")):
-            continue
-        frac = float(m.float().mean())
-        assert 0.05 <= frac <= 0.95, f"{what}hidden layer {tag}: {100 * frac:.1f}% active"
-
-
-def run_checked(core, spec, port, n_steps, seed, what):
-    """n_steps checked steps of `core` against `port`; returns (mask bits flipped at kinks, worst per-row deviation)."""
-    gen = torch.Generator().manual_seed(seed)
-    flips, worst = 0, 0.0
-    for i in range(n_steps):
-        b = cp.synthetic_batch(spec, seed=seed + 100 + i)
-        e1, e2 = _eps(spec, gen)
-        o, f = kink_checked_step(core, port, spec, b, e1, e2, care=True, want_intermediates=True)
-        flips += sum(f.values())
-        tag = f"{what} step {i}: "
-        check_active(core, spec, what=tag)
-        check_losses(core, o, what=tag)
-        check_port_state(core, port)               # after step 0, m = (1 - beta1) g: every gradient tensor as well
-        worst = max(worst, check_rows(core, spec, o, what=tag))
-    return flips, worst
-
-
-def plan_labels(spec, precision):
-    """Kernel labels of one eager step of a throwaway handle for `spec`, sampled from a device ring."""
-    from distributed_sac_b200.core import Replay, SacCore
-    core = SacCore(care_core_config(spec, precision=precision), 0, seed=0)
-    ring = Replay(core, 4 * spec.batch, "device", seed=1)
-    ring.fill_synthetic(4 * spec.batch, seed=2)
-    labels = [n for n, _ in core.profile_step(ring, iters=1)]
-    ring.close()
-    core.close()
-    return labels
-
-
 def check_path(name, spec, precision):
-    labels = plan_labels(spec, precision)
+    core = _core(spec, True, precision)
+    labels = plan_labels(core)
+    core.close()
     if fused(spec):
         assert "care_mixture_fwd+mix" in labels, f"{name}: expected the fused mixture kernel, plan {labels}"
         assert "care_mix" not in labels, f"{name}: fused case with a care_mix launch, plan {labels}"
@@ -281,14 +171,13 @@ def check_path(name, spec, precision):
 @pytest.mark.parametrize("name", list(CASES))
 def test_care_step_matches_oracle(cuda, name, precision):
     from distributed_sac_b200 import _lib
-    from distributed_sac_b200.core import SacCore
     spec = care_spec(name)
     check_path(name, spec, precision)
-    p = _params(spec, seed=7)
+    p = _params(spec, 7, care=True)
     port = cp.CarePortLearner(spec, p)
-    core = SacCore(care_core_config(spec, precision=precision), 0, seed=0)
+    core = _core(spec, True, precision)
     what = f"{name} precision {precision}"
-    flips, worst = run_checked(core, spec, port, 2, seed=13, what=what)
+    flips, worst = run_checked(core, spec, port, 2, seed=13, what=what, care=True)
     got = core.get_named(_lib.PARAMS)
     gm, gv = core.get_named(_lib.ADAM_M), core.get_named(_lib.ADAM_V)
     ref, st = port.params(), port.adam_state()
@@ -382,12 +271,11 @@ def test_replicas_with_different_parameters_match_their_oracles(cuda, precision)
     oracle; at precision 0 each also equals bit for bit an R = 1 handle given the same state and inputs (at precision 1 the
     tensor-core split / tile choice depends on R)."""
     from distributed_sac_b200 import _lib
-    from distributed_sac_b200.core import SacCore
     spec = cp.CareSpec(state_dim=20, num_tasks=5, num_encoders=4, mix_hidden=[40], mix_out=24, ctx_in=100, ctx_hidden=[30],
                        ctx_out=16, batch=105, **_MLP)
     assert fused(spec) and spec.batch % CMF_ROWS
     R = 3
-    params = [_params(spec, seed=30 + r) for r in range(R)]
+    params = [_params(spec, 30 + r, care=True) for r in range(R)]
     ports = [cp.CarePortLearner(spec, p) for p in params]
     batches = [cp.synthetic_batch(spec, seed=300 + r) for r in range(R)]
     gen = torch.Generator().manual_seed(3)
@@ -395,7 +283,7 @@ def test_replicas_with_different_parameters_match_their_oracles(cuda, precision)
     tids = [torch.argmax(b[0][:, -spec.num_tasks:], dim=1) for b in batches]
     assert not torch.equal(tids[0], tids[1]) and not torch.equal(tids[1], tids[2])
 
-    core = SacCore(care_core_config(spec, replicas=R, precision=precision), 0, seed=0)
+    core = _core(spec, True, precision, R)
     for r in range(R):
         sync_core_to_port(core, ports[r], r)
     core.step(*[torch.stack([b[j] for b in batches]) for j in range(5)],
@@ -405,15 +293,15 @@ def test_replicas_with_different_parameters_match_their_oracles(cuda, precision)
         with sp.ReluTape(forced) as tape:
             o = ports[r].update(*batches[r], *eps[r], want_intermediates=True)
         check_forced(tape, forced, f"replica {r}: ")
-        check_active(core, spec, r, f"replica {r}: ")
+        check_active(core, spec, r, f"replica {r}: ", care=True)
         check_losses(core, o, r, f"replica {r}: ")
         check_port_state(core, ports[r], replica=r)
-        check_rows(core, spec, o, r, f"replica {r}: ")
+        check_rows(core, spec, o, r, f"replica {r}: ", CARE_ROW_OUTPUTS)
     L3 = core.read_losses(1)[0]
     assert not torch.equal(L3[0], L3[1]) and not torch.equal(L3[1], L3[2])
 
     if precision == 0:
-        single = SacCore(care_core_config(spec, precision=0), 0, seed=0)
+        single = _core(spec, True, 0)
         for r in range(R):
             sync_core_to_port(single, cp.CarePortLearner(spec, params[r]))
             single.step(*batches[r], *eps[r])
@@ -432,10 +320,9 @@ def test_replicas_with_different_parameters_match_their_oracles(cuda, precision)
 @gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_act_matches_oracle_policy(cuda, name):
-    from distributed_sac_b200.core import SacCore
     spec = care_spec(name)
-    port = cp.CarePortLearner(spec, _params(spec, seed=11))
-    core = SacCore(care_core_config(spec, precision=0), 0, seed=0)
+    port = cp.CarePortLearner(spec, _params(spec, 11, care=True))
+    core = _core(spec, True, 0)
     sync_core_to_port(core, port)
     B, A = spec.batch, spec.act_dim
     b0, b1 = cp.synthetic_batch(spec, seed=41), cp.synthetic_batch(spec, seed=42)

@@ -17,17 +17,11 @@ import torch
 
 import redis_stub
 from _golden import REL, golden_file, load_npz, rel_l2, rel_scalar
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
 
 CASES = ["ref_ckpt_ll_small", "ref_ckpt_vs_small", "ref_ckpt_ms_small", "ref_ckpt_c10m_small", "ref_ckpt_c10o_small"]
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 def _learner(variant, cfg_path, tmp_path, checkpoint):

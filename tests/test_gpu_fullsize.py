@@ -12,22 +12,13 @@ equal that port's state; when no bit differed at all, the CUDA state must equal 
 import math
 
 import pytest
-import torch
 
 import sac_port as sp
 from _golden import (check_forced, FULL_CARE_CASES, FULL_CASES, REL, FullCase, care_core_config, check_port_state, core_config,
                      cuda_relu_masks, rel_l2, rel_scalar)
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def _cases():

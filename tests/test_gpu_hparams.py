@@ -6,7 +6,6 @@ created with each replica's values compute (every plan); the values mean what th
 oracle given the same values); a change lands exactly between the steps enqueued before and after it, also between
 graph launches and through the legacy-default-stream bridge; copy_replica copies the learner state and nothing else;
 bad values are rejected without a change."""
-import contextlib
 import dataclasses
 import math
 
@@ -15,52 +14,12 @@ import torch
 
 import care_port as cp
 import sac_port as sp
-from _golden import REL, CareCase, care_core_config, check_port_state, core_config, kink_checked_step, rel_scalar
+from _golden import REL, check_port_state, core_config, kink_checked_step, rel_scalar
+from _harness import ROWS, SMALL, _config, _inputs, _plan, _stream_run, cuda
 
 pytestmark = pytest.mark.gpu
 
-# one row per replica; every field differs between rows and from the cfg defaults
-ROWS = [
-    dict(gamma=0.97, reward_scale=0.5, tau=0.01, lr_critic=1e-3, lr_actor=2e-4, lr_alpha=5e-3, tau_se=0.1, lr_ctx=1e-3),
-    dict(gamma=0.95, reward_scale=2.0, tau=0.02, lr_critic=5e-4, lr_actor=7e-4, lr_alpha=1e-3, tau_se=0.03, lr_ctx=5e-4),
-    dict(gamma=0.9, reward_scale=1.5, tau=0.1, lr_critic=2e-3, lr_actor=1e-4, lr_alpha=3e-3, tau_se=0.2, lr_ctx=2e-4),
-]
 ARENAS = (0, 1, 2)     # _lib.PARAMS, ADAM_M, ADAM_V
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _plan(name):
-    """(spec, care, precision) of the four step plans: layer-chained fp32, per-layer wgmma with gradient slices
-    (batch >= 512) and per-task temperatures, CARE(M), CARE(O)."""
-    if name == "chained":
-        return sp.ll_spec(), False, 0
-    if name == "per_layer":
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=640, num_tasks=5), False, 1
-    return CareCase({"care_m": "care_small_s4", "care_o": "care_o_small_s4"}[name]).spec, True, 1
-
-
-def _config(spec, care, precision, replicas, **hp):
-    if not care:
-        hp = {k: v for k, v in hp.items() if k not in ("tau_se", "lr_ctx")}
-    return (care_core_config if care else core_config)(spec, replicas=replicas, precision=precision, **hp)
-
-
-def _inputs(spec, care, R, i):
-    """Step i's minibatch and noise, [R][B][w], a different draw per replica."""
-    gen = torch.Generator().manual_seed(1000 + i)
-    mod = cp if care else sp
-    bs = [mod.synthetic_batch(spec, seed=100 * i + r) for r in range(R)]
-    b = [torch.stack([x[j] for x in bs]) for j in range(5)]
-    e1, e2 = (torch.randn(R, spec.batch, spec.act_dim, generator=gen) for _ in range(2))
-    return b, e1, e2
 
 
 @pytest.mark.parametrize("plan", ["chained", "per_layer", "care_m", "care_o"])
@@ -130,33 +89,12 @@ def test_replica_hyperparameters_match_oracle(cuda, plan):
 B_ROW = dict(gamma=0.9, reward_scale=3.0, tau=0.05, lr_critic=2e-3, lr_actor=1e-3, lr_alpha=4e-3)
 
 
-def _stream_run(mode, set_b, sync_before_set):
-    """16 sampled steps of a small layer-chained learner; B_ROW set on every replica after step 8 if set_b."""
-    from distributed_sac_b200.core import Replay, SacCore
-    spec = sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=128)
-    core = SacCore(core_config(spec, replicas=2), 0, seed=7)
-    rb = Replay(core, capacity=4096, where="host" if mode == "host" else "device", seed=3)
-    stream = torch.cuda.Stream() if mode == "stream" else None
-    with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
-        rb.fill_synthetic(4096, seed=9)
-        core.prepare(rb)
+def _read(core):
+    return core.read_losses(16), core.export_arena(0, 0), core.export_arena(0, 1)
 
-        def eight():
-            if mode == "host":
-                for _ in range(8):
-                    core.update_sampled(rb)          # b200sac_update: one staged-graph step + its losses
-            else:
-                core.step_sampled(rb, 8)             # one 8-step graph launch
-        eight()
-        if sync_before_set:
-            torch.cuda.synchronize()
-        if set_b:
-            core.set_hparams(None, **B_ROW)
-        eight()
-        out = core.read_losses(16), core.export_arena(0, 0), core.export_arena(0, 1)
-    rb.close()
-    core.close()
-    return out
+
+def _set_b(core):
+    core.set_hparams(None, **B_ROW)
 
 
 @pytest.mark.parametrize("mode", ["stream", "legacy", "host"])
@@ -164,9 +102,9 @@ def test_set_hparams_is_stream_ordered(cuda, mode):
     """set_hparams enqueued right behind a graph launch without a synchronisation affects exactly the steps enqueued
     after it: the same as setting it on an idle device.  On a torch side stream, on the legacy default stream (bridged
     onto the handle's own stream) and with a pinned-host ring."""
-    lx, ax0, ax1 = _stream_run(mode, set_b=True, sync_before_set=False)
-    ly, ay0, ay1 = _stream_run(mode, set_b=True, sync_before_set=True)
-    lz, _, _ = _stream_run(mode, set_b=False, sync_before_set=False)
+    lx, ax0, ax1 = _stream_run(mode, _set_b, False, _read)
+    ly, ay0, ay1 = _stream_run(mode, _set_b, True, _read)
+    lz, _, _ = _stream_run(mode, None, False, _read)
     assert torch.equal(lx, ly)
     assert torch.equal(ax0, ay0) and torch.equal(ax1, ay1)
     assert torch.equal(lx[:8], lz[:8])            # the steps before the change used the old values ...
@@ -177,7 +115,7 @@ def test_copy_replica(cuda):
     """copy_replica between steps: dst == src (parameters, Adam moments, step counters), and the two stay bit-identical
     given identical inputs; dst keeps its own hyperparameters, so different values make them diverge."""
     from distributed_sac_b200.core import Replay, SacCore
-    spec = sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=128)
+    spec = SMALL
     R = 3
     core = SacCore(core_config(spec, replicas=R), 0, seed=11)
     core.set_steps((50, 60, 70), replica=0)      # distinct counters (and bias-correction products) in the source
@@ -218,7 +156,7 @@ def test_bad_hyperparameters_are_rejected(cuda):
     """NaN / inf, tau outside [0, 1], a negative learning rate and an out-of-range replica raise; nothing changes, on
     the host mirror or on the device (a step still equals a fresh handle's)."""
     from distributed_sac_b200.core import SacCore
-    spec = sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=128)
+    spec = SMALL
     cfg = core_config(spec, replicas=2, gamma=0.98, lr_alpha=1e-3)
     core, fresh = SacCore(cfg, 0, seed=1), SacCore(cfg, 0, seed=1)
     before = [core.get_hparams(r) for r in range(2)]

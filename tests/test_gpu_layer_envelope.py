@@ -5,7 +5,7 @@ The per-layer plan carries every precision = 1 learner, the 400-wide VS / MS sha
 every exact-fp32 learner outside the chained envelope.  Per launch group the plan builder picks an engine (wgmma 3xTF32,
 32x32 FFMA, or the thin input-layer kernel), a wgmma tile width (64 / 128 / 160) and a split-K factor (4 / 2 / 1); the head
 backward takes the 8-column or the 128-bit kernel, with or without row slices; large batches compute the policy-head output
-gradient in a kernel of its own.  The cases below reach each of those choices (test_sweep_covers_every_branch names any
+gradient in a kernel of its own.  The cases (_harness.LAYER_CASES) reach each of those choices (test_sweep_covers_every_branch names any
 that a change of the table stops reaching), at the shapes where kernels go wrong: batch 1 and 2048, odd pitches, K tails of
 split weight gradients, padded first layers, 1 and 8 hidden layers, act_dim 1 and 8, 33 and 64 tasks.  Every step is checked
 with the CUDA step's ReLU masks forced into the oracle (tests/_golden.py::kink_checked_step): losses, every parameter /
@@ -20,55 +20,15 @@ import torch
 
 import sac_port as sp
 from _golden import check_forced, check_port_state, core_config, cuda_relu_masks, kink_checked_step, sync_core_to_port
-from test_gpu_chain_envelope import _eps, _params, check_active, check_losses, check_rows, run_checked
+from _harness import (LAYER_CASES, REPLICA_SPEC, REPLICAS, _eps, _pad4, _params, _sms, chained_launches, check_active,
+                      check_losses, check_rows, cuda, plan_labels, run_checked)
 
 gpu = pytest.mark.gpu
-
-# id -> SacSpec fields.  Each case is outside the chained envelope through its own shape (a hidden width that is not a
-# multiple of 4 or above 256, or obs + act > 252), so precision 0 takes the per-layer plan too.
-#   b1         batch 1: every GEMM on FFMA at both precisions, thin input-layer gradients, one hidden layer each
-#   odd67      odd pitches everywhere (no wgmma at precision 1 either), La != Lc, the 8-column critic head at an odd batch
-#   in45       wgmma on padded first layers (critic 45 in 48, actor 41 in 44) at a batch that is not a multiple of 128
-#   in17       input width 17: FFMA (not thin) in a 20-float pitch
-#   mixed      precision 1 groups of wgmma-eligible and ineligible problems (one wgmma + one FFMA launch)
-#   deep8      8 actor hidden layers (widths 4, 33, 260, 512), one critic hidden layer: La != Lc the other way
-#   wide1024   1024-wide layers at batch 640: several column tiles, N tails of 128- and 160-wide tiles; the cost model picks
-#              every tile width and split factors 4, 2 and 1
-#   split517   batch 517: K slices 160/160/160/37 and head row slices 130/130/130/127; thin input-layer gradients on K slices
-#   b512n      the first sliced batch; 8-column critic head with row slices
-#   pdout257   policy_dout without gradient slices, just above B * A = 2048; act_dim 8 (policy head backward NO = 16)
-#   pdout256   B * A = 2048 exactly: the policy-head output gradient stays inside head_bwd
-#   b2048      the largest batch; 64 tasks, weighted loss; NO = 16 over 512-row slices; 8-column critic head with slices
-#   act1_2000  act_dim 1 with the in-kernel policy backward at row slices; a 600-deep thin input gradient (two K passes)
-#   tasks33    the upper half of the task table (task index 32) in plain SAC
-CASES = {
-    "b1": dict(state_dim=3, num_tasks=0, act_dim=1, actor_hidden=[37], critic_hidden=[29], batch=1),
-    "odd67": dict(state_dim=11, num_tasks=0, act_dim=3, actor_hidden=[37, 61], critic_hidden=[29, 45, 53], batch=67),
-    "in45": dict(state_dim=41, num_tasks=0, act_dim=4, actor_hidden=[260, 64], critic_hidden=[64, 260], batch=130),
-    "in17": dict(state_dim=15, num_tasks=0, act_dim=2, actor_hidden=[260, 36], critic_hidden=[36, 260], batch=96),
-    "mixed": dict(state_dim=36, num_tasks=0, act_dim=4, actor_hidden=[400, 64], critic_hidden=[24, 400], batch=256),
-    "deep8": dict(state_dim=9, num_tasks=0, act_dim=2, actor_hidden=[4, 33, 260, 512, 64, 36, 100, 20], critic_hidden=[130],
-                  batch=150),
-    "wide1024": dict(state_dim=39, num_tasks=0, act_dim=4, actor_hidden=[1024, 520], critic_hidden=[1024, 400], batch=640),
-    "split517": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[260, 96], critic_hidden=[96, 260], batch=517),
-    "b512n": dict(state_dim=17, num_tasks=0, act_dim=5, actor_hidden=[96, 260], critic_hidden=[72, 131], batch=512),
-    "pdout257": dict(state_dim=10, num_tasks=0, act_dim=8, actor_hidden=[64, 66], critic_hidden=[64, 66], batch=257),
-    "pdout256": dict(state_dim=10, num_tasks=0, act_dim=8, actor_hidden=[64, 66], critic_hidden=[64, 66], batch=256),
-    "b2048": dict(state_dim=30, num_tasks=64, act_dim=8, actor_hidden=[300, 128], critic_hidden=[128, 131], batch=2048,
-                  weighted_loss=True),
-    "act1_2000": dict(state_dim=12, num_tasks=0, act_dim=1, actor_hidden=[260, 64], critic_hidden=[600, 132], batch=2000),
-    "tasks33": dict(state_dim=10, num_tasks=33, act_dim=3, actor_hidden=[66, 64], critic_hidden=[64, 66], batch=99),
-}
 
 # A VS-like learner at precision 1 (batch >= 512 and not a multiple of 128) run with each wgmma tile forced:
 # id -> (B200SAC_TC_BN, B200SAC_TC_PAIR128)
 TILE_SPEC = dict(state_dim=39, num_tasks=0, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=1000)
 TILES = {"128x64": ("64", "0"), "128x128": ("128", "0"), "128x128-paired": ("128", "1"), "128x160": ("160", "0")}
-
-# three co-scheduled replicas with parameters, minibatches and task ids of their own; at precision 1 the mirror picks other
-# tile widths or split factors at R = 3 than at R = 1 for this shape
-REPLICA_SPEC = dict(state_dim=9, num_tasks=5, act_dim=3, actor_hidden=[400, 260], critic_hidden=[260, 130], batch=520)
-REPLICAS = 3
 
 H100_SMS = 132
 
@@ -88,10 +48,6 @@ Prob = namedtuple("Prob", "mode M N K lda ldb inp")
 # one plan launch: label, engine ("wgmma" | "ffma" | "thin" | None), tile width, split factor, the problems it runs and
 # whether its group also issued a launch on the other engine
 Launch = namedtuple("Launch", "label engine bn split probs mixed")
-
-
-def _pad4(x):
-    return (x + 3) // 4 * 4
 
 
 def tc_eligible(p):
@@ -303,14 +259,14 @@ WANT = {"cost model: tile 128x64", "cost model: tile 128x128", "cost model: tile
 # ---------------------------------------------------------------------------------------------------------------------
 # CPU: the sweep reaches every branch; the mirror agrees with shapes worked out by hand
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(LAYER_CASES))
 def test_case_is_outside_the_chained_envelope(name):
-    assert not chained(sp.SacSpec(**CASES[name]), 0), name
+    assert not chained(sp.SacSpec(**LAYER_CASES[name]), 0), name
 
 
 def test_sweep_covers_every_branch():
     have = set()
-    for c in CASES.values():
+    for c in LAYER_CASES.values():
         for precision in (0, 1):
             have |= features(sp.SacSpec(**c), precision)
     have |= features(sp.SacSpec(**REPLICA_SPEC), 1, R=REPLICAS)
@@ -327,59 +283,25 @@ def test_replica_shape_changes_the_tensor_core_choices():
 
 
 def test_mirror_matches_hand_worked_shapes():
-    s517 = sp.SacSpec(**CASES["split517"])
+    s517 = sp.SacSpec(**LAYER_CASES["split517"])
     assert [p.K for p in _splits(Prob(WGRAD, 96, 10, 517, 96, 12, True), 4, 4)] == [160, 160, 160, 37]
     rows_per = -(-517 // 4)
     assert [min(rows_per, 517 - r0) for r0 in range(0, 517, rows_per)] == [130, 130, 130, 127]
     thin = [ln for ln in mirror_plan(s517, 0) if ln.engine == "thin"]
     assert thin and all(ln.split == 4 for ln in thin if any(p.mode == WGRAD for p in ln.probs))
-    assert "policy_dout" in [ln.label for ln in mirror_plan(sp.SacSpec(**CASES["pdout257"]), 0)]
-    assert "policy_dout" not in [ln.label for ln in mirror_plan(sp.SacSpec(**CASES["pdout256"]), 0)]
+    assert "policy_dout" in [ln.label for ln in mirror_plan(sp.SacSpec(**LAYER_CASES["pdout257"]), 0)]
+    assert "policy_dout" not in [ln.label for ln in mirror_plan(sp.SacSpec(**LAYER_CASES["pdout256"]), 0)]
     # DESIGN.md 4.2: 29 launches per step for the 3-hidden-layer VS shape at precision 1, index sampling included
     vs = sp.vs_spec()
     assert len(mirror_plan(vs, 1)) + 1 == 29
     assert all(ln.engine == "wgmma" for ln in mirror_plan(vs, 1) if ln.engine and not any(p.inp for p in ln.probs))
-    b1 = mirror_plan(sp.SacSpec(**CASES["b1"]), 1)
+    b1 = mirror_plan(sp.SacSpec(**LAYER_CASES["b1"]), 1)
     assert all(ln.engine in (None, "ffma", "thin") for ln in b1)
 
 
 # ---------------------------------------------------------------------------------------------------------------------
 # helpers of the GPU tests
 # ---------------------------------------------------------------------------------------------------------------------
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-@pytest.fixture(scope="module")
-def chained_launches(cuda):
-    """Launches per step of the layer-chained plan (a LunarLander learner)."""
-    from distributed_sac_b200.core import SacCore
-    core = SacCore(core_config(sp.ll_spec(), precision=0), 0, seed=0)
-    n = core.launches_per_step
-    core.close()
-    return n
-
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
-
-def plan_labels(core):
-    """Kernel labels of one eager step of `core`, sampled from a device ring (the step changes the handle's state)."""
-    from distributed_sac_b200.core import Replay
-    B = core.cfg.batch
-    ring = Replay(core, 4 * B, "device", seed=1)
-    ring.fill_synthetic(4 * B, seed=2)
-    labels = [n for n, _ in core.profile_step(ring, iters=1)]
-    ring.close()
-    return labels
-
-
 def check_plan(spec, precision, what, R=1, env=None):
     """A throwaway handle created under `env` runs the per-layer plan the mirror predicts.  The labels are read with the
     environment restored: the handle keeps what it chose when it was built."""
@@ -445,9 +367,9 @@ def run_case(spec, precision, what, chained_launches, env=None, n_steps=2):
 # ---------------------------------------------------------------------------------------------------------------------
 @gpu
 @pytest.mark.parametrize("precision", [0, 1], ids=["fp32", "tc3xtf32"])
-@pytest.mark.parametrize("name", list(CASES))
+@pytest.mark.parametrize("name", list(LAYER_CASES))
 def test_per_layer_step_matches_oracle(cuda, chained_launches, name, precision):
-    run_case(sp.SacSpec(**CASES[name]), precision, f"{name} precision {precision}", chained_launches)
+    run_case(sp.SacSpec(**LAYER_CASES[name]), precision, f"{name} precision {precision}", chained_launches)
 
 
 # ---------------------------------------------------------------------------------------------------------------------

@@ -8,20 +8,9 @@ import torch
 
 import redis_stub
 from _golden import Case, REL, rel_l2, rel_scalar
+from _harness import LL_CFG, cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
-
-
-LL_CFG = {"num_tasks": 10, "device": "cuda", "buffer_size": 1e6, "reward_scale": 1, "batch_size": 256, "gamma": 0.99,
-          "lr_actor": 3e-4, "lr_critic": 3e-4, "log_alpha": 0, "tau": 0.005, "num_learn": 1, "num_time_step": 1,
-          "random_step": 5000, "start_memory_len": 5000}
 
 
 def _ll_learner(tmp_path, **kw):

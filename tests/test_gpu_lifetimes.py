@@ -10,19 +10,13 @@ import torch
 import care_port as cp
 import sac_port as sp
 from _golden import care_core_config, core_config
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
 
 MiB = 1 << 20
 TOL = 512 * MiB
 ERR_NOMEM = -3          # B200SAC_ERR_NOMEM (include/b200sac.h)
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 def _free():

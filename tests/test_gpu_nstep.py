@@ -14,24 +14,14 @@ import nstep_ref
 import per_ref
 import redis_stub
 import sac_port as sp
-from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks,
-                     rel_scalar, sync_core_to_port)
-from test_gpu_adam_exact import capture_grads, check_adam, check_grads, new_model, snapshot
-from test_oracle_nstep import _play, random_pushes
+from _golden import REL, check_forced, check_port_state, cuda_relu_masks, rel_scalar, sync_core_to_port
+from _harness import (LL_CFG, MTSAC_T4, PER_LAYER, SMALL, VS400, _core, _play, _tasks, capture_grads, care_t4, check_adam,
+                      check_grads, cuda, new_model, random_pushes, snapshot)
 
 pytestmark = pytest.mark.gpu
 
 PER = dict(alpha=0.6, beta=0.4, eps=1e-6)
 INVALID, STATE = -1, -4
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def _spec(name):
@@ -40,22 +30,16 @@ def _spec(name):
     if name == "chained":
         return sp.ll_spec(), False, 0
     if name in ("vsac_p0", "vsac_p1"):
-        return sp.SacSpec(state_dim=39, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=128), False, int(name[-1])
+        return sp.SacSpec(**VS400), False, int(name[-1])
     if name in ("per_layer_p0", "per_layer_p1"):
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=640), False, int(name[-1])
+        return sp.SacSpec(**PER_LAYER), False, int(name[-1])
     if name in ("mtsac", "mtsac_p0"):
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=160, num_tasks=4,
-                          weighted_loss=True), False, 0 if name.endswith("_p0") else 1
+        return sp.SacSpec(**MTSAC_T4), False, 0 if name.endswith("_p0") else 1
     if name == "tiny":
-        return sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=8), False, 0
+        return dataclasses.replace(SMALL, batch=8), False, 0
     if name == "tiny_mt":
-        return sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=8, num_tasks=4), False, 0
-    return dataclasses.replace(CareCase("care_small_s4").spec, num_tasks=4), True, 1
-
-
-def _core(spec, care, precision, replicas=1, seed=0):
-    from distributed_sac_b200.core import SacCore
-    return SacCore((care_core_config if care else core_config)(spec, replicas=replicas, precision=precision), 0, seed=seed)
+        return dataclasses.replace(SMALL, batch=8, num_tasks=4), False, 0
+    return care_t4(), True, 1
 
 
 def _episodes(spec, care, n, seed, n_streams=7, p_done=0.05, p_cut=0.03):
@@ -67,10 +51,6 @@ def _episodes(spec, care, n, seed, n_streams=7, p_done=0.05, p_cut=0.03):
     if spec.num_tasks > 0:                      # a player works on one task: its rows stay in one sub-ring
         sid = sid * spec.num_tasks + _tasks(spec, s)
     return (s, a, r, s2, d), sid.astype(np.int32), (rng.random(n) < p_cut).astype(np.uint8)
-
-
-def _tasks(spec, s):
-    return s[:, spec.state_dim:].argmax(1).numpy() if spec.num_tasks > 0 else np.zeros(len(s), np.int64)
 
 
 class Mirror:
@@ -334,10 +314,6 @@ def test_refusals_leave_everything_unchanged(cuda):
 
 
 # ---- 7. learner ------------------------------------------------------------------------------------------------------
-LL_CFG = {"num_tasks": 10, "device": "cuda", "buffer_size": 1e6, "reward_scale": 1, "batch_size": 256, "gamma": 0.99,
-          "lr_actor": 3e-4, "lr_critic": 3e-4, "log_alpha": 0, "tau": 0.005, "num_learn": 1, "num_time_step": 1,
-          "random_step": 5000, "start_memory_len": 5000}
-
 
 def test_learner_stitches_interleaved_players(cuda, tmp_path):
     """LunarLanderLearner(replay_where="device", n_step=3) fed through the Redis stub by interleaved players runs update(),

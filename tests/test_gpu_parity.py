@@ -9,17 +9,9 @@ import sac_manual as smn
 import sac_port as sp
 from _golden import (CASES, Case, REL, check_port_state, check_state, core_config, kink_checked_step, rel_l2, rel_scalar,
                      sync_core_to_port)
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def _load(core, case, replica=0):

@@ -1,7 +1,5 @@
 """GPU: prioritized experience replay on the device ring -- sum-tree sampling, importance-weighted critic loss and the
 in-graph priority update (include/b200sac.h, per_kernels.cuh), against oracle/per_ref.py and the autograd oracle."""
-import dataclasses
-
 import numpy as np
 import pytest
 import torch
@@ -10,21 +8,12 @@ from scipy import stats
 import care_port as cp
 import per_ref
 import sac_port as sp
-from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks,
-                     rel_scalar, sync_core_to_port)
+from _golden import REL, check_forced, check_port_state, cuda_relu_masks, rel_scalar, sync_core_to_port
+from _harness import MTSAC_T4, PER_LAYER, VS400, _core, _tasks, care_t4, cuda
 
 pytestmark = pytest.mark.gpu
 
 PER = dict(alpha=0.6, beta=0.4, eps=1e-6)
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def _spec(name):
@@ -33,18 +22,12 @@ def _spec(name):
     if name == "chained":
         return sp.ll_spec(), False, 0
     if name == "per_layer":
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=640), False, 1
+        return sp.SacSpec(**PER_LAYER), False, 1
     if name in ("wide_p0", "wide_p1"):
-        return sp.SacSpec(state_dim=39, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=128), False, int(name[-1])
+        return sp.SacSpec(**VS400), False, int(name[-1])
     if name == "mtsac":
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=160, num_tasks=4,
-                          weighted_loss=True), False, 1
-    return dataclasses.replace(CareCase("care_small_s4").spec, num_tasks=4), True, 1
-
-
-def _core(spec, care, precision, replicas=1, seed=0):
-    from distributed_sac_b200.core import SacCore
-    return SacCore((care_core_config if care else core_config)(spec, replicas=replicas, precision=precision), 0, seed=seed)
+        return sp.SacSpec(**MTSAC_T4), False, 1
+    return care_t4(), True, 1
 
 
 def _filled_ring(core, spec, care, n, cap, seed=5, replica=0, prioritized=PER, ring_seed=1):
@@ -56,7 +39,7 @@ def _filled_ring(core, spec, care, n, cap, seed=5, replica=0, prioritized=PER, r
     rb.push(s.numpy(), a.numpy(), r.numpy(), s2.numpy(), d.numpy(), replica=replica)
     T = max(spec.num_tasks, 1)
     cap_t = cap // T
-    tid = s[:, spec.state_dim:].argmax(1).numpy() if spec.num_tasks > 0 else np.zeros(n, np.int64)
+    tid = _tasks(spec, s)
     where = np.empty(n, np.int64)
     for t in range(T):
         rows = np.nonzero(tid == t)[0]

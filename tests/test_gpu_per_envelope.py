@@ -11,8 +11,6 @@ padding leaves (cap_per_task not a power of two), pushes that wrap a sub-ring at
 CPU-only test mirrors the geometry and names any branch the cases stop reaching.  Every tree is compared bit for bit with
 oracle/per_ref.build_tree, every draw with the descent model's strata, every weight with per_ref.is_weights.
 """
-import dataclasses
-
 import numpy as np
 import pytest
 import torch
@@ -21,8 +19,8 @@ from scipy import stats
 import care_port as cp
 import per_ref
 import sac_port as sp
-from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks, rel_l2,
-                     rel_scalar, sync_core_to_port)
+from _golden import REL, check_forced, check_port_state, cuda_relu_masks, rel_l2, rel_scalar, sync_core_to_port
+from _harness import _core, _sms, _tasks, care_t4, cuda, plan_rows
 
 gpu = pytest.mark.gpu
 
@@ -102,20 +100,6 @@ def test_cases_reach_every_branch():
     missing = BRANCHES - reached_branches()
     assert not missing, f"no case reaches: {sorted(missing)}"
     assert geometry(3, 3000, 768)["Lc"] == 10 and geometry(64, 65, 64)["Lc"] == 6 and geometry(0, 1 << 20, 1024)["Lc"] == 12
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _core(spec, care=False, precision=1, replicas=1):
-    from distributed_sac_b200.core import SacCore
-    return SacCore((care_core_config if care else core_config)(spec, replicas=replicas, precision=precision), 0, seed=0)
 
 
 def _tiny(T, B):
@@ -299,8 +283,8 @@ def _parity_case(name):
         return (sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=128,
                            num_tasks=64, weighted_loss=True), False, 1, 1)
     if name == "care_o":
-        return dataclasses.replace(CareCase("care_o_small_s4").spec, num_tasks=4), True, 1, 1
-    return dataclasses.replace(CareCase("care_small_s4").spec, num_tasks=4), True, 1, 2     # care_m_r2
+        return care_t4(False), True, 1, 1
+    return care_t4(), True, 1, 2     # care_m_r2
 
 
 PARITY = ["chained_b37", "chained_r3", "layer_p0_400", "layer_p1_b2048", "mtsac_t64", "care_o", "care_m_r2"]
@@ -322,7 +306,7 @@ def _parity_ring(core, spec, care, R, seed):
     for r in range(R):
         fill = np.array([cap_t - cap_t // 16 * ((r + 1) * t % 5) for t in range(T)])      # >= 3/4 cap_t >= 6 per
         rows = (cp if care else sp).synthetic_batch(spec, seed=seed + 10 * r, batch=T * cap_t)
-        tid = rows[0][:, spec.state_dim:].argmax(1).numpy() if spec.num_tasks > 0 else np.zeros(T * cap_t, np.int64)
+        tid = _tasks(spec, rows[0])
         rank = np.zeros(T * cap_t, np.int64)
         for t in range(T):
             k = np.nonzero(tid == t)[0]
@@ -355,8 +339,7 @@ def test_weighted_parity_envelope(cuda, name):
     spec, care, precision, R = _parity_case(name)
     core = _core(spec, care, precision, replicas=R)
     if name == "chained_r3":
-        from test_gpu_chain_envelope import plan_rows
-        sms = torch.cuda.get_device_properties(0).multi_processor_count
+        sms = _sms()
         rows3, rows1 = plan_rows(spec.batch, R, sms), plan_rows(spec.batch, 1, sms)
         print(f"[rows] R = 3: {rows3}, R = 1: {rows1} ({sms} SMs)")
         if sms == 132:

@@ -5,15 +5,9 @@ import torch
 
 import sac_port as sp
 from _golden import core_config
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 def _inputs(spec, seed):

@@ -7,20 +7,12 @@ import torch
 
 import sac_port as sp
 from _golden import core_config
+from _harness import cuda
 
 pytestmark = pytest.mark.gpu
 
 _SPEC = sp.SacSpec(state_dim=39, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=256)
 _KINDS = {"uniform": {}, "prioritized": dict(prioritized=dict(alpha=0.6, beta=0.4, eps=1e-6)), "linked": dict(trajectories=True)}
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
 
 
 def _run(kind, sync_before_refill):

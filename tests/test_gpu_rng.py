@@ -13,14 +13,9 @@ import pytest
 import torch
 from scipy import stats
 
+from _harness import cuda
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    return torch.device("cuda", 0)
 
 
 def _check_xavier(name, w):

@@ -8,8 +8,6 @@ about a third of the rows have d = 1, so that a lost or misplaced done flag chan
 noise is keyed by (seed, replica, step counter): a handle with the same seed that runs b200sac_step on the recovered rows
 (no injected noise) draws the same noise, and every sampled step must equal it bit for bit.
 """
-import dataclasses
-
 import numpy as np
 import pytest
 import torch
@@ -18,8 +16,8 @@ from scipy import stats
 
 import care_port as cp
 import sac_port as sp
-from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks, rel_l2,
-                     rel_scalar, sync_core_to_port)
+from _golden import REL, check_forced, check_port_state, cuda_relu_masks, rel_l2, rel_scalar, sync_core_to_port
+from _harness import VS400, _core, _tasks, care_t4, check_active, cuda, plan_labels
 
 pytestmark = pytest.mark.gpu
 
@@ -29,49 +27,24 @@ _REWARDS = np.random.default_rng(2026).permutation(np.linspace(-3.0, 3.0, 1 << 2
 _SMALL = dict(act_dim=3, actor_hidden=[64, 48], critic_hidden=[56, 64])
 
 
-def _care(modified):
-    """The CARE fixtures' learner (CARE(M) / CARE(O)) with T = 4: batch 120 = 4 x 30."""
-    return dataclasses.replace(CareCase("care_small_s4" if modified else "care_o_small_s4").spec, num_tasks=4)
-
-
 # id -> (spec, care, precision, replicas, plan)
 SHAPES = {
     "ll_chained": (sp.ll_spec(), False, 0, 1, "chained"),
     "odd37_chained": (sp.SacSpec(state_dim=8, batch=37, **_SMALL), False, 0, 1, "chained"),
-    "layer_p0": (sp.SacSpec(state_dim=39, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=128), False, 0,
-                 1, "per_layer"),
-    "layer_p1": (sp.SacSpec(state_dim=39, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=128), False, 1,
-                 1, "wgmma"),
+    "layer_p0": (sp.SacSpec(**VS400), False, 0, 1, "per_layer"),
+    "layer_p1": (sp.SacSpec(**VS400), False, 1, 1, "wgmma"),
     "mtsac_t10": (sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=130, num_tasks=10,
                              weighted_loss=True), False, 1, 1, "wgmma"),
-    "care_m": (_care(True), True, 1, 1, "care"),
-    "care_o": (_care(False), True, 0, 1, "care"),
+    "care_m": (care_t4(), True, 1, 1, "care"),       # batch 120 = 4 x 30
+    "care_o": (care_t4(False), True, 0, 1, "care"),
     "r3_wrapped": (sp.SacSpec(state_dim=9, num_tasks=3, batch=99, **_SMALL), False, 0, 3, "chained"),
 }
 
 
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _core(spec, care, precision, replicas=1, seed=0):
-    from distributed_sac_b200.core import SacCore
-    return SacCore((care_core_config if care else core_config)(spec, replicas=replicas, precision=precision), 0, seed=seed)
-
-
 def check_plan(spec, care, precision, replicas, plan):
     """A throwaway handle of the same configuration runs the plan the case is meant to cover (labels of one eager step)."""
-    from distributed_sac_b200.core import Replay
     core = _core(spec, care, precision, replicas)
-    ring = Replay(core, 4 * spec.batch, "device", seed=1)
-    ring.fill_synthetic(4 * spec.batch, seed=2)
-    labels = [n for n, _ in core.profile_step(ring, iters=1)]
-    ring.close()
+    labels = plan_labels(core)
     core.close()
     chained = any(n.startswith("chain_fwd") for n in labels)
     wgmma = any("wgmma" in n for n in labels)
@@ -80,7 +53,7 @@ def check_plan(spec, care, precision, replicas, plan):
     assert want, f"expected the {plan} plan, got {labels}"
 
 
-def _tasks(counts, seed):
+def _shuffled_tasks(counts, seed):
     """Task ids holding counts[t] rows of task t, shuffled."""
     t = np.repeat(np.arange(len(counts)), counts)
     return np.random.default_rng(seed).permutation(t)
@@ -130,7 +103,7 @@ class Ring:
         base = 0 if self.table is None else self.table[0].shape[0]
         self.table = list(batch) if self.table is None else [torch.cat([t, x]) for t, x in zip(self.table, batch)]
         self.index.update({k: base + i for i, k in enumerate(r)})
-        tid = s[:, self.spec.state_dim:].argmax(1).numpy() if self.spec.num_tasks > 0 else np.zeros(len(r), np.int64)
+        tid = _tasks(self.spec, s)
         for t in range(self.T):
             for i in np.nonzero(tid == t)[0][-self.cap_t:]:       # more than a full sub-ring: the newest cap_t survive
                 k = t * self.cap_t + int(self.head[replica, t])
@@ -174,15 +147,6 @@ def check_draw(ring, keys, slots, B, what=""):
     assert 0 < float(d.mean()) < 1, f"{what}d is constant over the minibatch"
 
 
-def check_active(core, spec, care, replica=0, what=""):
-    """Every hidden layer (and every mixture-encoder layer) of the step is 5-95 % active in the CUDA step's own masks."""
-    for tag, m in cuda_relu_masks(core, spec, replica, care).items():
-        if tag.startswith(("tanh:", "route:")):
-            continue
-        frac = float(m.float().mean())
-        assert 0.05 <= frac <= 0.95, f"{what}hidden layer {tag}: {100 * frac:.1f}% active"
-
-
 def stacked(rows_per_replica):
     return [torch.stack([rows[j] for rows in rows_per_replica]) for j in range(5)]
 
@@ -206,13 +170,13 @@ def _fill(ring, src, spec, R):
     sub-ring wrapped by 90 rows over two pushes."""
     T, per = ring.T, spec.batch // ring.T
     if R == 1:
-        ring.push(src.take(_tasks([per * (5 + t % 3) for t in range(T)], seed=1)))
+        ring.push(src.take(_shuffled_tasks([per * (5 + t % 3) for t in range(T)], seed=1)))
         return
     plans = [([140, 200, 170], [0, 0, 0]), ([200, 133, 150], [0, 0, 0]), ([100, 80, 150], [50, 80, 140])]
     for rep, chunks in enumerate(plans):
         for j, counts in enumerate(chunks):
             if sum(counts):
-                ring.push(src.take(_tasks(counts, seed=10 * rep + j)), replica=rep)
+                ring.push(src.take(_shuffled_tasks(counts, seed=10 * rep + j)), replica=rep)
     assert (ring.fill[2] == [150, 160, 200]).all() and ring.head[2, 2] == 90
 
 
@@ -237,7 +201,7 @@ def test_sampled_step_equals_split_step(cuda, name):
                 keys = ring.keys(a, rep)
                 check_draw(ring, keys, ring.slots(keys, rep), spec.batch, f"{name} step {step} replica {rep}: ")
                 if step == 0:
-                    check_active(a, spec, care, rep, f"{name} replica {rep}: ")
+                    check_active(a, spec, rep, f"{name} replica {rep}: ", care=care)
                 drawn.append(ring.rows(keys))
             c.step(*stacked(drawn))
             step += 1
@@ -267,7 +231,7 @@ def test_host_ring_equals_split_step(cuda):
     ring = Ring([a, b], spec, 4 * 128, where="host", seed=7)
     src = Source(spec, seed=8)
     for rep in range(R):
-        ring.push(src.take(_tasks([128, 100, 90 + 20 * rep, 110], seed=rep)), replica=rep)
+        ring.push(src.take(_shuffled_tasks([128, 100, 90 + 20 * rep, 110], seed=rep)), replica=rep)
     program = [("update", 1), ("sampled", 3), ("host", 1), ("sampled", 2), ("host", 1), ("host", 1), ("update", 1),
                ("sampled", 1), ("push", 0), ("sampled", 4), ("update", 1), ("sampled", 2)]
     step, after_push, overwritten = 0, False, 0
@@ -275,11 +239,11 @@ def test_host_ring_equals_split_step(cuda):
         if op == "push":                                     # overwrites 3/4 of every sub-ring of both replicas
             alive_before = [set(ring.slot[rep]) for rep in range(R)]
             for rep in range(R):
-                ring.push(src.take(_tasks([96] * 4, seed=20 + rep)), replica=rep)
+                ring.push(src.take(_shuffled_tasks([96] * 4, seed=20 + rep)), replica=rep)
             after_push = True
             continue
         if op == "host":
-            x = [src.take(_tasks([per] * 4, seed=30 + step + rep)) for rep in range(R)]
+            x = [src.take(_shuffled_tasks([per] * 4, seed=30 + step + rep)) for rep in range(R)]
             for core in (a, b):
                 core.step_host(*stacked(x), want_losses=False)
             c.step(*stacked(x))
@@ -296,7 +260,7 @@ def test_host_ring_equals_split_step(cuda):
                 keys = ring.keys(a, rep)
                 assert len(set(keys)) == spec.batch
                 if step == 0:
-                    check_active(a, spec, False, rep, f"replica {rep}: ")
+                    check_active(a, spec, rep, f"replica {rep}: ")
                 if after_push:                               # the prefetched minibatch: gathered before the push
                     assert set(keys) <= alive_before[rep], f"step {step} replica {rep}: a row not in the ring at draw time"
                     overwritten += len(set(keys) - set(ring.slot[rep]))
@@ -335,7 +299,7 @@ def test_push_then_step_on_a_side_stream(cuda):
             slots = ring.slots(keys)
             check_draw(ring, keys, slots, spec.batch, f"step {k}: ")
             if k == 0:
-                check_active(a, spec, False)
+                check_active(a, spec)
             c.step(*ring.rows(keys))
     torch.cuda.synchronize()
     assert ring.fill[0, 0] == 8 * 96 and ring.head[0, 0] == 4 * 96
@@ -371,7 +335,7 @@ def test_sampled_step_matches_oracle(cuda, name):
         check_draw(ring, keys, ring.slots(keys), B, f"{name} step {step}: ")
         batch = ring.rows(keys)
         eps = core.debug("psave").reshape(2 * B, A, 8)[:, :, 5]
-        check_active(core, spec, care, what=f"{name} step {step}: ")
+        check_active(core, spec, what=f"{name} step {step}: ", care=care)
         forced = cuda_relu_masks(core, spec, care=care)
         with sp.ReluTape(forced) as tape:
             out = (port.update if care else port.update_SAC)(*batch, eps[:B].clone(), eps[B:].clone(), want_intermediates=True)
@@ -419,7 +383,7 @@ def test_device_sampler_contract(cuda, T, batch):
     ring = Ring([core], spec, cap_t * Tn, seed=13)
     src = Source(spec, seed=14)
     for rep in range(2):
-        ring.push(src.take(_tasks(fills[rep], seed=rep)), replica=rep)
+        ring.push(src.take(_shuffled_tasks(fills[rep], seed=rep)), replica=rep)
         assert (ring.fill[rep] == fills[rep]).all()
     counts = np.zeros((2, cap_t * Tn), np.int64)
     prev = [None, None]
@@ -454,7 +418,7 @@ def test_refuses_a_ring_below_four_per_task_batches(cuda):
     core = _core(spec, False, 0, seed=1)
     ring = Ring([core], spec, 10 * 40)
     src = Source(spec, seed=15)
-    ring.push(src.take(_tasks([24] * 9 + [23], seed=0)))
+    ring.push(src.take(_shuffled_tasks([24] * 9 + [23], seed=0)))
     before = [core.export_arena(w) for w in (_lib.PARAMS, _lib.ADAM_M, _lib.ADAM_V)]
     with pytest.raises(RuntimeError, match="not ready"):
         core.step_sampled(ring.rbs[0], 1)

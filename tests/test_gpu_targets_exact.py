@@ -12,86 +12,20 @@ locals after the step and the targets before it.  So every element of q1_target.
 padded first layers included) must equal that expectation as a bit pattern, and nothing else outside the trainable prefix
 (the CARE embedding, the gaps between tensors) may change at all.
 """
-import json
-
 import numpy as np
 import pytest
 import torch
 
-import redis_stub
-import sac_port as sp
-from _golden import CareCase, care_core_config, core_config
-from test_gpu_care_envelope import _params as care_params
-from test_gpu_chain_envelope import CASES as CHAIN_CASES, _params as sac_params
-from test_gpu_hparams import ROWS, _inputs
-from test_gpu_layer_envelope import CASES as LAYER_CASES
+from _harness import PARAMS, ROWS, _bits, _handle, _inputs, _learner, cuda, export
 
 pytestmark = pytest.mark.gpu
 
-PARAMS = 0
-
-# a VS-like learner (400-wide, outside the chained envelope at either precision) and MTSAC at T = 10
-VS_LIKE = dict(state_dim=39, num_tasks=0, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=300)
-MT10 = dict(state_dim=39, num_tasks=10, act_dim=4, actor_hidden=[400, 400], critic_hidden=[400, 400], batch=320,
-            weighted_loss=True)
-
-# id -> (SacSpec fields, precision) | CARE fixture.  Chained: the LL shape, width-4 layers with 8 hidden layers, batch 531.
+# _harness.SAC_PLANS / CARE_PLANS ids.  Chained: the LL shape, width-4 layers with 8 hidden layers, batch 531.
 # Per-layer: fp32 FFMA and wgmma 3xTF32 at 400 wide; split-K weight-gradient slices and K tails (split517, wide1024).
-SAC_PLANS = {
-    "chained_ll": (sp.ll_spec().to_json(), 0),
-    "chained_deep8": (CHAIN_CASES["deep8"], 0),
-    "chained_big_odd": (CHAIN_CASES["big_odd"], 0),
-    "vs400_fp32": (VS_LIKE, 0),
-    "vs400_tc": (VS_LIKE, 1),
-    "split517_fp32": (LAYER_CASES["split517"], 0),
-    "split517_tc": (LAYER_CASES["split517"], 1),
-    "wide1024_tc": (LAYER_CASES["wide1024"], 1),
-    "mtsac_t10": (MT10, 1),
-}
-CARE_PLANS = {"care_m": "care_small_s4", "care_o": "care_o_small_s4"}
-PLANS = list(SAC_PLANS) + list(CARE_PLANS)
+PLANS = ["chained_ll", "chained_deep8", "chained_big_odd", "vs400_fp32", "vs400_tc", "split517_fp32", "split517_tc",
+         "wide1024_tc", "mtsac_t10", "care_m", "care_o"]
 # the R = 3 cases: one per step plan
 R3_PLANS = ["chained_ll", "chained_big_odd", "vs400_fp32", "vs400_tc", "split517_tc", "mtsac_t10", "care_m", "care_o"]
-
-
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _plan(name):
-    """(spec, care, precision)"""
-    if name in CARE_PLANS:
-        return CareCase(CARE_PLANS[name]).spec, True, 1
-    fields, precision = SAC_PLANS[name]
-    return sp.SacSpec(**fields), False, precision
-
-
-def _params(spec, care, seed):
-    """The envelopes' parameters (Xavier weights, random biases, a temperature per task) with every target tensor moved
-    off its local, so that no formula can pass by returning either operand."""
-    p = (care_params if care else sac_params)(spec, seed)
-    g = torch.Generator().manual_seed(seed + 2000)
-    for k in p:
-        if "_target." in k or k.startswith("tse."):
-            p[k] = p[k] + 0.02 * torch.randn(p[k].shape, generator=g)
-    return p
-
-
-def _handle(name, R=1, rows=None, seed=0):
-    """(core, spec, care) with each replica's own parameters and, if given, its own hyperparameter row."""
-    from distributed_sac_b200.core import SacCore
-    spec, care, precision = _plan(name)
-    core = SacCore((care_core_config if care else core_config)(spec, replicas=R, precision=precision), 0, seed=seed)
-    for r in range(R):
-        core.set_named(_params(spec, care, seed=11 + 7 * r), PARAMS, r)
-        if rows is not None:
-            core.set_hparams(r, **rows[r])
-    return core, spec, care
 
 
 def target_pairs(core):
@@ -108,14 +42,6 @@ def target_pairs(core):
 def polyak(local, target, tau):
     """fl(fl(ta * local) + fl(tb * target)) in fp32, (ta, tb) = ((float)tau, (float)(1 - tau)) -- one rounding per op."""
     return np.float32(tau) * local + np.float32(1.0 - tau) * target
-
-
-def _bits(x):
-    return np.ascontiguousarray(x, dtype=np.float32).view(np.uint32)
-
-
-def export(core, replica=0):
-    return core.export_arena(PARAMS, replica).numpy().copy()
 
 
 def check_targets(core, before, after, rates, moved, what, others=()):
@@ -285,21 +211,6 @@ def test_soft_update_is_exact(cuda, name, tau):
 # ---------------------------------------------------------------------------------------------------------------------
 # 5: Learner.soft_update(local_critic_k, target_critic_k, tau) updates that pair only
 # ---------------------------------------------------------------------------------------------------------------------
-LL_CFG = {"device": "cuda", "buffer_size": 1e5, "reward_scale": 1, "batch_size": 64, "gamma": 0.99, "lr_actor": 3e-4,
-          "lr_critic": 3e-4, "log_alpha": 0, "tau": 0.005, "start_memory_len": 1000}
-VS_CFG = {"device": "cuda", "buffer_size": 10000, "reward_scale": 1, "batch_size": 64, "gamma": 0.99, "lr_actor": 3e-4,
-          "lr_critic": 3e-4, "log_alpha": 0, "tau": 0.005, "start_memory_len": 1000, "print_period_learner": 10,
-          "update_delay": 1, "actor_hidden_dim": [64, 48], "critic_hidden_dim": [72, 40]}
-
-
-def _learner(family, tmp_path):
-    from distributed_sac_b200 import learner as L
-    p = tmp_path / f"{family}.json"
-    p.write_text(json.dumps(LL_CFG if family == "LL" else VS_CFG))
-    kw = dict(write_mode=False, server=redis_stub.StrictRedis(host=str(tmp_path) + family))
-    return (L.LunarLanderLearner if family == "LL" else L.VSACLearner)(str(p), **kw)
-
-
 def _scramble_targets(core, seed):
     g = torch.Generator().manual_seed(seed)
     named = core.get_named()

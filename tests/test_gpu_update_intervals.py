@@ -6,7 +6,6 @@ update, then the actor side and / or the targets put back) at the 1e-4 bar; what
 for bit; replicas with different intervals equal uniform handles; every step path and a change between graph launches
 follow the schedule in stream order; prioritized replay keeps rewriting priorities; bad values are rejected; the learner
 surface reports NaN actor losses on critic-only steps and keeps the phase across a checkpoint."""
-import contextlib
 import json
 import math
 import os
@@ -17,8 +16,8 @@ import torch
 import care_port as cp
 import redis_stub
 import sac_port as sp
-from _golden import (REL, CareCase, care_core_config, check_forced, check_port_state, core_config, cuda_relu_masks,
-                     rel_scalar, sync_core_to_port)
+from _golden import REL, check_forced, check_port_state, core_config, cuda_relu_masks, rel_scalar, sync_core_to_port
+from _harness import LL_CFG, SMALL, _config, _inputs, _plan, _stream_run, cuda
 
 pytestmark = pytest.mark.gpu
 
@@ -26,40 +25,8 @@ PARAMS, ADAM_M, ADAM_V = 0, 1, 2
 PLANS = ["chained", "per_layer", "mtsac_weighted", "care_m", "care_o"]
 
 
-@pytest.fixture(scope="module")
-def cuda():
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from distributed_sac_b200 import _lib
-    _lib.load()
-    return torch.device("cuda", 0)
-
-
-def _plan(name):
-    """(spec, care, precision): layer-chained fp32; per-layer wgmma with gradient slices (batch >= 512) and per-task
-    temperatures; MTSAC weighted loss on the per-layer FFMA plan (hidden width > 256, forked weight gradients); CARE(M);
-    CARE(O)."""
-    if name == "chained":
-        return sp.ll_spec(), False, 0
-    if name == "per_layer":
-        return sp.SacSpec(state_dim=17, act_dim=3, actor_hidden=[96, 80], critic_hidden=[72, 104], batch=640, num_tasks=5), False, 1
-    if name == "mtsac_weighted":
-        return sp.SacSpec(state_dim=12, act_dim=4, actor_hidden=[260, 64], critic_hidden=[264, 72], batch=200, num_tasks=4,
-                          weighted_loss=True), False, 0
-    return CareCase({"care_m": "care_small_s4", "care_o": "care_o_small_s4"}[name]).spec, True, 1
-
-
-def _config(spec, care, precision, replicas=1):
-    return (care_core_config if care else core_config)(spec, replicas=replicas, precision=precision)
-
-
-def _inputs(spec, care, R, i):
-    gen = torch.Generator().manual_seed(2000 + i)
-    mod = cp if care else sp
-    bs = [mod.synthetic_batch(spec, seed=100 * i + r + 7) for r in range(R)]
-    b = [torch.stack([x[j] for x in bs]) for j in range(5)]
-    e1, e2 = (torch.randn(R, spec.batch, spec.act_dim, generator=gen) for _ in range(2))
-    return b, e1, e2
+def _inputs_iv(spec, care, R, i):
+    return _inputs(spec, care, R, i, noise_seed=2000, batch_seed=7)
 
 
 def _is_actor(name):
@@ -152,7 +119,7 @@ def test_skipped_updates_leave_state_bit_identical(cuda, plan):
     core.set_update_intervals(2, 3)
     for i in range(6):
         before, sb = _state(core)
-        b, e1, e2 = _inputs(spec, care, 1, i)
+        b, e1, e2 = _inputs_iv(spec, care, 1, i)
         core.step(*b, e1, e2)
         after, sa = _state(core)
         actor, target = _kinds(sb[0] + 1, 2, 3)
@@ -193,7 +160,7 @@ def test_mixed_replicas_equal_uniform_handles(cuda, plan):
             core.set_named(params, replica=r)
     n = 6
     for i in range(n):
-        b, e1, e2 = _inputs(spec, care, R, i)
+        b, e1, e2 = _inputs_iv(spec, care, R, i)
         for core in [mixed] + uniform:
             core.step(*b, e1, e2)
     Lm = mixed.read_losses(n)
@@ -209,9 +176,6 @@ def test_mixed_replicas_equal_uniform_handles(cuda, plan):
 
 
 # ---- 4. paths and stream order ---------------------------------------------------------------------------------------
-SMALL = sp.SacSpec(state_dim=8, act_dim=2, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=128)
-
-
 def test_multi_step_graphs_equal_single_steps(cuda):
     """One step_sampled(ring, 13) call (8/4/2/1-step graphs) == 13 single calls, bit for bit."""
     from distributed_sac_b200.core import Replay, SacCore
@@ -245,7 +209,7 @@ def test_step_entry_points_follow_the_schedule(cuda):
     for c in (dev, host):
         c.set_update_intervals(2, 1)
     for i in range(4):
-        b, e1, e2 = _inputs(SMALL, False, 1, i)
+        b, e1, e2 = _inputs_iv(SMALL, False, 1, i)
         dev.step(*b, e1, e2)
         Lh = host.step_host(*b, e1, e2)
         Ld = dev.read_losses(1)[0]
@@ -264,41 +228,21 @@ def test_step_entry_points_follow_the_schedule(cuda):
     host.close()
 
 
-def _stream_run(mode, set_iv, sync_before_set):
-    """16 sampled steps; intervals (2, 3) set on every replica after step 8 if set_iv."""
-    from distributed_sac_b200.core import Replay, SacCore
-    core = SacCore(core_config(SMALL, replicas=2), 0, seed=7)
-    rb = Replay(core, capacity=4096, where="host" if mode == "host" else "device", seed=3)
-    stream = torch.cuda.Stream() if mode == "stream" else None
-    with torch.cuda.stream(stream) if stream is not None else contextlib.nullcontext():
-        rb.fill_synthetic(4096, seed=9)
-        core.prepare(rb)
+def _read(core):
+    return core.read_losses(16).nan_to_num(7.0), core.export_arena(0, 0), core.export_arena(1, 1), core.get_steps(1)
 
-        def eight():
-            if mode == "host":
-                for _ in range(8):
-                    core.update_sampled(rb)
-            else:
-                core.step_sampled(rb, 8)
-        eight()
-        if sync_before_set:
-            torch.cuda.synchronize()
-        if set_iv:
-            core.set_update_intervals(2, 3)
-        eight()
-        out = core.read_losses(16).nan_to_num(7.0), core.export_arena(0, 0), core.export_arena(1, 1), core.get_steps(1)
-    rb.close()
-    core.close()
-    return out
+
+def _set_iv(core):
+    core.set_update_intervals(2, 3)
 
 
 @pytest.mark.parametrize("mode", ["stream", "legacy", "host"])
 def test_set_update_intervals_is_stream_ordered(cuda, mode):
     """A change enqueued right behind a graph launch (after prepare) lands exactly between the steps before and after it:
     the same as setting it on an idle device.  On a side stream, on the legacy default stream and with a pinned-host ring."""
-    lx, ax, mx, sx = _stream_run(mode, True, False)
-    ly, ay, my, sy = _stream_run(mode, True, True)
-    lz, _, _, sz = _stream_run(mode, False, False)
+    lx, ax, mx, sx = _stream_run(mode, _set_iv, False, _read)
+    ly, ay, my, sy = _stream_run(mode, _set_iv, True, _read)
+    lz, _, _, sz = _stream_run(mode, None, False, _read)
     assert torch.equal(lx, ly) and torch.equal(ax, ay) and torch.equal(mx, my) and sx == sy
     assert torch.equal(lx[:8], lz[:8])
     assert (lx[8:, :, 1] == 7.0).sum() == 2 * 4 and (lz[:, :, 1] == 7.0).sum() == 0
@@ -347,7 +291,7 @@ def test_bad_intervals_are_rejected_and_copy_keeps_them(cuda):
     assert core.get_update_intervals(0) == (1, 1) and core.get_update_intervals(1) == (3, 2)
     core.set_update_intervals(2 ** 30, 2 ** 30, replica=1)                 # the largest accepted value
     core.set_update_intervals(3, 2, replica=1)
-    b, e1, e2 = _inputs(SMALL, False, 2, 0)
+    b, e1, e2 = _inputs_iv(SMALL, False, 2, 0)
     fresh.set_update_intervals(3, 2, replica=1)
     for c in (core, fresh):
         c.step(*b, e1, e2)
@@ -359,7 +303,7 @@ def test_bad_intervals_are_rejected_and_copy_keeps_them(cuda):
     core.copy_replica(1, 0)
     assert core.get_steps(0) == (5, 1, 1) and core.get_update_intervals(0) == (1, 1)
     core.set_update_intervals(3, 2, replica=0)
-    b, e1, e2 = _inputs(SMALL, False, 2, 1)
+    b, e1, e2 = _inputs_iv(SMALL, False, 2, 1)
     for t in b + [e1, e2]:
         t[0] = t[1]
     core.step(*b, e1, e2)                                # n = 6: an actor step and a target step for both
@@ -371,10 +315,6 @@ def test_bad_intervals_are_rejected_and_copy_keeps_them(cuda):
 
 
 # ---- 7. learner surface ----------------------------------------------------------------------------------------------
-LL_CFG = {"num_tasks": 10, "device": "cuda", "buffer_size": 1e6, "reward_scale": 1, "batch_size": 256, "gamma": 0.99,
-          "lr_actor": 3e-4, "lr_critic": 3e-4, "log_alpha": 0, "tau": 0.005, "num_learn": 1, "num_time_step": 1,
-          "random_step": 5000, "start_memory_len": 5000}
-
 
 def test_learner_update_intervals_and_checkpoint(cuda, tmp_path):
     """LunarLanderLearner(actor_update_interval=3, target_update_interval=2): update() returns NaN actor loss on critic-only

@@ -7,6 +7,8 @@ import re
 
 import pytest
 
+from _harness import BlobStubLib
+
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
@@ -74,36 +76,6 @@ def test_product_fails_loudly_without_cuda():
     from distributed_sac_b200.core import CoreConfig, SacCore
     with pytest.raises(RuntimeError, match="no CPU fallback"):
         SacCore(CoreConfig())
-
-
-class BlobStubLib:
-    """CPU stand-in for b200sac_blob_*: emulates the device gather (payload float j = arena[src[j]] -> image bytes at dst[j])."""
-
-    def __init__(self, arena):
-        self.arena = arena
-
-    def b200sac_blob_template(self, h, replica, image, image_bytes, n_floats, src, dst):
-        import ctypes as C
-        import numpy as np
-        self.image = np.ctypeslib.as_array(C.cast(image, C.POINTER(C.c_uint8)), shape=(image_bytes,)).copy()
-        self.src = np.ctypeslib.as_array(C.cast(src, C.POINTER(C.c_int32)), shape=(n_floats,)).copy()
-        self.dst = np.ctypeslib.as_array(C.cast(dst, C.POINTER(C.c_int32)), shape=(n_floats,)).copy()
-        return 0
-
-    def b200sac_blob_begin(self, h, stream):
-        import numpy as np
-        out = self.image.copy()
-        vals = np.ascontiguousarray(self.arena[self.src], dtype=np.float32).view(np.uint8).reshape(-1, 4)
-        for b in range(4):
-            out[self.dst + b] = vals[:, b]
-        self.out = out
-        return 0
-
-    def b200sac_blob_wait(self, h, ptr, n):
-        import ctypes as C
-        C.cast(ptr, C.POINTER(C.c_void_p))[0] = self.out.ctypes.data
-        C.cast(n, C.POINTER(C.c_int64))[0] = self.out.size
-        return 0
 
 
 def test_parameters_blob_device_image_round_trips():

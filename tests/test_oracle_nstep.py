@@ -6,24 +6,8 @@ import pytest
 
 import nstep_ref
 import redis_stub
+from _harness import _play, random_pushes
 from distributed_sac_b200.stitch import Stitcher
-
-
-def random_pushes(rng, n_pushes, T, streams, max_rows, plain_every=0):
-    """Random interleavings: per row a stream, a task (a stream mostly keeps its task), d and cut."""
-    task_of = {s: int(rng.integers(T)) for s in range(streams)}
-    for p in range(n_pushes):
-        n = int(rng.integers(1, max_rows + 1))
-        sid = rng.integers(streams, size=n).astype(np.int32)
-        for s in np.unique(sid):
-            if rng.random() < 0.1:
-                task_of[int(s)] = int(rng.integers(T))
-        task = np.array([task_of[int(s)] for s in sid])
-        d = (rng.random(n) < 0.08).astype(np.float32)
-        cut = (rng.random(n) < 0.05).astype(np.uint8)
-        r = rng.standard_normal(n).astype(np.float32)
-        plain = plain_every and p % plain_every == plain_every - 1
-        yield task, r, d, (None if plain else sid), (None if plain else cut)
 
 
 @pytest.mark.parametrize("T,cap,streams,max_rows", [(0, 64, 5, 12), (0, 16, 3, 40), (3, 48, 6, 20), (4, 32, 9, 70)])
@@ -67,24 +51,6 @@ def test_fold_equals_fp64_nstep_return():
                 assert dd[i] == want[2] and m[i] == want[3] and last[i] == i + m[i] - 1
             if n == 1:
                 assert np.array_equal(R, r) and np.all(disc == np.float32(gamma)) and np.array_equal(dd, d)
-
-
-def _play(rng, n_players, n_rows, time_limit):
-    """Interleaved transitions of n_players environments: (player, episode, t) per row plus the pickled payloads."""
-    state = [rng.standard_normal(8).astype(np.float32) for _ in range(n_players)]
-    ep, t = [0] * n_players, [0] * n_players
-    rows = []
-    for _ in range(n_rows):
-        p = int(rng.integers(n_players))
-        nxt = rng.standard_normal(8).astype(np.float32)
-        done = bool(rng.random() < 0.1)
-        rows.append(((p, ep[p], t[p]), (state[p], rng.standard_normal(2).astype(np.float32), float(rng.standard_normal()), nxt, done)))
-        t[p] += 1
-        if done or t[p] == time_limit:              # a time-limit reset carries no flag: the next state just does not match
-            state[p], ep[p], t[p] = rng.standard_normal(8).astype(np.float32), ep[p] + 1, 0
-        else:
-            state[p] = nxt
-    return rows
 
 
 def test_stitcher_rebuilds_trajectories_from_interleaved_players():

@@ -48,10 +48,10 @@ def test_published_blob_loads_into_the_reference_actor(tmp_path):
     assert list(km) == list(sd)
 
     # stand-in core: the arena of a LunarLander learner filled with the reference Actor's state; the device gather of
-    # b200sac_blob_* is emulated on the CPU (tests/test_host_logic.py::BlobStubLib)
+    # b200sac_blob_* is emulated on the CPU (tests/_harness.py::BlobStubLib)
     import distributed_sac_b200.core as core_mod
     from distributed_sac_b200.core import CoreConfig, SacCore, layout
-    from test_host_logic import BlobStubLib
+    from _harness import BlobStubLib
     cfg = CoreConfig(batch=64)
     table, arena, _tr = layout(cfg)
     flat = np.zeros(arena, np.float32)
