@@ -303,8 +303,28 @@ struct GraphKey {
   }
 };
 
+// The environment switches that select a plan path or tile for tests and measurement scripts (none is needed in
+// production).  env_switches() is the library's only reader of the environment: b200sac_create calls it once and the
+// handle keeps the result, so a handle launches what it chose when it was built; the wgmma GEMM test entry points call
+// it per call.
+struct EnvSwitches {
+  bool fuse = true;          // B200SAC_FUSE=0: the per-layer plan even where the layer-chained one is eligible
+  int tc_bn = 0;             // B200SAC_TC_BN: every wgmma launch takes this tile width (128 or 160; any other value 64); 0: unset
+  bool pair128 = false;      // B200SAC_TC_PAIR128=1: 128-wide wgmma tiles take the paired flavour
+  bool chain_dbg = false;    // B200SAC_CHAIN_DBG set: clock64 timelines of the layer-chained kernels (scripts/chain_timeline.py)
+};
+static EnvSwitches env_switches() {
+  EnvSwitches s;
+  if (const char* e = getenv("B200SAC_FUSE")) s.fuse = e[0] != '0';
+  if (const char* e = getenv("B200SAC_TC_BN")) { const int b = atoi(e); s.tc_bn = b == 128 ? 128 : (b == 160 ? 160 : 64); }
+  if (const char* e = getenv("B200SAC_TC_PAIR128")) s.pair128 = e[0] == '1';
+  s.chain_dbg = getenv("B200SAC_CHAIN_DBG") != nullptr;
+  return s;
+}
+
 struct b200sac {
   b200sac_cfg cfg;
+  EnvSwitches env;                // read at create
   int device = 0;
   Layout L;
   StepConst K;
@@ -375,7 +395,7 @@ struct b200sac {
   Event ev_blob_snap[2], ev_blob_done[2];
   DevMem<CUtensorMap> d_cmaps;    // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
                                   // weight-gradient operands [R][nw]
-  DevMem<long long> chain_dbg;    // B200SAC_CHAIN_DBG=1: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
+  DevMem<long long> chain_dbg;    // env.chain_dbg: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
   DevMem<float> step_d;           // b200sac_step: the caller's minibatch as packed rows [R][B][row_stride] (stable graph pointers)
   PinnedMem<float> loss_h;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
   float* loss_h_dev = nullptr;    // its device-side address
@@ -521,10 +541,9 @@ static bool tc_eligible(const GemmProb& p) {
   return p.M >= 32 && p.N >= 32 && p.K >= 32;
 }
 
-// Tile variants of the wgmma GEMM (gemm_tc.cuh): 128x64, 128x128 (B200SAC_TC_PAIR128=1: the paired flavour), 128x160.
-// A step plan reads the switch once, when it is built, and keeps the choice on its launches (Launch::pair128).
+// Tile variants of the wgmma GEMM (gemm_tc.cuh): 128x64, 128x128 (EnvSwitches::pair128: the paired flavour), 128x160.
+// A step plan keeps the choice on its launches (Launch::pair128).
 typedef void (*TcKernel)(const TcProb*, const int*, int, int);
-static bool tc_pair128() { const char* e = getenv("B200SAC_TC_PAIR128"); return e && e[0] == '1'; }
 static TcKernel tc_kernel(int bn, bool pair128) {
   if (bn == 160) return gemm_tc_kernel<160, false>;
   if (bn == 128) return pair128 ? (TcKernel)gemm_tc_kernel<128, true> : (TcKernel)gemm_tc_kernel<128, false>;
@@ -544,42 +563,28 @@ static cudaError_t tc_set_attrs() {
 // power limit): a tile costs a ~3k-cycle prologue, 1.2k + 11.7 bn cycles per 32-wide k chunk (1.9k / 2.65k / 3.05k at
 // bn = 64 / 128 / 160; 3.1k for the paired 128-wide tile) and an epilogue of ~38 bn cycles; tiles beyond one per SM wait for a second wave.  The plan
 // builder takes the cheapest width.
-static double tc_group_cost(const std::vector<GemmProb>& v, int bn, int R) {
+static double tc_group_cost(const std::vector<GemmProb>& v, int bn, int R, bool pair128) {
   long long tiles = 0;
   int nk = 1;
   for (auto& p : v) {
     tiles += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
     nk = std::max(nk, (p.K + TC_BK - 1) / TC_BK);
   }
-  const double chunk = (bn == 128 && tc_pair128()) ? 3100.0 : 1200.0 + 11.7 * bn;
+  const double chunk = (bn == 128 && pair128) ? 3100.0 : 1200.0 + 11.7 * bn;
   const double tile = 3000.0 + nk * chunk + 38.0 * bn;
   const int sms = sm_count();
   const long long waves = (tiles * R + sms - 1) / sms;
   return (double)waves * tile;
 }
-// B200SAC_TC_BN forces the tile width: 128 or 160 select that width, any other value 64; unset, `unforced` is returned.
-static int tc_forced_bn(int unforced) {
-  const char* e = getenv("B200SAC_TC_BN");
-  if (!e) return unforced;
-  const int b = atoi(e);
-  return b == 128 ? 128 : (b == 160 ? 160 : 64);
-}
-static int tc_pick_bn(const std::vector<GemmProb>& v, int R) {
-  if (const int b = tc_forced_bn(0)) return b;
+static int tc_pick_bn(const std::vector<GemmProb>& v, int R, const EnvSwitches& sw) {
+  if (sw.tc_bn) return sw.tc_bn;
   int maxN = 0;
   for (auto& p : v) maxN = std::max(maxN, p.N);
-  if (getenv("B200SAC_TC_OLDRULE")) {             // round-1 rule: 128 when the group still fills most of the GPU with 128x128 tiles
-    long long c128 = 0;
-    for (auto& p : v) c128 += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + 127) / 128);
-    return (maxN >= 256 && c128 * R >= 96) ? 128 : 64;
-  }
-  const bool no160 = getenv("B200SAC_TC_NO160") != nullptr;
   int best = 64;
-  double cost = tc_group_cost(v, 64, R);
+  double cost = tc_group_cost(v, 64, R, sw.pair128);
   for (int bn : {128, 160}) {
-    if (bn == 160 && no160) continue;
     if (maxN < 2 * bn - 64) continue;             // a lone, mostly empty wide tile is never better than 64-wide ones
-    const double c = tc_group_cost(v, bn, R);
+    const double c = tc_group_cost(v, bn, R, sw.pair128);
     if (c < cost) { cost = c; best = bn; }
   }
   return best;
@@ -622,9 +627,9 @@ static int make_tc_prob(const GemmProb& p, int rep, TcProb& t, int bn = 64) {
 //   E   chain_kernel<BWD>  {actor}: d(mu|log_std), input-gradient chain                          -> wgrad + Adam
 // Eligible: exact-fp32 mode, no CARE, every hidden width a multiple of 4 and <= 256, obs+act <= 252.
 // ------------------------------------------------------------------------------------------
-static bool fused_eligible(const b200sac_cfg& c) {
-  if (c.precision != 0 || c.care) return false;
-  if (const char* e = getenv("B200SAC_FUSE")) if (e[0] == '0') return false;
+static bool fused_eligible(const b200sac* h) {
+  const b200sac_cfg& c = h->cfg;
+  if (c.precision != 0 || c.care || !h->env.fuse) return false;
   for (int i = 0; i < c.n_actor_hidden; ++i) if (c.actor_hidden[i] % 4 || c.actor_hidden[i] > CH_MAXW) return false;
   for (int i = 0; i < c.n_critic_hidden; ++i) if (c.critic_hidden[i] % 4 || c.critic_hidden[i] > CH_MAXW) return false;
   if (c.state_dim + c.num_tasks + c.act_dim > CH_MAXW - 4) return false;
@@ -834,15 +839,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
         expand(s_, trial);
         const std::vector<GemmProb> o = tc_only(trial);
         if (o.empty()) { S = s_; break; }
-        if (getenv("B200SAC_TC_OLDRULE")) {          // round-1 rule: the finest split that fits one wave
-          const int bn = tc_pick_bn(o, R);
-          long long ct = 0;
-          for (auto& p : o) ct += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
-          S = s_;
-          if (ct * R <= sms) break;
-          continue;
-        }
-        const double cost = tc_group_cost(o, tc_pick_bn(o, R), R);
+        const double cost = tc_group_cost(o, tc_pick_bn(o, R, h->env), R, h->env.pair128);
         if (cost < best) { best = cost; S = s_; }
       }
     }
@@ -857,18 +854,11 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
       Launch l;
       int maxM = 0, maxN = 0;
       for (auto& p : tc) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; }
-      const int bn = tc_pick_bn(tc, R);          // tile width: the cheapest of 64 / 128 / 160 under tc_group_cost's model
-      if (getenv("B200SAC_PLAN_DBG")) {
-        long long tiles = 0;
-        for (auto& p : tc) tiles += (long long)((p.M + TC_BM - 1) / TC_BM) * ((p.N + bn - 1) / bn);
-        fprintf(stderr, "[plan] launch %zu: wgmma bn=%d problems=%zu tiles=%lld:", h->plan.size(), bn, tc.size(), tiles);
-        for (auto& p : tc) fprintf(stderr, " %s%dx%dx%d", p.mode == GEMM_FWD ? "F" : (p.mode == GEMM_DGRAD ? "D" : "W"), p.M, p.N, p.K);
-        fprintf(stderr, "\n");
-      }
+      const int bn = tc_pick_bn(tc, R, h->env);  // tile width: the cheapest of 64 / 128 / 160 under tc_group_cost's model
       l.kind = L_GEMM_TC;
       l.branch = branch;
       l.bn = bn;
-      l.pair128 = bn == 128 && tc_pair128();
+      l.pair128 = bn == 128 && h->env.pair128;
       l.sched = actor_side ? &h->cnt[0].sched : nullptr;
       l.split = split;
       l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
@@ -895,7 +885,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
     const std::vector<GemmProb> g(ps.begin() + i0, ps.begin() + std::min(ps.size(), i0 + GS_MAXG));
     Launch l;
     int maxM = 0, maxN = 0;
-    bool thin = getenv("B200SAC_NO_THIN") == nullptr;
+    bool thin = true;
     for (auto& p : g) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
     l.kind = L_GEMM_SMALL;
     l.branch = branch;
@@ -940,13 +930,12 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
   CareMixFwdArgs A;
   memset(&A, 0, sizeof(A));
   A.njobs = (int)jobs.size(); A.nl = nmix; A.K = Kenc; A.B = B;
-  if (const char* e = getenv("B200SAC_CMF_SKIP")) A.dbg_skip = atoi(e);
   A.params = h->params; A.rsP = rsP;
   A.XS = h->XS.p; A.rsXS = h->XS.rs; A.ldx = h->K.obs;
   A.tid = (const int*)h->tid.p; A.rsR = h->r.rs;
   A.row_w = h->care_row_w; A.off_att = h->care_off_att; A.off_ctx = h->care_off_ctx; A.mo = c.mix_out; A.co = c.ctx_out;
   A.sched = actor_side ? &h->cnt[0].sched : nullptr; A.sched_stride = kSchedStride;
-  bool ok = nmix >= 1 && nmix <= CMF_MAXL && (int)jobs.size() <= CMF_MAXJOBS && getenv("B200SAC_NO_CARE_FUSED") == nullptr;
+  bool ok = nmix >= 1 && nmix <= CMF_MAXL && (int)jobs.size() <= CMF_MAXJOBS;
   for (int l = 0; ok && l < nmix; ++l) {
     A.w_off[l] = L.mix[l].w; A.b_off[l] = L.mix[l].b; A.in[l] = L.mix[l].in; A.out[l] = L.mix[l].out;
     A.maxw = std::max(A.maxw, L.mix[l].out);
@@ -1054,7 +1043,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   // 128-bit column mapping when every row pitch / tensor offset involved is a multiple of 4 floats (l.bn = 4 marks it)
   // -- for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
   // few to fill the GPU
-  const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0 && getenv("B200SAC_HEADBWD_NARROW") == nullptr;
+  const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0;
   l.bn = wide ? 4 : 1;
   const int cols = wide ? kHb4Cols : kHbCols;
   l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
@@ -1113,7 +1102,7 @@ int PlanBuilder::build_plan_fused() {
   std::vector<WMap> wmaps;                 // weight-gradient operands [B rows][cols] that get a tensor map
   struct FMap { int64_t off; int K, N, ld; };
   std::vector<FMap> fmaps;                 // forward weight matrices that need a tensor map (one per chained forward stage)
-  if (getenv("B200SAC_CHAIN_DBG")) {
+  if (h->env.chain_dbg) {
     CU(cudaMalloc(h->chain_dbg.put(), sizeof(long long) * CH_DBG_SLOTS * 16));
     CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
   }
@@ -1374,7 +1363,7 @@ void PlanBuilder::build_plan_layered() {
   // FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads the rest of the
   // backward chain.  The weight-gradient launch goes to the fork stream and the chain continues at once (the kernels hold
   // <= 2 CTAs per SM, so both fit); Adam joins.  (tensor-core tiles own a whole SM each: grouping is better there.)
-  const bool use_fork = (c.precision == 0) && !c.care && getenv("B200SAC_NO_FORK") == nullptr;
+  const bool use_fork = (c.precision == 0) && !c.care;
   if (c.care) {
     // encoded states of [s'; s] with the critic's (== actor's, tied) encoder and of s' with the target's
     care_tables({0, 1});
@@ -1682,7 +1671,6 @@ static int build_plan(b200sac* h) {
 // drains; every kernel begins with griddepcontrol.wait (common.cuh::kstamp), so data dependencies hold.
 // CLUSTER_Y > 1: thread-block clusters of (1, CLUSTER_Y, 1) -- the CTAs with equal blockIdx.x / z are co-scheduled and can
 // read each other's shared memory.
-static bool g_use_pdl = true;
 template <int CLUSTER_Y = 1, typename... KArgs, typename... Args>
 static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
   cudaLaunchConfig_t cfg;
@@ -1695,11 +1683,9 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
     attr[n].val.clusterDim.x = 1; attr[n].val.clusterDim.y = CLUSTER_Y; attr[n].val.clusterDim.z = 1;
     ++n;
   }
-  if (g_use_pdl) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
+  attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[n].val.programmaticStreamSerializationAllowed = 1;
+  ++n;
   cfg.attrs = attr;
   cfg.numAttrs = n;
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
@@ -1872,10 +1858,9 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   b200sac* h = owner.get();
   if (!h) return fail(B200SAC_ERR_NOMEM, "out of host memory");
   h->cfg = *cfg;
+  h->env = env_switches();
   h->device = device;
   h->R = cfg->replicas;
-  // programmatic dependent launch with the exit-time trigger only (see common.cuh::KStamp); B200SAC_PDL=0 turns it off
-  if (const char* e = getenv("B200SAC_PDL")) g_use_pdl = (e[0] != '0');      // process-wide switch, read at every create
 
   build_layout(cfg, h->L);
   const Layout& L = h->L;
@@ -1905,7 +1890,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   CU(cudaMemset(h->adam_m, 0, sizeof(float) * L.trainable * R));
   CU(cudaMemset(h->adam_v, 0, sizeof(float) * L.trainable * R));
   CU(cudaMemset(h->grads, 0, sizeof(float) * L.trainable * R));
-  h->gslices = (cfg->batch >= kSplitKMin && getenv("B200SAC_NO_SPLITK") == nullptr) ? kSplitK : 1;   // K of every weight gradient = batch
+  h->gslices = cfg->batch >= kSplitKMin ? kSplitK : 1;   // K of every weight gradient = batch
   if (h->gslices > 1) {     // never-written entries of slices >= 1 must read as zero (Adam sums all slices)
     CU(cudaMalloc(h->grads_x.put(), sizeof(float) * L.trainable * R * (h->gslices - 1)));
     CU(cudaMemset(h->grads_x, 0, sizeof(float) * L.trainable * R * (h->gslices - 1)));
@@ -2077,7 +2062,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   CU(cudaEventCreateWithFlags(h->ev_in.put(), cudaEventDisableTiming));
   CU(cudaEventCreateWithFlags(h->ev_out.put(), cudaEventDisableTiming));
 
-  h->fused = fused_eligible(*cfg);
+  h->fused = fused_eligible(h);
   if (int rc = build_plan(h)) return rc;
   CU(cudaDeviceSynchronize());
   *out = owner.release();
@@ -2716,7 +2701,8 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   p.A = A; p.B = B; p.bias = bias; p.mask = mask; p.C = C; p.C2 = C2;
   p.M = M; p.N = N; p.K = K; p.lda = lda; p.ldb = ldb; p.ldc = ldc; p.ldmask = ldmask; p.mode = mode; p.relu = relu;
   if (!tc_eligible(p)) return fail(B200SAC_ERR_INVALID, "problem not eligible for the wgmma path (need 16-B aligned operands, lda/ldb %% 4 == 0, M,N,K >= 32)");
-  const int bn = tc_forced_bn(64);
+  const EnvSwitches sw = env_switches();
+  const int bn = sw.tc_bn ? sw.tc_bn : 64;
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   DevMem<TcProb> d;
@@ -2724,7 +2710,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
+  tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize((cudaStream_t)stream);
   if (e != cudaSuccess) return fail(B200SAC_ERR_CUDA, "gemm_tc_kernel failed: %s", cudaGetErrorString(e));
@@ -2742,7 +2728,8 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   memset(&p, 0, sizeof(p));
   p.A = A; p.B = B; p.C = C; p.M = M; p.N = N; p.K = K; p.mode = mode;
   p.lda = mode == GEMM_WGRAD ? M : K; p.ldb = mode == GEMM_FWD ? K : N; p.ldc = N;
-  const int bn = tc_forced_bn(64);
+  const EnvSwitches sw = env_switches();
+  const int bn = sw.tc_bn ? sw.tc_bn : 64;
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   t.dbg = dbg;
@@ -2751,7 +2738,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
   CU(tc_set_attrs());
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
-  for (int it = 0; it < 3; ++it) tc_kernel(bn, tc_pair128())<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
+  for (int it = 0; it < 3; ++it) tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out96, dbg, 96 * 8, cudaMemcpyDeviceToHost));
   return 0;

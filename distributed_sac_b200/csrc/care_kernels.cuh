@@ -413,7 +413,6 @@ struct CareMixFwdArgs {
   const int* tid; long long rsR;
   int row_w, off_att, off_ctx, mo, co;
   int maxw;                                // widest hidden / output layer
-  int dbg_skip;                            // measurement only (B200SAC_CMF_SKIP): 1 skip the encoder tasks, 2 the mix, 4 the weight load
   CareMixFwdJob job[CMF_MAXJOBS];
   int sched_stride; const int* sched;      // as in CareTabArgs
 };
@@ -460,7 +459,7 @@ __global__ void __launch_bounds__(CMF_THREADS, 1) care_mixfwd_kernel(const __gri
   const float* par = A.params + (long long)rep * A.rsP + J.inst_delta;
   if (!skip) {
     int wpos = 0, bpos = wtot;
-    for (int l = 0; l < A.nl && !(A.dbg_skip & 4); ++l) {
+    for (int l = 0; l < A.nl; ++l) {
       const int nW = K * A.out[l] * A.in[l], nb = K * A.out[l];
       const float* gW = par + A.w_off[l];
       const float* gb = par + A.b_off[l];
@@ -503,7 +502,7 @@ __global__ void __launch_bounds__(CMF_THREADS, 1) care_mixfwd_kernel(const __gri
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   __syncthreads();
   // ---- one task = (encoder k, group of 8 rows): walks the encoder's layers for its rows; tasks are independent ------------
-  for (int task = w; task < K * (CMF_ROWS / 8) && !(A.dbg_skip & 1); task += CMF_THREADS / 32) {
+  for (int task = w; task < K * (CMF_ROWS / 8); task += CMF_THREADS / 32) {
     const int k = task / (CMF_ROWS / 8), g = (task - k * (CMF_ROWS / 8)) * 8;
     int in_off = xs_off;                   // layer 0 reads the shared input tile; later layers this encoder's own hidden tile
     int in_pitch_k = 0;                    // 0: shared tile; else per-encoder stride
@@ -573,7 +572,6 @@ __global__ void __launch_bounds__(CMF_THREADS, 1) care_mixfwd_kernel(const __gri
   }
   __syncthreads();
   // ---- mix: [ctx[t] | sum_k att_k Z_k / sum_k att_k], k ascending ------------------------------------------------------------
-  if (A.dbg_skip & 2) return;
   for (int e = tid; e < nrows * A.co; e += CMF_THREADS) {
     const int r = e / A.co, j = e - r * A.co;
     const int rg = J.out_row0 + r0 + r;
