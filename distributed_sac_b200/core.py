@@ -48,6 +48,7 @@ class CoreConfig:
     care_original: bool = False          # CARE(O): trainable context encoder (use_modified_care: false)
     emb_dim: int = 50
     lr_ctx: float = 3e-4
+    grad_clip: bool = False              # the step plan with gradient-norm clipping and norms (SacCore.set_grad_clip)
 
     @property
     def obs_dim(self):
@@ -71,6 +72,7 @@ class CoreConfig:
         c.beta1, c.beta2, c.adam_eps = self.beta1, self.beta2, self.adam_eps
         c.log_alpha_init = self.log_alpha_init
         c.care = (2 if self.care_original else 1) if self.care else 0
+        c.grad_clip = int(self.grad_clip)
         if self.care:
             c.emb_dim, c.lr_ctx = self.emb_dim, self.lr_ctx
             c.num_encoders, c.mix_out, c.ctx_in, c.ctx_out = self.num_encoders, self.mix_out, self.ctx_in, self.ctx_out
@@ -324,9 +326,37 @@ class SacCore:
             t = t if target_every is None else int(target_every)
             _lib.check(self.lib.b200sac_set_update_intervals(self._h, r, a, t, _stream()))
 
+    # ---- gradient-norm clipping (b200sac_set/get_grad_clip, b200sac_read_grad_norms; handles with grad_clip=True) ------
+    CLIP_NAMES = ("critic", "actor", "ctx")
+
+    def get_grad_clip(self, replica=0) -> Dict[str, float]:
+        """{critic, actor, ctx} max-norm thresholds of one replica (no synchronisation); inf = no clipping."""
+        v = [C.c_double() for _ in self.CLIP_NAMES]
+        _lib.check(self.lib.b200sac_get_grad_clip(self._h, int(replica), *[C.byref(x) for x in v]))
+        return {k: x.value for k, x in zip(self.CLIP_NAMES, v)}
+
+    def set_grad_clip(self, critic=None, actor=None, ctx=None, replica=None):
+        """clip_grad_norm_ thresholds of the critic, actor and CARE(O) context-encoder optimizers of one replica
+        (replica=None: all of them) on the current stream; a name left out keeps its value, inf turns clipping off.
+        Steps enqueued afterwards use them."""
+        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+            cur = self.get_grad_clip(r)
+            for k, v in dict(critic=critic, actor=actor, ctx=ctx).items():
+                if v is not None:
+                    cur[k] = float(v)
+            _lib.check(self.lib.b200sac_set_grad_clip(self._h, r, cur["critic"], cur["actor"], cur["ctx"], _stream()))
+
+    def read_grad_norms(self, n_last: int = 1) -> torch.Tensor:
+        """Pre-clip gradient norms [n_last][R][3] (critic, actor, context encoder) of the last steps, aligned with read_losses;
+        NaN where that optimizer did not step."""
+        out = torch.empty(n_last, self.cfg.replicas, 3)
+        _lib.check(self.lib.b200sac_read_grad_norms(self._h, int(n_last), _ptr(out), _stream()))
+        return out
+
     def copy_replica(self, src: int, dst: int):
         """Replica dst's parameters (targets, log_alpha included), Adam moments and step counters become a copy of src's,
-        device to device on the current stream.  Hyperparameters, update intervals and replay data stay dst's own."""
+        device to device on the current stream.  Hyperparameters, update intervals, gradient-clipping thresholds and replay
+        data stay dst's own."""
         _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
 
     def soft_update(self, tau: float, critic: Optional[int] = None):

@@ -33,6 +33,7 @@
 #include "chain2.cuh"
 #include "per_kernels.cuh"
 #include "nstep_kernels.cuh"
+#include "clip_kernels.cuh"
 
 using namespace bsac;
 
@@ -124,6 +125,7 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->replicas < 1 || c->replicas > 4096) return fail(B200SAC_ERR_INVALID, "1 <= replicas <= 4096 required");
   if (c->precision != 0 && c->precision != 1) return fail(B200SAC_ERR_INVALID, "precision must be 0 (fp32 FFMA) or 1 (3xTF32 wgmma)");
   if (c->care != 0 && c->care != 1 && c->care != 2) return fail(B200SAC_ERR_INVALID, "care must be 0, 1 (CARE(M)) or 2 (CARE(O))");
+  if (c->grad_clip != 0 && c->grad_clip != 1) return fail(B200SAC_ERR_INVALID, "grad_clip must be 0 or 1");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -252,7 +254,7 @@ struct Buf {           // [R][n] fp32 (or int32) slab slice
   long long rs = 0;    // replica stride in floats
 };
 
-enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2 };
+enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2, L_GRADNORM };
 
 struct Launch {
   LaunchKind kind;
@@ -283,6 +285,8 @@ struct Launch {
   ChainArgs chain;
   Chain2Args chain2;
   WgradArgs wg;
+  bool store_only = false;   // L_WGRAD: the gradients alone, no optimizer step (grad_clip plans)
+  GradNormArgs gn;
   const char* label = nullptr;
 };
 
@@ -407,6 +411,16 @@ struct b200sac {
   // n-step returns (allocated with the first linked ring): [3][R][B] per-row discount of the step (K.disc), hops folded and
   // ring indices (int32), written by ingest_nstep_kernel
   DevMem<float> ns_buf;
+  // gradient-norm clipping (cfg.grad_clip): [R][3] thresholds (critic, actor, context encoder) and their host mirror, the
+  // step's clip coefficients, the mapped pinned norm ring [kLossSlots][R][3], and the norm launches' partial sums
+  // [3][R][kGradNormMaxBlocks] and tickets [3][R]
+  DevMem<double> clip_thr;
+  std::vector<double> clip_host;
+  DevMem<float> clip_coef;
+  PinnedMem<float> gnorm_h;
+  float* gnorm_h_dev = nullptr;
+  DevMem<double> gn_part;
+  DevMem<unsigned> gn_ticket;
 
   // The members release their resources; the publication stream's last copy lands first.
   ~b200sac() {
@@ -788,7 +802,9 @@ struct PlanBuilder {
   void care_tables(const std::vector<int>& insts);
   void care_encode(const std::vector<EncJob>& jobs);
   void head_bwd(bool policy, bool want_wgrad);
-  void adam(int which, bool tail_only);
+  void opt_slice(int which, int64_t& beg, int64_t& n) const;
+  void adam(int which, bool tail_only, bool with_tail = true);
+  void grad_norm(int which);
   int build_plan_fused();
   void build_plan_layered();
 };
@@ -1052,15 +1068,24 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   h->plan.push_back(l);
 }
 
+// the trainable slice of optimizer `which` (0 critic, 1 actor, 2 CARE(O) context encoder)
+void PlanBuilder::opt_slice(int which, int64_t& beg, int64_t& n) const {
+  beg = which == 0 ? L.critic_begin : (which == 1 ? L.actor_begin : L.cenc_begin);
+  n = which == 0 ? L.critic_n : (which == 1 ? L.actor_n : L.cenc_n);
+}
+
 // parameter update + the tail job (last CTA); tail_only: the tail job alone, on the fork stream, plus the critic-loss
-// reduction (the layer-chained plan, whose parameter updates are fused into the weight-gradient launches)
-void PlanBuilder::adam(int which, bool tail_only) {
+// reduction (the layer-chained plan, whose parameter updates are fused into the weight-gradient launches).
+// grad_clip handles: Adam runs on the clipped gradient and the grad_norm launch in front of it joins the fork stream;
+// with_tail = false drops the tail job (the layer-chained plan's forked tail has it).
+void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
   Launch l;
   l.kind = L_ADAM;
   AdamArgs& P = l.ad;
   memset(&P, 0, sizeof(P));
-  const int64_t beg = which == 0 ? L.critic_begin : (which == 1 ? L.actor_begin : L.cenc_begin);
-  const int64_t n = which == 0 ? L.critic_n : (which == 1 ? L.actor_n : L.cenc_n);
+  int64_t beg, n;
+  opt_slice(which, beg, n);
+  const bool clip = c.grad_clip && !tail_only;
   P.p = h->params + beg; P.m = h->adam_m + beg; P.v = h->adam_v + beg; P.g = h->grads + beg;
   P.rsP = rsP; P.rsM = rsG; P.n = n;
   P.gx = h->grads_x ? h->grads_x + beg : nullptr; P.xs = (long long)R * L.trainable; P.nx = h->gslices - 1;
@@ -1070,23 +1095,50 @@ void PlanBuilder::adam(int which, bool tail_only) {
   P.cnt = h->cnt;
   P.tail = which == 0 ? TAIL_CRITIC_LOSS : (which == 1 ? TAIL_ALPHA_AND_LOSSES : TAIL_NONE);
   if (tail_only) P.tail = TAIL_ALL;
+  if (!with_tail) P.tail = TAIL_NONE;
+  if (clip) {
+    P.coef = h->clip_coef + which;
+    if (h->fused) { P.gx = nullptr; P.nx = 0; }       // the chained weight-gradient launches write slice 0 only
+  }
   P.lq = h->lq.p; P.la = h->la.p; P.rsY = h->y.rs;
   P.logp_cur = h->logp.p + B; P.logstd_sum = h->logstd.p + B; P.rsLogp = h->logp.rs;
   P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
   P.log_alpha = h->params + L.off_alpha;
   P.m_alpha = h->adam_m + L.off_alpha; P.v_alpha = h->adam_v + L.off_alpha; P.g_alpha = h->grads + L.off_alpha;
   P.losses = h->losses; P.losses_host = h->loss_h_dev; P.R = R;
-  int nb = (int)((n + 256 * 4 - 1) / (256 * 4));
-  if (nb < 1) nb = 1;
-  if (nb > 592) nb = 592;
+  const int nb = elementwise_blocks(n);
   l.grid = dim3(nb + (P.tail != TAIL_NONE ? 1 : 0), R);
   l.block = dim3(256);
-  l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
+  l.join = !clip;                // every gradient of the slice must have landed, including the forked weight gradients
   if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
   h->plan.push_back(l);
 }
 
+// grad_clip handles: the gradient norm of optimizer `which` and the clip coefficient its Adam launch (next) applies
+void PlanBuilder::grad_norm(int which) {
+  Launch l;
+  l.kind = L_GRADNORM;
+  GradNormArgs& P = l.gn;
+  memset(&P, 0, sizeof(P));
+  int64_t beg, n;
+  opt_slice(which, beg, n);
+  P.g = h->grads + beg; P.rsM = rsG; P.n = n;
+  if (!h->fused && h->grads_x) { P.gx = h->grads_x + beg; P.xs = (long long)R * L.trainable; P.nx = h->gslices - 1; }
+  P.which = which == 2 ? 4 : which;
+  P.col = which;
+  P.cnt = h->cnt;
+  P.thr = h->clip_thr; P.coef = h->clip_coef; P.norms = h->gnorm_h_dev;
+  P.part = h->gn_part + (size_t)which * R * kGradNormMaxBlocks;
+  P.ticket = h->gn_ticket + (size_t)which * R;
+  P.R = R;
+  l.grid = dim3(elementwise_blocks(n), R);
+  l.block = dim3(256);
+  l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
+  h->plan.push_back(l);
+}
+
 int PlanBuilder::build_plan_fused() {
+  const bool clip = c.grad_clip != 0;
   ChainRows rw;
   memset(&rw, 0, sizeof(rw));
   rw.r = h->r.p; rw.d = h->d.p; rw.tid = (const int*)h->tid.p; rw.rsR = h->r.rs;
@@ -1202,10 +1254,11 @@ int PlanBuilder::build_plan_fused() {
   // weight-gradient launch of a group of networks; the CTA that reduces a gradient tile applies Adam (+ Polyak) to it
   struct WNet { const std::vector<LayerOff>* net; int nh; const std::vector<Buf>* dstore; const std::vector<Buf>* acts; long long act_row_off;
                 const float* X; long long rsX; int ldx; const float* dout; long long rsDout; int lddout; int net_idx; };
-  auto wgrad_launch = [&](const std::vector<WNet>& nets, const char* label, int which) -> int {
+  auto wgrad_launch = [&](const std::vector<WNet>& nets, const char* label, int which, bool store_only) -> int {
     Launch l;
     l.kind = L_WGRAD;
     l.label = label;
+    l.store_only = store_only;
     memset(&l.wg, 0, sizeof(l.wg));
     l.wg.M = B; l.wg.rsG = rsG;
     WgradAdam& O = l.wg.adam;
@@ -1286,7 +1339,11 @@ int PlanBuilder::build_plan_fused() {
     std::vector<WNet> nets;
     for (int net = 0; net < 2; ++net)
       nets.push_back(WNet{&L.q[net], Lc, &h->dhQ, &h->hQ, 0, h->XQ.p, h->XQ.rs, h->K.ldx, h->dq.p + (long long)net * B, h->dq.rs, 1, net});
-    if (int rc = wgrad_launch(nets, "wgrad+adam+polyak{q1,q2}", 0)) return rc;
+    if (int rc = wgrad_launch(nets, clip ? "wgrad{q1,q2}" : "wgrad+adam+polyak{q1,q2}", 0, clip)) return rc;
+  }
+  if (clip) {                    // the whole critic gradient first, then its norm, then Adam + Polyak on the clipped gradient
+    grad_norm(0);
+    adam(0, false, false);
   }
   // ---- D: actor pass through the updated critics ------------------------------------------------------------------------
   // (the launch right before this one is the critic Adam: no weight request before the dependency wait)
@@ -1306,7 +1363,11 @@ int PlanBuilder::build_plan_fused() {
     std::vector<WNet> nets;
     nets.push_back(WNet{&L.actor, La, &h->dhA, &h->hA, (long long)B, h->XA.p + (long long)B * h->K.ldxa, h->XA.rs, h->K.ldxa,
                         h->dout_dbg.p, h->dout_dbg.rs, 2 * A, 0});
-    if (int rc = wgrad_launch(nets, "wgrad+adam{actor}", 1)) return rc;
+    if (int rc = wgrad_launch(nets, clip ? "wgrad{actor}" : "wgrad+adam{actor}", 1, clip)) return rc;
+  }
+  if (clip) {
+    grad_norm(1);
+    adam(1, false, false);
   }
   // ---- tensor maps ---------------------------------------------------------------------------------------------------
   // forward weights [R][nf]: W [N][K] row-major (pitch ld), box {32 k, N rows}, SWIZZLE_128B, OOB k zero-filled;
@@ -1353,7 +1414,8 @@ int PlanBuilder::build_plan_fused() {
           return 0;
         }))
       return rc;
-  CU(cudaFuncSetAttribute(wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
+  CU(cudaFuncSetAttribute(wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
+  CU(cudaFuncSetAttribute(wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
   return 0;
 }
 
@@ -1548,6 +1610,7 @@ void PlanBuilder::build_plan_layered() {
       h->plan.push_back(l2);
     }
   }
+  if (c.grad_clip) grad_norm(0);
   adam(0, false);
   // ---- the actor update (D, E): every launch below returns at entry on a critic-only step; adam(1) skips its own body and
   // its tail writes NaN for the actor-side losses.  adam(2) (CARE(O) context encoder, trained by the critic loss) always runs.
@@ -1615,8 +1678,12 @@ void PlanBuilder::build_plan_layered() {
     }
   }
   actor_side = false;
+  if (c.grad_clip) grad_norm(1);          // (returns at entry on a critic-only step, like the launches of D and E)
   adam(1, false);
-  if (c.care == 2) adam(2, false);        // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
+  if (c.care == 2) {                      // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
+    if (c.grad_clip) grad_norm(2);
+    adam(2, false);
+  }
 }
 
 // Build the launch list of one gradient step (everything after the ingest kernel).
@@ -1774,7 +1841,10 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
         else launch_k(head_bwd_kernel, l.grid, l.block, l.smem, s, K, l.hb);
         break;
       case L_ADAM:
-        launch_k(adam_kernel, l.grid, l.block, 0, s, K, l.ad);
+        launch_k(l.ad.coef ? adam_kernel<true> : adam_kernel<false>, l.grid, l.block, 0, s, K, l.ad);
+        break;
+      case L_GRADNORM:
+        launch_k(grad_sqnorm_kernel, l.grid, l.block, 0, s, K, l.gn);
         break;
       case L_CHAIN: {
         ChainArgs a = l.chain;
@@ -1787,7 +1857,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
         break;
       }
       case L_WGRAD:
-        launch_k(wgrad_kernel, l.grid, l.block, l.smem, s, l.wg, K);
+        launch_k(l.store_only ? wgrad_kernel<true> : wgrad_kernel<false>, l.grid, l.block, l.smem, s, l.wg, K);
         break;
       case L_CHAIN2:
         with_chain_rows(l.bn, [&](auto rows) {
@@ -1915,6 +1985,21 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMalloc(h->ivl.put(), sizeof(int) * 2 * R));
     CU(cudaMemcpy(h->ivl, h->ivl_host.data(), sizeof(int) * 2 * R, cudaMemcpyHostToDevice));
     K.cnt = h->cnt;
+  }
+  if (cfg->grad_clip) {       // thresholds +inf (no clipping), coefficients 1, every norm NaN until a step writes it
+    const size_t n = (size_t)kClipCols * R;
+    h->clip_host.assign(n, INFINITY);
+    CU(cudaMalloc(h->clip_thr.put(), sizeof(double) * n));
+    CU(cudaMemcpy(h->clip_thr, h->clip_host.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
+    const std::vector<float> ones(n, 1.0f);
+    CU(cudaMalloc(h->clip_coef.put(), sizeof(float) * n));
+    CU(cudaMemcpy(h->clip_coef, ones.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
+    CU(cudaHostAlloc(h->gnorm_h.put(), sizeof(float) * kLossSlots * n, cudaHostAllocMapped));
+    std::fill(h->gnorm_h.get(), h->gnorm_h.get() + kLossSlots * n, NAN);
+    CU(cudaHostGetDevicePointer((void**)&h->gnorm_h_dev, h->gnorm_h, 0));
+    CU(cudaMalloc(h->gn_part.put(), sizeof(double) * kGradNormMaxBlocks * n));
+    CU(cudaMalloc(h->gn_ticket.put(), sizeof(unsigned) * n));
+    CU(cudaMemset(h->gn_ticket, 0, sizeof(unsigned) * n));
   }
 
   // work slab
@@ -2253,6 +2338,34 @@ extern "C" int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32
   return 0;
 }
 
+// Gradient-norm clipping thresholds: a device row [R][3] written in stream order like the hyperparameters, read by the
+// grad_norm launches of the step graphs.
+extern "C" int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double* actor, double* ctx) {
+  if (!h || !critic || !actor || !ctx) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  const double* t = h->clip_host.data() + (size_t)replica * kClipCols;
+  *critic = t[0]; *actor = t[1]; *ctx = t[2];
+  return 0;
+}
+
+extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double critic, double actor, double ctx, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (!(critic > 0.0) || !(actor > 0.0) || !(ctx > 0.0))       // (NaN fails every comparison)
+    return fail(B200SAC_ERR_INVALID, "gradient-norm thresholds must be > 0 (+inf: no clipping), got %g, %g, %g", critic, actor, ctx);
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  set_grad_clip_kernel<<<1, 1, 0, sb.run>>>(h->clip_thr, replica, critic, actor, ctx);
+  CU(cudaGetLastError());
+  if (int rc = sb.end()) return rc;
+  double* t = h->clip_host.data() + (size_t)replica * kClipCols;
+  t[0] = critic; t[1] = actor; t[2] = ctx;
+  return 0;
+}
+
 extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   if (src < 0 || src >= h->R || dst < 0 || dst >= h->R)
@@ -2537,18 +2650,20 @@ static int acquire_slot(b200sac* h, int* slot) {
   return 0;
 }
 
-static int fetch_losses(b200sac* h, cudaStream_t st, int n_last, float* out) {
+// the last n_last entries of a mapped pinned per-step ring [kLossSlots][R][width] (losses: width 4, gradient norms: 3)
+static int fetch_ring(b200sac* h, cudaStream_t st, int n_last, const float* ring, int width, float* out) {
   if (n_last < 1 || n_last > kLossSlots || n_last > h->host_steps)
     return fail(B200SAC_ERR_INVALID, "n_last=%d out of range (steps so far %lld, ring %d)", n_last, h->host_steps, kLossSlots);
-  const size_t per = (size_t)h->R * 4;
-  CU(cudaStreamSynchronize(st));       // the tail kernels wrote the mapped host ring directly
+  const size_t per = (size_t)h->R * width;
+  CU(cudaStreamSynchronize(st));       // the kernels wrote the mapped host ring directly
   for (int i = 0; i < n_last; ++i) {
     const long long step = h->host_steps - n_last + i;
     const long long slot = step % kLossSlots;
-    memcpy(out + (size_t)i * per, h->loss_h + (size_t)slot * per, per * sizeof(float));
+    memcpy(out + (size_t)i * per, ring + (size_t)slot * per, per * sizeof(float));
   }
   return 0;
 }
+static int fetch_losses(b200sac* h, cudaStream_t st, int n_last, float* out) { return fetch_ring(h, st, n_last, h->loss_h, 4, out); }
 
 extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, const float* r, const float* s2,
                                  const float* d, const float* eps_next, const float* eps_cur, float* out_losses, void* stream) {
@@ -2613,6 +2728,7 @@ static std::string launch_name(const Launch& l, const std::vector<GemmProb>& hp,
     case L_CHAIN:
     case L_CHAIN2:
     case L_WGRAD: return l.label ? l.label : "chain";
+    case L_GRADNORM: return l.gn.col == 0 ? "grad_norm{critic}" : (l.gn.col == 1 ? "grad_norm{actor}" : "grad_norm{context_encoder}");
     case L_ADAM:
       if (l.ad.which == 1 && l.branch == 1) return "alpha+losses(forked)";
       if (l.ad.which == 1 && l.ad.tail == TAIL_NONE) return "adam_actor";
@@ -2794,6 +2910,13 @@ extern "C" int b200sac_read_losses(b200sac_t* h, int32_t n_last, float* out_host
   return fetch_losses(h, (cudaStream_t)stream, n_last, out_host);
 }
 
+extern "C" int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void* stream) {
+  if (!h || !out_host) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  CU(cudaSetDevice(h->device));
+  return fetch_ring(h, (cudaStream_t)stream, n_last, h->gnorm_h, kClipCols, out_host);
+}
+
 // ------------------------------------------------------------------------------------------
 // Batched policy inference (SURVEY 8(f) rank 4): the actor forward + tanh-Gaussian head the step uses, on n <= 2B
 // caller-provided observation rows -- Actor.get_action (LunarLander_Distributed_SAC/src/model.py:67-82; MT: mtobs rows,
@@ -2965,6 +3088,10 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "disc" || nm == "nstep_m") {               // n-step returns: [B] per-row discount, hops folded (int32 bits)
     if (!h->ns_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a replay ring with trajectory links", name);
     src = h->ns_buf + ((nm == "disc" ? 0 : 1) * (size_t)h->R + replica) * B; n = B;
+  }
+  else if (nm == "clip") {                                  // [3] clip coefficients of the last step
+    if (!h->cfg.grad_clip) return fail(B200SAC_ERR_INVALID, "'clip' needs a handle created with grad_clip");
+    src = h->clip_coef + (size_t)replica * kClipCols; n = kClipCols;
   }
   else if (nm == "chain_dbg") {
     if (!h->chain_dbg) return fail(B200SAC_ERR_INVALID, "chain_dbg needs B200SAC_CHAIN_DBG=1 at create time");

@@ -637,6 +637,9 @@ B200_D void wg_stage(float* __restrict__ dst, const float* __restrict__ src, int
   }
 }
 
+// STORE_ONLY (grad_clip plans): the reduced tiles go to the gradient arena and nothing else; adam_kernel<true> applies the
+// optimizer once the whole gradient, and with it its norm, is known.
+template <bool STORE_ONLY = false>
 __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_constant__ WgradArgs A, StepConst K) {
   DbgStamp stamp(A.dbg);
   stamp();                                 // 0: entry
@@ -674,7 +677,7 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   // the operand tiles are in flight, instead of heading the epilogue
   float step_size = 0.f, bc2_sqrt = 1.f;
   const HParams& H = K.hp[rep];
-  adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
+  if constexpr (!STORE_ONLY) adam_scalars(H.lr[O.which], O.cnt[rep].b1p[O.which], O.cnt[rep].b2p[O.which], step_size, bc2_sqrt);
   // the step's schedule (same cache line as the counters just read); consumed once the first operand tiles have landed, so
   // that a full step never waits for it
   const int sched = sched_of(O.cnt, rep);
@@ -781,6 +784,26 @@ __global__ void __launch_bounds__(WG_THREADS, 2) wgrad_kernel(const __grid_const
   __syncthreads();
   stamp();                                 // partial tiles visible
   float* __restrict__ C = J.C + (long long)rep * A.rsG;
+  if constexpr (STORE_ONLY) {              // the same fixed-order sums as below, stored only
+    const int kk = tid >> 3, nn4 = (tid & 7) << 2;
+    if (k0 + kk < J.Kout && n0 + nn4 < J.Nin) {
+      float4 g4 = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+      for (int ww = 0; ww < 8; ++ww) {
+        const float4 q = *reinterpret_cast<const float4*>(part + ww * (WG_T * WG_T) + kk * WG_T + nn4);
+        g4.x += q.x; g4.y += q.y; g4.z += q.z; g4.w += q.w;
+      }
+      *reinterpret_cast<float4*>(C + (long long)(k0 + kk) * J.ldc + n0 + nn4) = g4;
+    }
+    if (bn == 0 && J.C2 != nullptr && tid < WG_T && k0 + tid < J.Kout) {
+      float v = 0.f;
+#pragma unroll
+      for (int ww = 0; ww < 8; ++ww) v += bpart[ww * WG_T + tid];
+      (J.C2 + (long long)rep * A.rsG)[k0 + tid] = v;
+    }
+    stamp.done();
+    return;
+  }
   // fused optimizer step: adam_one per element like adam_kernel
   const float w1 = (float)(1.0 - K.beta1), b2 = (float)K.beta2, omb2 = (float)(1.0 - K.beta2), eps = (float)K.adam_eps;
   // One thread = four consecutive columns of one row of the tile (128-bit accesses; row pitches, tile origins and tensor

@@ -898,6 +898,8 @@ struct AdamArgs {
   float* losses;                                     // [kLossSlots][R][4] device ring
   float* losses_host;                                // same ring in mapped pinned host memory (zero-copy D2H)
   int R;
+  const float* coef;                                 // adam_kernel<true>: coef[rep * 3] multiplies the gradient (the column of
+                                                     // this optimizer in the [R][3] clip coefficients grad_sqnorm_kernel wrote)
 };
 
 B200_D void adam_scalars(double lr, double b1_pow_t, double b2_pow_t, float& step_size, float& bc2_sqrt) {
@@ -915,12 +917,16 @@ B200_D void adam_one(float& p, float& m, float& v, float g, float w1, float b2, 
   p = p - step_size * (m / denom);            // param.addcdiv_(exp_avg, denom, value=-step_size)
 }
 
+// CLIP (grad_clip plans): Adam runs on g * coef, one fp32 multiply per element, with the replica's clip coefficient of this
+// optimizer (grad_sqnorm_kernel, clip_kernels.cuh); the gradient arena keeps g.
+template <bool CLIP = false>
 __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   KStamp ks_;
   const int rep = blockIdx.y;
   __shared__ float red[256];
   __shared__ float s_ss, s_bc, s_tau[4];
   __shared__ int s_sched;
+  __shared__ float s_coef;
   const bool is_tail = (P.tail != TAIL_NONE) && (blockIdx.x == gridDim.x - 1);
   if (!is_tail) {
     if (threadIdx.x == 0) {
@@ -928,6 +934,7 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       float a, b;
       adam_scalars(H.lr[P.which], P.cnt[rep].b1p[P.which], P.cnt[rep].b2p[P.which], a, b);
       s_ss = a; s_bc = b;
+      if constexpr (CLIP) s_coef = P.coef[rep * 3];
       s_sched = sched_of(P.cnt, rep);        // the step's schedule (same cache line as the counters)
       // Polyak rates: (tau, 1 - tau) of the target critics, then of the CARE state encoder.  Read from shared memory in
       // the loop: four more live registers would cost this kernel a resident CTA per SM.
@@ -970,6 +977,10 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       for (int sx = 3; sx < P.nx; ++sx) {
         const float4 ge = gx4[(long long)sx * xs4 + i];
         gv.x += ge.x; gv.y += ge.y; gv.z += ge.z; gv.w += ge.w;
+      }
+      if constexpr (CLIP) {
+        const float c = s_coef;
+        gv.x = gv.x * c; gv.y = gv.y * c; gv.z = gv.z * c; gv.w = gv.w * c;
       }
       adam_one(pv.x, mv.x, vv.x, gv.x, w1, b2, omb2, step_size, bc2_sqrt, eps);
       adam_one(pv.y, mv.y, vv.y, gv.y, w1, b2, omb2, step_size, bc2_sqrt, eps);

@@ -84,7 +84,7 @@ class _BaseLearner:
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
-                     n_step=1):
+                     n_step=1, max_grad_norm=None):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -93,6 +93,7 @@ class _BaseLearner:
         if int(n_step) > 1 and replay_where != "device":
             raise ValueError("n-step returns need replay_where='device' (the trajectory links live beside the device ring)")
         self.n_step = int(n_step)
+        self.max_grad_norm = max_grad_norm
         self.cfg = cfg_read(cfg_path)
         self.precision = precision
         self.write_mode = write_mode
@@ -113,6 +114,8 @@ class _BaseLearner:
         # only and reports NaN actor loss / entropy; the targets move when the count is a multiple of target_update_interval
         if (actor_update_interval, target_update_interval) != (1, 1):
             self.core.set_update_intervals(actor_update_interval, target_update_interval)
+        if max_grad_norm is not None:
+            self.set_max_grad_norm(max_grad_norm)
         self.memory = self._make_memory(replay_where)
         self.memory.start()
         self.save_model_path = os.path.join("saved_models", self.log_name, self.datetime)
@@ -128,6 +131,15 @@ class _BaseLearner:
             raise ValueError("this learner was built without prioritized=")
         self.memory.ring.set_beta(beta)
 
+    def set_max_grad_norm(self, max_norm: float):
+        """clip_grad_norm_(params, max_norm) before every optimizer step (critic, actor and the CARE(O) context encoder;
+        not the temperature), effective from the next update(); inf turns clipping off.  The learner must have been built
+        with max_grad_norm= (its step plan computes the gradient norms); core.read_grad_norms() returns them."""
+        if self.max_grad_norm is None:
+            raise ValueError("this learner was built without max_grad_norm=")
+        self.max_grad_norm = float(max_norm)
+        self.core.set_grad_clip(critic=max_norm, actor=max_norm, ctx=max_norm)
+
     def set_n_step(self, n: int):
         """Horizon of the n-step return, effective from the next update()."""
         if self.n_step == 1:
@@ -142,7 +154,7 @@ class _BaseLearner:
                           reward_scale=float(self.reward_scale), lr_actor=float(self.lr_actor),
                           lr_critic=float(self.lr_critic),
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
-                          log_alpha_init=float(c["log_alpha"]))
+                          log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None)
 
     # ---- reference method surface -------------------------------------------------------------
     def update(self):
@@ -422,11 +434,11 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
-                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1):
+                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
 
     def _set_dims(self):
         c = self.cfg
@@ -450,9 +462,9 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1, n_step=1):
+                 target_update_interval=1, n_step=1, max_grad_norm=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
 
     def _set_dims(self):
         c = self.cfg
@@ -478,10 +490,10 @@ class MTSACLearner(_BaseLearner):
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
-                 actor_update_interval=1, target_update_interval=1, n_step=1):
+                 actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
 
     def _set_dims(self):
         c = self.cfg

@@ -25,6 +25,9 @@
  *   b200sac_get/set_update_intervals
  *                            actor / target update intervals (TD3 policy_delay, pytorch_sac actor_update_frequency and
  *                            critic_target_update_frequency, SB3 target_update_interval), per replica
+ *   b200sac_set/get_grad_clip, b200sac_read_grad_norms
+ *                            torch.nn.utils.clip_grad_norm_ before each optimizer.step() (Ape-X's max-norm 40, the
+ *                            max_grad_norm of SAC / TD3 code bases) and the norms it returns, per replica and optimizer
  *   b200sac_blob_*           Learner.get_parameters() and server.set('parameters', _pickle.dumps(get_parameters())) in
  *                            Learner.run(), learner.py:272-276,298-299 (MT10_Distributed_CARE/src/learner.py:412-417,442-443):
  *                            the byte string, device-assembled
@@ -95,6 +98,8 @@ typedef struct b200sac_cfg {
   int32_t emb_dim;                   /* embedding_dim_contextEnc: CARE(O) header = Linear(ctx_in, 2e), Linear(2e, e) */
   double tau_se;                     /* state_encoder_tau */
   double lr_ctx;                     /* lr_contextEnc (CARE(O) context-encoder Adam) */
+  int32_t grad_clip;                 /* 0 = the default plan; 1 = the plan with gradient-norm clipping and gradient norms
+                                        (b200sac_set_grad_clip), every threshold +inf at create.  Fixed at create. */
 } b200sac_cfg;
 
 typedef struct b200sac_tensor_desc {
@@ -163,8 +168,8 @@ int b200sac_get_hparams(b200sac_t* h, int32_t replica, b200sac_hparams* out);
 int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp, void* stream);
 /* Enqueued on `stream`: replica `dst`'s learner state becomes a copy of `src`'s -- the whole parameter arena (targets,
  * log_alpha and the CARE embedding included), Adam m and v and the step counters -- device to device, without a host
- * round trip (the exploit step of population-based training).  Hyperparameters, gradients and replay rings are not
- * copied. */
+ * round trip (the exploit step of population-based training).  Hyperparameters, update intervals, gradient-clipping
+ * thresholds, gradients and replay rings are not copied. */
 int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream);
 
 /* Per-replica update intervals, both 1 (every step is a full step) after b200sac_create.  Let n be the replica's critic
@@ -184,6 +189,27 @@ int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream);
  * B200SAC_ERR_INVALID and nothing changes.  Get: the values last set (host mirror: does not synchronise). */
 int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32_t actor_every, int32_t target_every, void* stream);
 int b200sac_get_update_intervals(b200sac_t* h, int32_t replica, int32_t* actor_every, int32_t* target_every);
+
+/* Gradient-norm clipping, per replica and optimizer (handles created with cfg.grad_clip = 1; others: B200SAC_ERR_STATE).
+ * torch.nn.utils.clip_grad_norm_(params, max_norm) right before each optimizer's step(), for the critic (counter slot 0: q1,
+ * q2 and, with CARE, the critic state encoder), the actor (slot 1) and the CARE(O) context encoder (slot 4); the temperature
+ * log_alpha is not clipped.  Per step and optimizer, with g = the gradient Adam reads (what b200sac_export(GRADS) returns;
+ * pad columns and gaps are zero):
+ *   norm = sqrt(sum g_i^2), accumulated in fp64 over the whole slice in a fixed order (bit-reproducible, independent of the
+ *          replica count, no floating-point atomics);
+ *   coef = (float) min(1, max_norm / (norm + 1e-6)), in fp64 and rounded once (a NaN quotient gives 1);
+ *   Adam runs on g * coef (one fp32 multiply: m and v see the clipped gradient, as with torch); GRADS keeps g.
+ * A critic-only step (b200sac_set_update_intervals) leaves the actor untouched and reports its norm as NaN.
+ * Set: enqueued on `stream` like b200sac_set_hparams (applies to the steps enqueued after it, including launches of graphs
+ * already instantiated).  Every value must be > 0; +inf = no clipping (the norms are still reported); NaN, a value <= 0 or
+ * a bad replica give B200SAC_ERR_INVALID and nothing changes.  The thresholds are not copied by b200sac_copy_replica and not
+ * part of a checkpoint.  Get: the values last set (host mirror: does not synchronise). */
+int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double critic, double actor, double ctx, void* stream);
+int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double* actor, double* ctx);
+/* Pre-clip gradient norms of the most recent `n_last` steps (<= 1024 kept, slots aligned with b200sac_read_losses):
+ * out[n_last][replicas][3] = {critic, actor, context encoder}; NaN where that optimizer did not step (the actor on a
+ * critic-only step, the context encoder outside CARE(O)).  Synchronises the stream. */
+int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void* stream);
 
 /* One gradient step from caller-provided DEVICE minibatches, each
  * [replicas][batch][width] fp32: s,s2 width obs(=state_dim+num_tasks), a width act, r,d width 1.
@@ -269,7 +295,9 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
  * importance weights of its critic loss), "prio" [B] (the leaf values p it wrote) and "idx" [B] (its ring indices, int32
  * bit patterns).  After a step from a linked ring (n-step returns): "disc" [B] (the per-row discount of its TD target),
- * "nstep_m" [B] (hops folded, int32 bit patterns), "idx" as above, and "r" / "d" hold the folded values. */
+ * "nstep_m" [B] (hops folded, int32 bit patterns), "idx" as above, and "r" / "d" hold the folded values.  With
+ * cfg.grad_clip: "clip" [3] (the clip coefficients of the last step: critic, actor, context encoder; NaN for an actor that
+ * did not step; the context encoder's entry is meaningful for CARE(O) only). */
 int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replica, float* out_host, int64_t cap_floats,
                        int64_t* n_floats, void* stream);
 
