@@ -263,12 +263,11 @@ struct Launch {
   int branch = 0;        // 1: may run on the fork stream, concurrently with the launches that follow it on the main stream
   bool join = false;     // the main stream waits for the fork stream before this launch
   // payloads (only the one matching `kind` is used)
-  const GemmProb* probs = nullptr; int G = 0;
+  int G = 0;
   GemmGroup grp;
-  const TcProb* tprobs = nullptr;
+  int tprob0 = 0;        // L_GEMM_TC: index of the launch's first problem in the handle's d_tprobs
   int bn = 64;
   bool pair128 = false;  // L_GEMM_TC with bn = 128: the paired tile flavour (fixed when the plan is built)
-  int split = 1;         // GEMM launches: K slices of the group's weight gradients
   const int* sched = nullptr;   // L_GEMM_TC: actor-side launch, replica 0's schedule word (gemm_tc_kernel)
   PolicyDoutArgs pdo;
   CareTabArgs ctab;
@@ -287,7 +286,9 @@ struct Launch {
   WgradArgs wg;
   bool store_only = false;   // L_WGRAD: the gradients alone, no optimizer step (grad_clip plans)
   GradNormArgs gn;
-  const char* label = nullptr;
+  // What b200sac_profile_step calls the launch, set by the builder that makes it.  The part before '(' and the "wgmma"
+  // substring are what bench.py groups kernels by.
+  std::string label;
 };
 
 struct b200sac_replay;
@@ -344,7 +345,6 @@ struct b200sac {
   long long host_steps = 0;       // steps enqueued so far
   // work slab
   DevMem<float> slab;
-  size_t slab_floats = 0;
   Buf XA, XQ, XT, XP, r, d, tid, eps, pout, psave, act_out, logp, logstd, y, q, dq, lq, dqa, la, qmin, dxP,
       dout_dbg, dact_dbg, qt, qp, alpha;
   bool stamping = false;          // true while b200sac_graph_timeline runs on this handle (one unforked step per graph)
@@ -357,13 +357,10 @@ struct b200sac {
   int care_row_w = 0, care_off_att = 0, care_off_ctx = 0;
   std::vector<Buf> hA, dhA;       // per actor hidden layer
   std::vector<Buf> hQ, hT, hP, dhQ;   // per critic hidden layer, [2][B][H]
-  DevMem<GemmProb> d_probs;
-  std::vector<GemmProb> h_probs;
   DevMem<TcProb> d_tprobs;
   std::vector<TcProb> h_tprobs;
   std::vector<Launch> plan;
   IngestOut ing;
-  int use_eps_buf_idx = -1;       // index of the policy launch in plan (its use_eps_buf flag varies)
   // split-K weight gradients: slices 1..gslices-1 of the gradient arena, [slice-1][R][trainable] (slice 0 = grads)
   DevMem<float> grads_x;
   int gslices = 1;
@@ -499,16 +496,26 @@ static void unpack_rows(const b200sac* h, const float* rows, long long n, float*
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
-static Buf carve(size_t& cursor, size_t n_per_rep, int R) {
-  Buf b;
-  size_t n = align_up(n_per_rep, 64);
-  b.rs = (long long)n;
-  b.p = (float*)(uintptr_t)(cursor * sizeof(float));   // offset for now; rebased after allocation
-  cursor += n * (size_t)R;
-  return b;
-}
-
-static void rebase(Buf& b, float* base) { b.p = base + (size_t)(uintptr_t)b.p / sizeof(float); }
+// The work slab: every [R][n] buffer of a step in one allocation.  request() gives a buffer its replica stride (n rounded up
+// to 64 floats) and the next place in the slab; allocate() makes the slab, zeroed, and points every requested buffer into
+// it.  The order of the requests fixes every buffer's offset, and with it the 16-byte alignment that the plan builder tests
+// when it picks a GEMM engine or a tensor-mapped operand.
+struct SlabCarver {
+  int R;
+  size_t floats = 0;
+  std::vector<std::pair<Buf*, size_t>> at;     // requested buffer, its offset in floats
+  void request(Buf& b, size_t n_per_rep) {
+    b.rs = (long long)align_up(n_per_rep, 64);
+    at.emplace_back(&b, floats);
+    floats += (size_t)b.rs * R;
+  }
+  int allocate(DevMem<float>& slab) {
+    CU(cudaMalloc(slab.put(), floats * sizeof(float)));
+    CU(cudaMemset(slab, 0, floats * sizeof(float)));
+    for (auto& [b, off] : at) b->p = slab + off;
+    return 0;
+  }
+};
 
 // ---- TMA tensor maps (driver entry point resolved at run time: no link-time libcuda dependency) ----
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -809,6 +816,21 @@ struct PlanBuilder {
   void build_plan_layered();
 };
 
+// Label of a grouped GEMM launch of the problems g: their kind (a thin launch is named after its first problem alone), the
+// engine and wgmma tile (128x64 | 128x128 | 128x128 paired | 128x160) and, when the group holds weight gradients, their K
+// slices ("split S")
+static std::string gemm_label(const std::vector<GemmProb>& g, LaunchKind kind, int bn, bool pair128, int split) {
+  const GemmProb &p0 = g.front(), &pl = g.back();
+  bool wg = false;
+  for (auto& p : g) wg = wg || p.mode == GEMM_WGRAD;
+  std::string s = p0.mode == GEMM_FWD ? "gemm_fwd(" : p0.mode == GEMM_DGRAD ? "gemm_dgrad(" :
+                  (pl.mode == GEMM_DGRAD && kind != L_GEMM_THIN) ? "gemm_wgrad+dgrad(" : "gemm_wgrad(";
+  if (kind == L_GEMM_TC) s += "wgmma 128x" + std::to_string(bn) + (pair128 ? " paired" : "");
+  else s += kind == L_GEMM_THIN ? "thin" : "ffma";
+  if (wg) s += ", split " + std::to_string(split);
+  return s + ")";
+}
+
 void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
   // Split-K for the weight gradients: K = batch (1024 / 1280) is the long dimension and M x N = out x in gives only a
   // handful of tiles, so one CTA would walk 32-40 k chunks alone.
@@ -876,20 +898,18 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
       l.bn = bn;
       l.pair128 = bn == 128 && h->env.pair128;
       l.sched = actor_side ? &h->cnt[0].sched : nullptr;
-      l.split = split;
+      l.label = gemm_label(tc, L_GEMM_TC, bn, l.pair128, split);
       l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
       l.block = dim3(TC_THREADS);
       l.smem = tc_smem(bn);
       l.G = (int)tc.size();
-      l.tprobs = (const TcProb*)(uintptr_t)h->h_tprobs.size();
-      l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // keep the SIMT descriptors too (labels)
+      l.tprob0 = (int)h->h_tprobs.size();
       for (int rep = 0; rep < R; ++rep)
         for (auto& p : tc) {
           TcProb t;
           if (int e = make_tc_prob(p, rep, t, bn)) rc = e;
           h->h_tprobs.push_back(t);
         }
-      for (auto& p : tc) h->h_probs.push_back(p);
       h->plan.push_back(l);
     }
     ps = rest;
@@ -905,7 +925,6 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
     for (auto& p : g) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
     l.kind = L_GEMM_SMALL;
     l.branch = branch;
-    l.split = split;
     l.grid = dim3((maxN + GS_T - 1) / GS_T, (maxM + GS_T - 1) / GS_T, (unsigned)(g.size() * R));
     l.block = dim3(GS_THREADS);
     if (thin) {        // input-layer weight / input gradients (N = obs+act <= 16): gemm_thin.cuh
@@ -918,13 +937,11 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
       l.grid = dim3(1, rows, (unsigned)(g.size() * R));
       l.block = dim3(GT_THREADS);
     }
-    l.G = (int)g.size();
+    l.label = gemm_label(g, l.kind, 0, false, split);
     memset(&l.grp, 0, sizeof(l.grp));
-    l.grp.G = l.G;
+    l.grp.G = (int)g.size();
     l.grp.sched = actor_side ? &h->cnt[0].sched : nullptr; l.grp.sched_stride = kSchedStride;
     for (size_t i = 0; i < g.size(); ++i) l.grp.p[i] = g[i];
-    l.probs = (const GemmProb*)(uintptr_t)h->h_probs.size();   // index for now; rebased later
-    for (auto& p : g) h->h_probs.push_back(p);
     h->plan.push_back(l);
   }
 }
@@ -932,6 +949,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
 void PlanBuilder::care_tables(const std::vector<int>& insts) {
   Launch l;
   l.kind = L_CARE_TAB;
+  l.label = "care_tables";
   l.ctab = care_tab_args(h, -1, insts);
   l.ctab.sched = actor_side ? &h->cnt[0].sched : nullptr; l.ctab.sched_stride = kSchedStride;
   l.grid = dim3(c.num_tasks, (unsigned)insts.size(), R);
@@ -976,6 +994,7 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
       cudaFuncSetAttribute(care_mixfwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) == cudaSuccess) {
     Launch l;
     l.kind = L_CARE_MIXFWD;
+    l.label = "care_mixture_fwd+mix";
     l.cmf = A;
     l.grid = dim3(cta, R);
     l.block = dim3(CMF_THREADS);
@@ -991,6 +1010,7 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
   for (const EncJob& e : jobs) {
     Launch l;
     l.kind = L_CARE_MIX;
+    l.label = "care_mix";
     l.cmix = care_mix_args(h, -1, e);
     l.cmix.sched = actor_side ? &h->cnt[0].sched : nullptr; l.cmix.sched_stride = kSchedStride;
     l.grid = dim3((e.rows + 7) / 8, R);
@@ -1025,6 +1045,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
     if (split) {
       Launch pl;
       pl.kind = L_POLICY_DOUT;
+      pl.label = "policy_dout";
       PolicyDoutArgs& Q = pl.pdo;
       memset(&Q, 0, sizeof(Q));
       Q.dx = h->dxP.p; Q.rsDxNet = (long long)B * h->K.ldx; Q.rsDxRep = h->dxP.rs; Q.lddx = h->K.ldx;
@@ -1061,6 +1082,8 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   // few to fill the GPU
   const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0;
   l.bn = wide ? 4 : 1;
+  l.label = std::string(policy ? "head_bwd(policy, " : "head_bwd(q, ") + (wide ? "128-bit, " : "") + "row slices " +
+            std::to_string(P.row_slices) + ")";
   const int cols = wide ? kHb4Cols : kHbCols;
   l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
   l.block = dim3(256);
@@ -1081,6 +1104,8 @@ void PlanBuilder::opt_slice(int which, int64_t& beg, int64_t& n) const {
 void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
   Launch l;
   l.kind = L_ADAM;
+  l.label = which == 0 ? "adam_critic+polyak" : which == 2 ? "adam_context_encoder" :
+            tail_only ? "alpha+losses(forked)" : with_tail ? "adam_actor+alpha" : "adam_actor";
   AdamArgs& P = l.ad;
   memset(&P, 0, sizeof(P));
   int64_t beg, n;
@@ -1118,6 +1143,7 @@ void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
 void PlanBuilder::grad_norm(int which) {
   Launch l;
   l.kind = L_GRADNORM;
+  l.label = which == 0 ? "grad_norm{critic}" : which == 1 ? "grad_norm{actor}" : "grad_norm{context_encoder}";
   GradNormArgs& P = l.gn;
   memset(&P, 0, sizeof(P));
   int64_t beg, n;
@@ -1330,7 +1356,6 @@ int PlanBuilder::build_plan_fused() {
       const LayerOff& hd = mlp[nh];
       J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
     }
-    h->use_eps_buf_idx = (int)h->plan.size();
     finish_chain(l);
   }
   // ---- B + C: target critics over (s', a'), TD target, critic backward (one clustered launch), weight gradients, Adam ----
@@ -1458,10 +1483,10 @@ void PlanBuilder::build_plan_layered() {
   {  // policy head
     Launch l;
     l.kind = L_POLICY;
+    l.label = "policy_head";
     l.grid = dim3((2 * B + 7) / 8, R);
     l.block = dim3(256);
     l.pol = h->pol;
-    h->use_eps_buf_idx = (int)h->plan.size();
     h->plan.push_back(l);
   }
   // ---- Phase B: target critics over (s2, a') ---------------------------------------------
@@ -1478,6 +1503,7 @@ void PlanBuilder::build_plan_layered() {
   {  // critic heads: y, Q1, Q2, dQ
     Launch l;
     l.kind = L_CHEADS;
+    l.label = "critic_heads";
     l.join = true;                 // needs Q1,Q2 on (s,a), which may have run on the fork stream
     l.grid = dim3((B + 7) / 8, R);
     l.block = dim3(256);
@@ -1528,6 +1554,7 @@ void PlanBuilder::build_plan_layered() {
     {  // backward of the attention mix: dZk, d(att)
       Launch l;
       l.kind = L_CARE_MIXBWD;
+      l.label = "care_mix_bwd";
       CareMixBwdArgs& P = l.cmixb;
       memset(&P, 0, sizeof(P));
       P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
@@ -1577,6 +1604,7 @@ void PlanBuilder::build_plan_layered() {
     {  // per-task reduction + softmax backward, then the trunk / context-MLP weight gradients
       Launch l;
       l.kind = L_CARE_TABRED;
+      l.label = "care_tab_reduce";
       CareTabReduceArgs& P = l.ctred;
       memset(&P, 0, sizeof(P));
       P.datt = h->careDatt.p; P.rsDatt = h->careDatt.rs;
@@ -1590,6 +1618,7 @@ void PlanBuilder::build_plan_layered() {
       h->plan.push_back(l);
       Launch l2;
       l2.kind = L_CARE_TABWG;
+      l2.label = "care_tab_wgrad";
       CareTabWgradArgs& Q = l2.ctwg;
       memset(&Q, 0, sizeof(Q));
       Q.params = h->params; Q.rsP = rsP; Q.emb_off = L.off_emb;
@@ -1632,6 +1661,7 @@ void PlanBuilder::build_plan_layered() {
   {
     Launch l;
     l.kind = L_AQHEADS;
+    l.label = "actor_q_heads";
     l.grid = dim3((B + 7) / 8, R);
     l.block = dim3(256);
     ActorQHeadArgs& P = l.aq;
@@ -1711,19 +1741,11 @@ static int build_plan(b200sac* h) {
     pb.build_plan_layered();
   }
   if (pb.rc) return pb.rc;
-  // upload problem tables and rebase
+  // the wgmma launches' problem table (run_plan hands each launch its slice)
   if (!h->h_tprobs.empty()) {
     CU(cudaMalloc(h->d_tprobs.put(), h->h_tprobs.size() * sizeof(TcProb)));
     CU(cudaMemcpy(h->d_tprobs, h->h_tprobs.data(), h->h_tprobs.size() * sizeof(TcProb), cudaMemcpyHostToDevice));
     CU(tc_set_attrs());
-  }
-  if (!h->h_probs.empty()) {
-    CU(cudaMalloc(h->d_probs.put(), h->h_probs.size() * sizeof(GemmProb)));
-    CU(cudaMemcpy(h->d_probs, h->h_probs.data(), h->h_probs.size() * sizeof(GemmProb), cudaMemcpyHostToDevice));
-  }
-  for (auto& l : h->plan) {
-    if (l.kind == L_GEMM_SMALL || l.kind == L_GEMM_THIN || l.kind == L_GEMM_TC) l.probs = h->d_probs + (size_t)(uintptr_t)l.probs;
-    if (l.kind == L_GEMM_TC) l.tprobs = h->d_tprobs + (size_t)(uintptr_t)l.tprobs;
   }
   size_t max_smem = 0;
   for (auto& l : h->plan)
@@ -1822,7 +1844,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
         launch_k(gemm_thin_kernel, l.grid, l.block, 0, s, l.grp);
         break;
       case L_GEMM_TC:
-        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, l.tprobs, l.sched, l.G, kSchedStride);
+        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, h->d_tprobs + l.tprob0, l.sched, l.G, kSchedStride);
         break;
       case L_POLICY: {
         PolicyHeadArgs P = l.pol;
@@ -2002,52 +2024,36 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMemset(h->gn_ticket, 0, sizeof(unsigned) * n));
   }
 
-  // work slab
-  size_t cur = 0;
+  // work slab.  Buffers that a kernel addresses with one replica stride get one length: rsX (XQ, XT, XP), rsR (r, d, tid),
+  // rsY (y, lq, la, qmin; the [2][B] q, dq, dqa, qt, qp take 2 * rsY), rsLogp (logp, logstd), rsDbg (dout_dbg, dact_dbg).
+  SlabCarver slab{R};
   const int La = cfg->n_actor_hidden, Lc = cfg->n_critic_hidden;
-  h->XA = carve(cur, (size_t)2 * B * ldxa, R);
-  h->XQ = carve(cur, (size_t)B * ldx, R);
-  h->XT = carve(cur, (size_t)B * ldx, R);
-  h->XP = carve(cur, (size_t)B * ldx, R);
-  h->XT.rs = h->XP.rs = h->XQ.rs;
-  h->r = carve(cur, B, R);
-  h->d = carve(cur, B, R);
-  h->tid = carve(cur, B, R);
-  h->eps = carve(cur, (size_t)2 * B * A, R);
-  h->pout = carve(cur, (size_t)2 * B * 2 * A, R);
-  h->psave = carve(cur, (size_t)2 * B * A * kSaveW, R);
-  h->act_out = carve(cur, (size_t)2 * B * A, R);
-  h->logp = carve(cur, (size_t)2 * B, R);
-  h->logstd = carve(cur, (size_t)2 * B, R);
-  h->y = carve(cur, B, R);
-  h->lq = carve(cur, B, R);
-  h->la = carve(cur, B, R);
-  h->qmin = carve(cur, B, R);
-  // q, dq, dqa are [2][B] with replica stride 2 * y.rs
-  h->q = carve(cur, (size_t)2 * h->y.rs, R);
-  h->dq = carve(cur, (size_t)2 * h->y.rs, R);
-  h->dqa = carve(cur, (size_t)2 * h->y.rs, R);
-  h->qt = carve(cur, (size_t)2 * h->y.rs, R);
-  h->qp = carve(cur, (size_t)2 * h->y.rs, R);
-  h->alpha = carve(cur, 64, R);
-  h->dxP = carve(cur, (size_t)2 * B * ldx, R);
-  h->dout_dbg = carve(cur, (size_t)B * 2 * A, R);
-  h->dact_dbg = carve(cur, (size_t)B * 2 * A, R);
-  h->dact_dbg.rs = h->dout_dbg.rs;
+  const size_t nX = (size_t)B * ldx, rsB = align_up(B, 64), nLogp = (size_t)2 * B, nDbg = (size_t)B * 2 * A;
+  slab.request(h->XA, (size_t)2 * B * ldxa);
+  for (Buf* b : {&h->XQ, &h->XT, &h->XP}) slab.request(*b, nX);
+  for (Buf* b : {&h->r, &h->d, &h->tid}) slab.request(*b, rsB);
+  slab.request(h->eps, (size_t)2 * B * A);
+  slab.request(h->pout, (size_t)2 * B * 2 * A);
+  slab.request(h->psave, (size_t)2 * B * A * kSaveW);
+  slab.request(h->act_out, (size_t)2 * B * A);
+  for (Buf* b : {&h->logp, &h->logstd}) slab.request(*b, nLogp);
+  for (Buf* b : {&h->y, &h->lq, &h->la, &h->qmin}) slab.request(*b, rsB);
+  for (Buf* b : {&h->q, &h->dq, &h->dqa, &h->qt, &h->qp}) slab.request(*b, 2 * rsB);
+  slab.request(h->alpha, 64);
+  slab.request(h->dxP, (size_t)2 * B * ldx);
+  for (Buf* b : {&h->dout_dbg, &h->dact_dbg}) slab.request(*b, nDbg);
+  h->hA.resize(La); h->dhA.resize(La);
   for (int l = 0; l < La; ++l) {
-    h->hA.push_back(carve(cur, (size_t)2 * B * cfg->actor_hidden[l], R));
-    h->dhA.push_back(carve(cur, (size_t)B * cfg->actor_hidden[l], R));
+    slab.request(h->hA[l], (size_t)2 * B * cfg->actor_hidden[l]);
+    slab.request(h->dhA[l], (size_t)B * cfg->actor_hidden[l]);
   }
-  for (int l = 0; l < Lc; ++l) {
-    h->hQ.push_back(carve(cur, (size_t)2 * B * cfg->critic_hidden[l], R));
-    h->hT.push_back(carve(cur, (size_t)2 * B * cfg->critic_hidden[l], R));
-    h->hP.push_back(carve(cur, (size_t)2 * B * cfg->critic_hidden[l], R));
-    h->dhQ.push_back(carve(cur, (size_t)2 * B * cfg->critic_hidden[l], R));
-  }
+  h->hQ.resize(Lc); h->hT.resize(Lc); h->hP.resize(Lc); h->dhQ.resize(Lc);
+  for (int l = 0; l < Lc; ++l)
+    for (Buf* b : {&h->hQ[l], &h->hT[l], &h->hP[l], &h->dhQ[l]}) slab.request(*b, (size_t)2 * B * cfg->critic_hidden[l]);
   if (cfg->care) {
     const int Kenc = cfg->num_encoders, T = cfg->num_tasks;
     auto pitch = [](int w) { return (w + 3) & ~3; };
-    h->XS = carve(cur, (size_t)2 * B * obs, R);
+    slab.request(h->XS, (size_t)2 * B * obs);
     // per-task table row: trunk activations per layer, attention, context-MLP activations per layer
     int off = 0;
     CareNet& tr = h->care_trunk;
@@ -2062,34 +2068,20 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     for (int j = 0; j < cx.n; ++j) { cx.dims[j + 1] = cxl[j].out; cx.w[j] = cxl[j].w; cx.b[j] = cxl[j].b; cx.act_off[j] = off; off += cxl[j].out; }
     h->care_off_ctx = cx.act_off[cx.n - 1];
     h->care_row_w = off;
-    for (int i = 0; i < 3; ++i) h->careTab[i] = carve(cur, (size_t)T * off, R);
-    h->careDtab = carve(cur, (size_t)T * (Kenc + cfg->ctx_out), R);
-    h->careDatt = carve(cur, (size_t)B * Kenc, R);
+    for (int i = 0; i < 3; ++i) slab.request(h->careTab[i], (size_t)T * off);
+    slab.request(h->careDtab, (size_t)T * (Kenc + cfg->ctx_out));
+    slab.request(h->careDatt, (size_t)B * Kenc);
     const int rows_of[3] = {2 * B, B, B};
     for (int i = 0; i < 3; ++i) {
-      for (int l = 0; l < cfg->n_mix_hidden; ++l) h->mixH[i].push_back(carve(cur, (size_t)Kenc * rows_of[i] * pitch(cfg->mix_hidden[l]), R));
-      h->mixZ[i] = carve(cur, (size_t)Kenc * rows_of[i] * pitch(cfg->mix_out), R);
+      h->mixH[i].resize(cfg->n_mix_hidden);
+      for (int l = 0; l < cfg->n_mix_hidden; ++l) slab.request(h->mixH[i][l], (size_t)Kenc * rows_of[i] * pitch(cfg->mix_hidden[l]));
+      slab.request(h->mixZ[i], (size_t)Kenc * rows_of[i] * pitch(cfg->mix_out));
     }
-    for (int l = 0; l < cfg->n_mix_hidden; ++l) h->mixDH.push_back(carve(cur, (size_t)Kenc * B * pitch(cfg->mix_hidden[l]), R));
-    h->mixDZ = carve(cur, (size_t)Kenc * B * pitch(cfg->mix_out), R);
+    h->mixDH.resize(cfg->n_mix_hidden);
+    for (int l = 0; l < cfg->n_mix_hidden; ++l) slab.request(h->mixDH[l], (size_t)Kenc * B * pitch(cfg->mix_hidden[l]));
+    slab.request(h->mixDZ, (size_t)Kenc * B * pitch(cfg->mix_out));
   }
-  h->slab_floats = cur;
-  CU(cudaMalloc(h->slab.put(), cur * sizeof(float)));
-  CU(cudaMemset(h->slab, 0, cur * sizeof(float)));
-  for (Buf* b : {&h->XA, &h->XQ, &h->XT, &h->XP, &h->r, &h->d, &h->tid, &h->eps, &h->pout, &h->psave, &h->act_out, &h->logp,
-                 &h->logstd, &h->y, &h->lq, &h->la, &h->qmin, &h->q, &h->dq, &h->dqa, &h->dxP, &h->dout_dbg, &h->dact_dbg, &h->qt, &h->qp, &h->alpha})
-    rebase(*b, h->slab);
-  for (auto* v : {&h->hA, &h->dhA, &h->hQ, &h->hT, &h->hP, &h->dhQ})
-    for (auto& b : *v) rebase(b, h->slab);
-  if (cfg->care) {
-    for (Buf* b : {&h->XS, &h->careTab[0], &h->careTab[1], &h->careTab[2], &h->careDtab, &h->careDatt, &h->mixZ[0], &h->mixZ[1],
-                   &h->mixZ[2], &h->mixDZ})
-      rebase(*b, h->slab);
-    for (auto* v : {&h->mixH[0], &h->mixH[1], &h->mixH[2], &h->mixDH})
-      for (auto& b : *v) rebase(b, h->slab);
-  }
-  if (h->q.rs != 2 * h->y.rs || h->dq.rs != 2 * h->y.rs || h->dqa.rs != 2 * h->y.rs || h->qt.rs != 2 * h->y.rs || h->qp.rs != 2 * h->y.rs)
-    return fail(B200SAC_ERR_INVALID, "internal: q stride");
+  if (int rc = slab.allocate(h->slab)) return rc;
 
   IngestOut& O = h->ing;
   O.XA = h->XA.p; O.XQ = h->XQ.p; O.XT = h->XT.p; O.XP = h->XP.p; O.r = h->r.p; O.d = h->d.p; O.eps = h->eps.p;
@@ -2097,9 +2089,6 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   O.rsXA = h->XA.rs; O.rsXQ = h->XQ.rs; O.rsR = h->r.rs; O.rsEps = h->eps.rs;
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
-  if (h->d.rs != h->r.rs || h->tid.rs != h->r.rs || h->lq.rs != h->y.rs || h->la.rs != h->y.rs || h->qmin.rs != h->y.rs ||
-      h->logstd.rs != h->logp.rs)
-    return fail(B200SAC_ERR_INVALID, "internal: stride mismatch");
 
   // parameter init: Xavier-uniform weights, zero biases, log_alpha = cfg; targets = locals
   {
@@ -2689,54 +2678,6 @@ extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, c
   return sb.end();
 }
 
-// Label of a plan launch.  GEMM launches name the engine, the wgmma tile (128x64 | 128x128 | 128x128 paired | 128x160) and,
-// when the group holds weight gradients, their K slices ("split S"); head_bwd names the 128-bit column mapping and its row
-// slices.  The part before '(' and the "wgmma" substring are what bench.py groups kernels by.
-static std::string launch_name(const Launch& l, const std::vector<GemmProb>& hp, const GemmProb* dbase) {
-  switch (l.kind) {
-    case L_GEMM_TC:
-    case L_GEMM_SMALL:
-    case L_GEMM_THIN: {
-      const size_t i0 = (size_t)(l.probs - dbase);
-      const GemmProb& p0 = hp[i0];
-      const GemmProb& pl = hp[i0 + l.G - 1];
-      bool wg = false;
-      for (int i = 0; i < l.G; ++i) wg = wg || hp[i0 + i].mode == GEMM_WGRAD;
-      // (thin launches are named after their first problem alone, as they always have been)
-      std::string s = p0.mode == GEMM_FWD ? "gemm_fwd(" : p0.mode == GEMM_DGRAD ? "gemm_dgrad(" :
-                      (pl.mode == GEMM_DGRAD && l.kind != L_GEMM_THIN) ? "gemm_wgrad+dgrad(" : "gemm_wgrad(";
-      if (l.kind == L_GEMM_TC) s += "wgmma 128x" + std::to_string(l.bn) + (l.pair128 ? " paired" : "");
-      else s += l.kind == L_GEMM_THIN ? "thin" : "ffma";
-      if (wg) s += ", split " + std::to_string(l.split);
-      return s + ")";
-    }
-    case L_HEADBWD: {
-      std::string s = (l.hb.policy_mode || l.hb.NO > 1) ? "head_bwd(policy, " : "head_bwd(q, ";
-      if (l.bn == 4) s += "128-bit, ";
-      return s + "row slices " + std::to_string(l.hb.row_slices) + ")";
-    }
-    case L_POLICY_DOUT: return "policy_dout";
-    case L_CARE_TAB: return "care_tables";
-    case L_CARE_MIX: return "care_mix";
-    case L_CARE_MIXFWD: return "care_mixture_fwd+mix";
-    case L_CARE_MIXBWD: return "care_mix_bwd";
-    case L_CARE_TABRED: return "care_tab_reduce";
-    case L_CARE_TABWG: return "care_tab_wgrad";
-    case L_POLICY: return "policy_head";
-    case L_CHEADS: return "critic_heads";
-    case L_AQHEADS: return "actor_q_heads";
-    case L_CHAIN:
-    case L_CHAIN2:
-    case L_WGRAD: return l.label ? l.label : "chain";
-    case L_GRADNORM: return l.gn.col == 0 ? "grad_norm{critic}" : (l.gn.col == 1 ? "grad_norm{actor}" : "grad_norm{context_encoder}");
-    case L_ADAM:
-      if (l.ad.which == 1 && l.branch == 1) return "alpha+losses(forked)";
-      if (l.ad.which == 1 && l.ad.tail == TAIL_NONE) return "adam_actor";
-      return l.ad.which == 0 ? "adam_critic+polyak" : (l.ad.which == 1 ? "adam_actor+alpha" : "adam_context_encoder");
-  }
-  return "?";
-}
-
 // Eager (non-graph) run of `iters` sampled steps with a CUDA event between every launch.
 // out_ms[i] = mean device time of launch i (i = 0 is sampling + ingest); names are returned as a
 // ';'-separated list.  This is what bench.py uses for the per-kernel roofline numbers.
@@ -2765,7 +2706,7 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   for (int i = 0; i < n; ++i) out_ms[i] = (float)(acc[i] / iters);
   if (names && names_cap > 0) {
     std::string s = "sample+ingest";
-    for (auto& l : h->plan) { s += ";"; s += launch_name(l, h->h_probs, h->d_probs); }
+    for (auto& l : h->plan) s += ";" + l.label;
     snprintf(names, names_cap, "%s", s.c_str());
   }
   return sb.end();
