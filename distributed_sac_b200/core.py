@@ -448,6 +448,8 @@ class SacCore:
             return self._debug_raw(name, replica, cap).view(torch.int32)
         if name == "psave":
             cap = 2 * self.cfg.batch * self.cfg.act_dim * 8
+        elif name == "head":
+            cap = 2 * self.cfg.batch * 2 * self.cfg.act_dim
         elif name[0] == "h" or name.startswith("mixH"):
             widest = max(list(self.cfg.actor_hidden) + list(self.cfg.critic_hidden) + [4 * ((w + 3) // 4) * self.cfg.num_encoders
                                                                                         for w in self.cfg.mix_hidden])

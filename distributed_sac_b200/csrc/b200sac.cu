@@ -3017,6 +3017,7 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "dq_pi") { src = h->dqa.p + replica * 2 * h->y.rs; n = 2 * B; }      // [2][B]: d(actor loss)/dQk -- the min routing
   else if (nm == "d_action") { src = h->dact_dbg.p + replica * h->dact_dbg.rs; n = (int64_t)B * A; }
   else if (nm == "d_head") { src = h->dout_dbg.p + replica * h->dout_dbg.rs; n = (int64_t)B * 2 * A; }
+  else if (nm == "head") { src = h->pout.p + replica * h->pout.rs; n = (int64_t)2 * B * 2 * A; }      // [2B][2A]: mu | raw log-std
   else if (nm == "psave") { src = h->psave.p + replica * h->psave.rs; n = (int64_t)2 * B * A * kSaveW; }   // [2B][A][8]: std, diff, tanh, act, jac, EPS, mask, logp_j
   else if (nm == "isw" || nm == "prio" || nm == "idx") {   // prioritized replay: [B] weights, leaf values, ring indices (int32 bits)
     if (nm == "idx" && !h->per_buf && h->ns_buf) {          // a uniform linked ring: the indices its gather folded from

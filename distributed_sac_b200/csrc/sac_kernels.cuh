@@ -285,7 +285,7 @@ __device__ __noinline__ float log_f64r(float x) { return (float)log((double)x); 
 
 B200_D PolicyPoint policy_point(float mu, float raw, float eps, float k) {
   PolicyPoint p;
-  const float ls = fminf(fmaxf(raw, -20.f), 2.f);          // torch.clamp(x, -20, 2)
+  const float ls = raw < -20.f ? -20.f : (raw > 2.f ? 2.f : raw);   // torch.clamp(x, -20, 2), NaN included
   p.mask = (raw >= -20.f && raw <= 2.f) ? 1.f : 0.f;
   p.std = exp_f64r(ls);
   p.eps = eps;
@@ -578,7 +578,7 @@ B200_D void policy_dout_point(const StepConst& K, const float* __restrict__ sv, 
   const float g_u = g_u_t + glp * (-(diff) / var);
   dmu = g_u + glp * (diff / var);
   const float dstd = g_u * eps + glp * ((diff * diff) / (var * std) - 1.f / std);
-  dls = dstd * std * mask;
+  dls = mask != 0.f ? dstd * std : 0.f;          // torch.clamp's backward: zero outside [-20, 2], for a NaN log-std too
 }
 
 struct PolicyDoutArgs {

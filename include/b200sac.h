@@ -289,7 +289,8 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * name in {"y","q1","q2","a_next","logp_next","a_cur","logp_cur","qmin","d_action","d_head","r","d"}, "dq_pi" ([2][B]: d(actor loss)/dQ1, dQ2 -- which twin
  * min(Q1,Q2) routed the gradient to), "q_pi" ([2][B]: Q1, Q2 at (s, a~); layer-chained plan only), "psave" ([2B][act][8]:
  * what the policy head saved per (row, action) -- std, u-mu, tanh(u), action, Jacobian term, the NOISE it used, clamp mask,
- * log-prob term), or a hidden
+ * log-prob term), "head" ([2B][2*act]: the policy head's output as the head computed it, mu | log-std before the clamp;
+ * after b200sac_act its first n rows), or a hidden
  * activation whose sign pattern is the ReLU mask the step used: "hA.<l>" [2B][H] (rows [s';s]), "hQ.<l>" / "hP.<l>" /
  * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT),
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the

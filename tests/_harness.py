@@ -60,8 +60,8 @@ def _pad4(x):
 #   single   one hidden layer per network, act_dim 1, the CTA that holds both an s' row and an s row     2 / 2 / 2
 #   deep8    8 hidden layers each (15-stage chain2 table, 18 critic weight-gradient jobs), widths 4, 252, 256   4 / 2 / 2
 #   k32      actor input 27 and critic input 32, both evaluated directly                              8 / 4 / 2
-#   k33      critic input 33: the first input layer loaded through the weight pipeline                 8 / 8 / 4
-#   wide_in  a 248-wide critic input (8 chunks, padded pitch), act_dim 8 (kMaxAct)                    8 / 4 / 2
+#   k33      critic input 33: the first input layer loaded through the weight pipeline; action scale 1.5  8 / 8 / 4
+#   wide_in  a 248-wide critic input (8 chunks, padded pitch), act_dim 8 (kMaxAct), action scale 2.5  8 / 4 / 2
 #   tasks33  the upper half of TaskAlpha (task index 32)                                              4 / 2 / 2
 #   tasks64  all 64 task slots, weighted loss                                                         4 / 2 / 2
 #   big_odd  batch 531: a 19-row final weight-gradient pass, 8 rows per CTA in every chain launch     8 / 8 / 8
@@ -70,8 +70,10 @@ CHAIN_CASES = {
     "deep8": dict(state_dim=9, num_tasks=0, act_dim=2, actor_hidden=[4, 12, 36, 100, 256, 252, 8, 44],
                   critic_hidden=[252, 4, 68, 256, 12, 36, 100, 20], batch=101),
     "k32": dict(state_dim=27, num_tasks=0, act_dim=5, actor_hidden=[64, 48], critic_hidden=[40, 64], batch=203),
-    "k33": dict(state_dim=29, num_tasks=0, act_dim=4, actor_hidden=[64, 48], critic_hidden=[40, 64], batch=301),
-    "wide_in": dict(state_dim=240, num_tasks=0, act_dim=8, actor_hidden=[256, 132], critic_hidden=[196, 256], batch=203),
+    "k33": dict(state_dim=29, num_tasks=0, act_dim=4, actor_hidden=[64, 48], critic_hidden=[40, 64], batch=301,
+                action_scale=1.5),
+    "wide_in": dict(state_dim=240, num_tasks=0, act_dim=8, actor_hidden=[256, 132], critic_hidden=[196, 256], batch=203,
+                    action_scale=2.5),
     "tasks33": dict(state_dim=10, num_tasks=33, act_dim=3, actor_hidden=[64, 64], critic_hidden=[64, 64], batch=99),
     "tasks64": dict(state_dim=6, num_tasks=64, act_dim=2, actor_hidden=[48, 48], critic_hidden=[48, 48], batch=128,
                     weighted_loss=True),
@@ -81,32 +83,38 @@ CHAIN_CASES = {
 # The per-layer envelope, id -> SacSpec fields.  Each case is outside the chained envelope through its own shape (a hidden
 # width that is not a multiple of 4 or above 256, or obs + act > 252), so precision 0 takes the per-layer plan too.
 #   b1         batch 1: every GEMM on FFMA at both precisions, thin input-layer gradients, one hidden layer each
-#   odd67      odd pitches everywhere (no wgmma at precision 1 either), La != Lc, the 8-column critic head at an odd batch
+#   odd67      odd pitches everywhere (no wgmma at precision 1 either), La != Lc, the 8-column critic head at an odd batch;
+#              action scale 0.4 (the scale, like the others below that are not 1, is not a power of two: act / k rounds)
 #   in45       wgmma on padded first layers (critic 45 in 48, actor 41 in 44) at a batch that is not a multiple of 128
 #   in17       input width 17: FFMA (not thin) in a 20-float pitch
 #   mixed      precision 1 groups of wgmma-eligible and ineligible problems (one wgmma + one FFMA launch)
 #   deep8      8 actor hidden layers (widths 4, 33, 260, 512), one critic hidden layer: La != Lc the other way
 #   wide1024   1024-wide layers at batch 640: several column tiles, N tails of 128- and 160-wide tiles; the cost model picks
 #              every tile width and split factors 4, 2 and 1
-#   split517   batch 517: K slices 160/160/160/37 and head row slices 130/130/130/127; thin input-layer gradients on K slices
+#   split517   batch 517: K slices 160/160/160/37 and head row slices 130/130/130/127; thin input-layer gradients on K slices;
+#              action scale 3
 #   b512n      the first sliced batch; 8-column critic head with row slices
-#   pdout257   policy_dout without gradient slices, just above B * A = 2048; act_dim 8 (policy head backward NO = 16)
+#   pdout257   policy_dout without gradient slices, just above B * A = 2048; act_dim 8 (policy head backward NO = 16);
+#              action scale 1.5
 #   pdout256   B * A = 2048 exactly: the policy-head output gradient stays inside head_bwd
 #   b2048      the largest batch; 64 tasks, weighted loss; NO = 16 over 512-row slices; 8-column critic head with slices
 #   act1_2000  act_dim 1 with the in-kernel policy backward at row slices; a 600-deep thin input gradient (two K passes)
 #   tasks33    the upper half of the task table (task index 32) in plain SAC
 LAYER_CASES = {
     "b1": dict(state_dim=3, num_tasks=0, act_dim=1, actor_hidden=[37], critic_hidden=[29], batch=1),
-    "odd67": dict(state_dim=11, num_tasks=0, act_dim=3, actor_hidden=[37, 61], critic_hidden=[29, 45, 53], batch=67),
+    "odd67": dict(state_dim=11, num_tasks=0, act_dim=3, actor_hidden=[37, 61], critic_hidden=[29, 45, 53], batch=67,
+                  action_scale=0.4),
     "in45": dict(state_dim=41, num_tasks=0, act_dim=4, actor_hidden=[260, 64], critic_hidden=[64, 260], batch=130),
     "in17": dict(state_dim=15, num_tasks=0, act_dim=2, actor_hidden=[260, 36], critic_hidden=[36, 260], batch=96),
     "mixed": dict(state_dim=36, num_tasks=0, act_dim=4, actor_hidden=[400, 64], critic_hidden=[24, 400], batch=256),
     "deep8": dict(state_dim=9, num_tasks=0, act_dim=2, actor_hidden=[4, 33, 260, 512, 64, 36, 100, 20], critic_hidden=[130],
                   batch=150),
     "wide1024": dict(state_dim=39, num_tasks=0, act_dim=4, actor_hidden=[1024, 520], critic_hidden=[1024, 400], batch=640),
-    "split517": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[260, 96], critic_hidden=[96, 260], batch=517),
+    "split517": dict(state_dim=8, num_tasks=0, act_dim=2, actor_hidden=[260, 96], critic_hidden=[96, 260], batch=517,
+                     action_scale=3.0),
     "b512n": dict(state_dim=17, num_tasks=0, act_dim=5, actor_hidden=[96, 260], critic_hidden=[72, 131], batch=512),
-    "pdout257": dict(state_dim=10, num_tasks=0, act_dim=8, actor_hidden=[64, 66], critic_hidden=[64, 66], batch=257),
+    "pdout257": dict(state_dim=10, num_tasks=0, act_dim=8, actor_hidden=[64, 66], critic_hidden=[64, 66], batch=257,
+                     action_scale=1.5),
     "pdout256": dict(state_dim=10, num_tasks=0, act_dim=8, actor_hidden=[64, 66], critic_hidden=[64, 66], batch=256),
     "b2048": dict(state_dim=30, num_tasks=64, act_dim=8, actor_hidden=[300, 128], critic_hidden=[128, 131], batch=2048,
                   weighted_loss=True),

@@ -59,7 +59,11 @@ def act_masks(core, spec, n, replica):
     """{ReluTape tag: what act used} -- the sign patterns of its own hidden activations and its tanh(u)."""
     B = spec.batch
     m = {f"actor:act:{l}": core.debug(f"hA.{l}", replica).reshape(2 * B, H)[:n] > 0 for l, H in enumerate(spec.actor_hidden)}
-    m["tanh:act"] = core.debug("psave", replica).reshape(2 * B, spec.act_dim, 8)[:n, :, 2].double()
+    t = core.debug("psave", replica).reshape(2 * B, spec.act_dim, 8)[:n, :, 2]
+    # the reference takes log(k (1 - (a / k)^2 + 1e-6)) of its fp32 action a = k tanh(u); where tanh saturates, a / k as
+    # fp32 rounds it decides that term, so the fp64 oracle continues with that value (== tanh(u) at k = 1)
+    k = torch.tensor(spec.action_scale, dtype=torch.float32)
+    m["tanh:act"] = ((k * t) / k).double()
     return m
 
 

@@ -41,7 +41,8 @@ _O = dict(modified=False, weighted_loss=False)
 #   k1_t1         one encoder and one task: softmax of one logit (trunk untouched on both sides); a 33 -> 70 table layer
 #                 (remainder loop) and a 70-wide input (tail loop only); mix_out 9; a partial CTA in both mixfwd jobs
 #   k32           K = 32 everywhere: 128 (encoder, 8-row) tasks over 24 warps; K + ctx_out = 72; cmf 96 KB
-#   nl3           two mixture hidden layers (ha -> hb); a 256-wide table input (one 8-wide pass); cmf 187 KB
+#   nl3           two mixture hidden layers (ha -> hb); a 256-wide table input (one 8-wide pass); cmf 187 KB; action
+#                 scale 2
 #   deep4         three mixture hidden layers (ha reused); 68 / 72 / 66-wide layers (two o0 passes, the second partial);
 #                 trunk 36 -> 72 (remainder loop); ctx_in 1000 (24-, 8-wide and tail loops, lanes split)
 #   deep9         9 mixture layers: the fallback by depth; 9-layer trunk and context nets
@@ -58,7 +59,7 @@ CASES = {
     "k32": dict(state_dim=12, num_tasks=8, num_encoders=32, mix_hidden=[8], mix_out=8, ctx_in=768, ctx_hidden=[48], ctx_out=40,
                 batch=200),
     "nl3": dict(state_dim=39, num_tasks=3, num_encoders=7, mix_hidden=[40, 24], mix_out=20, ctx_in=256, ctx_hidden=[100],
-                ctx_out=20, batch=123),
+                ctx_out=20, batch=123, action_scale=2.0),
     "deep4": dict(state_dim=23, num_tasks=5, num_encoders=2, mix_hidden=[68, 36, 72], mix_out=66, ctx_in=1000,
                   ctx_hidden=[64, 65], ctx_out=30, batch=155),
     "deep9": dict(state_dim=39, num_tasks=3, num_encoders=4, mix_hidden=[16, 6, 32, 12, 8, 24, 40, 20], mix_out=14, ctx_in=64,

@@ -110,6 +110,33 @@ def test_run_loop_with_redis_stub(cuda, tmp_path):
     lrn.memory.stop()
 
 
+def test_mtsac_learner_action_bound_sets_the_action_scale(cuda, tmp_path):
+    """MTSACLearner reads action_bound from its cfg's actor block (MS/learner.py): [-2, 2] gives a core with action scale 2,
+    and acting in every mode stays within the bound and uses it (a head that ignored the scale would stay within 1)."""
+    from distributed_sac_b200.learner import MTSACLearner
+    T = 4
+    cfg = {"device": "cuda", "buffer_size": 4096, "reward_scale": 1, "batch_size": 64, "gamma": 0.99, "tau": 0.005,
+           "log_alpha": 0, "start_memory_len": 1000, "print_period_learner": 10, "update_delay": 1, "num_tasks": T,
+           "actor": {"lr_actor": 3e-4, "state_dim": 12, "action_dim": 3, "action_bound": [-2.0, 2.0], "actor_hidden_dim": [64, 64]},
+           "critic": {"lr_critic": 3e-4, "critic_hidden_dim": [64, 64]}}
+    p = tmp_path / "ms.json"
+    p.write_text(json.dumps(cfg))
+    lrn = MTSACLearner(None, [f"t{i}" for i in range(T)], str(p), write_mode=False, replay_where="device",
+                       server=redis_stub.StrictRedis(host=str(tmp_path) + "ms"))
+    try:
+        assert lrn.core.cfg.action_scale == 2.0
+        g = torch.Generator().manual_seed(0)
+        obs = torch.cat([3 * torch.randn(128, 12, generator=g), torch.eye(T)[torch.arange(128) % T]], 1)
+        for stochastic in (True, False):
+            a = lrn.act_batch(obs, stochastic=stochastic)
+            assert a.shape == (128, 3) and torch.isfinite(a).all()
+            assert float(a.abs().max()) <= 2.0 and float(a.abs().max()) > 1.0, (stochastic, float(a.abs().max()))
+        lrn.memory.ring.fill_synthetic(4096, seed=1)
+        assert all(x == x for x in lrn.update())
+    finally:
+        lrn.memory.stop()
+
+
 @pytest.mark.parametrize("modified", [True, False], ids=["CARE(M)", "CARE(O)"])
 def test_care_learner_surface(cuda, tmp_path, modified):
     """CARELearner: cfg 'encoder' block + metadata JSONs as in MT10_Distributed_CARE_cfg.json; published blob has the
