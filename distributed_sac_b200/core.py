@@ -49,6 +49,7 @@ class CoreConfig:
     emb_dim: int = 50
     lr_ctx: float = 3e-4
     grad_clip: bool = False              # the step plan with gradient-norm clipping and norms (SacCore.set_grad_clip)
+    pcgrad: bool = False                 # the per-layer plan with PCGrad gradient surgery (SacCore.set_pcgrad); num_tasks >= 2
 
     @property
     def obs_dim(self):
@@ -73,6 +74,7 @@ class CoreConfig:
         c.log_alpha_init = self.log_alpha_init
         c.care = (2 if self.care_original else 1) if self.care else 0
         c.grad_clip = int(self.grad_clip)
+        c.pcgrad = int(self.pcgrad)
         if self.care:
             c.emb_dim, c.lr_ctx = self.emb_dim, self.lr_ctx
             c.num_encoders, c.mix_out, c.ctx_in, c.ctx_out = self.num_encoders, self.mix_out, self.ctx_in, self.ctx_out
@@ -353,10 +355,50 @@ class SacCore:
         _lib.check(self.lib.b200sac_read_grad_norms(self._h, int(n_last), _ptr(out), _stream()))
         return out
 
+    # ---- PCGrad gradient surgery (b200sac_set/get/read_pcgrad, b200sac_export_task_grad; handles with pcgrad=True) --------
+    def get_pcgrad(self, replica=0) -> Dict[str, bool]:
+        """{critic, actor} surgery switches of one replica (no synchronisation)."""
+        c, a = C.c_int32(0), C.c_int32(0)
+        _lib.check(self.lib.b200sac_get_pcgrad(self._h, int(replica), C.byref(c), C.byref(a)))
+        return {"critic": bool(c.value), "actor": bool(a.value)}
+
+    def set_pcgrad(self, critic=None, actor=None, replica=None):
+        """Turn the critic's / actor's gradient surgery on or off for one replica (replica=None: all of them) on the current
+        stream; a switch left out keeps its value.  Off: Adam reads the plain sum of the task gradients, and the Gram matrix
+        is still computed.  Steps enqueued afterwards use the new switches."""
+        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+            cur = self.get_pcgrad(r)
+            for k, v in dict(critic=critic, actor=actor).items():
+                if v is not None:
+                    cur[k] = bool(v)
+            _lib.check(self.lib.b200sac_set_pcgrad(self._h, r, int(cur["critic"]), int(cur["actor"]), _stream()))
+
+    def read_pcgrad(self, replica=0) -> Dict[str, np.ndarray]:
+        """The last step's surgery record of one replica, index 0 critic and 1 actor: gram [2][T][T] (fp64), w [2][T],
+        perm [2][T][T] (row i = the order task i was projected in), projected [2][T][T] bool (task i onto task j), and
+        task_mismatch, the rows of the step that were not in task-block order."""
+        T = self.cfg.num_tasks
+        gram = np.empty((2, T, T), np.float64)
+        w = np.empty((2, T), np.float32)
+        perm = np.empty((2, T, T), np.int32)
+        mask = np.empty((2, T), np.uint64)
+        bad = C.c_int32(0)
+        _lib.check(self.lib.b200sac_read_pcgrad(self._h, int(replica), gram.ctypes.data, w.ctypes.data, perm.ctypes.data,
+                                                mask.ctypes.data, C.byref(bad), _stream()))
+        bits = np.uint64(1) << np.arange(T, dtype=np.uint64)
+        projected = (mask[:, :, None] & bits[None, None, :]) != 0
+        return {"gram": gram, "w": w, "perm": perm, "projected": projected, "task_mismatch": int(bad.value)}
+
+    def export_task_grad(self, task: int, replica=0) -> torch.Tensor:
+        """Gradient of the last step over the rows of task `task` alone (the trainable arena, CPU tensor)."""
+        out = torch.empty(self.trainable_floats, dtype=torch.float32)
+        _lib.check(self.lib.b200sac_export_task_grad(self._h, int(replica), int(task), _ptr(out), out.numel(), _stream()))
+        return out
+
     def copy_replica(self, src: int, dst: int):
         """Replica dst's parameters (targets, log_alpha included), Adam moments and step counters become a copy of src's,
-        device to device on the current stream.  Hyperparameters, update intervals, gradient-clipping thresholds and replay
-        data stay dst's own."""
+        device to device on the current stream.  Hyperparameters, update intervals, gradient-clipping thresholds, PCGrad
+        switches and replay data stay dst's own."""
         _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
 
     def soft_update(self, tau: float, critic: Optional[int] = None):

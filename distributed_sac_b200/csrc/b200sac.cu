@@ -34,6 +34,7 @@
 #include "per_kernels.cuh"
 #include "nstep_kernels.cuh"
 #include "clip_kernels.cuh"
+#include "pcgrad_kernels.cuh"
 
 using namespace bsac;
 
@@ -126,6 +127,9 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->precision != 0 && c->precision != 1) return fail(B200SAC_ERR_INVALID, "precision must be 0 (fp32 FFMA) or 1 (3xTF32 wgmma)");
   if (c->care != 0 && c->care != 1 && c->care != 2) return fail(B200SAC_ERR_INVALID, "care must be 0, 1 (CARE(M)) or 2 (CARE(O))");
   if (c->grad_clip != 0 && c->grad_clip != 1) return fail(B200SAC_ERR_INVALID, "grad_clip must be 0 or 1");
+  if (c->pcgrad != 0 && c->pcgrad != 1) return fail(B200SAC_ERR_INVALID, "pcgrad must be 0 or 1");
+  if (c->pcgrad && (c->num_tasks < 2 || c->care != 0 || c->grad_clip != 0))
+    return fail(B200SAC_ERR_INVALID, "pcgrad needs num_tasks >= 2, no CARE encoder and no grad_clip");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -254,7 +258,7 @@ struct Buf {           // [R][n] fp32 (or int32) slab slice
   long long rs = 0;    // replica stride in floats
 };
 
-enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2, L_GRADNORM };
+enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2, L_GRADNORM, L_PCGRAD };
 
 struct Launch {
   LaunchKind kind;
@@ -286,6 +290,7 @@ struct Launch {
   WgradArgs wg;
   bool store_only = false;   // L_WGRAD: the gradients alone, no optimizer step (grad_clip plans)
   GradNormArgs gn;
+  PcgArgs pc;
   // What b200sac_profile_step calls the launch, set by the builder that makes it.  The part before '(' and the "wgmma"
   // substring are what bench.py groups kernels by.
   std::string label;
@@ -418,6 +423,19 @@ struct b200sac {
   float* gnorm_h_dev = nullptr;
   DevMem<double> gn_part;
   DevMem<unsigned> gn_ticket;
+  // gradient surgery (cfg.pcgrad): [R][2] switches (critic, actor) and their host mirror, the pcgrad launches' partial
+  // products [2][R][kGradNormMaxBlocks][T(T+1)/2] and tickets [2][R], the last step's record per replica and optimizer
+  // (G [R][2][T][T], w [R][2][T] -- also what Adam reads --, permutations [R][2][T][T], projection masks [R][2][T]) and
+  // the rows of the last step whose task id was not i / P [R]
+  DevMem<int> pc_on;
+  std::vector<int> pc_on_host;
+  DevMem<double> pc_part;
+  DevMem<unsigned> pc_ticket;
+  DevMem<double> pc_G;
+  DevMem<float> pc_w;
+  DevMem<int> pc_perm;
+  DevMem<unsigned long long> pc_mask;
+  DevMem<int> pc_bad;
 
   // The members release their resources; the publication stream's last copy lands first.
   ~b200sac() {
@@ -650,7 +668,7 @@ static int make_tc_prob(const GemmProb& p, int rep, TcProb& t, int bn = 64) {
 // ------------------------------------------------------------------------------------------
 static bool fused_eligible(const b200sac* h) {
   const b200sac_cfg& c = h->cfg;
-  if (c.precision != 0 || c.care || !h->env.fuse) return false;
+  if (c.precision != 0 || c.care || c.pcgrad || !h->env.fuse) return false;
   for (int i = 0; i < c.n_actor_hidden; ++i) if (c.actor_hidden[i] % 4 || c.actor_hidden[i] > CH_MAXW) return false;
   for (int i = 0; i < c.n_critic_hidden; ++i) if (c.critic_hidden[i] % 4 || c.critic_hidden[i] > CH_MAXW) return false;
   if (c.state_dim + c.num_tasks + c.act_dim > CH_MAXW - 4) return false;
@@ -812,6 +830,7 @@ struct PlanBuilder {
   void opt_slice(int which, int64_t& beg, int64_t& n) const;
   void adam(int which, bool tail_only, bool with_tail = true);
   void grad_norm(int which);
+  void pcgrad(int which);
   int build_plan_fused();
   void build_plan_layered();
 };
@@ -836,11 +855,13 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
   // handful of tiles, so one CTA would walk 32-40 k chunks alone.
   // WGRAD operands are both [K][*] row-major, so a K slice is just a row offset: slice s of a problem becomes its own
   // problem writing gradient slice s; Adam adds the slices in index order (deterministic, no atomics).
+  // pcgrad handles: every weight gradient is cut into the T task blocks of B / T rows, slice t = task t's gradient.
+  auto sliced = [&](const GemmProb& p) { return p.mode == GEMM_WGRAD && (c.pcgrad || (p.K >= kSplitKMin && h->gslices > 1)); };
   auto expand = [&](int Smax, std::vector<GemmProb>& out) {
     for (auto& p : ps_in) {
-      const int S = (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) ? Smax : 1;
+      const int S = sliced(p) ? Smax : 1;
       if (S == 1) { out.push_back(p); continue; }
-      const int len = (((p.K + S - 1) / S) + 31) & ~31;
+      const int len = c.pcgrad ? p.K / S : (((p.K + S - 1) / S) + 31) & ~31;
       const long long coff = p.C - h->grads, c2off = p.C2 ? p.C2 - h->grads : 0;
       if (coff < 0 || coff >= L.trainable) { rc = fail(B200SAC_ERR_INVALID, "internal: split-K output outside the gradient arena"); out.push_back(p); continue; }
       for (int sidx = 0; sidx < S; ++sidx) {
@@ -869,8 +890,8 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
   std::vector<GemmProb> ps;
   int split = 1;                        // what expand did to this group's weight gradients (launch labels)
   {
-    int S = kSplitK;
-    if (c.precision == 1) {
+    int S = c.pcgrad ? h->gslices : kSplitK;
+    if (c.precision == 1 && !c.pcgrad) {
       double best = 1e300;
       for (int s_ = kSplitK; s_ >= 1; s_ >>= 1) {
         std::vector<GemmProb> trial;
@@ -883,7 +904,7 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
     }
     expand(S, ps);
     for (auto& p : ps_in)
-      if (p.mode == GEMM_WGRAD && p.K >= kSplitKMin && h->gslices > 1) split = S;
+      if (sliced(p)) split = S;
   }
   if (c.precision == 1) {
     std::vector<GemmProb> tc, rest;
@@ -1125,6 +1146,8 @@ void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
     P.coef = h->clip_coef + which;
     if (h->fused) { P.gx = nullptr; P.nx = 0; }       // the chained weight-gradient launches write slice 0 only
   }
+  const bool pcg = c.pcgrad && !tail_only && which < 2;
+  if (pcg) P.pcw = h->pc_w + (size_t)which * c.num_tasks;
   P.lq = h->lq.p; P.la = h->la.p; P.rsY = h->y.rs;
   P.logp_cur = h->logp.p + B; P.logstd_sum = h->logstd.p + B; P.rsLogp = h->logp.rs;
   P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
@@ -1134,7 +1157,7 @@ void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
   const int nb = elementwise_blocks(n);
   l.grid = dim3(nb + (P.tail != TAIL_NONE ? 1 : 0), R);
   l.block = dim3(256);
-  l.join = !clip;                // every gradient of the slice must have landed, including the forked weight gradients
+  l.join = !clip && !pcg;        // every gradient of the slice must have landed, including the forked weight gradients
   if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
   h->plan.push_back(l);
 }
@@ -1159,6 +1182,32 @@ void PlanBuilder::grad_norm(int which) {
   P.R = R;
   l.grid = dim3(elementwise_blocks(n), R);
   l.block = dim3(256);
+  l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
+  h->plan.push_back(l);
+}
+
+// pcgrad handles: the Gram matrix of optimizer `which`'s task slices, the surgery and the slice weights its Adam launch
+// (next) applies
+void PlanBuilder::pcgrad(int which) {
+  Launch l;
+  l.kind = L_PCGRAD;
+  l.label = which == 0 ? "pcgrad{critic}" : "pcgrad{actor}";
+  PcgArgs& P = l.pc;
+  memset(&P, 0, sizeof(P));
+  int64_t beg, n;
+  opt_slice(which, beg, n);
+  const int T = c.num_tasks;
+  P.g = h->grads + beg; P.gx = h->grads_x + beg; P.xs = (long long)R * L.trainable; P.rsM = rsG; P.n = n;
+  P.T = T; P.opt = which;
+  P.cnt = h->cnt; P.on = h->pc_on;
+  P.part = h->pc_part + (size_t)which * R * kGradNormMaxBlocks * pcgrad_pairs(T);
+  P.ticket = h->pc_ticket + (size_t)which * R;
+  P.G = h->pc_G; P.w = h->pc_w; P.perm = h->pc_perm; P.mask = h->pc_mask;
+  if (which == 0) { P.tid = (const int*)h->tid.p; P.rsR = h->r.rs; P.B = B; P.bad = h->pc_bad; }
+  P.seed = h->K.seed;
+  l.grid = dim3(elementwise_blocks(n), R);
+  l.block = dim3(256);
+  l.smem = pcgrad_smem(T);
   l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
   h->plan.push_back(l);
 }
@@ -1640,6 +1689,7 @@ void PlanBuilder::build_plan_layered() {
     }
   }
   if (c.grad_clip) grad_norm(0);
+  if (c.pcgrad) pcgrad(0);
   adam(0, false);
   // ---- the actor update (D, E): every launch below returns at entry on a critic-only step; adam(1) skips its own body and
   // its tail writes NaN for the actor-side losses.  adam(2) (CARE(O) context encoder, trained by the critic loss) always runs.
@@ -1709,6 +1759,7 @@ void PlanBuilder::build_plan_layered() {
   }
   actor_side = false;
   if (c.grad_clip) grad_norm(1);          // (returns at entry on a critic-only step, like the launches of D and E)
+  if (c.pcgrad) pcgrad(1);                // (likewise)
   adam(1, false);
   if (c.care == 2) {                      // update(): context_encoder_optimizer.step() (learner.py:399), gradients from the critic loss
     if (c.grad_clip) grad_norm(2);
@@ -1753,6 +1804,8 @@ static int build_plan(b200sac* h) {
   if (max_smem > 200 * 1024) return fail(B200SAC_ERR_INVALID, "batch * head width too large for head_bwd smem");
   CU(cudaFuncSetAttribute(head_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
   CU(cudaFuncSetAttribute(head_bwd4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
+  if (h->cfg.pcgrad)
+    CU(cudaFuncSetAttribute(pcgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcgrad_smem(h->cfg.num_tasks)));
   return 0;
 }
 
@@ -1863,7 +1916,10 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
         else launch_k(head_bwd_kernel, l.grid, l.block, l.smem, s, K, l.hb);
         break;
       case L_ADAM:
-        launch_k(l.ad.coef ? adam_kernel<true> : adam_kernel<false>, l.grid, l.block, 0, s, K, l.ad);
+        launch_k(l.ad.pcw ? adam_kernel<false, true> : l.ad.coef ? adam_kernel<true> : adam_kernel<false>, l.grid, l.block, 0, s, K, l.ad);
+        break;
+      case L_PCGRAD:
+        launch_k(pcgrad_kernel, l.grid, l.block, l.smem, s, K, l.pc);
         break;
       case L_GRADNORM:
         launch_k(grad_sqnorm_kernel, l.grid, l.block, 0, s, K, l.gn);
@@ -1983,6 +2039,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   CU(cudaMemset(h->adam_v, 0, sizeof(float) * L.trainable * R));
   CU(cudaMemset(h->grads, 0, sizeof(float) * L.trainable * R));
   h->gslices = cfg->batch >= kSplitKMin ? kSplitK : 1;   // K of every weight gradient = batch
+  if (cfg->pcgrad) h->gslices = cfg->num_tasks;         // one slice per task
   if (h->gslices > 1) {     // never-written entries of slices >= 1 must read as zero (Adam sums all slices)
     CU(cudaMalloc(h->grads_x.put(), sizeof(float) * L.trainable * R * (h->gslices - 1)));
     CU(cudaMemset(h->grads_x, 0, sizeof(float) * L.trainable * R * (h->gslices - 1)));
@@ -2022,6 +2079,28 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMalloc(h->gn_part.put(), sizeof(double) * kGradNormMaxBlocks * n));
     CU(cudaMalloc(h->gn_ticket.put(), sizeof(unsigned) * n));
     CU(cudaMemset(h->gn_ticket, 0, sizeof(unsigned) * n));
+  }
+  if (cfg->pcgrad) {          // switches on, weights 1, record NaN until a step writes it
+    const int T = cfg->num_tasks;
+    const size_t n2 = (size_t)2 * R;
+    h->pc_on_host.assign(n2, 1);
+    CU(cudaMalloc(h->pc_on.put(), sizeof(int) * n2));
+    CU(cudaMemcpy(h->pc_on, h->pc_on_host.data(), sizeof(int) * n2, cudaMemcpyHostToDevice));
+    CU(cudaMalloc(h->pc_part.put(), sizeof(double) * n2 * kGradNormMaxBlocks * pcgrad_pairs(T)));
+    CU(cudaMalloc(h->pc_ticket.put(), sizeof(unsigned) * n2));
+    CU(cudaMemset(h->pc_ticket, 0, sizeof(unsigned) * n2));
+    const std::vector<double> gnan(n2 * T * T, NAN);
+    CU(cudaMalloc(h->pc_G.put(), sizeof(double) * n2 * T * T));
+    CU(cudaMemcpy(h->pc_G, gnan.data(), sizeof(double) * n2 * T * T, cudaMemcpyHostToDevice));
+    const std::vector<float> ones(n2 * T, 1.0f);
+    CU(cudaMalloc(h->pc_w.put(), sizeof(float) * n2 * T));
+    CU(cudaMemcpy(h->pc_w, ones.data(), sizeof(float) * n2 * T, cudaMemcpyHostToDevice));
+    CU(cudaMalloc(h->pc_perm.put(), sizeof(int) * n2 * T * T));
+    CU(cudaMemset(h->pc_perm, 0, sizeof(int) * n2 * T * T));
+    CU(cudaMalloc(h->pc_mask.put(), sizeof(unsigned long long) * n2 * T));
+    CU(cudaMemset(h->pc_mask, 0, sizeof(unsigned long long) * n2 * T));
+    CU(cudaMalloc(h->pc_bad.put(), sizeof(int) * R));
+    CU(cudaMemset(h->pc_bad, 0, sizeof(int) * R));
   }
 
   // work slab.  Buffers that a kernel addresses with one replica stride get one length: rsX (XQ, XT, XP), rsR (r, d, tid),
@@ -2355,6 +2434,63 @@ extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double criti
   return 0;
 }
 
+// Gradient-surgery switches: a device row [R][2] written in stream order like the hyperparameters, read by the pcgrad
+// launches of the step graphs.
+extern "C" int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_t* actor_on) {
+  if (!h || !critic_on || !actor_on) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  *critic_on = h->pc_on_host[(size_t)replica * 2]; *actor_on = h->pc_on_host[(size_t)replica * 2 + 1];
+  return 0;
+}
+
+extern "C" int b200sac_set_pcgrad(b200sac_t* h, int32_t replica, int32_t critic_on, int32_t actor_on, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if ((critic_on != 0 && critic_on != 1) || (actor_on != 0 && actor_on != 1))
+    return fail(B200SAC_ERR_INVALID, "pcgrad switches must be 0 or 1, got %d, %d", critic_on, actor_on);
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  set_pcgrad_kernel<<<1, 1, 0, sb.run>>>(h->pc_on, replica, critic_on, actor_on);
+  CU(cudaGetLastError());
+  if (int rc = sb.end()) return rc;
+  h->pc_on_host[(size_t)replica * 2] = critic_on; h->pc_on_host[(size_t)replica * 2 + 1] = actor_on;
+  return 0;
+}
+
+extern "C" int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, int32_t* perm, uint64_t* mask,
+                                   int32_t* task_mismatch, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  const size_t T = (size_t)h->cfg.num_tasks, r2 = (size_t)replica * 2;
+  CU(cudaSetDevice(h->device));
+  cudaStream_t st = (cudaStream_t)stream;
+  CU(cudaStreamSynchronize(st));
+  if (gram) CU(cudaMemcpy(gram, h->pc_G + r2 * T * T, sizeof(double) * 2 * T * T, cudaMemcpyDeviceToHost));
+  if (w) CU(cudaMemcpy(w, h->pc_w + r2 * T, sizeof(float) * 2 * T, cudaMemcpyDeviceToHost));
+  if (perm) CU(cudaMemcpy(perm, h->pc_perm + r2 * T * T, sizeof(int) * 2 * T * T, cudaMemcpyDeviceToHost));
+  if (mask) CU(cudaMemcpy(mask, h->pc_mask + r2 * T, sizeof(uint64_t) * 2 * T, cudaMemcpyDeviceToHost));
+  if (task_mismatch) CU(cudaMemcpy(task_mismatch, h->pc_bad + replica, sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int b200sac_export_task_grad(b200sac_t* h, int32_t replica, int32_t task, float* buf, int64_t n_floats, void* stream) {
+  if (!h || !buf) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (task < 0 || task >= h->cfg.num_tasks) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
+  const int64_t n = h->L.trainable;
+  if (n_floats != n) return fail(B200SAC_ERR_INVALID, "the gradient arena holds %lld floats per replica, got %lld", (long long)n, (long long)n_floats);
+  const float* src = task == 0 ? h->grads.get() : h->grads_x + (size_t)(task - 1) * h->R * n;
+  CU(cudaSetDevice(h->device));
+  CU(cudaMemcpyAsync(buf, src + (size_t)replica * n, n * sizeof(float), cudaMemcpyDefault, (cudaStream_t)stream));
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
 extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   if (src < 0 || src >= h->R || dst < 0 || dst >= h->R)
@@ -2658,6 +2794,17 @@ extern "C" int b200sac_step_host(b200sac_t* h, const float* s, const float* a, c
                                  const float* d, const float* eps_next, const float* eps_cur, float* out_losses, void* stream) {
   if (!h || !s || !a || !r || !s2 || !d) return fail(B200SAC_ERR_INVALID, "null minibatch pointer");
   if ((eps_next == nullptr) != (eps_cur == nullptr)) return fail(B200SAC_ERR_INVALID, "eps_next and eps_cur must both be given or both NULL");
+  if (h->cfg.pcgrad) {          // row i must belong to task i / P (the first maximum of its one-hot, as the ingest reads it)
+    const int B = h->cfg.batch, T = h->cfg.num_tasks, obs = h->K.obs;
+    for (long long i = 0; i < (long long)h->R * B; ++i) {
+      const float* oh = s + i * obs + (obs - T);
+      int t = 0;
+      for (int q = 1; q < T; ++q) if (oh[q] > oh[t]) t = q;
+      if (t != (int)(i % B) / (B / T))
+        return fail(B200SAC_ERR_INVALID, "pcgrad: replica %lld row %lld belongs to task %d, not to task %d (rows in task blocks of batch / num_tasks)",
+                    i / B, i % B, t, (int)(i % B) / (B / T));
+    }
+  }
   CU(cudaSetDevice(h->device));
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
@@ -3396,7 +3543,9 @@ static int host_draw(b200sac_replay* rb, int replica, std::vector<long long>& id
       if (seen.insert(v).second) idx.push_back((long long)t * rb->cap_per_task + v);
     }
   }
-  if (rb->Teff > 1) std::shuffle(idx.begin(), idx.end(), rb->rng);   // MS/replay_buffers.py:83-84
+  // MS/replay_buffers.py:83-84.  A pcgrad handle keeps the task blocks: its plan cuts the minibatch into tasks at rows
+  // i / (B/T), and the losses are row sums, so the row order does not change what a step computes.
+  if (rb->Teff > 1 && !rb->h->cfg.pcgrad) std::shuffle(idx.begin(), idx.end(), rb->rng);
   return 0;
 }
 

@@ -900,6 +900,8 @@ struct AdamArgs {
   int R;
   const float* coef;                                 // adam_kernel<true>: coef[rep * 3] multiplies the gradient (the column of
                                                      // this optimizer in the [R][3] clip coefficients grad_sqnorm_kernel wrote)
+  const float* pcw;                                  // adam_kernel<false, true>: pcw[rep * 2 * (nx + 1) + k] weighs gradient
+                                                     // slice k (pcgrad_kernel's w of this optimizer)
 };
 
 B200_D void adam_scalars(double lr, double b1_pow_t, double b2_pow_t, float& step_size, float& bc2_sqrt) {
@@ -919,7 +921,9 @@ B200_D void adam_one(float& p, float& m, float& v, float g, float w1, float b2, 
 
 // CLIP (grad_clip plans): Adam runs on g * coef, one fp32 multiply per element, with the replica's clip coefficient of this
 // optimizer (grad_sqnorm_kernel, clip_kernels.cuh); the gradient arena keeps g.
-template <bool CLIP = false>
+// PCG (pcgrad plans): Adam runs on w_0 g_0 + w_1 g_1 + ... over the nx + 1 task slices, each product rounded to fp32 and
+// the products added in index order (pcgrad_kernels.cuh); the gradient arena keeps the slices.
+template <bool CLIP = false, bool PCG = false>
 __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   KStamp ks_;
   const int rep = blockIdx.y;
@@ -929,6 +933,8 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
   __shared__ float s_coef;
   const bool is_tail = (P.tail != TAIL_NONE) && (blockIdx.x == gridDim.x - 1);
   if (!is_tail) {
+    if constexpr (PCG)           // the slice weights (the tail job uses red[] for its sums)
+      if (threadIdx.x <= P.nx) red[threadIdx.x] = P.pcw[(long long)rep * 2 * (P.nx + 1) + threadIdx.x];
     if (threadIdx.x == 0) {
       const HParams& H = K.hp[rep];
       float a, b;
@@ -968,19 +974,30 @@ __global__ void __launch_bounds__(256) adam_kernel(StepConst K, AdamArgs P) {
       const float4 z4 = make_float4(0.f, 0.f, 0.f, 0.f);
       const float4* __restrict__ gx4 = reinterpret_cast<const float4*>(P.gx + rep * P.rsM);
       const long long xs4 = P.xs >> 2;               // (slice stride: a multiple of 4 floats like every arena)
-      const float4 ge0 = P.nx > 0 ? gx4[i] : z4, ge1 = P.nx > 1 ? gx4[xs4 + i] : z4, ge2 = P.nx > 2 ? gx4[2 * xs4 + i] : z4;
       float4 tv = z4;
-      if (t4) tv = t4[i];
-      if (P.nx > 0) { gv.x += ge0.x; gv.y += ge0.y; gv.z += ge0.z; gv.w += ge0.w; }
-      if (P.nx > 1) { gv.x += ge1.x; gv.y += ge1.y; gv.z += ge1.z; gv.w += ge1.w; }
-      if (P.nx > 2) { gv.x += ge2.x; gv.y += ge2.y; gv.z += ge2.z; gv.w += ge2.w; }
-      for (int sx = 3; sx < P.nx; ++sx) {
-        const float4 ge = gx4[(long long)sx * xs4 + i];
-        gv.x += ge.x; gv.y += ge.y; gv.z += ge.z; gv.w += ge.w;
-      }
-      if constexpr (CLIP) {
-        const float c = s_coef;
-        gv.x = gv.x * c; gv.y = gv.y * c; gv.z = gv.z * c; gv.w = gv.w * c;
+      if constexpr (PCG) {         // task slices: w_0 g_0 + w_1 g_1 + ..., each product rounded, added in index order
+        if (t4) tv = t4[i];
+        const float w0 = red[0];
+        gv.x = w0 * gv.x; gv.y = w0 * gv.y; gv.z = w0 * gv.z; gv.w = w0 * gv.w;
+        for (int sx = 0; sx < P.nx; ++sx) {
+          const float4 ge = gx4[(long long)sx * xs4 + i];
+          const float wk = red[sx + 1];
+          gv.x = gv.x + wk * ge.x; gv.y = gv.y + wk * ge.y; gv.z = gv.z + wk * ge.z; gv.w = gv.w + wk * ge.w;
+        }
+      } else {
+        const float4 ge0 = P.nx > 0 ? gx4[i] : z4, ge1 = P.nx > 1 ? gx4[xs4 + i] : z4, ge2 = P.nx > 2 ? gx4[2 * xs4 + i] : z4;
+        if (t4) tv = t4[i];
+        if (P.nx > 0) { gv.x += ge0.x; gv.y += ge0.y; gv.z += ge0.z; gv.w += ge0.w; }
+        if (P.nx > 1) { gv.x += ge1.x; gv.y += ge1.y; gv.z += ge1.z; gv.w += ge1.w; }
+        if (P.nx > 2) { gv.x += ge2.x; gv.y += ge2.y; gv.z += ge2.z; gv.w += ge2.w; }
+        for (int sx = 3; sx < P.nx; ++sx) {
+          const float4 ge = gx4[(long long)sx * xs4 + i];
+          gv.x += ge.x; gv.y += ge.y; gv.z += ge.z; gv.w += ge.w;
+        }
+        if constexpr (CLIP) {
+          const float c = s_coef;
+          gv.x = gv.x * c; gv.y = gv.y * c; gv.z = gv.z * c; gv.w = gv.w * c;
+        }
       }
       adam_one(pv.x, mv.x, vv.x, gv.x, w1, b2, omb2, step_size, bc2_sqrt, eps);
       adam_one(pv.y, mv.y, vv.y, gv.y, w1, b2, omb2, step_size, bc2_sqrt, eps);

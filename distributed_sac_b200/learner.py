@@ -80,11 +80,12 @@ class _BaseLearner:
     family = "LL"
     log_name = "LunarLander_Distributed_SAC"
     _iteration_key = "episode_idx"
+    _pcgrad_ok = False          # PCGrad needs task-block minibatches and an MTSAC network (no CARE encoder)
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
-                     n_step=1, max_grad_norm=None):
+                     n_step=1, max_grad_norm=None, pcgrad=False):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -94,6 +95,7 @@ class _BaseLearner:
             raise ValueError("n-step returns need replay_where='device' (the trajectory links live beside the device ring)")
         self.n_step = int(n_step)
         self.max_grad_norm = max_grad_norm
+        self.pcgrad = bool(pcgrad)
         self.cfg = cfg_read(cfg_path)
         self.precision = precision
         self.write_mode = write_mode
@@ -102,6 +104,9 @@ class _BaseLearner:
         self.episode_idx = 0
         self.datetime = str(datetime.now())[:-7]
         self._set_dims()
+        if self.pcgrad and not (self._pcgrad_ok and self.num_tasks >= 2):
+            raise ValueError(f"pcgrad=True needs a multi-task MTSAC learner with num_tasks >= 2 ({type(self).__name__}, "
+                             f"num_tasks {self.num_tasks})")
         self.device = torch.device(self.cfg.get("device", "cuda"))
         if self.device.type != "cuda":
             raise RuntimeError("the CUDA learner only runs on CUDA devices (cfg 'device' must be 'cuda')")
@@ -140,6 +145,14 @@ class _BaseLearner:
         self.max_grad_norm = float(max_norm)
         self.core.set_grad_clip(critic=max_norm, actor=max_norm, ctx=max_norm)
 
+    def set_pcgrad(self, critic=True, actor=True):
+        """Turn PCGrad gradient surgery of the critic / actor optimizer on or off, effective from the next update().  Off,
+        Adam reads the plain sum of the per-task gradients.  The learner must have been built with pcgrad=True;
+        core.read_pcgrad() returns the last update's Gram matrix, weights and projections."""
+        if not self.pcgrad:
+            raise ValueError("this learner was built without pcgrad=True")
+        self.core.set_pcgrad(critic=critic, actor=actor)
+
     def set_n_step(self, n: int):
         """Horizon of the n-step return, effective from the next update()."""
         if self.n_step == 1:
@@ -154,7 +167,7 @@ class _BaseLearner:
                           reward_scale=float(self.reward_scale), lr_actor=float(self.lr_actor),
                           lr_critic=float(self.lr_critic),
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
-                          log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None)
+                          log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None, pcgrad=self.pcgrad)
 
     # ---- reference method surface -------------------------------------------------------------
     def update(self):
@@ -434,11 +447,12 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
-                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None):
+                 precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
+                 pcgrad=False):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
 
     def _set_dims(self):
         c = self.cfg
@@ -462,9 +476,9 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1, n_step=1, max_grad_norm=None):
+                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
 
     def _set_dims(self):
         c = self.cfg
@@ -487,13 +501,14 @@ class MTSACLearner(_BaseLearner):
     family = "MS"
     log_name = "MT10_Distributed_MTSAC"
     _iteration_key = "update_iteration"
+    _pcgrad_ok = True
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
-                 actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None):
+                 actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
 
     def _set_dims(self):
         c = self.cfg
@@ -540,6 +555,7 @@ class CARELearner(MTSACLearner):
     critic's after every update (learner.py:402), so it is exported from the same tensors."""
     family = "C10"
     log_name = "MT10_Distributed_CARE"
+    _pcgrad_ok = False          # the critic optimizer also owns the state encoder, whose gradients are not task slices
 
     def _set_dims(self):
         super()._set_dims()

@@ -28,6 +28,9 @@
  *   b200sac_set/get_grad_clip, b200sac_read_grad_norms
  *                            torch.nn.utils.clip_grad_norm_ before each optimizer.step() (Ape-X's max-norm 40, the
  *                            max_grad_norm of SAC / TD3 code bases) and the norms it returns, per replica and optimizer
+ *   b200sac_set/get/read_pcgrad, b200sac_export_task_grad
+ *                            PCGrad gradient surgery (Yu et al., NeurIPS 2020) for the multi-task learners' optimizers,
+ *                            per replica and optimizer, with the step's Gram matrix and surgery decisions reported
  *   b200sac_blob_*           Learner.get_parameters() and server.set('parameters', _pickle.dumps(get_parameters())) in
  *                            Learner.run(), learner.py:272-276,298-299 (MT10_Distributed_CARE/src/learner.py:412-417,442-443):
  *                            the byte string, device-assembled
@@ -100,6 +103,9 @@ typedef struct b200sac_cfg {
   double lr_ctx;                     /* lr_contextEnc (CARE(O) context-encoder Adam) */
   int32_t grad_clip;                 /* 0 = the default plan; 1 = the plan with gradient-norm clipping and gradient norms
                                         (b200sac_set_grad_clip), every threshold +inf at create.  Fixed at create. */
+  int32_t pcgrad;                    /* 0 = the default plan; 1 = the per-layer plan with PCGrad gradient surgery
+                                        (b200sac_set_pcgrad), both switches on at create.  Needs num_tasks >= 2, care = 0
+                                        and grad_clip = 0.  Fixed at create. */
 } b200sac_cfg;
 
 typedef struct b200sac_tensor_desc {
@@ -211,6 +217,44 @@ int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double*
  * critic-only step, the context encoder outside CARE(O)).  Synchronises the stream. */
 int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void* stream);
 
+/* PCGrad gradient surgery, per replica and optimizer (handles created with cfg.pcgrad = 1; others: B200SAC_ERR_STATE).
+ * T = num_tasks, P = batch / T; row i of a step's minibatch belongs to task t(i) = i / P.  On a pcgrad handle
+ * b200sac_step_sampled, b200sac_update and b200sac_replay_sample draw P rows per task in this order, on the device and the
+ * pinned-host ring alike (the pinned-host ring skips its shuffle of the rows; the losses are row sums, so the order does
+ * not change what a step computes).  For each optimizer o (the critic: q1 and q2 together,
+ * counter slot 0; the actor: slot 1), with l_i = row i's term of o's loss exactly as the step defines it (the 1/B mean,
+ * weighted_loss's extra 1/B, importance weights and the per-task temperature included):
+ *   g_t  = the gradient of L_{o,t} = sum over the rows i of task t of l_i, so sum_t g_t is the ordinary step gradient.  The
+ *          published implementations use per-task means, T times this: the projections do not depend on the scale, Adam
+ *          only through its eps;
+ *   G_jk = sum_e g_j[e] g_k[e] over the optimizer's slice, in fp64 in a fixed order (bit-reproducible, independent of the
+ *          replica count, no floating-point atomics);
+ *   for every task i: a permutation pi_i of all T tasks (i included), Fisher-Yates from Philox keyed by (handle seed,
+ *          replica, step index, optimizer, i); c = 0 (fp64); for each j in pi_i: dot = G_ij - sum_k c_k G_kj (k ascending),
+ *          and if dot < 0, c_j += dot / G_jj.  This is "if g_i^PC . g_j < 0: g_i^PC -= (g_i^PC . g_j) / |g_j|^2 g_j" with
+ *          g_i^PC = g_i - sum_k c_k g_k; a zero or NaN g_j never projects (dot is 0 or NaN);
+ *   w_k  = (float)(1 - sum_i c^(i)_k), the sum in fp64 over i ascending;
+ *   Adam runs on w_0 g_0 + w_1 g_1 + ... + w_{T-1} g_{T-1}: each product rounded to fp32, added in index order, no FMA.
+ *          The Adam math and the Polyak update fused after it are unchanged.
+ * The temperature keeps its own per-task Adam and takes no part.  A critic-only step leaves the actor untouched and records
+ * NaN actor weights.  b200sac_export(GRADS) still returns the slices summed in index order: the unprojected gradient.
+ * Set: enqueued on `stream` like b200sac_set_hparams (applies to the steps enqueued after it, including launches of graphs
+ * already instantiated).  Each switch is 0 or 1, both 1 at create; off means w = 1 (Adam reads the plain slice sum) while
+ * G is still computed and reported.  The switches are not copied by b200sac_copy_replica and not part of a checkpoint.
+ * Get: the values last set (host mirror: does not synchronise). */
+int b200sac_set_pcgrad(b200sac_t* h, int32_t replica, int32_t critic_on, int32_t actor_on, void* stream);
+int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_t* actor_on);
+/* The last step's record of one replica, for both optimizers (index 0 critic, 1 actor); any output may be NULL:
+ * gram [2][T][T] (fp64), w [2][T], perm [2][T][T] (row i = pi_i), mask [2][T] (bit j of mask[o][i] set iff task i was
+ * projected onto task j), task_mismatch = the rows of the step whose one-hot task (its first maximum) was not t(i).
+ * Before the first step: gram NaN, w 1, perm and mask 0, task_mismatch 0.  After a critic-only step the actor's entries
+ * hold gram NaN, w NaN and mask 0, and its perm keeps the permutations of the last actor step.  Synchronises the stream. */
+int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, int32_t* perm, uint64_t* mask,
+                        int32_t* task_mismatch, void* stream);
+/* Gradient slice of task `task` (rows t(i) = task) of one replica, the whole trainable arena (n_floats = trainable floats)
+ * into host or device memory.  Synchronises the stream. */
+int b200sac_export_task_grad(b200sac_t* h, int32_t replica, int32_t task, float* buf, int64_t n_floats, void* stream);
+
 /* One gradient step from caller-provided DEVICE minibatches, each
  * [replicas][batch][width] fp32: s,s2 width obs(=state_dim+num_tasks), a width act, r,d width 1.
  * eps_next / eps_cur: [replicas][batch][act] standard-normal noise for the two
@@ -218,6 +262,8 @@ int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void*
  * Losses land in an internal device ring; fetch with b200sac_read_losses.
  * Every step entry point (b200sac_step, _step_host, _step_sampled, _update) follows each replica's update intervals
  * (b200sac_set_update_intervals): a critic-only step updates the critics only. */
+/* pcgrad handles: row i of every replica's minibatch must belong to task i / (batch / num_tasks); b200sac_read_pcgrad
+ * reports how many rows of the last step did not. */
 int b200sac_step(b200sac_t* h, const float* s, const float* a, const float* r, const float* s2,
                  const float* d, const float* eps_next, const float* eps_cur, void* stream);
 
@@ -225,6 +271,8 @@ int b200sac_step(b200sac_t* h, const float* s, const float* a, const float* r, c
  * double buffer with cudaMemcpyAsync on a side stream).  out_losses (host,
  * [replicas][4] = critic, actor, alpha-loss, entropy) may be NULL; if given the call
  * synchronises and fills it -- this is the reference's `update()` contract. */
+/* pcgrad handles: a minibatch with a row i whose one-hot task is not i / (batch / num_tasks) gives B200SAC_ERR_INVALID and
+ * enqueues nothing. */
 int b200sac_step_host(b200sac_t* h, const float* s, const float* a, const float* r, const float* s2,
                       const float* d, const float* eps_next, const float* eps_cur, float* out_losses,
                       void* stream);

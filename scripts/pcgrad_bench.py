@@ -1,0 +1,117 @@
+"""PCGrad gradient surgery: cost of the pcgrad plan against the default plan, and the in-graph times of its new launches.
+
+  python scripts/pcgrad_bench.py [--steps 1000] [--warmup 100] [--out FILE]
+
+Workload: the MT10 MTSAC shape (39 + 10 one-hot inputs, 4 actions, 400-wide 3-layer networks, batch 1280, 10 tasks,
+precision 1, per-layer plan) on a 128 Ki-transition device ring, for 1 learner and for 10 learners in one handle.  Each leg
+alternates three handles three times and reports the median: no pcgrad, pcgrad with both switches off (the Gram matrix
+only), and pcgrad on.  The card's name, power limit and SM clock are read in the same run (nvidia-smi, read-only query).
+"""
+import argparse
+import json
+import os
+import statistics
+import subprocess
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+MODES = ("default", "switch_off", "on")
+
+
+def card():
+    try:
+        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
+                           capture_output=True, text=True, timeout=30).stdout.strip().splitlines()[0]
+        name, power, clock = [x.strip() for x in q.split(",")]
+        return {"name": name, "power_limit": power, "max_sm_clock": clock}
+    except Exception as e:                     # noqa: BLE001 -- reported, not fatal
+        return {"error": repr(e)}
+
+
+def config(R, pcgrad):
+    from distributed_sac_b200.core import CoreConfig
+    return CoreConfig(state_dim=39, act_dim=4, actor_hidden=[400] * 3, critic_hidden=[400] * 3, batch=1280, num_tasks=10,
+                      weighted_loss=True, replicas=R, precision=1, pcgrad=pcgrad)
+
+
+def leg(R, ring_n, steps, warmup, mode, timeline):
+    import torch
+    from distributed_sac_b200.core import Replay, SacCore
+    core = SacCore(config(R, mode != "default"), 0, seed=11)
+    ring = Replay(core, ring_n, seed=3)
+    ring.fill_synthetic(ring_n, seed=5)
+    stream = torch.cuda.Stream()
+    with torch.cuda.stream(stream):
+        if mode == "switch_off":
+            core.set_pcgrad(critic=False, actor=False)
+        core.prepare(ring)
+        core.step_sampled(ring, warmup)
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        core.step_sampled(ring, steps)
+        e1.record()
+    e1.synchronize()
+    us = 1e3 * e0.elapsed_time(e1) / steps
+    assert torch.isfinite(core.read_losses(64)[:, :, 0]).all()
+    extra = {}
+    if mode != "default":
+        rec = core.read_pcgrad(0)
+        extra = {"critic_projections": int(rec["projected"][0].sum()), "actor_projections": int(rec["projected"][1].sum())}
+    tl = None
+    if timeline:
+        with torch.cuda.stream(stream):
+            names = ["sample", "ingest"] + [n for n, _ in core.profile_step(ring, iters=2)][1:]
+            t = core.graph_timeline(ring, iters=200)
+        torch.cuda.synchronize()
+        tl = {"new_launches_us": {f"{i}:{n}": t[i] for i, n in enumerate(names)
+                                  if n.startswith("pcgrad") or n in ("adam_critic+polyak", "adam_actor+alpha")},
+              "step_us": sum(t), "all_us": dict(zip(names, t))}
+    ring.close()
+    core.close()
+    return us, tl, extra
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=1000)
+    ap.add_argument("--warmup", type=int, default=100)
+    ap.add_argument("--out", default=None)
+    args = ap.parse_args()
+    import __graft_entry__ as ge
+    ge.build()
+    import torch
+    if not torch.cuda.is_available():
+        raise SystemExit("pcgrad_bench.py needs a CUDA device")
+    res = {"card": card(), "steps": args.steps, "warmup": args.warmup, "legs": {}}
+    for name, R, ring_n in (("MS_x1", 1, 1 << 17), ("MS_x10", 10, 1 << 17)):
+        us = {m: [] for m in MODES}
+        tls, extras = {}, {}
+        for k in range(3):
+            for m in MODES:
+                t, tl, ex = leg(R, ring_n, args.steps, args.warmup, m, timeline=(k == 0 and R == 1))
+                us[m].append(t)
+                extras[m] = ex
+                if tl is not None:
+                    tls[m] = tl
+        med = {m: statistics.median(v) for m, v in us.items()}
+        out = {"learners": R, "ring_per_learner": ring_n, "us_per_step": med,
+               "switch_off_over_default": med["switch_off"] / med["default"], "on_over_default": med["on"] / med["default"],
+               "last_step_projections": extras, "runs_us": us}
+        if tls:                        # start-to-start times of the unforked timeline run (b200sac_graph_timeline)
+            out["graph_timeline"] = tls
+        res["legs"][name] = out
+        print(json.dumps({name: {k: v for k, v in out.items() if k not in ("runs_us", "graph_timeline")}}), flush=True)
+    line = json.dumps(res)
+    print(line)
+    if args.out:
+        with open(args.out, "w") as f:
+            f.write(line + "\n")
+
+
+if __name__ == "__main__":
+    t0 = time.time()
+    main()
+    print(f"[pcgrad_bench] {time.time() - t0:.0f} s", file=sys.stderr)
