@@ -115,6 +115,11 @@ def _stream():
     return C.c_void_p(torch.cuda.current_stream().cuda_stream)
 
 
+def _replicas(n, replica):
+    """The replicas a per-replica setter writes: `replica`, or all n of them when it is None."""
+    return range(n) if replica is None else [int(replica)]
+
+
 class SacCore:
     def __init__(self, cfg: CoreConfig, device: int = 0, seed: int = 0):
         self.lib = _lib.load()
@@ -305,7 +310,7 @@ class SacCore:
         unknown = set(values) - set(self.HPARAMS)
         if unknown:
             raise TypeError(f"unknown hyperparameters {sorted(unknown)}; known: {self.HPARAMS}")
-        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.cfg.replicas, replica):
             cur = self.get_hparams(r)
             cur.update({k: float(v) for k, v in values.items()})
             hp = _lib.Hparams(**cur)
@@ -322,7 +327,7 @@ class SacCore:
         """Update the actor (and temperature) only on steps whose critic step count n is a multiple of actor_every, and the
         targets only when n is a multiple of target_every, for one replica (replica=None: all of them) on the current
         stream; an interval not named keeps its value.  Steps enqueued afterwards follow the new schedule."""
-        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.cfg.replicas, replica):
             a, t = self.get_update_intervals(r)
             a = a if actor_every is None else int(actor_every)
             t = t if target_every is None else int(target_every)
@@ -341,7 +346,7 @@ class SacCore:
         """clip_grad_norm_ thresholds of the critic, actor and CARE(O) context-encoder optimizers of one replica
         (replica=None: all of them) on the current stream; a name left out keeps its value, inf turns clipping off.
         Steps enqueued afterwards use them."""
-        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.cfg.replicas, replica):
             cur = self.get_grad_clip(r)
             for k, v in dict(critic=critic, actor=actor, ctx=ctx).items():
                 if v is not None:
@@ -366,7 +371,7 @@ class SacCore:
         """Turn the critic's / actor's gradient surgery on or off for one replica (replica=None: all of them) on the current
         stream; a switch left out keeps its value.  Off: Adam reads the plain sum of the task gradients, and the Gram matrix
         is still computed.  Steps enqueued afterwards use the new switches."""
-        for r in range(self.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.cfg.replicas, replica):
             cur = self.get_pcgrad(r)
             for k, v in dict(critic=critic, actor=actor).items():
                 if v is not None:
@@ -585,7 +590,7 @@ class Replay:
     # ---- prioritized replay -----------------------------------------------------------------
     def set_beta(self, beta: float, replica=None):
         """Importance-sampling exponent of one replica (None: all), in stream order: steps enqueued afterwards use it."""
-        for r in range(self.core.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.core.cfg.replicas, replica):
             _lib.check(self.lib.b200sac_replay_set_beta(self._h, r, float(beta), _stream()))
 
     def set_priorities(self, idx, prio, replica=0):
@@ -629,7 +634,7 @@ class Replay:
     # ---- n-step returns (ring with trajectory links) ---------------------------------------------
     def set_nstep(self, n: int, replica=None):
         """Horizon n in [1, 16] of one replica (None: all), in stream order: steps enqueued afterwards fold n-step returns."""
-        for r in range(self.core.cfg.replicas) if replica is None else [int(replica)]:
+        for r in _replicas(self.core.cfg.replicas, replica):
             _lib.check(self.lib.b200sac_replay_set_nstep(self._h, r, int(n), _stream()))
 
     def get_nstep(self, replica=0) -> int:

@@ -332,6 +332,31 @@ static EnvSwitches env_switches() {
   return s;
 }
 
+// A per-replica setting that may change between steps: a device table [R][N] of T that the step kernels read through a
+// pointer captured in the graphs, and its host mirror [R][N] of the values as given (Mirror: the hyperparameters keep the
+// caller's b200sac_hparams, the device gets hparams_row).  set() writes one row with a one-thread kernel in stream order
+// (bridged off the legacy default stream like a step), so graphs already instantiated read the new value at their next
+// launch, and updates the mirror once the write is enqueued, so a getter does not synchronise.
+template <class T, int N> struct TableRow { T v[N]; };
+template <class T, int N> __global__ void write_row_kernel(T* t, int r, TableRow<T, N> row) {
+  for (int i = 0; i < N; ++i) t[r * N + i] = row.v[i];
+}
+
+template <class T, int N = 1, class Mirror = T>
+struct ReplicaTable {
+  DevMem<T> dev;
+  std::vector<Mirror> host;
+  // every replica's row <- v[0, N); all or nothing (a failed call leaves the table as it was)
+  int init(int R, const Mirror* v);
+  int check(int replica) const {
+    if (replica < 0 || (size_t)replica >= host.size() / N) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+    return 0;
+  }
+  const Mirror* row(int replica) const { return host.data() + (size_t)replica * N; }
+  // row `replica` <- v[0, N) behind the work on `stream`; `written` (if given) is recorded right after the write
+  int set(b200sac* h, void* stream, int replica, const Mirror* v, cudaEvent_t written = nullptr);
+};
+
 struct b200sac {
   b200sac_cfg cfg;
   EnvSwitches env;                // read at create
@@ -342,10 +367,8 @@ struct b200sac {
   // arenas
   DevMem<float> params, adam_m, adam_v, grads;
   DevMem<Counters> cnt;
-  DevMem<HParams> hp;             // [R] per-replica hyperparameters (K.hp points here)
-  std::vector<b200sac_hparams> hp_host;   // host mirror of the values as given (b200sac_get_hparams does not synchronise)
-  DevMem<int> ivl;                // [R][2] update intervals (actor_every, target_every), read by the ingest
-  std::vector<int> ivl_host;      // host mirror (b200sac_get_update_intervals does not synchronise)
+  ReplicaTable<HParams, 1, b200sac_hparams> hp;   // [R] per-replica hyperparameters (K.hp points here)
+  ReplicaTable<int, 2> ivl;       // [R][2] update intervals (actor_every, target_every), read by the ingest
   DevMem<float> losses;           // [kLossSlots][R][4]
   long long host_steps = 0;       // steps enqueued so far
   // work slab
@@ -413,22 +436,20 @@ struct b200sac {
   // n-step returns (allocated with the first linked ring): [3][R][B] per-row discount of the step (K.disc), hops folded and
   // ring indices (int32), written by ingest_nstep_kernel
   DevMem<float> ns_buf;
-  // gradient-norm clipping (cfg.grad_clip): [R][3] thresholds (critic, actor, context encoder) and their host mirror, the
-  // step's clip coefficients, the mapped pinned norm ring [kLossSlots][R][3], and the norm launches' partial sums
+  // gradient-norm clipping (cfg.grad_clip): [R][3] thresholds (critic, actor, context encoder), the step's clip
+  // coefficients, the mapped pinned norm ring [kLossSlots][R][3], and the norm launches' partial sums
   // [3][R][kGradNormMaxBlocks] and tickets [3][R]
-  DevMem<double> clip_thr;
-  std::vector<double> clip_host;
+  ReplicaTable<double, kClipCols> clip_thr;
   DevMem<float> clip_coef;
   PinnedMem<float> gnorm_h;
   float* gnorm_h_dev = nullptr;
   DevMem<double> gn_part;
   DevMem<unsigned> gn_ticket;
-  // gradient surgery (cfg.pcgrad): [R][2] switches (critic, actor) and their host mirror, the pcgrad launches' partial
-  // products [2][R][kGradNormMaxBlocks][T(T+1)/2] and tickets [2][R], the last step's record per replica and optimizer
+  // gradient surgery (cfg.pcgrad): [R][2] switches (critic, actor), the pcgrad launches' partial products
+  // [2][R][kGradNormMaxBlocks][T(T+1)/2] and tickets [2][R], the last step's record per replica and optimizer
   // (G [R][2][T][T], w [R][2][T] -- also what Adam reads --, permutations [R][2][T][T], projection masks [R][2][T]) and
   // the rows of the last step whose task id was not i / P [R]
-  DevMem<int> pc_on;
-  std::vector<int> pc_on_host;
+  ReplicaTable<int, 2> pc_on;
   DevMem<double> pc_part;
   DevMem<unsigned> pc_ticket;
   DevMem<double> pc_G;
@@ -465,7 +486,7 @@ struct b200sac_replay {
   bool per = false;
   PerTree tr;                     // (tr.tree and tr.maxp point into tree and maxp)
   DevMem<float> tree, maxp;
-  DevMem<double> d_beta;          // [R]
+  ReplicaTable<double> beta;      // [R]
   std::vector<long long> draws;   // [R] b200sac_replay_sample_prioritized calls so far (its Philox counter)
   Stream st;                      // device ring: push (and prioritized set / get / sample) work, synchronised before those calls return
   DevMem<long long> s_lidx;       // scratch [kPerMaxB]
@@ -475,8 +496,7 @@ struct b200sac_replay {
   // trajectory links (nstep_kernels.cuh; b200sac_replay_enable_trajectories)
   bool traj = false;
   DevMem<int> d_link;             // [R][cap] sub-ring-local slot of the successor, or -1
-  DevMem<int> d_nstep;            // [R] horizon
-  std::vector<int> nstep_host;    // host mirror (b200sac_replay_get_nstep does not synchronise)
+  ReplicaTable<int> nstep;        // [R] horizon
   std::vector<int> link_h, pred_h;   // [R][cap] host mirror of link, and its inverse (sub-ring-local slot of the predecessor)
   std::vector<std::unordered_map<int, long long>> tail;      // [R] stream id -> ring index of the stream's open tail
   std::vector<std::unordered_map<long long, int>> tail_at;   // [R] its inverse
@@ -1176,7 +1196,7 @@ void PlanBuilder::grad_norm(int which) {
   P.which = which == 2 ? 4 : which;
   P.col = which;
   P.cnt = h->cnt;
-  P.thr = h->clip_thr; P.coef = h->clip_coef; P.norms = h->gnorm_h_dev;
+  P.thr = h->clip_thr.dev; P.coef = h->clip_coef; P.norms = h->gnorm_h_dev;
   P.part = h->gn_part + (size_t)which * R * kGradNormMaxBlocks;
   P.ticket = h->gn_ticket + (size_t)which * R;
   P.R = R;
@@ -1199,7 +1219,7 @@ void PlanBuilder::pcgrad(int which) {
   const int T = c.num_tasks;
   P.g = h->grads + beg; P.gx = h->grads_x + beg; P.xs = (long long)R * L.trainable; P.rsM = rsG; P.n = n;
   P.T = T; P.opt = which;
-  P.cnt = h->cnt; P.on = h->pc_on;
+  P.cnt = h->cnt; P.on = h->pc_on.dev;
   P.part = h->pc_part + (size_t)which * R * kGradNormMaxBlocks * pcgrad_pairs(T);
   P.ticket = h->pc_ticket + (size_t)which * R;
   P.G = h->pc_G; P.w = h->pc_w; P.perm = h->pc_perm; P.mask = h->pc_mask;
@@ -1836,7 +1856,7 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
 // Prioritized replay: the draw of one step (indices into rb->d_idx, importance weights into the handle's per_buf).
 static cudaError_t per_sample_on(b200sac* h, b200sac_replay* rb, cudaStream_t s) {
   return launch_k(per_sample_kernel, dim3(h->R), dim3(h->cfg.batch > 256 ? 512 : 256), 0, s, h->K, rb->tr, (const Counters*)h->cnt,
-                  0LL, 0, (const long long*)rb->d_fill, (const double*)rb->d_beta, rb->d_idx.get(), h->per_buf.get(), (long long)h->cfg.batch,
+                  0LL, 0, (const long long*)rb->d_fill, (const double*)rb->beta.dev, rb->d_idx.get(), h->per_buf.get(), (long long)h->cfg.batch,
                   rb->seed);
 }
 
@@ -2055,21 +2075,16 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     hp0.gamma = cfg->gamma; hp0.reward_scale = cfg->reward_scale; hp0.tau = cfg->tau;
     hp0.lr_critic = cfg->lr_critic; hp0.lr_actor = cfg->lr_actor; hp0.lr_alpha = cfg->lr_alpha;
     hp0.tau_se = cfg->tau_se; hp0.lr_ctx = cfg->lr_ctx;
-    h->hp_host.assign((size_t)R, hp0);
-    const std::vector<HParams> rows((size_t)R, hparams_row(hp0));
-    CU(cudaMalloc(h->hp.put(), sizeof(HParams) * R));
-    CU(cudaMemcpy(h->hp, rows.data(), sizeof(HParams) * R, cudaMemcpyHostToDevice));
-    K.hp = h->hp;
-    h->ivl_host.assign((size_t)2 * R, 1);          // every step updates the actor and the targets
-    CU(cudaMalloc(h->ivl.put(), sizeof(int) * 2 * R));
-    CU(cudaMemcpy(h->ivl, h->ivl_host.data(), sizeof(int) * 2 * R, cudaMemcpyHostToDevice));
+    if (int rc = h->hp.init(R, &hp0)) return rc;
+    K.hp = h->hp.dev;
+    const int every[2] = {1, 1};                   // every step updates the actor and the targets
+    if (int rc = h->ivl.init(R, every)) return rc;
     K.cnt = h->cnt;
   }
   if (cfg->grad_clip) {       // thresholds +inf (no clipping), coefficients 1, every norm NaN until a step writes it
     const size_t n = (size_t)kClipCols * R;
-    h->clip_host.assign(n, INFINITY);
-    CU(cudaMalloc(h->clip_thr.put(), sizeof(double) * n));
-    CU(cudaMemcpy(h->clip_thr, h->clip_host.data(), sizeof(double) * n, cudaMemcpyHostToDevice));
+    const double inf[kClipCols] = {INFINITY, INFINITY, INFINITY};
+    if (int rc = h->clip_thr.init(R, inf)) return rc;
     const std::vector<float> ones(n, 1.0f);
     CU(cudaMalloc(h->clip_coef.put(), sizeof(float) * n));
     CU(cudaMemcpy(h->clip_coef, ones.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
@@ -2083,9 +2098,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   if (cfg->pcgrad) {          // switches on, weights 1, record NaN until a step writes it
     const int T = cfg->num_tasks;
     const size_t n2 = (size_t)2 * R;
-    h->pc_on_host.assign(n2, 1);
-    CU(cudaMalloc(h->pc_on.put(), sizeof(int) * n2));
-    CU(cudaMemcpy(h->pc_on, h->pc_on_host.data(), sizeof(int) * n2, cudaMemcpyHostToDevice));
+    const int on[2] = {1, 1};
+    if (int rc = h->pc_on.init(R, on)) return rc;
     CU(cudaMalloc(h->pc_part.put(), sizeof(double) * n2 * kGradNormMaxBlocks * pcgrad_pairs(T)));
     CU(cudaMalloc(h->pc_ticket.put(), sizeof(unsigned) * n2));
     CU(cudaMemset(h->pc_ticket, 0, sizeof(unsigned) * n2));
@@ -2164,7 +2178,7 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
 
   IngestOut& O = h->ing;
   O.XA = h->XA.p; O.XQ = h->XQ.p; O.XT = h->XT.p; O.XP = h->XP.p; O.r = h->r.p; O.d = h->d.p; O.eps = h->eps.p;
-  O.tid = (int*)h->tid.p; O.cnt = h->cnt; O.ivl = h->ivl;
+  O.tid = (int*)h->tid.p; O.cnt = h->cnt; O.ivl = h->ivl.dev;
   O.rsXA = h->XA.rs; O.rsXQ = h->XQ.rs; O.rsR = h->r.rs; O.rsEps = h->eps.rs;
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
@@ -2343,20 +2357,53 @@ struct StreamBridge {
 };
 
 // ------------------------------------------------------------------------------------------
-// Per-replica hyperparameters.  The step reads them from a device table [R] (HParams), so replicas of one handle can
-// train with different values and a value can change between steps: the row is written by a one-thread kernel in stream
-// order, which the captured step graphs simply read at their next launch.
+// Per-replica settings (ReplicaTable): replicas of one handle can train with different values, and a value can change
+// between steps.  Each entry point checks its own arguments and leaves the write, its ordering and the mirror to the table.
 // ------------------------------------------------------------------------------------------
+template <class T, class Mirror> static T device_value(const Mirror& v) {
+  if constexpr (std::is_same_v<T, Mirror>) return v;
+  else return hparams_row(v);
+}
+
+template <class T, int N, class Mirror>
+int ReplicaTable<T, N, Mirror>::init(int R, const Mirror* v) {
+  ReplicaTable t;
+  std::vector<T> rows((size_t)R * N);
+  for (size_t i = 0; i < rows.size(); ++i) {
+    t.host.push_back(v[i % N]);
+    rows[i] = device_value<T>(v[i % N]);
+  }
+  CU(cudaMalloc(t.dev.put(), sizeof(T) * rows.size()));
+  CU(cudaMemcpy(t.dev, rows.data(), sizeof(T) * rows.size(), cudaMemcpyHostToDevice));
+  *this = std::move(t);
+  return 0;
+}
+
+template <class T, int N, class Mirror>
+int ReplicaTable<T, N, Mirror>::set(b200sac* h, void* stream, int replica, const Mirror* v, cudaEvent_t written) {
+  TableRow<T, N> row;
+  for (int i = 0; i < N; ++i) row.v[i] = device_value<T>(v[i]);
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  write_row_kernel<<<1, 1, 0, sb.run>>>(dev.get(), replica, row);
+  CU(cudaGetLastError());
+  if (written) CU(cudaEventRecord(written, sb.run));
+  if (int rc = sb.end()) return rc;
+  std::copy(v, v + N, host.begin() + (size_t)replica * N);
+  return 0;
+}
+
 extern "C" int b200sac_get_hparams(b200sac_t* h, int32_t replica, b200sac_hparams* out) {
   if (!h || !out) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  *out = h->hp_host[(size_t)replica];
+  if (int rc = h->hp.check(replica)) return rc;
+  *out = *h->hp.row(replica);
   return 0;
 }
 
 extern "C" int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp, void* stream) {
   if (!h || !hp) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = h->hp.check(replica)) return rc;
   const double all[8] = {hp->gamma, hp->reward_scale, hp->tau, hp->lr_critic, hp->lr_actor, hp->lr_alpha, hp->tau_se, hp->lr_ctx};
   for (double x : all)
     if (!std::isfinite(x)) return fail(B200SAC_ERR_INVALID, "hyperparameters must be finite");
@@ -2364,55 +2411,35 @@ extern "C" int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_
     return fail(B200SAC_ERR_INVALID, "0 <= tau, tau_se <= 1 required (got %g, %g)", hp->tau, hp->tau_se);
   if (hp->lr_critic < 0.0 || hp->lr_actor < 0.0 || hp->lr_alpha < 0.0 || hp->lr_ctx < 0.0)
     return fail(B200SAC_ERR_INVALID, "learning rates must be >= 0");
-  CU(cudaSetDevice(h->device));
-  StreamBridge sb(h, stream);
-  if (int rc = sb.begin()) return rc;
-  set_hparams_kernel<<<1, 1, 0, sb.run>>>(h->hp, replica, hparams_row(*hp));
-  CU(cudaGetLastError());
-  if (int rc = sb.end()) return rc;
-  h->hp_host[(size_t)replica] = *hp;
-  return 0;
+  return h->hp.set(h, stream, replica, hp);
 }
 
 // Per-replica update intervals: the ingest of each step turns them and the critic's step count into the step's schedule
-// (Counters::sched), so a change is ordered with the steps like set_hparams and reaches already instantiated graphs.
-__global__ void set_intervals_kernel(int* ivl, int replica, int actor_every, int target_every) {
-  ivl[2 * replica] = actor_every;
-  ivl[2 * replica + 1] = target_every;
-}
-
+// (Counters::sched).
 extern "C" int b200sac_get_update_intervals(b200sac_t* h, int32_t replica, int32_t* actor_every, int32_t* target_every) {
   if (!h || !actor_every || !target_every) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  *actor_every = h->ivl_host[2 * (size_t)replica];
-  *target_every = h->ivl_host[2 * (size_t)replica + 1];
+  if (int rc = h->ivl.check(replica)) return rc;
+  *actor_every = h->ivl.row(replica)[0];
+  *target_every = h->ivl.row(replica)[1];
   return 0;
 }
 
 extern "C" int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32_t actor_every, int32_t target_every, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = h->ivl.check(replica)) return rc;
   constexpr int32_t kMaxEvery = 1 << 30;
   if (actor_every < 1 || actor_every > kMaxEvery || target_every < 1 || target_every > kMaxEvery)
     return fail(B200SAC_ERR_INVALID, "update intervals must be in [1, 2^30] (got actor %d, target %d)", actor_every, target_every);
-  CU(cudaSetDevice(h->device));
-  StreamBridge sb(h, stream);
-  if (int rc = sb.begin()) return rc;
-  set_intervals_kernel<<<1, 1, 0, sb.run>>>(h->ivl, replica, actor_every, target_every);
-  CU(cudaGetLastError());
-  if (int rc = sb.end()) return rc;
-  h->ivl_host[2 * (size_t)replica] = actor_every;
-  h->ivl_host[2 * (size_t)replica + 1] = target_every;
-  return 0;
+  const int v[2] = {actor_every, target_every};
+  return h->ivl.set(h, stream, replica, v);
 }
 
-// Gradient-norm clipping thresholds: a device row [R][3] written in stream order like the hyperparameters, read by the
-// grad_norm launches of the step graphs.
+// Gradient-norm clipping thresholds, read by the grad_norm launches of the step graphs.
 extern "C" int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double* actor, double* ctx) {
   if (!h || !critic || !actor || !ctx) return fail(B200SAC_ERR_INVALID, "null argument");
   if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  const double* t = h->clip_host.data() + (size_t)replica * kClipCols;
+  if (int rc = h->clip_thr.check(replica)) return rc;
+  const double* t = h->clip_thr.row(replica);
   *critic = t[0]; *actor = t[1]; *ctx = t[2];
   return 0;
 }
@@ -2420,44 +2447,30 @@ extern "C" int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* crit
 extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double critic, double actor, double ctx, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = h->clip_thr.check(replica)) return rc;
   if (!(critic > 0.0) || !(actor > 0.0) || !(ctx > 0.0))       // (NaN fails every comparison)
     return fail(B200SAC_ERR_INVALID, "gradient-norm thresholds must be > 0 (+inf: no clipping), got %g, %g, %g", critic, actor, ctx);
-  CU(cudaSetDevice(h->device));
-  StreamBridge sb(h, stream);
-  if (int rc = sb.begin()) return rc;
-  set_grad_clip_kernel<<<1, 1, 0, sb.run>>>(h->clip_thr, replica, critic, actor, ctx);
-  CU(cudaGetLastError());
-  if (int rc = sb.end()) return rc;
-  double* t = h->clip_host.data() + (size_t)replica * kClipCols;
-  t[0] = critic; t[1] = actor; t[2] = ctx;
-  return 0;
+  const double v[kClipCols] = {critic, actor, ctx};
+  return h->clip_thr.set(h, stream, replica, v);
 }
 
-// Gradient-surgery switches: a device row [R][2] written in stream order like the hyperparameters, read by the pcgrad
-// launches of the step graphs.
+// Gradient-surgery switches, read by the pcgrad launches of the step graphs.
 extern "C" int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_t* actor_on) {
   if (!h || !critic_on || !actor_on) return fail(B200SAC_ERR_INVALID, "null argument");
   if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  *critic_on = h->pc_on_host[(size_t)replica * 2]; *actor_on = h->pc_on_host[(size_t)replica * 2 + 1];
+  if (int rc = h->pc_on.check(replica)) return rc;
+  *critic_on = h->pc_on.row(replica)[0]; *actor_on = h->pc_on.row(replica)[1];
   return 0;
 }
 
 extern "C" int b200sac_set_pcgrad(b200sac_t* h, int32_t replica, int32_t critic_on, int32_t actor_on, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = h->pc_on.check(replica)) return rc;
   if ((critic_on != 0 && critic_on != 1) || (actor_on != 0 && actor_on != 1))
     return fail(B200SAC_ERR_INVALID, "pcgrad switches must be 0 or 1, got %d, %d", critic_on, actor_on);
-  CU(cudaSetDevice(h->device));
-  StreamBridge sb(h, stream);
-  if (int rc = sb.begin()) return rc;
-  set_pcgrad_kernel<<<1, 1, 0, sb.run>>>(h->pc_on, replica, critic_on, actor_on);
-  CU(cudaGetLastError());
-  if (int rc = sb.end()) return rc;
-  h->pc_on_host[(size_t)replica * 2] = critic_on; h->pc_on_host[(size_t)replica * 2 + 1] = actor_on;
-  return 0;
+  const int v[2] = {critic_on, actor_on};
+  return h->pc_on.set(h, stream, replica, v);
 }
 
 extern "C" int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, int32_t* perm, uint64_t* mask,
@@ -2619,7 +2632,7 @@ extern "C" int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t
 enum { SAMPLE_INLINE = 0, SAMPLE_DONE = 1 };
 static NstepRing nstep_ring(const b200sac_replay* rb) {
   NstepRing N;
-  N.link = rb->d_link; N.nstep = rb->d_nstep; N.cap = rb->cap; N.cap_per_task = (int)rb->cap_per_task;
+  N.link = rb->d_link; N.nstep = rb->nstep.dev; N.cap = rb->cap; N.cap_per_task = (int)rb->cap_per_task;
   return N;
 }
 
@@ -3122,7 +3135,7 @@ extern "C" int b200sac_soft_update(b200sac_t* h, double tau, void* stream) {
   const bool hard = (tau == 1.0);
   polyak_kernel<<<dim3(128, h->R), 256, 0, (cudaStream_t)stream>>>(
       h->params + h->L.critic_begin, h->L.arena, h->L.critic_n, h->L.target_delta, (float)tau, (float)(1.0 - tau),
-      (h->cfg.care && !hard) ? (long long)(h->L.cse_begin - h->L.critic_begin) : -1LL, h->hp);
+      (h->cfg.care && !hard) ? (long long)(h->L.cse_begin - h->L.critic_begin) : -1LL, h->hp.dev);
   CU(cudaGetLastError());
   return 0;
 }
@@ -3666,13 +3679,11 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
   rb->draws.assign((size_t)h->R, 0);
   const size_t nt = (size_t)h->R * tr.T;
   const std::vector<float> maxp0(nt, 1.f);
-  const std::vector<double> beta0((size_t)h->R, beta);
   CU(cudaMalloc(rb->tree.put(), nt * 2 * (size_t)tr.P * sizeof(float)));
   CU(cudaMemset(rb->tree, 0, nt * 2 * (size_t)tr.P * sizeof(float)));
   CU(cudaMalloc(rb->maxp.put(), nt * sizeof(float)));
   CU(cudaMemcpy(rb->maxp, maxp0.data(), nt * sizeof(float), cudaMemcpyHostToDevice));
-  CU(cudaMalloc(rb->d_beta.put(), beta0.size() * sizeof(double)));
-  CU(cudaMemcpy(rb->d_beta, beta0.data(), beta0.size() * sizeof(double), cudaMemcpyHostToDevice));
+  if (int rc = rb->beta.init(h->R, &beta)) return rc;
   CU(cudaMalloc(rb->s_lidx.put(), kPerMaxB * sizeof(long long)));
   CU(cudaMalloc(rb->s_idx.put(), kPerMaxB * sizeof(int)));
   CU(cudaMalloc(rb->s_f.put(), kPerMaxB * sizeof(float)));
@@ -3698,10 +3709,7 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
 extern "C" int b200sac_replay_set_beta(b200sac_replay_t* rb, int32_t replica, double beta, void* stream) {
   if (int rc = ring_check(rb, replica, RING_PER)) return rc;
   if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "beta must be in [0, 1] (got %g)", beta);
-  CU(cudaSetDevice(rb->h->device));
-  per_set_beta_kernel<<<1, 1, 0, (cudaStream_t)stream>>>(rb->d_beta, replica, beta);
-  CU(cudaGetLastError());
-  return 0;
+  return rb->beta.set(rb->h, stream, replica, &beta);
 }
 
 extern "C" int b200sac_replay_set_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, const float* prio) {
@@ -3773,7 +3781,7 @@ extern "C" int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t r
   if (int rc = ring_ready(rb, replica, 4)) return rc;
   if (int rc = ring_quiesce(rb)) return rc;
   per_sample_kernel<<<1, B > 256 ? 512 : 256, 0, rb->st>>>(h->K, rb->tr, nullptr, rb->draws[(size_t)replica]++, replica,
-                                                           rb->d_fill, rb->d_beta, rb->s_idx, rb->s_f, (long long)B, rb->seed);
+                                                           rb->d_fill, rb->beta.dev, rb->s_idx, rb->s_f, (long long)B, rb->seed);
   per_gather_kernel<<<B, 128, 0, rb->st>>>(rb->rows + (size_t)replica * rb->rs_rows, rs, rb->s_idx, rb->s_rows);
   CU(cudaGetLastError());
   std::vector<int> ix((size_t)B);
@@ -3805,15 +3813,15 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   CU(cudaSetDevice(h->device));
   if (int rc = ring_quiesce(rb)) return rc;
   const size_t nl = (size_t)h->R * rb->cap;
-  const std::vector<int> nstep0((size_t)h->R, 1);
-  DevMem<int> link, nstep, f_m;
+  DevMem<int> link, f_m;
   DevMem<long long> f_idx;
   DevMem<float> f_rows, f_disc;
   Event ev;
   CU(cudaMalloc(link.put(), nl * sizeof(int)));
   CU(cudaMemset(link, 0xff, nl * sizeof(int)));
-  CU(cudaMalloc(nstep.put(), nstep0.size() * sizeof(int)));
-  CU(cudaMemcpy(nstep, nstep0.data(), nstep0.size() * sizeof(int), cudaMemcpyHostToDevice));
+  ReplicaTable<int> nstep;
+  const int one = 1;
+  if (int rc = nstep.init(h->R, &one)) return rc;
   CU(cudaMalloc(f_idx.put(), kNstepChunk * sizeof(long long)));
   CU(cudaMalloc(f_rows.put(), kNstepChunk * (size_t)h->row_stride * sizeof(float)));
   CU(cudaMalloc(f_disc.put(), kNstepChunk * sizeof(float)));
@@ -3827,9 +3835,8 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
     h->ns_buf = std::move(ns_buf);
   }
   drop_ring_graphs(h, rb);                         // they hold the unlinked gather
-  rb->d_link = std::move(link); rb->d_nstep = std::move(nstep); rb->f_idx = std::move(f_idx); rb->f_rows = std::move(f_rows);
+  rb->d_link = std::move(link); rb->nstep = std::move(nstep); rb->f_idx = std::move(f_idx); rb->f_rows = std::move(f_rows);
   rb->f_disc = std::move(f_disc); rb->f_m = std::move(f_m); rb->ev_nstep = std::move(ev);
-  rb->nstep_host.assign((size_t)h->R, 1);
   rb->link_h.assign(nl, -1);
   rb->pred_h.assign(nl, -1);
   rb->tail.assign((size_t)h->R, {});
@@ -3854,21 +3861,13 @@ extern "C" int b200sac_replay_close_streams(b200sac_replay_t* rb, int32_t replic
 extern "C" int b200sac_replay_set_nstep(b200sac_replay_t* rb, int32_t replica, int32_t n, void* stream) {
   if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (n < 1 || n > kNstepMax) return fail(B200SAC_ERR_INVALID, "n-step horizon must be in [1, %d] (got %d)", kNstepMax, n);
-  CU(cudaSetDevice(rb->h->device));
-  StreamBridge sb(rb->h, stream);
-  if (int rc = sb.begin()) return rc;
-  nstep_set_kernel<<<1, 1, 0, sb.run>>>(rb->d_nstep, replica, n);
-  CU(cudaGetLastError());
-  CU(cudaEventRecord(rb->ev_nstep, sb.run));
-  if (int rc = sb.end()) return rc;
-  rb->nstep_host[(size_t)replica] = n;
-  return 0;
+  return rb->nstep.set(rb->h, stream, replica, &n, rb->ev_nstep);
 }
 
 extern "C" int b200sac_replay_get_nstep(b200sac_replay_t* rb, int32_t replica, int32_t* n) {
   if (int rc = ring_check(rb, replica, RING_TRAJ)) return rc;
   if (!n) return fail(B200SAC_ERR_INVALID, "null argument");
-  *n = rb->nstep_host[(size_t)replica];
+  *n = *rb->nstep.row(replica);
   return 0;
 }
 
@@ -3901,7 +3900,7 @@ extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_
     const int c = (int)std::min<int64_t>(kNstepChunk, n_idx - i0);
     CU(cudaMemcpyAsync(rb->f_idx, idx + i0, c * sizeof(long long), cudaMemcpyHostToDevice, rb->st));
     nstep_fold_kernel<<<(c + 7) / 8, 256, 0, rb->st>>>(rb->rows + (size_t)replica * rb->rs_rows, rs, obs, A,
-                                                       rb->d_link + (size_t)replica * rb->cap, (int)rb->cap_per_task, rb->d_nstep, h->hp,
+                                                       rb->d_link + (size_t)replica * rb->cap, (int)rb->cap_per_task, rb->nstep.dev, h->hp.dev,
                                                        replica, rb->f_idx, c, rb->f_rows, rb->f_disc, rb->f_m);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(rows.data(), rb->f_rows, (size_t)c * rs * sizeof(float), cudaMemcpyDeviceToHost, rb->st));

@@ -111,11 +111,4 @@ __global__ void __launch_bounds__(256) grad_sqnorm_kernel(StepConst K, GradNormA
   }
 }
 
-// b200sac_set_grad_clip: one replica's thresholds, written in stream order
-__global__ void set_grad_clip_kernel(double* thr, int replica, double critic, double actor, double ctx) {
-  thr[replica * kClipCols] = critic;
-  thr[replica * kClipCols + 1] = actor;
-  thr[replica * kClipCols + 2] = ctx;
-}
-
 }  // namespace bsac

@@ -119,6 +119,4 @@ __global__ void nstep_fill_links_kernel(int* __restrict__ link, long long cap, i
   }
 }
 
-__global__ void nstep_set_kernel(int* nstep, int rep, int n) { nstep[rep] = n; }
-
 }  // namespace bsac

@@ -211,10 +211,4 @@ __global__ void __launch_bounds__(256) pcgrad_kernel(StepConst K, PcgArgs P) {
   }
 }
 
-// b200sac_set_pcgrad: one replica's switches, written in stream order
-__global__ void set_pcgrad_kernel(int* on, int replica, int critic, int actor) {
-  on[replica * 2] = critic;
-  on[replica * 2 + 1] = actor;
-}
-
 }  // namespace bsac

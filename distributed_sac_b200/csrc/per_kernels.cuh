@@ -201,6 +201,4 @@ __global__ void per_gather_kernel(const float* __restrict__ rows, int row_stride
   for (int j = threadIdx.x; j < row_stride; j += blockDim.x) out[(long long)blockIdx.x * row_stride + j] = src[j];
 }
 
-__global__ void per_set_beta_kernel(double* beta, int rep, double v) { beta[rep] = v; }
-
 }  // namespace bsac

@@ -1101,9 +1101,6 @@ __global__ void polyak_kernel(float* p, long long rsP, long long n, long long ta
   }
 }
 
-// b200sac_set_hparams: one replica's row, written in stream order (a kernel argument, so it is also capturable)
-__global__ void set_hparams_kernel(HParams* hp, int replica, HParams row) { hp[replica] = row; }
-
 // randn init of the mixture-of-encoders weights (state_encoder.py:146-153)
 __global__ void randn_kernel(float* w, long long rsP, long long n, unsigned long long seed, int tag) {
   const int rep = blockIdx.y;
