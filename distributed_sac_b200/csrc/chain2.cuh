@@ -8,9 +8,14 @@
 //                   (learner.py:221-225, model.py:84-88)
 // As two launches each pair paid a kernel boundary, a cold prologue and a restart of the weight pipeline.
 // Here the CTA that owns rows [row0, row0+ROWS) of twin k walks the forward chain, the two CTAs of a thread-block CLUSTER
-// (twin 0, twin 1 of the same rows) swap their ROWS head values through distributed shared memory (mapa + ld.shared::cluster
-// between two barrier.cluster phases), and each goes on into the backward chain of its own twin -- the TMA weight pipeline
-// never drains: the first backward chunks are requested while the forward head is still being computed.
+// (twin 0, twin 1 of the same rows) swap their ROWS head values through distributed shared memory, and each goes on into the
+// backward chain of its own twin -- the TMA weight pipeline never drains: the first backward chunks are requested while the
+// forward head is still being computed.
+// The swap is a remote st.async into the peer's xch, counted by the peer's exchange mbarrier (complete_tx), not a cluster
+// barrier: barrier.cluster.arrive.release compiles to MEMBAR.ALL.GPU, which waits for every outstanding memory access of the
+// thread while the producer warps of the whole grid keep the memory system full of weight requests -- 1 300 to 4 700 cycles
+// of the critic update on the H100.  The one cluster barrier phase before the swap (relaxed arrive after the mbarrier
+// initialisation, wait just before the first remote store) only guarantees that the peer's exchange mbarrier exists.
 #pragma once
 #include "chain.cuh"
 
@@ -43,16 +48,15 @@ struct Chain2Args {
   ChainRows rw;
 };
 
-B200_D void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-B200_D float ld_peer_f32(const float* my_smem_addr, uint32_t peer_rank) {
-  uint32_t ra;
+B200_D void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
+B200_D void cluster_wait() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
+// v -> the peer CTA's copy of *my_smem_addr, completing `bytes` of the transaction count of the peer's copy of *my_bar
+B200_D void st_async_peer_f32(const float* my_smem_addr, const uint64_t* my_bar, uint32_t peer_rank, float v) {
+  uint32_t ra, rb;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(ra) : "r"(smem_u32(my_smem_addr)), "r"(peer_rank));
-  float v;
-  asm volatile("ld.shared::cluster.f32 %0, [%1];" : "=f"(v) : "r"(ra) : "memory");
-  return v;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(rb) : "r"(smem_u32(my_bar)), "r"(peer_rank));
+  asm volatile("st.async.shared::cluster.mbarrier::complete_tx::bytes.b32 [%0], %1, [%2];" ::"r"(ra), "r"(__float_as_uint(v)), "r"(rb)
+               : "memory");
 }
 
 // GATED: the actor pass (C2_ACTORQ), skipped on critic-only steps; its own instantiation, so that the critic update's
@@ -72,7 +76,8 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
   float* headF = c.own_smem();             // [CH_INP] forward head row
   float* headB = headF + CH_INP;           // [CH_INP] backward (differentiated net's) head row
   float* sd = headB + CH_INP;              // [ROWS] d(head output) per row
-  float* xch = sd + CH_ROWS;               // [ROWS] this twin's forward head values (read by the peer CTA)
+  float* xch = sd + CH_ROWS;               // [ROWS] the PEER twin's forward head values (stored by the peer CTA)
+  uint64_t* xbar = c.bars + CH_NSTAGE;     // exchange mbarrier: completes when the peer's nrows values have landed in xch
   float* w0a = xch + CH_ROWS;
   c.part = w0a + C2_SM_W0A;
 
@@ -91,7 +96,10 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
   // leave together, before any cluster barrier.  The word is requested before griddepcontrol.wait (sched_word) and consumed
   // after it; a CTA that skips first drains what it requested early (no copy may outlive it).
   const int sched = GATED ? sched_of(K.cnt, rep) : SCHED_ACTOR;
-  if (tid == 0) c.start_pipeline(A.early_weights);
+  if (tid == 0) {
+    mbar_init(smem_u32(xbar), 1);          // (start_pipeline's fence.mbarrier_init publishes it to the cluster)
+    c.start_pipeline(A.early_weights);
+  }
   if (A.early_weights && tid < CH_THREADS) request_weights();
   KStamp ks_;
   c.stamp();
@@ -102,14 +110,14 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     return;
   }
   __syncthreads();                         // barriers initialised (all nine warps)
+  cluster_arrive_relaxed();                // both CTAs' exchange mbarriers exist once this phase completes
   if (tid >= CH_THREADS) {
-    // ---- producer warp: every remaining weight chunk of the forward AND the backward part, in order.  It takes part in the
-    // cluster barriers without ever blocking the twins' exchange: it arrives for the exchange phase right away (it needs
-    // nothing from it) and collects that phase when its work is done.
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
+    // ---- producer warp: every remaining weight chunk of the forward AND the backward part, in order.  It collects the
+    // initialisation phase when its work is done, so it never holds up the twins' exchange.
     c.produce(A.early_weights);
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-    cluster_sync_all();                    // the final one (nobody leaves while its twin may still read its shared memory)
+    cluster_wait();
+    cluster_arrive_relaxed();              // the final phase (nobody leaves while its twin may still store into its shared memory)
+    cluster_wait();
     return;
   }
   if (!A.early_weights) request_weights();
@@ -164,17 +172,19 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
     float a = 0.f;
     for (int k = lane; k < J.Hhf; k += 32) a = fmaf(hr[k], headF[k], a);
     q_own = warp_sum(a) + bq;
-    if (lane == 0) {
-      xch[w] = q_own;
-      (J.qf_out + (long long)rep * J.rsQf)[row] = q_own;
-    }
   }
   // ================================ the twins swap their head values ================================
-  cluster_sync_all();                      // (also a CTA-wide barrier: xch is complete in both CTAs)
+  cluster_wait();                          // the peer's exchange mbarrier is initialised
+  if (w < nrows && lane == 0) {
+    st_async_peer_f32(xch + w, xbar, my_rank ^ 1u, q_own);
+    (J.qf_out + (long long)rep * J.rsQf)[row] = q_own;
+  }
+  if (tid == 0) mbar_expect_tx(smem_u32(xbar), (uint32_t)nrows * 4u);    // (the peer has the same rows)
+  mbar_wait(smem_u32(xbar), 0u);
   c.stamp();
   const float alpha_row = alpha.of(__shfl_sync(0xffffffffu, t_row, 0));
   if (owner) {
-    const float q_peer = ld_peer_f32(xch + w, my_rank ^ 1u);
+    const float q_peer = xch[w];
     const float qa = J.net == 0 ? q_own : q_peer, qb = J.net == 0 ? q_peer : q_own;
     if (A.kind == C2_CRITIC) {             // qa, qb = Qt1, Qt2
       const float y = td_target(reward_scale * r_row, gamma * (1.f - d_row), qa, qb, alpha_row, lp_row);
@@ -255,7 +265,8 @@ __global__ void __launch_bounds__(CH_BLOCK, 1) chain2_kernel(const __grid_consta
   }
   c.stamp();
   c.stamp.done();
-  cluster_sync_all();                      // nobody leaves while its twin may still read its shared memory
+  cluster_arrive_relaxed();                // nobody leaves while its twin may still store into its shared memory
+  cluster_wait();
 }
 
 }  // namespace bsac
