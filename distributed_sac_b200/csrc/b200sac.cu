@@ -21,6 +21,7 @@
 #include <unordered_map>
 #include <unordered_set>
 #include <utility>
+#include <variant>
 #include <vector>
 
 #include "../../include/b200sac.h"
@@ -258,42 +259,37 @@ struct Buf {           // [R][n] fp32 (or int32) slab slice
   long long rs = 0;    // replica stride in floats
 };
 
-enum LaunchKind { L_POLICY_DOUT, L_CARE_TAB, L_CARE_MIXFWD, L_CARE_MIX, L_CARE_MIXBWD, L_CARE_TABRED, L_CARE_TABWG, L_GEMM_SMALL, L_GEMM_THIN, L_GEMM_TC, L_POLICY, L_CHEADS, L_AQHEADS, L_HEADBWD, L_ADAM, L_CHAIN, L_WGRAD, L_CHAIN2, L_GRADNORM, L_PCGRAD };
+// A plan launch's kernel, chosen by the builder that makes the launch, with its argument block.  The step kernels take
+// (StepConst, args), (args, StepConst) or (args); the StepConst is the step's, handed over when the plan runs.
+template <class P> struct StepFirst { void (*kern)(StepConst, P); P args; };
+template <class P> struct StepLast { void (*kern)(P, StepConst); P args; };
+template <class P> struct NoStep { void (*kern)(P); P args; };
+// the wgmma GEMM: its problems [R][G] (replica-major) and, on an actor-side launch, replica 0's schedule word
+typedef void (*TcKernel)(const TcProb*, const int*, int, int);
+struct TcCall { TcKernel kern; const TcProb* probs; const int* sched; int G, sched_stride; };
+using KernelCall = std::variant<StepFirst<PolicyDoutArgs>, StepFirst<PolicyHeadArgs>, StepFirst<CriticHeadArgs>,
+                                StepFirst<ActorQHeadArgs>, StepFirst<HeadBwdArgs>, StepFirst<AdamArgs>, StepFirst<PcgArgs>,
+                                StepFirst<GradNormArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
+                                NoStep<CareTabArgs>, NoStep<CareMixArgs>, NoStep<CareMixFwdArgs>, NoStep<CareMixBwdArgs>,
+                                NoStep<CareTabReduceArgs>, NoStep<CareTabWgradArgs>, NoStep<GemmGroup>, TcCall>;
+template <class P> static KernelCall bind(void (*kern)(StepConst, P), const P& args) { return StepFirst<P>{kern, args}; }
+template <class P> static KernelCall bind(void (*kern)(P, StepConst), const P& args) { return StepLast<P>{kern, args}; }
+template <class P> static KernelCall bind(void (*kern)(P), const P& args) { return NoStep<P>{kern, args}; }
+static KernelCall bind(TcKernel kern, const TcProb* probs, const int* sched, int G, int sched_stride) {
+  return TcCall{kern, probs, sched, G, sched_stride};
+}
 
 struct Launch {
-  LaunchKind kind;
-  dim3 grid, block;
-  size_t smem = 0;
-  int branch = 0;        // 1: may run on the fork stream, concurrently with the launches that follow it on the main stream
-  bool join = false;     // the main stream waits for the fork stream before this launch
-  // payloads (only the one matching `kind` is used)
-  int G = 0;
-  GemmGroup grp;
-  int tprob0 = 0;        // L_GEMM_TC: index of the launch's first problem in the handle's d_tprobs
-  int bn = 64;
-  bool pair128 = false;  // L_GEMM_TC with bn = 128: the paired tile flavour (fixed when the plan is built)
-  const int* sched = nullptr;   // L_GEMM_TC: actor-side launch, replica 0's schedule word (gemm_tc_kernel)
-  PolicyDoutArgs pdo;
-  CareTabArgs ctab;
-  CareMixArgs cmix;
-  CareMixFwdArgs cmf;
-  CareMixBwdArgs cmixb;
-  CareTabReduceArgs ctred;
-  CareTabWgradArgs ctwg;
-  PolicyHeadArgs pol;
-  CriticHeadArgs ch;
-  ActorQHeadArgs aq;
-  HeadBwdArgs hb;
-  AdamArgs ad;
-  ChainArgs chain;
-  Chain2Args chain2;
-  WgradArgs wg;
-  bool store_only = false;   // L_WGRAD: the gradients alone, no optimizer step (grad_clip plans)
-  GradNormArgs gn;
-  PcgArgs pc;
   // What b200sac_profile_step calls the launch, set by the builder that makes it.  The part before '(' and the "wgmma"
   // substring are what bench.py groups kernels by.
   std::string label;
+  dim3 grid, block;
+  size_t smem = 0;
+  int cluster_y = 1;     // > 1: thread-block clusters of (1, cluster_y, 1)
+  int branch = 0;        // 1: may run on the fork stream, concurrently with the launches that follow it on the main stream
+  bool join = false;     // the main stream waits for the fork stream before this launch
+  bool critic_loss = false;   // its rows carry the step's TD target and pre-update critic values (the PER priority update follows)
+  KernelCall call;
 };
 
 struct b200sac_replay;
@@ -385,9 +381,11 @@ struct b200sac {
   int care_row_w = 0, care_off_att = 0, care_off_ctx = 0;
   std::vector<Buf> hA, dhA;       // per actor hidden layer
   std::vector<Buf> hQ, hT, hP, dhQ;   // per critic hidden layer, [2][B][H]
-  DevMem<TcProb> d_tprobs;
-  std::vector<TcProb> h_tprobs;
   std::vector<Launch> plan;
+  // what the plan's launches read through their argument blocks: each wgmma launch's problems, each layer-chained launch's
+  // tensor maps
+  std::vector<DevMem<TcProb>> tprobs;
+  std::vector<DevMem<CUtensorMap>> tmaps;
   IngestOut ing;
   // split-K weight gradients: slices 1..gslices-1 of the gradient arena, [slice-1][R][trainable] (slice 0 = grads)
   DevMem<float> grads_x;
@@ -422,8 +420,6 @@ struct b200sac {
   int64_t blob_bytes = 0, blob_nf = 0;
   int blob_replica = 0, blob_head = 0, blob_pending = 0;
   Event ev_blob_snap[2], ev_blob_done[2];
-  DevMem<CUtensorMap> d_cmaps;    // layer-chained plan: 2-D tensor maps of the forward weight matrices [R][nf], then of the
-                                  // weight-gradient operands [R][nw]
   DevMem<long long> chain_dbg;    // env.chain_dbg: [plan launches][CH_DBG_SLOTS] clock64 timelines of the chain kernels
   DevMem<float> step_d;           // b200sac_step: the caller's minibatch as packed rows [R][B][row_stride] (stable graph pointers)
   PinnedMem<float> loss_h;        // mapped pinned loss ring [kLossSlots][R][4], written by the tail kernels
@@ -601,8 +597,7 @@ static bool tc_eligible(const GemmProb& p) {
 }
 
 // Tile variants of the wgmma GEMM (gemm_tc.cuh): 128x64, 128x128 (EnvSwitches::pair128: the paired flavour), 128x160.
-// A step plan keeps the choice on its launches (Launch::pair128).
-typedef void (*TcKernel)(const TcProb*, const int*, int, int);
+// A step plan binds the chosen instantiation to its launches.
 static TcKernel tc_kernel(int bn, bool pair128) {
   if (bn == 160) return gemm_tc_kernel<160, false>;
   if (bn == 128) return pair128 ? (TcKernel)gemm_tc_kernel<128, true> : (TcKernel)gemm_tc_kernel<128, false>;
@@ -611,11 +606,16 @@ static TcKernel tc_kernel(int bn, bool pair128) {
 static size_t tc_smem(int bn) {
   return bn == 160 ? TcCfg<160>::kSmemBytes : (bn == 128 ? TcCfg<128>::kSmemBytes : TcCfg<64>::kSmemBytes);
 }
-static cudaError_t tc_set_attrs() {
-  cudaError_t e = cudaFuncSetAttribute(gemm_tc_kernel<64, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<64>::kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc_kernel<128, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<128>::kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc_kernel<128, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<128>::kSmemBytes);
-  if (e == cudaSuccess) e = cudaFuncSetAttribute(gemm_tc_kernel<160, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, TcCfg<160>::kSmemBytes);
+// Lets `kern` launch with `smem` bytes of dynamic shared memory.  The limit is one per kernel and device for the whole
+// process, and every handle's plan launches the same kernels, so it is only ever raised.
+static cudaError_t allow_smem(const void* kern, size_t smem) {
+  if (smem == 0) return cudaSuccess;
+  static std::mutex mu;
+  std::lock_guard<std::mutex> lock(mu);
+  cudaFuncAttributes a;
+  cudaError_t e = cudaFuncGetAttributes(&a, kern);
+  if (e == cudaSuccess && (size_t)a.maxDynamicSharedSizeBytes < smem)
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   return e;
 }
 // Modelled cycles of one launch group with `bn`-wide tiles (constants from scripts/tc_timeline.py on an H100 SXM, 400 W
@@ -843,6 +843,30 @@ struct PlanBuilder {
   float* W(int64_t off) const { return h->params + off; }
   float* Gp(int64_t off) const { return h->grads + off; }
 
+  // appends launch l running kern(args), first letting kern take l.smem bytes of dynamic shared memory
+  template <class F, class... P> void push(Launch l, F kern, const P&... args) {
+    if (cudaError_t e = allow_smem((const void*)kern, l.smem)) {
+      cudaGetLastError();
+      rc = fail(B200SAC_ERR_CUDA, "%s: dynamic shared memory of %zu bytes refused: %s", l.label.c_str(), l.smem, cudaGetErrorString(e));
+    }
+    l.call = bind(kern, args...);
+    h->plan.push_back(std::move(l));
+  }
+  // a copy of v on the device, owned by the handle (empty: null)
+  template <class T> const T* upload(std::vector<DevMem<T>>& owner, const std::vector<T>& v) {
+    if (v.empty()) return nullptr;
+    DevMem<T> d;
+    cudaError_t e = cudaMalloc(d.put(), v.size() * sizeof(T));
+    if (e == cudaSuccess) e = cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      rc = fail(e == cudaErrorMemoryAllocation ? B200SAC_ERR_NOMEM : B200SAC_ERR_CUDA, "plan table upload failed: %s", cudaGetErrorString(e));
+      return nullptr;
+    }
+    owner.push_back(std::move(d));
+    return owner.back();
+  }
+
   void gemm_launch(const std::vector<GemmProb>& ps_in);
   void care_tables(const std::vector<int>& insts);
   void care_encode(const std::vector<EncJob>& jobs);
@@ -858,14 +882,13 @@ struct PlanBuilder {
 // Label of a grouped GEMM launch of the problems g: their kind (a thin launch is named after its first problem alone), the
 // engine and wgmma tile (128x64 | 128x128 | 128x128 paired | 128x160) and, when the group holds weight gradients, their K
 // slices ("split S")
-static std::string gemm_label(const std::vector<GemmProb>& g, LaunchKind kind, int bn, bool pair128, int split) {
+static std::string gemm_label(const std::vector<GemmProb>& g, const std::string& engine, int split) {
   const GemmProb &p0 = g.front(), &pl = g.back();
   bool wg = false;
   for (auto& p : g) wg = wg || p.mode == GEMM_WGRAD;
   std::string s = p0.mode == GEMM_FWD ? "gemm_fwd(" : p0.mode == GEMM_DGRAD ? "gemm_dgrad(" :
-                  (pl.mode == GEMM_DGRAD && kind != L_GEMM_THIN) ? "gemm_wgrad+dgrad(" : "gemm_wgrad(";
-  if (kind == L_GEMM_TC) s += "wgmma 128x" + std::to_string(bn) + (pair128 ? " paired" : "");
-  else s += kind == L_GEMM_THIN ? "thin" : "ffma";
+                  (pl.mode == GEMM_DGRAD && engine != "thin") ? "gemm_wgrad+dgrad(" : "gemm_wgrad(";
+  s += engine;
   if (wg) s += ", split " + std::to_string(split);
   return s + ")";
 }
@@ -934,24 +957,21 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
       int maxM = 0, maxN = 0;
       for (auto& p : tc) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; }
       const int bn = tc_pick_bn(tc, R, h->env);  // tile width: the cheapest of 64 / 128 / 160 under tc_group_cost's model
-      l.kind = L_GEMM_TC;
+      const bool pair128 = bn == 128 && h->env.pair128;
       l.branch = branch;
-      l.bn = bn;
-      l.pair128 = bn == 128 && h->env.pair128;
-      l.sched = actor_side ? &h->cnt[0].sched : nullptr;
-      l.label = gemm_label(tc, L_GEMM_TC, bn, l.pair128, split);
+      l.label = gemm_label(tc, "wgmma 128x" + std::to_string(bn) + (pair128 ? " paired" : ""), split);
       l.grid = dim3((maxN + bn - 1) / bn, (maxM + TC_BM - 1) / TC_BM, (unsigned)(tc.size() * R));
       l.block = dim3(TC_THREADS);
       l.smem = tc_smem(bn);
-      l.G = (int)tc.size();
-      l.tprob0 = (int)h->h_tprobs.size();
+      std::vector<TcProb> probs;
       for (int rep = 0; rep < R; ++rep)
         for (auto& p : tc) {
           TcProb t;
           if (int e = make_tc_prob(p, rep, t, bn)) rc = e;
-          h->h_tprobs.push_back(t);
+          probs.push_back(t);
         }
-      h->plan.push_back(l);
+      push(std::move(l), tc_kernel(bn, pair128), upload(h->tprobs, probs), actor_side ? &h->cnt[0].sched : nullptr,
+           (int)tc.size(), kSchedStride);
     }
     ps = rest;
   }
@@ -964,7 +984,6 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
     int maxM = 0, maxN = 0;
     bool thin = true;
     for (auto& p : g) { maxM = p.M > maxM ? p.M : maxM; maxN = p.N > maxN ? p.N : maxN; thin = thin && gemm_is_thin(p); }
-    l.kind = L_GEMM_SMALL;
     l.branch = branch;
     l.grid = dim3((maxN + GS_T - 1) / GS_T, (maxM + GS_T - 1) / GS_T, (unsigned)(g.size() * R));
     l.block = dim3(GS_THREADS);
@@ -974,28 +993,27 @@ void PlanBuilder::gemm_launch(const std::vector<GemmProb>& ps_in) {
         const int per = p.mode == GEMM_WGRAD ? GT_ROWS_WGRAD : GT_ROWS_DGRAD, r = (p.M + per - 1) / per;
         rows = r > rows ? r : rows;
       }
-      l.kind = L_GEMM_THIN;
       l.grid = dim3(1, rows, (unsigned)(g.size() * R));
       l.block = dim3(GT_THREADS);
     }
-    l.label = gemm_label(g, l.kind, 0, false, split);
-    memset(&l.grp, 0, sizeof(l.grp));
-    l.grp.G = (int)g.size();
-    l.grp.sched = actor_side ? &h->cnt[0].sched : nullptr; l.grp.sched_stride = kSchedStride;
-    for (size_t i = 0; i < g.size(); ++i) l.grp.p[i] = g[i];
-    h->plan.push_back(l);
+    l.label = gemm_label(g, thin ? "thin" : "ffma", split);
+    GemmGroup grp;
+    memset(&grp, 0, sizeof(grp));
+    grp.G = (int)g.size();
+    grp.sched = actor_side ? &h->cnt[0].sched : nullptr; grp.sched_stride = kSchedStride;
+    for (size_t i = 0; i < g.size(); ++i) grp.p[i] = g[i];
+    push(std::move(l), thin ? gemm_thin_kernel : gemm_simt_kernel, grp);
   }
 }
 
 void PlanBuilder::care_tables(const std::vector<int>& insts) {
   Launch l;
-  l.kind = L_CARE_TAB;
   l.label = "care_tables";
-  l.ctab = care_tab_args(h, -1, insts);
-  l.ctab.sched = actor_side ? &h->cnt[0].sched : nullptr; l.ctab.sched_stride = kSchedStride;
+  CareTabArgs P = care_tab_args(h, -1, insts);
+  P.sched = actor_side ? &h->cnt[0].sched : nullptr; P.sched_stride = kSchedStride;
   l.grid = dim3(c.num_tasks, (unsigned)insts.size(), R);
   l.block = dim3(512);
-  h->plan.push_back(l);
+  push(std::move(l), care_tables_kernel, P);
 }
 
 // mixture layers + attention mix of up to three encoder instances in ONE launch (care_mixfwd_kernel: all mixture weights of
@@ -1031,16 +1049,13 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
     J.dst1 = e.d1.p; J.rsD1 = e.d1.rs; J.ld1 = e.ld1; J.dst2 = e.d2.p; J.rsD2 = e.d2.rs; J.ld2 = e.ld2; J.row_off2 = e.off2;
   }
   const size_t smem = ok ? care_mixfwd_smem_floats(A) * sizeof(float) : 0;
-  if (ok && smem <= 225 * 1024 &&
-      cudaFuncSetAttribute(care_mixfwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 225 * 1024) == cudaSuccess) {
+  if (ok && smem <= 225 * 1024 && allow_smem((const void*)care_mixfwd_kernel, smem) == cudaSuccess) {
     Launch l;
-    l.kind = L_CARE_MIXFWD;
     l.label = "care_mixture_fwd+mix";
-    l.cmf = A;
     l.grid = dim3(cta, R);
     l.block = dim3(CMF_THREADS);
     l.smem = smem;
-    h->plan.push_back(l);
+    push(std::move(l), care_mixfwd_kernel, A);
     return;
   }
   for (int l = 0; l < nmix; ++l) {
@@ -1050,21 +1065,19 @@ void PlanBuilder::care_encode(const std::vector<EncJob>& jobs) {
   }
   for (const EncJob& e : jobs) {
     Launch l;
-    l.kind = L_CARE_MIX;
     l.label = "care_mix";
-    l.cmix = care_mix_args(h, -1, e);
-    l.cmix.sched = actor_side ? &h->cnt[0].sched : nullptr; l.cmix.sched_stride = kSchedStride;
+    CareMixArgs P = care_mix_args(h, -1, e);
+    P.sched = actor_side ? &h->cnt[0].sched : nullptr; P.sched_stride = kSchedStride;
     l.grid = dim3((e.rows + 7) / 8, R);
     l.block = dim3(256);
-    h->plan.push_back(l);
+    push(std::move(l), care_mix_kernel, P);
   }
 }
 
 void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   const int Hc = c.critic_hidden[Lc - 1], Ha = c.actor_hidden[La - 1];
   Launch l;
-  l.kind = L_HEADBWD;
-  HeadBwdArgs& P = l.hb;
+  HeadBwdArgs P;
   memset(&P, 0, sizeof(P));
   P.actor_side = (policy || !want_wgrad) ? 1 : 0;       // the actor pass / the policy backward, not the critic update
   P.M = B;
@@ -1085,9 +1098,8 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
     const bool split = (long long)B * A > 2048;      // large batch: one tiny kernel computes d(mu|log_std) for all rows
     if (split) {
       Launch pl;
-      pl.kind = L_POLICY_DOUT;
       pl.label = "policy_dout";
-      PolicyDoutArgs& Q = pl.pdo;
+      PolicyDoutArgs Q;
       memset(&Q, 0, sizeof(Q));
       Q.dx = h->dxP.p; Q.rsDxNet = (long long)B * h->K.ldx; Q.rsDxRep = h->dxP.rs; Q.lddx = h->K.ldx;
       Q.psave = h->psave.p + (long long)B * A * kSaveW; Q.rsSave = h->psave.rs;
@@ -1097,7 +1109,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
       Q.M = B;
       pl.grid = dim3((B * A + 255) / 256, R);
       pl.block = dim3(256);
-      h->plan.push_back(pl);
+      push(std::move(pl), policy_dout_kernel, Q);
     }
     P.NO = 2 * A; P.Kdim = Ha; P.nets = 1; P.policy_mode = split ? 0 : 1;
     if (split) { P.dout = h->dout_dbg.p; P.rsDoutNet = 0; P.rsDoutRep = h->dout_dbg.rs; }
@@ -1118,18 +1130,21 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   for (int net = 0; net < P.nets; ++net)
     if (P.dW[net] && h->grads_x) { P.dWx[net] = h->grads_x + (P.dW[net] - h->grads); P.dbx[net] = h->grads_x + (P.db[net] - h->grads); }
   const int rows_per = (B + P.row_slices - 1) / P.row_slices;
-  // 128-bit column mapping when every row pitch / tensor offset involved is a multiple of 4 floats (l.bn = 4 marks it)
-  // -- for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
+  // 128-bit column mapping (head_bwd4_kernel) when every row pitch / tensor offset involved is a multiple of 4 floats --
+  // for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
   // few to fill the GPU
   const bool wide = P.NO == 1 && (P.Kdim % 4) == 0 && (P.ldh % 4) == 0 && (P.lddh % 4) == 0;
-  l.bn = wide ? 4 : 1;
   l.label = std::string(policy ? "head_bwd(policy, " : "head_bwd(q, ") + (wide ? "128-bit, " : "") + "row slices " +
             std::to_string(P.row_slices) + ")";
   const int cols = wide ? kHb4Cols : kHbCols;
   l.grid = dim3(((P.Kdim + cols - 1) / cols) * ((B + rows_per - 1) / rows_per), P.nets, R);
   l.block = dim3(256);
   l.smem = ((((size_t)rows_per * P.NO + 3) & ~(size_t)3) + (wide ? 1024 : 256) * (size_t)P.NO) * sizeof(float);   // head_bwd4: red 16-B aligned
-  h->plan.push_back(l);
+  if (l.smem > 200 * 1024) {
+    rc = fail(B200SAC_ERR_INVALID, "batch * head width too large for head_bwd smem");
+    return;
+  }
+  push(std::move(l), wide ? head_bwd4_kernel<1> : head_bwd_kernel, P);
 }
 
 // the trainable slice of optimizer `which` (0 critic, 1 actor, 2 CARE(O) context encoder)
@@ -1144,10 +1159,9 @@ void PlanBuilder::opt_slice(int which, int64_t& beg, int64_t& n) const {
 // with_tail = false drops the tail job (the layer-chained plan's forked tail has it).
 void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
   Launch l;
-  l.kind = L_ADAM;
   l.label = which == 0 ? "adam_critic+polyak" : which == 2 ? "adam_context_encoder" :
             tail_only ? "alpha+losses(forked)" : with_tail ? "adam_actor+alpha" : "adam_actor";
-  AdamArgs& P = l.ad;
+  AdamArgs P;
   memset(&P, 0, sizeof(P));
   int64_t beg, n;
   opt_slice(which, beg, n);
@@ -1179,15 +1193,14 @@ void PlanBuilder::adam(int which, bool tail_only, bool with_tail) {
   l.block = dim3(256);
   l.join = !clip && !pcg;        // every gradient of the slice must have landed, including the forked weight gradients
   if (tail_only) { l.grid = dim3(1, R); l.join = false; l.branch = 1; }
-  h->plan.push_back(l);
+  push(std::move(l), pcg ? adam_kernel<false, true> : clip ? adam_kernel<true> : adam_kernel<false>, P);
 }
 
 // grad_clip handles: the gradient norm of optimizer `which` and the clip coefficient its Adam launch (next) applies
 void PlanBuilder::grad_norm(int which) {
   Launch l;
-  l.kind = L_GRADNORM;
   l.label = which == 0 ? "grad_norm{critic}" : which == 1 ? "grad_norm{actor}" : "grad_norm{context_encoder}";
-  GradNormArgs& P = l.gn;
+  GradNormArgs P;
   memset(&P, 0, sizeof(P));
   int64_t beg, n;
   opt_slice(which, beg, n);
@@ -1203,16 +1216,15 @@ void PlanBuilder::grad_norm(int which) {
   l.grid = dim3(elementwise_blocks(n), R);
   l.block = dim3(256);
   l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
-  h->plan.push_back(l);
+  push(std::move(l), grad_sqnorm_kernel, P);
 }
 
 // pcgrad handles: the Gram matrix of optimizer `which`'s task slices, the surgery and the slice weights its Adam launch
 // (next) applies
 void PlanBuilder::pcgrad(int which) {
   Launch l;
-  l.kind = L_PCGRAD;
   l.label = which == 0 ? "pcgrad{critic}" : "pcgrad{actor}";
-  PcgArgs& P = l.pc;
+  PcgArgs P;
   memset(&P, 0, sizeof(P));
   int64_t beg, n;
   opt_slice(which, beg, n);
@@ -1229,7 +1241,7 @@ void PlanBuilder::pcgrad(int which) {
   l.block = dim3(256);
   l.smem = pcgrad_smem(T);
   l.join = true;                 // every gradient of the slice must have landed, including the forked weight gradients
-  h->plan.push_back(l);
+  push(std::move(l), pcgrad_kernel, P);
 }
 
 int PlanBuilder::build_plan_fused() {
@@ -1245,10 +1257,6 @@ int PlanBuilder::build_plan_fused() {
   rw.psave = h->psave.p + (long long)B * A * kSaveW; rw.rsSave = h->psave.rs;
   rw.dout_dbg = h->dout_dbg.p; rw.dact_dbg = h->dact_dbg.p; rw.rsDbg = h->dout_dbg.rs;
 
-  struct WMap { const float* p; long long rs; int ld, cols; };
-  std::vector<WMap> wmaps;                 // weight-gradient operands [B rows][cols] that get a tensor map
-  struct FMap { int64_t off; int K, N, ld; };
-  std::vector<FMap> fmaps;                 // forward weight matrices that need a tensor map (one per chained forward stage)
   if (h->env.chain_dbg) {
     CU(cudaMalloc(h->chain_dbg.put(), sizeof(long long) * CH_DBG_SLOTS * 16));
     CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
@@ -1265,8 +1273,6 @@ int PlanBuilder::build_plan_fused() {
       const LayerOff& lo = net[lyr];
       ChainStage& S = st[lyr];
       S.W = W(lo.w); S.bias = W(lo.b); S.ldw = lo.ld; S.K = lo.in; S.N = lo.out;
-      S.tm_idx = (int)fmaps.size();
-      fmaps.push_back(FMap{lo.w, lo.in, lo.out, lo.ld});
       if (store) { S.out = (*store)[lyr].p + store_row * lo.out; S.rsOut = (*store)[lyr].rs; S.ldo = lo.out; }
     }
   };
@@ -1284,48 +1290,68 @@ int PlanBuilder::build_plan_fused() {
       if (dstore) { S.out = (*dstore)[lyr - 1].p + drow * lo.in; S.rsOut = (*dstore)[lyr - 1].rs; S.ldo = lo.in; }
     }
   };
-  // chain_kernel launch; its jobs are filled by the caller, then finish_chain sizes the grid
-  auto new_chain = [&](const char* label, int njobs, int early_weights) {
-    Launch l;
-    l.kind = L_CHAIN;
-    l.label = label;
-    memset(&l.chain, 0, sizeof(l.chain));
-    l.chain.njobs = njobs;
-    l.chain.early_weights = early_weights;
-    l.chain.rsP = rsP;
-    l.chain.pol = h->pol;
-    l.chain.rw = rw;
-    l.block = dim3(CH_BLOCK);
-    l.smem = CH_SMEM_BYTES;
-    return l;
+  // Tensor maps [R][n] of the forward stages fs (W [N][K] row-major, pitch ldw, box {32 k, N rows}, SWIZZLE_128B, OOB k
+  // zero-filled), owned by the handle: stage i of replica r reads tm + r * n
+  auto map_weights = [&](const std::vector<ChainStage*>& fs) {
+    const int n = (int)fs.size();
+    std::vector<CUtensorMap> maps((size_t)R * n);
+    for (int rep = 0; rep < R; ++rep)
+      for (int i = 0; i < n; ++i)
+        if (int e = make_map(&maps[(size_t)rep * n + i], fs[i]->W + (long long)rep * rsP, fs[i]->K, fs[i]->N, fs[i]->ldw, fs[i]->N)) rc = e;
+    const CUtensorMap* tm = upload(h->tmaps, maps);
+    for (int i = 0; i < n; ++i) { fs[i]->tm = tm + i; fs[i]->rsTm = n; }
   };
-  auto finish_chain = [&](Launch& l) {
-    l.chain.dbg = dbg_slot();
+  // chain_kernel launch; its jobs are filled by the caller, then finish_chain sizes the grid and appends it
+  auto new_chain = [&](int njobs, int early_weights) {
+    ChainArgs P;
+    memset(&P, 0, sizeof(P));
+    P.njobs = njobs;
+    P.early_weights = early_weights;
+    P.rsP = rsP;
+    P.pol = h->pol;
+    P.rw = rw;
+    return P;
+  };
+  auto finish_chain = [&](const char* label, ChainArgs& P) {
+    const bool fwd = P.job[0].kind == CJ_FWD;
+    if (fwd) {
+      std::vector<ChainStage*> fs;
+      for (int j = 0; j < P.njobs; ++j)
+        for (int s = 0; s < P.job[j].nstages; ++s) fs.push_back(&P.job[j].st[s]);
+      map_weights(fs);
+    }
+    P.dbg = dbg_slot();
     long long total = 0;
     int maxrows = 0;
-    for (int j = 0; j < l.chain.njobs; ++j) {
-      total += l.chain.job[j].rows;
-      maxrows = std::max(maxrows, l.chain.job[j].rows);
+    for (int j = 0; j < P.njobs; ++j) {
+      total += P.job[j].rows;
+      maxrows = std::max(maxrows, P.job[j].rows);
     }
-    l.bn = chain_rows(total, 1, R, sms);           // (bn is reused as "rows per CTA" for chain launches)
-    l.grid = dim3(std::max(1, (maxrows + l.bn - 1) / l.bn), l.chain.njobs, R);
-    h->plan.push_back(l);
+    const int rows = chain_rows(total, 1, R, sms);
+    Launch l;
+    l.label = label;
+    l.grid = dim3(std::max(1, (maxrows + rows - 1) / rows), P.njobs, R);
+    l.block = dim3(CH_BLOCK);
+    l.smem = CH_SMEM_BYTES;
+    push(std::move(l), with_chain_rows(rows, [&](auto r) {
+           constexpr int ROWS = decltype(r)::value;
+           return fwd ? chain_kernel<true, ROWS> : chain_kernel<false, ROWS>;
+         }), P);
   };
   // chain2_kernel launch: forward of the twins fnet[0..1] on X, their head values swapped, backward of the local critics
   auto pair_launch = [&](const char* label, int kind, int early, const std::vector<LayerOff>* fnet /* [2] */, const float* X, long long rsX,
                          const std::vector<Buf>* fstore, const Buf& qf, const std::vector<Buf>& acts, const std::vector<Buf>* dstore,
                          bool tail) {
-    Launch l;
-    l.kind = L_CHAIN2;
-    l.label = label;
-    memset(&l.chain2, 0, sizeof(l.chain2));
-    Chain2Args& P = l.chain2;
+    Chain2Args P;
+    memset(&P, 0, sizeof(P));
     P.kind = kind; P.rsP = rsP; P.rw = rw;
     P.early_weights = early;
+    std::vector<ChainStage*> fs;
     for (int net = 0; net < 2; ++net) {
       Chain2Job& J = P.job[net];
       J.rows = B; J.nfwd = Lc; J.nbwd = Lc - 1; J.net = net;
       fwd_stages(J, J.st, fnet[net], Lc, X, rsX, h->K.ldx, h->K.xw, fstore, (long long)net * B);
+      for (int s = 0; s < Lc; ++s) fs.push_back(&J.st[s]);
       const LayerOff& fh = fnet[net][Lc];
       J.Whf = W(fh.w); J.bhf = W(fh.b); J.Hhf = fh.in;
       J.qf_out = qf.p + (long long)net * B; J.rsQf = qf.rs;
@@ -1339,44 +1365,51 @@ int PlanBuilder::build_plan_fused() {
         J.dx = h->dxP.p + (long long)net * B * h->K.ldx; J.rsDx = h->dxP.rs; J.lddx = h->K.ldx;
       }
     }
+    map_weights(fs);
     P.dbg = dbg_slot();
-    l.bn = chain_rows(B, 2, R, sms);
-    l.grid = dim3((B + l.bn - 1) / l.bn, 2, R);
+    const int rows = chain_rows(B, 2, R, sms);
+    Launch l;
+    l.label = label;
+    l.critic_loss = kind == C2_CRITIC;
+    l.grid = dim3((B + rows - 1) / rows, 2, R);
     l.block = dim3(CH_BLOCK);
     l.smem = C2_SMEM_BYTES;
-    h->plan.push_back(l);
+    l.cluster_y = 2;
+    push(std::move(l), with_chain_rows(rows, [&](auto r) {
+           constexpr int ROWS = decltype(r)::value;
+           return kind == C2_ACTORQ ? chain2_kernel<ROWS, true> : chain2_kernel<ROWS, false>;
+         }), P);
   };
-  // weight-gradient launch of a group of networks; the CTA that reduces a gradient tile applies Adam (+ Polyak) to it
+  // weight-gradient launch of a group of networks; the CTA that reduces a gradient tile applies Adam (+ Polyak) to it,
+  // unless store_only (the gradients alone, no optimizer step: grad_clip plans)
   struct WNet { const std::vector<LayerOff>* net; int nh; const std::vector<Buf>* dstore; const std::vector<Buf>* acts; long long act_row_off;
                 const float* X; long long rsX; int ldx; const float* dout; long long rsDout; int lddout; int net_idx; };
   auto wgrad_launch = [&](const std::vector<WNet>& nets, const char* label, int which, bool store_only) -> int {
-    Launch l;
-    l.kind = L_WGRAD;
-    l.label = label;
-    l.store_only = store_only;
-    memset(&l.wg, 0, sizeof(l.wg));
-    l.wg.M = B; l.wg.rsG = rsG;
-    WgradAdam& O = l.wg.adam;
+    WgradArgs P;
+    memset(&P, 0, sizeof(P));
+    P.M = B; P.rsG = rsG;
+    WgradAdam& O = P.adam;
     O.which = which;
     O.params = h->params; O.m = h->adam_m; O.v = h->adam_v; O.grads = h->grads;
     O.rsP = rsP; O.rsM = rsG;
     O.target_delta = which == 0 ? L.target_delta : 0;
     O.cnt = h->cnt;
     int tiles = 0;
+    // operands a tensor map can address (16-byte row pitch and base) arrive by TMA, the others are staged by the threads
+    struct Operand { const CUtensorMap** tm; const float* p; long long rs; int ld, cols; };
+    std::vector<Operand> ops;
     auto add = [&](const float* Ap, long long rsA, int lda, const float* Bp, long long rsB, int ldb, int64_t offW, int ldc, int64_t offB,
                    int Kout, int Nin) -> int {
-      if (l.wg.njobs >= WG_MAXJOBS) return fail(B200SAC_ERR_INVALID, "too many weight-gradient jobs in one launch");
-      WgradJob& J = l.wg.job[l.wg.njobs++];
+      if (P.njobs >= WG_MAXJOBS) return fail(B200SAC_ERR_INVALID, "too many weight-gradient jobs in one launch");
+      WgradJob& J = P.job[P.njobs++];
       J.A = Ap; J.rsA = rsA; J.lda = lda; J.B = Bp; J.rsB = rsB; J.ldb = ldb;
       J.C = Gp(offW); J.C2 = Gp(offB); J.ldc = ldc; J.Kout = Kout; J.Nin = Nin;
       J.tile0 = tiles; J.tn = (Nin + WG_T - 1) / WG_T;
       J.shape = Kout <= 4 ? WG_KTHIN : (Nin <= 16 ? WG_NTHIN : WG_FULL);
       tiles += J.tn * ((Kout + WG_T - 1) / WG_T);
-      // operands a tensor map can address (16-byte row pitch and base) arrive by TMA, the others are staged by the threads
       auto tmable = [&](const float* p_, long long rs_, int ld_) { return (ld_ % 4) == 0 && (((uintptr_t)p_) & 15) == 0 && (rs_ % 4) == 0; };
-      J.tmA_idx = J.tmB_idx = -1;
-      if (tmable(Ap, rsA, lda)) { J.tmA_idx = (int)wmaps.size(); wmaps.push_back(WMap{Ap, rsA, lda, Kout}); }
-      if (tmable(Bp, rsB, ldb)) { J.tmB_idx = (int)wmaps.size(); wmaps.push_back(WMap{Bp, rsB, ldb, Nin}); }
+      if (tmable(Ap, rsA, lda)) ops.push_back(Operand{&J.tmA, Ap, rsA, lda, Kout});
+      if (tmable(Bp, rsB, ldb)) ops.push_back(Operand{&J.tmB, Bp, rsB, ldb, Nin});
       return 0;
     };
     for (const WNet& n : nets) {
@@ -1398,19 +1431,31 @@ int PlanBuilder::build_plan_fused() {
       const float* Bp = ab.p + ((long long)n.net_idx * B + n.act_row_off) * hd.in;
       if (int rc = add(n.dout, n.rsDout, n.lddout, Bp, ab.rs, hd.in, hd.w, hd.in, hd.b, hd.out, hd.in)) return rc;
     }
+    // maps [R][n] of the operands, [B rows][cols] row-major, box {32 cols, 256 rows}, dense: operand i of replica r at tm + r * n
+    const int n = (int)ops.size();
+    std::vector<CUtensorMap> maps((size_t)R * n);
+    for (int rep = 0; rep < R; ++rep)
+      for (int i = 0; i < n; ++i)
+        if (int rc = make_map(&maps[(size_t)rep * n + i], ops[i].p + (long long)rep * ops[i].rs, ops[i].cols, B, ops[i].ld, WG_ROWS, true))
+          return rc;
+    const CUtensorMap* tm = upload(h->tmaps, maps);
+    for (int i = 0; i < n; ++i) *ops[i].tm = tm + i;
+    for (int j = 0; j < P.njobs; ++j) P.job[j].rsTm = n;
+    P.dbg = dbg_slot();
+    Launch l;
+    l.label = label;
     l.grid = dim3(tiles, R);
     l.block = dim3(WG_THREADS);
     l.smem = WG_SMEM_BYTES;
-    l.wg.dbg = dbg_slot();
-    h->plan.push_back(l);
+    push(std::move(l), store_only ? wgrad_kernel<true> : wgrad_kernel<false>, P);
     return 0;
   };
 
   // ---- A: actor over [s';s], Q1/Q2 over (s,a) ----------------------------------------------------------------------
   {
-    Launch l = new_chain("chain_fwd{actor,q1,q2}", 3, 1);
+    ChainArgs P = new_chain(3, 1);
     for (int j = 0; j < 3; ++j) {
-      ChainJob& J = l.chain.job[j];
+      ChainJob& J = P.job[j];
       const int net = j - 1;
       const std::vector<LayerOff>& mlp = j == 0 ? L.actor : L.q[net];
       const int nh = j == 0 ? La : Lc;
@@ -1425,7 +1470,7 @@ int PlanBuilder::build_plan_fused() {
       const LayerOff& hd = mlp[nh];
       J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
     }
-    finish_chain(l);
+    finish_chain("chain_fwd{actor,q1,q2}", P);
   }
   // ---- B + C: target critics over (s', a'), TD target, critic backward (one clustered launch), weight gradients, Adam ----
   pair_launch("chain2{qt->y->bwd q}", C2_CRITIC, 1, L.qt, h->XT.p, h->XT.rs, nullptr, h->qt, h->hQ, &h->dhQ, false);
@@ -1447,13 +1492,13 @@ int PlanBuilder::build_plan_fused() {
   adam(1, true);
   // ---- E: policy backward, weight gradients, Adam ----------------------------------------------------------------------
   {
-    Launch l = new_chain("chain_bwd{actor}", 1, 1);
-    ChainJob& J = l.chain.job[0];
+    ChainArgs P = new_chain(1, 1);
+    ChainJob& J = P.job[0];
     J.kind = CJ_BWD_POLICY; J.rows = B; J.nstages = La - 1;
     const LayerOff& hd = L.actor[La];
     J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
     bwd_stages(J, J.st, L.actor, La, h->hA, (long long)B, &h->dhA, 0);
-    finish_chain(l);
+    finish_chain("chain_bwd{actor}", P);
     std::vector<WNet> nets;
     nets.push_back(WNet{&L.actor, La, &h->dhA, &h->hA, (long long)B, h->XA.p + (long long)B * h->K.ldxa, h->XA.rs, h->K.ldxa,
                         h->dout_dbg.p, h->dout_dbg.rs, 2 * A, 0});
@@ -1463,53 +1508,6 @@ int PlanBuilder::build_plan_fused() {
     grad_norm(1);
     adam(1, false, false);
   }
-  // ---- tensor maps ---------------------------------------------------------------------------------------------------
-  // forward weights [R][nf]: W [N][K] row-major (pitch ld), box {32 k, N rows}, SWIZZLE_128B, OOB k zero-filled;
-  // weight-gradient operands [R][nw]: [B rows][cols] row-major, box {32 cols, 256 rows}, dense
-  const int nf = (int)fmaps.size(), nw = (int)wmaps.size();
-  std::vector<CUtensorMap> maps((size_t)R * (nf + nw));
-  for (int rep = 0; rep < R; ++rep) {
-    for (int i = 0; i < nf; ++i)
-      if (int rc = make_map(&maps[(size_t)rep * nf + i], h->params + (long long)rep * rsP + fmaps[i].off, fmaps[i].K, fmaps[i].N,
-                            fmaps[i].ld, fmaps[i].N))
-        return rc;
-    for (int i = 0; i < nw; ++i)
-      if (int rc = make_map(&maps[(size_t)R * nf + (size_t)rep * nw + i], wmaps[i].p + (long long)rep * wmaps[i].rs, wmaps[i].cols, B,
-                            wmaps[i].ld, WG_ROWS, true))
-        return rc;
-  }
-  CU(cudaMalloc(h->d_cmaps.put(), maps.size() * sizeof(CUtensorMap)));
-  CU(cudaMemcpy(h->d_cmaps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
-  const CUtensorMap* fmap = h->d_cmaps;
-  const CUtensorMap* wmap = h->d_cmaps + (size_t)R * nf;
-  auto patch = [&](ChainStage* st, int n) {
-    for (int s = 0; s < n; ++s) { st[s].tm = fmap + st[s].tm_idx; st[s].rsTm = nf; }
-  };
-  for (auto& l : h->plan) {
-    if (l.kind == L_CHAIN && l.chain.job[0].kind == CJ_FWD)
-      for (int j = 0; j < l.chain.njobs; ++j) patch(l.chain.job[j].st, l.chain.job[j].nstages);
-    if (l.kind == L_CHAIN2)
-      for (int j = 0; j < 2; ++j) patch(l.chain2.job[j].st, l.chain2.job[j].nfwd);
-    if (l.kind == L_WGRAD)
-      for (int j = 0; j < l.wg.njobs; ++j) {
-        WgradJob& J = l.wg.job[j];
-        J.tmA = J.tmA_idx >= 0 ? wmap + J.tmA_idx : nullptr;
-        J.tmB = J.tmB_idx >= 0 ? wmap + J.tmB_idx : nullptr;
-        J.rsTm = nw;
-      }
-  }
-  for (int bn : {8, 4, 2})
-    if (int rc = with_chain_rows(bn, [](auto rows) -> int {
-          constexpr int r = decltype(rows)::value;
-          CU(cudaFuncSetAttribute(chain_kernel<true, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-          CU(cudaFuncSetAttribute(chain_kernel<false, r>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)CH_SMEM_BYTES));
-          CU(cudaFuncSetAttribute(chain2_kernel<r, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
-          CU(cudaFuncSetAttribute(chain2_kernel<r, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)C2_SMEM_BYTES));
-          return 0;
-        }))
-      return rc;
-  CU(cudaFuncSetAttribute(wgrad_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
-  CU(cudaFuncSetAttribute(wgrad_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)WG_SMEM_BYTES));
   return 0;
 }
 
@@ -1551,12 +1549,10 @@ void PlanBuilder::build_plan_layered() {
   }
   {  // policy head
     Launch l;
-    l.kind = L_POLICY;
     l.label = "policy_head";
     l.grid = dim3((2 * B + 7) / 8, R);
     l.block = dim3(256);
-    l.pol = h->pol;
-    h->plan.push_back(l);
+    push(std::move(l), policy_head_kernel, h->pol);
   }
   // ---- Phase B: target critics over (s2, a') ---------------------------------------------
   for (int l = 0; l < Lc; ++l) {
@@ -1571,12 +1567,12 @@ void PlanBuilder::build_plan_layered() {
   const int Hc = c.critic_hidden[Lc - 1];
   {  // critic heads: y, Q1, Q2, dQ
     Launch l;
-    l.kind = L_CHEADS;
     l.label = "critic_heads";
     l.join = true;                 // needs Q1,Q2 on (s,a), which may have run on the fork stream
+    l.critic_loss = true;
     l.grid = dim3((B + 7) / 8, R);
     l.block = dim3(256);
-    CriticHeadArgs& P = l.ch;
+    CriticHeadArgs P;
     memset(&P, 0, sizeof(P));
     P.hT = h->hT[Lc - 1].p; P.hQ = h->hQ[Lc - 1].p; P.rsHnet = (long long)B * Hc; P.rsHrep = h->hT[Lc - 1].rs; P.ldh = Hc;
     for (int net = 0; net < 2; ++net) {
@@ -1588,7 +1584,7 @@ void PlanBuilder::build_plan_layered() {
     P.logp = h->logp.p; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
     P.y = h->y.p; P.q = h->q.p; P.dq = h->dq.p; P.lq = h->lq.p; P.rsY = h->y.rs;
-    h->plan.push_back(l);
+    push(std::move(l), critic_heads_kernel, P);
   }
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
@@ -1622,9 +1618,8 @@ void PlanBuilder::build_plan_layered() {
   if (c.care) {
     {  // backward of the attention mix: dZk, d(att)
       Launch l;
-      l.kind = L_CARE_MIXBWD;
       l.label = "care_mix_bwd";
-      CareMixBwdArgs& P = l.cmixb;
+      CareMixBwdArgs P;
       memset(&P, 0, sizeof(P));
       P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
       P.Z = h->mixZ[0].p; P.rsZ = h->mixZ[0].rs; P.kstride = (long long)2 * B * pitch(c.mix_out); P.ldz = pitch(c.mix_out);
@@ -1636,7 +1631,7 @@ void PlanBuilder::build_plan_layered() {
       P.B = B; P.K = Kenc; P.mo = c.mix_out; P.co = c.ctx_out;
       l.grid = dim3((B + 7) / 8, R);
       l.block = dim3(256);
-      h->plan.push_back(l);
+      push(std::move(l), care_mix_bwd_kernel, P);
     }
     for (int l = nmix - 1; l >= 0; --l) {          // mixture-of-encoders backward, K problems per kind
       std::vector<GemmProb> ps;
@@ -1672,9 +1667,8 @@ void PlanBuilder::build_plan_layered() {
     }
     {  // per-task reduction + softmax backward, then the trunk / context-MLP weight gradients
       Launch l;
-      l.kind = L_CARE_TABRED;
       l.label = "care_tab_reduce";
-      CareTabReduceArgs& P = l.ctred;
+      CareTabReduceArgs P;
       memset(&P, 0, sizeof(P));
       P.datt = h->careDatt.p; P.rsDatt = h->careDatt.rs;
       P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
@@ -1684,11 +1678,10 @@ void PlanBuilder::build_plan_layered() {
       P.B = B; P.K = Kenc; P.co = c.ctx_out;
       l.grid = dim3(c.num_tasks, R);
       l.block = dim3(1024);
-      h->plan.push_back(l);
+      push(std::move(l), care_tab_reduce_kernel, P);
       Launch l2;
-      l2.kind = L_CARE_TABWG;
       l2.label = "care_tab_wgrad";
-      CareTabWgradArgs& Q = l2.ctwg;
+      CareTabWgradArgs Q;
       memset(&Q, 0, sizeof(Q));
       Q.params = h->params; Q.rsP = rsP; Q.emb_off = L.off_emb;
       Q.tab = h->careTab[0].p; Q.rsTab = h->careTab[0].rs; Q.row_w = h->care_row_w;
@@ -1705,7 +1698,7 @@ void PlanBuilder::build_plan_layered() {
       l2.smem = (size_t)Q.tchunk * fl * sizeof(float);
       l2.grid = dim3(sms, R);
       l2.block = dim3(256);
-      h->plan.push_back(l2);
+      push(std::move(l2), care_tab_wgrad_kernel, Q);
     }
   }
   if (c.grad_clip) grad_norm(0);
@@ -1730,11 +1723,10 @@ void PlanBuilder::build_plan_layered() {
   }
   {
     Launch l;
-    l.kind = L_AQHEADS;
     l.label = "actor_q_heads";
     l.grid = dim3((B + 7) / 8, R);
     l.block = dim3(256);
-    ActorQHeadArgs& P = l.aq;
+    ActorQHeadArgs P;
     memset(&P, 0, sizeof(P));
     P.hP = h->hP[Lc - 1].p; P.rsHnet = (long long)B * Hc; P.rsHrep = h->hP[Lc - 1].rs; P.ldh = Hc;
     for (int net = 0; net < 2; ++net) { P.Wq[net] = W(L.q[net][Lc].w); P.bq[net] = W(L.q[net][Lc].b); }
@@ -1743,7 +1735,7 @@ void PlanBuilder::build_plan_layered() {
     P.logp = h->logp.p + B; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
     P.dqa = h->dqa.p; P.la = h->la.p; P.qmin = h->qmin.p; P.rsY = h->y.rs;
-    h->plan.push_back(l);
+    push(std::move(l), actor_q_heads_kernel, P);
   }
   head_bwd(false, false);
   for (int l = Lc - 1; l >= 0; --l) {
@@ -1811,38 +1803,24 @@ static int build_plan(b200sac* h) {
   } else {
     pb.build_plan_layered();
   }
-  if (pb.rc) return pb.rc;
-  // the wgmma launches' problem table (run_plan hands each launch its slice)
-  if (!h->h_tprobs.empty()) {
-    CU(cudaMalloc(h->d_tprobs.put(), h->h_tprobs.size() * sizeof(TcProb)));
-    CU(cudaMemcpy(h->d_tprobs, h->h_tprobs.data(), h->h_tprobs.size() * sizeof(TcProb), cudaMemcpyHostToDevice));
-    CU(tc_set_attrs());
-  }
-  size_t max_smem = 0;
-  for (auto& l : h->plan)
-    if (l.kind == L_HEADBWD && l.smem > max_smem) max_smem = l.smem;
-  if (max_smem > 200 * 1024) return fail(B200SAC_ERR_INVALID, "batch * head width too large for head_bwd smem");
-  CU(cudaFuncSetAttribute(head_bwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
-  CU(cudaFuncSetAttribute(head_bwd4_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)max_smem));
-  if (h->cfg.pcgrad)
-    CU(cudaFuncSetAttribute(pcgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)pcgrad_smem(h->cfg.num_tasks)));
-  return 0;
+  return pb.rc;
 }
 
 // Launch with programmatic stream serialization (PDL): the kernel may start while its predecessor
 // drains; every kernel begins with griddepcontrol.wait (common.cuh::kstamp), so data dependencies hold.
-// CLUSTER_Y > 1: thread-block clusters of (1, CLUSTER_Y, 1) -- the CTAs with equal blockIdx.x / z are co-scheduled and can
+// cluster_y > 1: thread-block clusters of (1, cluster_y, 1) -- the CTAs with equal blockIdx.x / z are co-scheduled and can
 // read each other's shared memory.
-template <int CLUSTER_Y = 1, typename... KArgs, typename... Args>
-static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
+template <typename... KArgs, typename... Args>
+static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, int cluster_y, cudaStream_t st,
+                            Args... args) {
   cudaLaunchConfig_t cfg;
   memset(&cfg, 0, sizeof(cfg));
   cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
   cudaLaunchAttribute attr[2];
   int n = 0;
-  if (CLUSTER_Y > 1) {
+  if (cluster_y > 1) {
     attr[n].id = cudaLaunchAttributeClusterDimension;
-    attr[n].val.clusterDim.x = 1; attr[n].val.clusterDim.y = CLUSTER_Y; attr[n].val.clusterDim.z = 1;
+    attr[n].val.clusterDim.x = 1; attr[n].val.clusterDim.y = cluster_y; attr[n].val.clusterDim.z = 1;
     ++n;
   }
   attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -1855,13 +1833,34 @@ static cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
 
 // Prioritized replay: the draw of one step (indices into rb->d_idx, importance weights into the handle's per_buf).
 static cudaError_t per_sample_on(b200sac* h, b200sac_replay* rb, cudaStream_t s) {
-  return launch_k(per_sample_kernel, dim3(h->R), dim3(h->cfg.batch > 256 ? 512 : 256), 0, s, h->K, rb->tr, (const Counters*)h->cnt,
+  return launch_k(per_sample_kernel, dim3(h->R), dim3(h->cfg.batch > 256 ? 512 : 256), 0, 1, s, h->K, rb->tr, (const Counters*)h->cnt,
                   0LL, 0, (const long long*)rb->d_fill, (const double*)rb->beta.dev, rb->d_idx.get(), h->per_buf.get(), (long long)h->cfg.batch,
                   rb->seed);
 }
 
-// The launch whose rows carry the step's TD target and pre-update critic values (the priority update follows it).
-static bool forms_critic_loss(const Launch& l) { return l.kind == L_CHEADS || (l.kind == L_CHAIN2 && l.chain2.kind == C2_CRITIC); }
+// What a plan launch takes from the step when it runs: the StepConst, and the noise source (use_eps_buf) of the two
+// argument blocks that carry it.  Every other argument block runs as its builder left it.
+template <class P> static const P& with_noise(const P& a, int) { return a; }
+static PolicyHeadArgs with_noise(PolicyHeadArgs a, int use_eps_buf) { a.use_eps_buf = use_eps_buf; return a; }
+static ChainArgs with_noise(ChainArgs a, int use_eps_buf) { a.pol.use_eps_buf = use_eps_buf; return a; }
+struct RunLaunch {
+  const Launch& l;
+  cudaStream_t s;
+  const StepConst& K;
+  int use_eps_buf;
+  template <class P> cudaError_t operator()(const StepFirst<P>& c) const {
+    return launch_k(c.kern, l.grid, l.block, l.smem, l.cluster_y, s, K, with_noise(c.args, use_eps_buf));
+  }
+  template <class P> cudaError_t operator()(const StepLast<P>& c) const {
+    return launch_k(c.kern, l.grid, l.block, l.smem, l.cluster_y, s, with_noise(c.args, use_eps_buf), K);
+  }
+  template <class P> cudaError_t operator()(const NoStep<P>& c) const {
+    return launch_k(c.kern, l.grid, l.block, l.smem, l.cluster_y, s, c.args);
+  }
+  cudaError_t operator()(const TcCall& c) const {
+    return launch_k(c.kern, l.grid, l.block, l.smem, l.cluster_y, s, c.probs, c.sched, c.G, c.sched_stride);
+  }
+};
 
 // rb: the device ring of a sampled step.  Prioritized ring -- the critic loss is importance-weighted and the priority update
 // runs after the critic-loss launch (forked off the critical path when allow_fork, joined before the step ends); per_next:
@@ -1888,88 +1887,12 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
       CU(cudaStreamWaitEvent(h->fork, h->ev_fork_src, 0));
       s = h->fork;
     }
-    switch (l.kind) {
-      case L_POLICY_DOUT:
-        launch_k(policy_dout_kernel, l.grid, l.block, 0, s, K, l.pdo);
-        break;
-      case L_CARE_TAB:
-        launch_k(care_tables_kernel, l.grid, l.block, 0, s, l.ctab);
-        break;
-      case L_CARE_MIX:
-        launch_k(care_mix_kernel, l.grid, l.block, 0, s, l.cmix);
-        break;
-      case L_CARE_MIXFWD:
-        launch_k(care_mixfwd_kernel, l.grid, l.block, l.smem, s, l.cmf);
-        break;
-      case L_CARE_MIXBWD:
-        launch_k(care_mix_bwd_kernel, l.grid, l.block, 0, s, l.cmixb);
-        break;
-      case L_CARE_TABRED:
-        launch_k(care_tab_reduce_kernel, l.grid, l.block, 0, s, l.ctred);
-        break;
-      case L_CARE_TABWG:
-        launch_k(care_tab_wgrad_kernel, l.grid, l.block, l.smem, s, l.ctwg);
-        break;
-      case L_GEMM_SMALL:
-        launch_k(gemm_simt_kernel, l.grid, l.block, 0, s, l.grp);
-        break;
-      case L_GEMM_THIN:
-        launch_k(gemm_thin_kernel, l.grid, l.block, 0, s, l.grp);
-        break;
-      case L_GEMM_TC:
-        launch_k(tc_kernel(l.bn, l.pair128), l.grid, l.block, l.smem, s, h->d_tprobs + l.tprob0, l.sched, l.G, kSchedStride);
-        break;
-      case L_POLICY: {
-        PolicyHeadArgs P = l.pol;
-        P.use_eps_buf = use_eps_buf ? 1 : 0;
-        launch_k(policy_head_kernel, l.grid, l.block, 0, s, K, P);
-        break;
-      }
-      case L_CHEADS:
-        launch_k(critic_heads_kernel, l.grid, l.block, 0, s, K, l.ch);
-        break;
-      case L_AQHEADS:
-        launch_k(actor_q_heads_kernel, l.grid, l.block, 0, s, K, l.aq);
-        break;
-      case L_HEADBWD:
-        if (l.bn == 4) launch_k(head_bwd4_kernel<1>, l.grid, l.block, l.smem, s, K, l.hb);
-        else launch_k(head_bwd_kernel, l.grid, l.block, l.smem, s, K, l.hb);
-        break;
-      case L_ADAM:
-        launch_k(l.ad.pcw ? adam_kernel<false, true> : l.ad.coef ? adam_kernel<true> : adam_kernel<false>, l.grid, l.block, 0, s, K, l.ad);
-        break;
-      case L_PCGRAD:
-        launch_k(pcgrad_kernel, l.grid, l.block, l.smem, s, K, l.pc);
-        break;
-      case L_GRADNORM:
-        launch_k(grad_sqnorm_kernel, l.grid, l.block, 0, s, K, l.gn);
-        break;
-      case L_CHAIN: {
-        ChainArgs a = l.chain;
-        a.pol.use_eps_buf = use_eps_buf ? 1 : 0;
-        const bool f = a.job[0].kind == CJ_FWD;
-        with_chain_rows(l.bn, [&](auto rows) {
-          constexpr int r = decltype(rows)::value;
-          return launch_k(f ? chain_kernel<true, r> : chain_kernel<false, r>, l.grid, l.block, l.smem, s, a, K);
-        });
-        break;
-      }
-      case L_WGRAD:
-        launch_k(l.store_only ? wgrad_kernel<true> : wgrad_kernel<false>, l.grid, l.block, l.smem, s, l.wg, K);
-        break;
-      case L_CHAIN2:
-        with_chain_rows(l.bn, [&](auto rows) {
-          constexpr int r = decltype(rows)::value;
-          return launch_k<2>(l.chain2.kind == C2_ACTORQ ? chain2_kernel<r, true> : chain2_kernel<r, false>, l.grid, l.block, l.smem, s,
-                             l.chain2, K);
-        });
-        break;
-    }
+    std::visit(RunLaunch{l, s, K, use_eps_buf ? 1 : 0}, l.call);
     if (forked) {
       CU(cudaEventRecord(h->ev_fork_done, h->fork));
       fork_pending = true;
     }
-    if (per && forms_critic_loss(l)) {
+    if (per && l.critic_loss) {
       cudaStream_t ps = st;
       if (allow_fork) {
         CU(cudaEventRecord(h->ev_per_src, s));
@@ -1977,7 +1900,7 @@ static int run_plan(b200sac* h, cudaStream_t st, bool use_eps_buf, const Event* 
         ps = h->per_fork;
       }
       const int B = h->cfg.batch, R = h->R;
-      launch_k(per_update_kernel, dim3(R), dim3(256), 0, ps, per->tr, 0, (const int*)per->d_idx, (long long)B, B,
+      launch_k(per_update_kernel, dim3(R), dim3(256), 0, 1, ps, per->tr, 0, (const int*)per->d_idx, (long long)B, B,
                (const float*)h->y.p, (const float*)h->q.p, h->y.rs, (const float*)nullptr, h->per_buf + (size_t)R * B,
                (int*)(h->per_buf + (size_t)2 * R * B), (long long)B);
       if (allow_fork) {
@@ -2644,7 +2567,7 @@ static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, const 
   if (grid.x > 64) grid.x = 64;
   b200sac_replay* rb = key.ring;
   if (!rb) {
-    launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, key.rows, (long long)B * h->row_stride, h->row_stride,
+    launch_k(ingest_rows_kernel, grid, block, 0, 1, st, h->K, h->ing, key.rows, (long long)B * h->row_stride, h->row_stride,
              (const int*)nullptr, (long long)0);
     if (key.eps && key.eps != h->eps.p) {      // staged eps, [R][B][A] next, then [R][B][A] cur: into the step's buffer
       const float* e = key.eps;
@@ -2658,16 +2581,16 @@ static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, const 
   } else {
     auto sample_on = [&](cudaStream_t s2) {
       if (rb->per) return per_sample_on(h, rb, s2);
-      return launch_k(sample_indices_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, s2, h->K,   // __launch_bounds__(512): 512 threads fit
+      return launch_k(sample_indices_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, 1, s2, h->K,   // __launch_bounds__(512): 512 threads fit
                       (const Counters*)h->cnt, (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx.get(), (long long)B, rb->seed);
     };
     if (sample_mode == SAMPLE_INLINE) sample_on(st);
     else CU(cudaStreamWaitEvent(st, h->ev_sampled, 0));
     if (rb->traj)                               // linked ring: the same gather with the n-step fold in front of the scatter
-      launch_k(ingest_nstep_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
+      launch_k(ingest_nstep_kernel, grid, block, 0, 1, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
                (const int*)rb->d_idx, (long long)B, nstep_ring(rb), h->ns_buf.get());
     else
-      launch_k(ingest_rows_kernel, grid, block, 0, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
+      launch_k(ingest_rows_kernel, grid, block, 0, 1, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
                (const int*)rb->d_idx, (long long)B);
     if (fork_next && !rb->per) {                // (prioritized: the next draw follows this step's priority update)
       CU(cudaEventRecord(h->ev_ingested, st));
@@ -2925,7 +2848,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   DevMem<TcProb> d;
   CU(cudaMalloc(d.put(), sizeof(TcProb)));
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
-  CU(tc_set_attrs());
+  CU(allow_smem((const void*)tc_kernel(bn, sw.pair128), tc_smem(bn)));
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
   cudaError_t e = cudaGetLastError();
@@ -2953,7 +2876,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   DevMem<TcProb> d;
   CU(cudaMalloc(d.put(), sizeof(TcProb)));
   CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
-  CU(tc_set_attrs());
+  CU(allow_smem((const void*)tc_kernel(bn, sw.pair128), tc_smem(bn)));
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   for (int it = 0; it < 3; ++it) tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
   CU(cudaDeviceSynchronize());

@@ -47,6 +47,7 @@ struct Chain2Args {
   Chain2Job job[2];
   ChainRows rw;
 };
+static_assert(sizeof(Chain2Args) == 3424, "chain2_kernel argument layout changed");
 
 B200_D void cluster_arrive_relaxed() { asm volatile("barrier.cluster.arrive.relaxed.aligned;" ::: "memory"); }
 B200_D void cluster_wait() { asm volatile("barrier.cluster.wait.aligned;" ::: "memory"); }
