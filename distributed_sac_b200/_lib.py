@@ -72,6 +72,10 @@ SYMBOLS = {
     "b200sac_get_pcgrad": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_read_pcgrad": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _VP]),
     "b200sac_export_task_grad": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, C.c_int64, _VP]),
+    "b200sac_set_cagrad": (C.c_int, [_VP, C.c_int32, C.c_double, C.c_double, _VP]),
+    "b200sac_get_cagrad": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
+    "b200sac_read_cagrad": (C.c_int, [_VP, C.c_int32] + [_VP] * 6 + [_VP]),
+    "b200sac_cagrad_solve_test": (C.c_int, [C.c_int32, _VP, C.c_double] + [_VP] * 7),
     "b200sac_step": (C.c_int, [_VP] + [_VP] * 7 + [_VP]),
     "b200sac_step_host": (C.c_int, [_VP] + [_VP] * 7 + [_VP, _VP]),
     "b200sac_step_sampled": (C.c_int, [_VP, _VP, C.c_int32, _VP]),

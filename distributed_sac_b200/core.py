@@ -394,6 +394,37 @@ class SacCore:
         projected = (mask[:, :, None] & bits[None, None, :]) != 0
         return {"gram": gram, "w": w, "perm": perm, "projected": projected, "task_mismatch": int(bad.value)}
 
+    # ---- CAGrad (b200sac_set/get/read_cagrad; handles with pcgrad=True) ---------------------------------------------
+    def get_cagrad(self, replica=0) -> Dict[str, float]:
+        """{critic, actor} CAGrad coefficients c of one replica (no synchronisation); 0 = off."""
+        c, a = C.c_double(0), C.c_double(0)
+        _lib.check(self.lib.b200sac_get_cagrad(self._h, int(replica), C.byref(c), C.byref(a)))
+        return {"critic": c.value, "actor": a.value}
+
+    def set_cagrad(self, critic=None, actor=None, replica=None):
+        """CAGrad coefficient c of the critic's / actor's optimizer for one replica (replica=None: all of them) on the
+        current stream; a value left out keeps its value.  c > 0: Adam reads the CAGrad combination of the task gradients
+        whatever the PCGrad switch says; 0 turns CAGrad off.  Steps enqueued afterwards use the new values."""
+        for r in _replicas(self.cfg.replicas, replica):
+            cur = self.get_cagrad(r)
+            for k, v in dict(critic=critic, actor=actor).items():
+                if v is not None:
+                    cur[k] = float(v)
+            _lib.check(self.lib.b200sac_set_cagrad(self._h, r, cur["critic"], cur["actor"], _stream()))
+
+    def read_cagrad(self, replica=0) -> Dict[str, np.ndarray]:
+        """The last step's CAGrad record of one replica, index 0 critic and 1 actor: p [2][T] (the dual's weights p*),
+        lambda, best (best objective F), first (F at uniform weights), scale (s) [2] fp64, and ibest [2] (the iteration of
+        the best F; -1 = CAGrad did not run, -2 = degenerate Gram matrix).  The weights Adam read are read_pcgrad()["w"]."""
+        T = self.cfg.num_tasks
+        p = np.empty((2, T), np.float64)
+        f = {k: np.empty(2, np.float64) for k in ("lambda", "best", "first", "scale")}
+        ib = np.empty(2, np.int32)
+        _lib.check(self.lib.b200sac_read_cagrad(self._h, int(replica), p.ctypes.data, f["lambda"].ctypes.data,
+                                                f["best"].ctypes.data, f["first"].ctypes.data, f["scale"].ctypes.data,
+                                                ib.ctypes.data, _stream()))
+        return dict(p=p, ibest=ib, **f)
+
     def export_task_grad(self, task: int, replica=0) -> torch.Tensor:
         """Gradient of the last step over the rows of task `task` alone (the trainable arena, CPU tensor)."""
         out = torch.empty(self.trainable_floats, dtype=torch.float32)

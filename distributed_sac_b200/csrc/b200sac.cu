@@ -453,6 +453,11 @@ struct b200sac {
   DevMem<int> pc_perm;
   DevMem<unsigned long long> pc_mask;
   DevMem<int> pc_bad;
+  // CAGrad on the same handles: [R][2] coefficients c (0 = off) and the last step's solve per replica and optimizer
+  // (p* [R][2][T], lambda / best F / first F / s [R][2][kCagScalars], ibest [R][2])
+  ReplicaTable<double, 2> cg_c;
+  DevMem<double> cg_p, cg_f;
+  DevMem<int> cg_it;
 
   // The members release their resources; the publication stream's last copy lands first.
   ~b200sac() {
@@ -1235,6 +1240,7 @@ void PlanBuilder::pcgrad(int which) {
   P.part = h->pc_part + (size_t)which * R * kGradNormMaxBlocks * pcgrad_pairs(T);
   P.ticket = h->pc_ticket + (size_t)which * R;
   P.G = h->pc_G; P.w = h->pc_w; P.perm = h->pc_perm; P.mask = h->pc_mask;
+  P.cac = h->cg_c.dev; P.cgp = h->cg_p; P.cgf = h->cg_f; P.cgi = h->cg_it;
   if (which == 0) { P.tid = (const int*)h->tid.p; P.rsR = h->r.rs; P.B = B; P.bad = h->pc_bad; }
   P.seed = h->K.seed;
   l.grid = dim3(elementwise_blocks(n), R);
@@ -2038,6 +2044,16 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMemset(h->pc_mask, 0, sizeof(unsigned long long) * n2 * T));
     CU(cudaMalloc(h->pc_bad.put(), sizeof(int) * R));
     CU(cudaMemset(h->pc_bad, 0, sizeof(int) * R));
+    const double off[2] = {0.0, 0.0};      // CAGrad off, its record NaN / -1 until a step runs it
+    if (int rc = h->cg_c.init(R, off)) return rc;
+    const std::vector<double> pnan(n2 * std::max(T, kCagScalars), NAN);
+    CU(cudaMalloc(h->cg_p.put(), sizeof(double) * n2 * T));
+    CU(cudaMemcpy(h->cg_p, pnan.data(), sizeof(double) * n2 * T, cudaMemcpyHostToDevice));
+    CU(cudaMalloc(h->cg_f.put(), sizeof(double) * n2 * kCagScalars));
+    CU(cudaMemcpy(h->cg_f, pnan.data(), sizeof(double) * n2 * kCagScalars, cudaMemcpyHostToDevice));
+    const std::vector<int> none(n2, -1);
+    CU(cudaMalloc(h->cg_it.put(), sizeof(int) * n2));
+    CU(cudaMemcpy(h->cg_it, none.data(), sizeof(int) * n2, cudaMemcpyHostToDevice));
   }
 
   // work slab.  Buffers that a kernel addresses with one replica stride get one length: rsX (XQ, XT, XP), rsR (r, d, tid),
@@ -2410,6 +2426,71 @@ extern "C" int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, 
   if (perm) CU(cudaMemcpy(perm, h->pc_perm + r2 * T * T, sizeof(int) * 2 * T * T, cudaMemcpyDeviceToHost));
   if (mask) CU(cudaMemcpy(mask, h->pc_mask + r2 * T, sizeof(uint64_t) * 2 * T, cudaMemcpyDeviceToHost));
   if (task_mismatch) CU(cudaMemcpy(task_mismatch, h->pc_bad + replica, sizeof(int), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// CAGrad coefficients, read by the pcgrad launches of the step graphs.
+extern "C" int b200sac_get_cagrad(b200sac_t* h, int32_t replica, double* c_critic, double* c_actor) {
+  if (!h || !c_critic || !c_actor) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = h->cg_c.check(replica)) return rc;
+  *c_critic = h->cg_c.row(replica)[0]; *c_actor = h->cg_c.row(replica)[1];
+  return 0;
+}
+
+extern "C" int b200sac_set_cagrad(b200sac_t* h, int32_t replica, double c_critic, double c_actor, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = h->cg_c.check(replica)) return rc;
+  if (!(c_critic >= 0.0) || !(c_actor >= 0.0) || std::isinf(c_critic) || std::isinf(c_actor))   // (NaN fails >=)
+    return fail(B200SAC_ERR_INVALID, "CAGrad coefficients must be finite and >= 0, got %g, %g", c_critic, c_actor);
+  const double v[2] = {c_critic, c_actor};
+  return h->cg_c.set(h, stream, replica, v);
+}
+
+extern "C" int b200sac_read_cagrad(b200sac_t* h, int32_t replica, double* p, double* lambda, double* best, double* first,
+                                   double* scale, int32_t* ibest, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  const size_t T = (size_t)h->cfg.num_tasks, r2 = (size_t)replica * 2;
+  CU(cudaSetDevice(h->device));
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
+  double f[2][kCagScalars];
+  CU(cudaMemcpy(f, h->cg_f + r2 * kCagScalars, sizeof(f), cudaMemcpyDeviceToHost));
+  if (p) CU(cudaMemcpy(p, h->cg_p + r2 * T, sizeof(double) * 2 * T, cudaMemcpyDeviceToHost));
+  if (ibest) CU(cudaMemcpy(ibest, h->cg_it + r2, sizeof(int) * 2, cudaMemcpyDeviceToHost));
+  double* outs[kCagScalars] = {lambda, best, first, scale};
+  for (int k = 0; k < kCagScalars; ++k)
+    if (outs[k]) for (int o = 0; o < 2; ++o) outs[k][o] = f[o][k];
+  return 0;
+}
+
+// Stand-alone CAGrad solve (cagrad_test_kernel) on a HOST G [T][T] on the current device, like b200sac_gemm_test; outputs
+// as in b200sac_read_cagrad for one optimizer.
+extern "C" int b200sac_cagrad_solve_test(int32_t T, const double* G, double c, float* w, double* p, double* lambda,
+                                         double* best, double* first, double* scale, int32_t* ibest) {
+  if (!G || !w || T < 1 || T > kPcMaxTasks) return fail(B200SAC_ERR_INVALID, "bad argument (T in [1, %d], G and w non-null)", kPcMaxTasks);
+  if (!(c > 0.0) || std::isinf(c)) return fail(B200SAC_ERR_INVALID, "c must be finite and > 0, got %g", c);
+  const size_t nG = (size_t)T * T;
+  DevMem<double> dG, dp, df;
+  DevMem<float> dw;
+  DevMem<int> di;
+  CU(cudaMalloc(dG.put(), sizeof(double) * nG)); CU(cudaMalloc(dp.put(), sizeof(double) * T));
+  CU(cudaMalloc(df.put(), sizeof(double) * kCagScalars)); CU(cudaMalloc(dw.put(), sizeof(float) * T));
+  CU(cudaMalloc(di.put(), sizeof(int)));
+  CU(cudaMemcpy(dG, G, sizeof(double) * nG, cudaMemcpyHostToDevice));
+  cagrad_test_kernel<<<1, 32, sizeof(double) * (nG + kCagVecs * T), cudaStreamLegacy>>>(dG, T, c, CagOut{dw, dp, df, di});
+  CU(cudaGetLastError());
+  CU(cudaStreamSynchronize(cudaStreamLegacy));
+  double f[kCagScalars];
+  CU(cudaMemcpy(w, dw, sizeof(float) * T, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(f, df, sizeof(f), cudaMemcpyDeviceToHost));
+  if (p) CU(cudaMemcpy(p, dp, sizeof(double) * T, cudaMemcpyDeviceToHost));
+  if (ibest) CU(cudaMemcpy(ibest, di, sizeof(int), cudaMemcpyDeviceToHost));
+  double* outs[kCagScalars] = {lambda, best, first, scale};
+  for (int k = 0; k < kCagScalars; ++k)
+    if (outs[k]) *outs[k] = f[k];
   return 0;
 }
 

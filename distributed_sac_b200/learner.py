@@ -18,6 +18,7 @@ if none is given and `redis` is importable it connects to localhost like the ref
 """
 import itertools
 import json
+import math
 import os
 import pickle as _pickle
 import time
@@ -80,12 +81,12 @@ class _BaseLearner:
     family = "LL"
     log_name = "LunarLander_Distributed_SAC"
     _iteration_key = "episode_idx"
-    _pcgrad_ok = False          # PCGrad needs task-block minibatches and an MTSAC network (no CARE encoder)
+    _pcgrad_ok = False          # PCGrad and CAGrad need task-block minibatches and an MTSAC network (no CARE encoder)
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
-                     n_step=1, max_grad_norm=None, pcgrad=False):
+                     n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -96,6 +97,7 @@ class _BaseLearner:
         self.n_step = int(n_step)
         self.max_grad_norm = max_grad_norm
         self.pcgrad = bool(pcgrad)
+        self.cagrad = None if cagrad is None else float(cagrad)
         self.cfg = cfg_read(cfg_path)
         self.precision = precision
         self.write_mode = write_mode
@@ -107,6 +109,14 @@ class _BaseLearner:
         if self.pcgrad and not (self._pcgrad_ok and self.num_tasks >= 2):
             raise ValueError(f"pcgrad=True needs a multi-task MTSAC learner with num_tasks >= 2 ({type(self).__name__}, "
                              f"num_tasks {self.num_tasks})")
+        if self.cagrad is not None:
+            if self.pcgrad:
+                raise ValueError("pcgrad=True and cagrad= are exclusive (a CAGrad optimizer does not project)")
+            if not (self._pcgrad_ok and self.num_tasks >= 2):
+                raise ValueError(f"cagrad= needs a multi-task MTSAC learner with num_tasks >= 2 ({type(self).__name__}, "
+                                 f"num_tasks {self.num_tasks})")
+            if not (math.isfinite(self.cagrad) and self.cagrad >= 0):
+                raise ValueError(f"cagrad must be finite and >= 0 (got {cagrad})")
         self.device = torch.device(self.cfg.get("device", "cuda"))
         if self.device.type != "cuda":
             raise RuntimeError("the CUDA learner only runs on CUDA devices (cfg 'device' must be 'cuda')")
@@ -121,6 +131,9 @@ class _BaseLearner:
             self.core.set_update_intervals(actor_update_interval, target_update_interval)
         if max_grad_norm is not None:
             self.set_max_grad_norm(max_grad_norm)
+        if self.cagrad is not None:
+            self.core.set_pcgrad(critic=False, actor=False)
+            self.set_cagrad(self.cagrad)
         self.memory = self._make_memory(replay_where)
         self.memory.start()
         self.save_model_path = os.path.join("saved_models", self.log_name, self.datetime)
@@ -153,6 +166,15 @@ class _BaseLearner:
             raise ValueError("this learner was built without pcgrad=True")
         self.core.set_pcgrad(critic=critic, actor=actor)
 
+    def set_cagrad(self, c: float):
+        """CAGrad coefficient c of the critic and actor optimizers, effective from the next update(); 0 gives the plain
+        sum of the per-task gradients.  The learner must have been built with cagrad=; core.read_cagrad() returns the
+        last update's dual solution and core.read_pcgrad() its Gram matrix and weights."""
+        if self.cagrad is None:
+            raise ValueError("this learner was built without cagrad=")
+        self.core.set_cagrad(critic=c, actor=c)
+        self.cagrad = float(c)
+
     def set_n_step(self, n: int):
         """Horizon of the n-step return, effective from the next update()."""
         if self.n_step == 1:
@@ -167,7 +189,8 @@ class _BaseLearner:
                           reward_scale=float(self.reward_scale), lr_actor=float(self.lr_actor),
                           lr_critic=float(self.lr_critic),
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
-                          log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None, pcgrad=self.pcgrad)
+                          log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None,
+                          pcgrad=self.pcgrad or self.cagrad is not None)
 
     # ---- reference method surface -------------------------------------------------------------
     def update(self):
@@ -448,11 +471,12 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
-                 pcgrad=False):
+                 pcgrad=False, cagrad=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
+                          cagrad)
 
     def _set_dims(self):
         c = self.cfg
@@ -476,9 +500,10 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False):
+                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
+                          cagrad)
 
     def _set_dims(self):
         c = self.cfg
@@ -505,10 +530,12 @@ class MTSACLearner(_BaseLearner):
 
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
-                 actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False):
+                 actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
+                 cagrad=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
-                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad)
+                          precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
+                          cagrad)
 
     def _set_dims(self):
         c = self.cfg

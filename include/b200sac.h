@@ -31,6 +31,9 @@
  *   b200sac_set/get/read_pcgrad, b200sac_export_task_grad
  *                            PCGrad gradient surgery (Yu et al., NeurIPS 2020) for the multi-task learners' optimizers,
  *                            per replica and optimizer, with the step's Gram matrix and surgery decisions reported
+ *   b200sac_set/get/read_cagrad, b200sac_cagrad_solve_test
+ *                            CAGrad (Liu et al., NeurIPS 2021) on the same handles, per replica and optimizer, with the
+ *                            step's dual solution reported
  *   b200sac_blob_*           Learner.get_parameters() and server.set('parameters', _pickle.dumps(get_parameters())) in
  *                            Learner.run(), learner.py:272-276,298-299 (MT10_Distributed_CARE/src/learner.py:412-417,442-443):
  *                            the byte string, device-assembled
@@ -254,6 +257,46 @@ int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, i
 /* Gradient slice of task `task` (rows t(i) = task) of one replica, the whole trainable arena (n_floats = trainable floats)
  * into host or device memory.  Synchronises the stream. */
 int b200sac_export_task_grad(b200sac_t* h, int32_t replica, int32_t task, float* buf, int64_t n_floats, void* stream);
+
+/* CAGrad, conflict-averse gradient descent (Liu et al., NeurIPS 2021), on the same handles (cfg.pcgrad = 1; others:
+ * B200SAC_ERR_STATE) over the same slices g_t and Gram matrix G.  Each replica and optimizer (critic = counter slot 0,
+ * actor = slot 1) has a coefficient c, 0 at create.  c = 0: CAGrad is off and the PCGrad switch decides, as above.
+ * c > 0: the optimizer's Adam reads the CAGrad combination whatever its PCGrad switch says; the permutations are still
+ * drawn and G still computed and reported, the projection mask is 0 and b200sac_read_pcgrad's w holds the CAGrad weights.
+ * Per step, in fp64, on one warp, every sum over tasks in one fixed shuffle tree (pcgrad_kernels.cuh has the exact order
+ * of operations; p, A p, p.a and p.h are evaluated there through the unnormalised softmax numerators):
+ *   s  = (1/T) sum_t sqrt(G_tt); if s is 0 or not finite, or any G entry is not finite: w = 1 (plain sum), "degenerate"
+ *   A  = G / s^2 (the solve does not depend on the loss scale: the 1/B mean, weighted_loss's 1/B, T)
+ *   a_j = (1/T) sum_k A_jk;  abar = (1/T) sum_j a_j;  ce = c sqrt(abar + 1e-4)
+ *   x = 0, m = 0 (length T);  lr = 5c;  mu = 0.5;  best = +inf;  for it = 0 .. 20:
+ *     p = softmax(x) (max subtracted);  u = A p;  q = p.u;  r = sqrt(q + 1e-4);  F = p.a + ce r
+ *     if F < best: best = F, xbest = x, ibest = it
+ *     if it < 20: h = a + ce u / r;  d_j = p_j (h_j - p.h);  m = (it == 0 ? d : mu m + d);  x = x - lr m
+ *   p* = softmax(xbest);  lambda = ce / (sqrt(p*' A p* + 1e-4) + 1e-4);  w_t = (float)((1 + T lambda p*_t) / (1 + c^2))
+ *   Adam runs on sum_t fp32(w_t g_t) exactly as with PCGrad.
+ * This is CAGrad's update (g_0 + lambda g_w) / (1 + c^2) with g_0 the mean of the per-task mean gradients T g_t.  Its dual,
+ * min over the simplex of p' A b + ce sqrt(p' A p) (b uniform), is solved at a fixed cost as the authors' Metaworld code
+ * does, as far as that code is recalled here (softmax weights, 20 SGD steps with momentum 0.5, the best iterate); this
+ * definition, not that code, is the contract.  One deliberate difference: s has no epsilon, so the weights do not depend
+ * on the loss's absolute scale.
+ * Set: enqueued on `stream` like b200sac_set_hparams (applies to the steps enqueued after it, including launches of graphs
+ * already instantiated).  A negative, NaN or infinite c gives B200SAC_ERR_INVALID and nothing changes.  Not copied by
+ * b200sac_copy_replica and not part of a checkpoint.  Get: the values last set (host mirror: does not synchronise).
+ * The launch count of a step does not change. */
+int b200sac_set_cagrad(b200sac_t* h, int32_t replica, double c_critic, double c_actor, void* stream);
+int b200sac_get_cagrad(b200sac_t* h, int32_t replica, double* c_critic, double* c_actor);
+/* The last step's CAGrad record of one replica, index 0 critic and 1 actor; any output may be NULL: p [2][T] (p*),
+ * lambda [2], best [2] (best F), first [2] (F at iteration 0: uniform weights), scale [2] (s), ibest [2] (the iteration
+ * of the best F; -1 = CAGrad did not run for that optimizer on the last step, -2 = degenerate G).  Where ibest = -1 every
+ * fp64 entry is NaN; where it is -2, p, lambda, best and first are NaN and scale holds s.  Before the first step and for
+ * the actor of a critic-only step: ibest -1.  Synchronises the stream. */
+int b200sac_read_cagrad(b200sac_t* h, int32_t replica, double* p, double* lambda, double* best, double* first,
+                        double* scale, int32_t* ibest, void* stream);
+/* The same solve run stand-alone by one warp of the current device on a caller-given HOST G [T][T] (1 <= T <= 64,
+ * symmetric) with c > 0 (finite), outputs to HOST memory (w [T]; p [T] and the scalars nullable).  Enqueued on the legacy
+ * default stream, which it synchronises. */
+int b200sac_cagrad_solve_test(int32_t T, const double* G, double c, float* w, double* p, double* lambda, double* best,
+                              double* first, double* scale, int32_t* ibest);
 
 /* One gradient step from caller-provided DEVICE minibatches, each
  * [replicas][batch][width] fp32: s,s2 width obs(=state_dim+num_tasks), a width act, r,d width 1.

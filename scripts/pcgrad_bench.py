@@ -1,11 +1,12 @@
-"""PCGrad gradient surgery: cost of the pcgrad plan against the default plan, and the in-graph times of its new launches.
+"""PCGrad and CAGrad: cost of the pcgrad plan against the default plan, and the in-graph times of its new launches.
 
   python scripts/pcgrad_bench.py [--steps 1000] [--warmup 100] [--out FILE]
 
 Workload: the MT10 MTSAC shape (39 + 10 one-hot inputs, 4 actions, 400-wide 3-layer networks, batch 1280, 10 tasks,
 precision 1, per-layer plan) on a 128 Ki-transition device ring, for 1 learner and for 10 learners in one handle.  Each leg
-alternates three handles three times and reports the median: no pcgrad, pcgrad with both switches off (the Gram matrix
-only), and pcgrad on.  The card's name, power limit and SM clock are read in the same run (nvidia-smi, read-only query).
+alternates four handles three times and reports the median: no pcgrad, pcgrad with both switches off (the Gram
+matrix only), pcgrad on, and CAGrad (both PCGrad switches off, c = 0.5 on both optimizers).  The card's name, power
+limit and SM clock are read in the same run (nvidia-smi, read-only query).
 """
 import argparse
 import json
@@ -18,7 +19,8 @@ import time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-MODES = ("default", "switch_off", "on")
+MODES = ("default", "switch_off", "on", "cagrad")
+CAGRAD_C = 0.5
 
 
 def card():
@@ -45,8 +47,10 @@ def leg(R, ring_n, steps, warmup, mode, timeline):
     ring.fill_synthetic(ring_n, seed=5)
     stream = torch.cuda.Stream()
     with torch.cuda.stream(stream):
-        if mode == "switch_off":
+        if mode in ("switch_off", "cagrad"):
             core.set_pcgrad(critic=False, actor=False)
+        if mode == "cagrad":
+            core.set_cagrad(critic=CAGRAD_C, actor=CAGRAD_C)
         core.prepare(ring)
         core.step_sampled(ring, warmup)
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -60,6 +64,9 @@ def leg(R, ring_n, steps, warmup, mode, timeline):
     if mode != "default":
         rec = core.read_pcgrad(0)
         extra = {"critic_projections": int(rec["projected"][0].sum()), "actor_projections": int(rec["projected"][1].sum())}
+        if mode == "cagrad":
+            cg = core.read_cagrad(0)
+            extra = {"ibest": cg["ibest"].tolist(), "lambda": cg["lambda"].tolist(), "w": rec["w"].tolist()}
     tl = None
     if timeline:
         with torch.cuda.stream(stream):
@@ -99,9 +106,12 @@ def main():
         med = {m: statistics.median(v) for m, v in us.items()}
         out = {"learners": R, "ring_per_learner": ring_n, "us_per_step": med,
                "switch_off_over_default": med["switch_off"] / med["default"], "on_over_default": med["on"] / med["default"],
+               "cagrad_over_default": med["cagrad"] / med["default"], "cagrad_over_on": med["cagrad"] / med["on"],
                "last_step_projections": extras, "runs_us": us}
         if tls:                        # start-to-start times of the unforked timeline run (b200sac_graph_timeline)
             out["graph_timeline"] = tls
+            out["pcgrad_launches_us"] = {m: {k: v for k, v in tl["new_launches_us"].items() if "pcgrad" in k}
+                                         for m, tl in tls.items()}
         res["legs"][name] = out
         print(json.dumps({name: {k: v for k, v in out.items() if k not in ("runs_us", "graph_timeline")}}), flush=True)
     line = json.dumps(res)
