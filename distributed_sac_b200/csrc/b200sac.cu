@@ -129,8 +129,8 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->care != 0 && c->care != 1 && c->care != 2) return fail(B200SAC_ERR_INVALID, "care must be 0, 1 (CARE(M)) or 2 (CARE(O))");
   if (c->grad_clip != 0 && c->grad_clip != 1) return fail(B200SAC_ERR_INVALID, "grad_clip must be 0 or 1");
   if (c->pcgrad != 0 && c->pcgrad != 1) return fail(B200SAC_ERR_INVALID, "pcgrad must be 0 or 1");
-  if (c->pcgrad && (c->num_tasks < 2 || c->care != 0 || c->grad_clip != 0))
-    return fail(B200SAC_ERR_INVALID, "pcgrad needs num_tasks >= 2, no CARE encoder and no grad_clip");
+  if (c->pcgrad && (c->num_tasks < 2 || c->grad_clip != 0))
+    return fail(B200SAC_ERR_INVALID, "pcgrad needs num_tasks >= 2 and no grad_clip");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -1702,9 +1702,10 @@ void PlanBuilder::build_plan_layered() {
       if (fl > kCareTabWgradSmemFloats) rc = fail(B200SAC_ERR_INVALID, "internal: one task's CARE backward chains exceed %d floats", kCareTabWgradSmemFloats);
       Q.tchunk = std::max(1, std::min(c.num_tasks, kCareTabWgradSmemFloats / fl));
       l2.smem = (size_t)Q.tchunk * fl * sizeof(float);
+      if (c.pcgrad) { Q.grads_x = h->grads_x; Q.xs = (long long)R * L.trainable; }   // one gradient slice per task
       l2.grid = dim3(sms, R);
       l2.block = dim3(256);
-      push(std::move(l2), care_tab_wgrad_kernel, Q);
+      push(std::move(l2), c.pcgrad ? care_tab_wgrad_kernel<true> : care_tab_wgrad_kernel<false>, Q);
     }
   }
   if (c.grad_clip) grad_norm(0);

@@ -290,17 +290,26 @@ struct CareTabWgradArgs {
   int T, K, co;
   int original, off_ctx;              // CARE(O): trunk layer-0 input = z (table, off_ctx); ctx layer-0 input = relu(E[t])
   int tchunk;                         // tasks whose backward chains are held in shared memory at once
+  float* grads_x; long long xs;       // per-task instantiation: gradient slice t >= 1 at grads_x + (t-1) xs (+ rep rsG)
 };
 
 // Shared memory of care_tab_wgrad_kernel: the default 48 KiB (no opt-in).  One task's chains are at most
 // 8 x 512 + 32 (trunk) + 9 x 512 (context net) = 8 736 floats, so every configuration check_cfg accepts fits one task at least.
 constexpr int kCareTabWgradSmemFloats = 12288;
 
+// gradient slice t of replica rep (per-task instantiation): slice 0 is G itself
+__device__ __forceinline__ float* care_grad_slice(const CareTabWgradArgs& P, float* G, int rep, int t) {
+  return t == 0 ? G : P.grads_x + (long long)(t - 1) * P.xs + rep * P.rsG;
+}
+
 // grid (nblk, R), block 256.  Every CTA re-derives the (tiny) per-task backward chains in shared memory, then
 // takes a slice of the weight / bias gradient elements: dW_j[o][i] = sum_t dz_j[t][o] * a_{j-1}[t][i].
 // The tasks are taken in chunks of P.tchunk (T x the chains of one task can reach 2.2 MB): every gradient element's sum over
 // t continues from the value its thread stored after the previous chunk, so the summation order (t ascending) and with it
 // the result do not depend on the chunk size.
+// kPerTask (pcgrad handles): no sum over tasks -- task t's term goes to gradient slice t (slice 0 = grads, slice t >= 1 =
+// grads_x + (t-1) xs), fmaf(dz, a, 0) for a weight and dz for a bias, so every element of every slice is written each step.
+template <bool kPerTask>
 __global__ void __launch_bounds__(256) care_tab_wgrad_kernel(CareTabWgradArgs P) {
   KStamp ks_;
   extern __shared__ float sm[];
@@ -362,14 +371,19 @@ __global__ void __launch_bounds__(256) care_tab_wgrad_kernel(CareTabWgradArgs P)
                 a = emb[(long long)t * nin + i];
                 if (P.original) a = fmaxf(a, 0.f);                                                // header(relu(E))
               }
-              s = fmaf(sm[dz_off[n][j] + t * nout + o], a, s);
+              if constexpr (kPerTask) care_grad_slice(P, G, rep, t0 + t)[N.w[j] + q] = fmaf(sm[dz_off[n][j] + t * nout + o], a, 0.f);
+              else s = fmaf(sm[dz_off[n][j] + t * nout + o], a, s);
             }
-            G[N.w[j] + q] = s;
+            if constexpr (!kPerTask) G[N.w[j] + q] = s;
           } else {
             const int o = (int)(q - nw);
-            float s = t0 > 0 ? G[N.b[j] + o] : 0.f;
-            for (int t = 0; t < T; ++t) s += sm[dz_off[n][j] + t * nout + o];
-            G[N.b[j] + o] = s;
+            if constexpr (kPerTask) {
+              for (int t = 0; t < T; ++t) care_grad_slice(P, G, rep, t0 + t)[N.b[j] + o] = sm[dz_off[n][j] + t * nout + o];
+            } else {
+              float s = t0 > 0 ? G[N.b[j] + o] : 0.f;
+              for (int t = 0; t < T; ++t) s += sm[dz_off[n][j] + t * nout + o];
+              G[N.b[j] + o] = s;
+            }
           }
         }
       }

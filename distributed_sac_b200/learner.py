@@ -81,7 +81,7 @@ class _BaseLearner:
     family = "LL"
     log_name = "LunarLander_Distributed_SAC"
     _iteration_key = "episode_idx"
-    _pcgrad_ok = False          # PCGrad and CAGrad need task-block minibatches and an MTSAC network (no CARE encoder)
+    _pcgrad_ok = False          # PCGrad and CAGrad need task-block minibatches: the multi-task learners (MTSAC and CARE)
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
@@ -107,13 +107,13 @@ class _BaseLearner:
         self.datetime = str(datetime.now())[:-7]
         self._set_dims()
         if self.pcgrad and not (self._pcgrad_ok and self.num_tasks >= 2):
-            raise ValueError(f"pcgrad=True needs a multi-task MTSAC learner with num_tasks >= 2 ({type(self).__name__}, "
+            raise ValueError(f"pcgrad=True needs a multi-task MTSAC or CARE learner with num_tasks >= 2 ({type(self).__name__}, "
                              f"num_tasks {self.num_tasks})")
         if self.cagrad is not None:
             if self.pcgrad:
                 raise ValueError("pcgrad=True and cagrad= are exclusive (a CAGrad optimizer does not project)")
             if not (self._pcgrad_ok and self.num_tasks >= 2):
-                raise ValueError(f"cagrad= needs a multi-task MTSAC learner with num_tasks >= 2 ({type(self).__name__}, "
+                raise ValueError(f"cagrad= needs a multi-task MTSAC or CARE learner with num_tasks >= 2 ({type(self).__name__}, "
                                  f"num_tasks {self.num_tasks})")
             if not (math.isfinite(self.cagrad) and self.cagrad >= 0):
                 raise ValueError(f"cagrad must be finite and >= 0 (got {cagrad})")
@@ -572,6 +572,11 @@ class MTSACLearner(_BaseLearner):
         return one_hots @ self.log_alpha.reshape(-1, 1)
 
 
+class EncoderConfigError(KeyError, ValueError):
+    """A CARE cfg whose 'encoder' block lacks keys the learner needs (a KeyError, as the lookup raised before, and a
+    ValueError, as every other bad constructor argument raises)."""
+
+
 class CARELearner(MTSACLearner):
     """MT10_Distributed_CARE/src/learner.py with `use_modified_care: true` (CARE(M)):
     Learner(train_classes, train_tasks, cfg_path, write_mode, save_period, checkpoint_path).
@@ -582,7 +587,9 @@ class CARELearner(MTSACLearner):
     critic's after every update (learner.py:402), so it is exported from the same tensors."""
     family = "C10"
     log_name = "MT10_Distributed_CARE"
-    _pcgrad_ok = False          # the critic optimizer also owns the state encoder, whose gradients are not task slices
+    # the 'encoder' keys _core_config reads without a default
+    _encoder_keys = ("num_encoders", "hidden_dims_mixtureEnc", "output_dim_mixtureEnc", "hidden_dims_contextEnc",
+                     "output_dim_contextEnc", "embedding_dim_contextEnc", "lr_contextEnc")
 
     def _set_dims(self):
         super()._set_dims()
@@ -590,6 +597,9 @@ class CARELearner(MTSACLearner):
         self.use_modified_care = bool(c.get("use_modified_care", False))
         self.use_weighted_loss = self.use_modified_care    # learner.py:313,349: use_weighted_loss = use_modified_care
         self.encoder_cfg = c["encoder"]
+        missing = [k for k in self._encoder_keys if k not in self.encoder_cfg]
+        if missing:             # before any other check, so an incomplete cfg fails the same way with or without pcgrad
+            raise EncoderConfigError(f"cfg 'encoder' block lacks {missing}")
 
     def _core_config(self):
         cc = super()._core_config()

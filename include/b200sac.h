@@ -107,8 +107,8 @@ typedef struct b200sac_cfg {
   int32_t grad_clip;                 /* 0 = the default plan; 1 = the plan with gradient-norm clipping and gradient norms
                                         (b200sac_set_grad_clip), every threshold +inf at create.  Fixed at create. */
   int32_t pcgrad;                    /* 0 = the default plan; 1 = the per-layer plan with PCGrad gradient surgery
-                                        (b200sac_set_pcgrad), both switches on at create.  Needs num_tasks >= 2, care = 0
-                                        and grad_clip = 0.  Fixed at create. */
+                                        (b200sac_set_pcgrad), both switches on at create.  Needs num_tasks >= 2 and
+                                        grad_clip = 0; MTSAC and CARE (care = 1 | 2) alike.  Fixed at create. */
 } b200sac_cfg;
 
 typedef struct b200sac_tensor_desc {
@@ -224,8 +224,9 @@ int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void*
  * T = num_tasks, P = batch / T; row i of a step's minibatch belongs to task t(i) = i / P.  On a pcgrad handle
  * b200sac_step_sampled, b200sac_update and b200sac_replay_sample draw P rows per task in this order, on the device and the
  * pinned-host ring alike (the pinned-host ring skips its shuffle of the rows; the losses are row sums, so the order does
- * not change what a step computes).  For each optimizer o (the critic: q1 and q2 together,
- * counter slot 0; the actor: slot 1), with l_i = row i's term of o's loss exactly as the step defines it (the 1/B mean,
+ * not change what a step computes).  For each optimizer o (the critic: q1, q2 and, on CARE handles, the critic state
+ * encoder cse together, counter slot 0; the actor: its MLP, slot 1 -- the actor's state encoder is the tied copy of cse
+ * and has no optimizer), with l_i = row i's term of o's loss exactly as the step defines it (the 1/B mean,
  * weighted_loss's extra 1/B, importance weights and the per-task temperature included):
  *   g_t  = the gradient of L_{o,t} = sum over the rows i of task t of l_i, so sum_t g_t is the ordinary step gradient.  The
  *          published implementations use per-task means, T times this: the projections do not depend on the scale, Adam
@@ -239,7 +240,11 @@ int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void*
  *   w_k  = (float)(1 - sum_i c^(i)_k), the sum in fp64 over i ascending;
  *   Adam runs on w_0 g_0 + w_1 g_1 + ... + w_{T-1} g_{T-1}: each product rounded to fp32, added in index order, no FMA.
  *          The Adam math and the Polyak update fused after it are unchanged.
- * The temperature keeps its own per-task Adam and takes no part.  A critic-only step leaves the actor untouched and records
+ * The temperature keeps its own per-task Adam and takes no part; so does the CARE(O) context encoder (slot 4), whose Adam
+ * reads the plain sum of its T slices in index order (trained by the critic loss, it has slices like every optimizer).
+ * Rows out of task order (b200sac_step only, counted in task_mismatch): the weight-gradient GEMM and head parts of slice t
+ * come from the rows i with i / P = t, the CARE trunk and context-net parts (per-task table rows) from the rows whose
+ * one-hot task is t; the sum over the slices is the ordinary gradient either way.  A critic-only step leaves the actor untouched and records
  * NaN actor weights.  b200sac_export(GRADS) still returns the slices summed in index order: the unprojected gradient.
  * Set: enqueued on `stream` like b200sac_set_hparams (applies to the steps enqueued after it, including launches of graphs
  * already instantiated).  Each switch is 0 or 1, both 1 at create; off means w = 1 (Adam reads the plain slice sum) while
@@ -254,8 +259,9 @@ int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_
  * hold gram NaN, w NaN and mask 0, and its perm keeps the permutations of the last actor step.  Synchronises the stream. */
 int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, int32_t* perm, uint64_t* mask,
                         int32_t* task_mismatch, void* stream);
-/* Gradient slice of task `task` (rows t(i) = task) of one replica, the whole trainable arena (n_floats = trainable floats)
- * into host or device memory.  Synchronises the stream. */
+/* Gradient slice of task `task` (rows t(i) = task) of one replica, the whole trainable arena (n_floats = trainable floats;
+ * on CARE handles the critic state encoder and the CARE(O) context encoder included) into host or device memory.
+ * Synchronises the stream. */
 int b200sac_export_task_grad(b200sac_t* h, int32_t replica, int32_t task, float* buf, int64_t n_floats, void* stream);
 
 /* CAGrad, conflict-averse gradient descent (Liu et al., NeurIPS 2021), on the same handles (cfg.pcgrad = 1; others:

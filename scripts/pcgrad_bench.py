@@ -1,12 +1,17 @@
 """PCGrad and CAGrad: cost of the pcgrad plan against the default plan, and the in-graph times of its new launches.
 
-  python scripts/pcgrad_bench.py [--steps 1000] [--warmup 100] [--out FILE]
+  python scripts/pcgrad_bench.py [--steps 1000] [--warmup 100] [--legs MS_x1,MS_x10,C10M_x1,C10O_x1] [--out FILE]
 
-Workload: the MT10 MTSAC shape (39 + 10 one-hot inputs, 4 actions, 400-wide 3-layer networks, batch 1280, 10 tasks,
-precision 1, per-layer plan) on a 128 Ki-transition device ring, for 1 learner and for 10 learners in one handle.  Each leg
-alternates four handles three times and reports the median: no pcgrad, pcgrad with both switches off (the Gram
-matrix only), pcgrad on, and CAGrad (both PCGrad switches off, c = 0.5 on both optimizers).  The card's name, power
-limit and SM clock are read in the same run (nvidia-smi, read-only query).
+Workloads, each on a 128 Ki-transition device ring:
+  MS_x1, MS_x10   the MT10 MTSAC shape (39 + 10 one-hot inputs, 4 actions, 400-wide 3-layer networks, batch 1280, 10 tasks,
+                  precision 1, per-layer plan), 1 learner and 10 learners in one handle;
+  C10M_x1, C10O_x1  the MT10 CARE shape of the same MLPs (BASELINE config 5: K = 6 mixture encoders 39 -> 50 -> 50, 768-d
+                  task embedding, 50-wide context net), CARE(M) and CARE(O), 1 learner.
+Each leg alternates four handles three times and reports the median: no pcgrad, pcgrad with both switches off (the Gram
+matrix only), pcgrad on, and CAGrad (both PCGrad switches off, c = 0.5 on both optimizers).  The timeline run gives the
+in-graph times of the pcgrad launches and, on the CARE legs, of care_tab_wgrad and the mixture-encoder weight-gradient
+launches (the gemm launches between care_mix_bwd and care_tab_reduce).  The card's name, power limit and SM clock are read
+in the same run (nvidia-smi, read-only query).
 """
 import argparse
 import json
@@ -33,16 +38,29 @@ def card():
         return {"error": repr(e)}
 
 
-def config(R, pcgrad):
+def config(R, pcgrad, care=None):
+    """care: None (MTSAC), "M" or "O" (the CARE variant)."""
     from distributed_sac_b200.core import CoreConfig
+    kw = {}
+    if care:
+        kw = dict(care=True, num_encoders=6, mix_hidden=[50], mix_out=50, ctx_in=768, ctx_hidden=[50, 50], ctx_out=50,
+                  tau_se=0.05, care_original=care == "O", emb_dim=50, lr_ctx=3e-4)
     return CoreConfig(state_dim=39, act_dim=4, actor_hidden=[400] * 3, critic_hidden=[400] * 3, batch=1280, num_tasks=10,
-                      weighted_loss=True, replicas=R, precision=1, pcgrad=pcgrad)
+                      weighted_loss=care != "O", replicas=R, precision=1, pcgrad=pcgrad, **kw)
 
 
-def leg(R, ring_n, steps, warmup, mode, timeline):
+def _timed(names):
+    """Indices of the launches a timeline reports: the surgery's, the Adam launches after them and the CARE weight
+    gradients (care_tab_wgrad, and the mixture-encoder launches between care_mix_bwd and care_tab_reduce)."""
+    lo, hi = (names.index("care_mix_bwd"), names.index("care_tab_reduce")) if "care_mix_bwd" in names else (0, 0)
+    return [i for i, n in enumerate(names) if n.startswith("pcgrad") or lo < i < hi or
+            n in ("adam_critic+polyak", "adam_actor+alpha", "care_tab_wgrad")]
+
+
+def leg(R, ring_n, steps, warmup, mode, timeline, care=None):
     import torch
     from distributed_sac_b200.core import Replay, SacCore
-    core = SacCore(config(R, mode != "default"), 0, seed=11)
+    core = SacCore(config(R, mode != "default", care), 0, seed=11)
     ring = Replay(core, ring_n, seed=3)
     ring.fill_synthetic(ring_n, seed=5)
     stream = torch.cuda.Stream()
@@ -73,9 +91,8 @@ def leg(R, ring_n, steps, warmup, mode, timeline):
             names = ["sample", "ingest"] + [n for n, _ in core.profile_step(ring, iters=2)][1:]
             t = core.graph_timeline(ring, iters=200)
         torch.cuda.synchronize()
-        tl = {"new_launches_us": {f"{i}:{n}": t[i] for i, n in enumerate(names)
-                                  if n.startswith("pcgrad") or n in ("adam_critic+polyak", "adam_actor+alpha")},
-              "step_us": sum(t), "all_us": dict(zip(names, t))}
+        tl = {"new_launches_us": {f"{i}:{names[i]}": t[i] for i in _timed(names)},
+              "launches": len(names), "step_us": sum(t), "all_us": dict(zip(names, t))}
     ring.close()
     core.close()
     return us, tl, extra
@@ -85,6 +102,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=1000)
     ap.add_argument("--warmup", type=int, default=100)
+    ap.add_argument("--legs", default="MS_x1,MS_x10,C10M_x1,C10O_x1")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     import __graft_entry__ as ge
@@ -93,12 +111,16 @@ def main():
     if not torch.cuda.is_available():
         raise SystemExit("pcgrad_bench.py needs a CUDA device")
     res = {"card": card(), "steps": args.steps, "warmup": args.warmup, "legs": {}}
-    for name, R, ring_n in (("MS_x1", 1, 1 << 17), ("MS_x10", 10, 1 << 17)):
+    legs = (("MS_x1", 1, 1 << 17, None), ("MS_x10", 10, 1 << 17, None), ("C10M_x1", 1, 1 << 17, "M"),
+            ("C10O_x1", 1, 1 << 17, "O"))
+    for name, R, ring_n, care in legs:
+        if name not in args.legs.split(","):
+            continue
         us = {m: [] for m in MODES}
         tls, extras = {}, {}
         for k in range(3):
             for m in MODES:
-                t, tl, ex = leg(R, ring_n, args.steps, args.warmup, m, timeline=(k == 0 and R == 1))
+                t, tl, ex = leg(R, ring_n, args.steps, args.warmup, m, timeline=(k == 0 and R == 1), care=care)
                 us[m].append(t)
                 extras[m] = ex
                 if tl is not None:
