@@ -43,6 +43,17 @@ class TensorDesc(C.Structure):
                 ("trainable", C.c_int32), ("opt", C.c_int32), ("pitch", C.c_int32), ("reserved", C.c_int32)]
 
 
+RESET_ACTOR, RESET_CRITIC, RESET_ALPHA, RESET_ENCODER, RESET_CONTEXT, RESET_PARTS = 0, 1, 2, 3, 4, 5
+
+
+class ResetPart(C.Structure):
+    _fields_ = [("layers", C.c_int32), ("reserved", C.c_int32), ("shrink", C.c_double)]
+
+
+class ResetSpec(C.Structure):
+    _fields_ = [("part", ResetPart * RESET_PARTS)]
+
+
 _F = C.POINTER(C.c_float)
 _VP = C.c_void_p
 
@@ -63,6 +74,7 @@ SYMBOLS = {
     "b200sac_get_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams)]),
     "b200sac_set_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams), _VP]),
     "b200sac_copy_replica": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
+    "b200sac_reset": (C.c_int, [_VP, C.c_int32, C.POINTER(ResetSpec), C.c_uint64, _VP]),
     "b200sac_set_update_intervals": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, _VP]),
     "b200sac_get_update_intervals": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_set_grad_clip": (C.c_int, [_VP, C.c_int32, C.c_double, C.c_double, C.c_double, _VP]),

@@ -120,6 +120,53 @@ def _replicas(n, replica):
     return range(n) if replica is None else [int(replica)]
 
 
+RESET_PARTS = ("actor", "critic", "alpha", "encoder", "context")      # index of b200sac_reset_spec.part[]
+
+
+def reset_parts(cfg: CoreConfig):
+    """The parts a b200sac_reset of a handle with this config can touch."""
+    return RESET_PARTS[:3] + ((("encoder", "context") if cfg.care_original else ("encoder",)) if cfg.care else ())
+
+
+def reset_spec(cfg: CoreConfig, shrink=0.0, **parts):
+    """The b200sac_reset_spec of SacCore.reset's keywords (pure host function).  actor / critic: a Linear layer count
+    from the output layer (0 = untouched) or "all"; alpha / encoder / context: a bool; with no part given, every part the
+    handle has.  shrink: one lambda in [0, 1] for every part, or {part: lambda} (parts left out: 0).  Raises ValueError."""
+    unknown = set(parts) - set(RESET_PARTS)
+    if unknown:
+        raise ValueError(f"unknown reset parts {sorted(unknown)}; parts: {RESET_PARTS}")
+    given = dict(parts)
+    if all(v is None for v in given.values()):
+        given = {k: ("all" if k in ("actor", "critic") else True) for k in reset_parts(cfg)}
+    have = reset_parts(cfg)
+    if isinstance(shrink, dict):
+        unknown = set(shrink) - set(RESET_PARTS)
+        if unknown:
+            raise ValueError(f"shrink names unknown parts {sorted(unknown)}; parts: {RESET_PARTS}")
+        lam = {k: shrink.get(k, 0.0) for k in RESET_PARTS}
+    else:
+        lam = {k: shrink for k in RESET_PARTS}
+    spec = _lib.ResetSpec()
+    for i, k in enumerate(RESET_PARTS):
+        v, x = given.get(k), lam[k]
+        if isinstance(x, bool) or not isinstance(x, (int, float, np.integer, np.floating)) or not 0.0 <= float(x) <= 1.0:
+            raise ValueError(f"shrink of {k} must be a number in [0, 1], got {x!r}")
+        spec.part[i].shrink = float(x)
+        if v is None:
+            continue
+        if k in ("actor", "critic"):
+            if v == "all":
+                v = len(cfg.actor_hidden if k == "actor" else cfg.critic_hidden) + 1
+            if isinstance(v, bool) or not isinstance(v, (int, np.integer)) or v < 0:
+                raise ValueError(f"{k} takes a Linear layer count >= 0 or 'all', got {v!r}")
+        elif not isinstance(v, (bool, np.bool_)) and not (isinstance(v, (int, np.integer)) and v in (0, 1)):
+            raise ValueError(f"{k} takes a bool, got {v!r}")
+        if v and k not in have:
+            raise ValueError(f"this handle has no {k} to reset (parts: {have})")
+        spec.part[i].layers = int(v)
+    return spec
+
+
 class SacCore:
     def __init__(self, cfg: CoreConfig, device: int = 0, seed: int = 0):
         self.lib = _lib.load()
@@ -436,6 +483,16 @@ class SacCore:
         device to device on the current stream.  Hyperparameters, update intervals, gradient-clipping thresholds, PCGrad
         switches and replay data stay dst's own."""
         _lib.check(self.lib.b200sac_copy_replica(self._h, int(src), int(dst), _stream()))
+
+    def reset(self, seed: int, replica=None, actor=None, critic=None, alpha=None, encoder=None, context=None, shrink=0.0):
+        """Re-initialise networks of one replica (replica=None: every replica, one call each) on the current stream:
+        theta = shrink * theta + (1 - shrink) * theta0, theta0 the draw b200sac_create(seed) made, targets alike; the
+        owning optimizers restart.  actor / critic: Linear layers from the output ("all" = every layer); alpha, encoder
+        (CARE state encoder), context (CARE(O) context encoder): bools; no part given = every part the handle has (a full
+        reset).  shrink: a float or {part: float}.  Steps enqueued afterwards see the reset (include/b200sac.h)."""
+        spec = reset_spec(self.cfg, shrink, actor=actor, critic=critic, alpha=alpha, encoder=encoder, context=context)
+        for r in _replicas(self.cfg.replicas, replica):
+            _lib.check(self.lib.b200sac_reset(self._h, r, C.byref(spec), C.c_uint64(int(seed) % (1 << 64)), _stream()))
 
     def soft_update(self, tau: float, critic: Optional[int] = None):
         """Polyak update of the targets outside a step: both critics (CARE: and the target state encoder, with the replica's

@@ -238,6 +238,52 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
   L.arena = off;
 }
 
+// How every parameter tensor is initialised, in the order b200sac_create draws them: the one source of the (init kind, tag)
+// pairs that create and b200sac_reset both read.  Xavier weights and the CARE mixture's randn tensors take tags 0, 1, ...
+// in this order; biases are zero; log_alpha is cfg.log_alpha_init; the frozen CARE embedding (part -1, never reset) is
+// drawn under seed ^ 0x5EED.  depth: an actor or critic Linear layer's position counted from the network's output (1 = the
+// head); 0 for the all-or-nothing parts.
+struct InitTensor {
+  int64_t off;
+  int rows, cols, ld;
+  int kind;                 // ResetInit
+  int tag;
+  int part;                 // B200SAC_RESET_*, -1 = the embedding
+  int depth;                // 0 = reset with its part whatever the layer count
+  bool target;              // has a target copy at + target_delta (q1, q2, cse)
+  uint64_t seed_xor;
+};
+
+static std::vector<InitTensor> init_table(const b200sac_cfg* c, const Layout& L) {
+  std::vector<InitTensor> v;
+  int tag = 0;
+  auto linear = [&](const std::vector<LayerOff>& net, int part, bool target) {
+    const int n = (int)net.size();
+    for (int i = 0; i < n; ++i) {
+      const LayerOff& lo = net[i];
+      const int depth = part == B200SAC_RESET_ACTOR || part == B200SAC_RESET_CRITIC ? n - i : 0;
+      v.push_back({lo.w, lo.out, lo.in, lo.ld, RESET_XAVIER, tag++, part, depth, target, 0});
+      v.push_back({lo.b, lo.out, 1, 1, RESET_ZERO, -1, part, depth, target, 0});
+    }
+  };
+  linear(L.actor, B200SAC_RESET_ACTOR, false);
+  linear(L.q[0], B200SAC_RESET_CRITIC, true);
+  linear(L.q[1], B200SAC_RESET_CRITIC, true);
+  if (c->care) {
+    for (const auto& lo : L.mix) {
+      const int rows = c->num_encoders * lo.out;
+      v.push_back({lo.w, rows, lo.in, lo.in, RESET_RANDN, tag++, B200SAC_RESET_ENCODER, 0, true, 0});
+      v.push_back({lo.b, rows, 1, 1, RESET_RANDN, tag++, B200SAC_RESET_ENCODER, 0, true, 0});
+    }
+    linear(L.trunk, B200SAC_RESET_ENCODER, true);
+    linear(L.ctx, B200SAC_RESET_ENCODER, true);
+    linear(L.cenc, B200SAC_RESET_CONTEXT, false);
+    v.push_back({L.off_emb, c->num_tasks, c->ctx_in, c->ctx_in, RESET_RANDN, tag++, -1, 0, false, 0x5EEDull});
+  }
+  v.push_back({L.off_alpha, c->num_tasks > 0 ? c->num_tasks : 1, 1, 1, RESET_CONST, -1, B200SAC_RESET_ALPHA, 0, false, 0});
+  return v;
+}
+
 extern "C" int b200sac_layout(const b200sac_cfg* cfg, b200sac_tensor_desc* out, int32_t cap, int32_t* n,
                               int64_t* arena_floats, int64_t* trainable_floats) {
   if (int rc = check_cfg(cfg)) return rc;
@@ -2123,25 +2169,20 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
 
-  // parameter init: Xavier-uniform weights, zero biases, log_alpha = cfg; targets = locals
+  // parameter init: Xavier-uniform weights, zero biases (the memset above), log_alpha = cfg; targets = locals
   {
-    int tag = 0;
-    for (const auto* net : {&L.actor, &L.q[0], &L.q[1]})
-      for (const auto& lo : *net) {
-        xavier_kernel<<<dim3(64, R), 256>>>(h->params + lo.w, L.arena, lo.out, lo.in, lo.ld, seed, tag++);
+    for (const InitTensor& t : init_table(cfg, L)) {
+      const uint64_t key = seed ^ t.seed_xor;
+      if (t.kind == RESET_XAVIER) {
+        xavier_kernel<<<dim3(64, R), 256>>>(h->params + t.off, L.arena, t.rows, t.cols, t.ld, key, t.tag);
+      } else if (t.kind == RESET_RANDN) {
+        randn_kernel<<<dim3(t.cols > 1 ? 64 : 8, R), 256>>>(h->params + t.off, L.arena, (long long)t.rows * t.cols, key, t.tag);
+      } else if (t.kind == RESET_CONST) {
+        std::vector<float> la((size_t)t.rows, (float)cfg->log_alpha_init);
+        for (int rep = 0; rep < R; ++rep)
+          CU(cudaMemcpy(h->params + (size_t)rep * L.arena + t.off, la.data(), la.size() * sizeof(float), cudaMemcpyHostToDevice));
       }
-    if (cfg->care) {     // mixture weights ~ N(0,1) (state_encoder.py:146-153); trunk / context MLP Xavier; embedding random
-      for (const auto& lo : L.mix) {
-        randn_kernel<<<dim3(64, R), 256>>>(h->params + lo.w, L.arena, (long long)cfg->num_encoders * lo.out * lo.in, seed, tag++);
-        randn_kernel<<<dim3(8, R), 256>>>(h->params + lo.b, L.arena, (long long)cfg->num_encoders * lo.out, seed, tag++);
-      }
-      for (const auto* net : {&L.trunk, &L.ctx, &L.cenc})
-        for (const auto& lo : *net) xavier_kernel<<<dim3(64, R), 256>>>(h->params + lo.w, L.arena, lo.out, lo.in, lo.ld, seed, tag++);
-      randn_kernel<<<dim3(64, R), 256>>>(h->params + L.off_emb, L.arena, (long long)cfg->num_tasks * cfg->ctx_in, seed ^ 0x5EEDull, tag++);
     }
-    std::vector<float> la((size_t)(cfg->num_tasks > 0 ? cfg->num_tasks : 1), (float)cfg->log_alpha_init);
-    for (int rep = 0; rep < R; ++rep)
-      CU(cudaMemcpy(h->params + (size_t)rep * L.arena + L.off_alpha, la.data(), la.size() * sizeof(float), cudaMemcpyHostToDevice));
     polyak_kernel<<<dim3(128, R), 256>>>(h->params + L.critic_begin, L.arena, L.critic_n, L.target_delta, 1.0f, 0.0f);
     CU(cudaGetLastError());
   }
@@ -2522,6 +2563,70 @@ extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void
   CU(cudaMemcpyAsync(h->adam_m + dst * nt, h->adam_m + src * nt, nt * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
   CU(cudaMemcpyAsync(h->adam_v + dst * nt, h->adam_v + src * nt, nt * sizeof(float), cudaMemcpyDeviceToDevice, sb.run));
   CU(cudaMemcpyAsync(h->cnt + dst, h->cnt + src, sizeof(Counters), cudaMemcpyDeviceToDevice, sb.run));
+  return sb.end();
+}
+
+extern "C" int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_spec* spec, uint64_t seed, void* stream) {
+  if (!h || !spec) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  static const char* const kPart[B200SAC_RESET_PARTS] = {"actor", "critic", "alpha", "encoder", "context"};
+  for (int p = 0; p < B200SAC_RESET_PARTS; ++p) {
+    const b200sac_reset_part& q = spec->part[p];
+    if (q.layers < 0 || (p >= B200SAC_RESET_ALPHA && q.layers > 1))
+      return fail(B200SAC_ERR_INVALID, "%s: layers %d out of range", kPart[p], q.layers);
+    if (!(q.shrink >= 0.0 && q.shrink <= 1.0))       // (NaN fails both)
+      return fail(B200SAC_ERR_INVALID, "%s: shrink must be in [0, 1], got %g", kPart[p], q.shrink);
+  }
+  const b200sac_cfg& c = h->cfg;
+  if (spec->part[B200SAC_RESET_ENCODER].layers && !c.care) return fail(B200SAC_ERR_INVALID, "encoder reset on a handle without CARE");
+  if (spec->part[B200SAC_RESET_CONTEXT].layers && c.care != 2)
+    return fail(B200SAC_ERR_INVALID, "context reset on a handle that is not CARE(O)");
+
+  const Layout& L = h->L;
+  ResetArgs A;
+  memset(&A, 0, sizeof(A));
+  A.params = h->params + (size_t)replica * L.arena;
+  A.target_delta = L.target_delta;
+  A.key = seed + (uint64_t)replica;
+  for (int p = 0; p < B200SAC_RESET_PARTS; ++p) A.shrink[p] = spec->part[p].shrink;
+  int n = 0;
+  long long widest = 0;
+  for (const InitTensor& t : init_table(&c, L)) {
+    if (t.part < 0) continue;
+    const int layers = spec->part[t.part].layers;
+    if (layers == 0 || t.depth > layers) continue;
+    if (n == kResetMaxTensors) return fail(B200SAC_ERR_INVALID, "more than %d tensors to reset", kResetMaxTensors);
+    ResetTensor& r = A.t[n++];
+    r.off = t.off; r.rows = t.rows; r.cols = t.cols; r.ld = t.ld;
+    r.kind = (unsigned char)t.kind; r.part = (unsigned char)t.part; r.target = t.target ? 1 : 0;
+    r.tag = t.tag; r.c0 = (float)c.log_alpha_init;
+    widest = std::max(widest, (long long)t.rows * t.cols);
+  }
+  // optimizers that own a touched tensor: {counter slot, first trainable float, floats}
+  struct Owner { int slot; int64_t begin, n; };
+  std::vector<Owner> owners;
+  if (spec->part[B200SAC_RESET_CRITIC].layers || spec->part[B200SAC_RESET_ENCODER].layers)
+    owners.push_back({0, L.critic_begin, L.critic_n});
+  if (spec->part[B200SAC_RESET_ACTOR].layers) owners.push_back({1, L.actor_begin, L.actor_n});
+  if (spec->part[B200SAC_RESET_ALPHA].layers) owners.push_back({2, L.off_alpha, c.num_tasks > 0 ? c.num_tasks : 1});
+  if (spec->part[B200SAC_RESET_CONTEXT].layers) owners.push_back({4, L.cenc_begin, L.cenc_n});
+  if (n == 0) return 0;
+
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  const unsigned bx = (unsigned)std::min<long long>(64, (widest + 255) / 256);
+  reset_kernel<<<dim3(bx, n), 256, 0, sb.run>>>(A);
+  CU(cudaGetLastError());
+  int slots = 0;
+  const size_t nt = (size_t)L.trainable;
+  for (const Owner& o : owners) {
+    CU(cudaMemsetAsync(h->adam_m + replica * nt + o.begin, 0, o.n * sizeof(float), sb.run));
+    CU(cudaMemsetAsync(h->adam_v + replica * nt + o.begin, 0, o.n * sizeof(float), sb.run));
+    slots |= 1 << o.slot;
+  }
+  reset_counters_kernel<<<1, 1, 0, sb.run>>>(h->cnt + replica, slots);
+  CU(cudaGetLastError());
   return sb.end();
 }
 

@@ -1101,17 +1101,28 @@ __global__ void polyak_kernel(float* p, long long rsP, long long n, long long ta
   }
 }
 
+// ---- parameter init: the per-element draws b200sac_create and b200sac_reset share --------------------------------------
+// Element i of a tensor drawn under Philox key (seed + replica) and the tensor's tag.
+__device__ __forceinline__ float xavier_bound(int rows, int cols) { return sqrtf(6.f / (float)(rows + cols)); }
+__device__ __forceinline__ float xavier_draw(const Philox& ph, long long i, int tag, float bound) {
+  uint32_t rnd[4];
+  ph((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)tag, 0x1417u, rnd);
+  return (2.f * u01(rnd[0]) - 1.f) * bound;
+}
+__device__ __forceinline__ float randn_draw(const Philox& ph, long long i, int tag) {
+  uint32_t rnd[4];
+  ph((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)tag, 0x9A11u, rnd);
+  float z0, z1;
+  box_muller(rnd[0], rnd[1], z0, z1);
+  return z0;
+}
+
 // randn init of the mixture-of-encoders weights (state_encoder.py:146-153)
 __global__ void randn_kernel(float* w, long long rsP, long long n, unsigned long long seed, int tag) {
   const int rep = blockIdx.y;
   Philox ph(seed + (unsigned long long)rep);
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    uint32_t rnd[4];
-    ph((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)tag, 0x9A11u, rnd);
-    float z0, z1;
-    box_muller(rnd[0], rnd[1], z0, z1);
-    (w + rep * rsP)[i] = z0;
-  }
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    (w + rep * rsP)[i] = randn_draw(ph, i, tag);
 }
 
 // Synthetic replay fill (bench helper): rows [s | a | r | s2 | d | pad], SURVEY 8(d) distributions.
@@ -1156,13 +1167,58 @@ __global__ void fill_synthetic_kernel(float* rows, long long rs_rows, int row_st
 __global__ void xavier_kernel(float* w, long long rsP, int rows, int cols, int ld, unsigned long long seed, int tag) {
   const int rep = blockIdx.y;
   Philox ph(seed + (unsigned long long)rep);
-  const float bound = sqrtf(6.f / (float)(rows + cols));
+  const float bound = xavier_bound(rows, cols);
   const long long n = (long long)rows * cols;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    (w + rep * rsP)[(i / cols) * ld + (i % cols)] = xavier_draw(ph, i, tag, bound);
+}
+
+// b200sac_reset: every touched tensor of one replica re-drawn (theta0, the draw create made with the same key and tag)
+// and blended with its current value, the local and, where it has one, its target at + target_delta:
+//   shrink == 0: theta' = theta0 (a select, so a NaN or inf network comes back finite);
+//   otherwise:   theta' = (float)(shrink * theta + (1 - shrink) * theta0), in fp64 (the library has no FMA contraction).
+enum ResetInit { RESET_XAVIER = 0, RESET_RANDN = 1, RESET_ZERO = 2, RESET_CONST = 3 };
+struct ResetTensor {
+  long long off;                 // in floats, inside the replica's arena
+  int rows, cols, ld;            // element i sits at (i / cols) * ld + i % cols: pad columns are not written
+  unsigned char kind, part, target, pad;   // ResetInit; b200sac_reset part (index of shrink); 1 = has a target copy
+  int tag;                       // Philox tag (XAVIER / RANDN)
+  float c0;                      // CONST: the value
+};
+constexpr int kResetMaxTensors = 112;   // actor 18 + q1, q2 36 + encoder 54 or encoder 36 + context 18, + log_alpha
+struct ResetArgs {
+  float* params;                 // the replica's arena
+  long long target_delta;
+  unsigned long long key;        // seed + replica
+  double shrink[5];
+  ResetTensor t[kResetMaxTensors];
+};
+
+__device__ __forceinline__ float reset_blend(float x, float th0, double lam) {
+  return lam == 0.0 ? th0 : (float)(lam * (double)x + (1.0 - lam) * (double)th0);
+}
+
+__global__ void __launch_bounds__(256) reset_kernel(const __grid_constant__ ResetArgs A) {
+  const ResetTensor& t = A.t[blockIdx.y];
+  const Philox ph(A.key);
+  const double lam = A.shrink[t.part];
+  const float bound = xavier_bound(t.rows, t.cols);
+  const long long n = (long long)t.rows * t.cols;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    uint32_t rnd[4];
-    ph((uint32_t)i, (uint32_t)(i >> 32), (uint32_t)tag, 0x1417u, rnd);
-    (w + rep * rsP)[(i / cols) * ld + (i % cols)] = (2.f * u01(rnd[0]) - 1.f) * bound;
+    float th0 = t.c0;
+    if (t.kind == RESET_XAVIER) th0 = xavier_draw(ph, i, t.tag, bound);
+    else if (t.kind == RESET_RANDN) th0 = randn_draw(ph, i, t.tag);
+    else if (t.kind == RESET_ZERO) th0 = 0.f;
+    float* p = A.params + t.off + (i / t.cols) * t.ld + (i % t.cols);
+    *p = reset_blend(*p, th0, lam);
+    if (t.target) p[A.target_delta] = reset_blend(p[A.target_delta], th0, lam);
   }
+}
+
+// A fresh Adam state's counters (what b200sac_create writes) in the slots whose bit is set; the step index v[3] is kept.
+__global__ void reset_counters_kernel(Counters* c, int slots) {
+  for (int s = 0; s < 5; ++s)
+    if ((slots >> s) & 1) { c->v[s] = 0; c->b1p[s] = 1.0; c->b2p[s] = 1.0; }
 }
 
 }  // namespace bsac

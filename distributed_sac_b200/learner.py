@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib, names
-from .core import CoreConfig, Replay, SacCore
+from .core import CoreConfig, Replay, SacCore, reset_spec
 from .replay_buffer import ReplayBuffer, MTReplayBuffer
 
 
@@ -86,7 +86,7 @@ class _BaseLearner:
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
-                     n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None):
+                     n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -117,6 +117,19 @@ class _BaseLearner:
                                  f"num_tasks {self.num_tasks})")
             if not (math.isfinite(self.cagrad) and self.cagrad >= 0):
                 raise ValueError(f"cagrad must be finite and >= 0 (got {cagrad})")
+        # periodic network resets (primacy bias at high replay ratios; Nikishin et al. 2022, D'Oro et al. 2023): reset k
+        # (k = 1, 2, ...) with seed + k * 2^32 right before update k * reset_interval + 1, counted from construction
+        if reset is not None and reset_interval is None:
+            raise ValueError("reset= needs reset_interval=")
+        if reset_interval is not None and (isinstance(reset_interval, bool) or not isinstance(reset_interval, int)
+                                           or reset_interval < 1):
+            raise ValueError(f"reset_interval must be an int >= 1 (got {reset_interval!r})")
+        self.reset_interval = reset_interval
+        self.reset = dict(reset or {})
+        reset_spec(self._core_config(), **self.reset)          # ValueError on bad parts, before a handle is built
+        self.seed = int(seed)
+        self._n_updates = 0
+        self._n_manual_resets = 0
         self.device = torch.device(self.cfg.get("device", "cuda"))
         if self.device.type != "cuda":
             raise RuntimeError("the CUDA learner only runs on CUDA devices (cfg 'device' must be 'cuda')")
@@ -193,25 +206,51 @@ class _BaseLearner:
                           pcgrad=self.pcgrad or self.cagrad is not None)
 
     # ---- reference method surface -------------------------------------------------------------
+    def _chunks(self, n):
+        """Split n updates at the reset boundaries: yields the sizes of the runs of updates to enqueue, and enqueues reset k
+        (seed + k * 2^32) right before update k * reset_interval + 1."""
+        N = self.reset_interval
+        while n > 0:
+            u = self._n_updates
+            if N is not None and u > 0 and u % N == 0:
+                self.core.reset(self.seed + (u // N) * 2 ** 32, **self.reset)
+            c = n if N is None else min(n, N - u % N)
+            yield c
+            self._n_updates += c
+            n -= c
+
+    def reset_networks(self, seed=None, **parts):
+        """Reset networks now, on the current stream (SacCore.reset's part keywords and shrink; none = a full reset).
+        seed=None: the j-th such call uses seed + 2^63 + j * 2^32, apart from the scheduled resets' seeds.  Not part of
+        the update count that reset_interval follows; that count starts at construction (a loaded checkpoint included),
+        as the reference's checkpoint format does not hold it."""
+        if seed is None:
+            self._n_manual_resets += 1
+            seed = self.seed + 2 ** 63 + self._n_manual_resets * 2 ** 32
+        self.core.reset(seed, **parts)
+
     def update(self):
         """Learner.update(): sample a minibatch, one SAC gradient step, return python floats."""
-        l = self.memory.step_core(self.core)          # (critic, actor, alpha loss, entropy) python floats
+        for _ in self._chunks(1):
+            l = self.memory.step_core(self.core)      # (critic, actor, alpha loss, entropy) python floats
         return (l[0], l[1]) if self.num_tasks == 0 else (l[0], l[1], l[3])
 
     def update_SAC(self, states, actions, rewards, next_states, dones, alpha=None, retain_graph=False,
                    eps_next=None, eps_cur=None):
         """Learner.update_SAC() on an explicit minibatch (device or host tensors).  `alpha` is accepted
         for signature compatibility; the step uses exp(log_alpha) snapshotted in-kernel exactly like update()."""
-        if states.is_cuda:
-            self.core.step(states, actions, rewards, next_states, dones, eps_next, eps_cur)
-            losses = self.core.read_losses(1)[0]
-        else:
-            losses = self.core.step_host(states, actions, rewards, next_states, dones, eps_next, eps_cur)
+        for _ in self._chunks(1):
+            if states.is_cuda:
+                self.core.step(states, actions, rewards, next_states, dones, eps_next, eps_cur)
+                losses = self.core.read_losses(1)[0]
+            else:
+                losses = self.core.step_host(states, actions, rewards, next_states, dones, eps_next, eps_cur)
         return self._loss_tuple(losses)
 
     def update_many(self, n):
         """n pipelined update() calls; returns a [n][k] tensor of the per-step losses."""
-        self.core.step_sampled(self.memory.ring, n)
+        for c in self._chunks(n):
+            self.core.step_sampled(self.memory.ring, c)
         L = self.core.read_losses(min(n, 1024))[:, 0]
         return L[:, [0, 1]] if self.num_tasks == 0 else L[:, [0, 1, 3]]
 
@@ -412,7 +451,8 @@ class _BaseLearner:
         iters = (i for i in itertools.count() if i % self.update_delay == 0)
         update_iteration = next(iters)
         core = self.core
-        self.memory.enqueue_step(core)                 # update(), split so that everything below overlaps the GPU
+        for _ in self._chunks(1):
+            self.memory.enqueue_step(core)             # update(), split so that everything below overlaps the GPU
         core.blob_begin()
         while True:
             cur = update_iteration
@@ -422,7 +462,8 @@ class _BaseLearner:
                 self.save_checkpoint(cur)              # before step cur+1 is enqueued: the arena is the state after `cur`
             if not last:                               # the GPU goes on with step cur+1 while blob `cur` is still crossing PCIe
                 update_iteration = next(iters)
-                self.memory.enqueue_step(core)
+                for _ in self._chunks(1):              # a scheduled reset lands after checkpoint `cur` and blob `cur`
+                    self.memory.enqueue_step(core)
                 core.blob_begin()
             blob, extra = core.blob_wait()             # the OLDEST uncollected blob = the one of step `cur`
             self.server.set("update_iteration", _pickle.dumps(cur))
@@ -471,12 +512,12 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
-                 pcgrad=False, cagrad=None):
+                 pcgrad=False, cagrad=None, reset_interval=None, reset=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad)
+                          cagrad, reset_interval, reset)
 
     def _set_dims(self):
         c = self.cfg
@@ -500,10 +541,10 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None):
+                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad)
+                          cagrad, reset_interval, reset)
 
     def _set_dims(self):
         c = self.cfg
@@ -531,11 +572,11 @@ class MTSACLearner(_BaseLearner):
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
-                 cagrad=None):
+                 cagrad=None, reset_interval=None, reset=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad)
+                          cagrad, reset_interval, reset)
 
     def _set_dims(self):
         c = self.cfg

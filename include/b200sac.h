@@ -21,6 +21,8 @@
  *   b200sac_soft_update      Learner.soft_update()            learner.py:126-137
  *   b200sac_get/set_hparams, b200sac_copy_replica
  *                            the hyperparameters build_optimizer / update_SAC / soft_update fix per learner, made per replica
+ *   b200sac_reset            build_model + build_optimizer again for some networks of one replica (periodic resets,
+ *                            shrink-and-perturb), keeping the replay ring
  *                            LunarLander_Distributed_SAC/src/learner.py:115-137,210; MT10_Distributed_CARE/src/learner.py:136-158,361-367
  *   b200sac_get/set_update_intervals
  *                            actor / target update intervals (TD3 policy_delay, pytorch_sac actor_update_frequency and
@@ -180,6 +182,52 @@ int b200sac_set_hparams(b200sac_t* h, int32_t replica, const b200sac_hparams* hp
  * round trip (the exploit step of population-based training).  Hyperparameters, update intervals, gradient-clipping
  * thresholds, gradients and replay rings are not copied. */
 int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void* stream);
+
+/* Network resets and shrink-and-perturb, per replica (Nikishin et al. 2022; D'Oro et al. 2023; Ash & Adams 2020).
+ * Parts a reset can touch, index of b200sac_reset_spec.part[]:
+ *   ACTOR    the actor MLP (actor.*);
+ *   CRITIC   q1 and q2, the same depth for both; their targets follow;
+ *   ALPHA    log_alpha, every task;
+ *   ENCODER  the CARE critic state encoder cse.* (mixture, attention trunk and, CARE(M), the context MLP); its target tse
+ *            follows, and so does the actor's state encoder, which is its tied copy.  Not on a non-CARE handle;
+ *   CONTEXT  the CARE(O) context encoder cenc.*.  Only on CARE(O) handles.
+ * The frozen CARE embedding is never touched. */
+enum { B200SAC_RESET_ACTOR = 0, B200SAC_RESET_CRITIC = 1, B200SAC_RESET_ALPHA = 2,
+       B200SAC_RESET_ENCODER = 3, B200SAC_RESET_CONTEXT = 4, B200SAC_RESET_PARTS = 5 };
+typedef struct b200sac_reset_part {
+  int32_t layers;   /* ACTOR / CRITIC: Linear layers counted from the output layer (1 = the head only); 0 = untouched;
+                       >= the network's Linear count = all.  ALPHA / ENCODER / CONTEXT: 0 or 1 (all or nothing). */
+  int32_t reserved;
+  double shrink;    /* lambda in [0, 1]: 0 = fresh draw, 1 = keep the values (the optimizer state is still reset) */
+} b200sac_reset_part;
+typedef struct b200sac_reset_spec { b200sac_reset_part part[B200SAC_RESET_PARTS]; } b200sac_reset_spec;
+
+/* Enqueued on `stream`: re-initialise the parts `spec` names of replica `replica`.
+ * Fresh draw theta0 of every touched tensor: what b200sac_create(seed) gives replica `replica` -- the same Philox key
+ * (seed + replica) and per-tensor tag, Xavier-uniform weights, zero biases, N(0,1) CARE mixture weights and biases,
+ * cfg.log_alpha_init for log_alpha.  A reset with the create seed and shrink 0 therefore reproduces the created
+ * parameters bit for bit.
+ * Blend, per element, lambda = the part's shrink:
+ *   lambda = 0: theta' = theta0 (a select: a reset also recovers a NaN or inf network);
+ *   otherwise:  theta' = (float)(lambda * theta + (1 - lambda) * theta0), evaluated in fp64 with 1 - lambda in fp64 and
+ *               rounded once, no fused multiply-add.
+ * A touched critic or state-encoder tensor's target gets the same blend of its own value with the same theta0, so at
+ * lambda = 0 the targets equal the new locals, as after create.  Pad columns of first-layer weights stay zero.
+ * Optimizer state: every optimizer that owns a touched tensor starts afresh, as if the torch optimizer were re-created:
+ * Adam m = v = 0 over its whole slice, its step count 0 and its beta-power products 1 (the values create writes).  The
+ * owners are the critic (counter slot 0: q1, q2 and cse) for CRITIC or ENCODER, the actor (slot 1) for ACTOR, the
+ * temperature (slot 2) for ALPHA and the context encoder (slot 4) for CONTEXT.  This is all or nothing per optimizer,
+ * because the counters are per optimizer, not per tensor: a head-only critic reset restarts Adam for all of q1, q2 and cse.
+ * Left alone: the step index (the Philox noise stream and the loss-ring slots continue), gradient arenas and PCGrad
+ * slices, every per-replica setting (hyperparameters, update intervals, clip thresholds, PCGrad / CAGrad), replay rings,
+ * PER priorities and n-step links, and the other replicas.  The update-interval phase follows the critic count, as after
+ * b200sac_set_steps: a critic reset restarts it.
+ * Stream order as b200sac_set_hparams: steps enqueued before the call are unaffected and steps enqueued after it see the
+ * reset, including launches of the graphs b200sac_prepare instantiated (no graph is rebuilt); b200sac_act and the next
+ * b200sac_blob_begin see the new actor.
+ * A NULL spec, a bad replica, layers < 0, an all-or-nothing part with layers > 1, shrink outside [0, 1] or NaN, ENCODER on
+ * a non-CARE handle or CONTEXT on a handle that is not CARE(O) give B200SAC_ERR_INVALID, and nothing is enqueued. */
+int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_spec* spec, uint64_t seed, void* stream);
 
 /* Per-replica update intervals, both 1 (every step is a full step) after b200sac_create.  Let n be the replica's critic
  * Adam step count after a step (steps[0] of b200sac_get_steps).  The step is
