@@ -75,6 +75,8 @@ SYMBOLS = {
     "b200sac_set_hparams": (C.c_int, [_VP, C.c_int32, C.POINTER(Hparams), _VP]),
     "b200sac_copy_replica": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
     "b200sac_reset": (C.c_int, [_VP, C.c_int32, C.POINTER(ResetSpec), C.c_uint64, _VP]),
+    "b200sac_redo": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_double, C.c_double, C.c_uint64, _VP]),
+    "b200sac_read_redo": (C.c_int, [_VP, C.c_int32, _VP, _VP, C.c_int64, C.POINTER(C.c_int64), _VP]),
     "b200sac_set_update_intervals": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, _VP]),
     "b200sac_get_update_intervals": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_set_grad_clip": (C.c_int, [_VP, C.c_int32, C.c_double, C.c_double, C.c_double, _VP]),

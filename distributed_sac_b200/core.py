@@ -5,6 +5,7 @@ runs in the CUDA library.  The reference-shaped `Learner` classes
 (distributed_sac_b200/learner.py) are built on this.
 """
 import ctypes as C
+import math
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -165,6 +166,24 @@ def reset_spec(cfg: CoreConfig, shrink=0.0, **parts):
             raise ValueError(f"this handle has no {k} to reset (parts: {have})")
         spec.part[i].layers = int(v)
     return spec
+
+
+REDO_NETS = ("actor", "q1", "q2")        # the order of b200sac_redo's record
+
+
+def redo_taus(actor=None, critic=None):
+    """(tau_actor, tau_critic) of SacCore.redo's keywords (pure host function).  A threshold tau: neurons whose score is
+    <= tau are recycled; None = score only (-inf: a negative tau recycles nothing).  Raises ValueError on anything that is
+    not a number and on NaN."""
+    out = []
+    for k, v in (("actor", actor), ("critic", critic)):
+        if v is None:
+            out.append(-math.inf)
+            continue
+        if isinstance(v, (bool, np.bool_)) or not isinstance(v, (int, float, np.integer, np.floating)) or math.isnan(float(v)):
+            raise ValueError(f"{k} takes a dormancy threshold (a number, not NaN) or None, got {v!r}")
+        out.append(float(v))
+    return tuple(out)
 
 
 class SacCore:
@@ -493,6 +512,42 @@ class SacCore:
         spec = reset_spec(self.cfg, shrink, actor=actor, critic=critic, alpha=alpha, encoder=encoder, context=context)
         for r in _replicas(self.cfg.replicas, replica):
             _lib.check(self.lib.b200sac_reset(self._h, r, C.byref(spec), C.c_uint64(int(seed) % (1 << 64)), _stream()))
+
+    def redo(self, seed: int, obs, act, actor=None, critic=None, replica=None):
+        """Dormant-neuron recycling (ReDo) of one replica (replica=None: every replica, each under its own key seed +
+        replica) on the current stream.  Scores every hidden neuron of the actor, q1 and q2 on the rows obs [n][obs_dim]
+        and act [n][act_dim] (1 <= n <= batch, CPU or CUDA), then recycles those whose score is <= the network's threshold:
+        actor= for the actor, critic= for q1 and q2; None = score only.  Recycled rows take b200sac_create(seed)'s draw,
+        their biases and outgoing weights and the Adam moments there become 0 (include/b200sac.h).  read_redo() shows the
+        record; steps enqueued afterwards see the recycled networks."""
+        ta, tc = redo_taus(actor, critic)
+        obs = obs.to(torch.float32).contiguous()
+        act = act.to(torch.float32).contiguous()
+        n = obs.shape[0]
+        if obs.shape != (n, self.cfg.obs_dim) or act.shape != (n, self.cfg.act_dim):
+            raise ValueError(f"obs must be [n][{self.cfg.obs_dim}] and act [n][{self.cfg.act_dim}], got {tuple(obs.shape)} "
+                             f"and {tuple(act.shape)}")
+        for r in _replicas(self.cfg.replicas, replica):
+            _lib.check(self.lib.b200sac_redo(self._h, r, n, _ptr(obs), _ptr(act), ta, tc, C.c_uint64(int(seed) % (1 << 64)),
+                                             _stream()))
+
+    def read_redo(self, replica=0) -> Dict[str, Dict[str, List[np.ndarray]]]:
+        """The last redo() record of one replica: {"actor" | "q1" | "q2": {"score": [fp64 per hidden layer], "dormant":
+        [bool per hidden layer]}}; NaN scores and no dormant neuron before the first call."""
+        n = C.c_int64(0)
+        _lib.check(self.lib.b200sac_read_redo(self._h, int(replica), None, None, 0, C.byref(n), _stream()))
+        score, flag = np.empty(n.value, np.float64), np.empty(n.value, np.uint8)
+        _lib.check(self.lib.b200sac_read_redo(self._h, int(replica), C.c_void_p(score.ctypes.data),
+                                              C.c_void_p(flag.ctypes.data), n.value, C.byref(n), _stream()))
+        out, i = {}, 0
+        for net in REDO_NETS:
+            widths = self.cfg.actor_hidden if net == "actor" else self.cfg.critic_hidden
+            out[net] = {"score": [], "dormant": []}
+            for H in widths:
+                out[net]["score"].append(score[i:i + H])
+                out[net]["dormant"].append(flag[i:i + H].astype(bool))
+                i += H
+        return out
 
     def soft_update(self, tau: float, critic: Optional[int] = None):
         """Polyak update of the targets outside a step: both critics (CARE: and the target state encoder, with the replica's

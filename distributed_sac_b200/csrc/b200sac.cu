@@ -36,6 +36,7 @@
 #include "nstep_kernels.cuh"
 #include "clip_kernels.cuh"
 #include "pcgrad_kernels.cuh"
+#include "redo_kernels.cuh"
 
 using namespace bsac;
 
@@ -487,6 +488,11 @@ struct b200sac {
   float* gnorm_h_dev = nullptr;
   DevMem<double> gn_part;
   DevMem<unsigned> gn_ticket;
+  // dormant-neuron recycling (b200sac_redo): the last call's record per replica, [R][redo_n] neuron scores (NaN until a
+  // call writes them) and dormant flags, redo_n = the hidden neurons of the actor, q1 and q2
+  DevMem<double> redo_score;
+  DevMem<uint8_t> redo_flag;
+  int64_t redo_n = 0;
   // gradient surgery (cfg.pcgrad): [R][2] switches (critic, actor), the pcgrad launches' partial products
   // [2][R][kGradNormMaxBlocks][T(T+1)/2] and tickets [2][R], the last step's record per replica and optimizer
   // (G [R][2][T][T], w [R][2][T] -- also what Adam reads --, permutations [R][2][T][T], projection masks [R][2][T]) and
@@ -2071,6 +2077,15 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMalloc(h->gn_ticket.put(), sizeof(unsigned) * n));
     CU(cudaMemset(h->gn_ticket, 0, sizeof(unsigned) * n));
   }
+  {                           // ReDo record: scores NaN (all-ones bytes), flags 0
+    for (int l = 0; l < cfg->n_actor_hidden; ++l) h->redo_n += cfg->actor_hidden[l];
+    for (int l = 0; l < cfg->n_critic_hidden; ++l) h->redo_n += 2 * cfg->critic_hidden[l];
+    const size_t n = (size_t)h->redo_n * R;
+    CU(cudaMalloc(h->redo_score.put(), sizeof(double) * n));
+    CU(cudaMemset(h->redo_score, 0xFF, sizeof(double) * n));
+    CU(cudaMalloc(h->redo_flag.put(), n));
+    CU(cudaMemset(h->redo_flag, 0, n));
+  }
   if (cfg->pcgrad) {          // switches on, weights 1, record NaN until a step writes it
     const int T = cfg->num_tasks;
     const size_t n2 = (size_t)2 * R;
@@ -3167,8 +3182,9 @@ static void act_gemm(const std::vector<GemmProb>& ps, cudaStream_t st) {
 
 // CARE actors (MT10_Distributed_CARE/src/player.py:199-209: z = context_encoder(mtobs); actor.get_action(mtobs, z)):
 // encode the n observation rows sitting in XS[0..n) of `replica` with the critic's state encoder -- the actor's is its
-// hard copy (learner.py:402) -- into XA[0..n): per-task tables, K mixture encoders, attention mix.
-static int care_encode_rows(b200sac* h, cudaStream_t st, int replica, int n) {
+// hard copy (learner.py:402) -- into XA[0..n) and, when d2.p is set, into d2's rows [0, n) too (pitch ld2; b200sac_redo's
+// critic input XQ): per-task tables, K mixture encoders, attention mix.
+static int care_encode_rows(b200sac* h, cudaStream_t st, int replica, int n, Buf d2 = Buf{}, int ld2 = 0) {
   act_task_ids_kernel<<<(n + 255) / 256, 256, 0, st>>>(rep_view(h->XS, replica).p, h->K.obs, h->cfg.num_tasks, n,
                                                        (int*)rep_view(h->tid, replica).p);
   care_tables_kernel<<<dim3(h->cfg.num_tasks, 1, 1), 512, 0, st>>>(care_tab_args(h, replica, {0}));
@@ -3177,7 +3193,7 @@ static int care_encode_rows(b200sac* h, cudaStream_t st, int replica, int n) {
     mix_fwd_probs(h, replica, 0, l, 0, n, ps);
     act_gemm(ps, st);
   }
-  const EncJob job{0, 0, n, rep_view(h->XA, replica), h->K.ldxa, Buf{}, 0, 0};
+  const EncJob job{0, 0, n, rep_view(h->XA, replica), h->K.ldxa, d2, ld2, 0};
   care_mix_kernel<<<dim3((n + 7) / 8, 1), 256, 0, st>>>(care_mix_args(h, replica, job));
   CU(cudaGetLastError());
   return 0;
@@ -3233,6 +3249,98 @@ extern "C" int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(actions_out, h->act_out.p + (long long)replica * h->act_out.rs, (size_t)n * A * sizeof(float), cudaMemcpyDefault, st));
   if (int rc = sb.end()) return rc;
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
+// Dormant-neuron recycling (include/b200sac.h): the forward of b200sac_act's engine over (obs, act) into the step's XA / XQ /
+// hA / hQ rows [0, n), then redo_score_kernel and, unless both thresholds are negative, redo_recycle_kernel.
+extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* act, double tau_actor,
+                            double tau_critic, uint64_t seed, void* stream) {
+  if (!h || !obs || !act) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  const b200sac_cfg& c = h->cfg;
+  const int B = c.batch, A = c.act_dim, La = c.n_actor_hidden, Lc = c.n_critic_hidden;
+  if (n < 1 || n > B) return fail(B200SAC_ERR_INVALID, "n must be in [1, batch = %d], got %d", B, n);
+  if (std::isnan(tau_actor) || std::isnan(tau_critic)) return fail(B200SAC_ERR_INVALID, "tau must not be NaN");
+  const Layout& L = h->L;
+  RedoArgs RA;
+  memset(&RA, 0, sizeof(RA));
+  const size_t nt = (size_t)L.trainable;
+  RA.params = h->params + (size_t)replica * L.arena;
+  RA.m = h->adam_m + replica * nt; RA.v = h->adam_v + replica * nt;
+  RA.score = h->redo_score + replica * h->redo_n; RA.dormant = h->redo_flag + replica * h->redo_n;
+  RA.key = seed + (uint64_t)replica;
+  RA.tau[0] = tau_actor; RA.tau[1] = tau_critic;
+  RA.n = n;
+  std::unordered_map<int64_t, int> tag;                  // weight offset -> its Philox tag, as create drew it
+  for (const InitTensor& t : init_table(&c, L))
+    if (t.kind == RESET_XAVIER) tag[t.off] = t.tag;
+  long long rec = 0, widest = 0;
+  auto layers = [&](const std::vector<LayerOff>& net, int nh, const std::vector<Buf>& hb, int net_idx, int critic) {
+    for (int l = 0; l < nh; ++l) {
+      const LayerOff &lo = net[l], &nx = net[l + 1];
+      RedoLayer& t = RA.l[RA.nl++];
+      t.h = rep_view(hb[l], replica).p + (long long)net_idx * B * lo.out;
+      t.rec = rec; t.w = lo.w; t.b = lo.b; t.wn = nx.w; t.next_rec = l + 1 < nh ? rec + lo.out : -1;
+      t.H = lo.out; t.in = lo.in; t.ld = lo.ld; t.next_out = nx.out; t.tag = tag.at(lo.w); t.critic = critic;
+      rec += lo.out;
+      widest = std::max(widest, (long long)lo.out * (lo.in + 1 + nx.out));
+    }
+  };
+  layers(L.actor, La, h->hA, 0, 0);
+  layers(L.q[0], Lc, h->hQ, 0, 1);
+  layers(L.q[1], Lc, h->hQ, 1, 1);
+
+  CU(cudaSetDevice(h->device));
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  cudaStream_t st = sb.run;
+  const int obs_w = h->K.obs, ldx = h->K.ldx;
+  const Buf XA = rep_view(h->XA, replica), XQ = rep_view(h->XQ, replica);
+  if (c.care) {
+    CU(cudaMemcpyAsync(rep_view(h->XS, replica).p, obs, (size_t)n * obs_w * sizeof(float), cudaMemcpyDefault, st));
+    if (int rc = care_encode_rows(h, st, replica, n, XQ, ldx)) return rc;
+  } else {
+    for (const auto& [X, ld] : {std::make_pair(XA.p, h->K.ldxa), std::make_pair(XQ.p, ldx)})
+      CU(cudaMemcpy2DAsync(X, (size_t)ld * sizeof(float), obs, (size_t)obs_w * sizeof(float), (size_t)obs_w * sizeof(float),
+                           (size_t)n, cudaMemcpyDefault, st));
+  }
+  CU(cudaMemcpy2DAsync(XQ.p + L.in_w, (size_t)ldx * sizeof(float), act, (size_t)A * sizeof(float), (size_t)A * sizeof(float),
+                       (size_t)n, cudaMemcpyDefault, st));
+  const Buf par = rep_view(Buf{h->params, L.arena}, replica);
+  for (int l = 0; l < La; ++l) {
+    const Buf X = rep_view(l == 0 ? h->XA : h->hA[l - 1], replica), out = rep_view(h->hA[l], replica);
+    act_gemm({fwd_prob(par, X.p, X.rs, n, L.actor[l], out.p, out.rs)}, st);
+  }
+  for (int l = 0; l < Lc; ++l) {           // q1 and q2 in one launch: equal shapes
+    std::vector<GemmProb> ps;
+    for (int net = 0; net < 2; ++net) {
+      const LayerOff& lo = L.q[net][l];
+      const float* X = l == 0 ? XQ.p : rep_view(h->hQ[l - 1], replica).p + (long long)net * B * lo.in;
+      ps.push_back(fwd_prob(par, X, 0, n, lo, rep_view(h->hQ[l], replica).p + (long long)net * B * lo.out, 0));
+    }
+    act_gemm(ps, st);
+  }
+  redo_score_kernel<<<RA.nl, kRedoThreads, 0, st>>>(RA);
+  if (tau_actor >= 0.0 || tau_critic >= 0.0) {
+    const unsigned bx = (unsigned)std::min<long long>(64, (widest + kRedoThreads - 1) / kRedoThreads);
+    redo_recycle_kernel<<<dim3(bx, RA.nl), kRedoThreads, 0, st>>>(RA);
+  }
+  CU(cudaGetLastError());
+  return sb.end();
+}
+
+extern "C" int b200sac_read_redo(b200sac_t* h, int32_t replica, double* scores, uint8_t* dormant, int64_t cap,
+                                 int64_t* n_neurons, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (n_neurons) *n_neurons = h->redo_n;
+  if ((scores || dormant) && cap < h->redo_n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld", (long long)h->redo_n);
+  CU(cudaSetDevice(h->device));
+  const size_t n = (size_t)h->redo_n;
+  if (scores) CU(cudaMemcpyAsync(scores, h->redo_score + replica * n, n * sizeof(double), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
+  if (dormant) CU(cudaMemcpyAsync(dormant, h->redo_flag + replica * n, n, cudaMemcpyDeviceToHost, (cudaStream_t)stream));
   CU(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
 }

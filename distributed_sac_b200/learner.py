@@ -28,7 +28,7 @@ import numpy as np
 import torch
 
 from . import _lib, names
-from .core import CoreConfig, Replay, SacCore, reset_spec
+from .core import REDO_NETS, CoreConfig, Replay, SacCore, redo_taus, reset_spec
 from .replay_buffer import ReplayBuffer, MTReplayBuffer
 
 
@@ -86,7 +86,8 @@ class _BaseLearner:
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
-                     n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None):
+                     n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
+                     redo_interval=None, redo=None):
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -127,9 +128,20 @@ class _BaseLearner:
         self.reset_interval = reset_interval
         self.reset = dict(reset or {})
         reset_spec(self._core_config(), **self.reset)          # ValueError on bad parts, before a handle is built
+        # periodic dormant-neuron recycling (ReDo; Sokar et al. 2023): recycle k with seed + 2^62 + k * 2^32 right before
+        # update k * redo_interval + 1, after a reset that falls on the same update; redo = {actor: tau, critic: tau}
+        # (default: tau 0 for both, the neurons that are dead on the batch)
+        if redo is not None and redo_interval is None:
+            raise ValueError("redo= needs redo_interval=")
+        if redo_interval is not None and (isinstance(redo_interval, bool) or not isinstance(redo_interval, int)
+                                          or redo_interval < 1):
+            raise ValueError(f"redo_interval must be an int >= 1 (got {redo_interval!r})")
+        self.redo_interval = redo_interval
+        self.redo = self._redo_taus(dict(actor=0.0, critic=0.0) if redo is None else redo)
         self.seed = int(seed)
         self._n_updates = 0
         self._n_manual_resets = 0
+        self._n_manual_redos = 0
         self.device = torch.device(self.cfg.get("device", "cuda"))
         if self.device.type != "cuda":
             raise RuntimeError("the CUDA learner only runs on CUDA devices (cfg 'device' must be 'cuda')")
@@ -207,17 +219,33 @@ class _BaseLearner:
 
     # ---- reference method surface -------------------------------------------------------------
     def _chunks(self, n):
-        """Split n updates at the reset boundaries: yields the sizes of the runs of updates to enqueue, and enqueues reset k
-        (seed + k * 2^32) right before update k * reset_interval + 1."""
-        N = self.reset_interval
+        """Split n updates at the reset and recycle boundaries: yields the sizes of the runs of updates to enqueue, and
+        enqueues reset k (seed + k * 2^32) right before update k * reset_interval + 1 and recycle k (seed + 2^62 + k * 2^32)
+        right before update k * redo_interval + 1, the reset first when both fall on one update."""
+        Ns = [N for N in (self.reset_interval, self.redo_interval) if N is not None]
         while n > 0:
             u = self._n_updates
-            if N is not None and u > 0 and u % N == 0:
-                self.core.reset(self.seed + (u // N) * 2 ** 32, **self.reset)
-            c = n if N is None else min(n, N - u % N)
+            if u > 0 and self.reset_interval is not None and u % self.reset_interval == 0:
+                self.core.reset(self.seed + (u // self.reset_interval) * 2 ** 32, **self.reset)
+            if u > 0 and self.redo_interval is not None and u % self.redo_interval == 0:
+                self._recycle(self.seed + 2 ** 62 + (u // self.redo_interval) * 2 ** 32, self.redo)
+            c = min([n] + [N - u % N for N in Ns])
             yield c
             self._n_updates += c
             n -= c
+
+    @staticmethod
+    def _redo_taus(taus):
+        """{actor: tau, critic: tau} checked (redo_taus' rules; a network left out is scored only).  Raises ValueError."""
+        if not isinstance(taus, dict) or set(taus) - {"actor", "critic"}:
+            raise ValueError(f"redo takes dict(actor=tau, critic=tau), got {taus!r}")
+        redo_taus(**taus)
+        return dict(taus)
+
+    def _recycle(self, seed, taus):
+        """One SacCore.redo on a fresh reference-shaped draw from the ring (a prioritized ring's weights are ignored)."""
+        s, a = self.memory.sample()[:2]
+        self.core.redo(seed, s, a, **taus)
 
     def reset_networks(self, seed=None, **parts):
         """Reset networks now, on the current stream (SacCore.reset's part keywords and shrink; none = a full reset).
@@ -228,6 +256,24 @@ class _BaseLearner:
             self._n_manual_resets += 1
             seed = self.seed + 2 ** 63 + self._n_manual_resets * 2 ** 32
         self.core.reset(seed, **parts)
+
+    def recycle_dormant(self, seed=None, **taus):
+        """Recycle dormant neurons now, on the current stream, scored on a fresh replay batch: actor= / critic= thresholds
+        (none given: the learner's redo= thresholds).  seed=None: the j-th such call uses seed + 2^63 + 2^62 + j * 2^32,
+        apart from the reset and scheduled recycle seeds.  Not part of the update count that redo_interval follows."""
+        taus = self.redo if not taus else self._redo_taus(taus)
+        if seed is None:
+            self._n_manual_redos += 1
+            seed = self.seed + 2 ** 63 + 2 ** 62 + self._n_manual_redos * 2 ** 32
+        self._recycle(seed, taus)
+
+    def dormant_fraction(self, tau=0.0):
+        """The fraction of tau-dormant neurons (score <= tau) per network and hidden layer on a fresh replay batch: a
+        measure-only recycle call, nothing changes.  {"actor" | "q1" | "q2": [fraction per hidden layer]}."""
+        redo_taus(tau, tau)
+        self._recycle(self.seed, {})
+        rec = self.core.read_redo()
+        return {net: [float(np.mean(s <= tau)) for s in rec[net]["score"]] for net in REDO_NETS}
 
     def update(self):
         """Learner.update(): sample a minibatch, one SAC gradient step, return python floats."""
@@ -512,12 +558,12 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
-                 pcgrad=False, cagrad=None, reset_interval=None, reset=None):
+                 pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset)
+                          cagrad, reset_interval, reset, redo_interval, redo)
 
     def _set_dims(self):
         c = self.cfg
@@ -541,10 +587,11 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
 
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
-                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None):
+                 target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
+                 redo_interval=None, redo=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset)
+                          cagrad, reset_interval, reset, redo_interval, redo)
 
     def _set_dims(self):
         c = self.cfg
@@ -572,11 +619,11 @@ class MTSACLearner(_BaseLearner):
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
-                 cagrad=None, reset_interval=None, reset=None):
+                 cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset)
+                          cagrad, reset_interval, reset, redo_interval, redo)
 
     def _set_dims(self):
         c = self.cfg

@@ -24,6 +24,8 @@
  *   b200sac_reset            build_model + build_optimizer again for some networks of one replica (periodic resets,
  *                            shrink-and-perturb), keeping the replay ring
  *                            LunarLander_Distributed_SAC/src/learner.py:115-137,210; MT10_Distributed_CARE/src/learner.py:136-158,361-367
+ *   b200sac_redo, b200sac_read_redo
+ *                            dormant-neuron recycling (ReDo) of one replica and its record of neuron scores
  *   b200sac_get/set_update_intervals
  *                            actor / target update intervals (TD3 policy_delay, pytorch_sac actor_update_frequency and
  *                            critic_target_update_frequency, SB3 target_update_interval), per replica
@@ -228,6 +230,44 @@ typedef struct b200sac_reset_spec { b200sac_reset_part part[B200SAC_RESET_PARTS]
  * A NULL spec, a bad replica, layers < 0, an all-or-nothing part with layers > 1, shrink outside [0, 1] or NaN, ENCODER on
  * a non-CARE handle or CONTEXT on a handle that is not CARE(O) give B200SAC_ERR_INVALID, and nothing is enqueued. */
 int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_spec* spec, uint64_t seed, void* stream);
+
+/* Dormant-neuron recycling, ReDo (Sokar, Agarwal, Castro, Evci, ICML 2023), per replica.  Enqueued on `stream`:
+ * 1. Forward.  With replica `replica`'s current parameters, the actor's hidden layers on obs[n][state_dim + num_tasks]
+ *    and q1's and q2's on (obs, act[n][act_dim]), 1 <= n <= batch rows in host or device memory, on the per-layer fp32
+ *    FFMA engine b200sac_act uses, whatever the handle's plan or precision.  CARE handles first encode the rows as
+ *    b200sac_act does (the critic's state encoder cse, of which the actor's is the tied copy); the critic input is that
+ *    encoding with act appended, laid out as the step's XQ.  The results land in the step's own XA / XQ / hA / hQ
+ *    buffers, rows [0, n) of each network (the next step recomputes all of them), so debug_read("hA.<l>") and
+ *    debug_read("hQ.<l>") show them afterwards: hA rows [0, n), hQ rows [0, n) of q1 and [batch, batch + n) of q2.
+ * 2. Scores.  For every hidden layer of N in {actor, q1, q2} with H neurons: a_i = (1/n) sum_rows max(h_ri, 0),
+ *    mean = (1/H) sum_j a_j, s_i = a_i / mean (every s_i = 0 when mean = 0).  Both sums in fp64 in one fixed order that
+ *    does not depend on the replica count, no floating-point atomics.  Neuron i is dormant iff s_i <= tau, tau =
+ *    tau_actor for the actor and tau_critic for q1 and q2 (each critic scored on its own neurons); a NaN score is never
+ *    dormant, and a negative tau (-inf included) recycles nothing: the measure-only call.
+ * 3. Recycle, for every dormant neuron i of hidden layer l:
+ *    - row i of W_l becomes what b200sac_create(seed) draws for those elements: the same Philox key (seed + replica),
+ *      tag and element index as b200sac_reset's theta0; pad columns stay zero;
+ *    - b_l[i] = 0;
+ *    - column i of the next weight matrix (the next hidden layer's, or for the last hidden layer the head's: the Q head,
+ *      or the policy head's mu and log-std rows) = 0, except where that entry lies in a recycled row of the next hidden
+ *      layer, which takes the draw (that neuron's own outgoing column is zero, so the function is the same either way);
+ *    - Adam m = v = 0 at exactly those entries.  Step counters and beta-power products are unchanged: ReDo resets
+ *      moments, not optimizers.
+ *    Left alone: targets (the network's function is unchanged, so the Polyak average stays valid), log_alpha, the CARE
+ *    encoders, gradients and PCGrad slices, per-replica settings, replay rings and the other replicas.
+ * 4. Record.  Per replica, each hidden neuron's score (fp64) and dormant flag, actor layers, then q1's, then q2's, in
+ *    layer order; NaN scores and 0 flags before the first call.  b200sac_read_redo reads it.
+ * Stream order as b200sac_reset: steps enqueued before the call are unaffected, steps enqueued after it (launches of
+ * graphs b200sac_prepare instantiated included; no graph is rebuilt) see the recycled networks.  Does not synchronise.
+ * A bad replica, n outside [1, batch], a NULL obs or act, or a NaN tau give B200SAC_ERR_INVALID, and nothing is
+ * enqueued. */
+int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* act, double tau_actor,
+                 double tau_critic, uint64_t seed, void* stream);
+
+/* The last b200sac_redo record of replica `replica`: scores[*n_neurons] and dormant[*n_neurons] (either may be NULL), in
+ * the order b200sac_redo states; cap = the capacity of each.  Synchronises the stream. */
+int b200sac_read_redo(b200sac_t* h, int32_t replica, double* scores, uint8_t* dormant, int64_t cap, int64_t* n_neurons,
+                      void* stream);
 
 /* Per-replica update intervals, both 1 (every step is a full step) after b200sac_create.  Let n be the replica's critic
  * Adam step count after a step (steps[0] of b200sac_get_steps).  The step is
@@ -435,7 +475,7 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * min(Q1,Q2) routed the gradient to), "q_pi" ([2][B]: Q1, Q2 at (s, a~); layer-chained plan only), "psave" ([2B][act][8]:
  * what the policy head saved per (row, action) -- std, u-mu, tanh(u), action, Jacobian term, the NOISE it used, clamp mask,
  * log-prob term), "head" ([2B][2*act]: the policy head's output as the head computed it, mu | log-std before the clamp;
- * after b200sac_act its first n rows), or a hidden
+ * after b200sac_act its first n rows), or a hidden (after b200sac_redo: its forward's rows, see there)
  * activation whose sign pattern is the ReLU mask the step used: "hA.<l>" [2B][H] (rows [s';s]), "hQ.<l>" / "hP.<l>" /
  * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT),
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
