@@ -26,7 +26,7 @@ class Cfg(C.Structure):
         ("mix_out", C.c_int32), ("ctx_in", C.c_int32), ("n_ctx_hidden", C.c_int32),
         ("ctx_hidden", C.c_int32 * MAX_HIDDEN), ("ctx_out", C.c_int32), ("emb_dim", C.c_int32),
         ("tau_se", C.c_double), ("lr_ctx", C.c_double),
-        ("grad_clip", C.c_int32), ("pcgrad", C.c_int32),
+        ("grad_clip", C.c_int32), ("pcgrad", C.c_int32), ("critic_ln", C.c_int32),
     ]
 
 

@@ -51,6 +51,7 @@ class CoreConfig:
     lr_ctx: float = 3e-4
     grad_clip: bool = False              # the step plan with gradient-norm clipping and norms (SacCore.set_grad_clip)
     pcgrad: bool = False                 # the per-layer plan with PCGrad gradient surgery (SacCore.set_pcgrad); num_tasks >= 2
+    critic_layer_norm: bool = False      # LayerNorm between every hidden Linear and its ReLU in q1, q2 and their targets
 
     @property
     def obs_dim(self):
@@ -76,6 +77,7 @@ class CoreConfig:
         c.care = (2 if self.care_original else 1) if self.care else 0
         c.grad_clip = int(self.grad_clip)
         c.pcgrad = int(self.pcgrad)
+        c.critic_ln = int(self.critic_layer_norm)
         if self.care:
             c.emb_dim, c.lr_ctx = self.emb_dim, self.lr_ctx
             c.num_encoders, c.mix_out, c.ctx_in, c.ctx_out = self.num_encoders, self.mix_out, self.ctx_in, self.ctx_out
@@ -630,7 +632,8 @@ class SacCore:
 
     def debug(self, name: str, replica=0) -> torch.Tensor:
         """Per-step intermediates (b200sac_debug_read): y, q1, ..., and the hidden activations "hA.<l>", "hQ.<l>", "hP.<l>",
-        "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used.  After a step from a prioritized
+        "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used; with critic_layer_norm, "zQ.<l>",
+        "zP.<l>", "zT.<l>" before the normalization.  After a step from a prioritized
         ring: "isw" (importance weights), "prio" (leaf values written) and "idx" (ring indices, int32).  After a step from a
         ring with trajectory links: "disc" (per-row discount), "nstep_m" (hops folded, int32), "idx"; "r" and "d" are folded."""
         cap = self.cfg.batch * max(2 * self.cfg.act_dim, 1)
@@ -640,7 +643,7 @@ class SacCore:
             cap = 2 * self.cfg.batch * self.cfg.act_dim * 8
         elif name == "head":
             cap = 2 * self.cfg.batch * 2 * self.cfg.act_dim
-        elif name[0] == "h" or name.startswith("mixH"):
+        elif name[0] in "hz" or name.startswith("mixH"):
             widest = max(list(self.cfg.actor_hidden) + list(self.cfg.critic_hidden) + [4 * ((w + 3) // 4) * self.cfg.num_encoders
                                                                                         for w in self.cfg.mix_hidden])
             cap = 2 * self.cfg.batch * widest

@@ -37,6 +37,7 @@
 #include "clip_kernels.cuh"
 #include "pcgrad_kernels.cuh"
 #include "redo_kernels.cuh"
+#include "ln_kernels.cuh"
 
 using namespace bsac;
 
@@ -95,7 +96,9 @@ using GraphExec = Own<cudaGraphExec_t, cudaGraphExecDestroy>;
 // ------------------------------------------------------------------------------------------
 // layout
 // ------------------------------------------------------------------------------------------
-struct LayerOff { int64_t w, b; int in, out; int ld; };   // ld = row pitch of the weight matrix (>= in)
+// ld = row pitch of the weight matrix (>= in); g, c = the LayerNorm weight and bias after a critic_ln critic's hidden
+// Linear, -1 where there is none
+struct LayerOff { int64_t w, b; int in, out; int ld; int64_t g = -1, c = -1; };
 struct Layout {
   std::vector<b200sac_tensor_desc> descs;
   std::vector<LayerOff> actor, q[2], qt[2];
@@ -132,6 +135,9 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->pcgrad != 0 && c->pcgrad != 1) return fail(B200SAC_ERR_INVALID, "pcgrad must be 0 or 1");
   if (c->pcgrad && (c->num_tasks < 2 || c->grad_clip != 0))
     return fail(B200SAC_ERR_INVALID, "pcgrad needs num_tasks >= 2 and no grad_clip");
+  if (c->critic_ln != 0 && c->critic_ln != 1) return fail(B200SAC_ERR_INVALID, "critic_ln must be 0 or 1");
+  if (c->critic_ln && (c->care || c->pcgrad))
+    return fail(B200SAC_ERR_INVALID, "critic_ln is for the plain-MLP critics without gradient surgery (care = 0, pcgrad = 0)");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -170,8 +176,9 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
     return o;
   };
   char nm[48];
+  // ln: a LayerNorm weight and bias (out, 1) right after every hidden layer's bias
   auto add_net = [&](const char* net, std::vector<LayerOff>* v, int in0, const int* hid, int nh, int out, int tr, int opt,
-                     bool pad_first = false) {
+                     bool pad_first = false, bool ln = false) {
     int in = in0;
     for (int i = 0; i <= nh; ++i) {
       int o = (i < nh) ? hid[i] : out;
@@ -182,6 +189,12 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
       lo.w = add(nm, o, in, tr, opt, lo.ld);
       snprintf(nm, sizeof(nm), "%s.%d.bias", net, i);
       lo.b = add(nm, o, 1, tr, opt);
+      if (ln && i < nh) {
+        snprintf(nm, sizeof(nm), "%s.%d.ln.weight", net, i);
+        lo.g = add(nm, o, 1, tr, opt);
+        snprintf(nm, sizeof(nm), "%s.%d.ln.bias", net, i);
+        lo.c = add(nm, o, 1, tr, opt);
+      }
       if (v) v->push_back(lo);
       in = o;
     }
@@ -213,8 +226,9 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
   add_net("actor", &L.actor, L.in_w, c->actor_hidden, c->n_actor_hidden, 2 * c->act_dim, 1, 1, true);
   L.actor_n = off - L.actor_begin;
   L.critic_begin = off;
-  add_net("q1", &L.q[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true);
-  add_net("q2", &L.q[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true);
+  const bool ln = c->critic_ln != 0;
+  add_net("q1", &L.q[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true, ln);
+  add_net("q2", &L.q[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true, ln);
   L.cse_begin = off;
   if (c->care) add_encoder("cse", true, 1, 0);
   L.critic_n = off - L.critic_begin;
@@ -231,8 +245,8 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
   }
   L.trainable = off;
   int64_t tb = off;
-  add_net("q1_target", &L.qt[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true);
-  add_net("q2_target", &L.qt[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true);
+  add_net("q1_target", &L.qt[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true, ln);
+  add_net("q2_target", &L.qt[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true, ln);
   if (c->care) add_encoder("tse", false, 0, -1);
   L.target_delta = tb - L.critic_begin;
   if (c->care) L.off_emb = add("embedding", c->num_tasks, c->ctx_in, 0, -1);
@@ -241,7 +255,7 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
 
 // How every parameter tensor is initialised, in the order b200sac_create draws them: the one source of the (init kind, tag)
 // pairs that create and b200sac_reset both read.  Xavier weights and the CARE mixture's randn tensors take tags 0, 1, ...
-// in this order; biases are zero; log_alpha is cfg.log_alpha_init; the frozen CARE embedding (part -1, never reset) is
+// in this order; biases are zero; LayerNorm weights one and their biases zero (no tag); log_alpha is cfg.log_alpha_init; the frozen CARE embedding (part -1, never reset) is
 // drawn under seed ^ 0x5EED.  depth: an actor or critic Linear layer's position counted from the network's output (1 = the
 // head); 0 for the all-or-nothing parts.
 struct InitTensor {
@@ -265,6 +279,10 @@ static std::vector<InitTensor> init_table(const b200sac_cfg* c, const Layout& L)
       const int depth = part == B200SAC_RESET_ACTOR || part == B200SAC_RESET_CRITIC ? n - i : 0;
       v.push_back({lo.w, lo.out, lo.in, lo.ld, RESET_XAVIER, tag++, part, depth, target, 0});
       v.push_back({lo.b, lo.out, 1, 1, RESET_ZERO, -1, part, depth, target, 0});
+      if (lo.g >= 0) {
+        v.push_back({lo.g, lo.out, 1, 1, RESET_ONES, -1, part, depth, target, 0});
+        v.push_back({lo.c, lo.out, 1, 1, RESET_ZERO, -1, part, depth, target, 0});
+      }
     }
   };
   linear(L.actor, B200SAC_RESET_ACTOR, false);
@@ -316,7 +334,7 @@ typedef void (*TcKernel)(const TcProb*, const int*, int, int);
 struct TcCall { TcKernel kern; const TcProb* probs; const int* sched; int G, sched_stride; };
 using KernelCall = std::variant<StepFirst<PolicyDoutArgs>, StepFirst<PolicyHeadArgs>, StepFirst<CriticHeadArgs>,
                                 StepFirst<ActorQHeadArgs>, StepFirst<HeadBwdArgs>, StepFirst<AdamArgs>, StepFirst<PcgArgs>,
-                                StepFirst<GradNormArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
+                                StepFirst<GradNormArgs>, StepFirst<LnArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
                                 NoStep<CareTabArgs>, NoStep<CareMixArgs>, NoStep<CareMixFwdArgs>, NoStep<CareMixBwdArgs>,
                                 NoStep<CareTabReduceArgs>, NoStep<CareTabWgradArgs>, NoStep<GemmGroup>, TcCall>;
 template <class P> static KernelCall bind(void (*kern)(StepConst, P), const P& args) { return StepFirst<P>{kern, args}; }
@@ -428,6 +446,11 @@ struct b200sac {
   int care_row_w = 0, care_off_att = 0, care_off_ctx = 0;
   std::vector<Buf> hA, dhA;       // per actor hidden layer
   std::vector<Buf> hQ, hT, hP, dhQ;   // per critic hidden layer, [2][B][H]
+  // cfg.critic_ln: per critic hidden layer [2][B][H], the pre-normalization activations of hQ, hT and hP; the backward
+  // normalization's chunk column sums [R][2][chunks][2][max H] and tickets [R][2]
+  std::vector<Buf> zQ, zT, zP;
+  DevMem<double> ln_part;
+  DevMem<unsigned> ln_ticket;
   std::vector<Launch> plan;
   // what the plan's launches read through their argument blocks: each wgmma launch's problems, each layer-chained launch's
   // tensor maps
@@ -745,7 +768,7 @@ static int make_tc_prob(const GemmProb& p, int rep, TcProb& t, int bn = 64) {
 // ------------------------------------------------------------------------------------------
 static bool fused_eligible(const b200sac* h) {
   const b200sac_cfg& c = h->cfg;
-  if (c.precision != 0 || c.care || c.pcgrad || !h->env.fuse) return false;
+  if (c.precision != 0 || c.care || c.pcgrad || c.critic_ln || !h->env.fuse) return false;
   for (int i = 0; i < c.n_actor_hidden; ++i) if (c.actor_hidden[i] % 4 || c.actor_hidden[i] > CH_MAXW) return false;
   for (int i = 0; i < c.n_critic_hidden; ++i) if (c.critic_hidden[i] % 4 || c.critic_hidden[i] > CH_MAXW) return false;
   if (c.state_dim + c.num_tasks + c.act_dim > CH_MAXW - 4) return false;
@@ -932,6 +955,7 @@ struct PlanBuilder {
   void adam(int which, bool tail_only, bool with_tail = true);
   void grad_norm(int which);
   void pcgrad(int which);
+  void layer_norm(const char* pass, int l, bool target, const std::vector<Buf>& z, const std::vector<Buf>* hb, bool want_grads);
   int build_plan_fused();
   void build_plan_layered();
 };
@@ -1569,6 +1593,41 @@ int PlanBuilder::build_plan_fused() {
   return 0;
 }
 
+// critic_ln handles: the LayerNorm of hidden layer l of both critics (the targets' when `target`) over the [2][B][H]
+// pre-normalization buffer z[l], every replica in one launch.  Forward (hb set): hb[l] = relu(LN(z[l])).  Backward (hb
+// null): dhQ[l] becomes the gradient at z[l] in place, and with want_grads the LayerNorm weight and bias gradients land
+// in gradient slice 0 (the split-K slices hold zeros there, so Adam's slice sum reads them unchanged).
+void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::vector<Buf>& z, const std::vector<Buf>* hb,
+                             bool want_grads) {
+  const int H = c.critic_hidden[l];
+  Launch ln;
+  ln.label = std::string(hb ? "ln_fwd{" : "ln_bwd{") + pass + " " + std::to_string(l) + "}";
+  ln.branch = branch;
+  LnArgs P;
+  memset(&P, 0, sizeof(P));
+  P.z = z[l].p; P.rsZ = z[l].rs;
+  const Buf& out = hb ? (*hb)[l] : h->dhQ[l];
+  (hb ? P.h : P.dh) = out.p;
+  P.rsH = out.rs;
+  for (int net = 0; net < 2; ++net) {
+    const LayerOff& lo = (target ? L.qt : L.q)[net][l];
+    P.g[net] = W(lo.g); P.c[net] = W(lo.c);
+    if (want_grads) { P.dg[net] = Gp(lo.g); P.dc[net] = Gp(lo.c); }
+  }
+  P.rsP = rsP; P.rsG = rsG;
+  P.part = h->ln_part; P.ticket = h->ln_ticket;
+  P.B = B; P.H = H;
+  P.actor_side = actor_side ? 1 : 0;
+  ln.block = dim3(kLnThreads);
+  if (hb) {
+    ln.grid = dim3((2 * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
+    push(std::move(ln), ln_fwd_kernel, P);
+  } else {
+    ln.grid = dim3((B + kLnRows - 1) / kLnRows, 2, R);
+    push(std::move(ln), ln_bwd_kernel, P);
+  }
+}
+
 // ---- per-layer plan: one grouped GEMM launch per layer (and kind) of the networks --------------------------------
 void PlanBuilder::build_plan_layered() {
   const int Kenc = c.num_encoders, nmix = c.care ? (int)L.mix.size() : 0;
@@ -1582,6 +1641,14 @@ void PlanBuilder::build_plan_layered() {
     care_encode({EncJob{0, 0, 2 * B, h->XA, h->K.ldxa, h->XQ, h->K.ldx, B}, EncJob{1, 0, B, h->XT, h->K.ldx, Buf{}, 0, 0}});
   }
   auto netp = [&](const Buf& b, int net, int H) { return b.p + (long long)net * B * H; };
+  // critic_ln: a critic hidden layer's GEMM writes the pre-normalization buffer z (no ReLU), its layer_norm launch the
+  // post-ReLU h that the rest of the plan reads
+  const bool ln = c.critic_ln != 0;
+  auto critic_fwd = [&](const float* X, long long rsX, const LayerOff& lo, int net, const Buf& hb, const Buf* zb) {
+    GemmProb p = fwd_prob(par, X, rsX, B, lo, netp(zb ? *zb : hb, net, lo.out), (zb ? *zb : hb).rs);
+    if (zb) p.relu = 0;
+    return p;
+  };
   // ---- Phase A: actor over [s2; s] and Q1,Q2 over (s,a), layer by layer -----------------
   for (int l = 0; l < (La > Lc ? La : Lc); ++l) {
     std::vector<GemmProb> ps;
@@ -1593,16 +1660,20 @@ void PlanBuilder::build_plan_layered() {
     if (l < Lc)
       for (int net = 0; net < 2; ++net) {
         const LayerOff& lo = L.q[net][l];
-        ps.push_back(fwd_prob(par, l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in), l == 0 ? h->XQ.rs : h->hQ[l - 1].rs, B, lo,
-                         netp(h->hQ[l], net, lo.out), h->hQ[l].rs));
+        ps.push_back(critic_fwd(l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in), l == 0 ? h->XQ.rs : h->hQ[l - 1].rs, lo,
+                                net, h->hQ[l], ln ? &h->zQ[l] : nullptr));
       }
     if (use_fork && La == Lc) {
       // Q1,Q2 on (s,a) are not needed before critic_heads, while the actor's output heads the policy_head -> target-critic
       // chain: the critics' layer goes to the fork stream (joined at critic_heads), the actor's stays on the main stream.
-      branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end())); branch = 0;
+      branch = 1;
+      gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end()));
+      if (ln) layer_norm("critic", l, false, h->zQ, &h->hQ, false);
+      branch = 0;
       gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 1));
     } else {
       gemm_launch(ps);
+      if (ln && l < Lc) layer_norm("critic", l, false, h->zQ, &h->hQ, false);
     }
   }
   {  // policy head
@@ -1617,10 +1688,11 @@ void PlanBuilder::build_plan_layered() {
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.qt[net][l];
-      ps.push_back(fwd_prob(par, l == 0 ? h->XT.p : netp(h->hT[l - 1], net, lo.in), l == 0 ? h->XT.rs : h->hT[l - 1].rs, B, lo,
-                       netp(h->hT[l], net, lo.out), h->hT[l].rs));
+      ps.push_back(critic_fwd(l == 0 ? h->XT.p : netp(h->hT[l - 1], net, lo.in), l == 0 ? h->XT.rs : h->hT[l - 1].rs, lo,
+                              net, h->hT[l], ln ? &h->zT[l] : nullptr));
     }
     gemm_launch(ps);
+    if (ln) layer_norm("target", l, true, h->zT, &h->hT, false);
   }
   const int Hc = c.critic_hidden[Lc - 1];
   {  // critic heads: y, Q1, Q2, dQ
@@ -1647,6 +1719,8 @@ void PlanBuilder::build_plan_layered() {
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
   for (int l = Lc - 1; l >= 0; --l) {
+    // (on the main stream: the forked weight gradient below waits for it like the input gradient does)
+    if (ln) layer_norm("critic", l, false, h->zQ, nullptr, true);
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.q[net][l];
@@ -1775,10 +1849,11 @@ void PlanBuilder::build_plan_layered() {
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.q[net][l];
-      ps.push_back(fwd_prob(par, l == 0 ? h->XP.p : netp(h->hP[l - 1], net, lo.in), l == 0 ? h->XP.rs : h->hP[l - 1].rs, B, lo,
-                       netp(h->hP[l], net, lo.out), h->hP[l].rs));
+      ps.push_back(critic_fwd(l == 0 ? h->XP.p : netp(h->hP[l - 1], net, lo.in), l == 0 ? h->XP.rs : h->hP[l - 1].rs, lo,
+                              net, h->hP[l], ln ? &h->zP[l] : nullptr));
     }
     gemm_launch(ps);
+    if (ln) layer_norm("actor pass", l, false, h->zP, &h->hP, false);
   }
   {
     Launch l;
@@ -1798,6 +1873,7 @@ void PlanBuilder::build_plan_layered() {
   }
   head_bwd(false, false);
   for (int l = Lc - 1; l >= 0; --l) {
+    if (ln) layer_norm("actor pass", l, false, h->zP, nullptr, false);
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
       const LayerOff& lo = L.q[net][l];
@@ -2175,6 +2251,18 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     for (int l = 0; l < cfg->n_mix_hidden; ++l) slab.request(h->mixDH[l], (size_t)Kenc * B * pitch(cfg->mix_hidden[l]));
     slab.request(h->mixDZ, (size_t)Kenc * B * pitch(cfg->mix_out));
   }
+  if (cfg->critic_ln) {
+    h->zQ.resize(Lc); h->zT.resize(Lc); h->zP.resize(Lc);
+    int maxH = 0;
+    for (int l = 0; l < Lc; ++l) {
+      for (Buf* b : {&h->zQ[l], &h->zT[l], &h->zP[l]}) slab.request(*b, (size_t)2 * B * cfg->critic_hidden[l]);
+      maxH = std::max(maxH, cfg->critic_hidden[l]);
+    }
+    const size_t chunks = (size_t)(B + kLnRows - 1) / kLnRows;
+    CU(cudaMalloc(h->ln_part.put(), sizeof(double) * R * 2 * chunks * 2 * maxH));
+    CU(cudaMalloc(h->ln_ticket.put(), sizeof(unsigned) * R * 2));
+    CU(cudaMemset(h->ln_ticket, 0, sizeof(unsigned) * R * 2));
+  }
   if (int rc = slab.allocate(h->slab)) return rc;
 
   IngestOut& O = h->ing;
@@ -2184,7 +2272,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   O.XS = cfg->care ? h->XS.p : nullptr; O.rsXS = cfg->care ? h->XS.rs : 0;
   O.log_alpha = h->params + L.off_alpha; O.rsP = L.arena; O.alpha = h->alpha.p; O.rsAlpha = h->alpha.rs;
 
-  // parameter init: Xavier-uniform weights, zero biases (the memset above), log_alpha = cfg; targets = locals
+  // parameter init: Xavier-uniform weights, zero biases (the memset above), LayerNorm weights 1, log_alpha = cfg;
+  // targets = locals
   {
     for (const InitTensor& t : init_table(cfg, L)) {
       const uint64_t key = seed ^ t.seed_xor;
@@ -2192,8 +2281,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
         xavier_kernel<<<dim3(64, R), 256>>>(h->params + t.off, L.arena, t.rows, t.cols, t.ld, key, t.tag);
       } else if (t.kind == RESET_RANDN) {
         randn_kernel<<<dim3(t.cols > 1 ? 64 : 8, R), 256>>>(h->params + t.off, L.arena, (long long)t.rows * t.cols, key, t.tag);
-      } else if (t.kind == RESET_CONST) {
-        std::vector<float> la((size_t)t.rows, (float)cfg->log_alpha_init);
+      } else if (t.kind == RESET_CONST || t.kind == RESET_ONES) {
+        std::vector<float> la((size_t)t.rows, t.kind == RESET_ONES ? 1.0f : (float)cfg->log_alpha_init);
         for (int rep = 0; rep < R; ++rep)
           CU(cudaMemcpy(h->params + (size_t)rep * L.arena + t.off, la.data(), la.size() * sizeof(float), cudaMemcpyHostToDevice));
       }
@@ -2614,7 +2703,7 @@ extern "C" int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_
     ResetTensor& r = A.t[n++];
     r.off = t.off; r.rows = t.rows; r.cols = t.cols; r.ld = t.ld;
     r.kind = (unsigned char)t.kind; r.part = (unsigned char)t.part; r.target = t.target ? 1 : 0;
-    r.tag = t.tag; r.c0 = (float)c.log_alpha_init;
+    r.tag = t.tag; r.c0 = t.kind == RESET_ONES ? 1.0f : (float)c.log_alpha_init;
     widest = std::max(widest, (long long)t.rows * t.cols);
   }
   // optimizers that own a touched tensor: {counter slot, first trainable float, floats}
@@ -3258,6 +3347,8 @@ extern "C" int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float
 extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* act, double tau_actor,
                             double tau_critic, uint64_t seed, void* stream) {
   if (!h || !obs || !act) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (h->cfg.critic_ln)     // its forward has no LayerNorm, and one recycled unit would move its whole row's statistics
+    return fail(B200SAC_ERR_STATE, "ReDo does not run on a handle created with critic_ln");
   if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
   const b200sac_cfg& c = h->cfg;
   const int B = c.batch, A = c.act_dim, La = c.n_actor_hidden, Lc = c.n_critic_hidden;
@@ -3419,7 +3510,8 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   }
   else {
     // hidden activations (the ReLU masks of the step): "hA.<l>" [2B][H] rows [s';s]; "hQ.<l>" / "hT.<l>" / "hP.<l>" [2][B][H]
-    // (critic update pass / target pass -- not kept by the layer-chained plan -- / actor pass); CARE mixture encoders
+    // (critic update pass / target pass -- not kept by the layer-chained plan -- / actor pass); critic_ln handles
+    // "zQ.<l>" / "zT.<l>" / "zP.<l>" [2][B][H], the same passes' pre-normalization activations; CARE mixture encoders
     // "mixH.<inst>.<l>" [K][rows][pitch4(H)], inst 0 = critic's on [s';s] (rows 2B), 1 = target's on s', 2 = updated critic's on s
     int l = -1, inst = -1;
     char kind[8] = "";
@@ -3434,6 +3526,11 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
       if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
       b = &v[l];
       n = (int64_t)2 * B * (kind[0] == 'A' ? h->cfg.actor_hidden[l] : h->cfg.critic_hidden[l]);
+    } else if (sscanf(name, "z%1[QTP].%d", kind, &l) == 2) {
+      const std::vector<Buf>& v = kind[0] == 'Q' ? h->zQ : (kind[0] == 'T' ? h->zT : h->zP);
+      if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
+      b = &v[l];
+      n = (int64_t)2 * B * h->cfg.critic_hidden[l];
     } else {
       return fail(B200SAC_ERR_INVALID, "unknown debug tensor '%s'", name);
     }

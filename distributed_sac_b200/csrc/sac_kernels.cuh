@@ -1177,13 +1177,14 @@ __global__ void xavier_kernel(float* w, long long rsP, int rows, int cols, int l
 // and blended with its current value, the local and, where it has one, its target at + target_delta:
 //   shrink == 0: theta' = theta0 (a select, so a NaN or inf network comes back finite);
 //   otherwise:   theta' = (float)(shrink * theta + (1 - shrink) * theta0), in fp64 (the library has no FMA contraction).
-enum ResetInit { RESET_XAVIER = 0, RESET_RANDN = 1, RESET_ZERO = 2, RESET_CONST = 3 };
+// RESET_CONST and RESET_ONES (the LayerNorm weights of critic_ln handles) draw c0.
+enum ResetInit { RESET_XAVIER = 0, RESET_RANDN = 1, RESET_ZERO = 2, RESET_CONST = 3, RESET_ONES = 4 };
 struct ResetTensor {
   long long off;                 // in floats, inside the replica's arena
   int rows, cols, ld;            // element i sits at (i / cols) * ld + i % cols: pad columns are not written
   unsigned char kind, part, target, pad;   // ResetInit; b200sac_reset part (index of shrink); 1 = has a target copy
   int tag;                       // Philox tag (XAVIER / RANDN)
-  float c0;                      // CONST: the value
+  float c0;                      // CONST / ONES: the value
 };
 constexpr int kResetMaxTensors = 112;   // actor 18 + q1, q2 36 + encoder 54 or encoder 36 + context 18, + log_alpha
 struct ResetArgs {

@@ -82,12 +82,14 @@ class _BaseLearner:
     log_name = "LunarLander_Distributed_SAC"
     _iteration_key = "episode_idx"
     _pcgrad_ok = False          # PCGrad and CAGrad need task-block minibatches: the multi-task learners (MTSAC and CARE)
+    _critic_ln_ok = True        # LayerNorm in the critics' hidden layers: the plain-MLP critics (not CARE's)
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
                      n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                     redo_interval=None, redo=None):
+                     redo_interval=None, redo=None, critic_layer_norm=False):
+        self.critic_layer_norm = bool(critic_layer_norm)
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -107,6 +109,14 @@ class _BaseLearner:
         self.episode_idx = 0
         self.datetime = str(datetime.now())[:-7]
         self._set_dims()
+        if self.critic_layer_norm:
+            if not self._critic_ln_ok:
+                raise ValueError(f"critic_layer_norm=True needs plain-MLP critics ({type(self).__name__} has CARE critics)")
+            if self.pcgrad or self.cagrad is not None:
+                raise ValueError("critic_layer_norm=True and pcgrad= / cagrad= are exclusive")
+            if redo is not None or redo_interval is not None:
+                raise ValueError("critic_layer_norm=True and redo= / redo_interval= are exclusive (recycling a unit would "
+                                 "change its LayerNorm row's statistics, so it would not preserve the network's function)")
         if self.pcgrad and not (self._pcgrad_ok and self.num_tasks >= 2):
             raise ValueError(f"pcgrad=True needs a multi-task MTSAC or CARE learner with num_tasks >= 2 ({type(self).__name__}, "
                              f"num_tasks {self.num_tasks})")
@@ -215,7 +225,7 @@ class _BaseLearner:
                           lr_critic=float(self.lr_critic),
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
                           log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None,
-                          pcgrad=self.pcgrad or self.cagrad is not None)
+                          pcgrad=self.pcgrad or self.cagrad is not None, critic_layer_norm=self.critic_layer_norm)
 
     # ---- reference method surface -------------------------------------------------------------
     def _chunks(self, n):
@@ -244,6 +254,8 @@ class _BaseLearner:
 
     def _recycle(self, seed, taus):
         """One SacCore.redo on a fresh reference-shaped draw from the ring (a prioritized ring's weights are ignored)."""
+        if self.critic_layer_norm:
+            raise ValueError("dormant-neuron recycling and scoring do not run on a learner with critic_layer_norm=True")
         s, a = self.memory.sample()[:2]
         self.core.redo(seed, s, a, **taus)
 
@@ -271,6 +283,8 @@ class _BaseLearner:
         """The fraction of tau-dormant neurons (score <= tau) per network and hidden layer on a fresh replay batch: a
         measure-only recycle call, nothing changes.  {"actor" | "q1" | "q2": [fraction per hidden layer]}."""
         redo_taus(tau, tau)
+        if self.critic_layer_norm:
+            raise ValueError("dormant_fraction() does not run on a learner with critic_layer_norm=True")
         self._recycle(self.seed, {})
         rec = self.core.read_redo()
         return {net: [float(np.mean(s <= tau)) for s in rec[net]["score"]] for net in REDO_NETS}
@@ -390,7 +404,7 @@ class _BaseLearner:
         if net == "actor":
             return names.actor_key_map(self.family, na)
         which = 1 if "1" in net else 2
-        return names.critic_key_map(self.family, nc, which, target="target" in net)
+        return names.critic_key_map(self.family, nc, which, target="target" in net, layer_norm=self.critic_layer_norm)
 
     def _module_state_dict(self, net, which=_lib.PARAMS, named=None):
         named = named if named is not None else self.core.get_named(which)
@@ -558,12 +572,13 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, update_delay=3, print_period=10, write_mode=True, save_period=1000,
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
-                 pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None):
+                 pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None,
+                 critic_layer_norm=False):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
 
     def _set_dims(self):
         c = self.cfg
@@ -588,10 +603,10 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
                  target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                 redo_interval=None, redo=None):
+                 redo_interval=None, redo=None, critic_layer_norm=False):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
 
     def _set_dims(self):
         c = self.cfg
@@ -619,11 +634,11 @@ class MTSACLearner(_BaseLearner):
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
-                 cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None):
+                 cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None, critic_layer_norm=False):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
 
     def _set_dims(self):
         c = self.cfg
@@ -675,6 +690,7 @@ class CARELearner(MTSACLearner):
     critic's after every update (learner.py:402), so it is exported from the same tensors."""
     family = "C10"
     log_name = "MT10_Distributed_CARE"
+    _critic_ln_ok = False
     # the 'encoder' keys _core_config reads without a default
     _encoder_keys = ("num_encoders", "hidden_dims_mixtureEnc", "output_dim_mixtureEnc", "hidden_dims_contextEnc",
                      "output_dim_contextEnc", "embedding_dim_contextEnc", "lr_contextEnc")

@@ -11,8 +11,12 @@ reference's key names are a compatibility contract:
   MS        Actor : mu_log_std_layer.{2i}.*                  (MT10_Distributed_MTSAC/src/model.py:27-33, utils.py:36-57)
             Critic: Q_function_1.{2i}.*, Q_function_2.{2i}.* (model.py:136-149)
 
+Layer-normalized critics (critic_layer_norm) add a LayerNorm after every hidden Linear: `layer_norms.{i}.*` beside the LL / VS
+Critic's Linear keys, and the natural nn.Sequential(Linear, LayerNorm, ReLU, ...) numbering Q_function_{w}.{3i}.* (Linear i),
+Q_function_{w}.{3i+1}.* (its LayerNorm) for MS.
+
 Canonical names (used by the C ABI's layout table): `<net>.<i>.weight|bias`
-with net in {actor,q1,q2,q1_target,q2_target} and `log_alpha`.
+with net in {actor,q1,q2,q1_target,q2_target}, `<net>.<i>.ln.weight|bias` for a critic's LayerNorm and `log_alpha`.
 """
 
 
@@ -31,22 +35,29 @@ def actor_key_map(family: str, n_layers: int):
     return m
 
 
-def critic_key_map(family: str, n_layers: int, which: int, target: bool = False):
-    """{reference key: canonical key} for Q-function `which` (1|2).
+def critic_key_map(family: str, n_layers: int, which: int, target: bool = False, layer_norm: bool = False):
+    """{reference key: canonical key} for Q-function `which` (1|2), in the canonical layout order; n_layers counts the
+    head.
 
     LL/VS: keys of ONE Critic module (local_critic_{which});
-    MS   : keys of the twin Critic module restricted to Q_function_{which}."""
+    MS   : keys of the twin Critic module restricted to Q_function_{which}.
+    layer_norm: the critics with a LayerNorm after every hidden Linear (the module docstring gives the keys)."""
+    if family not in ("LL", "VS", "MS"):
+        raise ValueError(family)
     net = f"q{which}" + ("_target" if target else "")
+    step = 3 if layer_norm else 2          # MS: modules per hidden layer of the nn.Sequential
     m = {}
     for i in range(n_layers):
         for kind in ("weight", "bias"):
             if family in ("LL", "VS"):
                 ref = f"first_layer.{kind}" if i == 0 else f"layer_module.{i - 1}.{kind}"
-            elif family == "MS":
-                ref = f"Q_function_{which}.{2 * i}.{kind}"
             else:
-                raise ValueError(family)
+                ref = f"Q_function_{which}.{step * i}.{kind}"
             m[ref] = f"{net}.{i}.{kind}"
+        if layer_norm and i < n_layers - 1:
+            for kind in ("weight", "bias"):
+                ref = f"layer_norms.{i}.{kind}" if family in ("LL", "VS") else f"Q_function_{which}.{3 * i + 1}.{kind}"
+                m[ref] = f"{net}.{i}.ln.{kind}"
     return m
 
 

@@ -113,7 +113,40 @@ typedef struct b200sac_cfg {
   int32_t pcgrad;                    /* 0 = the default plan; 1 = the per-layer plan with PCGrad gradient surgery
                                         (b200sac_set_pcgrad), both switches on at create.  Needs num_tasks >= 2 and
                                         grad_clip = 0; MTSAC and CARE (care = 1 | 2) alike.  Fixed at create. */
+  int32_t critic_ln;                 /* 0 = the default plan; 1 = LayerNorm in the critics' hidden layers.  Fixed at create.
+                                        See "Layer-normalized critics" below. */
 } b200sac_cfg;
+
+/* Layer-normalized critics (cfg.critic_ln = 1; Ba et al. 2016, as high-replay-ratio SAC uses it: DroQ, Lyle et al. 2023,
+ * BRO).  Every hidden layer l of q1, q2, q1_target and q2_target, width H, is nn.Sequential(Linear, nn.LayerNorm(H,
+ * eps=1e-5), ReLU):
+ *   z = W_l x + b_l;  mu = (1/H) sum_j z_j;  var = (1/H) sum_j (z_j - mu)^2 (biased);  rstd = 1 / sqrt(var + 1e-5);
+ *   xhat = (z - mu) * rstd;  h = relu(g_l * xhat + c_l).
+ * The heads and the actor are unchanged.  Numerics (fp64 throughout, no fused multiply-add, one rounding to fp32 at the
+ * end of each output):
+ *   - a row sum over j: lane k of one warp adds j = k, k + 32, ... in increasing order from 0.0, then the 32 lane sums are
+ *     combined by the xor butterfly with offsets 16, 8, 4, 2, 1.  mu and var are such sums divided by H; h is
+ *     (float)(g * xhat + c) with a negative value replaced by 0 (a NaN stays NaN);
+ *   - backward, dy = the ReLU-masked gradient at h: a = (row sum of g*dy) / H, b = (row sum of g*dy*xhat) / H, and
+ *     dz = (float)(rstd * ((g*dy - a) - xhat * b));
+ *   - dg_l = sum over the batch of dy*xhat and dc_l = sum of dy, per critic: rows cut into chunks of 16 in row order, each
+ *     chunk's sum over its rows in increasing order from 0.0, then the chunk sums added in chunk order and rounded once.
+ *     No floating-point atomics: the result is bit-reproducible and does not depend on the replica count.
+ * Parameters: <net>.<l>.ln.weight and <net>.<l>.ln.bias, shape (H, 1), right after <net>.<l>.bias; trainable with opt 0
+ * in q1 / q2, trainable 0 and opt -1 in the targets (at + target_delta, like every target tensor).  q1, q2 and their
+ * targets stay contiguous, so the critic Adam, the Polyak updates, b200sac_soft_update(_critic), b200sac_copy_replica,
+ * export / import and the gradient-clipping norm cover them.  Create: g = 1, c = 0, targets = locals; they take no Philox
+ * tag, so every Linear tensor is bit-identical to the same cfg with critic_ln = 0.  b200sac_reset: the LayerNorm of
+ * hidden Linear i goes with that Linear's depth; its fresh draw is g = 1, c = 0.
+ * Plan: always the per-layer plan (never the layer-chained one), at precision 0 and 1.  Each of the passes A (critics
+ * on (s, a)), B (targets on (s', a')) and D (critics on (s, a~), the actor pass) runs its hidden GEMMs without ReLU into
+ * the pre-normalization buffers and one forward LayerNorm launch per layer for both critics and every replica; the
+ * critic backward (C) and the actor pass's input gradient (D) run one backward launch per layer before that layer's
+ * weight and input gradients.  A step has 5 * n_critic_hidden launches more than the same cfg's per-layer plan
+ * without critic_ln; they are labelled "ln_fwd{critic|target|actor pass <l>}" and "ln_bwd{critic|actor pass <l>}".
+ * The actor-pass launches return at entry on a critic-only step.
+ * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_ln outside {0, 1}, or together with
+ * care != 0 or pcgrad = 1.  b200sac_redo on such a handle gives B200SAC_ERR_STATE (see there). */
 
 typedef struct b200sac_tensor_desc {
   char name[48];                     /* canonical name, e.g. "q1_target.2.weight" */
@@ -260,7 +293,9 @@ int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_spec* spec,
  * Stream order as b200sac_reset: steps enqueued before the call are unaffected, steps enqueued after it (launches of
  * graphs b200sac_prepare instantiated included; no graph is rebuilt) see the recycled networks.  Does not synchronise.
  * A bad replica, n outside [1, batch], a NULL obs or act, or a NaN tau give B200SAC_ERR_INVALID, and nothing is
- * enqueued. */
+ * enqueued.  A handle created with critic_ln gives B200SAC_ERR_STATE and nothing is enqueued: this forward has no
+ * LayerNorm, and recycling one unit would change its whole row's statistics, so the recycle would not preserve the
+ * network's function. */
 int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* act, double tau_actor,
                  double tau_critic, uint64_t seed, void* stream);
 
@@ -477,7 +512,8 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * log-prob term), "head" ([2B][2*act]: the policy head's output as the head computed it, mu | log-std before the clamp;
  * after b200sac_act its first n rows), or a hidden (after b200sac_redo: its forward's rows, see there)
  * activation whose sign pattern is the ReLU mask the step used: "hA.<l>" [2B][H] (rows [s';s]), "hQ.<l>" / "hP.<l>" /
- * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT),
+ * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT); with
+ * cfg.critic_ln, "zQ.<l>" / "zP.<l>" / "zT.<l>" [2][B][H], the same passes' pre-normalization activations W x + b;
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
  * importance weights of its critic loss), "prio" [B] (the leaf values p it wrote) and "idx" [B] (its ring indices, int32
  * bit patterns).  After a step from a linked ring (n-step returns): "disc" [B] (the per-row discount of its TD target),
