@@ -52,6 +52,7 @@ class CoreConfig:
     grad_clip: bool = False              # the step plan with gradient-norm clipping and norms (SacCore.set_grad_clip)
     pcgrad: bool = False                 # the per-layer plan with PCGrad gradient surgery (SacCore.set_pcgrad); num_tasks >= 2
     critic_layer_norm: bool = False      # LayerNorm between every hidden Linear and its ReLU in q1, q2 and their targets
+    critic_dropout: bool = False         # with critic_layer_norm: dropout before every critic LayerNorm (SacCore.set_critic_dropout)
 
     @property
     def obs_dim(self):
@@ -78,6 +79,7 @@ class CoreConfig:
         c.grad_clip = int(self.grad_clip)
         c.pcgrad = int(self.pcgrad)
         c.critic_ln = int(self.critic_layer_norm)
+        c.critic_dropout = int(self.critic_dropout)
         if self.care:
             c.emb_dim, c.lr_ctx = self.emb_dim, self.lr_ctx
             c.num_encoders, c.mix_out, c.ctx_in, c.ctx_out = self.num_encoders, self.mix_out, self.ctx_in, self.ctx_out
@@ -421,6 +423,19 @@ class SacCore:
                     cur[k] = float(v)
             _lib.check(self.lib.b200sac_set_grad_clip(self._h, r, cur["critic"], cur["actor"], cur["ctx"], _stream()))
 
+    # ---- critic dropout (b200sac_set/get_critic_dropout; handles with critic_dropout=True) --------------------------------
+    def get_critic_dropout(self, replica=0) -> float:
+        """The critic dropout rate p of one replica (no synchronisation)."""
+        p = C.c_double()
+        _lib.check(self.lib.b200sac_get_critic_dropout(self._h, int(replica), C.byref(p)))
+        return p.value
+
+    def set_critic_dropout(self, p, replica=None):
+        """Dropout rate p in [0, 1) before every critic LayerNorm of one replica (replica=None: all of them), on the current
+        stream.  Steps enqueued afterwards use it."""
+        for r in _replicas(self.cfg.replicas, replica):
+            _lib.check(self.lib.b200sac_set_critic_dropout(self._h, r, float(p), _stream()))
+
     def read_grad_norms(self, n_last: int = 1) -> torch.Tensor:
         """Pre-clip gradient norms [n_last][R][3] (critic, actor, context encoder) of the last steps, aligned with read_losses;
         NaN where that optimizer did not step."""
@@ -633,7 +648,8 @@ class SacCore:
     def debug(self, name: str, replica=0) -> torch.Tensor:
         """Per-step intermediates (b200sac_debug_read): y, q1, ..., and the hidden activations "hA.<l>", "hQ.<l>", "hP.<l>",
         "hT.<l>", "mixH.<inst>.<l>" whose sign patterns are the ReLU masks the step used; with critic_layer_norm, "zQ.<l>",
-        "zP.<l>", "zT.<l>" before the normalization.  After a step from a prioritized
+        "zP.<l>", "zT.<l>" before the normalization (after the dropout with critic_dropout); with critic_dropout, "mQ.<l>",
+        "mP.<l>", "mT.<l>" the keep masks (0.0 / 1.0).  After a step from a prioritized
         ring: "isw" (importance weights), "prio" (leaf values written) and "idx" (ring indices, int32).  After a step from a
         ring with trajectory links: "disc" (per-row discount), "nstep_m" (hops folded, int32), "idx"; "r" and "d" are folded."""
         cap = self.cfg.batch * max(2 * self.cfg.act_dim, 1)
@@ -643,7 +659,7 @@ class SacCore:
             cap = 2 * self.cfg.batch * self.cfg.act_dim * 8
         elif name == "head":
             cap = 2 * self.cfg.batch * 2 * self.cfg.act_dim
-        elif name[0] in "hz" or name.startswith("mixH"):
+        elif name[0] in "hzm":
             widest = max(list(self.cfg.actor_hidden) + list(self.cfg.critic_hidden) + [4 * ((w + 3) // 4) * self.cfg.num_encoders
                                                                                         for w in self.cfg.mix_hidden])
             cap = 2 * self.cfg.batch * widest

@@ -138,6 +138,9 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->critic_ln != 0 && c->critic_ln != 1) return fail(B200SAC_ERR_INVALID, "critic_ln must be 0 or 1");
   if (c->critic_ln && (c->care || c->pcgrad))
     return fail(B200SAC_ERR_INVALID, "critic_ln is for the plain-MLP critics without gradient surgery (care = 0, pcgrad = 0)");
+  if (c->critic_dropout != 0 && c->critic_dropout != 1) return fail(B200SAC_ERR_INVALID, "critic_dropout must be 0 or 1");
+  if (c->critic_dropout && !c->critic_ln)
+    return fail(B200SAC_ERR_INVALID, "critic_dropout needs critic_ln = 1 (the dropout sits before each critic LayerNorm)");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -451,6 +454,10 @@ struct b200sac {
   std::vector<Buf> zQ, zT, zP;
   DevMem<double> ln_part;
   DevMem<unsigned> ln_ticket;
+  // cfg.critic_dropout: per pass (A critics on (s, a), B targets, D actor pass) and critic hidden layer the keep-mask bits
+  // [2][B][ceil(H / 32)] (uint32 words in float slots); [R] dropout rates p (host mirror) and their DropRate
+  std::vector<Buf> dmask[3];
+  ReplicaTable<DropRate, 1, double> drop;
   std::vector<Launch> plan;
   // what the plan's launches read through their argument blocks: each wgmma launch's problems, each layer-chained launch's
   // tensor maps
@@ -1596,7 +1603,9 @@ int PlanBuilder::build_plan_fused() {
 // critic_ln handles: the LayerNorm of hidden layer l of both critics (the targets' when `target`) over the [2][B][H]
 // pre-normalization buffer z[l], every replica in one launch.  Forward (hb set): hb[l] = relu(LN(z[l])).  Backward (hb
 // null): dhQ[l] becomes the gradient at z[l] in place, and with want_grads the LayerNorm weight and bias gradients land
-// in gradient slice 0 (the split-K slices hold zeros there, so Adam's slice sum reads them unchanged).
+// in gradient slice 0 (the split-K slices hold zeros there, so Adam's slice sum reads them unchanged).  critic_dropout
+// handles run the dropout instantiations on the same launches: the pass of z (zQ: A, zT: B, zP: D) picks the mask
+// buffer and the Philox tag.
 void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::vector<Buf>& z, const std::vector<Buf>* hb,
                              bool want_grads) {
   const int H = c.critic_hidden[l];
@@ -1618,13 +1627,21 @@ void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::ve
   P.part = h->ln_part; P.ticket = h->ln_ticket;
   P.B = B; P.H = H;
   P.actor_side = actor_side ? 1 : 0;
+  const bool drop = c.critic_dropout != 0;
+  if (drop) {
+    const int pass = &z == &h->zQ ? 0 : (&z == &h->zT ? 1 : 2);
+    P.drop = h->drop.dev; P.mbits = (unsigned*)h->dmask[pass][l].p; P.rsM = h->dmask[pass][l].rs;
+    P.tag0 = (pass * 8 + l) * 2;
+  }
   ln.block = dim3(kLnThreads);
   if (hb) {
     ln.grid = dim3((2 * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
-    push(std::move(ln), ln_fwd_kernel, P);
+    if (drop) push(std::move(ln), ln_fwd_kernel<true>, P);
+    else push(std::move(ln), ln_fwd_kernel<false>, P);
   } else {
     ln.grid = dim3((B + kLnRows - 1) / kLnRows, 2, R);
-    push(std::move(ln), ln_bwd_kernel, P);
+    if (drop) push(std::move(ln), ln_bwd_kernel<true>, P);
+    else push(std::move(ln), ln_bwd_kernel<false>, P);
   }
 }
 
@@ -2263,6 +2280,14 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMalloc(h->ln_ticket.put(), sizeof(unsigned) * R * 2));
     CU(cudaMemset(h->ln_ticket, 0, sizeof(unsigned) * R * 2));
   }
+  if (cfg->critic_dropout) {  // rate 0 on every replica; masks all zero until a step draws them
+    for (std::vector<Buf>& v : h->dmask) {
+      v.resize(Lc);
+      for (int l = 0; l < Lc; ++l) slab.request(v[l], (size_t)2 * B * ((cfg->critic_hidden[l] + 31) / 32));
+    }
+    const double p0 = 0.0;
+    if (int rc = h->drop.init(R, &p0)) return rc;
+  }
   if (int rc = slab.allocate(h->slab)) return rc;
 
   IngestOut& O = h->ing;
@@ -2445,8 +2470,12 @@ struct StreamBridge {
 // Per-replica settings (ReplicaTable): replicas of one handle can train with different values, and a value can change
 // between steps.  Each entry point checks its own arguments and leaves the write, its ordering and the mirror to the table.
 // ------------------------------------------------------------------------------------------
+// t = floor(p * 2^32) and s = 1 / (1 - p), both in fp64, s rounded to fp32 once
+static DropRate drop_rate(double p) { return DropRate{(unsigned)floor(p * 4294967296.0), (float)(1.0 / (1.0 - p))}; }
+
 template <class T, class Mirror> static T device_value(const Mirror& v) {
   if constexpr (std::is_same_v<T, Mirror>) return v;
+  else if constexpr (std::is_same_v<T, DropRate>) return drop_rate(v);
   else return hparams_row(v);
 }
 
@@ -2537,6 +2566,24 @@ extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double criti
     return fail(B200SAC_ERR_INVALID, "gradient-norm thresholds must be > 0 (+inf: no clipping), got %g, %g, %g", critic, actor, ctx);
   const double v[kClipCols] = {critic, actor, ctx};
   return h->clip_thr.set(h, stream, replica, v);
+}
+
+// Critic dropout rates, read by the dropout LayerNorm launches of the step graphs.
+extern "C" int b200sac_get_critic_dropout(b200sac_t* h, int32_t replica, double* p) {
+  if (!h || !p) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (!h->cfg.critic_dropout) return fail(B200SAC_ERR_STATE, "the handle was created without critic_dropout");
+  if (int rc = h->drop.check(replica)) return rc;
+  *p = *h->drop.row(replica);
+  return 0;
+}
+
+extern "C" int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double p, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (!h->cfg.critic_dropout) return fail(B200SAC_ERR_STATE, "the handle was created without critic_dropout");
+  if (int rc = h->drop.check(replica)) return rc;
+  if (!(p >= 0.0 && p < 1.0))                                   // (NaN fails every comparison)
+    return fail(B200SAC_ERR_INVALID, "the critic dropout rate must be in [0, 1), got %g", p);
+  return h->drop.set(h, stream, replica, &p);
 }
 
 // Gradient-surgery switches, read by the pcgrad launches of the step graphs.
@@ -3511,7 +3558,8 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else {
     // hidden activations (the ReLU masks of the step): "hA.<l>" [2B][H] rows [s';s]; "hQ.<l>" / "hT.<l>" / "hP.<l>" [2][B][H]
     // (critic update pass / target pass -- not kept by the layer-chained plan -- / actor pass); critic_ln handles
-    // "zQ.<l>" / "zT.<l>" / "zP.<l>" [2][B][H], the same passes' pre-normalization activations; CARE mixture encoders
+    // "zQ.<l>" / "zT.<l>" / "zP.<l>" [2][B][H], the same passes' pre-normalization activations (critic_dropout: after the
+    // dropout), critic_dropout handles "mQ.<l>" / "mT.<l>" / "mP.<l>" their keep masks; CARE mixture encoders
     // "mixH.<inst>.<l>" [K][rows][pitch4(H)], inst 0 = critic's on [s';s] (rows 2B), 1 = target's on s', 2 = updated critic's on s
     int l = -1, inst = -1;
     char kind[8] = "";
@@ -3531,6 +3579,21 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
       if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
       b = &v[l];
       n = (int64_t)2 * B * h->cfg.critic_hidden[l];
+    } else if (sscanf(name, "m%1[QTP].%d", kind, &l) == 2) {
+      // critic_dropout: the keep masks of the passes as 0.0 / 1.0, expanded from their bits
+      const std::vector<Buf>& v = h->dmask[kind[0] == 'Q' ? 0 : (kind[0] == 'T' ? 1 : 2)];
+      if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
+      const int H = h->cfg.critic_hidden[l], words = (H + 31) / 32;
+      n = (int64_t)2 * B * H;
+      if (n_floats) *n_floats = n;
+      if (cap_floats < n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld floats", (long long)n);
+      std::vector<uint32_t> bits((size_t)2 * B * words);
+      CU(cudaMemcpyAsync(bits.data(), v[l].p + replica * v[l].rs, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                         (cudaStream_t)stream));
+      CU(cudaStreamSynchronize((cudaStream_t)stream));
+      for (int64_t row = 0; row < 2 * B; ++row)
+        for (int j = 0; j < H; ++j) out_host[row * H + j] = (float)((bits[row * words + j / 32] >> (j % 32)) & 1u);
+      return 0;
     } else {
       return fail(B200SAC_ERR_INVALID, "unknown debug tensor '%s'", name);
     }

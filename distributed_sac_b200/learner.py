@@ -88,8 +88,16 @@ class _BaseLearner:
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
                      n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                     redo_interval=None, redo=None, critic_layer_norm=False):
+                     redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None):
         self.critic_layer_norm = bool(critic_layer_norm)
+        # DroQ (Hiraoka et al. 2022): dropout at rate p before every critic LayerNorm; it needs the LayerNorm critics
+        if critic_dropout is not None:
+            if not self.critic_layer_norm:
+                raise ValueError("critic_dropout= needs critic_layer_norm=True (DroQ's critics are Linear -> Dropout -> "
+                                 "LayerNorm -> ReLU)")
+            if isinstance(critic_dropout, bool) or not 0.0 <= float(critic_dropout) < 1.0:     # (NaN fails too)
+                raise ValueError(f"critic_dropout must be a rate in [0, 1) (got {critic_dropout!r})")
+        self.critic_dropout = None if critic_dropout is None else float(critic_dropout)
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
         self.prioritized = prioritized
@@ -166,6 +174,8 @@ class _BaseLearner:
             self.core.set_update_intervals(actor_update_interval, target_update_interval)
         if max_grad_norm is not None:
             self.set_max_grad_norm(max_grad_norm)
+        if self.critic_dropout is not None:
+            self.core.set_critic_dropout(self.critic_dropout)
         if self.cagrad is not None:
             self.core.set_pcgrad(critic=False, actor=False)
             self.set_cagrad(self.cagrad)
@@ -225,7 +235,8 @@ class _BaseLearner:
                           lr_critic=float(self.lr_critic),
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
                           log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None,
-                          pcgrad=self.pcgrad or self.cagrad is not None, critic_layer_norm=self.critic_layer_norm)
+                          pcgrad=self.pcgrad or self.cagrad is not None, critic_layer_norm=self.critic_layer_norm,
+                          critic_dropout=self.critic_dropout is not None)
 
     # ---- reference method surface -------------------------------------------------------------
     def _chunks(self, n):
@@ -404,7 +415,8 @@ class _BaseLearner:
         if net == "actor":
             return names.actor_key_map(self.family, na)
         which = 1 if "1" in net else 2
-        return names.critic_key_map(self.family, nc, which, target="target" in net, layer_norm=self.critic_layer_norm)
+        return names.critic_key_map(self.family, nc, which, target="target" in net, layer_norm=self.critic_layer_norm,
+                                    dropout=self.critic_dropout is not None)
 
     def _module_state_dict(self, net, which=_lib.PARAMS, named=None):
         named = named if named is not None else self.core.get_named(which)
@@ -488,6 +500,8 @@ class _BaseLearner:
         self._load_adam(ck["log_alpha_optimizer"], ["log_alpha"], 2)
         if "alpha" in ck:
             self.alpha = ck["alpha"].detach().reshape(-1).clone()
+        if self.critic_dropout is not None:         # the rate is a setting of the learner, not part of the checkpoint
+            self.core.set_critic_dropout(self.critic_dropout)
 
     # ---- Redis-facing loop (LL/learner.py:191-201,278-316) -------------------------------------
     def write(self, update_iteration, critic_loss, actor_loss, entropy=None, log_alpha=None):
@@ -573,12 +587,12 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
                  pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None,
-                 critic_layer_norm=False):
+                 critic_layer_norm=False, critic_dropout=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
 
     def _set_dims(self):
         c = self.cfg
@@ -603,10 +617,10 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
                  target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                 redo_interval=None, redo=None, critic_layer_norm=False):
+                 redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
 
     def _set_dims(self):
         c = self.cfg
@@ -634,11 +648,12 @@ class MTSACLearner(_BaseLearner):
     def __init__(self, train_classes, train_tasks, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None,
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
-                 cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None, critic_layer_norm=False):
+                 cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None, critic_layer_norm=False,
+                 critic_dropout=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
 
     def _set_dims(self):
         c = self.cfg

@@ -13,7 +13,9 @@ reference's key names are a compatibility contract:
 
 Layer-normalized critics (critic_layer_norm) add a LayerNorm after every hidden Linear: `layer_norms.{i}.*` beside the LL / VS
 Critic's Linear keys, and the natural nn.Sequential(Linear, LayerNorm, ReLU, ...) numbering Q_function_{w}.{3i}.* (Linear i),
-Q_function_{w}.{3i+1}.* (its LayerNorm) for MS.
+Q_function_{w}.{3i+1}.* (its LayerNorm) for MS.  Dropout Q-functions (critic_dropout) keep the LL / VS keys (the dropout
+has no parameters) and number MS as nn.Sequential(Linear, Dropout, LayerNorm, ReLU, ...): Q_function_{w}.{4i}.* (Linear i),
+Q_function_{w}.{4i+2}.* (its LayerNorm).
 
 Canonical names (used by the C ABI's layout table): `<net>.<i>.weight|bias`
 with net in {actor,q1,q2,q1_target,q2_target}, `<net>.<i>.ln.weight|bias` for a critic's LayerNorm and `log_alpha`.
@@ -35,17 +37,21 @@ def actor_key_map(family: str, n_layers: int):
     return m
 
 
-def critic_key_map(family: str, n_layers: int, which: int, target: bool = False, layer_norm: bool = False):
+def critic_key_map(family: str, n_layers: int, which: int, target: bool = False, layer_norm: bool = False,
+                   dropout: bool = False):
     """{reference key: canonical key} for Q-function `which` (1|2), in the canonical layout order; n_layers counts the
     head.
 
     LL/VS: keys of ONE Critic module (local_critic_{which});
     MS   : keys of the twin Critic module restricted to Q_function_{which}.
-    layer_norm: the critics with a LayerNorm after every hidden Linear (the module docstring gives the keys)."""
+    layer_norm: the critics with a LayerNorm after every hidden Linear; dropout (with layer_norm): a Dropout between them
+    (the module docstring gives the keys)."""
+    if dropout and not layer_norm:
+        raise ValueError("dropout=True describes the DroQ critics, which have layer_norm=True")
     if family not in ("LL", "VS", "MS"):
         raise ValueError(family)
     net = f"q{which}" + ("_target" if target else "")
-    step = 3 if layer_norm else 2          # MS: modules per hidden layer of the nn.Sequential
+    step = 4 if dropout else (3 if layer_norm else 2)      # MS: modules per hidden layer of the nn.Sequential
     m = {}
     for i in range(n_layers):
         for kind in ("weight", "bias"):
@@ -56,7 +62,7 @@ def critic_key_map(family: str, n_layers: int, which: int, target: bool = False,
             m[ref] = f"{net}.{i}.{kind}"
         if layer_norm and i < n_layers - 1:
             for kind in ("weight", "bias"):
-                ref = f"layer_norms.{i}.{kind}" if family in ("LL", "VS") else f"Q_function_{which}.{3 * i + 1}.{kind}"
+                ref = f"layer_norms.{i}.{kind}" if family in ("LL", "VS") else f"Q_function_{which}.{step * i + step - 2}.{kind}"
                 m[ref] = f"{net}.{i}.ln.{kind}"
     return m
 

@@ -35,6 +35,9 @@
  *   b200sac_set/get/read_pcgrad, b200sac_export_task_grad
  *                            PCGrad gradient surgery (Yu et al., NeurIPS 2020) for the multi-task learners' optimizers,
  *                            per replica and optimizer, with the step's Gram matrix and surgery decisions reported
+ *   b200sac_set/get_critic_dropout
+ *                            Dropout Q-functions (DroQ, Hiraoka et al., ICLR 2022): dropout before every critic LayerNorm,
+ *                            with a rate per replica
  *   b200sac_set/get/read_cagrad, b200sac_cagrad_solve_test
  *                            CAGrad (Liu et al., NeurIPS 2021) on the same handles, per replica and optimizer, with the
  *                            step's dual solution reported
@@ -115,6 +118,9 @@ typedef struct b200sac_cfg {
                                         grad_clip = 0; MTSAC and CARE (care = 1 | 2) alike.  Fixed at create. */
   int32_t critic_ln;                 /* 0 = the default plan; 1 = LayerNorm in the critics' hidden layers.  Fixed at create.
                                         See "Layer-normalized critics" below. */
+  int32_t critic_dropout;            /* 0 = the critic_ln plan; 1 = dropout before every critic LayerNorm (DroQ), the rate
+                                        set per replica by b200sac_set_critic_dropout.  Needs critic_ln = 1.  Fixed at
+                                        create.  See "Dropout Q-functions" below. */
 } b200sac_cfg;
 
 /* Layer-normalized critics (cfg.critic_ln = 1; Ba et al. 2016, as high-replay-ratio SAC uses it: DroQ, Lyle et al. 2023,
@@ -147,6 +153,31 @@ typedef struct b200sac_cfg {
  * The actor-pass launches return at entry on a critic-only step.
  * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_ln outside {0, 1}, or together with
  * care != 0 or pcgrad = 1.  b200sac_redo on such a handle gives B200SAC_ERR_STATE (see there). */
+
+/* Dropout Q-functions (cfg.critic_dropout = 1; DroQ, Hiraoka et al., ICLR 2022).  On a critic_ln handle, every hidden
+ * layer l of q1, q2, q1_target and q2_target becomes nn.Sequential(Linear, Dropout(p), LayerNorm, ReLU), in training
+ * mode on every critic evaluation of the step: pass A (critics on (s, a)), pass B (targets on (s', a')) and pass D
+ * (critics on (s, a~), the actor pass).  With p the replica's rate (b200sac_set_critic_dropout; 0 at create):
+ *   z' = z * (m ? s : 0) with z = W_l x + b_l, then h = relu(LN(z')) as under "Layer-normalized critics";
+ *   s = (float)(1 / (1 - p)), evaluated in fp64 and rounded once; the product is one fp32 multiply;
+ *   m in {0, 1}: an element is dropped iff its 32-bit Philox word is below t = floor(p * 2^32) (fp64, on the host).
+ * p = 0 drops nothing and multiplies by 1: the step is bit-identical to the same handle with critic_dropout = 0.
+ * Random stream: Philox4x32-10 with key = seed ^ (0xE7037ED1A0B428DB * (replica + 1)) (mod 2^64; seed = b200sac_create's,
+ * the policy noise's; key[0] = its low 32 bits, key[1] = its high 32 bits), a multiplier no other draw of the library uses;
+ * counter (c0, c1, c2, c3) = (step & 0xFFFFFFFF, step >> 32, b, (tag << 24) | (j / 4)) where step = the replica's step
+ * index the policy noise uses (the number of steps the replica has run, this one included; 1 on the first), b the row of
+ * the minibatch (0..batch-1), j the column (0..H-1) and tag = (pass * 8 + l) * 2 + net with pass A = 0, B = 1, D = 2 and
+ * net = 0 for q1 / q1_target, 1 for q2 / q2_target.  Column j takes output word j % 4.  Masks therefore do not depend on
+ * the replica count, and differ per step, pass, layer, net and replica.
+ * Backward: dz = dz' * (m ? s : 0), dz' the LayerNorm backward's output as without dropout; the weight and input
+ * gradients and the LayerNorm weight / bias gradients follow unchanged.  On a critic-only step the pass-D launches return
+ * at entry: no pass-D masks are drawn.
+ * Plan: the same launches and labels as the critic_ln plan; the LayerNorm launches draw, apply and keep the masks (bits
+ * [2][batch][ceil(H / 32)] per replica, pass and layer; column j is bit j % 32 of word j / 32).  No parameters: the layout
+ * is that of the same cfg with critic_dropout = 0.  The rate is not copied by b200sac_copy_replica and not part of the
+ * parameter arenas.  No inference path runs the critics, so there is no evaluation mode.
+ * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_dropout outside {0, 1}, or 1 with
+ * critic_ln = 0. */
 
 typedef struct b200sac_tensor_desc {
   char name[48];                     /* canonical name, e.g. "q1_target.2.weight" */
@@ -338,6 +369,14 @@ int b200sac_get_update_intervals(b200sac_t* h, int32_t replica, int32_t* actor_e
  * part of a checkpoint.  Get: the values last set (host mirror: does not synchronise). */
 int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double critic, double actor, double ctx, void* stream);
 int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double* actor, double* ctx);
+
+/* Critic dropout rate p of one replica ("Dropout Q-functions" above).  Set: stream-ordered like b200sac_set_grad_clip --
+ * steps enqueued after the call (launches of graphs b200sac_prepare instantiated included; no graph is rebuilt) use the
+ * new rate, steps enqueued before it do not.  p in [0, 1); NaN, p < 0, p >= 1 or a bad replica give B200SAC_ERR_INVALID
+ * and change nothing.  A handle created without critic_dropout gives B200SAC_ERR_STATE.  Get reads the host mirror of
+ * the last accepted value (no synchronisation). */
+int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double p, void* stream);
+int b200sac_get_critic_dropout(b200sac_t* h, int32_t replica, double* p);
 /* Pre-clip gradient norms of the most recent `n_last` steps (<= 1024 kept, slots aligned with b200sac_read_losses):
  * out[n_last][replicas][3] = {critic, actor, context encoder}; NaN where that optimizer did not step (the actor on a
  * critic-only step, the context encoder outside CARE(O)).  Synchronises the stream. */
@@ -513,7 +552,9 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
  * after b200sac_act its first n rows), or a hidden (after b200sac_redo: its forward's rows, see there)
  * activation whose sign pattern is the ReLU mask the step used: "hA.<l>" [2B][H] (rows [s';s]), "hQ.<l>" / "hP.<l>" /
  * "hT.<l>" [2][B][H] (critic-update pass / actor pass / target pass; the layer-chained plan does not keep hT); with
- * cfg.critic_ln, "zQ.<l>" / "zP.<l>" / "zT.<l>" [2][B][H], the same passes' pre-normalization activations W x + b;
+ * cfg.critic_ln, "zQ.<l>" / "zP.<l>" / "zT.<l>" [2][B][H], the same passes' pre-normalization activations W x + b (with
+ * cfg.critic_dropout: z', after the dropout); with cfg.critic_dropout, "mQ.<l>" / "mP.<l>" / "mT.<l>" [2][B][H], the same
+ * passes' keep masks as 0.0 / 1.0;
  * "mixH.<inst>.<l>" [K][rows][pitch4(H)] (CARE mixture encoders).  After a step from a prioritized ring: "isw" [B] (the
  * importance weights of its critic loss), "prio" [B] (the leaf values p it wrote) and "idx" [B] (its ring indices, int32
  * bit patterns).  After a step from a linked ring (n-step returns): "disc" [B] (the per-row discount of its TD target),
