@@ -421,6 +421,22 @@ struct ReplicaTable {
   int set(b200sac* h, void* stream, int replica, const Mirror* v, cudaEvent_t written = nullptr);
 };
 
+// The twin critics are evaluated on three sets of rows per step, each a pass with its own buffers; the index of a pass is
+// its Philox pass index (dropout masks).  Q: the local critics on (s, a) for the critic update (phase A, backward in C);
+// T: the target critics on (s', a') for the TD target (phase B); P: the updated local critics on (s, a~) for the actor
+// loss (phase D, forward and backward).  Every [2][B] / [2][B][H] buffer holds q1's rows, then q2's.
+enum { PASS_Q = 0, PASS_T = 1, PASS_P = 2 };
+struct CriticPass {
+  const std::vector<LayerOff>* net;   // [2]: the networks the pass runs (L.q or L.qt)
+  const Buf* X;                       // input rows [B][ldx] (XQ, XT, XP)
+  const Buf* q;                       // head values [2][B] (q, qt, qp)
+  const char* label;                  // in its LayerNorm launches' labels
+  char letter;                        // in its debug names (b200sac_debug_read)
+  // per critic hidden layer [2][B][H]: the post-ReLU activations; critic_ln: the pre-normalization activations (after the
+  // dropout on critic_dropout handles); critic_dropout: the keep-mask bits [2][B][ceil(H / 32)] (uint32 words in float slots)
+  std::vector<Buf> h, z, m;
+};
+
 struct b200sac {
   b200sac_cfg cfg;
   EnvSwitches env;                // read at create
@@ -448,15 +464,12 @@ struct b200sac {
   CareNet care_trunk, care_ctx;
   int care_row_w = 0, care_off_att = 0, care_off_ctx = 0;
   std::vector<Buf> hA, dhA;       // per actor hidden layer
-  std::vector<Buf> hQ, hT, hP, dhQ;   // per critic hidden layer, [2][B][H]
-  // cfg.critic_ln: per critic hidden layer [2][B][H], the pre-normalization activations of hQ, hT and hP; the backward
-  // normalization's chunk column sums [R][2][chunks][2][max H] and tickets [R][2]
-  std::vector<Buf> zQ, zT, zP;
+  CriticPass pass[3] = {{L.q, &XQ, &q, "critic", 'Q'}, {L.qt, &XT, &qt, "target", 'T'}, {L.q, &XP, &qp, "actor pass", 'P'}};
+  std::vector<Buf> dhQ;           // per critic hidden layer [2][B][H]: the critic backward's gradients (passes Q and P)
+  // cfg.critic_ln: the backward normalization's chunk column sums [R][2][chunks][2][max H] and tickets [R][2]
   DevMem<double> ln_part;
   DevMem<unsigned> ln_ticket;
-  // cfg.critic_dropout: per pass (A critics on (s, a), B targets, D actor pass) and critic hidden layer the keep-mask bits
-  // [2][B][ceil(H / 32)] (uint32 words in float slots); [R] dropout rates p (host mirror) and their DropRate
-  std::vector<Buf> dmask[3];
+  // cfg.critic_dropout: [R] dropout rates p (host mirror) and their DropRate
   ReplicaTable<DropRate, 1, double> drop;
   std::vector<Launch> plan;
   // what the plan's launches read through their argument blocks: each wgmma launch's problems, each layer-chained launch's
@@ -921,14 +934,25 @@ struct PlanBuilder {
   const long long rsP, rsG;
   const Buf par, grd;       // parameter and gradient arenas
   int branch = 0;           // branch tag given to the launches gemm_launch creates
+  // per-layer plan, FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads
+  // the rest of the backward chain.  The weight-gradient launch goes to the fork stream and the chain continues at once (the
+  // kernels hold <= 2 CTAs per SM, so both fit); Adam joins.  (tensor-core tiles own a whole SM each: grouping is better there.)
+  const bool use_fork;
   bool actor_side = false;  // the launches being built belong to the actor update: skipped on critic-only steps
   int rc = 0;               // error met by a builder that cannot return one; build_plan returns it
 
   explicit PlanBuilder(b200sac* hh)
       : h(hh), c(hh->cfg), L(hh->L), B(c.batch), R(hh->R), A(c.act_dim), La(c.n_actor_hidden), Lc(c.n_critic_hidden),
-        sms(sm_count()), rsP(L.arena), rsG(L.trainable), par{hh->params, L.arena}, grd{hh->grads, L.trainable} {}
+        sms(sm_count()), rsP(L.arena), rsG(L.trainable), par{hh->params, L.arena}, grd{hh->grads, L.trainable},
+        use_fork(c.precision == 0 && !c.care) {}
   float* W(int64_t off) const { return h->params + off; }
   float* Gp(int64_t off) const { return h->grads + off; }
+  // network net's rows of a [2][B][H] buffer
+  float* netp(const Buf& b, int net, int H) const { return b.p + (long long)net * B * H; }
+  // network net's input rows at critic hidden layer l of pass cp: its input rows X, or layer l - 1's activations
+  Buf critic_in(const CriticPass& cp, int net, int l) const {
+    return l == 0 ? *cp.X : Buf{netp(cp.h[l - 1], net, cp.net[net][l].in), cp.h[l - 1].rs};
+  }
 
   // appends launch l running kern(args), first letting kern take l.smem bytes of dynamic shared memory
   template <class F, class... P> void push(Launch l, F kern, const P&... args) {
@@ -962,7 +986,9 @@ struct PlanBuilder {
   void adam(int which, bool tail_only, bool with_tail = true);
   void grad_norm(int which);
   void pcgrad(int which);
-  void layer_norm(const char* pass, int l, bool target, const std::vector<Buf>& z, const std::vector<Buf>* hb, bool want_grads);
+  void layer_norm(int pass, int l, bool fwd, bool want_grads);
+  void critic_fwd(int pass, int l, std::vector<GemmProb> ps = {});
+  void critic_bwd(int pass, int l, bool want_wgrad);
   int build_plan_fused();
   void build_plan_layered();
 };
@@ -1177,7 +1203,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
       P.dW[net] = want_wgrad ? Gp(L.q[net][Lc].w) : nullptr;
       P.db[net] = want_wgrad ? Gp(L.q[net][Lc].b) : nullptr;
     }
-    const Buf& hb = want_wgrad ? h->hQ[Lc - 1] : h->hP[Lc - 1];
+    const Buf& hb = h->pass[want_wgrad ? PASS_Q : PASS_P].h[Lc - 1];
     const Buf& dq = want_wgrad ? h->dq : h->dqa;
     P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = 2 * h->y.rs;
     P.h = hb.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hb.rs; P.ldh = Hc;
@@ -1427,10 +1453,11 @@ int PlanBuilder::build_plan_fused() {
            return fwd ? chain_kernel<true, ROWS> : chain_kernel<false, ROWS>;
          }), P);
   };
-  // chain2_kernel launch: forward of the twins fnet[0..1] on X, their head values swapped, backward of the local critics
-  auto pair_launch = [&](const char* label, int kind, int early, const std::vector<LayerOff>* fnet /* [2] */, const float* X, long long rsX,
-                         const std::vector<Buf>* fstore, const Buf& qf, const std::vector<Buf>& acts, const std::vector<Buf>* dstore,
-                         bool tail) {
+  // chain2_kernel launch: forward of pass fwd's twins, their head values swapped, backward of pass bwd's (local) twins.
+  // The forward's activations are stored only when the backward gates on them (fwd == bwd); the critic job stores its
+  // input gradients for the weight gradients, the actor-pass job runs on to d(action).
+  auto pair_launch = [&](const char* label, int kind, int early, int fwd, int bwd) {
+    const CriticPass &f = h->pass[fwd], &b = h->pass[bwd];
     Chain2Args P;
     memset(&P, 0, sizeof(P));
     P.kind = kind; P.rsP = rsP; P.rw = rw;
@@ -1439,16 +1466,15 @@ int PlanBuilder::build_plan_fused() {
     for (int net = 0; net < 2; ++net) {
       Chain2Job& J = P.job[net];
       J.rows = B; J.nfwd = Lc; J.nbwd = Lc - 1; J.net = net;
-      fwd_stages(J, J.st, fnet[net], Lc, X, rsX, h->K.ldx, h->K.xw, fstore, (long long)net * B);
+      fwd_stages(J, J.st, f.net[net], Lc, f.X->p, f.X->rs, h->K.ldx, h->K.xw, fwd == bwd ? &f.h : nullptr, (long long)net * B);
       for (int s = 0; s < Lc; ++s) fs.push_back(&J.st[s]);
-      const LayerOff& fh = fnet[net][Lc];
+      const LayerOff& fh = f.net[net][Lc];
       J.Whf = W(fh.w); J.bhf = W(fh.b); J.Hhf = fh.in;
-      J.qf_out = qf.p + (long long)net * B; J.rsQf = qf.rs;
-      // backward through the LOCAL twin
-      const std::vector<LayerOff>& bn = L.q[net];
-      bwd_stages(J, J.st + Lc, bn, Lc, acts, (long long)net * B, dstore, (long long)net * B);
+      J.qf_out = f.q->p + (long long)net * B; J.rsQf = f.q->rs;
+      const std::vector<LayerOff>& bn = b.net[net];
+      bwd_stages(J, J.st + Lc, bn, Lc, b.h, (long long)net * B, kind == C2_CRITIC ? &h->dhQ : nullptr, (long long)net * B);
       J.Whb = W(bn[Lc].w); J.Hhb = bn[Lc].in;
-      if (tail) {
+      if (kind == C2_ACTORQ) {
         const LayerOff& lo = bn[0];
         J.W0 = W(lo.w); J.ldw0 = lo.ld; J.col0 = h->K.in_w; J.nact = A; J.H0 = lo.out;
         J.dx = h->dxP.p + (long long)net * B * h->K.ldx; J.rsDx = h->dxP.rs; J.lddx = h->K.ldx;
@@ -1540,21 +1566,22 @@ int PlanBuilder::build_plan_fused() {
     return 0;
   };
 
+  const CriticPass& Q = h->pass[PASS_Q];
   // ---- A: actor over [s';s], Q1/Q2 over (s,a) ----------------------------------------------------------------------
   {
     ChainArgs P = new_chain(3, 1);
     for (int j = 0; j < 3; ++j) {
       ChainJob& J = P.job[j];
       const int net = j - 1;
-      const std::vector<LayerOff>& mlp = j == 0 ? L.actor : L.q[net];
+      const std::vector<LayerOff>& mlp = j == 0 ? L.actor : Q.net[net];
       const int nh = j == 0 ? La : Lc;
       J.kind = CJ_FWD; J.nstages = nh;
       if (j == 0) {
         J.rows = 2 * B; J.head = CH_HEAD_POLICY;
         fwd_stages(J, J.st, mlp, nh, h->XA.p, h->XA.rs, h->K.ldxa, h->K.in_w, &h->hA, 0);
       } else {
-        J.rows = B; J.head = CH_HEAD_SCALAR; J.qout = h->q.p + (long long)net * B; J.rsQ = h->q.rs;
-        fwd_stages(J, J.st, mlp, nh, h->XQ.p, h->XQ.rs, h->K.ldx, h->K.xw, &h->hQ, (long long)net * B);
+        J.rows = B; J.head = CH_HEAD_SCALAR; J.qout = Q.q->p + (long long)net * B; J.rsQ = Q.q->rs;
+        fwd_stages(J, J.st, mlp, nh, Q.X->p, Q.X->rs, h->K.ldx, h->K.xw, &Q.h, (long long)net * B);
       }
       const LayerOff& hd = mlp[nh];
       J.Wh = W(hd.w); J.bh = W(hd.b); J.NO = hd.out; J.Hh = hd.in;
@@ -1562,11 +1589,11 @@ int PlanBuilder::build_plan_fused() {
     finish_chain("chain_fwd{actor,q1,q2}", P);
   }
   // ---- B + C: target critics over (s', a'), TD target, critic backward (one clustered launch), weight gradients, Adam ----
-  pair_launch("chain2{qt->y->bwd q}", C2_CRITIC, 1, L.qt, h->XT.p, h->XT.rs, nullptr, h->qt, h->hQ, &h->dhQ, false);
+  pair_launch("chain2{qt->y->bwd q}", C2_CRITIC, 1, PASS_T, PASS_Q);
   {
     std::vector<WNet> nets;
     for (int net = 0; net < 2; ++net)
-      nets.push_back(WNet{&L.q[net], Lc, &h->dhQ, &h->hQ, 0, h->XQ.p, h->XQ.rs, h->K.ldx, h->dq.p + (long long)net * B, h->dq.rs, 1, net});
+      nets.push_back(WNet{&Q.net[net], Lc, &h->dhQ, &Q.h, 0, Q.X->p, Q.X->rs, h->K.ldx, h->dq.p + (long long)net * B, h->dq.rs, 1, net});
     if (int rc = wgrad_launch(nets, clip ? "wgrad{q1,q2}" : "wgrad+adam+polyak{q1,q2}", 0, clip)) return rc;
   }
   if (clip) {                    // the whole critic gradient first, then its norm, then Adam + Polyak on the clipped gradient
@@ -1575,7 +1602,7 @@ int PlanBuilder::build_plan_fused() {
   }
   // ---- D: actor pass through the updated critics ------------------------------------------------------------------------
   // (the launch right before this one is the critic Adam: no weight request before the dependency wait)
-  pair_launch("chain2{q(s,a~)->min->bwd->d(action)}", C2_ACTORQ, 0, L.q, h->XP.p, h->XP.rs, &h->hP, h->qp, h->hP, nullptr, true);
+  pair_launch("chain2{q(s,a~)->min->bwd->d(action)}", C2_ACTORQ, 0, PASS_P, PASS_P);
   // actor loss / entropy / temperature gradient + its Adam step need only what D produced (the step's alpha is the
   // snapshot taken at ingest): they run on the fork stream beside the policy backward instead of trailing the actor Adam
   adam(1, true);
@@ -1600,26 +1627,25 @@ int PlanBuilder::build_plan_fused() {
   return 0;
 }
 
-// critic_ln handles: the LayerNorm of hidden layer l of both critics (the targets' when `target`) over the [2][B][H]
-// pre-normalization buffer z[l], every replica in one launch.  Forward (hb set): hb[l] = relu(LN(z[l])).  Backward (hb
-// null): dhQ[l] becomes the gradient at z[l] in place, and with want_grads the LayerNorm weight and bias gradients land
-// in gradient slice 0 (the split-K slices hold zeros there, so Adam's slice sum reads them unchanged).  critic_dropout
-// handles run the dropout instantiations on the same launches: the pass of z (zQ: A, zT: B, zP: D) picks the mask
-// buffer and the Philox tag.
-void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::vector<Buf>& z, const std::vector<Buf>* hb,
-                             bool want_grads) {
+// critic_ln handles: the LayerNorm of hidden layer l of both of pass `pass`'s networks over the [2][B][H]
+// pre-normalization buffer z[l], every replica in one launch.  Forward: h[l] = relu(LN(z[l])).  Backward: dhQ[l] becomes
+// the gradient at z[l] in place, and with want_grads the LayerNorm weight and bias gradients land in gradient slice 0 (the
+// split-K slices hold zeros there, so Adam's slice sum reads them unchanged).  critic_dropout handles run the dropout
+// instantiations on the same launches, with the pass's mask buffer and Philox tag.
+void PlanBuilder::layer_norm(int pass, int l, bool fwd, bool want_grads) {
+  const CriticPass& cp = h->pass[pass];
   const int H = c.critic_hidden[l];
   Launch ln;
-  ln.label = std::string(hb ? "ln_fwd{" : "ln_bwd{") + pass + " " + std::to_string(l) + "}";
+  ln.label = std::string(fwd ? "ln_fwd{" : "ln_bwd{") + cp.label + " " + std::to_string(l) + "}";
   ln.branch = branch;
   LnArgs P;
   memset(&P, 0, sizeof(P));
-  P.z = z[l].p; P.rsZ = z[l].rs;
-  const Buf& out = hb ? (*hb)[l] : h->dhQ[l];
-  (hb ? P.h : P.dh) = out.p;
+  P.z = cp.z[l].p; P.rsZ = cp.z[l].rs;
+  const Buf& out = fwd ? cp.h[l] : h->dhQ[l];
+  (fwd ? P.h : P.dh) = out.p;
   P.rsH = out.rs;
   for (int net = 0; net < 2; ++net) {
-    const LayerOff& lo = (target ? L.qt : L.q)[net][l];
+    const LayerOff& lo = cp.net[net][l];
     P.g[net] = W(lo.g); P.c[net] = W(lo.c);
     if (want_grads) { P.dg[net] = Gp(lo.g); P.dc[net] = Gp(lo.c); }
   }
@@ -1629,12 +1655,11 @@ void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::ve
   P.actor_side = actor_side ? 1 : 0;
   const bool drop = c.critic_dropout != 0;
   if (drop) {
-    const int pass = &z == &h->zQ ? 0 : (&z == &h->zT ? 1 : 2);
-    P.drop = h->drop.dev; P.mbits = (unsigned*)h->dmask[pass][l].p; P.rsM = h->dmask[pass][l].rs;
+    P.drop = h->drop.dev; P.mbits = (unsigned*)cp.m[l].p; P.rsM = cp.m[l].rs;
     P.tag0 = (pass * 8 + l) * 2;
   }
   ln.block = dim3(kLnThreads);
-  if (hb) {
+  if (fwd) {
     ln.grid = dim3((2 * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
     if (drop) push(std::move(ln), ln_fwd_kernel<true>, P);
     else push(std::move(ln), ln_fwd_kernel<false>, P);
@@ -1645,27 +1670,58 @@ void PlanBuilder::layer_norm(const char* pass, int l, bool target, const std::ve
   }
 }
 
+// Forward of pass `pass`'s twins at critic hidden layer l, in one grouped launch after the problems ps already holds.
+// critic_ln: the GEMMs write the pre-normalization buffer z (no ReLU), the layer_norm launch the post-ReLU h that the rest
+// of the plan reads.
+void PlanBuilder::critic_fwd(int pass, int l, std::vector<GemmProb> ps) {
+  const CriticPass& cp = h->pass[pass];
+  const bool ln = c.critic_ln != 0;
+  const Buf& out = ln ? cp.z[l] : cp.h[l];
+  for (int net = 0; net < 2; ++net) {
+    const LayerOff& lo = cp.net[net][l];
+    const Buf x = critic_in(cp, net, l);
+    GemmProb p = fwd_prob(par, x.p, x.rs, B, lo, netp(out, net, lo.out), out.rs);
+    if (ln) p.relu = 0;
+    ps.push_back(p);
+  }
+  gemm_launch(ps);
+  if (ln) layer_norm(pass, l, true, false);
+}
+
+// Backward of pass `pass`'s twins at critic hidden layer l from dhQ[l]: with want_wgrad the weight gradients (the critic
+// update), and the input gradients, gated by the layer's input activations, into dhQ[l - 1]; at layer 0 into dxP, which
+// the actor pass needs and, on CARE handles, the critic update too (it trains the critic's state encoder).
+void PlanBuilder::critic_bwd(int pass, int l, bool want_wgrad) {
+  const CriticPass& cp = h->pass[pass];
+  // (on the main stream: a forked weight gradient below waits for it like the input gradient does)
+  if (c.critic_ln) layer_norm(pass, l, false, want_wgrad);
+  std::vector<GemmProb> ps, dg;
+  for (int net = 0; net < 2; ++net) {
+    const LayerOff& lo = cp.net[net][l];
+    const Buf x = critic_in(cp, net, l), dz{netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs};
+    if (want_wgrad) ps.push_back(wgrad_prob(grd, dz.p, dz.rs, x.p, x.rs, lo, B));
+    if (l > 0)
+      dg.push_back(dgrad_prob(par, dz.p, dz.rs, lo, x.p, x.rs, netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs, B));
+    else if (!want_wgrad || c.care)
+      dg.push_back(dgrad_prob(par, dz.p, dz.rs, lo, nullptr, 0, h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs, B));
+  }
+  if (want_wgrad && use_fork && l > 0) {
+    branch = 1; gemm_launch(ps); branch = 0;
+    gemm_launch(dg);
+  } else {
+    ps.insert(ps.end(), dg.begin(), dg.end());      // {wgrad q1, wgrad q2, dgrad q1, dgrad q2}
+    gemm_launch(ps);
+  }
+}
+
 // ---- per-layer plan: one grouped GEMM launch per layer (and kind) of the networks --------------------------------
 void PlanBuilder::build_plan_layered() {
   const int Kenc = c.num_encoders, nmix = c.care ? (int)L.mix.size() : 0;
-  // FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads the rest of the
-  // backward chain.  The weight-gradient launch goes to the fork stream and the chain continues at once (the kernels hold
-  // <= 2 CTAs per SM, so both fit); Adam joins.  (tensor-core tiles own a whole SM each: grouping is better there.)
-  const bool use_fork = (c.precision == 0) && !c.care;
   if (c.care) {
     // encoded states of [s'; s] with the critic's (== actor's, tied) encoder and of s' with the target's
     care_tables({0, 1});
     care_encode({EncJob{0, 0, 2 * B, h->XA, h->K.ldxa, h->XQ, h->K.ldx, B}, EncJob{1, 0, B, h->XT, h->K.ldx, Buf{}, 0, 0}});
   }
-  auto netp = [&](const Buf& b, int net, int H) { return b.p + (long long)net * B * H; };
-  // critic_ln: a critic hidden layer's GEMM writes the pre-normalization buffer z (no ReLU), its layer_norm launch the
-  // post-ReLU h that the rest of the plan reads
-  const bool ln = c.critic_ln != 0;
-  auto critic_fwd = [&](const float* X, long long rsX, const LayerOff& lo, int net, const Buf& hb, const Buf* zb) {
-    GemmProb p = fwd_prob(par, X, rsX, B, lo, netp(zb ? *zb : hb, net, lo.out), (zb ? *zb : hb).rs);
-    if (zb) p.relu = 0;
-    return p;
-  };
   // ---- Phase A: actor over [s2; s] and Q1,Q2 over (s,a), layer by layer -----------------
   for (int l = 0; l < (La > Lc ? La : Lc); ++l) {
     std::vector<GemmProb> ps;
@@ -1674,23 +1730,17 @@ void PlanBuilder::build_plan_layered() {
       ps.push_back(fwd_prob(par, l == 0 ? h->XA.p : h->hA[l - 1].p, l == 0 ? h->XA.rs : h->hA[l - 1].rs, 2 * B, lo,
                        h->hA[l].p, h->hA[l].rs));
     }
-    if (l < Lc)
-      for (int net = 0; net < 2; ++net) {
-        const LayerOff& lo = L.q[net][l];
-        ps.push_back(critic_fwd(l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in), l == 0 ? h->XQ.rs : h->hQ[l - 1].rs, lo,
-                                net, h->hQ[l], ln ? &h->zQ[l] : nullptr));
-      }
     if (use_fork && La == Lc) {
       // Q1,Q2 on (s,a) are not needed before critic_heads, while the actor's output heads the policy_head -> target-critic
       // chain: the critics' layer goes to the fork stream (joined at critic_heads), the actor's stays on the main stream.
       branch = 1;
-      gemm_launch(std::vector<GemmProb>(ps.begin() + 1, ps.end()));
-      if (ln) layer_norm("critic", l, false, h->zQ, &h->hQ, false);
+      critic_fwd(PASS_Q, l);
       branch = 0;
-      gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 1));
+      gemm_launch(ps);
+    } else if (l < Lc) {
+      critic_fwd(PASS_Q, l, ps);
     } else {
       gemm_launch(ps);
-      if (ln && l < Lc) layer_norm("critic", l, false, h->zQ, &h->hQ, false);
     }
   }
   {  // policy head
@@ -1701,16 +1751,7 @@ void PlanBuilder::build_plan_layered() {
     push(std::move(l), policy_head_kernel, h->pol);
   }
   // ---- Phase B: target critics over (s2, a') ---------------------------------------------
-  for (int l = 0; l < Lc; ++l) {
-    std::vector<GemmProb> ps;
-    for (int net = 0; net < 2; ++net) {
-      const LayerOff& lo = L.qt[net][l];
-      ps.push_back(critic_fwd(l == 0 ? h->XT.p : netp(h->hT[l - 1], net, lo.in), l == 0 ? h->XT.rs : h->hT[l - 1].rs, lo,
-                              net, h->hT[l], ln ? &h->zT[l] : nullptr));
-    }
-    gemm_launch(ps);
-    if (ln) layer_norm("target", l, true, h->zT, &h->hT, false);
-  }
+  for (int l = 0; l < Lc; ++l) critic_fwd(PASS_T, l);
   const int Hc = c.critic_hidden[Lc - 1];
   {  // critic heads: y, Q1, Q2, dQ
     Launch l;
@@ -1721,7 +1762,8 @@ void PlanBuilder::build_plan_layered() {
     l.block = dim3(256);
     CriticHeadArgs P;
     memset(&P, 0, sizeof(P));
-    P.hT = h->hT[Lc - 1].p; P.hQ = h->hQ[Lc - 1].p; P.rsHnet = (long long)B * Hc; P.rsHrep = h->hT[Lc - 1].rs; P.ldh = Hc;
+    const Buf &hT = h->pass[PASS_T].h[Lc - 1], &hQ = h->pass[PASS_Q].h[Lc - 1];
+    P.hT = hT.p; P.hQ = hQ.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hT.rs; P.ldh = Hc;
     for (int net = 0; net < 2; ++net) {
       P.Wt[net] = W(L.qt[net][Lc].w); P.bt[net] = W(L.qt[net][Lc].b);
       P.Wq[net] = W(L.q[net][Lc].w); P.bq[net] = W(L.q[net][Lc].b);
@@ -1735,35 +1777,7 @@ void PlanBuilder::build_plan_layered() {
   }
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
-  for (int l = Lc - 1; l >= 0; --l) {
-    // (on the main stream: the forked weight gradient below waits for it like the input gradient does)
-    if (ln) layer_norm("critic", l, false, h->zQ, nullptr, true);
-    std::vector<GemmProb> ps;
-    for (int net = 0; net < 2; ++net) {
-      const LayerOff& lo = L.q[net][l];
-      const float* X = l == 0 ? h->XQ.p : netp(h->hQ[l - 1], net, lo.in);
-      const long long rsX = l == 0 ? h->XQ.rs : h->hQ[l - 1].rs;
-      ps.push_back(wgrad_prob(grd, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, X, rsX, lo, B));
-    }
-    if (l > 0)
-      for (int net = 0; net < 2; ++net) {
-        const LayerOff& lo = L.q[net][l];
-        ps.push_back(dgrad_prob(par, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hQ[l - 1], net, lo.in), h->hQ[l - 1].rs,
-                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs, B));
-      }
-    else if (c.care)     // the critic loss also trains the critic's state encoder: need d(loss)/d(encoded state)
-      for (int net = 0; net < 2; ++net) {
-        const LayerOff& lo = L.q[net][0];
-        ps.push_back(dgrad_prob(par, netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
-                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs, B));
-      }
-    if (use_fork && l > 0) {        // ps = {wgrad q1, wgrad q2, dgrad q1, dgrad q2}
-      branch = 1; gemm_launch(std::vector<GemmProb>(ps.begin(), ps.begin() + 2)); branch = 0;
-      gemm_launch(std::vector<GemmProb>(ps.begin() + 2, ps.end()));
-    } else {
-      gemm_launch(ps);
-    }
-  }
+  for (int l = Lc - 1; l >= 0; --l) critic_bwd(PASS_Q, l, true);
   if (c.care) {
     {  // backward of the attention mix: dZk, d(att)
       Launch l;
@@ -1862,16 +1876,7 @@ void PlanBuilder::build_plan_layered() {
     care_encode({EncJob{2, B, B, h->XP, h->K.ldx, Buf{}, 0, 0}});
   }
   // ---- Phase D: actor pass through the updated critics ---------------------------------------
-  for (int l = 0; l < Lc; ++l) {
-    std::vector<GemmProb> ps;
-    for (int net = 0; net < 2; ++net) {
-      const LayerOff& lo = L.q[net][l];
-      ps.push_back(critic_fwd(l == 0 ? h->XP.p : netp(h->hP[l - 1], net, lo.in), l == 0 ? h->XP.rs : h->hP[l - 1].rs, lo,
-                              net, h->hP[l], ln ? &h->zP[l] : nullptr));
-    }
-    gemm_launch(ps);
-    if (ln) layer_norm("actor pass", l, false, h->zP, &h->hP, false);
-  }
+  for (int l = 0; l < Lc; ++l) critic_fwd(PASS_P, l);
   {
     Launch l;
     l.label = "actor_q_heads";
@@ -1879,7 +1884,8 @@ void PlanBuilder::build_plan_layered() {
     l.block = dim3(256);
     ActorQHeadArgs P;
     memset(&P, 0, sizeof(P));
-    P.hP = h->hP[Lc - 1].p; P.rsHnet = (long long)B * Hc; P.rsHrep = h->hP[Lc - 1].rs; P.ldh = Hc;
+    const Buf& hP = h->pass[PASS_P].h[Lc - 1];
+    P.hP = hP.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hP.rs; P.ldh = Hc;
     for (int net = 0; net < 2; ++net) { P.Wq[net] = W(L.q[net][Lc].w); P.bq[net] = W(L.q[net][Lc].b); }
     P.rsP = rsP;
     P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
@@ -1889,20 +1895,7 @@ void PlanBuilder::build_plan_layered() {
     push(std::move(l), actor_q_heads_kernel, P);
   }
   head_bwd(false, false);
-  for (int l = Lc - 1; l >= 0; --l) {
-    if (ln) layer_norm("actor pass", l, false, h->zP, nullptr, false);
-    std::vector<GemmProb> ps;
-    for (int net = 0; net < 2; ++net) {
-      const LayerOff& lo = L.q[net][l];
-      if (l > 0)
-        ps.push_back(dgrad_prob(par, netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs, lo, netp(h->hP[l - 1], net, lo.in), h->hP[l - 1].rs,
-                           netp(h->dhQ[l - 1], net, lo.in), h->dhQ[l - 1].rs, B));
-      else
-        ps.push_back(dgrad_prob(par, netp(h->dhQ[0], net, lo.out), h->dhQ[0].rs, lo, nullptr, 0,
-                           h->dxP.p + (long long)net * B * h->K.ldx, h->dxP.rs, B));
-    }
-    gemm_launch(ps);
-  }
+  for (int l = Lc - 1; l >= 0; --l) critic_bwd(PASS_P, l, false);
   // ---- Phase E: policy backward + Adam + temperature -----------------------------------------
   head_bwd(true, true);
   for (int l = La - 1; l >= 0; --l) {
@@ -2234,9 +2227,12 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     slab.request(h->hA[l], (size_t)2 * B * cfg->actor_hidden[l]);
     slab.request(h->dhA[l], (size_t)B * cfg->actor_hidden[l]);
   }
-  h->hQ.resize(Lc); h->hT.resize(Lc); h->hP.resize(Lc); h->dhQ.resize(Lc);
-  for (int l = 0; l < Lc; ++l)
-    for (Buf* b : {&h->hQ[l], &h->hT[l], &h->hP[l], &h->dhQ[l]}) slab.request(*b, (size_t)2 * B * cfg->critic_hidden[l]);
+  for (CriticPass& p : h->pass) p.h.resize(Lc);
+  h->dhQ.resize(Lc);
+  for (int l = 0; l < Lc; ++l) {
+    for (CriticPass& p : h->pass) slab.request(p.h[l], (size_t)2 * B * cfg->critic_hidden[l]);
+    slab.request(h->dhQ[l], (size_t)2 * B * cfg->critic_hidden[l]);
+  }
   if (cfg->care) {
     const int Kenc = cfg->num_encoders, T = cfg->num_tasks;
     auto pitch = [](int w) { return (w + 3) & ~3; };
@@ -2269,10 +2265,10 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     slab.request(h->mixDZ, (size_t)Kenc * B * pitch(cfg->mix_out));
   }
   if (cfg->critic_ln) {
-    h->zQ.resize(Lc); h->zT.resize(Lc); h->zP.resize(Lc);
+    for (CriticPass& p : h->pass) p.z.resize(Lc);
     int maxH = 0;
     for (int l = 0; l < Lc; ++l) {
-      for (Buf* b : {&h->zQ[l], &h->zT[l], &h->zP[l]}) slab.request(*b, (size_t)2 * B * cfg->critic_hidden[l]);
+      for (CriticPass& p : h->pass) slab.request(p.z[l], (size_t)2 * B * cfg->critic_hidden[l]);
       maxH = std::max(maxH, cfg->critic_hidden[l]);
     }
     const size_t chunks = (size_t)(B + kLnRows - 1) / kLnRows;
@@ -2281,9 +2277,9 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     CU(cudaMemset(h->ln_ticket, 0, sizeof(unsigned) * R * 2));
   }
   if (cfg->critic_dropout) {  // rate 0 on every replica; masks all zero until a step draws them
-    for (std::vector<Buf>& v : h->dmask) {
-      v.resize(Lc);
-      for (int l = 0; l < Lc; ++l) slab.request(v[l], (size_t)2 * B * ((cfg->critic_hidden[l] + 31) / 32));
+    for (CriticPass& p : h->pass) {
+      p.m.resize(Lc);
+      for (int l = 0; l < Lc; ++l) slab.request(p.m[l], (size_t)2 * B * ((cfg->critic_hidden[l] + 31) / 32));
     }
     const double p0 = 0.0;
     if (int rc = h->drop.init(R, &p0)) return rc;
@@ -3426,16 +3422,17 @@ extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const floa
       widest = std::max(widest, (long long)lo.out * (lo.in + 1 + nx.out));
     }
   };
+  const CriticPass& Q = h->pass[PASS_Q];
   layers(L.actor, La, h->hA, 0, 0);
-  layers(L.q[0], Lc, h->hQ, 0, 1);
-  layers(L.q[1], Lc, h->hQ, 1, 1);
+  layers(Q.net[0], Lc, Q.h, 0, 1);
+  layers(Q.net[1], Lc, Q.h, 1, 1);
 
   CU(cudaSetDevice(h->device));
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   cudaStream_t st = sb.run;
   const int obs_w = h->K.obs, ldx = h->K.ldx;
-  const Buf XA = rep_view(h->XA, replica), XQ = rep_view(h->XQ, replica);
+  const Buf XA = rep_view(h->XA, replica), XQ = rep_view(*Q.X, replica);
   if (c.care) {
     CU(cudaMemcpyAsync(rep_view(h->XS, replica).p, obs, (size_t)n * obs_w * sizeof(float), cudaMemcpyDefault, st));
     if (int rc = care_encode_rows(h, st, replica, n, XQ, ldx)) return rc;
@@ -3454,9 +3451,9 @@ extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const floa
   for (int l = 0; l < Lc; ++l) {           // q1 and q2 in one launch: equal shapes
     std::vector<GemmProb> ps;
     for (int net = 0; net < 2; ++net) {
-      const LayerOff& lo = L.q[net][l];
-      const float* X = l == 0 ? XQ.p : rep_view(h->hQ[l - 1], replica).p + (long long)net * B * lo.in;
-      ps.push_back(fwd_prob(par, X, 0, n, lo, rep_view(h->hQ[l], replica).p + (long long)net * B * lo.out, 0));
+      const LayerOff& lo = Q.net[net][l];
+      const float* X = l == 0 ? XQ.p : rep_view(Q.h[l - 1], replica).p + (long long)net * B * lo.in;
+      ps.push_back(fwd_prob(par, X, 0, n, lo, rep_view(Q.h[l], replica).p + (long long)net * B * lo.out, 0));
     }
     act_gemm(ps, st);
   }
@@ -3556,44 +3553,44 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
     src = reinterpret_cast<const float*>(h->chain_dbg.get()); n = 2 * CH_DBG_SLOTS * 16;     // int64 stamps viewed as float pairs
   }
   else {
-    // hidden activations (the ReLU masks of the step): "hA.<l>" [2B][H] rows [s';s]; "hQ.<l>" / "hT.<l>" / "hP.<l>" [2][B][H]
-    // (critic update pass / target pass -- not kept by the layer-chained plan -- / actor pass); critic_ln handles
-    // "zQ.<l>" / "zT.<l>" / "zP.<l>" [2][B][H], the same passes' pre-normalization activations (critic_dropout: after the
-    // dropout), critic_dropout handles "mQ.<l>" / "mT.<l>" / "mP.<l>" their keep masks; CARE mixture encoders
-    // "mixH.<inst>.<l>" [K][rows][pitch4(H)], inst 0 = critic's on [s';s] (rows 2B), 1 = target's on s', 2 = updated critic's on s
+    // hidden activations (the ReLU masks of the step): "hA.<l>" [2B][H] rows [s';s]; per critic pass (letter Q, T or P)
+    // "h<pass>.<l>" [2][B][H] (the target pass's are not kept by the layer-chained plan), on critic_ln handles
+    // "z<pass>.<l>", the pre-normalization activations (critic_dropout: after the dropout), on critic_dropout handles
+    // "m<pass>.<l>", the keep masks as 0.0 / 1.0; CARE mixture encoders "mixH.<inst>.<l>" [K][rows][pitch4(H)], inst 0 =
+    // critic's on [s';s] (rows 2B), 1 = target's on s', 2 = updated critic's on s
     int l = -1, inst = -1;
-    char kind[8] = "";
+    char kind[2] = "", letter[2] = "";
     const Buf* b = nullptr;
     if (sscanf(name, "mixH.%d.%d", &inst, &l) == 2) {
       if (!h->cfg.care || inst < 0 || inst > 2 || l < 0 || l >= (int)h->mixH[inst].size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
       b = &h->mixH[inst][l];
       const int rows = inst == 0 ? 2 * B : B, pw = (h->cfg.mix_hidden[l] + 3) & ~3;
       n = (int64_t)h->cfg.num_encoders * rows * pw;
-    } else if (sscanf(name, "h%1[AQTP].%d", kind, &l) == 2) {
-      const std::vector<Buf>& v = kind[0] == 'A' ? h->hA : (kind[0] == 'Q' ? h->hQ : (kind[0] == 'T' ? h->hT : h->hP));
+    } else if (sscanf(name, "hA.%d", &l) == 1) {
+      if (l < 0 || l >= (int)h->hA.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
+      b = &h->hA[l];
+      n = (int64_t)2 * B * h->cfg.actor_hidden[l];
+    } else if (sscanf(name, "%1[hzm]%1[QTP].%d", kind, letter, &l) == 3) {
+      const CriticPass* cp = nullptr;
+      for (const CriticPass& p : h->pass)
+        if (p.letter == letter[0]) cp = &p;
+      const std::vector<Buf>& v = kind[0] == 'h' ? cp->h : (kind[0] == 'z' ? cp->z : cp->m);
       if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
-      b = &v[l];
-      n = (int64_t)2 * B * (kind[0] == 'A' ? h->cfg.actor_hidden[l] : h->cfg.critic_hidden[l]);
-    } else if (sscanf(name, "z%1[QTP].%d", kind, &l) == 2) {
-      const std::vector<Buf>& v = kind[0] == 'Q' ? h->zQ : (kind[0] == 'T' ? h->zT : h->zP);
-      if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
-      b = &v[l];
-      n = (int64_t)2 * B * h->cfg.critic_hidden[l];
-    } else if (sscanf(name, "m%1[QTP].%d", kind, &l) == 2) {
-      // critic_dropout: the keep masks of the passes as 0.0 / 1.0, expanded from their bits
-      const std::vector<Buf>& v = h->dmask[kind[0] == 'Q' ? 0 : (kind[0] == 'T' ? 1 : 2)];
-      if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
-      const int H = h->cfg.critic_hidden[l], words = (H + 31) / 32;
+      const int H = h->cfg.critic_hidden[l];
       n = (int64_t)2 * B * H;
-      if (n_floats) *n_floats = n;
-      if (cap_floats < n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld floats", (long long)n);
-      std::vector<uint32_t> bits((size_t)2 * B * words);
-      CU(cudaMemcpyAsync(bits.data(), v[l].p + replica * v[l].rs, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost,
-                         (cudaStream_t)stream));
-      CU(cudaStreamSynchronize((cudaStream_t)stream));
-      for (int64_t row = 0; row < 2 * B; ++row)
-        for (int j = 0; j < H; ++j) out_host[row * H + j] = (float)((bits[row * words + j / 32] >> (j % 32)) & 1u);
-      return 0;
+      if (kind[0] == 'm') {
+        if (n_floats) *n_floats = n;
+        if (cap_floats < n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld floats", (long long)n);
+        const int words = (H + 31) / 32;
+        std::vector<uint32_t> bits((size_t)2 * B * words);
+        CU(cudaMemcpyAsync(bits.data(), v[l].p + replica * v[l].rs, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost,
+                           (cudaStream_t)stream));
+        CU(cudaStreamSynchronize((cudaStream_t)stream));
+        for (int64_t row = 0; row < 2 * B; ++row)
+          for (int j = 0; j < H; ++j) out_host[row * H + j] = (float)((bits[row * words + j / 32] >> (j % 32)) & 1u);
+        return 0;
+      }
+      b = &v[l];
     } else {
       return fail(B200SAC_ERR_INVALID, "unknown debug tensor '%s'", name);
     }
