@@ -101,6 +101,8 @@ SYMBOLS = {
     "b200sac_soft_update": (C.c_int, [_VP, C.c_double, _VP]),
     "b200sac_soft_update_critic": (C.c_int, [_VP, C.c_int32, C.c_double, _VP]),
     "b200sac_act": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP, _VP, C.c_int32, _VP, _VP]),
+    "b200sac_critic_values": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, _VP, C.c_int32, _VP, _VP]),
+    "b200sac_critic_values_chunk": (C.c_int, [_VP, C.POINTER(C.c_int64)]),
     "b200sac_blob_template": (C.c_int, [_VP, C.c_int32, _VP, C.c_int64, C.c_int64, _VP, _VP]),
     "b200sac_blob_begin": (C.c_int, [_VP, _VP]),
     "b200sac_blob_wait": (C.c_int, [_VP, C.POINTER(_VP), C.POINTER(C.c_int64)]),
@@ -129,6 +131,7 @@ SYMBOLS = {
     "b200sac_replay_get_nstep": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32)]),
     "b200sac_replay_get_links": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int64, _VP]),
     "b200sac_replay_fold": (C.c_int, [_VP, C.c_int32, C.c_int64] + [_VP] * 8),
+    "b200sac_replay_refresh_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, C.c_uint64, C.c_int32, _VP]),
 }
 
 _lib = None

@@ -267,6 +267,29 @@ class SacCore:
         _lib.check(self.lib.b200sac_act(self._h, replica, n, _ptr(obs), _ptr(e), 1 if stochastic else (-1 if no_tanh else 0), _ptr(out), _stream()))
         return out
 
+    def critic_values(self, obs, act, target=False, replica=0):
+        """(q1, q2) of one replica on n >= 1 rows obs [n][obs_dim] and act [n][act_dim] (CPU or CUDA tensors), or of
+        q1_target and q2_target with target=True: two [n] tensors on the device obs is on.  Eval mode (no dropout), any n,
+        every row's values independent of the others (b200sac_critic_values).  Synchronises the current stream."""
+        if not isinstance(target, (bool, np.bool_)):
+            raise ValueError(f"target must be a bool, got {target!r}")
+        obs = torch.as_tensor(obs).to(torch.float32).contiguous()
+        act = torch.as_tensor(act).to(obs.device, torch.float32).contiguous()
+        n = obs.shape[0] if obs.dim() == 2 else 0
+        if n < 1 or obs.shape != (n, self.cfg.obs_dim) or act.shape != (n, self.cfg.act_dim):
+            raise ValueError(f"obs must be [n][{self.cfg.obs_dim}] and act [n][{self.cfg.act_dim}] with n >= 1, got "
+                             f"{tuple(obs.shape)} and {tuple(act.shape)}")
+        out = torch.empty(2, n, device=obs.device)
+        _lib.check(self.lib.b200sac_critic_values(self._h, int(replica), n, _ptr(obs), _ptr(act), 1 if target else 0, _ptr(out),
+                                                  _stream()))
+        return out[0], out[1]
+
+    def critic_values_chunk(self) -> int:
+        """Rows critic_values and Replay.refresh_priorities evaluate per launch sequence (their scratch holds that many)."""
+        n = C.c_int64(0)
+        _lib.check(self.lib.b200sac_critic_values_chunk(self._h, C.byref(n)))
+        return n.value
+
     def read_named(self, name, which=_lib.PARAMS, replica=0) -> torch.Tensor:
         """One small tensor (e.g. log_alpha) straight from the device: a few floats cross PCIe, not the arena."""
         off, rows, cols, _t, _o, pitch = self.table[name]
@@ -792,6 +815,24 @@ class Replay:
         _lib.check(self.lib.b200sac_replay_sample_prioritized(self._h, int(replica), _ptr(s), _ptr(a), _ptr(r), _ptr(s2), _ptr(d),
                                                               _ptr(idx), _ptr(w)))
         return s, a, r, s2, d, idx, w
+
+    def refresh_priorities(self, seed, idx=None, replica=None, stochastic=True):
+        """Recompute priorities with the current networks (b200sac_replay_refresh_priorities): the filled slots `idx` of one
+        replica, or with idx=None every filled slot of every task; replica=None means every replica and needs idx=None (slot
+        lists are per replica).  stochastic=False evaluates the TD target at the policy's mean action; True draws the next
+        action's noise keyed by (seed, replica, slot).  Synchronous; sees every reset and recycle enqueued before it."""
+        if idx is not None and replica is None:
+            raise ValueError("refresh_priorities with idx= needs replica= (slot lists are per replica)")
+        if not isinstance(stochastic, (bool, np.bool_)):
+            raise ValueError(f"stochastic must be a bool, got {stochastic!r}")
+        if idx is not None:
+            idx = np.ascontiguousarray(np.asarray(idx, dtype=np.int64).reshape(-1))
+        for r in _replicas(self.core.cfg.replicas, replica):
+            n, p = (0, C.c_void_p(0)) if idx is None else (idx.size, C.c_void_p(idx.ctypes.data))
+            if idx is not None and n == 0:
+                continue
+            _lib.check(self.lib.b200sac_replay_refresh_priorities(self._h, int(r), n, p, C.c_uint64(int(seed) % (1 << 64)),
+                                                                  1 if stochastic else 0, _stream()))
 
     # ---- n-step returns (ring with trajectory links) ---------------------------------------------
     def set_nstep(self, n: int, replica=None):

@@ -38,6 +38,7 @@
 #include "pcgrad_kernels.cuh"
 #include "redo_kernels.cuh"
 #include "ln_kernels.cuh"
+#include "eval_kernels.cuh"
 
 using namespace bsac;
 
@@ -437,6 +438,26 @@ struct CriticPass {
   std::vector<Buf> h, z, m;
 };
 
+// The evaluation scratch of b200sac_critic_values and b200sac_replay_refresh_priorities: one replica's rows, `rows` at a
+// time, in an allocation of its own (at most kEvalScratchBytes, made by the first call), so that the step's slab and
+// everything the next step reads stay untouched.  Each buffer holds `rows` rows:
+//   XQ, XT [ldx]      critic inputs (s | a) and (s' | a')
+//   hc[2] [2][Hc]     critic hidden activations, layer l in hc[l % 2]; z [2][Hc] pre-normalization (critic_ln)
+//   ha[2] [Ha]        actor hidden activations, layer l in ha[l % 2]
+//   q, qt [2]         q1 / q2 and their targets (row i of q1, then row i of q2)
+//   pout [2A], psave [A][kSaveW], act [A], logp, logstd, eps [A]   the policy head's outputs and noise
+//   R, d, g, task, idx                                             the refresh's folded rows and ring slots
+// plus tmax [T] and tasks [T] for the refresh's per-task bookkeeping.
+constexpr size_t kEvalScratchBytes = 64ull << 20;
+struct EvalScratch {
+  DevMem<float> mem;
+  long long rows = 0;
+  float *XQ, *XT, *hc[2], *z, *ha[2], *q, *qt, *pout, *psave, *act, *logp, *logstd, *eps, *R, *d, *g;
+  int *task, *tasks;
+  long long* idx;
+  unsigned* tmax;
+};
+
 struct b200sac {
   b200sac_cfg cfg;
   EnvSwitches env;                // read at create
@@ -553,6 +574,7 @@ struct b200sac {
   ReplicaTable<double, 2> cg_c;
   DevMem<double> cg_p, cg_f;
   DevMem<int> cg_it;
+  EvalScratch ev;                 // b200sac_critic_values / b200sac_replay_refresh_priorities (allocated by the first call)
 
   // The members release their resources; the publication stream's last copy lands first.
   ~b200sac() {
@@ -3480,6 +3502,129 @@ extern "C" int b200sac_read_redo(b200sac_t* h, int32_t replica, double* scores, 
   return 0;
 }
 
+// ------------------------------------------------------------------------------------------
+// Critic evaluation outside the step (eval_kernels.cuh): b200sac_critic_values and the priority refresh
+// ------------------------------------------------------------------------------------------
+// The evaluation scratch's buffers in carving order: the pointer each sets and its floats per row.  With n = 0 nothing
+// is set and the sum is the floats of one row, alignment padding excluded.
+static long long eval_carve(const b200sac* h, long long n, float* base) {
+  const b200sac_cfg& c = h->cfg;
+  const int A = c.act_dim, T = h->K.T > 0 ? h->K.T : 1;
+  int Hc = 0, Ha = 0;
+  for (int l = 0; l < c.n_critic_hidden; ++l) Hc = std::max(Hc, c.critic_hidden[l]);
+  for (int l = 0; l < c.n_actor_hidden; ++l) Ha = std::max(Ha, c.actor_hidden[l]);
+  EvalScratch& E = const_cast<b200sac*>(h)->ev;
+  const std::pair<void**, long long> rowbufs[] = {
+      {(void**)&E.XQ, h->K.ldx}, {(void**)&E.XT, h->K.ldx}, {(void**)&E.hc[0], 2 * Hc}, {(void**)&E.hc[1], 2 * Hc},
+      {(void**)&E.z, c.critic_ln ? 2 * Hc : 0}, {(void**)&E.ha[0], Ha}, {(void**)&E.ha[1], Ha}, {(void**)&E.q, 2},
+      {(void**)&E.qt, 2}, {(void**)&E.pout, 2 * A}, {(void**)&E.psave, A * kSaveW}, {(void**)&E.act, A},
+      {(void**)&E.logp, 1}, {(void**)&E.logstd, 1}, {(void**)&E.eps, A}, {(void**)&E.R, 1}, {(void**)&E.d, 1},
+      {(void**)&E.g, 1}, {(void**)&E.task, 1}, {(void**)&E.idx, 2}};
+  if (n == 0) {
+    long long w = 0;
+    for (const auto& b : rowbufs) w += b.second;
+    return w;
+  }
+  long long off = 0;
+  auto take = [&](void** p, long long floats) {     // every buffer starts 256-byte aligned
+    if (base) *p = base + off;
+    off += (floats + 63) / 64 * 64;
+  };
+  for (const auto& b : rowbufs) take(b.first, n * b.second);
+  take((void**)&E.tmax, T);
+  take((void**)&E.tasks, T);
+  return off;
+}
+
+// Rows per chunk: as many as fit kEvalScratchBytes, a multiple of 32, at most 65536 (the GEMM grid's row dimension).
+static long long eval_rows(const b200sac* h) {
+  const long long slack = 64 * 24 + 2 * (h->K.T + 64);    // alignment padding and the per-task buffers
+  const long long n = ((long long)(kEvalScratchBytes / sizeof(float)) - slack) / eval_carve(h, 0, nullptr) / 32 * 32;
+  return std::min<long long>(65536, n);
+}
+
+static int eval_alloc(b200sac* h) {
+  EvalScratch& E = h->ev;
+  if (E.mem) return 0;
+  const long long n = eval_rows(h);
+  const long long floats = eval_carve(h, n, nullptr);
+  DevMem<float> mem;
+  CU(cudaMalloc(mem.put(), (size_t)floats * sizeof(float)));
+  CU(cudaMemset(mem, 0, (size_t)floats * sizeof(float)));
+  eval_carve(h, n, mem);
+  E.rows = n;
+  E.mem = std::move(mem);
+  return 0;
+}
+
+// Q of nets[0] and nets[1] (L.q: q1 and q2; L.qt: their targets) of replica `rep` on n <= E.rows rows X [n][ldx] into
+// out [2][n], in eval mode: b200sac_act's per-layer gemm_simt_kernel and, on critic_ln handles, ln_fwd_kernel<false> between
+// each hidden GEMM and its ReLU (no dropout, whatever the replica's rate).  Each output row depends on its input row alone.
+static void eval_critics(b200sac* h, cudaStream_t st, int rep, const std::vector<LayerOff>* nets, const float* X, int n, float* out) {
+  const EvalScratch& E = h->ev;
+  const Buf par = rep_view(Buf{h->params, h->L.arena}, rep);
+  const int Lc = h->cfg.n_critic_hidden;
+  const bool ln = h->cfg.critic_ln != 0;
+  for (int l = 0; l <= Lc; ++l) {
+    std::vector<GemmProb> ps;
+    for (int net = 0; net < 2; ++net) {
+      const LayerOff& lo = nets[net][l];
+      const float* in = l == 0 ? X : E.hc[(l - 1) & 1] + (long long)net * n * lo.in;
+      float* o = l == Lc ? out + (long long)net * n : (ln ? E.z : E.hc[l & 1]) + (long long)net * n * lo.out;
+      GemmProb p = fwd_prob(par, in, 0, n, lo, o, 0);
+      if (l == 0) p.lda = h->K.ldx;
+      p.relu = l < Lc && !ln;
+      ps.push_back(p);
+    }
+    act_gemm(ps, st);
+    if (ln && l < Lc) {
+      LnArgs P;
+      memset(&P, 0, sizeof(P));
+      P.z = E.z; P.h = E.hc[l & 1];
+      for (int net = 0; net < 2; ++net) { P.g[net] = par.p + nets[net][l].g; P.c[net] = par.p + nets[net][l].c; }
+      P.B = n; P.H = nets[0][l].out;
+      ln_fwd_kernel<false><<<dim3((2 * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, P);
+    }
+  }
+}
+
+extern "C" int b200sac_critic_values_chunk(b200sac_t* h, int64_t* rows) {
+  if (!h || !rows) return fail(B200SAC_ERR_INVALID, "null argument");
+  *rows = eval_rows(h);
+  return 0;
+}
+
+extern "C" int b200sac_critic_values(b200sac_t* h, int32_t replica, int64_t n, const float* obs, const float* act, int32_t which,
+                                     float* q_out, void* stream) {
+  if (!h || !obs || !act || !q_out) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (n < 1) return fail(B200SAC_ERR_INVALID, "n must be >= 1, got %lld", (long long)n);
+  if (which != 0 && which != 1) return fail(B200SAC_ERR_INVALID, "which must be 0 (q1, q2) or 1 (their targets), got %d", which);
+  if (h->cfg.care) return fail(B200SAC_ERR_STATE, "critic_values does not run on a CARE handle");
+  CU(cudaSetDevice(h->device));
+  if (int rc = eval_alloc(h)) return rc;
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  cudaStream_t st = sb.run;
+  const EvalScratch& E = h->ev;
+  const int obs_w = h->K.obs, A = h->K.act;
+  const size_t ldx = (size_t)h->K.ldx * sizeof(float);
+  for (int64_t i0 = 0; i0 < n; i0 += E.rows) {
+    const int m = (int)std::min<int64_t>(E.rows, n - i0);
+    CU(cudaMemcpy2DAsync(E.XQ, ldx, obs + i0 * obs_w, (size_t)obs_w * sizeof(float), (size_t)obs_w * sizeof(float), (size_t)m,
+                         cudaMemcpyDefault, st));
+    CU(cudaMemcpy2DAsync(E.XQ + h->K.in_w, ldx, act + i0 * A, (size_t)A * sizeof(float), (size_t)A * sizeof(float), (size_t)m,
+                         cudaMemcpyDefault, st));
+    eval_critics(h, st, replica, which ? h->L.qt : h->L.q, E.XQ, m, E.q);
+    CU(cudaGetLastError());
+    for (int net = 0; net < 2; ++net)
+      CU(cudaMemcpyAsync(q_out + net * n + i0, E.q + (long long)net * m, (size_t)m * sizeof(float), cudaMemcpyDefault, st));
+  }
+  if (int rc = sb.end()) return rc;
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
+  return 0;
+}
+
 extern "C" int b200sac_soft_update(b200sac_t* h, double tau, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
   CU(cudaSetDevice(h->device));
@@ -4284,5 +4429,108 @@ extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_
     CU(cudaStreamSynchronize(rb->st));
     unpack_rows(h, rows.data(), c, f, i0);
   }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// priority refresh (eval_kernels.cuh): a prioritized ring's leaves re-scored by the replica's current networks
+// ------------------------------------------------------------------------------------------
+extern "C" int b200sac_replay_refresh_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, uint64_t seed,
+                                                 int32_t stochastic, void* stream) {
+  if (int rc = ring_check(rb, replica, RING_PER)) return rc;
+  b200sac* h = rb->h;
+  if (h->cfg.care) return fail(B200SAC_ERR_STATE, "the priority refresh does not run on a CARE handle");
+  if (n < 0 || (n > 0 && !idx)) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (stochastic != 0 && stochastic != 1) return fail(B200SAC_ERR_INVALID, "stochastic must be 0 or 1, got %d", stochastic);
+  CU(cudaSetDevice(h->device));
+  std::lock_guard<std::mutex> lk(rb->mu);
+  const long long cpt = rb->cap_per_task;
+  const int T = rb->Teff;
+  const bool full = idx == nullptr;
+  std::vector<long long> slots;          // the slots to refresh: every filled one, or the caller's
+  std::vector<char> touched((size_t)T, 0);
+  if (full) {
+    for (int t = 0; t < T; ++t) {
+      const long long f = rb->fill[(size_t)replica * T + t];
+      touched[(size_t)t] = f > 0;
+      for (long long k = 0; k < f; ++k) slots.push_back(t * cpt + k);
+    }
+  } else {
+    slots.resize((size_t)n);
+    for (int64_t i = 0; i < n; ++i) {
+      if (int rc = filled_slot(rb, replica, idx[i])) return rc;
+      slots[(size_t)i] = idx[i];
+      touched[(size_t)(idx[i] / cpt)] = 1;
+    }
+  }
+  std::vector<int> tasks;
+  for (int t = 0; t < T; ++t)
+    if (touched[(size_t)t]) tasks.push_back(t);
+  if (tasks.empty()) return 0;
+  if (int rc = eval_alloc(h)) return rc;
+  if (int rc = ring_quiesce(rb)) return rc;
+  StreamBridge sb(h, stream);
+  if (int rc = sb.begin()) return rc;
+  cudaStream_t st = sb.run;
+  if (rb->traj) CU(cudaStreamWaitEvent(st, rb->ev_nstep, 0));
+  const EvalScratch& E = h->ev;
+  const Layout& L = h->L;
+  const int La = h->cfg.n_actor_hidden;
+  const Buf par = rep_view(Buf{h->params, L.arena}, replica);
+  CU(cudaMemcpyAsync(E.tasks, tasks.data(), tasks.size() * sizeof(int), cudaMemcpyHostToDevice, st));
+  CU(cudaMemsetAsync(E.tmax, 0, (size_t)T * sizeof(unsigned), st));
+
+  RefreshGather G;
+  memset(&G, 0, sizeof(G));
+  G.rows = rb->rows + (size_t)replica * rb->rs_rows;
+  if (rb->traj) { G.link = rb->d_link + (size_t)replica * rb->cap; G.nstep = rb->nstep.dev; }
+  G.hp = h->hp.dev; G.idx = E.idx; G.XQ = E.XQ; G.XT = E.XT;
+  G.R = E.R; G.d = E.d; G.g = E.g; G.eps = E.eps; G.task = E.task;
+  G.key = seed ^ (kRefreshKeyMul * (unsigned long long)(replica + 1));
+  G.row_stride = h->row_stride; G.obs = h->K.obs; G.act = h->K.act; G.ldx = h->K.ldx; G.cap_per_task = (int)cpt;
+  G.rep = replica; G.stochastic = stochastic;
+  PolicyHeadArgs P;                      // one replica's head over the chunk's rows; every row is below K.B, so a' lands in XT
+  memset(&P, 0, sizeof(P));
+  const LayerOff& head = L.actor[La];
+  P.h = E.ha[(La - 1) & 1]; P.ldh = head.in;
+  P.W = par.p + head.w; P.b = par.p + head.b;
+  P.eps = E.eps; P.use_eps_buf = 1;
+  P.pout = E.pout; P.psave = E.psave; P.XT = E.XT; P.XP = E.XT; P.act_out = E.act; P.logp = E.logp; P.logstd_sum = E.logstd;
+  P.cnt = h->cnt;
+  StepConst K = h->K;
+  K.B = (int)E.rows;
+  RefreshTd D;
+  memset(&D, 0, sizeof(D));
+  D.Tr = rb->tr; D.idx = E.idx; D.R = E.R; D.d = E.d; D.g = E.g; D.task = E.task; D.logp = E.logp; D.q = E.q; D.qt = E.qt;
+  D.log_alpha = par.p + L.off_alpha; D.hp = h->hp.dev; D.tmax = E.tmax; D.rep = replica;
+
+  const long long total = (long long)slots.size();
+  for (long long i0 = 0; i0 < total; i0 += E.rows) {
+    const int m = (int)std::min<long long>(E.rows, total - i0);
+    CU(cudaMemcpyAsync(E.idx, slots.data() + i0, (size_t)m * sizeof(long long), cudaMemcpyHostToDevice, st));
+    G.n = m;
+    refresh_gather_kernel<<<(m + 7) / 8, 256, 0, st>>>(G);
+    for (int l = 0; l < La; ++l) {
+      GemmProb p = fwd_prob(par, l == 0 ? E.XT : E.ha[(l - 1) & 1], 0, m, L.actor[l], E.ha[l & 1], 0);
+      if (l == 0) p.lda = h->K.ldx;
+      act_gemm({p}, st);
+    }
+    P.rows = m;
+    policy_head_kernel<<<dim3((m + 7) / 8, 1), 256, 0, st>>>(K, P);
+    eval_critics(h, st, replica, L.qt, E.XT, m, E.qt);
+    eval_critics(h, st, replica, L.q, E.XQ, m, E.q);
+    D.n = m;
+    refresh_td_kernel<<<(m + 255) / 256, 256, 0, st>>>(D);
+    CU(cudaGetLastError());
+  }
+  for (int lv = 1; lv <= rb->tr.levels; ++lv) {
+    const long long nodes = rb->tr.P >> lv;
+    per_rebuild_level_kernel<<<dim3((unsigned)std::min<long long>(1024, (nodes + 255) / 256), (unsigned)tasks.size()), 256, 0, st>>>(
+        rb->tr, replica, E.tasks, lv);
+  }
+  refresh_maxp_kernel<<<1, 256, 0, st>>>(rb->tr, replica, E.tasks, (int)tasks.size(), E.tmax, full ? 1 : 0);
+  CU(cudaGetLastError());
+  if (int rc = sb.end()) return rc;
+  CU(cudaStreamSynchronize((cudaStream_t)stream));
   return 0;
 }

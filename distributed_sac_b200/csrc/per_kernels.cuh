@@ -99,6 +99,10 @@ __global__ void __launch_bounds__(512) per_sample_kernel(StepConst K, PerTree Tr
 }
 
 B200_D float per_leaf_value(const PerTree& Tr, double prio) { return (float)pow(prio + Tr.eps, Tr.alpha); }
+// a row's priority from its TD target and both critics' values, in fp64
+B200_D double td_priority(float y, float q1, float q2) {
+  return 0.5 * (fabs((double)y - (double)q1) + fabs((double)y - (double)q2));
+}
 
 // One CTA per replica (rep = rep0 + blockIdx.x): n <= kPerMaxB priorities for the ring indices idx[0..n), either the raw
 // values prio_in[i] or, when prio_in is null, the step's (|y - Q1| + |y - Q2|) / 2 (n = B, q = [2][B]).  Writes the leaves
@@ -132,7 +136,7 @@ __global__ void __launch_bounds__(512) per_update_kernel(PerTree Tr, int rep0, c
     } else {
       const float yv = (y + (long long)rep * rsY)[i];
       const float* Q = q + (long long)rep * 2 * rsY;
-      prio = 0.5 * (fabs((double)yv - (double)Q[i]) + fabs((double)yv - (double)Q[n + i]));
+      prio = td_priority(yv, Q[i], Q[n + i]);
     }
     pv[k] = per_leaf_value(Tr, prio);
     unsigned hsh = ((unsigned)key[k] * 2654435761u) % (unsigned)kHash;

@@ -100,6 +100,17 @@ class _BaseLearner:
         self.critic_dropout = None if critic_dropout is None else float(critic_dropout)
         if prioritized is not None and replay_where != "device":
             raise ValueError("prioritized replay needs replay_where='device' (the sum-trees live beside the device ring)")
+        # prioritized=dict(..., refresh_after_reset=True): every reset and recycle is followed by a full priority refresh of
+        # every replica under that reset's or recycle's seed, so the sampler does not follow the discarded network's errors
+        self.refresh_after_reset = False
+        if prioritized is not None:
+            prioritized = dict(prioritized)
+            self.refresh_after_reset = prioritized.pop("refresh_after_reset", False)
+            if not isinstance(self.refresh_after_reset, (bool, np.bool_)):
+                raise ValueError(f"refresh_after_reset must be a bool (got {self.refresh_after_reset!r})")
+            self.refresh_after_reset = bool(self.refresh_after_reset)
+            if self.refresh_after_reset and not self._critic_ln_ok:
+                raise ValueError(f"refresh_after_reset=True needs plain-MLP critics ({type(self).__name__} has CARE critics)")
         self.prioritized = prioritized
         if not 1 <= int(n_step) <= 16:
             raise ValueError(f"n_step must be in [1, 16] (got {n_step})")
@@ -160,6 +171,7 @@ class _BaseLearner:
         self._n_updates = 0
         self._n_manual_resets = 0
         self._n_manual_redos = 0
+        self._n_manual_refreshes = 0
         self.device = torch.device(self.cfg.get("device", "cuda"))
         if self.device.type != "cuda":
             raise RuntimeError("the CUDA learner only runs on CUDA devices (cfg 'device' must be 'cuda')")
@@ -247,9 +259,13 @@ class _BaseLearner:
         while n > 0:
             u = self._n_updates
             if u > 0 and self.reset_interval is not None and u % self.reset_interval == 0:
-                self.core.reset(self.seed + (u // self.reset_interval) * 2 ** 32, **self.reset)
+                seed = self.seed + (u // self.reset_interval) * 2 ** 32
+                self.core.reset(seed, **self.reset)
+                self._refresh_after(seed)
             if u > 0 and self.redo_interval is not None and u % self.redo_interval == 0:
-                self._recycle(self.seed + 2 ** 62 + (u // self.redo_interval) * 2 ** 32, self.redo)
+                seed = self.seed + 2 ** 62 + (u // self.redo_interval) * 2 ** 32
+                self._recycle(seed, self.redo)
+                self._refresh_after(seed)
             c = min([n] + [N - u % N for N in Ns])
             yield c
             self._n_updates += c
@@ -279,6 +295,7 @@ class _BaseLearner:
             self._n_manual_resets += 1
             seed = self.seed + 2 ** 63 + self._n_manual_resets * 2 ** 32
         self.core.reset(seed, **parts)
+        self._refresh_after(seed)
 
     def recycle_dormant(self, seed=None, **taus):
         """Recycle dormant neurons now, on the current stream, scored on a fresh replay batch: actor= / critic= thresholds
@@ -289,6 +306,30 @@ class _BaseLearner:
             self._n_manual_redos += 1
             seed = self.seed + 2 ** 63 + 2 ** 62 + self._n_manual_redos * 2 ** 32
         self._recycle(seed, taus)
+        self._refresh_after(seed)
+
+    def _refresh_after(self, seed):
+        """With refresh_after_reset: a full priority refresh of every replica right after a reset or recycle, same seed."""
+        if self.refresh_after_reset:
+            self.memory.ring.refresh_priorities(seed)
+
+    def refresh_priorities(self, seed=None):
+        """Recompute every filled slot's priority with the current networks now (Replay.refresh_priorities, stochastic next
+        actions).  seed=None: the j-th such call uses seed + 2^63 + 2^61 + j * 2^32.  The learner must have been built with
+        prioritized=."""
+        if self.prioritized is None:
+            raise ValueError("this learner was built without prioritized=")
+        if seed is None:
+            self._n_manual_refreshes += 1
+            seed = self.seed + 2 ** 63 + 2 ** 61 + self._n_manual_refreshes * 2 ** 32
+        self.memory.ring.refresh_priorities(seed)
+
+    def q_values(self, states, actions, target=False):
+        """(q1, q2), or their targets with target=True, on rows of states and actions: two (n, 1) tensors on the learner's
+        device, as Critic.forward returns them, in eval mode (no dropout)."""
+        q1, q2 = self.core.critic_values(torch.as_tensor(states).to(self.device), torch.as_tensor(actions).to(self.device),
+                                         target=target)
+        return q1.reshape(-1, 1), q2.reshape(-1, 1)
 
     def dormant_fraction(self, tau=0.0):
         """The fraction of tau-dormant neurons (score <= tau) per network and hidden layer on a fresh replay batch: a

@@ -46,6 +46,10 @@
  *                            the byte string, device-assembled
  *   b200sac_act              Actor.get_action() for a batch of environments
  *                            LunarLander_Distributed_SAC/src/model.py:67-82; MT10_Distributed_CARE/src/player.py:199-209 (CARE handles)
+ *   b200sac_critic_values    Critic.forward() (q1, q2 or their targets) for any number of rows, in eval mode
+ *                            LunarLander_Distributed_SAC/src/model.py (Critic); not on CARE handles
+ *   b200sac_replay_refresh_priorities
+ *                            PER priorities of a ring's slots recomputed with the current networks (after resets, ReDo)
  *
  * Conventions: plain pointers and sizes only (no torch types).  Every function
  * returns 0 on success or a negative b200sac_status; a message for the calling
@@ -175,7 +179,8 @@ typedef struct b200sac_cfg {
  * Plan: the same launches and labels as the critic_ln plan; the LayerNorm launches draw, apply and keep the masks (bits
  * [2][batch][ceil(H / 32)] per replica, pass and layer; column j is bit j % 32 of word j / 32).  No parameters: the layout
  * is that of the same cfg with critic_dropout = 0.  The rate is not copied by b200sac_copy_replica and not part of the
- * parameter arenas.  No inference path runs the critics, so there is no evaluation mode.
+ * parameter arenas.  b200sac_critic_values and b200sac_replay_refresh_priorities evaluate the critics in eval mode: no
+ * dropout, whatever the rate.
  * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_dropout outside {0, 1}, or 1 with
  * critic_ln = 0. */
 
@@ -529,6 +534,28 @@ int b200sac_soft_update_critic(b200sac_t* h, int32_t critic, double tau, void* s
 int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* eps, int32_t stochastic,
                 float* actions_out, void* stream);
 
+/* Critic inference: Q1 and Q2 of replica `replica` on n >= 1 rows obs[n][state_dim + num_tasks] and act[n][act_dim] (host
+ * or device memory).  which = 0: q1 and q2; which = 1: q1_target and q2_target.  q_out[2][n] (host or device): row i of
+ * q1 at q_out[i], row i of q2 at q_out[n + i] -- Critic.forward (LunarLander_Distributed_SAC/src/model.py) vectorised over
+ * rows, e.g. for Q against Monte-Carlo returns (overestimation bias) or for priorities of fresh rows.
+ *   Engine: b200sac_act's per-layer fp32 FFMA engine, whatever the handle's plan or precision.  critic_ln handles apply
+ *     the LayerNorm forward with the numerics of "Layer-normalized critics" (the step's own row routine).  Eval mode, as
+ *     torch's .eval(): no dropout, whatever the replica's critic_dropout rate, so a rate of 0.5 gives the values of 0.
+ *   Chunk independence: row i's values depend only on the parameters and row i -- bit-identical whatever n is, wherever
+ *     the row sits in the call and whatever the handle's replica count.
+ *   Scratch: the rows are evaluated b200sac_critic_values_chunk rows at a time in an evaluation scratch of the handle's
+ *     own (at most 64 MiB, allocated by the first call of this function or of b200sac_replay_refresh_priorities; a handle
+ *     that calls neither pays nothing).  The step's buffers are not touched: the next step is bit-identical whether or
+ *     not this call ran in between.
+ *   Stream order and synchronisation as b200sac_act: it sees every reset, recycle and step enqueued before it.
+ * A bad replica, n < 1, a NULL pointer or which outside {0, 1} give B200SAC_ERR_INVALID; a CARE handle gives
+ * B200SAC_ERR_STATE (no per-task encoding of arbitrary rows yet). */
+int b200sac_critic_values(b200sac_t* h, int32_t replica, int64_t n, const float* obs, const float* act, int32_t which,
+                          float* q_out, void* stream);
+/* Rows per chunk of the evaluation scratch (pure host function): the most rows of this handle's shapes that fit 64 MiB, a
+ * multiple of 32, at most 65536. */
+int b200sac_critic_values_chunk(b200sac_t* h, int64_t* rows);
+
 /* Blob publication: the byte string Learner.run() stores under the Redis key 'parameters' after every update
  * (LunarLander_Distributed_SAC/src/learner.py:298-299: _pickle.dumps({'actor': state_dict}); read back by
  * Player.pull_parameters, player.py:75-85) assembled on the device.  blob_template: `image` = the constant bytes of the
@@ -643,6 +670,33 @@ int b200sac_replay_get_tree(b200sac_replay_t* rb, int32_t replica, int32_t task,
  * of the step counter; rows, ring indices (nullable) and importance weights (nullable) to HOST arrays. */
 int b200sac_replay_sample_prioritized(b200sac_replay_t* rb, int32_t replica, float* s, float* a, float* r, float* s2,
                                       float* d, int64_t* idx_out, float* w_out);
+/* Priority refresh: recompute the priorities of n filled slots idx[n] of replica `replica`'s sub-rings (ring indices as
+ * b200sac_replay_set_priorities takes them; idx == NULL with n = 0: every filled slot of every task) with the replica's
+ * current networks -- after b200sac_reset or b200sac_redo every leaf still holds the TD error of the discarded network
+ * until its slot is sampled again.  Per slot i with task t:
+ *   1. Row: what the step would train on.  Linked ring: the n-step fold with the replica's current horizon and gamma
+ *      ("n-step returns"), (s_i, a_i, R, s'_j, d_j, g); otherwise (s, a, r, s', d) with g = gamma.
+ *   2. Next action: a' and log pi' from the actor on s'_j through the step's policy head, with noise eps per action k:
+ *      stochastic = 0: eps = 0 (the mean action); stochastic = 1: eps = z0 of box_muller(w0, w1), (w0, w1) the first two
+ *      words of Philox4x32-10 with key = seed ^ (0xC2B2AE3D27D4EB4F * (replica + 1)) (mod 2^64; a multiplier no other draw
+ *      of the library uses) and counter (i & 0xFFFFFFFF, i >> 32, t, 0x7E00 + k).  The noise depends on the slot only, not
+ *      on n, the chunking or the order of idx.
+ *   3. Critic values: Qt1, Qt2 (targets) on (s'_j, a') and Q1, Q2 (locals) on (s_i, a_i) as b200sac_critic_values computes
+ *      them (eval mode).
+ *   4. TD target: y = rs R + g (1 - d_j)(min(Qt1, Qt2) - alpha log pi'), alpha = (float)exp((double)log_alpha[t]), formed
+ *      as the step forms it.
+ *   5. Leaf: prio = (|y - Q1| + |y - Q2|) / 2 in fp64, p = (prio + eps)^alpha as the step's priority update writes it.
+ *   6. Tree: every internal node of each touched (replica, task) tree is recomputed from its children; slots not refreshed
+ *      keep their leaves bit for bit.  A duplicated index is harmless: every copy computes the same value.
+ *   7. Max p: idx == NULL: each task's running max p becomes the largest of its refreshed leaves (rows pushed later get
+ *      it); otherwise max p is only raised, as by set_priorities.  A task with no filled slots is untouched.
+ * Synchronous, like set_priorities: ordered after everything enqueued on `stream` (a b200sac_reset / b200sac_redo enqueued
+ * just before it included), after every enqueued step, push and set_nstep, and done under the ring's lock.  Runs through
+ * the handle's evaluation scratch (b200sac_critic_values); the step's buffers and plan are untouched.
+ * A ring that is not prioritized, a bad replica, n < 0, n > 0 with a NULL idx, an idx that is not a filled slot or
+ * stochastic outside {0, 1} give B200SAC_ERR_INVALID; a CARE handle gives B200SAC_ERR_STATE; nothing changes then. */
+int b200sac_replay_refresh_priorities(b200sac_replay_t* rb, int32_t replica, int64_t n, const int64_t* idx, uint64_t seed,
+                                      int32_t stochastic, void* stream);
 
 /* ---- n-step returns (device ring only) --------------------------------------------------
  * A linked ring records, next to its 1-step transitions, which slot follows which: link[replica][slot] (int32) is the
