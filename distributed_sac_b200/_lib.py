@@ -132,6 +132,9 @@ SYMBOLS = {
     "b200sac_replay_get_links": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int64, _VP]),
     "b200sac_replay_fold": (C.c_int, [_VP, C.c_int32, C.c_int64] + [_VP] * 8),
     "b200sac_replay_refresh_priorities": (C.c_int, [_VP, C.c_int32, C.c_int64, _VP, C.c_uint64, C.c_int32, _VP]),
+    "b200sac_replay_attach_prior": (C.c_int, [_VP, _VP]),
+    "b200sac_replay_set_prior_rows": (C.c_int, [_VP, C.c_int32, C.c_int32, _VP]),
+    "b200sac_replay_get_prior_rows": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32)]),
 }
 
 _lib = None

@@ -706,6 +706,7 @@ class Replay:
         self.core = core
         self.lib = core.lib
         self._h = C.c_void_p(0)
+        self._prior = None
         self.capacity = int(capacity)
         w = {"device": 0, "host": 1}[where]
         self.prioritized = None if prioritized is None else dict(prioritized)
@@ -730,8 +731,9 @@ class Replay:
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value and self.core._h.value:
-            self.lib.b200sac_replay_destroy(self._h)
+            self.lib.b200sac_replay_destroy(self._h)         # (detaches the prior first, or from the ring it is the prior of)
         self._h = C.c_void_p(0)
+        self._prior = None
 
     def __del__(self):
         try:
@@ -833,6 +835,28 @@ class Replay:
                 continue
             _lib.check(self.lib.b200sac_replay_refresh_priorities(self._h, int(r), n, p, C.c_uint64(int(seed) % (1 << 64)),
                                                                   1 if stochastic else 0, _stream()))
+
+    # ---- prior-data rings (symmetric sampling) -------------------------------------------------
+    def attach_prior(self, prior: Optional["Replay"]):
+        """Make `prior` (a uniform, unlinked device Replay of the same core) this ring's prior-data ring, or detach with
+        None.  Steps then take set_prior_rows(m) rows of every task block from the prior (0 until set).  The ring keeps a
+        reference to the prior while it is attached."""
+        if prior is not None and not isinstance(prior, Replay):
+            raise ValueError(f"attach_prior takes a Replay or None (got {type(prior).__name__})")
+        _lib.check(self.lib.b200sac_replay_attach_prior(self._h, None if prior is None else prior._h))
+        self._prior = prior
+
+    def set_prior_rows(self, m: int, replica=None):
+        """Prior rows m in [0, batch / num_tasks] of every task block of one replica's steps (None: all), in stream order."""
+        if isinstance(m, bool) or int(m) != m:
+            raise ValueError(f"prior rows must be an int (got {m!r})")
+        for r in _replicas(self.core.cfg.replicas, replica):
+            _lib.check(self.lib.b200sac_replay_set_prior_rows(self._h, r, int(m), _stream()))
+
+    def get_prior_rows(self, replica=0) -> int:
+        m = C.c_int32(0)
+        _lib.check(self.lib.b200sac_replay_get_prior_rows(self._h, int(replica), C.byref(m)))
+        return m.value
 
     # ---- n-step returns (ring with trajectory links) ---------------------------------------------
     def set_nstep(self, n: int, replica=None):

@@ -575,6 +575,10 @@ struct b200sac {
   DevMem<double> cg_p, cg_f;
   DevMem<int> cg_it;
   EvalScratch ev;                 // b200sac_critic_values / b200sac_replay_refresh_priorities (allocated by the first call)
+  // prior-data rings (allocated with the first attach): [R][B] the encoded indices the last mixed gather read, and whether
+  // the last sampled step from a device ring was a mixed one (debug_read "idx")
+  DevMem<int> mix_idx;
+  bool idx_mixed = false;
 
   // The members release their resources; the publication stream's last copy lands first.
   ~b200sac() {
@@ -624,6 +628,11 @@ struct b200sac_replay {
   DevMem<long long> f_idx;        // fold scratch [kNstepChunk], with f_rows [kNstepChunk][row_stride], f_disc, f_m
   DevMem<float> f_rows, f_disc;
   DevMem<int> f_m;
+  // prior-data rings (b200sac_replay_attach_prior): the ring whose rows fill the first prior_rows rows of every task block
+  // of this ring's steps, and the ring this one is the prior of; both are changed under both rings' locks
+  b200sac_replay* prior = nullptr;
+  b200sac_replay* prior_of = nullptr;
+  ReplicaTable<int> prior_rows;   // [R] m, read by sample_mixed_kernel (made by the attach)
 };
 
 // Transition rows [s | a | r | s' | d], padded to row_stride floats: the format of the replay ring, the staging slots and
@@ -2901,6 +2910,43 @@ extern "C" int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t
   return 0;
 }
 
+static int ring_ready(const b200sac_replay* rb, int replica, int batches);
+
+// A ring's lock and, while it has a prior, the prior's as well, for the entry points that enqueue steps from the ring.  The
+// two are taken together (std::lock), never one while waiting for the other, and the prior is read again under both: an
+// attach or detach may have run in between.
+struct RingLocks {
+  std::unique_lock<std::mutex> own, pri;
+  explicit RingLocks(b200sac_replay* rb) : own(rb->mu) {
+    while (b200sac_replay* p = rb->prior) {
+      own.unlock();
+      pri = std::unique_lock<std::mutex>(p->mu, std::defer_lock);
+      std::lock(own, pri);
+      if (rb->prior == p) return;
+      pri.unlock();
+    }
+  }
+};
+
+// (under RingLocks) Every replica that draws prior rows finds every task sub-ring of the prior ready (ring_ready's rule).
+static int prior_ready(const b200sac_replay* rb) {
+  if (!rb->prior) return 0;
+  for (int rep = 0; rep < rb->h->R; ++rep)
+    if (*rb->prior_rows.row(rep) > 0)
+      if (int rc = ring_ready(rb->prior, rep, 4)) return rc;
+  return 0;
+}
+
+// (under RingLocks) The steps just enqueued on `st` read the ring and its prior: a writer of either waits for them.
+static int record_gather(b200sac_replay* rb, cudaStream_t st) {
+  for (b200sac_replay* x : {rb, rb->prior}) {
+    if (!x) continue;
+    CU(cudaEventRecord(x->ev_gather, st));
+    x->gather_pending = true;
+  }
+  return 0;
+}
+
 // ------------------------------------------------------------------------------------------
 // the step: from packed rows (a staging slot or b200sac_step's buffer) or sampled from a device ring
 // ------------------------------------------------------------------------------------------
@@ -2937,6 +2983,10 @@ static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, const 
   } else {
     auto sample_on = [&](cudaStream_t s2) {
       if (rb->per) return per_sample_on(h, rb, s2);
+      if (rb->prior)
+        return launch_k(sample_mixed_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, 1, s2, h->K, (const Counters*)h->cnt,
+                        (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx.get(), (long long)B, rb->seed,
+                        PriorDraw{rb->prior_rows.dev, rb->prior->d_fill, rb->prior->cap_per_task, rb->prior->seed});
       return launch_k(sample_indices_kernel, dim3(R), dim3(B > 256 ? 512 : 256), 0, 1, s2, h->K,   // __launch_bounds__(512): 512 threads fit
                       (const Counters*)h->cnt, (const long long*)rb->d_fill, rb->cap_per_task, rb->d_idx.get(), (long long)B, rb->seed);
     };
@@ -2945,6 +2995,10 @@ static int enqueue_body(b200sac* h, cudaStream_t st, const GraphKey& key, const 
     if (rb->traj)                               // linked ring: the same gather with the n-step fold in front of the scatter
       launch_k(ingest_nstep_kernel, grid, block, 0, 1, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
                (const int*)rb->d_idx, (long long)B, nstep_ring(rb), h->ns_buf.get());
+    else if (rb->prior)                         // ring with a prior: online and prior rows through one encoded index
+      launch_k(ingest_mixed_kernel, grid, block, 0, 1, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows,
+               (const float*)rb->prior->rows, rb->prior->rs_rows, h->row_stride, (const int*)rb->d_idx, (long long)B,
+               h->mix_idx.get());
     else
       launch_k(ingest_rows_kernel, grid, block, 0, 1, st, h->K, h->ing, (const float*)rb->rows, rb->rs_rows, h->row_stride,
                (const int*)rb->d_idx, (long long)B);
@@ -3003,6 +3057,7 @@ extern "C" int b200sac_prepare(b200sac_t* h, b200sac_replay_t* rb, void* stream)
   if (int rc = sb.begin()) return rc;
   cudaGraphExec_t ge = nullptr;
   if (rb->where == 0) {
+    RingLocks lk(rb);                           // the graphs capture the prior's rows and fill (capture enqueues no work)
     for (int n = kGraphSteps; n >= 1; n >>= 1)
       if (int rc = get_graph(h, sb.run, GraphKey{rb, rb->rows, nullptr, n, h->stamping}, &ge)) return rc;
   } else {
@@ -3127,6 +3182,8 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   const int n = (int)h->plan.size() + 1;
   *n_out = n;
   if (cap < n) return fail(B200SAC_ERR_INVALID, "need room for %d launches", n);
+  RingLocks lk(rb);
+  if (int rc = prior_ready(rb)) return rc;
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   std::vector<Event> evs((size_t)n + 1);
@@ -3135,6 +3192,8 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   for (int it = 0; it < iters; ++it) {
     if (int rc = enqueue_body(h, sb.run, GraphKey{rb, rb->rows, nullptr, 1, h->stamping}, evs.data())) return rc;
     h->host_steps += 1;
+    h->idx_mixed = rb->prior != nullptr;
+    if (int rc = record_gather(rb, sb.run)) return rc;
     CU(cudaStreamSynchronize(sb.run));
     for (int i = 0; i < n; ++i) {
       float ms = 0.f;
@@ -3144,7 +3203,7 @@ extern "C" int b200sac_profile_step(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   }
   for (int i = 0; i < n; ++i) out_ms[i] = (float)(acc[i] / iters);
   if (names && names_cap > 0) {
-    std::string s = "sample+ingest";
+    std::string s = rb->prior ? "sample_mixed+ingest_mixed" : "sample+ingest";
     for (auto& l : h->plan) s += ";" + l.label;
     snprintf(names, names_cap, "%s", s.c_str());
   }
@@ -3678,7 +3737,9 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "head") { src = h->pout.p + replica * h->pout.rs; n = (int64_t)2 * B * 2 * A; }      // [2B][2A]: mu | raw log-std
   else if (nm == "psave") { src = h->psave.p + replica * h->psave.rs; n = (int64_t)2 * B * A * kSaveW; }   // [2B][A][8]: std, diff, tanh, act, jac, EPS, mask, logp_j
   else if (nm == "isw" || nm == "prio" || nm == "idx") {   // prioritized replay: [B] weights, leaf values, ring indices (int32 bits)
-    if (nm == "idx" && !h->per_buf && h->ns_buf) {          // a uniform linked ring: the indices its gather folded from
+    if (nm == "idx" && h->idx_mixed) {                      // a ring with a prior: online k as k, prior k as -1 - k
+      src = reinterpret_cast<const float*>(h->mix_idx.get()) + (size_t)replica * B; n = B;
+    } else if (nm == "idx" && !h->per_buf && h->ns_buf) {   // a uniform linked ring: the indices its gather folded from
       src = h->ns_buf + ((size_t)2 * h->R + replica) * B; n = B;
     } else {
       if (!h->per_buf) return fail(B200SAC_ERR_INVALID, "'%s' needs a prioritized replay ring", name);
@@ -3846,6 +3907,8 @@ extern "C" int b200sac_replay_destroy(b200sac_replay_t* rb) {
   if (!rb) return 0;
   cudaSetDevice(rb->h->device);
   if (rb->h->prefetch_rb == rb) { rb->h->prefetch_slot = -1; rb->h->prefetch_rb = nullptr; }
+  if (rb->prior) b200sac_replay_attach_prior(rb, nullptr);
+  if (rb->prior_of) b200sac_replay_attach_prior(rb->prior_of, nullptr);
   drop_ring_graphs(rb->h, rb);
   delete rb;
   return 0;
@@ -4112,12 +4175,10 @@ extern "C" int b200sac_step_sampled(b200sac_t* h, b200sac_replay_t* rb, int32_t 
   if (int rc = sb.begin()) return rc;
   cudaStream_t st = sb.run;
   const int B = h->cfg.batch;
-  {
-    std::lock_guard<std::mutex> lk(rb->mu);
-    if (int rc = ring_ready(rb, kAllReplicas, 4)) return rc;
-  }
   if (rb->where == 0) {
-    std::lock_guard<std::mutex> lk(rb->mu);           // ordered against the ring's writers (ring_quiesce)
+    RingLocks lk(rb);                           // ordered against the writers of the ring and its prior (ring_quiesce)
+    if (int rc = ring_ready(rb, kAllReplicas, 4)) return rc;
+    if (int rc = prior_ready(rb)) return rc;
     int i = 0;
     if (!h->stamping)                           // (the in-graph timeline wants one step per graph)
       for (int n = kGraphSteps; n > 1; n >>= 1)
@@ -4125,9 +4186,13 @@ extern "C" int b200sac_step_sampled(b200sac_t* h, b200sac_replay_t* rb, int32_t 
           if (int rc = launch_step(h, st, GraphKey{rb, rb->rows, nullptr, n, h->stamping})) return rc;
     for (; i < n_steps; ++i)
       if (int rc = launch_step(h, st, GraphKey{rb, rb->rows, nullptr, 1, h->stamping})) return rc;
-    CU(cudaEventRecord(rb->ev_gather, st));
-    rb->gather_pending = true;
+    if (int rc = record_gather(rb, st)) return rc;
+    h->idx_mixed = rb->prior != nullptr;
     return sb.end();
+  }
+  {
+    std::lock_guard<std::mutex> lk(rb->mu);
+    if (int rc = ring_ready(rb, kAllReplicas, 4)) return rc;
   }
   // pinned-host ring: draw + gather on the host into the pinned slot, H2D on the side stream.  The NEXT
   // minibatch is prepared right after the current step has been launched, so host sampling, the gather and
@@ -4328,6 +4393,7 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   b200sac* h = rb->h;
   std::lock_guard<std::mutex> lk(rb->mu);
   if (rb->traj) return fail(B200SAC_ERR_STATE, "the ring already has trajectory links");
+  if (rb->prior || rb->prior_of) return fail(B200SAC_ERR_STATE, "the ring takes part in a prior-data attachment");
   for (auto f : rb->fill)
     if (f != 0) return fail(B200SAC_ERR_STATE, "trajectory links can only be enabled on an empty ring");
   CU(cudaSetDevice(h->device));
@@ -4429,6 +4495,76 @@ extern "C" int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_
     CU(cudaStreamSynchronize(rb->st));
     unpack_rows(h, rows.data(), c, f, i0);
   }
+  return 0;
+}
+
+// ------------------------------------------------------------------------------------------
+// prior-data rings (sample_mixed_kernel, ingest_mixed_kernel): a second uniform device ring whose rows fill the first m rows
+// of every task block of the online ring's steps
+// ------------------------------------------------------------------------------------------
+// (under both rings' locks) rb goes back to a plain ring; its steps no longer read the prior once they have gathered.
+static int detach_prior(b200sac_replay* rb) {
+  b200sac_replay* p = rb->prior;
+  if (int rc = ring_quiesce(rb)) return rc;
+  if (int rc = ring_quiesce(p)) return rc;
+  drop_ring_graphs(rb->h, rb);
+  rb->prior = nullptr;
+  p->prior_of = nullptr;
+  std::fill(rb->prior_rows.host.begin(), rb->prior_rows.host.end(), 0);
+  return 0;
+}
+
+extern "C" int b200sac_replay_attach_prior(b200sac_replay_t* rb, b200sac_replay_t* prior) {
+  if (!rb) return fail(B200SAC_ERR_INVALID, "null ring");
+  b200sac* h = rb->h;
+  CU(cudaSetDevice(h->device));
+  if (!prior) {
+    RingLocks lk(rb);
+    return rb->prior ? detach_prior(rb) : 0;
+  }
+  if (prior == rb) return fail(B200SAC_ERR_INVALID, "a ring cannot be its own prior");
+  if (prior->h != h) return fail(B200SAC_ERR_INVALID, "the prior belongs to another handle");
+  std::scoped_lock lk(rb->mu, prior->mu);
+  for (const b200sac_replay* x : {rb, prior}) {
+    if (x->where != 0) return fail(B200SAC_ERR_INVALID, "prior-data rings are device rings (not pinned-host)");
+    if (x->per) return fail(B200SAC_ERR_INVALID, "prior-data rings are uniform (not prioritized)");
+    if (x->traj) return fail(B200SAC_ERR_INVALID, "prior-data rings are unlinked (no trajectory links)");
+  }
+  if (rb->prior) return fail(B200SAC_ERR_STATE, "the ring already has a prior");
+  if (prior->prior_of) return fail(B200SAC_ERR_STATE, "the prior is already the prior of a ring");
+  if (prior->prior) return fail(B200SAC_ERR_STATE, "the prior has a prior itself");
+  ReplicaTable<int> m;
+  const int zero = 0;
+  if (int rc = m.init(h->R, &zero)) return rc;
+  if (!h->mix_idx) {                               // the handle's step buffer, with its first attachment
+    DevMem<int> mix_idx;
+    CU(cudaMalloc(mix_idx.put(), (size_t)h->R * h->cfg.batch * sizeof(int)));
+    CU(cudaMemset(mix_idx, 0, (size_t)h->R * h->cfg.batch * sizeof(int)));
+    h->mix_idx = std::move(mix_idx);
+  }
+  if (int rc = ring_quiesce(rb)) return rc;
+  if (int rc = ring_quiesce(prior)) return rc;
+  drop_ring_graphs(h, rb);                         // they hold the plain draw and gather
+  rb->prior_rows = std::move(m);
+  rb->prior = prior;
+  prior->prior_of = rb;
+  return 0;
+}
+
+extern "C" int b200sac_replay_set_prior_rows(b200sac_replay_t* rb, int32_t replica, int32_t m, void* stream) {
+  if (int rc = ring_check(rb, replica)) return rc;
+  const int P = rb->h->cfg.batch / rb->Teff;
+  if (m < 0 || m > P) return fail(B200SAC_ERR_INVALID, "prior rows must be in [0, %d] (got %d)", P, m);
+  std::lock_guard<std::mutex> lk(rb->mu);
+  if (!rb->prior) return fail(B200SAC_ERR_STATE, "the ring has no prior (b200sac_replay_attach_prior)");
+  return rb->prior_rows.set(rb->h, stream, replica, &m);
+}
+
+extern "C" int b200sac_replay_get_prior_rows(b200sac_replay_t* rb, int32_t replica, int32_t* m) {
+  if (int rc = ring_check(rb, replica)) return rc;
+  if (!m) return fail(B200SAC_ERR_INVALID, "null argument");
+  std::lock_guard<std::mutex> lk(rb->mu);
+  *m = rb->prior_rows.host.empty() ? 0 : *rb->prior_rows.row(replica);
   return 0;
 }
 

@@ -166,6 +166,27 @@ __global__ void ingest_rows_kernel(StepConst K, IngestOut O, const float* __rest
   }
 }
 
+// The gather of a step from a ring with a prior attached: index k >= 0 is online row k, -1 - k prior row k.  The indices
+// are kept in idx_keep [R][B] (b200sac_debug_read "idx"): the next step's draw may already be overwriting idx.
+__global__ void ingest_mixed_kernel(StepConst K, IngestOut O, const float* __restrict__ rows, long long rs_rows,
+                                    const float* __restrict__ prior_rows, long long prior_rs_rows, int row_stride,
+                                    const int* __restrict__ idx, long long rs_idx, int* __restrict__ idx_keep) {
+  KStamp ks_;
+  const int rep = blockIdx.y;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32, wpb = blockDim.x / 32;
+  const int B = K.B;
+  if (blockIdx.x == 0 && threadIdx.x == 0) bump_counters(O, rep, K.beta1, K.beta2);
+  if (blockIdx.x == gridDim.x - 1) snapshot_alpha(K, O, rep, threadIdx.x);
+  for (int i = blockIdx.x * wpb + warp; i < B; i += gridDim.x * wpb) {
+    const int k = idx[rep * rs_idx + i];
+    const float* row = k >= 0 ? rows + rep * rs_rows + (long long)k * row_stride
+                              : prior_rows + rep * prior_rs_rows + (long long)(-1 - k) * row_stride;
+    if (lane == 0) idx_keep[rep * rs_idx + i] = k;
+    ingest_row(K, O, rep, i, row, row + K.obs, row[K.obs + K.act], row + K.obs + K.act + 1,
+               row[2 * K.obs + K.act + 1], lane, 32);
+  }
+}
+
 // ------------------------------------------------------------------------------------------
 // Replay index sampling: uniform WITHOUT replacement (random.sample, LL/replay_buffer.py:65),
 // per task B/T when T > 0 (MS/replay_buffers.py:73-74).  One CTA per replica.  Duplicates are
@@ -174,9 +195,22 @@ __global__ void ingest_rows_kernel(StepConst K, IngestOut O, const float* __rest
 // ------------------------------------------------------------------------------------------
 constexpr int kHashSlots = 4096;   // >= 2 * max batch (batch <= 2048)
 
-__global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const Counters* __restrict__ cnt, const long long* __restrict__ fill,
-                                      long long cap_per_task, int* __restrict__ idx_out, long long rs_idx,
-                                      unsigned long long seed) {
+// The prior part of a mixed draw (b200sac_replay_attach_prior): in every task block t of the minibatch, slots
+// [tP, tP + m[rep]) draw from task t's sub-ring of the prior ring, the rest from the online ring.
+struct PriorDraw {
+  const int* m;                   // [R] prior rows per task block
+  const long long* fill;          // [R][Teff] the prior's per-task fill
+  long long cap_per_task;
+  unsigned long long seed;
+};
+
+// The draw of sample_indices_kernel (kMix = false) and sample_mixed_kernel.  A prior slot draws like an online slot (same
+// Philox counter) under the prior's key and fill; its table key is -2 - k (an online k and a prior k never compete) and its
+// output -1 - k.
+template <bool kMix>
+B200_D void draw_indices(const StepConst& K, const Counters* __restrict__ cnt, const long long* __restrict__ fill,
+                         long long cap_per_task, int* __restrict__ idx_out, long long rs_idx, unsigned long long seed,
+                         const PriorDraw& pr) {
   KStamp ks_;
   __shared__ int keys[kHashSlots];
   __shared__ int owner[kHashSlots];
@@ -186,6 +220,12 @@ __global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const 
   const long long step = cnt[rep].v[3];   // value BEFORE this step's bump
   Philox ph(seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(rep + 1));
   int* out = idx_out + rep * rs_idx;
+  int m = 0;
+  unsigned long long key_prior = 0;
+  if constexpr (kMix) {
+    m = pr.m[rep];
+    key_prior = pr.seed + 0x9E3779B97F4A7C15ull * (unsigned long long)(rep + 1);
+  }
   for (int i = threadIdx.x; i < kHashSlots; i += blockDim.x) { keys[i] = -1; owner[i] = 0x7fffffff; }
   // per-slot state lives in registers of the thread that owns slots i = threadIdx.x + j*blockDim.x
   constexpr int kMaxPer = 8;     // batch <= 8 * blockDim.x
@@ -202,12 +242,23 @@ __global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const 
       const int i = threadIdx.x + j * blockDim.x;
       if (i >= B || done[j]) continue;
       const int task = i / per;
-      const long long n = fill[rep * Teff + (task < Teff ? task : Teff - 1)];
-      uint32_t rnd[4];
-      ph((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)i, (uint32_t)att[j], rnd);
-      const unsigned long long r64 = ((unsigned long long)rnd[0] << 32) | rnd[1];
-      const long long local = (long long)(r64 % (unsigned long long)n);
-      const int key = (int)((long long)task * cap_per_task + local);
+      int key;
+      if constexpr (kMix) {
+        const bool prior = i - task * per < m;
+        const long long n = (prior ? pr.fill : fill)[rep * Teff + (task < Teff ? task : Teff - 1)];
+        uint32_t rnd[4];
+        (prior ? Philox(key_prior) : ph)((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)i, (uint32_t)att[j], rnd);
+        const unsigned long long r64 = ((unsigned long long)rnd[0] << 32) | rnd[1];
+        const long long local = (long long)(r64 % (unsigned long long)n);
+        key = prior ? (int)(-2 - ((long long)task * pr.cap_per_task + local)) : (int)((long long)task * cap_per_task + local);
+      } else {
+        const long long n = fill[rep * Teff + (task < Teff ? task : Teff - 1)];
+        uint32_t rnd[4];
+        ph((uint32_t)step, (uint32_t)(step >> 32), (uint32_t)i, (uint32_t)att[j], rnd);
+        const unsigned long long r64 = ((unsigned long long)rnd[0] << 32) | rnd[1];
+        const long long local = (long long)(r64 % (unsigned long long)n);
+        key = (int)((long long)task * cap_per_task + local);
+      }
       cur[j] = key;
       unsigned h = ((unsigned)key * 2654435761u) >> 20;   // 12 bits
       int probes = 0;
@@ -228,7 +279,7 @@ __global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const 
     for (int j = 0; j < kMaxPer; ++j) {
       const int i = threadIdx.x + j * blockDim.x;
       if (i >= B || done[j]) continue;
-      out[i] = cur[j];                 // always leave a valid index behind
+      out[i] = kMix && cur[j] < 0 ? cur[j] + 1 : cur[j];   // always leave a valid index behind
       if (pos[j] < 0 || owner[pos[j]] == i) {
         done[j] = true;
       } else {
@@ -249,6 +300,19 @@ __global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const 
     __syncthreads();
     if (pending == 0) break;
   }
+}
+
+__global__ void __launch_bounds__(512) sample_indices_kernel(StepConst K, const Counters* __restrict__ cnt, const long long* __restrict__ fill,
+                                      long long cap_per_task, int* __restrict__ idx_out, long long rs_idx,
+                                      unsigned long long seed) {
+  draw_indices<false>(K, cnt, fill, cap_per_task, idx_out, rs_idx, seed, PriorDraw{});
+}
+
+// The draw of a step from a ring with a prior attached: online indices k as k, prior indices k as -1 - k.
+__global__ void __launch_bounds__(512) sample_mixed_kernel(StepConst K, const Counters* __restrict__ cnt, const long long* __restrict__ fill,
+                                                           long long cap_per_task, int* __restrict__ idx_out, long long rs_idx,
+                                                           unsigned long long seed, PriorDraw prior) {
+  draw_indices<true>(K, cnt, fill, cap_per_task, idx_out, rs_idx, seed, prior);
 }
 
 // ------------------------------------------------------------------------------------------

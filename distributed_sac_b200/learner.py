@@ -88,7 +88,7 @@ class _BaseLearner:
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
                      n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                     redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None):
+                     redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None):
         self.critic_layer_norm = bool(critic_layer_norm)
         # DroQ (Hiraoka et al. 2022): dropout at rate p before every critic LayerNorm; it needs the LayerNorm critics
         if critic_dropout is not None:
@@ -117,6 +117,20 @@ class _BaseLearner:
         if int(n_step) > 1 and replay_where != "device":
             raise ValueError("n-step returns need replay_where='device' (the trajectory links live beside the device ring)")
         self.n_step = int(n_step)
+        # prior=dict(capacity=N, fraction=f): a prior-data ring beside the online ring, and every minibatch takes
+        # floor(f * P + 0.5) rows of each task block of P rows from it (RLPD's symmetric sampling: f = 0.5)
+        self.prior = None
+        if prior is not None:
+            if not isinstance(prior, dict) or set(prior) != {"capacity", "fraction"}:
+                raise ValueError(f"prior= takes exactly capacity and fraction (got {prior!r})")
+            if replay_where != "device":
+                raise ValueError("prior= needs replay_where='device' (the prior ring is a device ring)")
+            if prioritized is not None or self.n_step > 1:
+                raise ValueError("prior= needs a uniform, unlinked online ring (no prioritized=, n_step=1)")
+            cap = prior["capacity"]
+            if isinstance(cap, bool) or not isinstance(cap, (int, np.integer)) or cap < 1:
+                raise ValueError(f"prior capacity must be an int >= 1 (got {cap!r})")
+            self.prior = dict(capacity=int(cap), fraction=self._prior_fraction(prior["fraction"]))
         self.max_grad_norm = max_grad_norm
         self.pcgrad = bool(pcgrad)
         self.cagrad = None if cagrad is None else float(cagrad)
@@ -192,6 +206,9 @@ class _BaseLearner:
             self.core.set_pcgrad(critic=False, actor=False)
             self.set_cagrad(self.cagrad)
         self.memory = self._make_memory(replay_where)
+        if self.prior is not None:
+            self.memory.attach_prior(self.prior["capacity"])
+            self.set_prior_fraction(self.prior["fraction"])
         self.memory.start()
         self.save_model_path = os.path.join("saved_models", self.log_name, self.datetime)
         self.log_file = os.path.join("log", "log_" + self.log_name, f"{self.log_name}_log_{self.datetime}.txt")
@@ -231,6 +248,29 @@ class _BaseLearner:
             raise ValueError("this learner was built without cagrad=")
         self.core.set_cagrad(critic=c, actor=c)
         self.cagrad = float(c)
+
+    @staticmethod
+    def _prior_fraction(f):
+        if isinstance(f, bool) or not isinstance(f, (int, float, np.integer, np.floating)) or not 0.0 <= float(f) <= 1.0:
+            raise ValueError(f"the prior fraction must be a number in [0, 1] (got {f!r})")      # (NaN fails too)
+        return float(f)
+
+    def set_prior_fraction(self, f: float):
+        """Share f of every task block that the next update()s take from the prior ring: floor(f * P + 0.5) rows of each
+        block of P = batch / num_tasks rows.  The learner must have been built with prior=."""
+        if self.prior is None:
+            raise ValueError("this learner was built without prior=")
+        f = self._prior_fraction(f)
+        P = self.batch_size // max(self.num_tasks, 1)
+        self.memory.ring.set_prior_rows(math.floor(f * P + 0.5))
+        self.prior["fraction"] = f
+
+    def push_prior(self, states, actions, rewards, next_states, dones):
+        """Append prior-data transitions (the reference's tuple layout, the multi-task one-hot inside the states).  Not part
+        of a checkpoint, like the online ring."""
+        if self.prior is None:
+            raise ValueError("this learner was built without prior=")
+        self.memory.add_prior(states, actions, rewards, next_states, dones)
 
     def set_n_step(self, n: int):
         """Horizon of the n-step return, effective from the next update()."""
@@ -392,7 +432,8 @@ class _BaseLearner:
         self.core.soft_update(float(tau), critic=pairs[key])
 
     def wait_until_memoryReady(self):
-        while len(self.memory) <= self.start_memory_len:
+        # (with prior rows in the minibatch, the prior must also hold what the step's sampler needs)
+        while len(self.memory) <= self.start_memory_len or not self.memory.prior_ready():
             time.sleep(0.1)
 
     def act_batch(self, states, stochastic=True):
@@ -628,12 +669,13 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
                  pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None,
-                 critic_layer_norm=False, critic_dropout=None):
+                 critic_layer_norm=False, critic_dropout=None, prior=None):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
+                          prior)
 
     def _set_dims(self):
         c = self.cfg
@@ -658,10 +700,11 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
                  target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                 redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None):
+                 redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
+                          prior)
 
     def _set_dims(self):
         c = self.cfg
@@ -690,11 +733,12 @@ class MTSACLearner(_BaseLearner):
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
                  cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None, critic_layer_norm=False,
-                 critic_dropout=None):
+                 critic_dropout=None, prior=None):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
-                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout)
+                          cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
+                          prior)
 
     def _set_dims(self):
         c = self.cfg

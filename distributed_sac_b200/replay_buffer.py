@@ -39,8 +39,10 @@ class ReplayBuffer(threading.Thread):
         # n_step > 1: the ring keeps trajectory links and the steps train on n-step returns.  The players push single
         # transitions, interleaved, so add_many stitches every drain back into trajectories (stitch.Stitcher)
         self.n_step = int(n_step)
-        self.ring = Replay(core, int(buffer_size), where=where, seed=int(seed), prioritized=prioritized,
+        self.seed = int(seed)
+        self.ring = Replay(core, int(buffer_size), where=where, seed=self.seed, prioritized=prioritized,
                            trajectories=self.n_step > 1)
+        self.prior = None               # attach_prior: the prior-data ring
         self.stitcher = Stitcher() if self.n_step > 1 else None
         if self.n_step > 1:
             self.ring.set_nstep(self.n_step)
@@ -60,6 +62,26 @@ class ReplayBuffer(threading.Thread):
         self.ring.push(s, f(actions, c.act_dim), f(rewards, 1), s2, d, stream=stream)
         if self.stitcher is not None:
             self.ring.close_streams(self.stitcher.take_abandoned())
+
+    def attach_prior(self, capacity):
+        """A prior-data device ring of `capacity` transitions beside the online ring, attached to it.  Its seed is the online
+        ring's + 1, so the two rings draw different indices."""
+        self.prior = Replay(self.core, int(capacity), where="device", seed=self.seed + 1)
+        self.ring.attach_prior(self.prior)
+
+    def add_prior(self, states, actions, rewards, next_states, dones):
+        """Append rows to the prior ring (add_many's layout; no trajectories)."""
+        n = len(rewards)
+        f = lambda x, w: np.asarray(x, dtype=np.float32).reshape(n, w)
+        c = self.core.cfg
+        self.prior.push(f(states, c.obs_dim), f(actions, c.act_dim), f(rewards, 1), f(next_states, c.obs_dim),
+                        f(np.asarray(dones).astype(np.uint8), 1))
+
+    def prior_ready(self):
+        """False while steps take prior rows and a task of the prior holds fewer than 4 per-task batches (the step's rule)."""
+        if self.prior is None or self.ring.get_prior_rows() == 0:
+            return True
+        return self.prior.size() >= 4 * (self.batch_size // max(self.core.cfg.num_tasks, 1))
 
     def drain_once(self):
         pipe = self.server.pipeline()

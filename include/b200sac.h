@@ -743,6 +743,37 @@ int b200sac_replay_get_links(b200sac_replay_t* rb, int32_t replica, int32_t task
 int b200sac_replay_fold(b200sac_replay_t* rb, int32_t replica, int64_t n_idx, const int64_t* idx, float* s, float* a, float* R,
                         float* s2, float* d, float* disc, int32_t* m);
 
+/* ---- prior-data rings (device rings only) ----------------------------------------------
+ * Symmetric sampling (RLPD, Ball et al. 2023): every minibatch takes a fixed number of its rows from a fixed prior dataset
+ * (demonstrations, scripted rollouts, an earlier run's buffer) and the rest from the online ring, drawn and gathered inside
+ * the step's graph.  The prior is an ordinary ring of the same handle, filled by push / fill_synthetic.
+ * Split: with P = batch / num_tasks (batch when num_tasks = 0) and m = the replica's prior-row count, rows [tP, tP + m) of
+ * every task block t come from task t's sub-ring of the prior and rows [tP + m, (t + 1)P) from the online ring, so the
+ * minibatch keeps its task blocks (pcgrad handles see task_mismatch = 0).
+ * Draw: batch slot i of replica r draws exactly as the online ring's plain draw does -- Philox4x32-10 key
+ * seed + 0x9E3779B97F4A7C15 * (r + 1), counter (step, step >> 32, i, attempt), index (w0 << 32 | w1) % fill_t -- with the
+ * prior's seed and per-task fill for a prior slot.  Slots are distinct within each (task block, part): the lowest slot keeps
+ * a contested index and the others redraw with attempt + 1.  An online index and a prior index never compete.  So m = 0 is
+ * the plain ring's minibatch and step bit for bit, and m = P is that of a plain ring with the prior's seed and rows.
+ * Gather: the step trains on the drawn rows.  After a step from a ring with a prior, b200sac_debug_read "idx" [B] holds the
+ * encoded indices (int32 bit patterns): online ring index k as k, prior ring index k as -1 - k.  The launch count of a step
+ * is unchanged (b200sac_profile_step labels the launch "sample_mixed+ingest_mixed").
+ * Readiness: a step needs the online ring ready as before and, for every replica with m > 0, every task sub-ring of the
+ * prior holding >= 4 per-task batches; else B200SAC_ERR_STATE and nothing is enqueued.  b200sac_step_sampled, b200sac_update,
+ * b200sac_prepare, b200sac_profile_step and b200sac_graph_timeline hold both rings' locks while they enqueue, and a push into
+ * either ring waits for the steps that read it.  b200sac_replay_sample still draws from the online ring only. */
+/* Make `prior` the prior ring of `rb`; prior == NULL detaches (every replica's m back to 0: rb is a plain ring again).  Both
+ * must be uniform, unlinked device rings of one handle, prior != rb, else B200SAC_ERR_INVALID; rb already having a prior,
+ * prior already being a ring's prior or having a prior itself give B200SAC_ERR_STATE; nothing changes then.  Waits for the
+ * gathers both rings have pending and drops rb's graphs (rebuilt on next use).  b200sac_replay_destroy of either ring
+ * detaches first; b200sac_replay_enable_trajectories on an attached ring gives B200SAC_ERR_STATE. */
+int b200sac_replay_attach_prior(b200sac_replay_t* rb, b200sac_replay_t* prior);
+/* m of one replica, in [0, P], in stream order on `stream` like b200sac_replay_set_beta: steps enqueued afterwards use it,
+ * including launches of graphs b200sac_prepare instantiated (no graph is rebuilt).  m outside [0, P] or a bad replica:
+ * B200SAC_ERR_INVALID; a ring without a prior: B200SAC_ERR_STATE.  Get: the value last set (host mirror; 0 by default). */
+int b200sac_replay_set_prior_rows(b200sac_replay_t* rb, int32_t replica, int32_t m, void* stream);
+int b200sac_replay_get_prior_rows(b200sac_replay_t* rb, int32_t replica, int32_t* m);
+
 #ifdef __cplusplus
 }
 #endif
