@@ -69,7 +69,7 @@ extern "C" const char* b200sac_last_error(void) { return g_err; }
 extern "C" const char* b200sac_version(void) { return "b200sac 0.1 (sm_90a)"; }
 
 // Sole owner of one CUDA resource (memory, event, stream, graph): released by Release when the owner is destroyed or
-// reset, and nowhere else.  put() hands the empty slot to the allocating call, e.g. CU(cudaMalloc(buf.put(), bytes)).
+// reset, and nowhere else.  put() hands the empty slot to the allocating call, e.g. CU(cudaMallocHost(buf.put(), bytes)).
 template <class H, auto Release>
 class Own {
  public:
@@ -93,6 +93,30 @@ using Event = Own<cudaEvent_t, cudaEventDestroy>;
 using Stream = Own<cudaStream_t, cudaStreamDestroy>;
 using Graph = Own<cudaGraph_t, cudaGraphDestroy>;
 using GraphExec = Own<cudaGraphExec_t, cudaGraphExecDestroy>;
+
+// New device buffers, events and streams for the owners above.  Each returns the first failing CUDA call's error, so that
+// a caller wraps it in CU like any CUDA call: CU(dev_fill(buf, n, 0.f)).
+// n elements of T, uninitialised: scratch that is written before it is read
+template <class T> cudaError_t dev_alloc(DevMem<T>& m, size_t n) { return cudaMalloc(m.put(), n * sizeof(T)); }
+// n elements of T copied from the host array src
+template <class T> cudaError_t dev_copy(DevMem<T>& m, const T* src, size_t n) {
+  cudaError_t e = dev_alloc(m, n);
+  return e != cudaSuccess ? e : cudaMemcpy(m, src, n * sizeof(T), cudaMemcpyHostToDevice);
+}
+// n elements of T, each v (T comes from m alone, so that v may be written 0, -1 or NAN): a value whose bytes are all equal
+// (0, -1, an all-ones NaN) is set by cudaMemset, any other is copied from the host
+template <class T> cudaError_t dev_fill(DevMem<T>& m, size_t n, std::common_type_t<T> v) {
+  unsigned char b[sizeof(T)];
+  memcpy(b, &v, sizeof(T));
+  if (std::all_of(b, b + sizeof(T), [&](unsigned char x) { return x == b[0]; })) {
+    cudaError_t e = dev_alloc(m, n);
+    return e != cudaSuccess ? e : cudaMemset(m, b[0], n * sizeof(T));
+  }
+  const std::vector<T> host(n, v);
+  return dev_copy(m, host.data(), n);
+}
+static cudaError_t new_event(Event& e) { return cudaEventCreateWithFlags(e.put(), cudaEventDisableTiming); }
+static cudaError_t new_stream(Stream& s) { return cudaStreamCreateWithFlags(s.put(), cudaStreamNonBlocking); }
 
 // ------------------------------------------------------------------------------------------
 // layout
@@ -587,6 +611,17 @@ struct b200sac {
   }
 };
 
+// The argument checks the entry points share, each with its one error text.
+static int check_replica(const b200sac* h, int replica) {
+  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  return 0;
+}
+// on: the handle's cfg flag of the feature called `name`
+static int need_feature(int on, const char* name) {
+  if (!on) return fail(B200SAC_ERR_STATE, "the handle was created without %s", name);
+  return 0;
+}
+
 struct b200sac_replay {
   b200sac* h = nullptr;
   int where = 0;
@@ -675,8 +710,7 @@ struct SlabCarver {
     floats += (size_t)b.rs * R;
   }
   int allocate(DevMem<float>& slab) {
-    CU(cudaMalloc(slab.put(), floats * sizeof(float)));
-    CU(cudaMemset(slab, 0, floats * sizeof(float)));
+    CU(dev_fill(slab, floats, 0.f));
     for (auto& [b, off] : at) b->p = slab + off;
     return 0;
   }
@@ -998,9 +1032,7 @@ struct PlanBuilder {
   template <class T> const T* upload(std::vector<DevMem<T>>& owner, const std::vector<T>& v) {
     if (v.empty()) return nullptr;
     DevMem<T> d;
-    cudaError_t e = cudaMalloc(d.put(), v.size() * sizeof(T));
-    if (e == cudaSuccess) e = cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice);
-    if (e != cudaSuccess) {
+    if (cudaError_t e = dev_copy(d, v.data(), v.size())) {
       cudaGetLastError();
       rc = fail(e == cudaErrorMemoryAllocation ? B200SAC_ERR_NOMEM : B200SAC_ERR_CUDA, "plan table upload failed: %s", cudaGetErrorString(e));
       return nullptr;
@@ -1403,10 +1435,7 @@ int PlanBuilder::build_plan_fused() {
   rw.psave = h->psave.p + (long long)B * A * kSaveW; rw.rsSave = h->psave.rs;
   rw.dout_dbg = h->dout_dbg.p; rw.dact_dbg = h->dact_dbg.p; rw.rsDbg = h->dout_dbg.rs;
 
-  if (h->env.chain_dbg) {
-    CU(cudaMalloc(h->chain_dbg.put(), sizeof(long long) * CH_DBG_SLOTS * 16));
-    CU(cudaMemset(h->chain_dbg, 0, sizeof(long long) * CH_DBG_SLOTS * 16));
-  }
+  if (h->env.chain_dbg) CU(dev_fill(h->chain_dbg, CH_DBG_SLOTS * 16, 0));
   auto dbg_slot = [&]() { return (h->chain_dbg && h->plan.size() < 16) ? h->chain_dbg + h->plan.size() * CH_DBG_SLOTS : nullptr; };
 
   // Stage tables of one MLP.  Forward: input rows X, hidden layers 0..nh-1, outputs stored to store[l] from row store_row.
@@ -2147,28 +2176,19 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   K.beta1 = cfg->beta1; K.beta2 = cfg->beta2; K.adam_eps = cfg->adam_eps;
   K.seed = seed;
 
-  CU(cudaMalloc(h->params.put(), sizeof(float) * L.arena * R));
-  CU(cudaMalloc(h->adam_m.put(), sizeof(float) * L.trainable * R));
-  CU(cudaMalloc(h->adam_v.put(), sizeof(float) * L.trainable * R));
-  CU(cudaMalloc(h->grads.put(), sizeof(float) * L.trainable * R));
-  CU(cudaMalloc(h->cnt.put(), sizeof(Counters) * R));
-  CU(cudaMalloc(h->losses.put(), sizeof(float) * kLossSlots * R * 4));
-  CU(cudaMemset(h->params, 0, sizeof(float) * L.arena * R));
-  CU(cudaMemset(h->adam_m, 0, sizeof(float) * L.trainable * R));
-  CU(cudaMemset(h->adam_v, 0, sizeof(float) * L.trainable * R));
-  CU(cudaMemset(h->grads, 0, sizeof(float) * L.trainable * R));
+  Counters c0;
+  memset(&c0, 0, sizeof(c0));
+  for (int i = 0; i < 5; ++i) c0.b1p[i] = c0.b2p[i] = 1.0;
+  CU(dev_fill(h->params, (size_t)L.arena * R, 0.f));
+  CU(dev_fill(h->adam_m, (size_t)L.trainable * R, 0.f));
+  CU(dev_fill(h->adam_v, (size_t)L.trainable * R, 0.f));
+  CU(dev_fill(h->grads, (size_t)L.trainable * R, 0.f));
+  CU(dev_fill(h->cnt, R, c0));
+  CU(dev_fill(h->losses, (size_t)kLossSlots * R * 4, 0.f));
   h->gslices = cfg->batch >= kSplitKMin ? kSplitK : 1;   // K of every weight gradient = batch
   if (cfg->pcgrad) h->gslices = cfg->num_tasks;         // one slice per task
-  if (h->gslices > 1) {     // never-written entries of slices >= 1 must read as zero (Adam sums all slices)
-    CU(cudaMalloc(h->grads_x.put(), sizeof(float) * L.trainable * R * (h->gslices - 1)));
-    CU(cudaMemset(h->grads_x, 0, sizeof(float) * L.trainable * R * (h->gslices - 1)));
-  }
-  {
-    std::vector<Counters> c0((size_t)R);
-    for (auto& c : c0) { memset(&c, 0, sizeof(c)); for (int i = 0; i < 5; ++i) c.b1p[i] = c.b2p[i] = 1.0; }
-    CU(cudaMemcpy(h->cnt, c0.data(), sizeof(Counters) * R, cudaMemcpyHostToDevice));
-  }
-  CU(cudaMemset(h->losses, 0, sizeof(float) * kLossSlots * R * 4));
+  if (h->gslices > 1)       // never-written entries of slices >= 1 must read as zero (Adam sums all slices)
+    CU(dev_fill(h->grads_x, (size_t)L.trainable * R * (h->gslices - 1), 0.f));
   {
     b200sac_hparams hp0;
     hp0.gamma = cfg->gamma; hp0.reward_scale = cfg->reward_scale; hp0.tau = cfg->tau;
@@ -2184,55 +2204,39 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     const size_t n = (size_t)kClipCols * R;
     const double inf[kClipCols] = {INFINITY, INFINITY, INFINITY};
     if (int rc = h->clip_thr.init(R, inf)) return rc;
-    const std::vector<float> ones(n, 1.0f);
-    CU(cudaMalloc(h->clip_coef.put(), sizeof(float) * n));
-    CU(cudaMemcpy(h->clip_coef, ones.data(), sizeof(float) * n, cudaMemcpyHostToDevice));
+    CU(dev_fill(h->clip_coef, n, 1.f));
     CU(cudaHostAlloc(h->gnorm_h.put(), sizeof(float) * kLossSlots * n, cudaHostAllocMapped));
     std::fill(h->gnorm_h.get(), h->gnorm_h.get() + kLossSlots * n, NAN);
     CU(cudaHostGetDevicePointer((void**)&h->gnorm_h_dev, h->gnorm_h, 0));
-    CU(cudaMalloc(h->gn_part.put(), sizeof(double) * kGradNormMaxBlocks * n));
-    CU(cudaMalloc(h->gn_ticket.put(), sizeof(unsigned) * n));
-    CU(cudaMemset(h->gn_ticket, 0, sizeof(unsigned) * n));
+    CU(dev_alloc(h->gn_part, kGradNormMaxBlocks * n));
+    CU(dev_fill(h->gn_ticket, n, 0));
   }
   {                           // ReDo record: scores NaN (all-ones bytes), flags 0
     for (int l = 0; l < cfg->n_actor_hidden; ++l) h->redo_n += cfg->actor_hidden[l];
     for (int l = 0; l < cfg->n_critic_hidden; ++l) h->redo_n += 2 * cfg->critic_hidden[l];
     const size_t n = (size_t)h->redo_n * R;
-    CU(cudaMalloc(h->redo_score.put(), sizeof(double) * n));
-    CU(cudaMemset(h->redo_score, 0xFF, sizeof(double) * n));
-    CU(cudaMalloc(h->redo_flag.put(), n));
-    CU(cudaMemset(h->redo_flag, 0, n));
+    double nan_ones;
+    memset(&nan_ones, 0xFF, sizeof(nan_ones));
+    CU(dev_fill(h->redo_score, n, nan_ones));
+    CU(dev_fill(h->redo_flag, n, 0));
   }
   if (cfg->pcgrad) {          // switches on, weights 1, record NaN until a step writes it
     const int T = cfg->num_tasks;
     const size_t n2 = (size_t)2 * R;
     const int on[2] = {1, 1};
     if (int rc = h->pc_on.init(R, on)) return rc;
-    CU(cudaMalloc(h->pc_part.put(), sizeof(double) * n2 * kGradNormMaxBlocks * pcgrad_pairs(T)));
-    CU(cudaMalloc(h->pc_ticket.put(), sizeof(unsigned) * n2));
-    CU(cudaMemset(h->pc_ticket, 0, sizeof(unsigned) * n2));
-    const std::vector<double> gnan(n2 * T * T, NAN);
-    CU(cudaMalloc(h->pc_G.put(), sizeof(double) * n2 * T * T));
-    CU(cudaMemcpy(h->pc_G, gnan.data(), sizeof(double) * n2 * T * T, cudaMemcpyHostToDevice));
-    const std::vector<float> ones(n2 * T, 1.0f);
-    CU(cudaMalloc(h->pc_w.put(), sizeof(float) * n2 * T));
-    CU(cudaMemcpy(h->pc_w, ones.data(), sizeof(float) * n2 * T, cudaMemcpyHostToDevice));
-    CU(cudaMalloc(h->pc_perm.put(), sizeof(int) * n2 * T * T));
-    CU(cudaMemset(h->pc_perm, 0, sizeof(int) * n2 * T * T));
-    CU(cudaMalloc(h->pc_mask.put(), sizeof(unsigned long long) * n2 * T));
-    CU(cudaMemset(h->pc_mask, 0, sizeof(unsigned long long) * n2 * T));
-    CU(cudaMalloc(h->pc_bad.put(), sizeof(int) * R));
-    CU(cudaMemset(h->pc_bad, 0, sizeof(int) * R));
+    CU(dev_alloc(h->pc_part, n2 * kGradNormMaxBlocks * pcgrad_pairs(T)));
+    CU(dev_fill(h->pc_ticket, n2, 0));
+    CU(dev_fill(h->pc_G, n2 * T * T, NAN));
+    CU(dev_fill(h->pc_w, n2 * T, 1.f));
+    CU(dev_fill(h->pc_perm, n2 * T * T, 0));
+    CU(dev_fill(h->pc_mask, n2 * T, 0));
+    CU(dev_fill(h->pc_bad, R, 0));
     const double off[2] = {0.0, 0.0};      // CAGrad off, its record NaN / -1 until a step runs it
     if (int rc = h->cg_c.init(R, off)) return rc;
-    const std::vector<double> pnan(n2 * std::max(T, kCagScalars), NAN);
-    CU(cudaMalloc(h->cg_p.put(), sizeof(double) * n2 * T));
-    CU(cudaMemcpy(h->cg_p, pnan.data(), sizeof(double) * n2 * T, cudaMemcpyHostToDevice));
-    CU(cudaMalloc(h->cg_f.put(), sizeof(double) * n2 * kCagScalars));
-    CU(cudaMemcpy(h->cg_f, pnan.data(), sizeof(double) * n2 * kCagScalars, cudaMemcpyHostToDevice));
-    const std::vector<int> none(n2, -1);
-    CU(cudaMalloc(h->cg_it.put(), sizeof(int) * n2));
-    CU(cudaMemcpy(h->cg_it, none.data(), sizeof(int) * n2, cudaMemcpyHostToDevice));
+    CU(dev_fill(h->cg_p, n2 * T, NAN));
+    CU(dev_fill(h->cg_f, n2 * kCagScalars, NAN));
+    CU(dev_fill(h->cg_it, n2, -1));
   }
 
   // work slab.  Buffers that a kernel addresses with one replica stride get one length: rsX (XQ, XT, XP), rsR (r, d, tid),
@@ -2303,9 +2307,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
       maxH = std::max(maxH, cfg->critic_hidden[l]);
     }
     const size_t chunks = (size_t)(B + kLnRows - 1) / kLnRows;
-    CU(cudaMalloc(h->ln_part.put(), sizeof(double) * R * 2 * chunks * 2 * maxH));
-    CU(cudaMalloc(h->ln_ticket.put(), sizeof(unsigned) * R * 2));
-    CU(cudaMemset(h->ln_ticket, 0, sizeof(unsigned) * R * 2));
+    CU(dev_alloc(h->ln_part, R * 2 * chunks * 2 * maxH));
+    CU(dev_fill(h->ln_ticket, (size_t)R * 2, 0));
   }
   if (cfg->critic_dropout) {  // rate 0 on every replica; masks all zero until a step draws them
     for (CriticPass& p : h->pass) {
@@ -2349,22 +2352,15 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   h->stage_floats = (size_t)R * B * h->row_stride + (size_t)2 * R * B * A;   // rows + eps_next/eps_cur
   for (int i = 0; i < 2; ++i) {
     CU(cudaMallocHost(h->stage_h[i].put(), h->stage_floats * sizeof(float)));
-    CU(cudaMalloc(h->stage_d[i].put(), h->stage_floats * sizeof(float)));
-    CU(cudaEventCreateWithFlags(h->ev_copied[i].put(), cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(h->ev_consumed[i].put(), cudaEventDisableTiming));
+    CU(dev_alloc(h->stage_d[i], h->stage_floats));
+    CU(new_event(h->ev_copied[i]));
+    CU(new_event(h->ev_consumed[i]));
   }
   CU(cudaHostAlloc(h->loss_h.put(), sizeof(float) * R * 4 * kLossSlots, cudaHostAllocMapped));
   memset(h->loss_h, 0, sizeof(float) * R * 4 * kLossSlots);
   CU(cudaHostGetDevicePointer((void**)&h->loss_h_dev, h->loss_h, 0));
-  CU(cudaStreamCreateWithFlags(h->side.put(), cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(h->own.put(), cudaStreamNonBlocking));
-  CU(cudaStreamCreateWithFlags(h->fork.put(), cudaStreamNonBlocking));
-  CU(cudaEventCreateWithFlags(h->ev_ingested.put(), cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(h->ev_sampled.put(), cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(h->ev_fork_src.put(), cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(h->ev_fork_done.put(), cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(h->ev_in.put(), cudaEventDisableTiming));
-  CU(cudaEventCreateWithFlags(h->ev_out.put(), cudaEventDisableTiming));
+  for (Stream* s : {&h->side, &h->own, &h->fork}) CU(new_stream(*s));
+  for (Event* e : {&h->ev_ingested, &h->ev_sampled, &h->ev_fork_src, &h->ev_fork_done, &h->ev_in, &h->ev_out}) CU(new_event(*e));
 
   h->fused = fused_eligible(h);
   if (int rc = build_plan(h)) return rc;
@@ -2397,7 +2393,7 @@ extern "C" int b200sac_export(b200sac_t* h, int32_t which, int32_t replica, floa
   if (!h || !buf) return fail(B200SAC_ERR_INVALID, "null argument");
   float* p; int64_t n;
   if (int rc = arena_of(h, which, &p, &n)) return rc;
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (n_floats != n) return fail(B200SAC_ERR_INVALID, "arena %d holds %lld floats per replica, got %lld", which, (long long)n, (long long)n_floats);
   CU(cudaSetDevice(h->device));
   CU(cudaMemcpyAsync(buf, p + (size_t)replica * n, n * sizeof(float), cudaMemcpyDefault, (cudaStream_t)stream));
@@ -2423,7 +2419,7 @@ extern "C" int b200sac_read_range(b200sac_t* h, int32_t which, int32_t replica, 
   if (!h || !out_host) return fail(B200SAC_ERR_INVALID, "null argument");
   float* p; int64_t n;
   if (int rc = arena_of(h, which, &p, &n)) return rc;
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (offset < 0 || n_floats < 1 || offset + n_floats > n) return fail(B200SAC_ERR_INVALID, "range [%lld, +%lld) outside the arena", (long long)offset, (long long)n_floats);
   CU(cudaSetDevice(h->device));
   CU(cudaMemcpyAsync(out_host, p + (size_t)replica * n + offset, (size_t)n_floats * sizeof(float), cudaMemcpyDeviceToHost, (cudaStream_t)stream));
@@ -2435,7 +2431,7 @@ extern "C" int b200sac_import(b200sac_t* h, int32_t which, int32_t replica, cons
   if (!h || !buf) return fail(B200SAC_ERR_INVALID, "null argument");
   float* p; int64_t n;
   if (int rc = arena_of(h, which, &p, &n)) return rc;
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (n_floats != n) return fail(B200SAC_ERR_INVALID, "arena %d holds %lld floats per replica, got %lld", which, (long long)n, (long long)n_floats);
   CU(cudaSetDevice(h->device));
   CU(cudaMemcpyAsync(p + (size_t)replica * n, buf, n * sizeof(float), cudaMemcpyDefault, (cudaStream_t)stream));
@@ -2444,7 +2440,8 @@ extern "C" int b200sac_import(b200sac_t* h, int32_t which, int32_t replica, cons
 }
 
 extern "C" int b200sac_get_steps(b200sac_t* h, int32_t replica, int64_t steps[4]) {
-  if (!h || !steps || replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (!h || !steps) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (int rc = check_replica(h, replica)) return rc;
   CU(cudaSetDevice(h->device));
   Counters c;
   CU(cudaMemcpy(&c, h->cnt + replica, sizeof(c), cudaMemcpyDeviceToHost));
@@ -2453,7 +2450,8 @@ extern "C" int b200sac_get_steps(b200sac_t* h, int32_t replica, int64_t steps[4]
 }
 
 extern "C" int b200sac_set_steps(b200sac_t* h, int32_t replica, const int64_t steps[4]) {
-  if (!h || !steps || replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (!h || !steps) return fail(B200SAC_ERR_INVALID, "bad argument");
+  if (int rc = check_replica(h, replica)) return rc;
   CU(cudaSetDevice(h->device));
   Counters c;
   CU(cudaMemcpy(&c, h->cnt + replica, sizeof(c), cudaMemcpyDeviceToHost));
@@ -2514,8 +2512,7 @@ int ReplicaTable<T, N, Mirror>::init(int R, const Mirror* v) {
     t.host.push_back(v[i % N]);
     rows[i] = device_value<T>(v[i % N]);
   }
-  CU(cudaMalloc(t.dev.put(), sizeof(T) * rows.size()));
-  CU(cudaMemcpy(t.dev, rows.data(), sizeof(T) * rows.size(), cudaMemcpyHostToDevice));
+  CU(dev_copy(t.dev, rows.data(), rows.size()));
   *this = std::move(t);
   return 0;
 }
@@ -2578,7 +2575,7 @@ extern "C" int b200sac_set_update_intervals(b200sac_t* h, int32_t replica, int32
 // Gradient-norm clipping thresholds, read by the grad_norm launches of the step graphs.
 extern "C" int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double* actor, double* ctx) {
   if (!h || !critic || !actor || !ctx) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  if (int rc = need_feature(h->cfg.grad_clip, "grad_clip")) return rc;
   if (int rc = h->clip_thr.check(replica)) return rc;
   const double* t = h->clip_thr.row(replica);
   *critic = t[0]; *actor = t[1]; *ctx = t[2];
@@ -2587,7 +2584,7 @@ extern "C" int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* crit
 
 extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double critic, double actor, double ctx, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  if (int rc = need_feature(h->cfg.grad_clip, "grad_clip")) return rc;
   if (int rc = h->clip_thr.check(replica)) return rc;
   if (!(critic > 0.0) || !(actor > 0.0) || !(ctx > 0.0))       // (NaN fails every comparison)
     return fail(B200SAC_ERR_INVALID, "gradient-norm thresholds must be > 0 (+inf: no clipping), got %g, %g, %g", critic, actor, ctx);
@@ -2598,7 +2595,7 @@ extern "C" int b200sac_set_grad_clip(b200sac_t* h, int32_t replica, double criti
 // Critic dropout rates, read by the dropout LayerNorm launches of the step graphs.
 extern "C" int b200sac_get_critic_dropout(b200sac_t* h, int32_t replica, double* p) {
   if (!h || !p) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.critic_dropout) return fail(B200SAC_ERR_STATE, "the handle was created without critic_dropout");
+  if (int rc = need_feature(h->cfg.critic_dropout, "critic_dropout")) return rc;
   if (int rc = h->drop.check(replica)) return rc;
   *p = *h->drop.row(replica);
   return 0;
@@ -2606,7 +2603,7 @@ extern "C" int b200sac_get_critic_dropout(b200sac_t* h, int32_t replica, double*
 
 extern "C" int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double p, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.critic_dropout) return fail(B200SAC_ERR_STATE, "the handle was created without critic_dropout");
+  if (int rc = need_feature(h->cfg.critic_dropout, "critic_dropout")) return rc;
   if (int rc = h->drop.check(replica)) return rc;
   if (!(p >= 0.0 && p < 1.0))                                   // (NaN fails every comparison)
     return fail(B200SAC_ERR_INVALID, "the critic dropout rate must be in [0, 1), got %g", p);
@@ -2616,7 +2613,7 @@ extern "C" int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double 
 // Gradient-surgery switches, read by the pcgrad launches of the step graphs.
 extern "C" int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_t* actor_on) {
   if (!h || !critic_on || !actor_on) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
   if (int rc = h->pc_on.check(replica)) return rc;
   *critic_on = h->pc_on.row(replica)[0]; *actor_on = h->pc_on.row(replica)[1];
   return 0;
@@ -2624,7 +2621,7 @@ extern "C" int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic
 
 extern "C" int b200sac_set_pcgrad(b200sac_t* h, int32_t replica, int32_t critic_on, int32_t actor_on, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
   if (int rc = h->pc_on.check(replica)) return rc;
   if ((critic_on != 0 && critic_on != 1) || (actor_on != 0 && actor_on != 1))
     return fail(B200SAC_ERR_INVALID, "pcgrad switches must be 0 or 1, got %d, %d", critic_on, actor_on);
@@ -2635,8 +2632,8 @@ extern "C" int b200sac_set_pcgrad(b200sac_t* h, int32_t replica, int32_t critic_
 extern "C" int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, float* w, int32_t* perm, uint64_t* mask,
                                    int32_t* task_mismatch, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
+  if (int rc = check_replica(h, replica)) return rc;
   const size_t T = (size_t)h->cfg.num_tasks, r2 = (size_t)replica * 2;
   CU(cudaSetDevice(h->device));
   cudaStream_t st = (cudaStream_t)stream;
@@ -2652,7 +2649,7 @@ extern "C" int b200sac_read_pcgrad(b200sac_t* h, int32_t replica, double* gram, 
 // CAGrad coefficients, read by the pcgrad launches of the step graphs.
 extern "C" int b200sac_get_cagrad(b200sac_t* h, int32_t replica, double* c_critic, double* c_actor) {
   if (!h || !c_critic || !c_actor) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
   if (int rc = h->cg_c.check(replica)) return rc;
   *c_critic = h->cg_c.row(replica)[0]; *c_actor = h->cg_c.row(replica)[1];
   return 0;
@@ -2660,7 +2657,7 @@ extern "C" int b200sac_get_cagrad(b200sac_t* h, int32_t replica, double* c_criti
 
 extern "C" int b200sac_set_cagrad(b200sac_t* h, int32_t replica, double c_critic, double c_actor, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
   if (int rc = h->cg_c.check(replica)) return rc;
   if (!(c_critic >= 0.0) || !(c_actor >= 0.0) || std::isinf(c_critic) || std::isinf(c_actor))   // (NaN fails >=)
     return fail(B200SAC_ERR_INVALID, "CAGrad coefficients must be finite and >= 0, got %g, %g", c_critic, c_actor);
@@ -2671,8 +2668,8 @@ extern "C" int b200sac_set_cagrad(b200sac_t* h, int32_t replica, double c_critic
 extern "C" int b200sac_read_cagrad(b200sac_t* h, int32_t replica, double* p, double* lambda, double* best, double* first,
                                    double* scale, int32_t* ibest, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
+  if (int rc = check_replica(h, replica)) return rc;
   const size_t T = (size_t)h->cfg.num_tasks, r2 = (size_t)replica * 2;
   CU(cudaSetDevice(h->device));
   CU(cudaStreamSynchronize((cudaStream_t)stream));
@@ -2696,10 +2693,7 @@ extern "C" int b200sac_cagrad_solve_test(int32_t T, const double* G, double c, f
   DevMem<double> dG, dp, df;
   DevMem<float> dw;
   DevMem<int> di;
-  CU(cudaMalloc(dG.put(), sizeof(double) * nG)); CU(cudaMalloc(dp.put(), sizeof(double) * T));
-  CU(cudaMalloc(df.put(), sizeof(double) * kCagScalars)); CU(cudaMalloc(dw.put(), sizeof(float) * T));
-  CU(cudaMalloc(di.put(), sizeof(int)));
-  CU(cudaMemcpy(dG, G, sizeof(double) * nG, cudaMemcpyHostToDevice));
+  CU(dev_copy(dG, G, nG)); CU(dev_alloc(dp, T)); CU(dev_alloc(df, kCagScalars)); CU(dev_alloc(dw, T)); CU(dev_alloc(di, 1));
   cagrad_test_kernel<<<1, 32, sizeof(double) * (nG + kCagVecs * T), cudaStreamLegacy>>>(dG, T, c, CagOut{dw, dp, df, di});
   CU(cudaGetLastError());
   CU(cudaStreamSynchronize(cudaStreamLegacy));
@@ -2716,8 +2710,8 @@ extern "C" int b200sac_cagrad_solve_test(int32_t T, const double* G, double c, f
 
 extern "C" int b200sac_export_task_grad(b200sac_t* h, int32_t replica, int32_t task, float* buf, int64_t n_floats, void* stream) {
   if (!h || !buf) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.pcgrad) return fail(B200SAC_ERR_STATE, "the handle was created without pcgrad");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = need_feature(h->cfg.pcgrad, "pcgrad")) return rc;
+  if (int rc = check_replica(h, replica)) return rc;
   if (task < 0 || task >= h->cfg.num_tasks) return fail(B200SAC_ERR_INVALID, "task %d out of range", task);
   const int64_t n = h->L.trainable;
   if (n_floats != n) return fail(B200SAC_ERR_INVALID, "the gradient arena holds %lld floats per replica, got %lld", (long long)n, (long long)n_floats);
@@ -2746,7 +2740,7 @@ extern "C" int b200sac_copy_replica(b200sac_t* h, int32_t src, int32_t dst, void
 
 extern "C" int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_spec* spec, uint64_t seed, void* stream) {
   if (!h || !spec) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   static const char* const kPart[B200SAC_RESET_PARTS] = {"actor", "critic", "alpha", "encoder", "context"};
   for (int p = 0; p < B200SAC_RESET_PARTS; ++p) {
     const b200sac_reset_part& q = spec->part[p];
@@ -2832,7 +2826,7 @@ __global__ void __launch_bounds__(256) blob_pack_kernel(const float* __restrict_
 extern "C" int b200sac_blob_template(b200sac_t* h, int32_t replica, const uint8_t* image, int64_t image_bytes, int64_t n_floats,
                                      const int32_t* src_index, const int32_t* dst_byte) {
   if (!h || !image || image_bytes <= 0 || n_floats <= 0 || !src_index || !dst_byte) return fail(B200SAC_ERR_INVALID, "bad argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (n_floats > 0x7fffffffLL || image_bytes > 0x7fffffffLL) return fail(B200SAC_ERR_INVALID, "image too large");
   for (int64_t j = 0; j < n_floats; ++j) {
     if (src_index[j] < 0 || src_index[j] >= h->L.arena) return fail(B200SAC_ERR_INVALID, "payload float %lld reads arena index %d outside [0, %lld)", (long long)j, src_index[j], (long long)h->L.arena);
@@ -2844,10 +2838,10 @@ extern "C" int b200sac_blob_template(b200sac_t* h, int32_t replica, const uint8_
   if (!h->pub) {
     Stream pub;
     Event snap[2], done[2];
-    CU(cudaStreamCreateWithFlags(pub.put(), cudaStreamNonBlocking));
+    CU(new_stream(pub));
     for (int i = 0; i < 2; ++i) {
-      CU(cudaEventCreateWithFlags(snap[i].put(), cudaEventDisableTiming));
-      CU(cudaEventCreateWithFlags(done[i].put(), cudaEventDisableTiming));
+      CU(new_event(snap[i]));
+      CU(new_event(done[i]));
     }
     h->pub = std::move(pub);
     for (int i = 0; i < 2; ++i) { h->ev_blob_snap[i] = std::move(snap[i]); h->ev_blob_done[i] = std::move(done[i]); }
@@ -2856,14 +2850,11 @@ extern "C" int b200sac_blob_template(b200sac_t* h, int32_t replica, const uint8_
   PinnedMem<uint8_t> img_h[2];
   DevMem<int> src, dst;
   for (int i = 0; i < 2; ++i) {
-    CU(cudaMalloc(img_d[i].put(), (size_t)image_bytes));
+    CU(dev_copy(img_d[i], image, (size_t)image_bytes));
     CU(cudaHostAlloc(img_h[i].put(), (size_t)image_bytes, cudaHostAllocDefault));
-    CU(cudaMemcpy(img_d[i], image, (size_t)image_bytes, cudaMemcpyHostToDevice));
   }
-  CU(cudaMalloc(src.put(), (size_t)n_floats * sizeof(int)));
-  CU(cudaMalloc(dst.put(), (size_t)n_floats * sizeof(int)));
-  CU(cudaMemcpy(src, src_index, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
-  CU(cudaMemcpy(dst, dst_byte, (size_t)n_floats * sizeof(int), cudaMemcpyHostToDevice));
+  CU(dev_copy(src, src_index, (size_t)n_floats));
+  CU(dev_copy(dst, dst_byte, (size_t)n_floats));
   CU(cudaStreamSynchronize(h->pub));             // no copy of the old images is in flight
   for (int i = 0; i < 2; ++i) { std::swap(h->blob_d[i], img_d[i]); std::swap(h->blob_h[i], img_h[i]); }
   std::swap(h->blob_src, src);
@@ -3079,7 +3070,7 @@ extern "C" int b200sac_step(b200sac_t* h, const float* s, const float* a, const 
   // call.  The transitions become rows laid out like a staging slot's (the staged step's graph body), the noise goes
   // straight into the step's noise buffer.
   const size_t RB = (size_t)h->R * h->cfg.batch, nA = (size_t)h->cfg.batch * h->cfg.act_dim;
-  if (!h->step_d) CU(cudaMalloc(h->step_d.put(), RB * h->row_stride * sizeof(float)));
+  if (!h->step_d) CU(dev_alloc(h->step_d, RB * h->row_stride));
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   const RowFields F = row_fields(h);
@@ -3261,8 +3252,7 @@ static int tc_gemm_test_impl(int32_t mode, int32_t M, int32_t N, int32_t K, cons
   TcProb t;
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   DevMem<TcProb> d;
-  CU(cudaMalloc(d.put(), sizeof(TcProb)));
-  CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
+  CU(dev_copy(d, &t, 1));
   CU(allow_smem((const void*)tc_kernel(bn, sw.pair128), tc_smem(bn)));
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn), (cudaStream_t)stream>>>(d, nullptr, 1, 0);
@@ -3277,8 +3267,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   DevMem<float> A, B, C;
   DevMem<long long> dbg;
   const size_t na = (size_t)(mode == GEMM_WGRAD ? K * M : M * K), nb = (size_t)(mode == GEMM_FWD ? N * K : K * N);
-  CU(cudaMalloc(A.put(), na * 4)); CU(cudaMalloc(B.put(), nb * 4)); CU(cudaMalloc(C.put(), (size_t)M * N * 4)); CU(cudaMalloc(dbg.put(), 96 * 8));
-  CU(cudaMemset(A, 0, na * 4)); CU(cudaMemset(B, 0, nb * 4)); CU(cudaMemset(dbg, 0, 96 * 8));
+  CU(dev_fill(A, na, 0.f)); CU(dev_fill(B, nb, 0.f)); CU(dev_alloc(C, (size_t)M * N)); CU(dev_fill(dbg, 96, 0));
   GemmProb p;
   memset(&p, 0, sizeof(p));
   p.A = A; p.B = B; p.C = C; p.M = M; p.N = N; p.K = K; p.mode = mode;
@@ -3289,8 +3278,7 @@ extern "C" int b200sac_tc_gemm_timeline(int32_t mode, int32_t M, int32_t N, int3
   if (int rc = make_tc_prob(p, 0, t, bn)) return rc;
   t.dbg = dbg;
   DevMem<TcProb> d;
-  CU(cudaMalloc(d.put(), sizeof(TcProb)));
-  CU(cudaMemcpy(d, &t, sizeof(TcProb), cudaMemcpyHostToDevice));
+  CU(dev_copy(d, &t, 1));
   CU(allow_smem((const void*)tc_kernel(bn, sw.pair128), tc_smem(bn)));
   dim3 grid((N + bn - 1) / bn, (M + TC_BM - 1) / TC_BM, 1);
   for (int it = 0; it < 3; ++it) tc_kernel(bn, sw.pair128)<<<grid, TC_THREADS, tc_smem(bn)>>>(d, nullptr, 1, 0);
@@ -3312,9 +3300,8 @@ extern "C" int b200sac_graph_timeline(b200sac_t* h, b200sac_replay_t* rb, int32_
   const int total = n * (iters + 1);
   DevMem<unsigned long long> dt;
   DevMem<int> di;
-  CU(cudaMalloc(dt.put(), sizeof(unsigned long long) * total));
-  CU(cudaMalloc(di.put(), sizeof(int)));
-  CU(cudaMemset(di, 0, sizeof(int)));
+  CU(dev_alloc(dt, total));
+  CU(dev_fill(di, 1, 0));
   StampBuf sb_on = {dt, di, total}, sb_off = {nullptr, nullptr, 0};
   if (int rc = b200sac_step_sampled(h, rb, 5, stream)) return rc;     // warm (graph instantiated)
   CU(cudaDeviceSynchronize());
@@ -3351,7 +3338,7 @@ extern "C" int b200sac_read_losses(b200sac_t* h, int32_t n_last, float* out_host
 
 extern "C" int b200sac_read_grad_norms(b200sac_t* h, int32_t n_last, float* out_host, void* stream) {
   if (!h || !out_host) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (!h->cfg.grad_clip) return fail(B200SAC_ERR_STATE, "the handle was created without grad_clip");
+  if (int rc = need_feature(h->cfg.grad_clip, "grad_clip")) return rc;
   CU(cudaSetDevice(h->device));
   return fetch_ring(h, (cudaStream_t)stream, n_last, h->gnorm_h, kClipCols, out_host);
 }
@@ -3415,7 +3402,7 @@ static int care_encode_rows(b200sac* h, cudaStream_t st, int replica, int n, Buf
 extern "C" int b200sac_act(b200sac_t* h, int32_t replica, int32_t n, const float* obs, const float* eps, int32_t stochastic,
                            float* actions_out, void* stream) {
   if (!h || !obs || !actions_out) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   const b200sac_cfg& c = h->cfg;
   const int B = c.batch, A = c.act_dim, La = c.n_actor_hidden;
   const int nmax = c.care ? B : 2 * B;           // CARE: one task id per row lives in the [batch] task-id buffer
@@ -3473,7 +3460,7 @@ extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const floa
   if (!h || !obs || !act) return fail(B200SAC_ERR_INVALID, "null argument");
   if (h->cfg.critic_ln)     // its forward has no LayerNorm, and one recycled unit would move its whole row's statistics
     return fail(B200SAC_ERR_STATE, "ReDo does not run on a handle created with critic_ln");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   const b200sac_cfg& c = h->cfg;
   const int B = c.batch, A = c.act_dim, La = c.n_actor_hidden, Lc = c.n_critic_hidden;
   if (n < 1 || n > B) return fail(B200SAC_ERR_INVALID, "n must be in [1, batch = %d], got %d", B, n);
@@ -3550,7 +3537,7 @@ extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const floa
 extern "C" int b200sac_read_redo(b200sac_t* h, int32_t replica, double* scores, uint8_t* dormant, int64_t cap,
                                  int64_t* n_neurons, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (n_neurons) *n_neurons = h->redo_n;
   if ((scores || dormant) && cap < h->redo_n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld", (long long)h->redo_n);
   CU(cudaSetDevice(h->device));
@@ -3608,8 +3595,7 @@ static int eval_alloc(b200sac* h) {
   const long long n = eval_rows(h);
   const long long floats = eval_carve(h, n, nullptr);
   DevMem<float> mem;
-  CU(cudaMalloc(mem.put(), (size_t)floats * sizeof(float)));
-  CU(cudaMemset(mem, 0, (size_t)floats * sizeof(float)));
+  CU(dev_fill(mem, (size_t)floats, 0.f));
   eval_carve(h, n, mem);
   E.rows = n;
   E.mem = std::move(mem);
@@ -3656,7 +3642,7 @@ extern "C" int b200sac_critic_values_chunk(b200sac_t* h, int64_t* rows) {
 extern "C" int b200sac_critic_values(b200sac_t* h, int32_t replica, int64_t n, const float* obs, const float* act, int32_t which,
                                      float* q_out, void* stream) {
   if (!h || !obs || !act || !q_out) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
+  if (int rc = check_replica(h, replica)) return rc;
   if (n < 1) return fail(B200SAC_ERR_INVALID, "n must be >= 1, got %lld", (long long)n);
   if (which != 0 && which != 1) return fail(B200SAC_ERR_INVALID, "which must be 0 (q1, q2) or 1 (their targets), got %d", which);
   if (h->cfg.care) return fail(B200SAC_ERR_STATE, "critic_values does not run on a CARE handle");
@@ -3714,7 +3700,7 @@ extern "C" int b200sac_soft_update_critic(b200sac_t* h, int32_t critic, double t
 extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replica, float* out_host, int64_t cap_floats,
                                   int64_t* n_floats, void* stream) {
   if (!h || !name || !out_host) return fail(B200SAC_ERR_INVALID, "null argument");
-  if (replica < 0 || replica >= h->R) return fail(B200SAC_ERR_INVALID, "replica out of range");
+  if (int rc = check_replica(h, replica)) return rc;
   CU(cudaSetDevice(h->device));
   const int B = h->cfg.batch, A = h->cfg.act_dim;
   const float* src = nullptr;
@@ -3826,8 +3812,7 @@ static int ring_check(const b200sac_replay* rb, int32_t replica, int kind = RING
   if (kind == RING_PER && !rb->per) return fail(B200SAC_ERR_INVALID, "not a prioritized ring (b200sac_replay_create_prioritized)");
   if (kind == RING_TRAJ && !rb->traj)
     return fail(B200SAC_ERR_STATE, "the ring has no trajectory links (b200sac_replay_enable_trajectories)");
-  if (replica < 0 || replica >= rb->h->R) return fail(B200SAC_ERR_INVALID, "replica %d out of range", replica);
-  return 0;
+  return check_replica(rb->h, replica);
 }
 
 // Waits (under rb->mu) until every step enqueued so far has gathered its rows and updated its priorities.
@@ -3888,13 +3873,12 @@ extern "C" int b200sac_replay_create(b200sac_t* h, int64_t capacity, int32_t whe
   rb->head.assign((size_t)h->R * Teff, 0);
   const size_t n = (size_t)h->R * rb->rs_rows;
   if (where == 0) {
-    CU(cudaMalloc(rb->rows_dev.put(), n * sizeof(float)));
+    CU(dev_alloc(rb->rows_dev, n));
     rb->rows = rb->rows_dev;
-    CU(cudaMalloc(rb->d_fill.put(), (size_t)h->R * Teff * sizeof(long long)));
-    CU(cudaMemset(rb->d_fill, 0, (size_t)h->R * Teff * sizeof(long long)));
-    CU(cudaMalloc(rb->d_idx.put(), (size_t)h->R * h->cfg.batch * sizeof(int)));
-    CU(cudaEventCreateWithFlags(rb->ev_gather.put(), cudaEventDisableTiming));
-    CU(cudaStreamCreateWithFlags(rb->st.put(), cudaStreamNonBlocking));
+    CU(dev_fill(rb->d_fill, (size_t)h->R * Teff, 0));
+    CU(dev_alloc(rb->d_idx, (size_t)h->R * h->cfg.batch));
+    CU(new_event(rb->ev_gather));
+    CU(new_stream(rb->st));
   } else {
     CU(cudaMallocHost(rb->rows_pinned.put(), n * sizeof(float)));
     rb->rows = rb->rows_pinned;
@@ -4031,7 +4015,7 @@ static int push_impl(b200sac_replay_t* rb, int32_t replica, int64_t n, const flo
     const size_t m = touched.size();
     if (m > rb->f_cap) {
       rb->f_at.reset(); rb->f_cap = 0;
-      CU(cudaMalloc(rb->f_at.put(), 2 * m * sizeof(int)));
+      CU(dev_alloc(rb->f_at, 2 * m));
       rb->f_cap = m;
     }
     vals.resize(m);
@@ -4081,7 +4065,7 @@ extern "C" int b200sac_replay_fill_synthetic(b200sac_replay_t* rb, int64_t n, ui
   float* dev_rows = rb->rows;
   DevMem<float> tmp;
   if (rb->where == 1) {   // generate on the device, copy down into the pinned ring
-    CU(cudaMalloc(tmp.put(), (size_t)h->R * rb->rs_rows * sizeof(float)));
+    CU(dev_alloc(tmp, (size_t)h->R * rb->rs_rows));
     dev_rows = tmp;
   }
   CU(cudaMemsetAsync(dev_rows, 0, (size_t)h->R * rb->rs_rows * sizeof(float), st));
@@ -4263,27 +4247,22 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
   while (tr.P < tr.cap) { tr.P <<= 1; ++tr.levels; }
   rb->draws.assign((size_t)h->R, 0);
   const size_t nt = (size_t)h->R * tr.T;
-  const std::vector<float> maxp0(nt, 1.f);
-  CU(cudaMalloc(rb->tree.put(), nt * 2 * (size_t)tr.P * sizeof(float)));
-  CU(cudaMemset(rb->tree, 0, nt * 2 * (size_t)tr.P * sizeof(float)));
-  CU(cudaMalloc(rb->maxp.put(), nt * sizeof(float)));
-  CU(cudaMemcpy(rb->maxp, maxp0.data(), nt * sizeof(float), cudaMemcpyHostToDevice));
+  CU(dev_fill(rb->tree, nt * 2 * (size_t)tr.P, 0.f));
+  CU(dev_fill(rb->maxp, nt, 1.f));
   if (int rc = rb->beta.init(h->R, &beta)) return rc;
-  CU(cudaMalloc(rb->s_lidx.put(), kPerMaxB * sizeof(long long)));
-  CU(cudaMalloc(rb->s_idx.put(), kPerMaxB * sizeof(int)));
-  CU(cudaMalloc(rb->s_f.put(), kPerMaxB * sizeof(float)));
-  CU(cudaMalloc(rb->s_rows.put(), (size_t)h->cfg.batch * h->row_stride * sizeof(float)));
+  CU(dev_alloc(rb->s_lidx, kPerMaxB));
+  CU(dev_alloc(rb->s_idx, kPerMaxB));
+  CU(dev_alloc(rb->s_f, kPerMaxB));
+  CU(dev_alloc(rb->s_rows, (size_t)h->cfg.batch * h->row_stride));
   tr.tree = rb->tree; tr.maxp = rb->maxp;
   if (!h->per_buf) {                               // the handle's step buffers, with its first prioritized ring
-    const size_t nb = (size_t)3 * h->R * h->cfg.batch * sizeof(float);
     DevMem<float> per_buf;
     Stream per_fork;
     Event ev_src, ev_done;
-    CU(cudaMalloc(per_buf.put(), nb));
-    CU(cudaMemset(per_buf, 0, nb));
-    CU(cudaStreamCreateWithFlags(per_fork.put(), cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(ev_src.put(), cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(ev_done.put(), cudaEventDisableTiming));
+    CU(dev_fill(per_buf, (size_t)3 * h->R * h->cfg.batch, 0.f));
+    CU(new_stream(per_fork));
+    CU(new_event(ev_src));
+    CU(new_event(ev_done));
     h->per_buf = std::move(per_buf); h->per_fork = std::move(per_fork);
     h->ev_per_src = std::move(ev_src); h->ev_per_done = std::move(ev_done);
   }
@@ -4403,21 +4382,18 @@ extern "C" int b200sac_replay_enable_trajectories(b200sac_replay_t* rb) {
   DevMem<long long> f_idx;
   DevMem<float> f_rows, f_disc;
   Event ev;
-  CU(cudaMalloc(link.put(), nl * sizeof(int)));
-  CU(cudaMemset(link, 0xff, nl * sizeof(int)));
+  CU(dev_fill(link, nl, -1));
   ReplicaTable<int> nstep;
   const int one = 1;
   if (int rc = nstep.init(h->R, &one)) return rc;
-  CU(cudaMalloc(f_idx.put(), kNstepChunk * sizeof(long long)));
-  CU(cudaMalloc(f_rows.put(), kNstepChunk * (size_t)h->row_stride * sizeof(float)));
-  CU(cudaMalloc(f_disc.put(), kNstepChunk * sizeof(float)));
-  CU(cudaMalloc(f_m.put(), kNstepChunk * sizeof(int)));
-  CU(cudaEventCreateWithFlags(ev.put(), cudaEventDisableTiming));
+  CU(dev_alloc(f_idx, kNstepChunk));
+  CU(dev_alloc(f_rows, kNstepChunk * (size_t)h->row_stride));
+  CU(dev_alloc(f_disc, kNstepChunk));
+  CU(dev_alloc(f_m, kNstepChunk));
+  CU(new_event(ev));
   if (!h->ns_buf) {                                // the handle's step buffer, with its first linked ring
-    const size_t nb = (size_t)3 * h->R * h->cfg.batch * sizeof(float);
     DevMem<float> ns_buf;
-    CU(cudaMalloc(ns_buf.put(), nb));
-    CU(cudaMemset(ns_buf, 0, nb));
+    CU(dev_fill(ns_buf, (size_t)3 * h->R * h->cfg.batch, 0.f));
     h->ns_buf = std::move(ns_buf);
   }
   drop_ring_graphs(h, rb);                         // they hold the unlinked gather
@@ -4538,8 +4514,7 @@ extern "C" int b200sac_replay_attach_prior(b200sac_replay_t* rb, b200sac_replay_
   if (int rc = m.init(h->R, &zero)) return rc;
   if (!h->mix_idx) {                               // the handle's step buffer, with its first attachment
     DevMem<int> mix_idx;
-    CU(cudaMalloc(mix_idx.put(), (size_t)h->R * h->cfg.batch * sizeof(int)));
-    CU(cudaMemset(mix_idx, 0, (size_t)h->R * h->cfg.batch * sizeof(int)));
+    CU(dev_fill(mix_idx, (size_t)h->R * h->cfg.batch, 0));
     h->mix_idx = std::move(mix_idx);
   }
   if (int rc = ring_quiesce(rb)) return rc;
