@@ -26,7 +26,8 @@ class Cfg(C.Structure):
         ("mix_out", C.c_int32), ("ctx_in", C.c_int32), ("n_ctx_hidden", C.c_int32),
         ("ctx_hidden", C.c_int32 * MAX_HIDDEN), ("ctx_out", C.c_int32), ("emb_dim", C.c_int32),
         ("tau_se", C.c_double), ("lr_ctx", C.c_double),
-        ("grad_clip", C.c_int32), ("pcgrad", C.c_int32), ("critic_ln", C.c_int32), ("critic_dropout", C.c_int32),
+        ("grad_clip", C.c_int32), ("pcgrad", C.c_int32), ("critic_ensemble", C.c_int32), ("critic_ln", C.c_int32),
+        ("critic_dropout", C.c_int32),
     ]
 
 
@@ -84,6 +85,8 @@ SYMBOLS = {
     "b200sac_read_grad_norms": (C.c_int, [_VP, C.c_int32, _VP, _VP]),
     "b200sac_set_critic_dropout": (C.c_int, [_VP, C.c_int32, C.c_double, _VP]),
     "b200sac_get_critic_dropout": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_double)]),
+    "b200sac_set_ensemble": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, _VP]),
+    "b200sac_get_ensemble": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_set_pcgrad": (C.c_int, [_VP, C.c_int32, C.c_int32, C.c_int32, _VP]),
     "b200sac_get_pcgrad": (C.c_int, [_VP, C.c_int32, C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
     "b200sac_read_pcgrad": (C.c_int, [_VP, C.c_int32, _VP, _VP, _VP, _VP, C.POINTER(C.c_int32), _VP]),

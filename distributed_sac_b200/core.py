@@ -53,6 +53,7 @@ class CoreConfig:
     pcgrad: bool = False                 # the per-layer plan with PCGrad gradient surgery (SacCore.set_pcgrad); num_tasks >= 2
     critic_layer_norm: bool = False      # LayerNorm between every hidden Linear and its ReLU in q1, q2 and their targets
     critic_dropout: bool = False         # with critic_layer_norm: dropout before every critic LayerNorm (SacCore.set_critic_dropout)
+    critic_ensemble: int = 0             # 0: twin critics; E in [2, 10]: critics q1 .. qE with a target subset (SacCore.set_ensemble)
 
     @property
     def obs_dim(self):
@@ -80,6 +81,7 @@ class CoreConfig:
         c.pcgrad = int(self.pcgrad)
         c.critic_ln = int(self.critic_layer_norm)
         c.critic_dropout = int(self.critic_dropout)
+        c.critic_ensemble = int(self.critic_ensemble)
         if self.care:
             c.emb_dim, c.lr_ctx = self.emb_dim, self.lr_ctx
             c.num_encoders, c.mix_out, c.ctx_in, c.ctx_out = self.num_encoders, self.mix_out, self.ctx_in, self.ctx_out
@@ -125,6 +127,7 @@ def _replicas(n, replica):
     return range(n) if replica is None else [int(replica)]
 
 
+ENSEMBLE_ACTOR = ("min", "mean")     # the actor's reduction over a critic ensemble, by its b200sac_set_ensemble code
 RESET_PARTS = ("actor", "critic", "alpha", "encoder", "context")      # index of b200sac_reset_spec.part[]
 
 
@@ -269,8 +272,9 @@ class SacCore:
 
     def critic_values(self, obs, act, target=False, replica=0):
         """(q1, q2) of one replica on n >= 1 rows obs [n][obs_dim] and act [n][act_dim] (CPU or CUDA tensors), or of
-        q1_target and q2_target with target=True: two [n] tensors on the device obs is on.  Eval mode (no dropout), any n,
-        every row's values independent of the others (b200sac_critic_values).  Synchronises the current stream."""
+        q1_target and q2_target with target=True: two [n] tensors on the device obs is on; on a critic_ensemble handle one
+        [E][n] tensor of q1 .. qE (or their targets).  Eval mode (no dropout), any n, every row's values independent of the
+        others (b200sac_critic_values).  Synchronises the current stream."""
         if not isinstance(target, (bool, np.bool_)):
             raise ValueError(f"target must be a bool, got {target!r}")
         obs = torch.as_tensor(obs).to(torch.float32).contiguous()
@@ -279,10 +283,15 @@ class SacCore:
         if n < 1 or obs.shape != (n, self.cfg.obs_dim) or act.shape != (n, self.cfg.act_dim):
             raise ValueError(f"obs must be [n][{self.cfg.obs_dim}] and act [n][{self.cfg.act_dim}] with n >= 1, got "
                              f"{tuple(obs.shape)} and {tuple(act.shape)}")
-        out = torch.empty(2, n, device=obs.device)
+        out = torch.empty(self.n_critics, n, device=obs.device)
         _lib.check(self.lib.b200sac_critic_values(self._h, int(replica), n, _ptr(obs), _ptr(act), 1 if target else 0, _ptr(out),
                                                   _stream()))
-        return out[0], out[1]
+        return out if self.cfg.critic_ensemble else (out[0], out[1])
+
+    @property
+    def n_critics(self) -> int:
+        """Critics per replica: cfg.critic_ensemble, or 2 (the twins)."""
+        return int(self.cfg.critic_ensemble) or 2
 
     def critic_values_chunk(self) -> int:
         """Rows critic_values and Replay.refresh_priorities evaluate per launch sequence (their scratch holds that many)."""
@@ -459,6 +468,23 @@ class SacCore:
         for r in _replicas(self.cfg.replicas, replica):
             _lib.check(self.lib.b200sac_set_critic_dropout(self._h, r, float(p), _stream()))
 
+    # ---- critic ensembles (b200sac_set/get_ensemble; handles with critic_ensemble=E) ---------------------------------------
+    ENSEMBLE_ACTOR = ENSEMBLE_ACTOR
+
+    def get_ensemble(self, replica=0):
+        """(m, actor) of one replica: the target subset size and "mean" or "min" (no synchronisation)."""
+        m, mean = C.c_int32(), C.c_int32()
+        _lib.check(self.lib.b200sac_get_ensemble(self._h, int(replica), C.byref(m), C.byref(mean)))
+        return m.value, self.ENSEMBLE_ACTOR[mean.value]
+
+    def set_ensemble(self, m, actor="mean", replica=None):
+        """Target subset size m in [1, E] and the actor's reduction over the E critics ("mean" or "min") of one replica
+        (replica=None: all of them), on the current stream.  Steps enqueued afterwards use them."""
+        if actor not in self.ENSEMBLE_ACTOR:
+            raise ValueError(f"actor must be 'mean' or 'min', got {actor!r}")
+        for r in _replicas(self.cfg.replicas, replica):
+            _lib.check(self.lib.b200sac_set_ensemble(self._h, r, int(m), self.ENSEMBLE_ACTOR.index(actor), _stream()))
+
     def read_grad_norms(self, n_last: int = 1) -> torch.Tensor:
         """Pre-clip gradient norms [n_last][R][3] (critic, actor, context encoder) of the last steps, aligned with read_losses;
         NaN where that optimizer did not step."""
@@ -591,7 +617,7 @@ class SacCore:
 
     def soft_update(self, tau: float, critic: Optional[int] = None):
         """Polyak update of the targets outside a step: both critics (CARE: and the target state encoder, with the replica's
-        tau_se unless tau == 1), or with critic=1 / 2 only q1_target / q2_target."""
+        tau_se unless tau == 1), or with critic=k only q<k>_target (k in [1, 2], or [1, E] on a critic_ensemble handle)."""
         if critic is None:
             _lib.check(self.lib.b200sac_soft_update(self._h, float(tau), _stream()))
         else:
@@ -685,7 +711,9 @@ class SacCore:
         elif name[0] in "hzm":
             widest = max(list(self.cfg.actor_hidden) + list(self.cfg.critic_hidden) + [4 * ((w + 3) // 4) * self.cfg.num_encoders
                                                                                         for w in self.cfg.mix_hidden])
-            cap = 2 * self.cfg.batch * widest
+            cap = max(2, self.n_critics) * self.cfg.batch * widest
+        elif name in ("q_pi", "dq_pi"):
+            cap = self.n_critics * self.cfg.batch
         return self._debug_raw(name, replica, cap)
 
     def _debug_raw(self, name, replica, cap):

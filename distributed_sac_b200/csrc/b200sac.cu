@@ -39,6 +39,7 @@
 #include "redo_kernels.cuh"
 #include "ln_kernels.cuh"
 #include "eval_kernels.cuh"
+#include "ensemble_kernels.cuh"
 
 using namespace bsac;
 
@@ -126,7 +127,7 @@ static cudaError_t new_stream(Stream& s) { return cudaStreamCreateWithFlags(s.pu
 struct LayerOff { int64_t w, b; int in, out; int ld; int64_t g = -1, c = -1; };
 struct Layout {
   std::vector<b200sac_tensor_desc> descs;
-  std::vector<LayerOff> actor, q[2], qt[2];
+  std::vector<LayerOff> actor, q[kMaxEns], qt[kMaxEns];   // critics q1 .. qE and their targets (E = 2 on twin handles)
   // CARE: the critic's state encoder (the target's sits at + target_delta with the same relative layout)
   std::vector<LayerOff> mix, trunk, ctx;      // mix: w = [K][out][in], b = [K][out]
   std::vector<LayerOff> cenc;                 // CARE(O): the trainable context encoder (header + mlp), no target copy
@@ -166,6 +167,10 @@ static int check_cfg(const b200sac_cfg* c) {
   if (c->critic_dropout != 0 && c->critic_dropout != 1) return fail(B200SAC_ERR_INVALID, "critic_dropout must be 0 or 1");
   if (c->critic_dropout && !c->critic_ln)
     return fail(B200SAC_ERR_INVALID, "critic_dropout needs critic_ln = 1 (the dropout sits before each critic LayerNorm)");
+  if (c->critic_ensemble != 0 && (c->critic_ensemble < 2 || c->critic_ensemble > B200SAC_MAX_ENSEMBLE))
+    return fail(B200SAC_ERR_INVALID, "critic_ensemble must be 0 or in [2, %d], got %d", B200SAC_MAX_ENSEMBLE, c->critic_ensemble);
+  if (c->critic_ensemble && (c->care || c->pcgrad))
+    return fail(B200SAC_ERR_INVALID, "critic_ensemble is for the plain-MLP critics without gradient surgery (care = 0, pcgrad = 0)");
   if (c->care == 2) {
     if (c->emb_dim < 1 || c->emb_dim > 256) return fail(B200SAC_ERR_INVALID, "1 <= emb_dim <= 256 required for CARE(O)");
     if (c->emb_dim != c->ctx_out)
@@ -257,6 +262,11 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
   const bool ln = c->critic_ln != 0;
   add_net("q1", &L.q[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true, ln);
   add_net("q2", &L.q[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true, ln);
+  for (int k = 2; k < c->critic_ensemble; ++k) {
+    snprintf(nm, sizeof(nm), "q%d", k + 1);
+    const std::string net(nm);
+    add_net(net.c_str(), &L.q[k], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 1, 0, true, ln);
+  }
   L.cse_begin = off;
   if (c->care) add_encoder("cse", true, 1, 0);
   L.critic_n = off - L.critic_begin;
@@ -275,6 +285,11 @@ static void build_layout(const b200sac_cfg* c, Layout& L) {
   int64_t tb = off;
   add_net("q1_target", &L.qt[0], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true, ln);
   add_net("q2_target", &L.qt[1], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true, ln);
+  for (int k = 2; k < c->critic_ensemble; ++k) {
+    snprintf(nm, sizeof(nm), "q%d_target", k + 1);
+    const std::string net(nm);
+    add_net(net.c_str(), &L.qt[k], L.in_w + c->act_dim, c->critic_hidden, c->n_critic_hidden, 1, 0, -1, true, ln);
+  }
   if (c->care) add_encoder("tse", false, 0, -1);
   L.target_delta = tb - L.critic_begin;
   if (c->care) L.off_emb = add("embedding", c->num_tasks, c->ctx_in, 0, -1);
@@ -316,6 +331,7 @@ static std::vector<InitTensor> init_table(const b200sac_cfg* c, const Layout& L)
   linear(L.actor, B200SAC_RESET_ACTOR, false);
   linear(L.q[0], B200SAC_RESET_CRITIC, true);
   linear(L.q[1], B200SAC_RESET_CRITIC, true);
+  for (int k = 2; k < c->critic_ensemble; ++k) linear(L.q[k], B200SAC_RESET_CRITIC, true);
   if (c->care) {
     for (const auto& lo : L.mix) {
       const int rows = c->num_encoders * lo.out;
@@ -362,7 +378,9 @@ typedef void (*TcKernel)(const TcProb*, const int*, int, int);
 struct TcCall { TcKernel kern; const TcProb* probs; const int* sched; int G, sched_stride; };
 using KernelCall = std::variant<StepFirst<PolicyDoutArgs>, StepFirst<PolicyHeadArgs>, StepFirst<CriticHeadArgs>,
                                 StepFirst<ActorQHeadArgs>, StepFirst<HeadBwdArgs>, StepFirst<AdamArgs>, StepFirst<PcgArgs>,
-                                StepFirst<GradNormArgs>, StepFirst<LnArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
+                                StepFirst<GradNormArgs>, StepFirst<LnArgs>, StepFirst<CriticHeadEnsArgs>,
+                                StepFirst<ActorQHeadEnsArgs>, StepFirst<HeadBwdEnsArgs>, StepFirst<PolicyDoutEnsArgs>,
+                                StepFirst<LnEnsArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
                                 NoStep<CareTabArgs>, NoStep<CareMixArgs>, NoStep<CareMixFwdArgs>, NoStep<CareMixBwdArgs>,
                                 NoStep<CareTabReduceArgs>, NoStep<CareTabWgradArgs>, NoStep<GemmGroup>, TcCall>;
 template <class P> static KernelCall bind(void (*kern)(StepConst, P), const P& args) { return StepFirst<P>{kern, args}; }
@@ -449,7 +467,8 @@ struct ReplicaTable {
 // The twin critics are evaluated on three sets of rows per step, each a pass with its own buffers; the index of a pass is
 // its Philox pass index (dropout masks).  Q: the local critics on (s, a) for the critic update (phase A, backward in C);
 // T: the target critics on (s', a') for the TD target (phase B); P: the updated local critics on (s, a~) for the actor
-// loss (phase D, forward and backward).  Every [2][B] / [2][B][H] buffer holds q1's rows, then q2's.
+// loss (phase D, forward and backward).  Every [2][B] / [2][B][H] buffer holds q1's rows, then q2's; on a critic_ensemble
+// handle [E][B] / [E][B][H], the rows of q1 .. qE.
 enum { PASS_Q = 0, PASS_T = 1, PASS_P = 2 };
 struct CriticPass {
   const std::vector<LayerOff>* net;   // [2]: the networks the pass runs (L.q or L.qt)
@@ -466,7 +485,8 @@ struct CriticPass {
 // time, in an allocation of its own (at most kEvalScratchBytes, made by the first call), so that the step's slab and
 // everything the next step reads stay untouched.  Each buffer holds `rows` rows:
 //   XQ, XT [ldx]      critic inputs (s | a) and (s' | a')
-//   hc[2] [2][Hc]     critic hidden activations, layer l in hc[l % 2]; z [2][Hc] pre-normalization (critic_ln)
+//   hc[2] [2][Hc]     critic hidden activations, layer l in hc[l % 2]; z [2][Hc] pre-normalization (critic_ln); [E][Hc]
+//                     on a critic_ensemble handle, like q and qt
 //   ha[2] [Ha]        actor hidden activations, layer l in ha[l % 2]
 //   q, qt [2]         q1 / q2 and their targets (row i of q1, then row i of q2)
 //   pout [2A], psave [A][kSaveW], act [A], logp, logstd, eps [A]   the policy head's outputs and noise
@@ -516,6 +536,11 @@ struct b200sac {
   DevMem<unsigned> ln_ticket;
   // cfg.critic_dropout: [R] dropout rates p (host mirror) and their DropRate
   ReplicaTable<DropRate, 1, double> drop;
+  // critics per pass: cfg.critic_ensemble, or 2 (the twins).  Ensemble handles: [R][2] (target subset size m, actor
+  // reduction 1 = mean / 0 = min) and the last step's subset [R][E] as 0 / 1 (debug_read "tsub")
+  int E = 2;
+  ReplicaTable<int, 2> ens;
+  Buf tsub;
   std::vector<Launch> plan;
   // what the plan's launches read through their argument blocks: each wgmma launch's problems, each layer-chained launch's
   // tensor maps
@@ -853,7 +878,7 @@ static int make_tc_prob(const GemmProb& p, int rep, TcProb& t, int bn = 64) {
 // ------------------------------------------------------------------------------------------
 static bool fused_eligible(const b200sac* h) {
   const b200sac_cfg& c = h->cfg;
-  if (c.precision != 0 || c.care || c.pcgrad || c.critic_ln || !h->env.fuse) return false;
+  if (c.precision != 0 || c.care || c.pcgrad || c.critic_ln || c.critic_ensemble || !h->env.fuse) return false;
   for (int i = 0; i < c.n_actor_hidden; ++i) if (c.actor_hidden[i] % 4 || c.actor_hidden[i] > CH_MAXW) return false;
   for (int i = 0; i < c.n_critic_hidden; ++i) if (c.critic_hidden[i] % 4 || c.critic_hidden[i] > CH_MAXW) return false;
   if (c.state_dim + c.num_tasks + c.act_dim > CH_MAXW - 4) return false;
@@ -998,6 +1023,11 @@ struct PlanBuilder {
   const int B, R, A, La, Lc, sms;
   const long long rsP, rsG;
   const Buf par, grd;       // parameter and gradient arenas
+  // critics per pass (2: the twins) and, on a critic_ensemble handle, the distance from one critic to the next in the
+  // parameter and gradient arenas (the critics share one layout and sit back to back)
+  const int E;
+  const bool ens;
+  const long long rsNet;
   int branch = 0;           // branch tag given to the launches gemm_launch creates
   // per-layer plan, FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads
   // the rest of the backward chain.  The weight-gradient launch goes to the fork stream and the chain continues at once (the
@@ -1009,10 +1039,10 @@ struct PlanBuilder {
   explicit PlanBuilder(b200sac* hh)
       : h(hh), c(hh->cfg), L(hh->L), B(c.batch), R(hh->R), A(c.act_dim), La(c.n_actor_hidden), Lc(c.n_critic_hidden),
         sms(sm_count()), rsP(L.arena), rsG(L.trainable), par{hh->params, L.arena}, grd{hh->grads, L.trainable},
-        use_fork(c.precision == 0 && !c.care) {}
+        E(hh->E), ens(c.critic_ensemble != 0), rsNet(L.q[1][0].w - L.q[0][0].w), use_fork(c.precision == 0 && !c.care) {}
   float* W(int64_t off) const { return h->params + off; }
   float* Gp(int64_t off) const { return h->grads + off; }
-  // network net's rows of a [2][B][H] buffer
+  // network net's rows of a [2][B][H] ([E][B][H]) buffer
   float* netp(const Buf& b, int net, int H) const { return b.p + (long long)net * B * H; }
   // network net's input rows at critic hidden layer l of pass cp: its input rows X, or layer l - 1's activations
   Buf critic_in(const CriticPass& cp, int net, int l) const {
@@ -1260,7 +1290,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   P.M = B;
   P.rsP = rsP; P.rsG = rsG;
   if (!policy) {
-    P.NO = 1; P.Kdim = Hc; P.nets = 2;
+    P.NO = 1; P.Kdim = Hc; P.nets = E;
     for (int net = 0; net < 2; ++net) {
       P.W[net] = W(L.q[net][Lc].w);
       P.dW[net] = want_wgrad ? Gp(L.q[net][Lc].w) : nullptr;
@@ -1268,7 +1298,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
     }
     const Buf& hb = h->pass[want_wgrad ? PASS_Q : PASS_P].h[Lc - 1];
     const Buf& dq = want_wgrad ? h->dq : h->dqa;
-    P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = 2 * h->y.rs;
+    P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = E * h->y.rs;
     P.h = hb.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hb.rs; P.ldh = Hc;
     P.dh = h->dhQ[Lc - 1].p; P.rsDhNet = (long long)B * Hc; P.rsDhRep = h->dhQ[Lc - 1].rs; P.lddh = Hc;
   } else {
@@ -1286,7 +1316,8 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
       Q.M = B;
       pl.grid = dim3((B * A + 255) / 256, R);
       pl.block = dim3(256);
-      push(std::move(pl), policy_dout_kernel, Q);
+      if (ens) push(std::move(pl), policy_dout_ens_kernel, PolicyDoutEnsArgs{Q, E});
+      else push(std::move(pl), policy_dout_kernel, Q);
     }
     P.NO = 2 * A; P.Kdim = Ha; P.nets = 1; P.policy_mode = split ? 0 : 1;
     if (split) { P.dout = h->dout_dbg.p; P.rsDoutNet = 0; P.rsDoutRep = h->dout_dbg.rs; }
@@ -1304,7 +1335,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   // partial head-weight gradient in gradient slice s, exactly like the split-K GEMM weight gradients
   P.row_slices = h->gslices;
   P.xs = (long long)R * L.trainable;
-  for (int net = 0; net < P.nets; ++net)
+  for (int net = 0; net < std::min(P.nets, 2); ++net)     // (ensembles: critic k's slots follow critic 0's at + k * rsNet)
     if (P.dW[net] && h->grads_x) { P.dWx[net] = h->grads_x + (P.dW[net] - h->grads); P.dbx[net] = h->grads_x + (P.db[net] - h->grads); }
   const int rows_per = (B + P.row_slices - 1) / P.row_slices;
   // 128-bit column mapping (head_bwd4_kernel) when every row pitch / tensor offset involved is a multiple of 4 floats --
@@ -1321,7 +1352,8 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
     rc = fail(B200SAC_ERR_INVALID, "batch * head width too large for head_bwd smem");
     return;
   }
-  push(std::move(l), wide ? head_bwd4_kernel<1> : head_bwd_kernel, P);
+  if (ens) push(std::move(l), wide ? head_bwd4_ens_kernel : head_bwd_ens_kernel, HeadBwdEnsArgs{P, rsNet, E});
+  else push(std::move(l), wide ? head_bwd4_kernel<1> : head_bwd_kernel, P);
 }
 
 // the trainable slice of optimizer `which` (0 critic, 1 actor, 2 CARE(O) context encoder)
@@ -1719,7 +1751,19 @@ void PlanBuilder::layer_norm(int pass, int l, bool fwd, bool want_grads) {
     P.tag0 = (pass * 8 + l) * 2;
   }
   ln.block = dim3(kLnThreads);
-  if (fwd) {
+  if (ens) {
+    if (drop) P.tag0 = (pass * 8 + l) * E;
+    const LnEnsArgs PE{P, rsNet, E};
+    if (fwd) {
+      ln.grid = dim3((E * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
+      if (drop) push(std::move(ln), ln_fwd_ens_kernel<true>, PE);
+      else push(std::move(ln), ln_fwd_ens_kernel<false>, PE);
+    } else {
+      ln.grid = dim3((B + kLnRows - 1) / kLnRows, E, R);
+      if (drop) push(std::move(ln), ln_bwd_ens_kernel<true>, PE);
+      else push(std::move(ln), ln_bwd_ens_kernel<false>, PE);
+    }
+  } else if (fwd) {
     ln.grid = dim3((2 * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
     if (drop) push(std::move(ln), ln_fwd_kernel<true>, P);
     else push(std::move(ln), ln_fwd_kernel<false>, P);
@@ -1737,7 +1781,7 @@ void PlanBuilder::critic_fwd(int pass, int l, std::vector<GemmProb> ps) {
   const CriticPass& cp = h->pass[pass];
   const bool ln = c.critic_ln != 0;
   const Buf& out = ln ? cp.z[l] : cp.h[l];
-  for (int net = 0; net < 2; ++net) {
+  for (int net = 0; net < E; ++net) {
     const LayerOff& lo = cp.net[net][l];
     const Buf x = critic_in(cp, net, l);
     GemmProb p = fwd_prob(par, x.p, x.rs, B, lo, netp(out, net, lo.out), out.rs);
@@ -1756,7 +1800,7 @@ void PlanBuilder::critic_bwd(int pass, int l, bool want_wgrad) {
   // (on the main stream: a forked weight gradient below waits for it like the input gradient does)
   if (c.critic_ln) layer_norm(pass, l, false, want_wgrad);
   std::vector<GemmProb> ps, dg;
-  for (int net = 0; net < 2; ++net) {
+  for (int net = 0; net < E; ++net) {
     const LayerOff& lo = cp.net[net][l];
     const Buf x = critic_in(cp, net, l), dz{netp(h->dhQ[l], net, lo.out), h->dhQ[l].rs};
     if (want_wgrad) ps.push_back(wgrad_prob(grd, dz.p, dz.rs, x.p, x.rs, lo, B));
@@ -1769,7 +1813,7 @@ void PlanBuilder::critic_bwd(int pass, int l, bool want_wgrad) {
     branch = 1; gemm_launch(ps); branch = 0;
     gemm_launch(dg);
   } else {
-    ps.insert(ps.end(), dg.begin(), dg.end());      // {wgrad q1, wgrad q2, dgrad q1, dgrad q2}
+    ps.insert(ps.end(), dg.begin(), dg.end());      // {wgrad q1, wgrad q2, dgrad q1, dgrad q2}; ensembles: E of each
     gemm_launch(ps);
   }
 }
@@ -1833,7 +1877,19 @@ void PlanBuilder::build_plan_layered() {
     P.logp = h->logp.p; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
     P.y = h->y.p; P.q = h->q.p; P.dq = h->dq.p; P.lq = h->lq.p; P.rsY = h->y.rs;
-    push(std::move(l), critic_heads_kernel, P);
+    if (ens) {
+      CriticHeadEnsArgs Q;
+      memset(&Q, 0, sizeof(Q));
+      Q.hT = P.hT; Q.hQ = P.hQ; Q.rsHnet = P.rsHnet; Q.rsHrep = P.rsHrep; Q.ldh = P.ldh;
+      Q.Wt = P.Wt[0]; Q.bt = P.bt[0]; Q.Wq = P.Wq[0]; Q.bq = P.bq[0]; Q.rsNet = rsNet; Q.rsP = rsP;
+      Q.r = P.r; Q.d = P.d; Q.tid = P.tid; Q.rsR = P.rsR;
+      Q.logp = P.logp; Q.rsLogp = P.rsLogp; Q.log_alpha = P.log_alpha;
+      Q.y = P.y; Q.q = P.q; Q.dq = P.dq; Q.lq = P.lq; Q.rsY = P.rsY;
+      Q.ens = h->ens.dev; Q.tsub = h->tsub.p; Q.rsTsub = h->tsub.rs; Q.E = E;
+      push(std::move(l), critic_heads_ens_kernel, Q);
+    } else {
+      push(std::move(l), critic_heads_kernel, P);
+    }
   }
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
@@ -1952,7 +2008,18 @@ void PlanBuilder::build_plan_layered() {
     P.logp = h->logp.p + B; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
     P.dqa = h->dqa.p; P.la = h->la.p; P.qmin = h->qmin.p; P.rsY = h->y.rs;
-    push(std::move(l), actor_q_heads_kernel, P);
+    if (ens) {
+      ActorQHeadEnsArgs Q;
+      memset(&Q, 0, sizeof(Q));
+      Q.hP = P.hP; Q.rsHnet = P.rsHnet; Q.rsHrep = P.rsHrep; Q.ldh = P.ldh;
+      Q.Wq = P.Wq[0]; Q.bq = P.bq[0]; Q.rsNet = rsNet; Q.rsP = rsP;
+      Q.tid = P.tid; Q.rsR = P.rsR; Q.logp = P.logp; Q.rsLogp = P.rsLogp; Q.log_alpha = P.log_alpha;
+      Q.dqa = P.dqa; Q.qp = h->qp.p; Q.la = P.la; Q.qmin = P.qmin; Q.rsY = P.rsY;
+      Q.ens = h->ens.dev; Q.E = E;
+      push(std::move(l), actor_q_heads_ens_kernel, Q);
+    } else {
+      push(std::move(l), actor_q_heads_kernel, P);
+    }
   }
   head_bwd(false, false);
   for (int l = Lc - 1; l >= 0; --l) critic_bwd(PASS_P, l, false);
@@ -2253,9 +2320,10 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   slab.request(h->act_out, (size_t)2 * B * A);
   for (Buf* b : {&h->logp, &h->logstd}) slab.request(*b, nLogp);
   for (Buf* b : {&h->y, &h->lq, &h->la, &h->qmin}) slab.request(*b, rsB);
-  for (Buf* b : {&h->q, &h->dq, &h->dqa, &h->qt, &h->qp}) slab.request(*b, 2 * rsB);
+  const int E = h->E = cfg->critic_ensemble ? cfg->critic_ensemble : 2;
+  for (Buf* b : {&h->q, &h->dq, &h->dqa, &h->qt, &h->qp}) slab.request(*b, E * rsB);
   slab.request(h->alpha, 64);
-  slab.request(h->dxP, (size_t)2 * B * ldx);
+  slab.request(h->dxP, (size_t)E * B * ldx);
   for (Buf* b : {&h->dout_dbg, &h->dact_dbg}) slab.request(*b, nDbg);
   h->hA.resize(La); h->dhA.resize(La);
   for (int l = 0; l < La; ++l) {
@@ -2265,8 +2333,8 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
   for (CriticPass& p : h->pass) p.h.resize(Lc);
   h->dhQ.resize(Lc);
   for (int l = 0; l < Lc; ++l) {
-    for (CriticPass& p : h->pass) slab.request(p.h[l], (size_t)2 * B * cfg->critic_hidden[l]);
-    slab.request(h->dhQ[l], (size_t)2 * B * cfg->critic_hidden[l]);
+    for (CriticPass& p : h->pass) slab.request(p.h[l], (size_t)E * B * cfg->critic_hidden[l]);
+    slab.request(h->dhQ[l], (size_t)E * B * cfg->critic_hidden[l]);
   }
   if (cfg->care) {
     const int Kenc = cfg->num_encoders, T = cfg->num_tasks;
@@ -2303,20 +2371,25 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     for (CriticPass& p : h->pass) p.z.resize(Lc);
     int maxH = 0;
     for (int l = 0; l < Lc; ++l) {
-      for (CriticPass& p : h->pass) slab.request(p.z[l], (size_t)2 * B * cfg->critic_hidden[l]);
+      for (CriticPass& p : h->pass) slab.request(p.z[l], (size_t)E * B * cfg->critic_hidden[l]);
       maxH = std::max(maxH, cfg->critic_hidden[l]);
     }
     const size_t chunks = (size_t)(B + kLnRows - 1) / kLnRows;
-    CU(dev_alloc(h->ln_part, R * 2 * chunks * 2 * maxH));
-    CU(dev_fill(h->ln_ticket, (size_t)R * 2, 0));
+    CU(dev_alloc(h->ln_part, R * E * chunks * 2 * maxH));
+    CU(dev_fill(h->ln_ticket, (size_t)R * E, 0));
   }
   if (cfg->critic_dropout) {  // rate 0 on every replica; masks all zero until a step draws them
     for (CriticPass& p : h->pass) {
       p.m.resize(Lc);
-      for (int l = 0; l < Lc; ++l) slab.request(p.m[l], (size_t)2 * B * ((cfg->critic_hidden[l] + 31) / 32));
+      for (int l = 0; l < Lc; ++l) slab.request(p.m[l], (size_t)E * B * ((cfg->critic_hidden[l] + 31) / 32));
     }
     const double p0 = 0.0;
     if (int rc = h->drop.init(R, &p0)) return rc;
+  }
+  if (cfg->critic_ensemble) {  // REDQ's and RLPD's defaults: a subset of 2, the mean over the ensemble for the actor
+    slab.request(h->tsub, E);
+    const int e0[2] = {2, 1};
+    if (int rc = h->ens.init(R, e0)) return rc;
   }
   if (int rc = slab.allocate(h->slab)) return rc;
 
@@ -2610,6 +2683,25 @@ extern "C" int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double 
   return h->drop.set(h, stream, replica, &p);
 }
 
+// Target subset size and actor reduction of an ensemble handle, read by its head launches.
+extern "C" int b200sac_get_ensemble(b200sac_t* h, int32_t replica, int32_t* m, int32_t* actor_mean) {
+  if (!h || !m || !actor_mean) return fail(B200SAC_ERR_INVALID, "null argument");
+  if (int rc = need_feature(h->cfg.critic_ensemble, "critic_ensemble")) return rc;
+  if (int rc = h->ens.check(replica)) return rc;
+  *m = h->ens.row(replica)[0]; *actor_mean = h->ens.row(replica)[1];
+  return 0;
+}
+
+extern "C" int b200sac_set_ensemble(b200sac_t* h, int32_t replica, int32_t m, int32_t actor_mean, void* stream) {
+  if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
+  if (int rc = need_feature(h->cfg.critic_ensemble, "critic_ensemble")) return rc;
+  if (int rc = h->ens.check(replica)) return rc;
+  if (m < 1 || m > h->E) return fail(B200SAC_ERR_INVALID, "the target subset size must be in [1, %d], got %d", h->E, m);
+  if (actor_mean != 0 && actor_mean != 1) return fail(B200SAC_ERR_INVALID, "actor_mean must be 0 (min) or 1 (mean), got %d", actor_mean);
+  const int row[2] = {m, actor_mean};
+  return h->ens.set(h, stream, replica, row);
+}
+
 // Gradient-surgery switches, read by the pcgrad launches of the step graphs.
 extern "C" int b200sac_get_pcgrad(b200sac_t* h, int32_t replica, int32_t* critic_on, int32_t* actor_on) {
   if (!h || !critic_on || !actor_on) return fail(B200SAC_ERR_INVALID, "null argument");
@@ -2761,19 +2853,22 @@ extern "C" int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_
   A.target_delta = L.target_delta;
   A.key = seed + (uint64_t)replica;
   for (int p = 0; p < B200SAC_RESET_PARTS; ++p) A.shrink[p] = spec->part[p].shrink;
-  int n = 0;
+  // the touched tensors, kResetMaxTensors per launch (critic ensembles can have more)
+  std::vector<ResetTensor> ts;
   long long widest = 0;
   for (const InitTensor& t : init_table(&c, L)) {
     if (t.part < 0) continue;
     const int layers = spec->part[t.part].layers;
     if (layers == 0 || t.depth > layers) continue;
-    if (n == kResetMaxTensors) return fail(B200SAC_ERR_INVALID, "more than %d tensors to reset", kResetMaxTensors);
-    ResetTensor& r = A.t[n++];
+    ResetTensor r;
+    memset(&r, 0, sizeof(r));
     r.off = t.off; r.rows = t.rows; r.cols = t.cols; r.ld = t.ld;
     r.kind = (unsigned char)t.kind; r.part = (unsigned char)t.part; r.target = t.target ? 1 : 0;
     r.tag = t.tag; r.c0 = t.kind == RESET_ONES ? 1.0f : (float)c.log_alpha_init;
     widest = std::max(widest, (long long)t.rows * t.cols);
+    ts.push_back(r);
   }
+  const int n = (int)ts.size();
   // optimizers that own a touched tensor: {counter slot, first trainable float, floats}
   struct Owner { int slot; int64_t begin, n; };
   std::vector<Owner> owners;
@@ -2788,8 +2883,12 @@ extern "C" int b200sac_reset(b200sac_t* h, int32_t replica, const b200sac_reset_
   StreamBridge sb(h, stream);
   if (int rc = sb.begin()) return rc;
   const unsigned bx = (unsigned)std::min<long long>(64, (widest + 255) / 256);
-  reset_kernel<<<dim3(bx, n), 256, 0, sb.run>>>(A);
-  CU(cudaGetLastError());
+  for (int i0 = 0; i0 < n; i0 += kResetMaxTensors) {
+    const int k = std::min(n - i0, kResetMaxTensors);
+    std::copy(ts.begin() + i0, ts.begin() + i0 + k, A.t);
+    reset_kernel<<<dim3(bx, k), 256, 0, sb.run>>>(A);
+    CU(cudaGetLastError());
+  }
   int slots = 0;
   const size_t nt = (size_t)L.trainable;
   for (const Owner& o : owners) {
@@ -3460,6 +3559,7 @@ extern "C" int b200sac_redo(b200sac_t* h, int32_t replica, int32_t n, const floa
   if (!h || !obs || !act) return fail(B200SAC_ERR_INVALID, "null argument");
   if (h->cfg.critic_ln)     // its forward has no LayerNorm, and one recycled unit would move its whole row's statistics
     return fail(B200SAC_ERR_STATE, "ReDo does not run on a handle created with critic_ln");
+  if (h->cfg.critic_ensemble) return fail(B200SAC_ERR_STATE, "ReDo does not run on a handle created with critic_ensemble");
   if (int rc = check_replica(h, replica)) return rc;
   const b200sac_cfg& c = h->cfg;
   const int B = c.batch, A = c.act_dim, La = c.n_actor_hidden, Lc = c.n_critic_hidden;
@@ -3560,10 +3660,11 @@ static long long eval_carve(const b200sac* h, long long n, float* base) {
   for (int l = 0; l < c.n_critic_hidden; ++l) Hc = std::max(Hc, c.critic_hidden[l]);
   for (int l = 0; l < c.n_actor_hidden; ++l) Ha = std::max(Ha, c.actor_hidden[l]);
   EvalScratch& E = const_cast<b200sac*>(h)->ev;
+  const int nets = h->E;
   const std::pair<void**, long long> rowbufs[] = {
-      {(void**)&E.XQ, h->K.ldx}, {(void**)&E.XT, h->K.ldx}, {(void**)&E.hc[0], 2 * Hc}, {(void**)&E.hc[1], 2 * Hc},
-      {(void**)&E.z, c.critic_ln ? 2 * Hc : 0}, {(void**)&E.ha[0], Ha}, {(void**)&E.ha[1], Ha}, {(void**)&E.q, 2},
-      {(void**)&E.qt, 2}, {(void**)&E.pout, 2 * A}, {(void**)&E.psave, A * kSaveW}, {(void**)&E.act, A},
+      {(void**)&E.XQ, h->K.ldx}, {(void**)&E.XT, h->K.ldx}, {(void**)&E.hc[0], nets * Hc}, {(void**)&E.hc[1], nets * Hc},
+      {(void**)&E.z, c.critic_ln ? nets * Hc : 0}, {(void**)&E.ha[0], Ha}, {(void**)&E.ha[1], Ha}, {(void**)&E.q, nets},
+      {(void**)&E.qt, nets}, {(void**)&E.pout, 2 * A}, {(void**)&E.psave, A * kSaveW}, {(void**)&E.act, A},
       {(void**)&E.logp, 1}, {(void**)&E.logstd, 1}, {(void**)&E.eps, A}, {(void**)&E.R, 1}, {(void**)&E.d, 1},
       {(void**)&E.g, 1}, {(void**)&E.task, 1}, {(void**)&E.idx, 2}};
   if (n == 0) {
@@ -3602,8 +3703,8 @@ static int eval_alloc(b200sac* h) {
   return 0;
 }
 
-// Q of nets[0] and nets[1] (L.q: q1 and q2; L.qt: their targets) of replica `rep` on n <= E.rows rows X [n][ldx] into
-// out [2][n], in eval mode: b200sac_act's per-layer gemm_simt_kernel and, on critic_ln handles, ln_fwd_kernel<false> between
+// Q of nets[0] and nets[1] (L.q: q1 and q2; L.qt: their targets; nets[0 .. E) on a critic_ensemble handle) of replica
+// `rep` on n <= E.rows rows X [n][ldx] into out [2][n] ([E][n]), in eval mode: b200sac_act's per-layer gemm_simt_kernel and, on critic_ln handles, ln_fwd_kernel<false> between
 // each hidden GEMM and its ReLU (no dropout, whatever the replica's rate).  Each output row depends on its input row alone.
 static void eval_critics(b200sac* h, cudaStream_t st, int rep, const std::vector<LayerOff>* nets, const float* X, int n, float* out) {
   const EvalScratch& E = h->ev;
@@ -3612,7 +3713,7 @@ static void eval_critics(b200sac* h, cudaStream_t st, int rep, const std::vector
   const bool ln = h->cfg.critic_ln != 0;
   for (int l = 0; l <= Lc; ++l) {
     std::vector<GemmProb> ps;
-    for (int net = 0; net < 2; ++net) {
+    for (int net = 0; net < h->E; ++net) {
       const LayerOff& lo = nets[net][l];
       const float* in = l == 0 ? X : E.hc[(l - 1) & 1] + (long long)net * n * lo.in;
       float* o = l == Lc ? out + (long long)net * n : (ln ? E.z : E.hc[l & 1]) + (long long)net * n * lo.out;
@@ -3628,6 +3729,11 @@ static void eval_critics(b200sac* h, cudaStream_t st, int rep, const std::vector
       P.z = E.z; P.h = E.hc[l & 1];
       for (int net = 0; net < 2; ++net) { P.g[net] = par.p + nets[net][l].g; P.c[net] = par.p + nets[net][l].c; }
       P.B = n; P.H = nets[0][l].out;
+      if (h->cfg.critic_ensemble) {
+        const LnEnsArgs PE{P, nets[1][l].g - nets[0][l].g, h->E};
+        ln_fwd_ens_kernel<false><<<dim3((h->E * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, PE);
+        continue;
+      }
       ln_fwd_kernel<false><<<dim3((2 * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, P);
     }
   }
@@ -3662,7 +3768,7 @@ extern "C" int b200sac_critic_values(b200sac_t* h, int32_t replica, int64_t n, c
                          cudaMemcpyDefault, st));
     eval_critics(h, st, replica, which ? h->L.qt : h->L.q, E.XQ, m, E.q);
     CU(cudaGetLastError());
-    for (int net = 0; net < 2; ++net)
+    for (int net = 0; net < h->E; ++net)
       CU(cudaMemcpyAsync(q_out + net * n + i0, E.q + (long long)net * m, (size_t)m * sizeof(float), cudaMemcpyDefault, st));
   }
   if (int rc = sb.end()) return rc;
@@ -3685,12 +3791,12 @@ extern "C" int b200sac_soft_update(b200sac_t* h, double tau, void* stream) {
 
 extern "C" int b200sac_soft_update_critic(b200sac_t* h, int32_t critic, double tau, void* stream) {
   if (!h) return fail(B200SAC_ERR_INVALID, "null handle");
-  if (critic != 1 && critic != 2) return fail(B200SAC_ERR_INVALID, "critic must be 1 or 2, got %d", critic);
+  if (critic < 1 || critic > h->E) return fail(B200SAC_ERR_INVALID, "critic must be in [1, %d], got %d", h->E, critic);
   CU(cudaSetDevice(h->device));
-  // q1 and q2 are each contiguous in [critic_begin, cse_begin), q2 right behind q1; their targets sit at + target_delta
+  // q1, q2 (.. qE) are each contiguous in [critic_begin, cse_begin), each right behind the one before; their targets sit at
+  // + target_delta
   const Layout& L = h->L;
-  const int64_t q2_begin = L.q[1][0].w;
-  const int64_t beg = critic == 1 ? L.critic_begin : q2_begin, end = critic == 1 ? q2_begin : L.cse_begin;
+  const int64_t beg = L.q[critic - 1][0].w, end = critic < h->E ? L.q[critic][0].w : L.cse_begin;
   polyak_kernel<<<dim3(128, h->R), 256, 0, (cudaStream_t)stream>>>(h->params + beg, L.arena, end - beg, L.target_delta,
                                                                   (float)tau, (float)(1.0 - tau));
   CU(cudaGetLastError());
@@ -3709,6 +3815,9 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   if (nm == "y") { src = h->y.p + replica * h->y.rs; n = B; }
   else if (nm == "q1") { src = h->q.p + replica * h->q.rs; n = B; }
   else if (nm == "q2") { src = h->q.p + replica * h->q.rs + B; n = B; }
+  else if (int k = 0; h->cfg.critic_ensemble && sscanf(name, "q%d", &k) == 1 && nm == "q" + std::to_string(k) && k >= 1 && k <= h->E) {
+    src = h->q.p + replica * h->q.rs + (int64_t)(k - 1) * B; n = B;
+  }
   else if (nm == "a_next") { src = h->act_out.p + replica * h->act_out.rs; n = (int64_t)B * A; }
   else if (nm == "a_cur") { src = h->act_out.p + replica * h->act_out.rs + (int64_t)B * A; n = (int64_t)B * A; }
   else if (nm == "logp_next") { src = h->logp.p + replica * h->logp.rs; n = B; }
@@ -3716,8 +3825,12 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
   else if (nm == "r") { src = h->r.p + replica * h->r.rs; n = B; }
   else if (nm == "d") { src = h->d.p + replica * h->d.rs; n = B; }
   else if (nm == "qmin") { src = h->qmin.p + replica * h->qmin.rs; n = B; }
-  else if (nm == "q_pi") { src = h->qp.p + replica * 2 * h->y.rs; n = 2 * B; }        // [2][B]: Q1, Q2 at (s, a~) (actor pass)
-  else if (nm == "dq_pi") { src = h->dqa.p + replica * 2 * h->y.rs; n = 2 * B; }      // [2][B]: d(actor loss)/dQk -- the min routing
+  else if (nm == "q_pi") { src = h->qp.p + replica * h->E * h->y.rs; n = h->E * B; }        // [2][B]: Q1, Q2 at (s, a~) (actor pass); [E][B]
+  else if (nm == "dq_pi") { src = h->dqa.p + replica * h->E * h->y.rs; n = h->E * B; }      // [2][B]: d(actor loss)/dQk -- the min routing; [E][B]
+  else if (nm == "tsub") {                                  // critic_ensemble: [E] the last step's target subset as 0 / 1
+    if (!h->cfg.critic_ensemble) return fail(B200SAC_ERR_INVALID, "'tsub' needs a handle created with critic_ensemble");
+    src = h->tsub.p + replica * h->tsub.rs; n = h->E;
+  }
   else if (nm == "d_action") { src = h->dact_dbg.p + replica * h->dact_dbg.rs; n = (int64_t)B * A; }
   else if (nm == "d_head") { src = h->dout_dbg.p + replica * h->dout_dbg.rs; n = (int64_t)B * 2 * A; }
   else if (nm == "head") { src = h->pout.p + replica * h->pout.rs; n = (int64_t)2 * B * 2 * A; }      // [2B][2A]: mu | raw log-std
@@ -3769,16 +3882,16 @@ extern "C" int b200sac_debug_read(b200sac_t* h, const char* name, int32_t replic
       const std::vector<Buf>& v = kind[0] == 'h' ? cp->h : (kind[0] == 'z' ? cp->z : cp->m);
       if (l < 0 || l >= (int)v.size()) return fail(B200SAC_ERR_INVALID, "no such tensor '%s'", name);
       const int H = h->cfg.critic_hidden[l];
-      n = (int64_t)2 * B * H;
+      n = (int64_t)h->E * B * H;
       if (kind[0] == 'm') {
         if (n_floats) *n_floats = n;
         if (cap_floats < n) return fail(B200SAC_ERR_INVALID, "buffer too small: need %lld floats", (long long)n);
         const int words = (H + 31) / 32;
-        std::vector<uint32_t> bits((size_t)2 * B * words);
+        std::vector<uint32_t> bits((size_t)h->E * B * words);
         CU(cudaMemcpyAsync(bits.data(), v[l].p + replica * v[l].rs, bits.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost,
                            (cudaStream_t)stream));
         CU(cudaStreamSynchronize((cudaStream_t)stream));
-        for (int64_t row = 0; row < 2 * B; ++row)
+        for (int64_t row = 0; row < (int64_t)h->E * B; ++row)
           for (int j = 0; j < H; ++j) out_host[row * H + j] = (float)((bits[row * words + j / 32] >> (j % 32)) & 1u);
         return 0;
       }
@@ -4227,6 +4340,8 @@ extern "C" int b200sac_replay_create_prioritized(b200sac_t* h, int64_t capacity,
                                                  double eps, b200sac_replay_t** out) {
   if (!h || !out) return fail(B200SAC_ERR_INVALID, "null argument");
   *out = nullptr;
+  if (h->cfg.critic_ensemble)
+    return fail(B200SAC_ERR_INVALID, "prioritized replay is not available on a handle created with critic_ensemble");
   if (!(alpha >= 0.0) || !std::isfinite(alpha)) return fail(B200SAC_ERR_INVALID, "prioritized replay: alpha must be finite and >= 0 (got %g)", alpha);
   if (!(beta >= 0.0 && beta <= 1.0)) return fail(B200SAC_ERR_INVALID, "prioritized replay: beta must be in [0, 1] (got %g)", beta);
   if (!(eps > 0.0) || !std::isfinite(eps)) return fail(B200SAC_ERR_INVALID, "prioritized replay: eps must be finite and > 0 (got %g)", eps);

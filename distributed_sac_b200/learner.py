@@ -19,6 +19,7 @@ if none is given and `redis` is importable it connects to localhost like the ref
 import itertools
 import json
 import math
+import re
 import os
 import pickle as _pickle
 import time
@@ -28,7 +29,7 @@ import numpy as np
 import torch
 
 from . import _lib, names
-from .core import REDO_NETS, CoreConfig, Replay, SacCore, redo_taus, reset_spec
+from .core import ENSEMBLE_ACTOR, REDO_NETS, CoreConfig, Replay, SacCore, redo_taus, reset_spec
 from .replay_buffer import ReplayBuffer, MTReplayBuffer
 
 
@@ -83,12 +84,15 @@ class _BaseLearner:
     _iteration_key = "episode_idx"
     _pcgrad_ok = False          # PCGrad and CAGrad need task-block minibatches: the multi-task learners (MTSAC and CARE)
     _critic_ln_ok = True        # LayerNorm in the critics' hidden layers: the plain-MLP critics (not CARE's)
+    critic_ensemble = None      # E critics (critic_ensemble=E), None: the twins; target_subset and actor_q go with it
+    target_subset, actor_q = 2, "mean"
 
     # ---- construction ---------------------------------------------------------------------
     def _init_common(self, cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed,
                      replay_where, precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1,
                      n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                     redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None):
+                     redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None,
+                     critic_ensemble=None, target_subset=2, actor_q="mean"):
         self.critic_layer_norm = bool(critic_layer_norm)
         # DroQ (Hiraoka et al. 2022): dropout at rate p before every critic LayerNorm; it needs the LayerNorm critics
         if critic_dropout is not None:
@@ -150,6 +154,7 @@ class _BaseLearner:
             if redo is not None or redo_interval is not None:
                 raise ValueError("critic_layer_norm=True and redo= / redo_interval= are exclusive (recycling a unit would "
                                  "change its LayerNorm row's statistics, so it would not preserve the network's function)")
+        self._check_ensemble(critic_ensemble, target_subset, actor_q, prioritized, redo, redo_interval)
         if self.pcgrad and not (self._pcgrad_ok and self.num_tasks >= 2):
             raise ValueError(f"pcgrad=True needs a multi-task MTSAC or CARE learner with num_tasks >= 2 ({type(self).__name__}, "
                              f"num_tasks {self.num_tasks})")
@@ -202,6 +207,8 @@ class _BaseLearner:
             self.set_max_grad_norm(max_grad_norm)
         if self.critic_dropout is not None:
             self.core.set_critic_dropout(self.critic_dropout)
+        if self.critic_ensemble:
+            self.core.set_ensemble(self.target_subset, self.actor_q)
         if self.cagrad is not None:
             self.core.set_pcgrad(critic=False, actor=False)
             self.set_cagrad(self.cagrad)
@@ -216,6 +223,56 @@ class _BaseLearner:
         if checkpoint_path is not None:
             self.load_checkpoint(checkpoint_path)
             print("######## load checkpoint completely ########")
+
+    def _check_ensemble(self, E, m, actor_q, prioritized, redo, redo_interval):
+        """critic_ensemble=E (None: the twin critics), target_subset=m and actor_q= checked before any handle is built.
+        Raises ValueError."""
+        self.critic_ensemble, self.target_subset, self.actor_q = None, 2, "mean"
+        if E is None:
+            return
+        if isinstance(E, bool) or not isinstance(E, (int, np.integer)) or not 2 <= E <= 10:
+            raise ValueError(f"critic_ensemble must be an int in [2, 10] (got {E!r})")
+        if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 1 <= m <= E:
+            raise ValueError(f"target_subset must be an int in [1, critic_ensemble = {E}] (got {m!r})")
+        if actor_q not in ENSEMBLE_ACTOR:
+            raise ValueError(f"actor_q must be 'mean' or 'min' (got {actor_q!r})")
+        if not self._critic_ln_ok:
+            raise ValueError(f"critic_ensemble= needs plain-MLP critics ({type(self).__name__} has CARE critics)")
+        if self.pcgrad or self.cagrad is not None:
+            raise ValueError("critic_ensemble= and pcgrad= / cagrad= are exclusive")
+        if redo is not None or redo_interval is not None:
+            raise ValueError("critic_ensemble= and redo= / redo_interval= are exclusive")
+        if prioritized is not None:
+            raise ValueError("critic_ensemble= and prioritized= are exclusive")
+        self.critic_ensemble, self.target_subset, self.actor_q = int(E), int(m), actor_q
+
+    @property
+    def n_critics(self) -> int:
+        """Q-functions of the learner: critic_ensemble, or 2 (the twins)."""
+        return self.critic_ensemble or 2
+
+    @property
+    def _critic_nets(self):
+        return tuple(f"q{k}" for k in range(1, self.n_critics + 1))
+
+    def set_ensemble(self, target_subset=None, actor_q=None):
+        """Target subset size m in [1, E] and the actor's reduction over the E critics ("mean" or "min"), effective from
+        the next update(); None keeps the current value.  The learner must have been built with critic_ensemble=."""
+        if not self.critic_ensemble:
+            raise ValueError("this learner was built without critic_ensemble=")
+        m = self.target_subset if target_subset is None else target_subset
+        a = self.actor_q if actor_q is None else actor_q
+        if isinstance(m, bool) or not isinstance(m, (int, np.integer)) or not 1 <= m <= self.critic_ensemble:
+            raise ValueError(f"target_subset must be an int in [1, {self.critic_ensemble}] (got {m!r})")
+        if a not in ENSEMBLE_ACTOR:
+            raise ValueError(f"actor_q must be 'mean' or 'min' (got {a!r})")
+        self.core.set_ensemble(int(m), a)
+        self.target_subset, self.actor_q = int(m), a
+
+    def _check_checkpoint_critics(self, present):
+        """present: the critic indices k a checkpoint holds.  A checkpoint of another ensemble size raises ValueError."""
+        if sorted(present) != list(range(1, self.n_critics + 1)):
+            raise ValueError(f"the checkpoint holds critics {sorted(present)}, this learner has {self.n_critics}")
 
     def set_per_beta(self, beta: float):
         """Importance-sampling exponent of the prioritized ring (annealing), effective from the next update()."""
@@ -288,7 +345,7 @@ class _BaseLearner:
                           action_scale=(self.action_bound[1] - self.action_bound[0]) / 2,
                           log_alpha_init=float(c["log_alpha"]), grad_clip=self.max_grad_norm is not None,
                           pcgrad=self.pcgrad or self.cagrad is not None, critic_layer_norm=self.critic_layer_norm,
-                          critic_dropout=self.critic_dropout is not None)
+                          critic_dropout=self.critic_dropout is not None, critic_ensemble=self.critic_ensemble or 0)
 
     # ---- reference method surface -------------------------------------------------------------
     def _chunks(self, n):
@@ -323,6 +380,8 @@ class _BaseLearner:
         """One SacCore.redo on a fresh reference-shaped draw from the ring (a prioritized ring's weights are ignored)."""
         if self.critic_layer_norm:
             raise ValueError("dormant-neuron recycling and scoring do not run on a learner with critic_layer_norm=True")
+        if self.critic_ensemble:
+            raise ValueError("dormant-neuron recycling and scoring do not run on a learner with critic_ensemble=")
         s, a = self.memory.sample()[:2]
         self.core.redo(seed, s, a, **taus)
 
@@ -366,7 +425,11 @@ class _BaseLearner:
 
     def q_values(self, states, actions, target=False):
         """(q1, q2), or their targets with target=True, on rows of states and actions: two (n, 1) tensors on the learner's
-        device, as Critic.forward returns them, in eval mode (no dropout)."""
+        device, as Critic.forward returns them, in eval mode (no dropout).  With critic_ensemble=E: one (E, n) tensor of
+        q1 .. qE (or their targets)."""
+        if self.critic_ensemble:
+            return self.core.critic_values(torch.as_tensor(states).to(self.device), torch.as_tensor(actions).to(self.device),
+                                           target=target)
         q1, q2 = self.core.critic_values(torch.as_tensor(states).to(self.device), torch.as_tensor(actions).to(self.device),
                                          target=target)
         return q1.reshape(-1, 1), q2.reshape(-1, 1)
@@ -424,7 +487,7 @@ class _BaseLearner:
         if local_model is None and target_model is None:
             self.core.soft_update(float(tau))
             return
-        pairs = {("q1", "q1_target"): 1, ("q2", "q2_target"): 2}
+        pairs = {(f"q{k}", f"q{k}_target"): k for k in range(1, self.n_critics + 1)}
         key = (getattr(local_model, "net", None), getattr(target_model, "net", None))
         if (key not in pairs or getattr(local_model, "_learner", None) is not self
                 or getattr(target_model, "_learner", None) is not self):
@@ -496,7 +559,7 @@ class _BaseLearner:
         na, nc = len(self.actor_hidden_dim) + 1, len(self.critic_hidden_dim) + 1
         if net == "actor":
             return names.actor_key_map(self.family, na)
-        which = 1 if "1" in net else 2
+        which = int(net.split("_")[0][1:])          # q<k> / q<k>_target
         return names.critic_key_map(self.family, nc, which, target="target" in net, layer_norm=self.critic_layer_norm,
                                     dropout=self.critic_dropout is not None)
 
@@ -559,7 +622,7 @@ class _BaseLearner:
         # (MS/learner.py:159,178; C10:180,202; C1:147,169)
         state = {self._iteration_key: episode_idx, "total_step": self.total_step}
         state.update(self._critic_checkpoint_entries(named))
-        state["critic_optimizer"] = self._adam_state_dict(self._canon(("q1", "q2")), self.lr_critic, sc)
+        state["critic_optimizer"] = self._adam_state_dict(self._canon(self._critic_nets), self.lr_critic, sc)
         state["actor"] = self._module_state_dict("actor", named=named)
         state["actor_optimizer"] = self._adam_state_dict(self._canon(("actor",)), self.lr_actor, sa)
         state["log_alpha"] = named["log_alpha"].clone()
@@ -577,7 +640,7 @@ class _BaseLearner:
         self._load_critic_checkpoint_entries(ck)
         self._load_module_state_dict("actor", ck["actor"])
         self.core.set_named({"log_alpha": ck["log_alpha"].detach().reshape(-1)}, strict=False)
-        self._load_adam(ck["critic_optimizer"], self._canon(("q1", "q2")), 0)
+        self._load_adam(ck["critic_optimizer"], self._canon(self._critic_nets), 0)
         self._load_adam(ck["actor_optimizer"], self._canon(("actor",)), 1)
         self._load_adam(ck["log_alpha_optimizer"], ["log_alpha"], 2)
         if "alpha" in ck:
@@ -635,17 +698,28 @@ class _BaseLearner:
 
 
 class _TwoCriticMixin:
-    """LL / VS: four separate Critic modules in the checkpoint."""
+    """LL / VS: separate Critic modules in the checkpoint, local_critic_k and target_critic_k for k = 1, 2 (1 .. E with
+    critic_ensemble=E)."""
+
+    def _critic_entries(self):
+        return [(f"{side}_critic_{k}", f"q{k}" + ("_target" if side == "target" else ""))
+                for side in ("local", "target") for k in range(1, self.n_critics + 1)]
 
     def _critic_checkpoint_entries(self, named):
-        return {k: self._module_state_dict(net, named=named) for k, net in
-                (("local_critic_1", "q1"), ("local_critic_2", "q2"), ("target_critic_1", "q1_target"),
-                 ("target_critic_2", "q2_target"))}
+        return {k: self._module_state_dict(net, named=named) for k, net in self._critic_entries()}
 
     def _load_critic_checkpoint_entries(self, ck):
-        for k, net in (("local_critic_1", "q1"), ("local_critic_2", "q2"), ("target_critic_1", "q1_target"),
-                       ("target_critic_2", "q2_target")):
+        self._check_checkpoint_critics({int(m.group(1)) for m in (re.fullmatch(r"local_critic_(\d+)", k) for k in ck) if m})
+        for k, net in self._critic_entries():
             self._load_module_state_dict(net, ck[k])
+
+    def __getattr__(self, name):
+        # local_critic_k / target_critic_k for every critic k of an ensemble (1 and 2 are the properties below)
+        m = re.fullmatch(r"(local|target)_critic_(\d+)", name)
+        E = self.__dict__.get("critic_ensemble") or 2
+        if m and 1 <= int(m.group(2)) <= E:
+            return _Handle(self, f"q{m.group(2)}" + ("_target" if m.group(1) == "target" else ""))
+        raise AttributeError(name)
 
     @property
     def local_critic_1(self): return _Handle(self, "q1")
@@ -669,13 +743,14 @@ class LunarLanderLearner(_TwoCriticMixin, _BaseLearner):
                  checkpoint_path=None, *, server=None, device_index=0, seed=0, replay_where="host", buffer_size=None,
                  precision=1, prioritized=None, actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None,
                  pcgrad=False, cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None,
-                 critic_layer_norm=False, critic_dropout=None, prior=None):
+                 critic_layer_norm=False, critic_dropout=None, prior=None,
+                 critic_ensemble=None, target_subset=2, actor_q="mean"):
         self.update_delay, self.print_period = update_delay, print_period
         self._buffer_size_override = buffer_size
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
                           cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
-                          prior)
+                          prior, critic_ensemble=critic_ensemble, target_subset=target_subset, actor_q=actor_q)
 
     def _set_dims(self):
         c = self.cfg
@@ -700,11 +775,12 @@ class VSACLearner(_TwoCriticMixin, _BaseLearner):
     def __init__(self, cfg_path, write_mode=True, save_period=1000, checkpoint_path=None, *, server=None,
                  device_index=0, seed=0, replay_where="host", precision=1, prioritized=None, actor_update_interval=1,
                  target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False, cagrad=None, reset_interval=None, reset=None,
-                 redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None):
+                 redo_interval=None, redo=None, critic_layer_norm=False, critic_dropout=None, prior=None,
+                 critic_ensemble=None, target_subset=2, actor_q="mean"):
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
                           cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
-                          prior)
+                          prior, critic_ensemble=critic_ensemble, target_subset=target_subset, actor_q=actor_q)
 
     def _set_dims(self):
         c = self.cfg
@@ -733,12 +809,13 @@ class MTSACLearner(_BaseLearner):
                  *, server=None, device_index=0, seed=0, replay_where="host", precision=1, prioritized=None,
                  actor_update_interval=1, target_update_interval=1, n_step=1, max_grad_norm=None, pcgrad=False,
                  cagrad=None, reset_interval=None, reset=None, redo_interval=None, redo=None, critic_layer_norm=False,
-                 critic_dropout=None, prior=None):
+                 critic_dropout=None, prior=None,
+                 critic_ensemble=None, target_subset=2, actor_q="mean"):
         self.train_classes, self.train_tasks = train_classes, train_tasks
         self._init_common(cfg_path, write_mode, save_period, checkpoint_path, server, device_index, seed, replay_where,
                           precision, prioritized, actor_update_interval, target_update_interval, n_step, max_grad_norm, pcgrad,
                           cagrad, reset_interval, reset, redo_interval, redo, critic_layer_norm, critic_dropout,
-                          prior)
+                          prior, critic_ensemble=critic_ensemble, target_subset=target_subset, actor_q=actor_q)
 
     def _set_dims(self):
         c = self.cfg
@@ -760,12 +837,17 @@ class MTSACLearner(_BaseLearner):
                               core=self.core, where=where, prioritized=self.prioritized, n_step=self.n_step)
 
     def _critic_checkpoint_entries(self, named):
-        loc = {**self._module_state_dict("q1", named=named), **self._module_state_dict("q2", named=named)}
-        tgt = {**self._module_state_dict("q1_target", named=named), **self._module_state_dict("q2_target", named=named)}
+        # one Critic module holding Q_function_1 .. Q_function_E
+        loc, tgt = {}, {}
+        for q in self._critic_nets:
+            loc.update(self._module_state_dict(q, named=named))
+            tgt.update(self._module_state_dict(q + "_target", named=named))
         return {"local_critic": loc, "target_critic": tgt}
 
     def _load_critic_checkpoint_entries(self, ck):
-        for net in ("q1", "q2"):
+        if self._critic_ln_ok:                     # (CARE's Critic also holds its state encoder, keyed differently)
+            self._check_checkpoint_critics({int(m.group(1)) for m in (re.match(r"Q_function_(\d+)\.", k) for k in ck["local_critic"]) if m})
+        for net in self._critic_nets:
             self._load_module_state_dict(net, ck["local_critic"])
             self._load_module_state_dict(net + "_target", ck["target_critic"])
 

@@ -39,8 +39,8 @@ def actor_key_map(family: str, n_layers: int):
 
 def critic_key_map(family: str, n_layers: int, which: int, target: bool = False, layer_norm: bool = False,
                    dropout: bool = False):
-    """{reference key: canonical key} for Q-function `which` (1|2), in the canonical layout order; n_layers counts the
-    head.
+    """{reference key: canonical key} for Q-function `which` (1|2; 1 .. E on a critic ensemble), in the canonical layout
+    order; n_layers counts the head.
 
     LL/VS: keys of ONE Critic module (local_critic_{which});
     MS   : keys of the twin Critic module restricted to Q_function_{which}.

@@ -120,12 +120,17 @@ typedef struct b200sac_cfg {
   int32_t pcgrad;                    /* 0 = the default plan; 1 = the per-layer plan with PCGrad gradient surgery
                                         (b200sac_set_pcgrad), both switches on at create.  Needs num_tasks >= 2 and
                                         grad_clip = 0; MTSAC and CARE (care = 1 | 2) alike.  Fixed at create. */
+  int32_t critic_ensemble;           /* 0 = the twin critics q1, q2; E in [2, B200SAC_MAX_ENSEMBLE] = E critics q1 .. qE with
+                                        a per-replica target subset (b200sac_set_ensemble).  Fixed at create.  See "Critic
+                                        ensembles" below. */
   int32_t critic_ln;                 /* 0 = the default plan; 1 = LayerNorm in the critics' hidden layers.  Fixed at create.
                                         See "Layer-normalized critics" below. */
   int32_t critic_dropout;            /* 0 = the critic_ln plan; 1 = dropout before every critic LayerNorm (DroQ), the rate
                                         set per replica by b200sac_set_critic_dropout.  Needs critic_ln = 1.  Fixed at
                                         create.  See "Dropout Q-functions" below. */
 } b200sac_cfg;
+
+#define B200SAC_MAX_ENSEMBLE 10
 
 /* Layer-normalized critics (cfg.critic_ln = 1; Ba et al. 2016, as high-replay-ratio SAC uses it: DroQ, Lyle et al. 2023,
  * BRO).  Every hidden layer l of q1, q2, q1_target and q2_target, width H, is nn.Sequential(Linear, nn.LayerNorm(H,
@@ -183,6 +188,38 @@ typedef struct b200sac_cfg {
  * dropout, whatever the rate.
  * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_dropout outside {0, 1}, or 1 with
  * critic_ln = 0. */
+
+/* Critic ensembles (cfg.critic_ensemble = E in [2, 10]; REDQ, Chen et al., ICLR 2021; RLPD, Ball et al., ICML 2023).
+ * Networks: q1 .. qE and q1_target .. qE_target, all of the shape of q1.  q3 .. qE follow q2 in the trainable critic block
+ * and q3_target .. follow q2_target, so every critic k has its target at + target_delta and the critic Adam, the Polyak
+ * updates, b200sac_copy_replica, export / import and the critic gradient-clipping norm cover all E.  The Xavier tags of
+ * q3 .. qE come after q2's: actor, q1, q2, their targets and log_alpha are bit-identical to a twin handle created with
+ * the same seed.  critic_ln / critic_dropout parameters and masks follow per critic as for the twins.
+ * Per replica (b200sac_set_ensemble; m = 2 and MEAN at create): the subset size m in [1, E] and the actor reduction.
+ *   Critic loss: sum over k of the mean((y - Q_k)^2) terms with the twin plan's weighting; dL/dQ_k = 2 c (Q_k - y), with
+ *     the squared errors added in index order.
+ *   TD target: y = rs r + gamma (1 - d)(min_{k in S} Qt_k - alpha logpi'), the min folded with fminf in increasing index
+ *     order.  All E targets are evaluated; S holds m of them.
+ *   Subset S, one per replica and step (every row of the minibatch): m = E takes all E without a draw.  Otherwise
+ *     Philox4x32-10 with key = seed ^ (0x8EBC6AF09C88C6E3 * (replica + 1)) (mod 2^64; seed = b200sac_create's; a multiplier
+ *     no other draw uses) and counter (step & 0xFFFFFFFF, step >> 32, 0, q) gives words w_{4q} .. w_{4q+3}; S is the m
+ *     indices k with the smallest pairs (w_k, k).  step = the replica's step index the policy noise uses.  The draw does
+ *     not depend on the replica count and runs on critic-only steps too.  debug_read "tsub" [E] holds the last step's S
+ *     as 0.0 / 1.0.
+ *   Actor loss (the actor pass): MEAN: Q = (sum_k Q_k) / E, the sum in index order, each critic gets -c / E.  MIN: Q =
+ *     the fminf fold over all E; the gradient -c is split evenly among the critics equal to the minimum (torch.amin's
+ *     backward).  The action's input gradient adds the E critics' contributions in index order.
+ *   critic_dropout: the tag of critic k's masks is (pass * 8 + l) * E + k (the twin formula at E = 2).
+ * E = 2 with m = 2 and MIN computes exactly what the twin per-layer plan computes, bit for bit.
+ * Plan: always the per-layer plan (never the layer-chained one), at precision 0 and 1.  The extra critics are extra problems
+ * in the same grouped launches; a step has the launches and labels of the same cfg with critic_ensemble = 0 on the
+ * per-layer plan, plus any launch a grouped GEMM's GS_MAXG split adds.
+ * Entry points: b200sac_critic_values writes q_out[E][n]; b200sac_soft_update_critic takes critic in [1, E];
+ * b200sac_debug_read gains "q<k>" (k <= E) and "tsub", and "q_pi", "dq_pi" and the per-pass "h/z/m<pass>.<l>" hold E
+ * critics; b200sac_reset's CRITIC part re-draws all E with the same depth rule.
+ * Refused with B200SAC_ERR_INVALID by b200sac_layout and b200sac_create: critic_ensemble outside {0} and [2, 10], or with
+ * care != 0 or pcgrad = 1.  b200sac_redo gives B200SAC_ERR_STATE and b200sac_replay_create_prioritized B200SAC_ERR_INVALID
+ * on an ensemble handle. */
 
 typedef struct b200sac_tensor_desc {
   char name[48];                     /* canonical name, e.g. "q1_target.2.weight" */
@@ -382,6 +419,13 @@ int b200sac_get_grad_clip(b200sac_t* h, int32_t replica, double* critic, double*
  * the last accepted value (no synchronisation). */
 int b200sac_set_critic_dropout(b200sac_t* h, int32_t replica, double p, void* stream);
 int b200sac_get_critic_dropout(b200sac_t* h, int32_t replica, double* p);
+/* Target subset size m and actor reduction of one replica ("Critic ensembles" above): actor_mean = 1 takes the mean of the
+ * E critics, 0 their minimum.  Set: stream-ordered like b200sac_set_critic_dropout (prepared graphs read the new values
+ * without a rebuild; steps enqueued before the call do not).  m outside [1, E] or actor_mean outside {0, 1} give
+ * B200SAC_ERR_INVALID and change nothing; a handle created without critic_ensemble gives B200SAC_ERR_STATE.  Get reads the
+ * host mirror (no synchronisation).  Not copied by b200sac_copy_replica. */
+int b200sac_set_ensemble(b200sac_t* h, int32_t replica, int32_t m, int32_t actor_mean, void* stream);
+int b200sac_get_ensemble(b200sac_t* h, int32_t replica, int32_t* m, int32_t* actor_mean);
 /* Pre-clip gradient norms of the most recent `n_last` steps (<= 1024 kept, slots aligned with b200sac_read_losses):
  * out[n_last][replicas][3] = {critic, actor, context encoder}; NaN where that optimizer did not step (the actor on a
  * critic-only step, the context encoder outside CARE(O)).  Synchronises the stream. */
