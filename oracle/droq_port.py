@@ -25,10 +25,11 @@ TAGS = ("cur", "next", "pi")
 _masks = None        # {(net, tag, layer): float32 [B][H] of m * s} while _droq_mlp runs
 
 
-def step_masks(spec, seed, step, p, replica=0):
-    """{(net, tag, layer): bool [B][H]} of one step of one replica: the keep masks the CUDA step draws."""
-    return {(net, tag, l): torch.from_numpy(pr.drop_masks(seed, replica, step, tag, l, net, spec.batch, H, p))
-            for net in (0, 1) for tag in TAGS for l, H in enumerate(spec.critic_hidden)}
+def step_masks(spec, seed, step, p, replica=0, nets=2):
+    """{(net, tag, layer): bool [B][H]} of one step of one replica: the keep masks the CUDA step draws (nets = E: the
+    masks of a critic ensemble's E critics, keyed like oracle/redq_port.ensemble_dropout's)."""
+    return {(net, tag, l): torch.from_numpy(pr.drop_masks(seed, replica, step, tag, l, net, spec.batch, H, p, nets))
+            for net in range(nets) for tag in TAGS for l, H in enumerate(spec.critic_hidden)}
 
 
 def scaled(masks, p):

@@ -6,7 +6,8 @@ philox4x32 with 10 rounds): key (k0, k1) = the low and high 32 bits of the 64-bi
 
 drop_masks(...) is the keep mask of include/b200sac.h "Dropout Q-functions":
   key     = seed ^ (0xE7037ED1A0B428DB * (replica + 1)) mod 2^64;
-  counter = (step & 0xFFFFFFFF, step >> 32, row, (tag << 24) | (j // 4)),  tag = (pass * 8 + layer) * 2 + net;
+  counter = (step & 0xFFFFFFFF, step >> 32, row, (tag << 24) | (j // 4)),  tag = (pass * 8 + layer) * nets + net
+            (nets = 2 for the twin critics, E for a critic ensemble);
   keep    = word[j % 4] >= floor(p * 2^32).
 """
 import numpy as np
@@ -49,10 +50,11 @@ def scale(p):
     return np.float32(1.0 / (1.0 - float(p)))
 
 
-def drop_masks(seed, replica, step, pass_, layer, net, B, H, p):
-    """The keep mask [B][H] (bool) of one (step, replica, pass, layer, net); pass_ in {0, 1, 2} or "cur"/"next"/"pi"."""
+def drop_masks(seed, replica, step, pass_, layer, net, B, H, p, nets=2):
+    """The keep mask [B][H] (bool) of one (step, replica, pass, layer, net); pass_ in {0, 1, 2} or "cur"/"next"/"pi".
+    nets: the critics of the handle (2 for the twins, E for a critic ensemble), tag = (pass * 8 + layer) * nets + net."""
     pass_ = PASSES.get(pass_, pass_)
-    tag = (int(pass_) * 8 + int(layer)) * 2 + int(net)
+    tag = (int(pass_) * 8 + int(layer)) * int(nets) + int(net)
     j = np.arange(H)
     rows = np.arange(B, dtype=np.uint32)[:, None]
     step = int(step)

@@ -3,10 +3,12 @@
 oracle/sac_port.py's step with E critics q1 .. qE and their targets (include/b200sac.h "Critic ensembles"):
   y      = rs r + gamma (1 - d)(min over the step's subset S of Qt_k - alpha logpi'), S from oracle/redq_ref.py;
   L_Q    = sum_k mean((y - Q_k)^2) (/ B with weighted_loss);
-  actor  = mean((alpha logpi - Q)), Q = mean over the E critics ("mean") or torch.amin over them ("min").
+  actor  = mean((alpha logpi - Q)), Q = mean over the E critics ("mean") or torch.amin over them ("min"; amin_tagged lets
+         a test force the device's routing, tag "amin:pi").
 The critic Adam holds every tensor of q1 .. qE (LayerNorm weights included) and the Polyak update every target tensor.
 Networks run through sac_port.mlp, so critic_ln_port._layer_norm_mlp() gives the LayerNorm critics, and
-ensemble_dropout(masks, p) the DroQ critics with the masks of critic k keyed (k - 1, tag, layer).  At E = 2, m = 2 and "min" the step is sac_port's
+ensemble_dropout(masks, p) the DroQ critics with the masks of critic k keyed (k - 1, tag, layer); either way every critic
+ReLU is tagged "<net>:<pass>:<layer>", so sac_port.ReluTape can force the device's masks.  At E = 2, m = 2 and "min" the step is sac_port's
 (test_critic_ensemble_host.py checks it).
 """
 import contextlib
@@ -66,7 +68,7 @@ def ensemble_dropout(masks, p):
                 if g is not None:
                     x = x * scaled[(k, tag, i)]
                     x = F.layer_norm(x, (x.shape[-1],), g, params[f"{net}.{i}.ln.bias"], eps=lnp.EPS)
-                x = sp.relu_tagged(x, None)
+                x = sp.relu_tagged(x, None if tag is None else f"{net}:{tag}:{i}")
         return x
     saved = sp.mlp
     sp.mlp = mlp
@@ -74,6 +76,24 @@ def ensemble_dropout(masks, p):
         yield
     finally:
         sp.mlp = saved
+
+
+def amin_tagged(qn, tag):
+    """torch.amin(qn, 0) of the actor's "min" reduction over the E critics' Q [E][B][1], under sac_port's test hook (the
+    style of sac_port.min_tagged): which critics sit at the minimum routes the actor gradient, the step's discontinuity.
+    The tape records z = Q_k - min [E][B] (z == 0 <=> critic k is at the minimum) and, if `forced` holds a boolean mask
+    [E][B] for the tag, splits the row's gradient evenly over the critics the mask sets -- the library's rule, and
+    torch.amin's own among exactly tied values.  A row's value is then the mean of its forced critics' Q, which differs
+    from the minimum only where a forced critic is a near-tie (what check_forced asserts)."""
+    tape = sp.ReluTape.current
+    if tape is None or tag is None:
+        return qn.amin(0)
+    tape.z[tag] = (qn - qn.amin(0, keepdim=True)).detach().reshape(qn.shape[0], -1)
+    m = tape.forced.get(tag)
+    if m is None:
+        return qn.amin(0)
+    w = m.reshape(qn.shape).to(qn.dtype)
+    return (qn * w).sum(0) / w.sum(0)
 
 
 class RedqPortLearner(sp.PortLearner):
@@ -101,7 +121,23 @@ class RedqPortLearner(sp.PortLearner):
                                        "exp_avg": torch.as_tensor(st["m"][name]).clone().float(),
                                        "exp_avg_sq": torch.as_tensor(st["v"][name]).clone().float()}
 
-    def update_SAC(self, s, a, r, s2, d, eps_next, eps_cur):
+    def adam_state(self):
+        """{"m", "v", "step"} as load_adam takes it, over the actor, q1 .. qE (LayerNorm tensors included) and log_alpha."""
+        m, v = {}, {}
+        steps = {"critic": 0, "actor": 0, "alpha": 0}
+        for name in sp.param_names(self.spec, ("actor",), False) + self.critic_names + ["log_alpha"]:
+            which = "alpha" if name == "log_alpha" else ("actor" if name.startswith("actor.") else "critic")
+            st = self._opt_of(name).state.get(self.p[name], None)
+            if not st:
+                m[name], v[name] = torch.zeros_like(self.p[name].data), torch.zeros_like(self.p[name].data)
+            else:
+                m[name], v[name] = st["exp_avg"].clone(), st["exp_avg_sq"].clone()
+                steps[which] = int(st["step"])
+        return {"m": m, "v": v, "step": (steps["critic"], steps["actor"], steps["alpha"])}
+
+    def update_SAC(self, s, a, r, s2, d, eps_next, eps_cur, want_intermediates=False):
+        """One step; want_intermediates: the per-row outputs as tests/_harness.check_rows reads them, q1 .. qE included
+        (the actor-pass reduction as "qmin", d(actor loss)/d(action) summed over the critics as "d_action")."""
         spec, p, E = self.spec, self.p, self.E
         self.step += 1
         S = redq_ref.subset(self.seed, self.replica, self.step, E, self.m)
@@ -125,10 +161,13 @@ class RedqPortLearner(sp.PortLearner):
         self.grads = grad_of(self.critic_names)      # each optimizer's gradient, as Adam reads it
         self.opt_critic.step()
 
-        a_cur, logp, log_std = sp.policy_sample(spec, p, s, eps_cur, "cur")
+        keep = {} if want_intermediates else None
+        a_cur, logp, log_std = sp.policy_sample(spec, p, s, eps_cur, "cur", keep)
         xa = torch.cat([s, a_cur], -1)
+        if want_intermediates:
+            xa.retain_grad()
         qn = torch.stack([sp.mlp(p, q, xa, "pi") for q in nets(E)])
-        qred = qn.mean(0) if self.actor == "mean" else qn.amin(0)
+        qred = qn.mean(0) if self.actor == "mean" else amin_tagged(qn, "amin:pi")
         pi_loss = torch.mean(-(qred - alpha * logp)) / div
         pi_loss.backward()
         self.grads.update(grad_of(sp.param_names(spec, ("actor",), False)))
@@ -146,5 +185,10 @@ class RedqPortLearner(sp.PortLearner):
                 t, l = p[f"{q}_target.{rest}"], p[name]
                 t.copy_(spec.tau * l + (1.0 - spec.tau) * t)
         entropy = (0.5 * spec.act_dim * (1.0 + math.log(2 * math.pi)) + log_std.detach().sum(-1)).mean()
-        return {"critic_loss": q_loss.item(), "actor_loss": pi_loss.item(), "alpha_loss": alpha_loss.item(),
-                "entropy": entropy.item(), "y": y, "q": torch.stack([q.detach() for q in qs])}
+        out = {"critic_loss": q_loss.item(), "actor_loss": pi_loss.item(), "alpha_loss": alpha_loss.item(),
+               "entropy": entropy.item(), "y": y, "q": torch.stack([q.detach() for q in qs])}
+        if want_intermediates:
+            out.update({f"q{k + 1}": q.detach() for k, q in enumerate(qs)})
+            out.update(a_next=a2, logp_next=logp2, a_cur=a_cur.detach(), logp_cur=logp.detach(), qmin=qred.detach(),
+                       d_action=xa.grad[:, spec.obs_dim:].clone(), d_head=keep["head"].grad.clone())
+        return out

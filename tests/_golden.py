@@ -168,17 +168,19 @@ def sync_core_to_port(core, port, replica=0):
     core.set_steps(st["step"], replica)
 
 
-def cuda_relu_masks(core, spec, replica=0, care=False):
-    """{ReluTape tag: bool mask} from the activations the last CUDA step stored."""
+def cuda_relu_masks(core, spec, replica=0, care=False, E=2):
+    """{ReluTape tag: bool mask} from the activations the last CUDA step stored.  E: the critics of a critic_ensemble
+    handle, whose hQ / hP are [E][B][H]; with E > 2 the actor routing of a "min" replica is "amin:pi" [E][B] (critic k
+    took a share of the actor gradient: oracle/redq_port.amin_tagged), and a "mean" replica has none."""
     B = spec.batch
     masks = {}
     for l, H in enumerate(spec.actor_hidden):
         hA = core.debug(f"hA.{l}", replica).reshape(2 * B, H) > 0
         masks[f"actor:next:{l}"], masks[f"actor:cur:{l}"] = hA[:B], hA[B:]
     for l, H in enumerate(spec.critic_hidden):
-        hQ = core.debug(f"hQ.{l}", replica).reshape(2, B, H) > 0
-        hP = core.debug(f"hP.{l}", replica).reshape(2, B, H) > 0
-        for net in range(2):
+        hQ = core.debug(f"hQ.{l}", replica).reshape(E, B, H) > 0
+        hP = core.debug(f"hP.{l}", replica).reshape(E, B, H) > 0
+        for net in range(E):
             masks[f"q{net + 1}:cur:{l}"], masks[f"q{net + 1}:pi:{l}"] = hQ[net], hP[net]
     # saturated tanh: the policy head's own tanh(u) per (row, action) -- value + derivative forced into the oracle, which then
     # has to agree with it to the parity tolerance (sac_port.tanh_tagged; psave = [2B][A][8], entry 2 = tanh(u))
@@ -186,7 +188,10 @@ def cuda_relu_masks(core, spec, replica=0, care=False):
     masks["tanh:next"], masks["tanh:cur"] = t[:B].clone(), t[B:].clone()
     # the other discontinuity of the step: which twin min(Q1, Q2)(s, a~) routes the actor gradient to (tag "route:pi",
     # True = Q1).  Handled like a ReLU bit: forced into the oracle, and a differing bit must sit on |Q1 - Q2| ~ 0
-    masks["route:pi"] = (core.debug("dq_pi", replica).reshape(2, B)[0] != 0).reshape(B, 1)
+    if E == 2:
+        masks["route:pi"] = (core.debug("dq_pi", replica).reshape(2, B)[0] != 0).reshape(B, 1)
+    elif core.get_ensemble(replica)[1] == "min":
+        masks["amin:pi"] = core.debug("dq_pi", replica).reshape(E, B) != 0
     if care:
         K = spec.num_encoders
         for l, H in enumerate(spec.mix_hidden):
@@ -201,7 +206,8 @@ def cuda_relu_masks(core, spec, replica=0, care=False):
 
 def check_forced(tape, forced, what=""):
     """Every forced bit that differs from the oracle's own decision must sit on a numerically-zero pre-activation (a ReLU
-    kink / a tie of min(Q1,Q2)); every forced tanh value must agree with the oracle's own to the parity tolerance.
+    kink / a tie of min(Q1,Q2) / a critic within rounding of an ensemble's minimum, where the tape's z = Q_k - min and the
+    oracle's own bit is z <= 0); every forced tanh value must agree with the oracle's own to the parity tolerance.
     Returns {tag: differing bits}."""
     flips = {}
     for tag, m in forced.items():
@@ -210,7 +216,7 @@ def check_forced(tape, forced, what=""):
             worst = float((z - m.reshape(z.shape)).abs().max())
             assert worst <= REL, f"{what}tanh(u) of {tag} differs by {worst:.3e} > {REL}"
             continue
-        diff = (z > 0) != m
+        diff = ((z <= 0) if tag.startswith("amin:") else (z > 0)) != m
         n = int(diff.sum())
         if n:
             tol = REL * max(1.0, float(z.abs().mean()))
@@ -220,13 +226,14 @@ def check_forced(tape, forced, what=""):
     return flips
 
 
-def kink_checked_step(core, port, spec, batch, e1, e2, replica=0, care=False, step_cuda=None, want_intermediates=False):
+def kink_checked_step(core, port, spec, batch, e1, e2, replica=0, care=False, step_cuda=None, want_intermediates=False,
+                      E=2):
     """One step of `core` (from the port's state) and of `port` with the CUDA masks forced; returns (port outputs,
     {tag: flipped bits}).  Raises AssertionError if a flipped bit is not a kink.  want_intermediates: the port's outputs
-    include its per-row intermediates (computed with the forced masks)."""
+    include its per-row intermediates (computed with the forced masks).  E: the handle's critics (cuda_relu_masks)."""
     sync_core_to_port(core, port, replica)
     (step_cuda or (lambda: core.step(*batch, e1, e2)))()
-    forced = cuda_relu_masks(core, spec, replica, care)
+    forced = cuda_relu_masks(core, spec, replica, care, E)
     with sp.ReluTape(forced) as tape:
         out = (port.update if care else port.update_SAC)(*batch, e1, e2, want_intermediates=want_intermediates)
     flips = check_forced(tape, forced)

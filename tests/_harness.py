@@ -335,12 +335,12 @@ def check_losses(core, o, replica=0, what=""):
         assert rel_scalar(float(L[i]), o[k]) <= REL, f"{what}{k}: {float(L[i])} vs oracle {o[k]}"
 
 
-def check_active(core, spec, replica=0, what="", care=False):
-    """Every hidden layer of every network (actor on s' and s, Q1/Q2 on (s, a) and (s, a~); care: every mixture hidden
-    layer of all three encoder instances too) has between 5 % and 95 % active units in the CUDA step's own masks: a sweep
-    over dead or saturated layers would prove little."""
-    for tag, m in cuda_relu_masks(core, spec, replica, care).items():
-        if tag.startswith(("tanh:", "route:")):
+def check_active(core, spec, replica=0, what="", care=False, E=2):
+    """Every hidden layer of every network (actor on s' and s, Q1/Q2 -- or the E critics of an ensemble -- on (s, a) and
+    (s, a~); care: every mixture hidden layer of all three encoder instances too) has between 5 % and 95 % active units in
+    the CUDA step's own masks: a sweep over dead or saturated layers would prove little."""
+    for tag, m in cuda_relu_masks(core, spec, replica, care, E).items():
+        if tag.startswith(("tanh:", "route:", "amin:")):
             continue
         frac = float(m.float().mean())
         assert 0.05 <= frac <= 0.95, f"{what}hidden layer {tag}: {100 * frac:.1f}% active"
