@@ -39,7 +39,6 @@
 #include "redo_kernels.cuh"
 #include "ln_kernels.cuh"
 #include "eval_kernels.cuh"
-#include "ensemble_kernels.cuh"
 
 using namespace bsac;
 
@@ -378,9 +377,8 @@ typedef void (*TcKernel)(const TcProb*, const int*, int, int);
 struct TcCall { TcKernel kern; const TcProb* probs; const int* sched; int G, sched_stride; };
 using KernelCall = std::variant<StepFirst<PolicyDoutArgs>, StepFirst<PolicyHeadArgs>, StepFirst<CriticHeadArgs>,
                                 StepFirst<ActorQHeadArgs>, StepFirst<HeadBwdArgs>, StepFirst<AdamArgs>, StepFirst<PcgArgs>,
-                                StepFirst<GradNormArgs>, StepFirst<LnArgs>, StepFirst<CriticHeadEnsArgs>,
-                                StepFirst<ActorQHeadEnsArgs>, StepFirst<HeadBwdEnsArgs>, StepFirst<PolicyDoutEnsArgs>,
-                                StepFirst<LnEnsArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>, StepLast<WgradArgs>,
+                                StepFirst<GradNormArgs>, StepFirst<LnArgs>, StepLast<ChainArgs>, StepLast<Chain2Args>,
+                                StepLast<WgradArgs>,
                                 NoStep<CareTabArgs>, NoStep<CareMixArgs>, NoStep<CareMixFwdArgs>, NoStep<CareMixBwdArgs>,
                                 NoStep<CareTabReduceArgs>, NoStep<CareTabWgradArgs>, NoStep<GemmGroup>, TcCall>;
 template <class P> static KernelCall bind(void (*kern)(StepConst, P), const P& args) { return StepFirst<P>{kern, args}; }
@@ -536,8 +534,9 @@ struct b200sac {
   DevMem<unsigned> ln_ticket;
   // cfg.critic_dropout: [R] dropout rates p (host mirror) and their DropRate
   ReplicaTable<DropRate, 1, double> drop;
-  // critics per pass: cfg.critic_ensemble, or 2 (the twins).  Ensemble handles: [R][2] (target subset size m, actor
-  // reduction 1 = mean / 0 = min) and the last step's subset [R][E] as 0 / 1 (debug_read "tsub")
+  // critics per pass: cfg.critic_ensemble, or 2 (the twins).  [R][2] (target subset size m, actor reduction 1 = mean /
+  // 0 = min; the twins' is fixed at (2, min)) and the last step's subset [R][E] as 0 / 1 (debug_read "tsub" on ensemble
+  // handles)
   int E = 2;
   ReplicaTable<int, 2> ens;
   Buf tsub;
@@ -1023,10 +1022,9 @@ struct PlanBuilder {
   const int B, R, A, La, Lc, sms;
   const long long rsP, rsG;
   const Buf par, grd;       // parameter and gradient arenas
-  // critics per pass (2: the twins) and, on a critic_ensemble handle, the distance from one critic to the next in the
-  // parameter and gradient arenas (the critics share one layout and sit back to back)
+  // critics per pass (2: the twins) and the distance from one critic to the next in the parameter and gradient arenas
+  // (the critics share one layout and sit back to back)
   const int E;
-  const bool ens;
   const long long rsNet;
   int branch = 0;           // branch tag given to the launches gemm_launch creates
   // per-layer plan, FFMA back-end, plain SAC nets: a layer's weight gradient only feeds Adam, while its input gradient heads
@@ -1039,7 +1037,7 @@ struct PlanBuilder {
   explicit PlanBuilder(b200sac* hh)
       : h(hh), c(hh->cfg), L(hh->L), B(c.batch), R(hh->R), A(c.act_dim), La(c.n_actor_hidden), Lc(c.n_critic_hidden),
         sms(sm_count()), rsP(L.arena), rsG(L.trainable), par{hh->params, L.arena}, grd{hh->grads, L.trainable},
-        E(hh->E), ens(c.critic_ensemble != 0), rsNet(L.q[1][0].w - L.q[0][0].w), use_fork(c.precision == 0 && !c.care) {}
+        E(hh->E), rsNet(L.q[1][0].w - L.q[0][0].w), use_fork(c.precision == 0 && !c.care) {}
   float* W(int64_t off) const { return h->params + off; }
   float* Gp(int64_t off) const { return h->grads + off; }
   // network net's rows of a [2][B][H] ([E][B][H]) buffer
@@ -1288,14 +1286,12 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   memset(&P, 0, sizeof(P));
   P.actor_side = (policy || !want_wgrad) ? 1 : 0;       // the actor pass / the policy backward, not the critic update
   P.M = B;
-  P.rsP = rsP; P.rsG = rsG;
+  P.rsP = rsP; P.rsG = rsG; P.rsNet = rsNet; P.E = E;
   if (!policy) {
     P.NO = 1; P.Kdim = Hc; P.nets = E;
-    for (int net = 0; net < 2; ++net) {
-      P.W[net] = W(L.q[net][Lc].w);
-      P.dW[net] = want_wgrad ? Gp(L.q[net][Lc].w) : nullptr;
-      P.db[net] = want_wgrad ? Gp(L.q[net][Lc].b) : nullptr;
-    }
+    P.W = W(L.q[0][Lc].w);
+    P.dW = want_wgrad ? Gp(L.q[0][Lc].w) : nullptr;
+    P.db = want_wgrad ? Gp(L.q[0][Lc].b) : nullptr;
     const Buf& hb = h->pass[want_wgrad ? PASS_Q : PASS_P].h[Lc - 1];
     const Buf& dq = want_wgrad ? h->dq : h->dqa;
     P.dout = dq.p; P.rsDoutNet = B; P.rsDoutRep = E * h->y.rs;
@@ -1313,16 +1309,15 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
       Q.tid = (const int*)h->tid.p; Q.rsR = h->r.rs;
       Q.log_alpha = W(L.off_alpha); Q.rsP = rsP;
       Q.dout = h->dout_dbg.p; Q.dact = h->dact_dbg.p; Q.rsDout = h->dout_dbg.rs;
-      Q.M = B;
+      Q.M = B; Q.E = E;
       pl.grid = dim3((B * A + 255) / 256, R);
       pl.block = dim3(256);
-      if (ens) push(std::move(pl), policy_dout_ens_kernel, PolicyDoutEnsArgs{Q, E});
-      else push(std::move(pl), policy_dout_kernel, Q);
+      push(std::move(pl), policy_dout_kernel, Q);
     }
     P.NO = 2 * A; P.Kdim = Ha; P.nets = 1; P.policy_mode = split ? 0 : 1;
     if (split) { P.dout = h->dout_dbg.p; P.rsDoutNet = 0; P.rsDoutRep = h->dout_dbg.rs; }
     const LayerOff& lo = L.actor[La];
-    P.W[0] = W(lo.w); P.dW[0] = Gp(lo.w); P.db[0] = Gp(lo.b);
+    P.W = W(lo.w); P.dW = Gp(lo.w); P.db = Gp(lo.b);
     P.h = h->hA[La - 1].p + (long long)B * Ha; P.rsHrep = h->hA[La - 1].rs; P.ldh = Ha;   // rows B..2B-1 (= s half)
     P.dh = h->dhA[La - 1].p; P.rsDhRep = h->dhA[La - 1].rs; P.lddh = Ha;
     P.dx = h->dxP.p; P.rsDxNet = (long long)B * h->K.ldx; P.rsDxRep = h->dxP.rs; P.lddx = h->K.ldx;
@@ -1335,8 +1330,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
   // partial head-weight gradient in gradient slice s, exactly like the split-K GEMM weight gradients
   P.row_slices = h->gslices;
   P.xs = (long long)R * L.trainable;
-  for (int net = 0; net < std::min(P.nets, 2); ++net)     // (ensembles: critic k's slots follow critic 0's at + k * rsNet)
-    if (P.dW[net] && h->grads_x) { P.dWx[net] = h->grads_x + (P.dW[net] - h->grads); P.dbx[net] = h->grads_x + (P.db[net] - h->grads); }
+  if (P.dW && h->grads_x) { P.dWx = h->grads_x + (P.dW - h->grads); P.dbx = h->grads_x + (P.db - h->grads); }
   const int rows_per = (B + P.row_slices - 1) / P.row_slices;
   // 128-bit column mapping (head_bwd4_kernel) when every row pitch / tensor offset involved is a multiple of 4 floats --
   // for the scalar critic heads; the policy head (NO = 2 x act outputs, one network) would be left with 28 CTAs, too
@@ -1352,8 +1346,7 @@ void PlanBuilder::head_bwd(bool policy, bool want_wgrad) {
     rc = fail(B200SAC_ERR_INVALID, "batch * head width too large for head_bwd smem");
     return;
   }
-  if (ens) push(std::move(l), wide ? head_bwd4_ens_kernel : head_bwd_ens_kernel, HeadBwdEnsArgs{P, rsNet, E});
-  else push(std::move(l), wide ? head_bwd4_kernel<1> : head_bwd_kernel, P);
+  push(std::move(l), wide ? head_bwd4_kernel : head_bwd_kernel, P);
 }
 
 // the trainable slice of optimizer `which` (0 critic, 1 actor, 2 CARE(O) context encoder)
@@ -1719,7 +1712,7 @@ int PlanBuilder::build_plan_fused() {
   return 0;
 }
 
-// critic_ln handles: the LayerNorm of hidden layer l of both of pass `pass`'s networks over the [2][B][H]
+// critic_ln handles: the LayerNorm of hidden layer l of every network of pass `pass` over the [E][B][H]
 // pre-normalization buffer z[l], every replica in one launch.  Forward: h[l] = relu(LN(z[l])).  Backward: dhQ[l] becomes
 // the gradient at z[l] in place, and with want_grads the LayerNorm weight and bias gradients land in gradient slice 0 (the
 // split-K slices hold zeros there, so Adam's slice sum reads them unchanged).  critic_dropout handles run the dropout
@@ -1736,39 +1729,25 @@ void PlanBuilder::layer_norm(int pass, int l, bool fwd, bool want_grads) {
   const Buf& out = fwd ? cp.h[l] : h->dhQ[l];
   (fwd ? P.h : P.dh) = out.p;
   P.rsH = out.rs;
-  for (int net = 0; net < 2; ++net) {
-    const LayerOff& lo = cp.net[net][l];
-    P.g[net] = W(lo.g); P.c[net] = W(lo.c);
-    if (want_grads) { P.dg[net] = Gp(lo.g); P.dc[net] = Gp(lo.c); }
-  }
-  P.rsP = rsP; P.rsG = rsG;
+  const LayerOff& lo = cp.net[0][l];
+  P.g = W(lo.g); P.c = W(lo.c);
+  if (want_grads) { P.dg = Gp(lo.g); P.dc = Gp(lo.c); }
+  P.rsP = rsP; P.rsG = rsG; P.rsNet = rsNet;
   P.part = h->ln_part; P.ticket = h->ln_ticket;
-  P.B = B; P.H = H;
+  P.B = B; P.H = H; P.E = E;
   P.actor_side = actor_side ? 1 : 0;
   const bool drop = c.critic_dropout != 0;
   if (drop) {
     P.drop = h->drop.dev; P.mbits = (unsigned*)cp.m[l].p; P.rsM = cp.m[l].rs;
-    P.tag0 = (pass * 8 + l) * 2;
+    P.tag0 = (pass * 8 + l) * E;
   }
   ln.block = dim3(kLnThreads);
-  if (ens) {
-    if (drop) P.tag0 = (pass * 8 + l) * E;
-    const LnEnsArgs PE{P, rsNet, E};
-    if (fwd) {
-      ln.grid = dim3((E * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
-      if (drop) push(std::move(ln), ln_fwd_ens_kernel<true>, PE);
-      else push(std::move(ln), ln_fwd_ens_kernel<false>, PE);
-    } else {
-      ln.grid = dim3((B + kLnRows - 1) / kLnRows, E, R);
-      if (drop) push(std::move(ln), ln_bwd_ens_kernel<true>, PE);
-      else push(std::move(ln), ln_bwd_ens_kernel<false>, PE);
-    }
-  } else if (fwd) {
-    ln.grid = dim3((2 * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
+  if (fwd) {
+    ln.grid = dim3((E * B + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), R);
     if (drop) push(std::move(ln), ln_fwd_kernel<true>, P);
     else push(std::move(ln), ln_fwd_kernel<false>, P);
   } else {
-    ln.grid = dim3((B + kLnRows - 1) / kLnRows, 2, R);
+    ln.grid = dim3((B + kLnRows - 1) / kLnRows, E, R);
     if (drop) push(std::move(ln), ln_bwd_kernel<true>, P);
     else push(std::move(ln), ln_bwd_kernel<false>, P);
   }
@@ -1868,28 +1847,15 @@ void PlanBuilder::build_plan_layered() {
     memset(&P, 0, sizeof(P));
     const Buf &hT = h->pass[PASS_T].h[Lc - 1], &hQ = h->pass[PASS_Q].h[Lc - 1];
     P.hT = hT.p; P.hQ = hQ.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hT.rs; P.ldh = Hc;
-    for (int net = 0; net < 2; ++net) {
-      P.Wt[net] = W(L.qt[net][Lc].w); P.bt[net] = W(L.qt[net][Lc].b);
-      P.Wq[net] = W(L.q[net][Lc].w); P.bq[net] = W(L.q[net][Lc].b);
-    }
-    P.rsP = rsP;
+    P.Wt = W(L.qt[0][Lc].w); P.bt = W(L.qt[0][Lc].b);
+    P.Wq = W(L.q[0][Lc].w); P.bq = W(L.q[0][Lc].b);
+    P.rsNet = rsNet; P.rsP = rsP;
     P.r = h->r.p; P.d = h->d.p; P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
     P.logp = h->logp.p; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
     P.y = h->y.p; P.q = h->q.p; P.dq = h->dq.p; P.lq = h->lq.p; P.rsY = h->y.rs;
-    if (ens) {
-      CriticHeadEnsArgs Q;
-      memset(&Q, 0, sizeof(Q));
-      Q.hT = P.hT; Q.hQ = P.hQ; Q.rsHnet = P.rsHnet; Q.rsHrep = P.rsHrep; Q.ldh = P.ldh;
-      Q.Wt = P.Wt[0]; Q.bt = P.bt[0]; Q.Wq = P.Wq[0]; Q.bq = P.bq[0]; Q.rsNet = rsNet; Q.rsP = rsP;
-      Q.r = P.r; Q.d = P.d; Q.tid = P.tid; Q.rsR = P.rsR;
-      Q.logp = P.logp; Q.rsLogp = P.rsLogp; Q.log_alpha = P.log_alpha;
-      Q.y = P.y; Q.q = P.q; Q.dq = P.dq; Q.lq = P.lq; Q.rsY = P.rsY;
-      Q.ens = h->ens.dev; Q.tsub = h->tsub.p; Q.rsTsub = h->tsub.rs; Q.E = E;
-      push(std::move(l), critic_heads_ens_kernel, Q);
-    } else {
-      push(std::move(l), critic_heads_kernel, P);
-    }
+    P.ens = h->ens.dev; P.tsub = h->tsub.p; P.rsTsub = h->tsub.rs; P.E = E;
+    push(std::move(l), critic_heads_kernel, P);
   }
   // ---- Phase C: critic backward + Adam/Polyak ----------------------------------------------
   head_bwd(false, true);
@@ -2002,24 +1968,14 @@ void PlanBuilder::build_plan_layered() {
     memset(&P, 0, sizeof(P));
     const Buf& hP = h->pass[PASS_P].h[Lc - 1];
     P.hP = hP.p; P.rsHnet = (long long)B * Hc; P.rsHrep = hP.rs; P.ldh = Hc;
-    for (int net = 0; net < 2; ++net) { P.Wq[net] = W(L.q[net][Lc].w); P.bq[net] = W(L.q[net][Lc].b); }
-    P.rsP = rsP;
+    P.Wq = W(L.q[0][Lc].w); P.bq = W(L.q[0][Lc].b);
+    P.rsNet = rsNet; P.rsP = rsP;
     P.tid = (const int*)h->tid.p; P.rsR = h->r.rs;
     P.logp = h->logp.p + B; P.rsLogp = h->logp.rs;
     P.log_alpha = W(L.off_alpha);
-    P.dqa = h->dqa.p; P.la = h->la.p; P.qmin = h->qmin.p; P.rsY = h->y.rs;
-    if (ens) {
-      ActorQHeadEnsArgs Q;
-      memset(&Q, 0, sizeof(Q));
-      Q.hP = P.hP; Q.rsHnet = P.rsHnet; Q.rsHrep = P.rsHrep; Q.ldh = P.ldh;
-      Q.Wq = P.Wq[0]; Q.bq = P.bq[0]; Q.rsNet = rsNet; Q.rsP = rsP;
-      Q.tid = P.tid; Q.rsR = P.rsR; Q.logp = P.logp; Q.rsLogp = P.rsLogp; Q.log_alpha = P.log_alpha;
-      Q.dqa = P.dqa; Q.qp = h->qp.p; Q.la = P.la; Q.qmin = P.qmin; Q.rsY = P.rsY;
-      Q.ens = h->ens.dev; Q.E = E;
-      push(std::move(l), actor_q_heads_ens_kernel, Q);
-    } else {
-      push(std::move(l), actor_q_heads_kernel, P);
-    }
+    P.dqa = h->dqa.p; P.qp = h->qp.p; P.la = h->la.p; P.qmin = h->qmin.p; P.rsY = h->y.rs;
+    P.ens = h->ens.dev; P.E = E;
+    push(std::move(l), actor_q_heads_kernel, P);
   }
   head_bwd(false, false);
   for (int l = Lc - 1; l >= 0; --l) critic_bwd(PASS_P, l, false);
@@ -2386,9 +2342,10 @@ extern "C" int b200sac_create(const b200sac_cfg* cfg, int32_t device, uint64_t s
     const double p0 = 0.0;
     if (int rc = h->drop.init(R, &p0)) return rc;
   }
-  if (cfg->critic_ensemble) {  // REDQ's and RLPD's defaults: a subset of 2, the mean over the ensemble for the actor
+  {  // ensembles: REDQ's and RLPD's defaults, a subset of 2 and the mean over the ensemble for the actor; twins: both
+     // critics and the min, which the head kernels then compute as the twin step does
     slab.request(h->tsub, E);
-    const int e0[2] = {2, 1};
+    const int e0[2] = {2, cfg->critic_ensemble ? 1 : 0};
     if (int rc = h->ens.init(R, e0)) return rc;
   }
   if (int rc = slab.allocate(h->slab)) return rc;
@@ -3727,14 +3684,9 @@ static void eval_critics(b200sac* h, cudaStream_t st, int rep, const std::vector
       LnArgs P;
       memset(&P, 0, sizeof(P));
       P.z = E.z; P.h = E.hc[l & 1];
-      for (int net = 0; net < 2; ++net) { P.g[net] = par.p + nets[net][l].g; P.c[net] = par.p + nets[net][l].c; }
-      P.B = n; P.H = nets[0][l].out;
-      if (h->cfg.critic_ensemble) {
-        const LnEnsArgs PE{P, nets[1][l].g - nets[0][l].g, h->E};
-        ln_fwd_ens_kernel<false><<<dim3((h->E * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, PE);
-        continue;
-      }
-      ln_fwd_kernel<false><<<dim3((2 * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, P);
+      P.g = par.p + nets[0][l].g; P.c = par.p + nets[0][l].c; P.rsNet = nets[1][l].g - nets[0][l].g;
+      P.B = n; P.H = nets[0][l].out; P.E = h->E;
+      ln_fwd_kernel<false><<<dim3((h->E * n + kLnThreads / kWarp - 1) / (kLnThreads / kWarp), 1), kLnThreads, 0, st>>>(h->K, P);
     }
   }
 }

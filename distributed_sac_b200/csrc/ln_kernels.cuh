@@ -1,6 +1,7 @@
 // LayerNorm in the critics' hidden layers (b200sac_cfg.critic_ln): h = relu(g * (z - mu) * rstd + c) after each hidden
-// Linear of q1, q2 and their targets, torch's nn.LayerNorm(H, eps=1e-5) between the Linear and its ReLU.
-//   ln_fwd_kernel   one warp per row of the [2][B][H] pre-normalization buffer z (both critics): the row statistics, then
+// Linear of the E critics (q1, q2 on a twin handle) and their targets, torch's nn.LayerNorm(H, eps=1e-5) between the
+// Linear and its ReLU.  Critic k's g, c (and their gradient slots) sit at critic 0's + k * rsNet.
+//   ln_fwd_kernel   one warp per row of the [E][B][H] pre-normalization buffer z (every critic): the row statistics, then
 //                   h = relu(g * xhat + c), in fp64, rounded to fp32 once.
 //   ln_bwd_kernel   one CTA per (chunk of kLnRows rows, critic, replica): the ReLU-masked gradient dy in dh becomes dz in
 //                   place, dz = rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)); with dg / dc set, each CTA leaves its
@@ -26,21 +27,22 @@ constexpr double kLnEps = 1e-5;
 struct DropRate { unsigned t; float s; };
 
 struct LnArgs {
-  const float* z;          // [R][2][B][H] pre-normalization activations, replica stride rsZ (the dropout forward
+  const float* z;          // [R][E][B][H] pre-normalization activations, replica stride rsZ (the dropout forward
                            // writes z' over them)
-  float* h;                // ln_fwd: [R][2][B][H] post-ReLU output, replica stride rsH
-  float* dh;               // ln_bwd: [R][2][B][H] dy in, dz out, replica stride rsH
-  const float* g[2];       // per critic: the layer's LayerNorm weight and bias (replica 0; replica stride rsP)
-  const float* c[2];
-  float* dg[2];            // ln_bwd: gradient-arena slots of g and c (replica stride rsG); null: the input gradient only
-  float* dc[2];
-  double* part;            // ln_bwd with dg: [R][2][chunks][2][H] chunk column sums (dy*xhat, dy)
-  unsigned* ticket;        // [R][2] CTAs done; the last one resets it
+  float* h;                // ln_fwd: [R][E][B][H] post-ReLU output, replica stride rsH
+  float* dh;               // ln_bwd: [R][E][B][H] dy in, dz out, replica stride rsH
+  const float* g;          // critic 0's LayerNorm weight and bias of the layer (replica 0; replica stride rsP)
+  const float* c;
+  float* dg;               // ln_bwd: gradient-arena slots of g and c (replica stride rsG); null: the input gradient only
+  float* dc;
+  double* part;            // ln_bwd with dg: [R][E][chunks][2][H] chunk column sums (dy*xhat, dy)
+  unsigned* ticket;        // [R][E] CTAs done; the last one resets it
   long long rsZ, rsH, rsP, rsG;
-  int B, H;
+  long long rsNet;         // from one critic's g, c, dg, dc to the next's
+  int B, H, E;
   int actor_side;          // 1: the actor pass (returns at entry on a critic-only step)
-  // critic_dropout only: the rate table [R], the pass's mask bits [R][2][B][ceil(H / 32)] (replica stride rsM) and
-  // (pass * 8 + layer) * 2, the tag of q1's masks in this launch (q2's is one more)
+  // critic_dropout only: the rate table [R], the pass's mask bits [R][E][B][ceil(H / 32)] (replica stride rsM) and
+  // (pass * 8 + layer) * E, the tag of q1's masks in this launch (critic k's is k more)
   const DropRate* drop;
   unsigned* mbits;
   long long rsM;
@@ -96,7 +98,7 @@ B200_D void ln_row_stats(const float* z, int H, int lane, double& mu, double& rs
   rstd = 1.0 / sqrt(warp_sum_d(v) / (double)H + kLnEps);
 }
 
-// grid ((2B + 7) / 8, R), 256 threads: warp w of CTA x normalizes row 8x + w of [2][B] (critic row / B)
+// grid ((E B + 7) / 8, R), 256 threads: warp w of CTA x normalizes row 8x + w of [E][B] (critic row / B)
 template <bool kDrop>
 __global__ void __launch_bounds__(kLnThreads) ln_fwd_kernel(StepConst K, LnArgs P) {
   const int rep = blockIdx.y;
@@ -104,12 +106,12 @@ __global__ void __launch_bounds__(kLnThreads) ln_fwd_kernel(StepConst K, LnArgs 
   KStamp ks_;
   if (skip) return;
   const int lane = threadIdx.x & 31, row = blockIdx.x * (kLnThreads / kWarp) + (threadIdx.x >> 5);
-  if (row >= 2 * P.B) return;
+  if (row >= P.E * P.B) return;
   const int net = row / P.B, H = P.H;
   const float* z = P.z + rep * P.rsZ + (long long)row * H;
   float* h = P.h + rep * P.rsH + (long long)row * H;
-  const float* g = P.g[net] + rep * P.rsP;
-  const float* c = P.c[net] + rep * P.rsP;
+  const float* g = P.g + net * P.rsNet + rep * P.rsP;
+  const float* c = P.c + net * P.rsNet + rep * P.rsP;
   if constexpr (kDrop) {
     const int words = (H + 31) / 32;
     const Philox ph(K.seed ^ (kDropKeyMul * (unsigned long long)(rep + 1)));
@@ -124,7 +126,7 @@ __global__ void __launch_bounds__(kLnThreads) ln_fwd_kernel(StepConst K, LnArgs 
   }
 }
 
-// grid (ceil(B / kLnRows), 2, R), 256 threads.  Rows of one CTA: [blockIdx.x * kLnRows, +kLnRows) of critic blockIdx.y.
+// grid (ceil(B / kLnRows), E, R), 256 threads.  Rows of one CTA: [blockIdx.x * kLnRows, +kLnRows) of critic blockIdx.y.
 // Row sums (one warp per row, the order of ln_row_stats): a = (sum_j g_j dy_j) / H, b = (sum_j g_j dy_j xhat_j) / H,
 // xhat_j = (z_j - mu) * rstd; then thread t owns columns t, t + 256, ...: dz = (float)(rstd * ((g dy - a) - xhat * b)) and,
 // with dg, its chunk's sums of dy*xhat and dy over the rows in increasing order.  The last CTA adds the chunks' sums in
@@ -132,7 +134,7 @@ __global__ void __launch_bounds__(kLnThreads) ln_fwd_kernel(StepConst K, LnArgs 
 // Dropout: dz is then multiplied by m ? s : 0, m read from the forward's mask bits.
 template <bool kDrop>
 __global__ void __launch_bounds__(kLnThreads) ln_bwd_kernel(StepConst K, LnArgs P) {
-  const int rep = blockIdx.z, net = blockIdx.y;
+  const int rep = blockIdx.z, net = blockIdx.y, E = P.E;
   const bool skip = P.actor_side && !(sched_of(K.cnt, rep) & SCHED_ACTOR);
   KStamp ks_;
   __shared__ double st[kLnRows][4];       // mu, rstd, a, b of each row
@@ -143,7 +145,7 @@ __global__ void __launch_bounds__(kLnThreads) ln_bwd_kernel(StepConst K, LnArgs 
   const long long base = ((long long)net * P.B + r0) * H;
   const float* z = P.z + rep * P.rsZ + base;
   float* dh = P.dh + rep * P.rsH + base;
-  const float* g = P.g[net] + rep * P.rsP;
+  const float* g = P.g + net * P.rsNet + rep * P.rsP;
   for (int r = warp; r < nr; r += kLnThreads / kWarp) {
     const float* zr = z + (long long)r * H;
     const float* dr = dh + (long long)r * H;
@@ -160,9 +162,9 @@ __global__ void __launch_bounds__(kLnThreads) ln_bwd_kernel(StepConst K, LnArgs 
     if (lane == 0) { st[r][0] = mu; st[r][1] = rstd; st[r][2] = sa / (double)H; st[r][3] = sb / (double)H; }
   }
   __syncthreads();
-  const bool wg = P.dg[net] != nullptr;
+  const bool wg = P.dg != nullptr;
   const int chunks = gridDim.x;
-  double* part = wg ? P.part + (((long long)rep * 2 + net) * chunks) * 2 * H : nullptr;
+  double* part = wg ? P.part + (((long long)rep * E + net) * chunks) * 2 * H : nullptr;
   const int words = (H + 31) / 32;
   const unsigned* mb = kDrop ? P.mbits + rep * P.rsM + ((long long)net * P.B + r0) * words : nullptr;
   const float ds = kDrop ? P.drop[rep].s : 0.f;
@@ -191,13 +193,13 @@ __global__ void __launch_bounds__(kLnThreads) ln_bwd_kernel(StepConst K, LnArgs 
   if (!wg) return;
   __threadfence();
   __syncthreads();
-  unsigned* ticket = P.ticket + rep * 2 + net;
+  unsigned* ticket = P.ticket + rep * E + net;
   if (threadIdx.x == 0) s_last = atomicAdd(ticket, 1u) == (unsigned)(chunks - 1);
   __syncthreads();
   if (!s_last) return;
   __threadfence();
-  float* dg = P.dg[net] + rep * P.rsG;
-  float* dc = P.dc[net] + rep * P.rsG;
+  float* dg = P.dg + net * P.rsNet + rep * P.rsG;
+  float* dc = P.dc + net * P.rsNet + rep * P.rsG;
   for (int j = threadIdx.x; j < H; j += kLnThreads) {
     double sg = 0.0, sc = 0.0;
     for (int k = 0; k < chunks; ++k) {

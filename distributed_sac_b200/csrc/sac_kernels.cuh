@@ -465,18 +465,49 @@ __global__ void __launch_bounds__(256) policy_head_kernel(StepConst K, PolicyHea
 }
 
 // ------------------------------------------------------------------------------------------
-// Critic heads for the critic update: scalar heads of Qt1,Qt2 (target pass) and Q1,Q2 (s,a),
-// TD target and MSE gradient in one pass, one warp per row.
-//   y = rs*r + gamma*(1-d)*(min(Qt1,Qt2) - alpha*logp')          LL/learner.py:210
+// Critic heads for the critic update: scalar heads of the E target critics Qt_k (target pass) and the E critics Q_k
+// (s, a), TD target and MSE gradients in one pass, one warp per row.  Critic k's head sits at critic 0's + k * rsNet
+// (the critics share one layout and sit back to back; E = 2 on a twin handle).
+//   y = rs*r + gamma*(1-d)*(min_{k in S} Qt_k - alpha*logp')    LL/learner.py:210; S: the replica's target subset
 //   dL/dQk = 2c (Qk - y)                                        LL/model.py:139-140
 // ------------------------------------------------------------------------------------------
+constexpr int kMaxEns = 10;
+constexpr unsigned long long kEnsKeyMul = 0x8EBC6AF09C88C6E3ull;
+
+// The step's target subset of replica rep as a bit set (bit k: critic k is in S): all E when m >= E; otherwise the m
+// indices with the smallest (w_k, k), w_{4q..4q+3} = Philox(key = seed ^ (kEnsKeyMul * (rep + 1)), counter (step low,
+// step high, 0, q)).
+B200_D unsigned ens_subset(unsigned long long seed, int rep, long long step, int E, int m) {
+  if (m >= E) return (1u << E) - 1u;
+  const Philox ph(seed ^ (kEnsKeyMul * (unsigned long long)(rep + 1)));
+  uint32_t w0[4], w1[4], w2[4];
+  ph((uint32_t)step, (uint32_t)(step >> 32), 0u, 0u, w0);
+  ph((uint32_t)step, (uint32_t)(step >> 32), 0u, 1u, w1);
+  ph((uint32_t)step, (uint32_t)(step >> 32), 0u, 2u, w2);
+  const uint32_t w[12] = {w0[0], w0[1], w0[2], w0[3], w1[0], w1[1], w1[2], w1[3], w2[0], w2[1], w2[2], w2[3]};
+  unsigned s = 0;
+#pragma unroll
+  for (int k = 0; k < kMaxEns; ++k) {
+    int rank = 0;
+#pragma unroll
+    for (int j = 0; j < kMaxEns; ++j)
+      if (j < E && (w[j] < w[k] || (w[j] == w[k] && j < k))) ++rank;
+    if (k < E && rank < m) s |= 1u << k;
+  }
+  return s;
+}
+
 struct CriticHeadArgs {
-  const float* hT; const float* hQ; long long rsHnet, rsHrep; int ldh;   // [net][B][Hc] per replica
-  const float* Wt[2]; const float* bt[2]; const float* Wq[2]; const float* bq[2]; long long rsP;
+  const float* hT; const float* hQ; long long rsHnet, rsHrep; int ldh;   // [E][B][Hc] per replica
+  const float* Wt; const float* bt; const float* Wq; const float* bq;   // critic 0's heads; critic k at + k * rsNet
+  long long rsNet, rsP;
   const float* r; const float* d; const int* tid; long long rsR;
   const float* logp; long long rsLogp;   // logp[0..B) = next-state half
   const float* log_alpha;                // param arena pointer (per replica rsP)
-  float* y; float* q; float* dq; float* lq; long long rsY;   // y[B], q[2][B], dq[2][B], lq[B]
+  float* y; float* q; float* dq; float* lq; long long rsY;   // y[B], q[E][B], dq[E][B] (replica stride E * rsY), lq[B]
+  const int* ens;                                            // [R][2] (m, actor_mean)
+  float* tsub; long long rsTsub;                             // [E] per replica: the subset as 0 / 1
+  int E;
 };
 
 // Lane-strided dot product; eight strides (256 columns) of both operands are in flight before the first FMA so a
@@ -501,7 +532,7 @@ B200_D float warp_dot(const float* __restrict__ x, const float* __restrict__ w, 
   return warp_sum(warp_dot_partial(x, w, n, lane));
 }
 
-// SAC per-row math shared by the per-layer heads kernels and chain2_kernel.
+// SAC per-row math of the twin critics shared by chain2_kernel and refresh_td_kernel.
 // TD target y = rs r + gamma (1-d)(min(Qt1, Qt2) - alpha logpi') (LL/learner.py:210); the caller forms t1 = rs r and
 // t2 = gamma (1-d) as soon as their operands land.
 B200_D float td_target(float t1, float t2, float qt1, float qt2, float alpha, float lp) {
@@ -516,95 +547,136 @@ B200_D void min_route(float q1, float q2, float c_loss, float& g1, float& g2) {
   else { g1 = 0.f; g2 = -c_loss; }
 }
 
-__global__ void critic_heads_kernel(StepConst K, CriticHeadArgs P) {
+// The row's TD-target terms rs*r and gamma*(1-d) are formed as soon as their operands land; qt_min takes the critics of
+// S in index order, so E = 2 with S = {1, 2} is td_target's fminf(Qt1, Qt2), and the squared errors are added in index
+// order.  Replica rep's subset goes to tsub from row 0.
+__global__ void __launch_bounds__(256) critic_heads_kernel(StepConst K, CriticHeadArgs P) {
   KStamp ks_;
   const int rep = blockIdx.y;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int row = blockIdx.x * (blockDim.x / 32) + warp;
-  const int B = K.B, H = K.Hc;
+  const int B = K.B, H = K.Hc, E = P.E;
   if (row >= B) return;
   const float* hT = P.hT + rep * P.rsHrep + (long long)row * P.ldh;
   const float* hQ = P.hQ + rep * P.rsHrep + (long long)row * P.ldh;
   const long long po = rep * P.rsP;
-  // per-row scalars and the four heads' operands are all requested before anything is consumed
   const int t = (P.tid + rep * P.rsR)[row];
   const float r = (P.r + rep * P.rsR)[row], d = (P.d + rep * P.rsR)[row];
-  // the row's TD-target terms rs*r and gamma*(1-d) are formed as soon as their operands land: holding gamma and rs next
-  // to r and d across the dot products would take two more registers, which this 32-register kernel pays for by
-  // serialising the loads of a head
   const float t1 = K.hp[rep].reward_scale * r;
   const float t2 = (K.disc ? K.disc[(long long)rep * B + row] : K.hp[rep].gamma) * (1.f - d);
   const float lp = (P.logp + rep * P.rsLogp)[row];
-  const float b_t1 = (P.bt[0] + po)[0], b_t2 = (P.bt[1] + po)[0], b_q1 = (P.bq[0] + po)[0], b_q2 = (P.bq[1] + po)[0];
-  const float p_t1 = warp_dot_partial(hT, P.Wt[0] + po, H, lane), p_t2 = warp_dot_partial(hT + P.rsHnet, P.Wt[1] + po, H, lane);
-  const float p_q1 = warp_dot_partial(hQ, P.Wq[0] + po, H, lane), p_q2 = warp_dot_partial(hQ + P.rsHnet, P.Wq[1] + po, H, lane);
   const float la_t = (P.log_alpha + po)[t];
-  const float qt1 = warp_sum(p_t1) + b_t1, qt2 = warp_sum(p_t2) + b_t2, q1 = warp_sum(p_q1) + b_q1, q2 = warp_sum(p_q2) + b_q2;
+  const unsigned S = ens_subset(K.seed, rep, K.cnt[rep].v[3], E, P.ens[2 * rep]);
+  float qv[kMaxEns], qt_min = 0.f;
+  bool first = true;
+#pragma unroll
+  for (int k = 0; k < kMaxEns; ++k) {
+    qv[k] = 0.f;
+    if (k < E) {
+      const long long pk = po + k * P.rsNet;
+      const float b_t = (P.bt + pk)[0], b_q = (P.bq + pk)[0];
+      const float p_t = warp_dot_partial(hT + k * P.rsHnet, P.Wt + pk, H, lane);
+      const float p_q = warp_dot_partial(hQ + k * P.rsHnet, P.Wq + pk, H, lane);
+      const float qt = warp_sum(p_t) + b_t;
+      qv[k] = warp_sum(p_q) + b_q;
+      if ((S >> k) & 1u) { qt_min = first ? qt : fminf(qt_min, qt); first = false; }
+    }
+  }
   if (lane == 0) {
     const float alpha = (float)exp((double)la_t);
-    const float y = td_target(t1, t2, qt1, qt2, alpha, lp);
-    const float e1 = y - q1, e2 = y - q2;
-    float* Y = P.y + rep * P.rsY;
-    Y[row] = y;
-    float* Q = P.q + rep * 2 * P.rsY;
-    Q[row] = q1; Q[B + row] = q2;
-    float g1 = 2.f * K.c_loss * (q1 - y), g2 = 2.f * K.c_loss * (q2 - y), l = e1 * e1 + e2 * e2;
-    if (K.isw) {                                 // prioritized replay: importance-weighted critic loss
-      const float w = K.isw[(long long)rep * B + row];
-      g1 = g1 * w; g2 = g2 * w; l = l * w;
-    }
-    float* DQ = P.dq + rep * 2 * P.rsY;
-    DQ[row] = g1;
-    DQ[B + row] = g2;
+    const float y = t1 + t2 * (qt_min - alpha * lp);
+    (P.y + rep * P.rsY)[row] = y;
+    float* Q = P.q + rep * E * P.rsY;
+    float* DQ = P.dq + rep * E * P.rsY;
+    const float w = K.isw ? K.isw[(long long)rep * B + row] : 1.f;   // prioritized replay: importance-weighted loss
+    float l = 0.f;
+#pragma unroll
+    for (int k = 0; k < kMaxEns; ++k)
+      if (k < E) {
+        const float e = y - qv[k];
+        l = k == 0 ? e * e : l + e * e;
+        float g = 2.f * K.c_loss * (qv[k] - y);
+        if (K.isw) g = g * w;
+        Q[k * B + row] = qv[k];
+        DQ[k * B + row] = g;
+        if (row == 0) (P.tsub + rep * P.rsTsub)[k] = ((S >> k) & 1u) ? 1.f : 0.f;
+      }
+    if (K.isw) l = l * w;
     (P.lq + rep * P.rsY)[row] = l;
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// Actor-pass heads: Q1,Q2 at (s, a~) with the already-updated critics, min and its gradient
-// routing (LL/learner.py:222-223; torch.minimum backward: the smaller head gets the gradient,
-// ties split it), plus the per-row policy-loss term (LL/model.py:84-88).
+// Actor-pass heads: Q_k at (s, a~) with the already-updated critics, the replica's reduction over them and its gradient
+// routing, plus the per-row policy-loss term (LL/model.py:84-88).  The min splits the gradient evenly among tied critics
+// (LL/learner.py:222-223; torch.minimum backward: the smaller head gets the gradient, ties split it); the mean gives
+// every critic 1 / E of it.
 // ------------------------------------------------------------------------------------------
 struct ActorQHeadArgs {
   const float* hP; long long rsHnet, rsHrep; int ldh;
-  const float* Wq[2]; const float* bq[2]; long long rsP;
+  const float* Wq; const float* bq; long long rsNet, rsP;   // critic 0's head; critic k at + k * rsNet
   const int* tid; long long rsR;
   const float* logp; long long rsLogp;    // +B offset applied by the host: current-state half
   const float* log_alpha;
-  float* dqa; float* la; float* qmin; long long rsY;   // dqa[2][B], la[B], qmin[B]
+  float* dqa; float* qp; float* la; float* qmin; long long rsY;   // dqa[E][B], qp[E][B] (replica stride E * rsY), la[B], qmin[B]
+  const int* ens;                          // [R][2] (m, actor_mean)
+  int E;
 };
 
-__global__ void actor_q_heads_kernel(StepConst K, ActorQHeadArgs P) {
+__global__ void __launch_bounds__(256) actor_q_heads_kernel(StepConst K, ActorQHeadArgs P) {
   const int rep = blockIdx.y;
   const int sched = sched_of(K.cnt, rep);
   KStamp ks_;
   if (!(sched & SCHED_ACTOR)) return;
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const int row = blockIdx.x * (blockDim.x / 32) + warp;
-  const int B = K.B, H = K.Hc;
+  const int B = K.B, H = K.Hc, E = P.E;
   if (row >= B) return;
   const float* hP = P.hP + rep * P.rsHrep + (long long)row * P.ldh;
   const long long po = rep * P.rsP;
   const int t = (P.tid + rep * P.rsR)[row];
   const float lp = (P.logp + rep * P.rsLogp)[row];
-  const float b_q1 = (P.bq[0] + po)[0], b_q2 = (P.bq[1] + po)[0];
-  const float p_q1 = warp_dot_partial(hP, P.Wq[0] + po, H, lane), p_q2 = warp_dot_partial(hP + P.rsHnet, P.Wq[1] + po, H, lane);
   const float la_t = (P.log_alpha + po)[t];
-  const float q1 = warp_sum(p_q1) + b_q1, q2 = warp_sum(p_q2) + b_q2;
+  const bool mean = P.ens[2 * rep + 1] != 0;
+  float qv[kMaxEns], red = 0.f;
+#pragma unroll
+  for (int k = 0; k < kMaxEns; ++k) {
+    qv[k] = 0.f;
+    if (k < E) {
+      const long long pk = po + k * P.rsNet;
+      const float b_q = (P.bq + pk)[0];
+      qv[k] = warp_sum(warp_dot_partial(hP + k * P.rsHnet, P.Wq + pk, H, lane)) + b_q;
+      red = k == 0 ? qv[k] : (mean ? red + qv[k] : fminf(red, qv[k]));
+    }
+  }
   if (lane == 0) {
     const float alpha = (float)exp((double)la_t);
-    const float qm = fminf(q1, q2);
-    float g1, g2;
-    min_route(q1, q2, K.c_loss, g1, g2);
-    float* DQ = P.dqa + rep * 2 * P.rsY;
-    DQ[row] = g1; DQ[B + row] = g2;
-    (P.la + rep * P.rsY)[row] = -(qm - alpha * lp);
-    (P.qmin + rep * P.rsY)[row] = qm;
+    float g_all = 0.f;
+    int ties = 0;
+    if (mean) {
+      red = red / (float)E;
+      g_all = -K.c_loss / (float)E;
+    } else {
+#pragma unroll
+      for (int k = 0; k < kMaxEns; ++k)
+        if (k < E && qv[k] == red) ++ties;
+      g_all = ties > 0 ? -K.c_loss / (float)ties : 0.f;
+    }
+    float* DQ = P.dqa + rep * E * P.rsY;
+    float* QP = P.qp + rep * E * P.rsY;
+#pragma unroll
+    for (int k = 0; k < kMaxEns; ++k)
+      if (k < E) {
+        DQ[k * B + row] = (mean || qv[k] == red) ? g_all : 0.f;
+        QP[k * B + row] = qv[k];
+      }
+    (P.la + rep * P.rsY)[row] = -(red - alpha * lp);
+    (P.qmin + rep * P.rsY)[row] = red;
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// Backward of a narrow output layer (N_out <= 16: the scalar Q heads and the 2*act policy
+// Backward of a narrow output layer (N_out <= 16: the E scalar Q heads and the 2*act policy
 // head).  One CTA per 32-column slab of the hidden width, looping over all rows:
 //   dh[m][k] = (sum_j dout[m][j] W[j][k]) * [h[m][k] > 0]
 //   dW[j][k] = sum_m dout[m][j] h[m][k],  db[j] = sum_m dout[m][j]
@@ -612,16 +684,18 @@ __global__ void actor_q_heads_kernel(StepConst K, ActorQHeadArgs P) {
 // policy head (closed-form backward of LL/model.py:50-60, oracle/sac_manual.py).
 // ------------------------------------------------------------------------------------------
 struct HeadBwdArgs {
-  int M, NO, Kdim, nets;
+  int M, NO, Kdim, nets;                                     // nets: E (critic heads) or 1 (the policy head)
   const float* dout; long long rsDoutNet, rsDoutRep;         // [net][M][NO] (critic mode)
-  const float* W[2]; long long rsP;                          // head weights [NO][Kdim]
+  const float* W; long long rsP;                             // head weights [NO][Kdim]
   const float* h; long long rsHnet, rsHrep; int ldh;         // [net][M][Kdim]
   float* dh; long long rsDhNet, rsDhRep; int lddh;
-  float* dW[2]; float* db[2]; long long rsG;                 // grad arena (null -> no wgrad)
+  float* dW; float* db; long long rsG;                       // grad arena (null -> no wgrad)
   int row_slices;                                            // rows are cut into this many slices (grid.x = col blocks x slices);
-  float* dWx[2]; float* dbx[2]; long long xs;                // slice s >= 1 writes gradient slice s (summed by Adam, like split-K)
+  float* dWx; float* dbx; long long xs;                      // slice s >= 1 writes gradient slice s (summed by Adam, like split-K)
+  long long rsNet;                                           // W, dW, db, dWx, dbx: critic 0's; critic net's at + net * rsNet
   int policy_mode;
-  const float* dx; long long rsDxNet, rsDxRep; int lddx;     // [2][B][xw] critic input grads
+  const float* dx; long long rsDxNet, rsDxRep; int lddx;     // [E][B][xw] critic input grads
+  int E;                                                     // policy mode: the critics whose action gradients are summed
   const float* psave; long long rsSave;                      // rows B..2B-1 pre-offset by host
   const int* tid; long long rsR;
   const float* log_alpha;
@@ -645,13 +719,20 @@ B200_D void policy_dout_point(const StepConst& K, const float* __restrict__ sv, 
   dls = mask != 0.f ? dstd * std : 0.f;          // torch.clamp's backward: zero outside [-20, 2], for a NaN log-std too
 }
 
+// d(action) of row m, action j: the E critics' input gradients [E][B][xw] (net stride rsDxNet) added in index order
+B200_D float sum_dact(const float* __restrict__ dx0, long long rsDxNet, int E) {
+  float da = dx0[0];
+  for (int k = 1; k < E; ++k) da = da + dx0[k * rsDxNet];
+  return da;
+}
+
 struct PolicyDoutArgs {
   const float* dx; long long rsDxNet, rsDxRep; int lddx;
   const float* psave; long long rsSave;
   const int* tid; long long rsR;
   const float* log_alpha; long long rsP;
   float* dout; float* dact; long long rsDout;     // [M][2A], [M][A]
-  int M;
+  int M, E;
 };
 
 // Large batches: compute the policy-head output gradient once (instead of in every head_bwd CTA).
@@ -664,8 +745,7 @@ __global__ void __launch_bounds__(256) policy_dout_kernel(StepConst K, PolicyDou
   if (e >= P.M * A) return;
   const int m = e / A, j = e % A;
   const float* __restrict__ sv = P.psave + rep * P.rsSave + ((long long)m * A + j) * kSaveW;
-  const float* __restrict__ dx0 = P.dx + rep * P.rsDxRep + (long long)m * P.lddx + K.in_w + j;
-  const float da = dx0[0] + dx0[P.rsDxNet];
+  const float da = sum_dact(P.dx + rep * P.rsDxRep + (long long)m * P.lddx + K.in_w + j, P.rsDxNet, P.E);
   const float alpha = (float)exp((double)(P.log_alpha + rep * P.rsP)[(P.tid + rep * P.rsR)[m]]);
   float dmu, dls;
   policy_dout_point(K, sv, da, alpha, dmu, dls);
@@ -678,7 +758,8 @@ __global__ void __launch_bounds__(256) policy_dout_kernel(StepConst K, PolicyDou
 constexpr int kHbCols = 8;     // hidden columns per CTA
 constexpr int kHbRows = 32;    // row groups per CTA (256 threads = 8 cols x 32 row groups)
 
-__global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs P) {
+// (256, 1): without the occupancy target ptxas keeps this kernel at 64 registers and spills
+__global__ void __launch_bounds__(256, 1) head_bwd_kernel(StepConst K, HeadBwdArgs P) {
   const int net = blockIdx.y, rep = blockIdx.z;
   const bool skip = P.actor_side && !(sched_of(K.cnt, rep) & SCHED_ACTOR);
   KStamp ks_;
@@ -694,6 +775,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs 
   float* sd = sm;                       // [M][NO]
   float* red = sm + (size_t)rows_per * NO;     // [32][8][NO] partial dW / scratch (>= 256 floats)
   const int tid = threadIdx.x, tx = tid % kHbCols, ty = tid / kHbCols;
+  const long long no = net * P.rsNet;
 
   if (P.policy_mode) {
     const int A = K.act;
@@ -704,8 +786,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs 
     for (int e = tid; e < M * A; e += 256) {
       const int ml = e / A, j = e % A, m = r0 + ml;
       const float* __restrict__ sv = P.psave + rep * P.rsSave + ((long long)m * A + j) * kSaveW;
-      const float* __restrict__ dx0 = P.dx + rep * P.rsDxRep + (long long)m * P.lddx + K.in_w + j;
-      const float da = dx0[0] + dx0[P.rsDxNet];
+      const float da = sum_dact(P.dx + rep * P.rsDxRep + (long long)m * P.lddx + K.in_w + j, P.rsDxNet, P.E);
       const int tk = (P.tid + rep * P.rsR)[m];
       float dmu, dls;
       policy_dout_point(K, sv, da, s_alpha[tk], dmu, dls);
@@ -724,7 +805,7 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs 
 
   const int kcol = cb * kHbCols + tx;
   const bool kin = kcol < KD;
-  const float* __restrict__ W = P.W[net] + rep * P.rsP;
+  const float* __restrict__ W = P.W + no + rep * P.rsP;
   float w[kMaxHeadOut], gw[kMaxHeadOut];
 #pragma unroll
   for (int j = 0; j < kMaxHeadOut; ++j) {        // head weights requested before the staging barrier
@@ -759,9 +840,9 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs 
       }
     }
   }
-  if (P.dW[net] != nullptr) {
-    float* __restrict__ dWp = (slice == 0 ? P.dW[net] : P.dWx[net] + (long long)(slice - 1) * P.xs) + rep * P.rsG;
-    float* __restrict__ dbp = (slice == 0 ? P.db[net] : P.dbx[net] + (long long)(slice - 1) * P.xs) + rep * P.rsG;
+  if (P.dW != nullptr) {
+    float* __restrict__ dWp = (slice == 0 ? P.dW : P.dWx + (long long)(slice - 1) * P.xs) + no + rep * P.rsG;
+    float* __restrict__ dbp = (slice == 0 ? P.db : P.dbx + (long long)(slice - 1) * P.xs) + no + rep * P.rsG;
 #pragma unroll
     for (int j = 0; j < kMaxHeadOut; ++j)
       if (j < NO) red[(ty * kHbCols + tx) * NO + j] = gw[j];
@@ -798,68 +879,40 @@ __global__ void __launch_bounds__(256) head_bwd_kernel(StepConst K, HeadBwdArgs 
   }
 }
 
-// The same backward with 128-bit column accesses: thread = 4 consecutive hidden columns x one of 16 row groups, CTA = 64
-// columns x one row slice.  The 8-column mapping above reads and writes 32 bytes per row per warp quarter (four sectors per
-// warp instruction) and needs 50 column blocks x 4 slices x 2 nets = 400 CTAs at the 400-wide shapes; here a warp
-// instruction moves two full 256-byte row segments.  Used
-// when the hidden width is a multiple of 4 (row pitches then are too); same fixed-order reductions, different grouping.
+// The scalar critic heads' backward (NO = 1, critic mode) with 128-bit column accesses: thread = 4 consecutive hidden
+// columns x one of 16 row groups, CTA = 64 columns x one row slice.  The 8-column mapping above reads and writes 32 bytes
+// per row per warp quarter (four sectors per warp instruction) and needs 50 column blocks x 4 slices x 2 nets = 400 CTAs
+// at the 400-wide shapes; here a warp instruction moves two full 256-byte row segments.  Used when the hidden width is a
+// multiple of 4 (row pitches then are too); same fixed-order reductions, different grouping.
 constexpr int kHb4Cols = 64;   // hidden columns per CTA (16 threads x float4)
 constexpr int kHb4Rows = 16;   // row groups per CTA
 
-template <int NOMAX>
-__global__ void __launch_bounds__(256) head_bwd4_kernel(StepConst K, HeadBwdArgs P) {
+__global__ void __launch_bounds__(256, 1) head_bwd4_kernel(StepConst K, HeadBwdArgs P) {
   const int net = blockIdx.y, rep = blockIdx.z;
   const bool skip = P.actor_side && !(sched_of(K.cnt, rep) & SCHED_ACTOR);
   KStamp ks_;
   extern __shared__ float sm[];
   if (skip) return;
-  const int NO = P.NO, KD = P.Kdim;
+  const int KD = P.Kdim;
   const int ncb = (KD + kHb4Cols - 1) / kHb4Cols;
   const int slice = blockIdx.x / ncb, cb = blockIdx.x - slice * ncb;
   const int rows_per = (P.M + P.row_slices - 1) / P.row_slices;
   const int r0 = slice * rows_per, r1 = (r0 + rows_per < P.M) ? r0 + rows_per : P.M;
   const int M = r1 - r0;
   if (M <= 0) return;
-  float* sd = sm;                                   // [M][NO]
-  float* red = sm + (((size_t)rows_per * NO + 3) & ~(size_t)3);   // [16 row groups][16 col quads][NO][4], 16-B aligned (float4)
+  float* sd = sm;                                   // [M]
+  float* red = sm + (((size_t)rows_per + 3) & ~(size_t)3);   // [16 row groups][16 col quads][4], 16-B aligned (float4)
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-
-  if (P.policy_mode) {
-    const int A = K.act;
-    __shared__ float s_alpha[64];
-    const int Teff = K.T > 0 ? K.T : 1;
-    if (tid < Teff) s_alpha[tid] = (float)exp((double)(P.log_alpha + rep * P.rsP)[tid]);
-    __syncthreads();
-    for (int e = tid; e < M * A; e += 256) {
-      const int ml = e / A, j = e % A, m = r0 + ml;
-      const float* __restrict__ sv = P.psave + rep * P.rsSave + ((long long)m * A + j) * kSaveW;
-      const float* __restrict__ dx0 = P.dx + rep * P.rsDxRep + (long long)m * P.lddx + K.in_w + j;
-      const float da = dx0[0] + dx0[P.rsDxNet];
-      const int tk = (P.tid + rep * P.rsR)[m];
-      float dmu, dls;
-      policy_dout_point(K, sv, da, s_alpha[tk], dmu, dls);
-      sd[ml * NO + j] = dmu;
-      sd[ml * NO + A + j] = dls;
-      if (P.dout_dbg && cb == 0) {
-        (P.dout_dbg + rep * P.rsDbg)[(long long)m * NO + j] = dmu;
-        (P.dout_dbg + rep * P.rsDbg)[(long long)m * NO + A + j] = dls;
-        (P.dact_dbg + rep * P.rsDbg)[(long long)m * A + j] = da;
-      }
-    }
-  } else {
-    const float* __restrict__ src = P.dout + rep * P.rsDoutRep + net * P.rsDoutNet + (long long)r0 * NO;
-    for (int e = tid; e < M * NO; e += 256) sd[e] = src[e];
+  const long long no = net * P.rsNet;
+  {
+    const float* __restrict__ src = P.dout + rep * P.rsDoutRep + net * P.rsDoutNet + (long long)r0;
+    for (int e = tid; e < M; e += 256) sd[e] = src[e];
   }
-
   const int kcol = cb * kHb4Cols + 4 * tx;          // first of this thread's four columns (KD % 4 == 0: all four valid or none)
   const bool kin = kcol < KD;
-  const float* __restrict__ W = P.W[net] + rep * P.rsP;
-  float4 w[NOMAX], gw[NOMAX];
-#pragma unroll
-  for (int j = 0; j < NOMAX; ++j) {                 // head weights requested before the staging barrier
-    w[j] = (j < NO && kin) ? *reinterpret_cast<const float4*>(W + (long long)j * KD + kcol) : make_float4(0.f, 0.f, 0.f, 0.f);
-    gw[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+  const float* __restrict__ W = P.W + no + rep * P.rsP;
+  const float4 w = kin ? *reinterpret_cast<const float4*>(W + kcol) : make_float4(0.f, 0.f, 0.f, 0.f);
+  float4 gw = make_float4(0.f, 0.f, 0.f, 0.f);
   __syncthreads();
   const float* __restrict__ h = P.h + rep * P.rsHrep + net * P.rsHnet + (long long)r0 * P.ldh;
   float* __restrict__ dh = P.dh + rep * P.rsDhRep + net * P.rsDhNet + (long long)r0 * P.lddh;
@@ -876,60 +929,42 @@ __global__ void __launch_bounds__(256) head_bwd4_kernel(StepConst K, HeadBwdArgs
       const int m = mb + u * kHb4Rows;
       if (m < M) {
         float4 ds = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-        for (int j = 0; j < NOMAX; ++j) {
-          if (j < NO) {
-            const float dv = sd[m * NO + j];
-            ds.x = fmaf(dv, w[j].x, ds.x); ds.y = fmaf(dv, w[j].y, ds.y); ds.z = fmaf(dv, w[j].z, ds.z); ds.w = fmaf(dv, w[j].w, ds.w);
-            gw[j].x = fmaf(dv, hv[u].x, gw[j].x); gw[j].y = fmaf(dv, hv[u].y, gw[j].y);
-            gw[j].z = fmaf(dv, hv[u].z, gw[j].z); gw[j].w = fmaf(dv, hv[u].w, gw[j].w);
-          }
-        }
+        const float dv = sd[m];
+        ds.x = fmaf(dv, w.x, ds.x); ds.y = fmaf(dv, w.y, ds.y); ds.z = fmaf(dv, w.z, ds.z); ds.w = fmaf(dv, w.w, ds.w);
+        gw.x = fmaf(dv, hv[u].x, gw.x); gw.y = fmaf(dv, hv[u].y, gw.y);
+        gw.z = fmaf(dv, hv[u].z, gw.z); gw.w = fmaf(dv, hv[u].w, gw.w);
         if (kin)
           *reinterpret_cast<float4*>(dh + (long long)m * P.lddh + kcol) =
               make_float4(hv[u].x > 0.f ? ds.x : 0.f, hv[u].y > 0.f ? ds.y : 0.f, hv[u].z > 0.f ? ds.z : 0.f, hv[u].w > 0.f ? ds.w : 0.f);
       }
     }
   }
-  if (P.dW[net] != nullptr) {
-    float* __restrict__ dWp = (slice == 0 ? P.dW[net] : P.dWx[net] + (long long)(slice - 1) * P.xs) + rep * P.rsG;
-    float* __restrict__ dbp = (slice == 0 ? P.db[net] : P.dbx[net] + (long long)(slice - 1) * P.xs) + rep * P.rsG;
-#pragma unroll
-    for (int j = 0; j < NOMAX; ++j)
-      if (j < NO) *reinterpret_cast<float4*>(red + ((size_t)(ty * 16 + tx) * NO + j) * 4) = gw[j];
+  if (P.dW != nullptr) {
+    float* __restrict__ dWp = (slice == 0 ? P.dW : P.dWx + (long long)(slice - 1) * P.xs) + no + rep * P.rsG;
+    float* __restrict__ dbp = (slice == 0 ? P.db : P.dbx + (long long)(slice - 1) * P.xs) + no + rep * P.rsG;
+    *reinterpret_cast<float4*>(red + (size_t)(ty * 16 + tx) * 4) = gw;
     __syncthreads();
-    for (int o = tid; o < NO * kHb4Cols; o += 256) {   // (output j, column cc): fixed-order sum over the 16 row groups
-      const int j = o / kHb4Cols, cc = o - j * kHb4Cols;
+    for (int cc = tid; cc < kHb4Cols; cc += 256) {   // column cc: fixed-order sum over the 16 row groups
       const int col = cb * kHb4Cols + cc;
       if (col < KD) {
         float ssum = 0.f;
 #pragma unroll
-        for (int q = 0; q < kHb4Rows; ++q) ssum += red[((size_t)(q * 16 + (cc >> 2)) * NO + j) * 4 + (cc & 3)];
-        dWp[(long long)j * KD + col] = ssum;
+        for (int q = 0; q < kHb4Rows; ++q) ssum += red[(size_t)(q * 16 + (cc >> 2)) * 4 + (cc & 3)];
+        dWp[col] = ssum;
       }
     }
     if (cb == 0) {                     // bias gradient: per-thread row sums -> warp shuffle tree -> 8 warp partials (fixed order)
       __syncthreads();
-      float part[NOMAX];
-#pragma unroll
-      for (int j = 0; j < NOMAX; ++j) part[j] = 0.f;
-      for (int m = tid; m < M; m += 256) {
-#pragma unroll
-        for (int j = 0; j < NOMAX; ++j)
-          if (j < NO) part[j] += sd[m * NO + j];
-      }
-#pragma unroll
-      for (int j = 0; j < NOMAX; ++j)
-        if (j < NO) {
-          const float v = warp_sum(part[j]);
-          if ((tid & 31) == 0) red[(tid >> 5) * kMaxHeadOut + j] = v;
-        }
+      float part = 0.f;
+      for (int m = tid; m < M; m += 256) part += sd[m];
+      const float v = warp_sum(part);
+      if ((tid & 31) == 0) red[(tid >> 5) * kMaxHeadOut] = v;
       __syncthreads();
-      if (tid < NO) {
+      if (tid == 0) {
         float ssum = 0.f;
 #pragma unroll
-        for (int wq = 0; wq < 8; ++wq) ssum += red[wq * kMaxHeadOut + tid];
-        dbp[tid] = ssum;
+        for (int wq = 0; wq < 8; ++wq) ssum += red[wq * kMaxHeadOut];
+        dbp[0] = ssum;
       }
     }
   }

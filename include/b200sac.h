@@ -210,6 +210,7 @@ typedef struct b200sac_cfg {
  *     the fminf fold over all E; the gradient -c is split evenly among the critics equal to the minimum (torch.amin's
  *     backward).  The action's input gradient adds the E critics' contributions in index order.
  *   critic_dropout: the tag of critic k's masks is (pass * 8 + l) * E + k (the twin formula at E = 2).
+ * A twin handle runs the same kernels with its table fixed at m = 2 and MIN (b200sac_get/set_ensemble still refuse it), so
  * E = 2 with m = 2 and MIN computes exactly what the twin per-layer plan computes, bit for bit.
  * Plan: always the per-layer plan (never the layer-chained one), at precision 0 and 1.  The extra critics are extra problems
  * in the same grouped launches; a step has the launches and labels of the same cfg with critic_ensemble = 0 on the
@@ -617,7 +618,7 @@ int b200sac_blob_wait(b200sac_t* h, const uint8_t** host_ptr, int64_t* n_bytes);
 
 /* Debug / parity access to per-step intermediates of replica `replica`:
  * name in {"y","q1","q2","a_next","logp_next","a_cur","logp_cur","qmin","d_action","d_head","r","d"}, "dq_pi" ([2][B]: d(actor loss)/dQ1, dQ2 -- which twin
- * min(Q1,Q2) routed the gradient to), "q_pi" ([2][B]: Q1, Q2 at (s, a~); layer-chained plan only), "psave" ([2B][act][8]:
+ * min(Q1,Q2) routed the gradient to), "q_pi" ([2][B]: Q1, Q2 at (s, a~)), "psave" ([2B][act][8]:
  * what the policy head saved per (row, action) -- std, u-mu, tanh(u), action, Jacobian term, the NOISE it used, clamp mask,
  * log-prob term), "head" ([2B][2*act]: the policy head's output as the head computed it, mu | log-std before the clamp;
  * after b200sac_act its first n rows), or a hidden (after b200sac_redo: its forward's rows, see there)

@@ -2,12 +2,12 @@
 DroQ) and critic ensembles (critic_ensemble, REDQ / RLPD) -- over the per-layer plan's envelope at both precisions, against
 the autograd oracles (oracle/critic_ln_port.py, oracle/droq_port.py, oracle/redq_port.py).
 
-The variants' own kernels (ln_kernels.cuh; the E-critic head, head-backward, policy-dout and LayerNorm kernels of
-ensemble_kernels.cuh) go wrong where their loops and index arithmetic change shape: a partial last ln_bwd chunk (batch not a
+The variants' own kernels (ln_kernels.cuh; the E-critic head, head-backward and policy-dout kernels of sac_kernels.cuh)
+go wrong where their loops and index arithmetic change shape: a partial last ln_bwd chunk (batch not a
 multiple of kLnRows = 16) and 128 chunks through its ticket (batch 2048), a second pass of ln_bwd's column loop (H > 256),
 drop_row's group loop past its first 32 groups (H > 128) and odd widths, split-K weight gradients and row-sliced head
-gradients (batch >= 512, critic k's slots at + k * rsNet), head_bwd_ens_kernel in critic mode (last width not a multiple of
-4), policy_dout_ens_kernel's E-sum (batch * act > 2048), a grouped GEMM cut into several launches (E = 10 at batch >= 512),
+gradients (batch >= 512, critic k's slots at + k * rsNet), head_bwd_kernel in critic mode (last width not a multiple of
+4), policy_dout_kernel's E-sum (batch * act > 2048), a grouped GEMM cut into several launches (E = 10 at batch >= 512),
 and the actor's "min" routing over E critics.  CASES reaches each of these (test_cases_reach_every_edge fails if an edit of
 the table stops reaching one):
 
@@ -55,9 +55,9 @@ CASES = {
     "ln-b2048": (LAYER_CASES["b2048"], dict(ln=True), (0, 1)),              # 128 ln_bwd chunks, 64 tasks, act_dim 8
     "droq-b2048": (LAYER_CASES["b2048"], dict(ln=True, p=0.05), (1,)),
     "ln-ms1280": (sp.ms_spec().to_json(), dict(ln=True), (1,)),             # the MTSAC learner: 3 x 400, batch 1280
-    "ens3-odd67": (LAYER_CASES["odd67"], dict(E=3, ens=(1, "min")), (0, 1)),    # head_bwd_ens_kernel in critic mode
+    "ens3-odd67": (LAYER_CASES["odd67"], dict(E=3, ens=(1, "min")), (0, 1)),    # head_bwd_kernel in critic mode
     "ens10-b1": (LAYER_CASES["b1"], dict(E=10, ens=(10, "mean")), (0, 1)),
-    "ens5-pdout257": (LAYER_CASES["pdout257"], dict(E=5, ens=(2, "min")), (0, 1)),     # policy_dout_ens_kernel
+    "ens5-pdout257": (LAYER_CASES["pdout257"], dict(E=5, ens=(2, "min")), (0, 1)),     # policy_dout_kernel
     "ens3-pdout256": (LAYER_CASES["pdout256"], dict(E=3, ens=(3, "mean")), (0, 1)),    # the E-sum inside head_bwd
     "ens10-split517": (LAYER_CASES["split517"], dict(E=10, ens=(2, "min")), (0, 1)),   # > 24 problems per group
     "ens10-b2048": (LAYER_CASES["b2048"], dict(E=10, ens=(2, "mean")), (0, 1)),
@@ -121,8 +121,8 @@ def edges(name):
     if v["E"] > 2:
         E = v["E"]
         if hid[-1] % 4 and E in (3, 10):
-            have.add(f"E1: critic-mode head_bwd_ens_kernel, E = {E}")
-        have.add("E2: policy_dout_ens_kernel" if B * A > 2048 else "E2: E-sum in head_bwd")
+            have.add(f"E1: critic-mode head_bwd_kernel, E = {E}")
+        have.add("E2: policy_dout_kernel" if B * A > 2048 else "E2: E-sum in head_bwd")
         if E == 10 and B >= SPLIT_K_MIN and set(CASES[name][2]) == {0, 1}:
             have.add("E3: E = 10 at batch >= 512, both precisions")
         for m, actor in v["ens_rows"]:
@@ -142,8 +142,8 @@ WANT = ({f"L1 {k}: {e}" for k in ("LN", "DroQ", "E") for e in ("batch 1", "batch
         | {f"L4 {k}: {e}" for k in ("LN", "DroQ", "E") for e in ("batch >= 512", "batch 2048")}
         | {f"L5 {k}: {e}" for k in ("LN", "DroQ") for e in ("1 hidden layer", "3 hidden layers")}
         | {f"L6 {k}: {e}" for k in ("LN", "E") for e in ("64 tasks, weighted", "act_dim 8")}
-        | {"E1: critic-mode head_bwd_ens_kernel, E = 3", "E1: critic-mode head_bwd_ens_kernel, E = 10",
-           "E2: policy_dout_ens_kernel", "E2: E-sum in head_bwd", "E3: E = 10 at batch >= 512, both precisions",
+        | {"E1: critic-mode head_bwd_kernel, E = 3", "E1: critic-mode head_bwd_kernel, E = 10",
+           "E2: policy_dout_kernel", "E2: E-sum in head_bwd", "E3: E = 10 at batch >= 512, both precisions",
            "E4: m = 1", "E4: m = 2", "E4: m = E", "E4: mean", "E4: min", "E4: E = 3", "E4: E = 5", "E4: E = 10",
            "R: 3 replicas, LN + DroQ + E, own rates and (m, reduction)", "X: RLPD / DroQ at width 256, batch 256"})
 
